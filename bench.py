@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- mash.Sketch throughput on B200 (BASELINE.json metric) and the rest of SURVEY.md 8d.
+"""bench.py -- mash.Sketch throughput on H100 (BASELINE.json metric) and the rest of SURVEY.md 8d.
 
 A "step" is one pass of the Sketch hot path over one batch of synthetic reads:
 BASELINE configs[1] = 10 M x 150 bp reads, k=21, sketchSize=1000 per GPU (reads are
@@ -14,7 +14,7 @@ N=8 is configs[3], 80 M reads).
              4*s-byte Sketches array per read, pageable); host_bw: bare cudaMemcpyAsync D2H / H2D
              from the same pinned buffers, all ranks at once -- the platform cap of e2e
   roofline   algorithmic bytes (L + 4*min(L-k, s) per read, SURVEY 8d) / kernel time vs the
-             measured HBM copy peak (MEASURED_PEAKS.json)
+             measured HBM copy peak (MEASURED_PEAKS.json; else the H100 SXM data-sheet 3.35 TB/s)
   cpu_baseline  C restatement of the Go algorithm (oracle/, "port") on the host cores; thread
              count = best of a small sweep bounded by the schedulable cores (affinity, cgroup quota)
   secondary  (N=1) configs[2] and configs[4] on this GPU: cfg3 sketch (K2), cfg3 all-pairs (K3),
@@ -26,8 +26,13 @@ N=8 is configs[3], 80 M reads).
              gather -> row-block all-pairs); in-run assertions: fused == NCCL, and a sample of every
              rank's gathered buffer == the oracle
 
-`--impl reference` times the CPU restatement alone (the Go reference cannot run here:
-no Go toolchain, see DESIGN.md) on a bounded sample of the same workload.
+`--impl reference` times the CPU restatement alone (the Go reference is not built by this
+project, see DESIGN.md) on a bounded sample of the same workload.
+
+`--dump-outputs DIR` writes what the timed path computed in its last step: a fixed, seeded sample of
+the sketch rows (DIR/sketch_rows.npy, float64 read indices) and their words (DIR/sketches.npy,
+float64 [rows][129]).  The reads come from a fixed seed, so the same arguments give the same inputs.
+Under torchrun only rank 0 writes, so the sample covers rank 0's shard (reads [0, --reads)) only.
 """
 from __future__ import annotations
 
@@ -49,7 +54,9 @@ READ_LEN, KMER, SKETCH = 150, 21, 1000
 NK = READ_LEN - KMER  # 129 informative words per read
 BYTES_PER_READ = READ_LEN + 4 * min(NK, SKETCH)  # 666 (SURVEY 8d)
 METRIC = "mash.Sketch Gbases/s"
-NVLINK_PEER_PEAK_GBS = 770.0  # measured peer-copy bandwidth per direction, B200_PROFILING.md
+NVLINK_PEER_PEAK_GBS = 450.0  # H100 SXM data sheet: NVLink 4, 900 GB/s both directions; not measured here
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet; the denominator when MEASURED_PEAKS.json is absent
+DUMP_ROWS = 16384  # sketch rows in --dump-outputs (16384 x 129 float64 = 17 MB)
 
 
 def parse():
@@ -64,11 +71,13 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
     ap.add_argument("--no-pipeline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's sketches as DIR/*.npy (float64); with N > 1 ranks, of rank 0's shard only")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -194,7 +203,7 @@ def _cpu_desc(n, threads, dt, value, cores, sweep):
     return {"value": value, "unit": "Gbases/s", "cores": threads, "kind": "port", "schedulable_cores": cores,
             "thread_sweep_gbases_per_s": sweep,
             "sample": f"first {n} reads of the 10M x 150bp k=21 s=1000 workload per step; C restatement of the Go algorithm "
-                      f"(mash.go:59-104, not Go: no Go toolchain here), static parallel-for over reads on {threads} threads "
+                      f"(mash.go:59-104, not Go), static parallel-for over reads on {threads} threads "
                       f"(best of the sweep; {cores} schedulable cores), {dt:.2f} s per step"}
 
 
@@ -208,7 +217,7 @@ def cpu_reference_leg(budget_s: float):
 
 def run_reference(args, rank: int, world: int):
     """`--impl reference`: the reference's own CPU implementation of the path.  The Go code
-    cannot run here, so this is its C restatement on the schedulable host threads; each step is one
+    is not built by this project, so this is its C restatement on the schedulable host threads; each step is one
     pass over a bounded sample of the cfg2 workload (same metric / unit / config as our arm)."""
     if rank != 0:
         return
@@ -356,8 +365,8 @@ def e2e_leg(cx, args, d_in, d_out):
         # bounded slice so that the 4 kB/read fits.  (a) PG_SKETCH_PAD_ZERO: the library writes all 4 kB per read
         # (everything a fresh []*Mash costs, into warm memory); (b) PG_SKETCH_TAIL_KEEP into an array the caller
         # zeroed beforehand (outside the timed region): the library's share when the host language already hands out
-        # zeroed memory, as Go's make does.  First-touching a FRESH 8 GB slab inside the step costs ~1 s on this box
-        # (page faults; measured once, DESIGN.md section 6) -- for any implementation, the CPU reference included.
+        # zeroed memory, as Go's make does.  First-touching a FRESH 8 GB slab inside the step would time page faults
+        # (DESIGN.md section 6) -- for any implementation, the CPU reference included.
         m = min(n, 2_000_000)
         g_out = np.empty((m, SKETCH), dtype=np.uint32)
 
@@ -404,7 +413,10 @@ def secondary_leg(cx, clocks_mhz):
     L, dev, st = cx.L, cx.dev, cx.stream
     cores = schedulable_cores()
     out = []
-    clk = (clocks_mhz or 1965.0) * 1e6
+    clk = (clocks_mhz or 1980.0) * 1e6  # H100 SXM maximum SM clock when no sample was taken
+    sms = C.c_int(0)
+    cx.check(L.pg_device_sm_count(C.byref(sms)))
+    sms = sms.value
     # ---- cfg3 sketch (K2) ----
     n, RL, k, s = 100_000, 10_000, 31, 2000
     d_reads = torch.empty(n * RL, dtype=torch.uint8, device=dev)
@@ -423,12 +435,12 @@ def secondary_leg(cx, clocks_mhz):
     # integer-issue ceiling of the formulation (SURVEY 7.2): murmur3 of a 31-mer with shared block pre-mixes needs
     # >= 7 body rounds x 3 + pre-mix 3 + 3-byte tail 4 + length xor 1 + fmix 8 = 37 thread instructions per k-mer
     inst = 37
-    ceiling = 148 * 4 * clk * 32 / inst  # SMs x sub-partitions x issue/clk x lanes / instructions per k-mer
+    ceiling = sms * 4 * clk * 32 / inst  # SMs x sub-partitions x issue/clk x lanes / instructions per k-mer
     out.append({"name": "cfg3 sketch (K2)", "config": "configs[2]: 100k x 10 kbp long reads, k=31, sketchSize=2000",
                 "kernel": "sketch_thresh_walk_kernel + sketch_thresh_select_kernel (+ sketch_select_walk_kernel over the retry list, empty here)",
                 "ms": ms, "value": n * RL / ms / 1e6, "unit": "Gbases/s", "gpu_launches_per_pass": launches,
                 "bound": "integer issue (not HBM: 1.8 B/base)", "int_issue_ceiling_gbases_per_s": ceiling / 1e9,
-                "int_issue_ceiling_derivation": f"148 SMs x 4 sub-partitions x {clk / 1e6:.0f} MHz x 32 lanes / {inst} instructions per 31-mer "
+                "int_issue_ceiling_derivation": f"{sms} SMs x 4 sub-partitions x {clk / 1e6:.0f} MHz x 32 lanes / {inst} instructions per 31-mer "
                                                 "(7 body rounds x 3, pre-mix 3, tail 4, len 1, fmix 8); selection work excluded",
                 "frac_of_int_issue_ceiling": (n * RL / ms * 1e3) / ceiling, "algorithmic_GBps": n * (RL + 4 * s) / ms / 1e6,
                 "frac_of_hbm_peak": n * (RL + 4 * s) / ms / 1e6 / cx.peak, "parity_vs_oracle": parity, "parity_sample": f"first {m} reads, all {s} words",
@@ -484,11 +496,11 @@ def secondary_leg(cx, clocks_mhz):
     cells = m * PL * TL
     k4_name = (L.pg_last_kernel() or b"").decode()
     per_cell = 2 if "x2" in k4_name else 4  # 3 DPX add-max + 1 max per DP step; the packed int16 kernel advances two cells per step
-    alu_ceiling = 148 * 64 * clk / per_cell  # ALU pipe: 64 lanes/clk/SM
+    alu_ceiling = sms * 64 * clk / per_cell  # ALU pipe: 64 lanes/clk/SM
     out.append({"name": "cfg5 Smith-Waterman score (K4)", "config": "configs[4]: 1M x 25 bp primers vs a 10 kb template, +3/-3, gap -2",
                 "kernel": k4_name, "ms": ms, "value": cells / ms / 1e9, "unit": "TCUPS",
                 "bound": "integer ALU / DPX issue", "alu_issue_ceiling_tcups": alu_ceiling / 1e12,
-                "alu_issue_ceiling_derivation": f"148 SMs x 64 ALU lanes x {clk / 1e6:.0f} MHz / {per_cell} ALU-pipe instructions per cell"
+                "alu_issue_ceiling_derivation": f"{sms} SMs x 64 ALU lanes x {clk / 1e6:.0f} MHz / {per_cell} ALU-pipe instructions per cell"
                                                 + (" (4 per DP step of the 2 x int16 packed kernel, two cells per step)" if per_cell == 2 else ""),
                 "frac_of_alu_issue_ceiling": (cells / ms * 1e3) / alu_ceiling,
                 "parity_vs_oracle": rc == 0 and bool(np.array_equal(score[:mc].cpu().numpy(), want_sc)) and int(ec.abs().max().item()) == 0,
@@ -538,10 +550,16 @@ def pipeline_leg(cx, d_in, d_out):
     # ---- B: cfg4 shape -- every rank sketches its 10M reads; all-gather of the compact sketches ----
     plan = ShardPlan(n * world, rank, world)
     local_sk = d_out.view(n, NK)  # K1 output of the headline step (reads [rank*n, (rank+1)*n))
-    gathered, t_ag = timed(lambda: all_gather_rows(local_sk, plan))
-    gathered, t_ag2 = timed(lambda: all_gather_rows(local_sk, plan))
+    # A full gathered copy is world x n x 129 x 4 B per rank (41.3 GB at N = 8, 10 M reads per rank), so at most one
+    # is alive at a time on an 80 GB GPU: the timed NCCL output is freed on return, before the fused buffer exists.
+    def nccl_allgather():
+        all_gather_rows(local_sk, plan)
+
+    _, t_ag = timed(nccl_allgather)
+    _, t_ag2 = timed(nccl_allgather)
     t_ag = min(t_ag, t_ag2)
     _, t_sk = timed(lambda: cx.check(L.pg_mash_sketch_uniform_dev(d_in.data_ptr(), n, READ_LEN, KMER, SKETCH, 0, d_out.data_ptr(), NK, None, cx.stream)))
+    torch.cuda.empty_cache()  # the gathered buffer is a cudaMalloc of its own, outside torch's cache
     buf = GatheredBuffer(plan, NK)
     fused = lambda: fused_sketch_gather(d_in, READ_LEN, KMER, SKETCH, buf, sync=False)  # noqa: E731
     fused(); barrier(cx)
@@ -550,8 +568,15 @@ def pipeline_leg(cx, d_in, d_out):
     t_f = min(t_f, t_f2)
     barrier(cx)
     fused_t = buf.as_tensor()
-    # parity 1: the fused buffer equals the NCCL all-gather, whole buffer, on every rank
-    eq = all_true(cx, bool(torch.equal(fused_t, gathered)))
+    # parity 1: the fused buffer equals the NCCL all-gather, whole buffer, on every rank; the all-gather runs over
+    # chunks of 2^20 rows per rank (4.1 GB at N = 8) so that it never needs a second full copy
+    eq, chunk = True, 1 << 20
+    for c in range(0, n, chunk):
+        part = torch.empty((world, min(chunk, n - c), NK), dtype=torch.int32, device=dev)
+        dist.all_gather_into_tensor(part, local_sk[c: c + chunk].contiguous())
+        eq = eq and all(bool(torch.equal(fused_t[r * n + c: r * n + c + part.shape[1]], part[r])) for r in range(world))
+        del part
+    eq = all_true(cx, eq)
     # parity 2: on every rank, the first 256 rows of EVERY rank's block equal the oracle
     ok = True
     for r in range(world):
@@ -583,7 +608,7 @@ def pipeline_leg(cx, d_in, d_out):
                    "parity": {"fused_equals_nccl_allgather_all_rows_all_ranks": eq,
                               "every_rank_block_first_256_rows_equal_oracle_on_all_ranks": ok,
                               "distance_sample_equals_oracle": ok_d and max_same == 0}}
-    del same, same0, sub, gathered, fused_t
+    del same, same0, sub, fused_t
     buf.close()
     torch.cuda.empty_cache()
 
@@ -695,6 +720,18 @@ def make_all_pairs(cx):
     return all_pairs, check
 
 
+def dump_outputs(out_dir, d_out, n):
+    """A fixed, seeded sample of rank 0's sketch rows of the last timed step, as float64 (exact for u32)."""
+    import numpy as np
+    import torch
+
+    rows = np.sort(np.random.default_rng(0x706F6C79).choice(n, size=min(n, DUMP_ROWS), replace=False))
+    got = d_out.view(n, NK)[torch.from_numpy(rows).to(d_out.device)].cpu().numpy().view(np.uint32)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "sketch_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "sketches.npy"), got.astype(np.float64))
+
+
 def main():
     args = parse()
     rank = int(os.environ.get("RANK", "0"))
@@ -730,7 +767,7 @@ def main():
     if os.path.exists(peaks_path):
         cx.peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     else:
-        cx.peak, peak_src = 6650.0, "B200_PROFILING.md fallback (of fallback)"
+        cx.peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet (not measured)"
     cx.all_pairs, cx.all_pairs_check = make_all_pairs(cx)
 
     d_in = torch.empty(n * READ_LEN, dtype=torch.uint8, device=dev)
@@ -774,6 +811,9 @@ def main():
     ms_per_step = ms / args.steps
     value = world * n * READ_LEN / (ms_per_step * 1e-3) / 1e9  # whole-job Gbases/s
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_out, n)
+
     # in-run parity of the headline result on EVERY rank: head of this rank's shard vs the oracle
     import oracle_ffi
     m = 2048
@@ -795,17 +835,8 @@ def main():
         return
 
     achieved = n * BYTES_PER_READ / (ms_per_step * 1e-3) / 1e9
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "k1_traffic.json")
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            traffic = tj["dram_bytes_per_read"] * n  # per launch, scaled from the ncu capture's reads
-            traffic_src = f"profiles/k1_traffic.json: ncu --set full dram__bytes_read.sum + dram__bytes_write.sum of {tj.get('source', 'the committed capture')}, per read x {n} reads (not measured in this run: ncu cannot run inside the timed bench)"
-        except Exception:
-            traffic = None
     roofline = {"bound": "hbm", "achieved": achieved, "peak": cx.peak, "unit": "GB/s", "frac": achieved / cx.peak,
-                "traffic": traffic, "traffic_source": traffic_src, "kernel": kernel_name, "algorithmic_bytes_per_launch": n * BYTES_PER_READ,
+                "traffic": None, "traffic_source": "not measured", "kernel": kernel_name, "algorithmic_bytes_per_launch": n * BYTES_PER_READ,
                 "peak_source": peak_src, "avg_launch_ms": ms_per_step}
 
     del d_in, d_out
@@ -829,7 +860,7 @@ def main():
         "config": {"workload": "configs[1]: 10M x 150bp short reads, k=21, sketchSize=1000 per GPU"
                    + (" (x8 = configs[3], 80M reads)" if world == 8 else ""),
                    "reads_per_gpu": n, "read_len": READ_LEN, "k": KMER, "sketch_size": SKETCH,
-                   "l2": "inputs (1.5 GB) + outputs (5.2 GB) per step are larger than L2 (126 MB); no explicit flush",
+                   "l2": "inputs (1.5 GB) + outputs (5.2 GB) per step are larger than L2 (50 MB); no explicit flush",
                    "parallelism": f"reads sharded over {world} GPU(s), no data-path collective"},
         "parity": {"head_of_every_rank_shard_equals_oracle": headline_parity},
         "roofline": roofline, "cpu_baseline": cpu_baseline, "e2e": e2e, "e2e_variants": e2e_variants, "host_bw": host_bw,

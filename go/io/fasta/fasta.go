@@ -1,4 +1,4 @@
-// Package fasta is the B200-backed drop-in for bebop/poly's io/fasta parser entry points
+// Package fasta is the H100-backed drop-in for bebop/poly's io/fasta parser entry points
 // (io/fasta/fasta.go:66-77,89-99): same exported names and results, the parsing itself runs on
 // the GPU through libpolyb200.so (pg_fasta_ingest).  The writer half of the reference package
 // (Build / Write) and the channel-based ParseConcurrent are untouched pure Go and stay as they are.

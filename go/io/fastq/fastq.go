@@ -1,4 +1,4 @@
-// Package fastq is the B200-backed drop-in for the record parser of bebop/poly's io/fastq
+// Package fastq is the H100-backed drop-in for the record parser of bebop/poly's io/fastq
 // (io/fastq/fastq.go:46-99,117-214): Parse returns the same []Fastq and the same error for the same
 // bytes.  The line index, the reference's per-record checks (in its order) and the dense copy of the
 // sequences run on the GPU (pg_fastq_ingest_records); Identifier, Optionals and Quality are cut out of

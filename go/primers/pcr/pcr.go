@@ -1,4 +1,4 @@
-// Package pcr is the B200-backed drop-in for bebop/poly's primers/pcr (primers/pcr/pcr.go): same
+// Package pcr is the H100-backed drop-in for bebop/poly's primers/pcr (primers/pcr/pcr.go): same
 // exported functions and results.  The Tm searches (DesignPrimers*: pcr.go:44-60; the minimal-primer
 // loop of SimulateSimple: pcr.go:93-100) and the binding-site search the reference does with a suffix
 // array (pcr.go:87,110-115) run on the GPU through libpolyb200.so; the fragment assembly

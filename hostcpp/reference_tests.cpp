@@ -3,7 +3,7 @@
 //   search/mash/mash_test.go:9-62, search/mash/example_test.go:9-22,
 //   search/align/align_test.go:139-292, search/align/example_test.go:49-111,
 //   primers/primers_test.go:29-84, primers/pcr/pcr_test.go:12-101, primers/pcr/example_test.go:10-69.
-// Needs a B200: every call below lands in libpolyb200.so.  Run by tests/test_gpu_hostcpp.py.
+// Needs an H100: every call below lands in libpolyb200.so.  Run by tests/test_gpu_hostcpp.py.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>

@@ -1,12 +1,12 @@
 /*
- * poly_b200.h -- C ABI of libpolyb200.so: the B200 (sm_100a) implementation of
+ * poly_b200.h -- C ABI of libpolyb200.so: the H100 (sm_90a) implementation of
  * bebop/poly's search/mash sketching hot path plus the two secondary batched
  * kernels (search/align.SmithWaterman score, primers.SantaLucia).
  *
  * The reference is pure Go and has NO FFI/plugin interface (SURVEY.md 8b); the
  * drop-in boundary is the exported Go API of three leaf packages.  Each entry
- * point below names the reference function it replaces (file:line under
- * /root/reference); INTEGRATION.md shows the cgo binding for each.
+ * point below names the reference function it replaces (file:line in
+ * bebop/poly); INTEGRATION.md shows the cgo binding for each.
  *
  * Conventions
  *   - plain C: pointers + sizes, no C++/torch types, no exceptions across the ABI;
@@ -26,7 +26,7 @@
  *     pg_fasta_ingest_dev (they return counts and the error position by value), and
  *     pg_mash_sketch_batch_dev for ragged batches the threshold path does not take
  *     (s < 2, or more than 4 Mi row x item slots) when they hold few long sequences;
- *   - there is NO CPU fallback: without a usable sm_100 device every compute entry
+ *   - there is NO CPU fallback: without a usable sm_90 device every compute entry
  *     point fails with PG_ERR_NO_DEVICE.
  */
 #ifndef POLY_B200_H
@@ -42,7 +42,7 @@ extern "C" {
 #define PG_OK 0
 #define PG_ERR_CUDA 1        /* a CUDA runtime call failed (see pg_last_error)          */
 #define PG_ERR_ARG 2         /* invalid argument                                         */
-#define PG_ERR_NO_DEVICE 3   /* no CUDA device / not an sm_100 part                      */
+#define PG_ERR_NO_DEVICE 3   /* no CUDA device / not an sm_90 part                       */
 #define PG_ERR_PANIC 4       /* >= 1 item hits an input on which the Go reference panics */
 #define PG_ERR_UNSUPPORTED 5 /* >= 1 item is outside the supported domain                */
 #define PG_ERR_NOMEM 6

@@ -1,4 +1,4 @@
-"""poly_b200 -- B200 (sm_100a) implementation of bebop/poly's search/mash sketching
+"""poly_b200 -- H100 (sm_90a) implementation of bebop/poly's search/mash sketching
 hot path plus the secondary search/align Smith-Waterman scorer and primers SantaLucia
 Tm kernels.  Host-side mirrors of the reference's Go API live in mash / align /
 primers; all compute happens in libpolyb200.so (hand-written CUDA, C ABI in

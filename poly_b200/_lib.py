@@ -1,7 +1,7 @@
 """ctypes binding of libpolyb200.so (include/poly_b200.h).
 
 The library is the product: there is no Python/NumPy/PyTorch compute fallback.  If the
-shared object is missing, or no sm_100 device is usable, importing works (so that the
+shared object is missing, or no sm_90 device is usable, importing works (so that the
 CPU-only test tier can check the exported symbols) but every compute call raises.
 """
 from __future__ import annotations

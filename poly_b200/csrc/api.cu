@@ -1,6 +1,6 @@
 // api.cu -- the C ABI of libpolyb200.so (include/poly_b200.h): argument checking,
 // device selection, host<->device staging for the host-pointer entry points, and
-// dispatch to the kernel launchers.  No compute happens on the host: when no sm_100
+// dispatch to the kernel launchers.  No compute happens on the host: when no sm_90
 // device is usable every compute entry point fails with PG_ERR_NO_DEVICE.
 #include <algorithm>
 #include <atomic>
@@ -176,7 +176,7 @@ void note_launch(const char *name) {
     t_last_kernel = name;
     g_launches.fetch_add(1, std::memory_order_relaxed);
 }
-int sm_count() { return t_ctx && t_ctx->sms > 0 ? t_ctx->sms : 148; }
+int sm_count() { return t_ctx && t_ctx->sms > 0 ? t_ctx->sms : 132; }
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (device, kernel, size class): function
 // attributes live in the device's context, so the cache is per device and lock-protected (several
@@ -199,8 +199,8 @@ static int ctx_create_locked(int device) {
     if (c.ready.load(std::memory_order_acquire)) return PG_OK;
     cudaDeviceProp prop;
     PG_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        set_error("device %d is sm_%d%d; libpolyb200 is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("device %d is sm_%d%d; libpolyb200 is built for sm_90a only", device, prop.major, prop.minor);
         return PG_ERR_NO_DEVICE;
     }
     PG_CUDA(cudaSetDevice(device));

@@ -13,7 +13,7 @@
 //     murmur3 arithmetic is kept off that pipe: for k % 4 == 1 the tail pre-mix comes from
 //     a 256-entry shared-memory table (2 LSU instructions, table address formed by IMAD on
 //     the FMA pipe), the main loop has no bounds tests or predicated stores, and raw words
-//     are fetched one step ahead (DESIGN.md "K1", profiles/);
+//     are fetched one step ahead (DESIGN.md "K1");
 //   * hashes are staged in shared memory ([read][pos], stride L-k words: bank-conflict
 //     free when L-k is odd) and leave as ONE bulk store per tile (the compact output
 //     [n][L-k] of a tile is contiguous in HBM).

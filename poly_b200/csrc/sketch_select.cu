@@ -417,8 +417,7 @@ sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restri
 // multiset), a partial last chunk stores them positionally; afterwards the walk itself tests each hash
 // against the admission limit and appends the few that pass (one shared-memory atomic each) --
 // for long sequences almost nothing passes, so the steady state is pure hashing.
-// Half the instructions of the generic kernel (ncu: 0.74 G vs 1.46 G warp instructions on 20 k
-// cfg3 reads); 256 threads x 3 CTAs per SM keep the issue slots busy.
+// About half the instructions of the generic kernel; 256 threads x 3 CTAs per SM keep the issue slots busy.
 constexpr int SELW_THREADS = 256;
 constexpr int SELW_SEG = 20;  // bytes between the segments of adjacent lanes = 5 words: conflict-free smem reads
 constexpr int SELW_CHUNK = SELW_THREADS * SELW_SEG;                      // 5120 k-mer positions
@@ -766,7 +765,7 @@ struct SeltGeom {
 };
 constexpr int SELT_ITEM_CHUNKS = 8;
 // rolled body (groups of 3 steps, then a ring rotation) from NB = 6 (k >= 24) on; k = 21 (NB = 5) keeps the unrolled 5-step
-// body: 1.38 vs 1.43 ms (profiles/r02_k2_tuning.md)
+// body, which is short enough not to stall on instruction fetch
 #define SELT_ROLLED_DEFAULT(K_) ((K_) / 4 >= 6)
 constexpr int SELT_SEL_THREADS = 256;
 

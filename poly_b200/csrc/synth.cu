@@ -75,12 +75,12 @@ int launch_synth_reads(uint8_t *d_bases, uint64_t first_read, uint64_t n_reads, 
     const uint64_t count = n_reads * (uint64_t)read_len;
     if (kind == 0) {
         const uint64_t words = (count >> 5) + 2;
-        const unsigned blocks = (unsigned)std::min<uint64_t>((words + 255) / 256, 148 * 32);
+        const unsigned blocks = (unsigned)std::min<uint64_t>((words + 255) / 256, (uint64_t)sm_count() * 32);
         synth_independent_kernel<<<blocks, 256, 0, st>>>(d_bases, first_read * read_len, count, seed);
         PG_LAUNCH_CHECK("synth_independent_kernel");
     } else if (kind == 1) {
         if (family == 0) { set_error("family must be > 0"); return PG_ERR_ARG; }
-        const unsigned blocks = (unsigned)std::min<uint64_t>((count + 255) / 256, 148 * 32);
+        const unsigned blocks = (unsigned)std::min<uint64_t>((count + 255) / 256, (uint64_t)sm_count() * 32);
         synth_family_kernel<<<blocks, 256, 0, st>>>(d_bases, first_read, n_reads, read_len, seed, family);
         PG_LAUNCH_CHECK("synth_family_kernel");
     } else {

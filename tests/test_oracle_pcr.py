@@ -1,12 +1,14 @@
 """Pins the CPU restatement of pcr.Simulate (tests/pcr_util.py, Tm from oracle/) on the expectations of
-the reference's own tests: primers/pcr/example_test.go:10-36,58-69 and pcr_test.go:13-101."""
-import re
+the reference's own tests: primers/pcr/example_test.go:10-36,58-69 and pcr_test.go:13-101 (the
+sequences those files use are stored in tests/golden/pcr_goldens.json)."""
+import json
+import os
 
 import pytest
 
 import pcr_util as P
 
-REF_EXAMPLE = "/root/reference/primers/pcr/example_test.go"
+GOLD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "pcr_goldens.json")))
 
 
 def test_reference_expectations():
@@ -15,16 +17,12 @@ def test_reference_expectations():
         assert ok(fr, err), primers
 
 
-@pytest.mark.skipif(not __import__("os").path.exists(REF_EXAMPLE), reason="reference only exists in the build container")
 def test_constants_equal_the_reference_test_files():
-    ex = open(REF_EXAMPLE).read()
-    want = re.search(r"// Output: \[(\w+)\]", ex).group(1)
-    assert P.FULL_AMPLICON == want
-    assert P.GENE.decode() == re.search(r'gene := "(\w+)"', ex).group(1)
-    assert P.BAD_FRAGMENT.decode() == re.search(r'badFragment := "(\w+)"', ex).group(1)
-    t = open("/root/reference/primers/pcr/pcr_test.go").read()
-    assert P.CIRCULAR_TARGET == re.search(r'targetFragment := "(\w+)"', t).group(1)
-    assert P.FULL_AMPLICON == re.search(r'want := "(\w+)"', t).group(1)
+    assert P.FULL_AMPLICON == GOLD["example_output"]
+    assert P.GENE.decode() == GOLD["example_gene"]
+    assert P.BAD_FRAGMENT.decode() == GOLD["example_bad_fragment"]
+    assert P.CIRCULAR_TARGET == GOLD["test_target_fragment"]
+    assert P.FULL_AMPLICON == GOLD["test_want"]
 
 
 def test_minimal_length_quirks():

@@ -10,13 +10,12 @@ import json
 import os
 import sys
 
-import numpy as np
 import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from poly_b200 import _lib, synth  # noqa: E402
-from poly_b200.dist import GatheredBuffer, ShardPlan, all_gather_rows, cuda_distance_block, cuda_sketch_uniform  # noqa: E402
+from poly_b200.dist import GatheredBuffer, ShardPlan, all_gather_rows, cuda_distance_block, cuda_sketch_uniform, fused_sketch_gather  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--long-reads", type=int, default=100_000)
@@ -89,30 +88,28 @@ report(stage="B cfg4 shape", n_gpus=world, reads_per_rank=m, sketch_ms=t_sk, ske
        allgather_ms=t_ag, allgather_GB_recv_per_rank=(world - 1) * m * nk * 4 / 1e9,
        allgather_GBps_per_rank=(world - 1) * m * nk * 4 / t_ag / 1e6, capped_rows=rows, capped_cols=cols * world, distance_ms=t_d,
        max_same=int(same.max().item()), note="reference semantics: n=129 < s=1000 -> zero-padded unsorted sketches -> every pair early-outs (distance 1.0)")
-del same, sub
+# rows of the NCCL result the fused buffer is checked against; a full gathered copy is world x m x 129 x 4 B
+# (41.3 GB at 8 ranks of 10 M reads), so it is freed before the fused buffer is allocated: one copy at a time
+ref_rows = {r: gathered[r * m: r * m + 4096].clone() for r in (0, world - 1)}
+del same, sub, gathered
 # ---- C: the same exchange fused into the sketch kernel (TMA bulk stores to peer memory) -------
 torch.cuda.empty_cache()
-buf = GatheredBuffer(m, nk, plan)
+buf = GatheredBuffer(plan, nk)
 
 
 def fused():
-    _lib.check(L.pg_mash_sketch_uniform_gather_dev(reads.data_ptr(), m, SL, k, s, buf._arr, world, rank, st))
+    fused_sketch_gather(reads, SL, k, s, buf, sync=False)
 
 
 fused(); torch.cuda.synchronize(); dist.barrier()
 _, t_f = timed(fused)
 _, t_f2 = timed(fused)
 # verify against the NCCL all-gather result (rows of the LAST rank and of rank 0)
-mine = torch.empty((2, 4096, nk), dtype=torch.int32, device=dev)
-import ctypes as C
-_lib.check(L.pg_memcpy_d2h(mine[0].cpu().numpy().ctypes.data, buf.ptr, 0, None))  # no-op; keeps the API exercised
-chk = np.empty((4096, nk), dtype=np.uint32)
-ok = True
-for r in (0, world - 1):
-    _lib.check(L.pg_memcpy_d2h(chk.ctypes.data, buf.ptr + r * m * nk * 4, chk.nbytes, None)); _lib.check(L.pg_stream_sync(None))
-    ok = ok and bool(np.array_equal(chk, gathered[r * m: r * m + 4096].cpu().numpy().view(np.uint32)))
+got = buf.as_tensor()
+ok = all(bool(torch.equal(got[r * m: r * m + 4096], ref_rows[r])) for r in ref_rows)
 report(stage="C cfg4 fused sketch+gather (peer stores)", n_gpus=world, reads_per_rank=m, fused_ms=min(t_f, t_f2), separate_ms=t_sk + t_ag,
        bytes_out_per_rank_GB=(world - 1) * m * nk * 4 / 1e9, nvlink_GBps_out_per_rank=(world - 1) * m * nk * 4 / min(t_f, t_f2) / 1e6,
        matches_allgather=ok)
+del got
 buf.close()
 dist.destroy_process_group()

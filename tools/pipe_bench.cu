@@ -1,7 +1,7 @@
 // tools/pipe_bench.cu -- measures issue throughput (cycles per warp instruction per SMSP)
-// of the integer instructions K1 is made of, on the B200 this runs on.  Evidence for the
+// of the integer instructions K1 is made of, on the GPU this runs on.  Evidence for the
 // pipe-balancing choices in DESIGN.md ("K1: integer-issue co-limit").
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipe_bench pipe_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipe_bench pipe_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -54,10 +54,11 @@ __global__ void bench(uint32_t *out, uint32_t a, uint32_t b, long long *cycles) 
 template <int OP>
 void run(const char *name, int n_instr_per_op, int warps_per_smsp) {
     uint32_t *out; long long *cyc, h;
-    int threads = 128 * warps_per_smsp;
-    cudaMalloc(&out, 148 * threads * 4); cudaMalloc(&cyc, 8);
-    bench<OP><<<148, threads>>>(out, 0x10000u, 0x2000u, cyc);
-    bench<OP><<<148, threads>>>(out, 0x10000u, 0x2000u, cyc);
+    int threads = 128 * warps_per_smsp, sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&out, (size_t)sms * threads * 4); cudaMalloc(&cyc, 8);
+    bench<OP><<<sms, threads>>>(out, 0x10000u, 0x2000u, cyc);
+    bench<OP><<<sms, threads>>>(out, 0x10000u, 0x2000u, cyc);
     cudaMemcpy(&h, cyc, 8, cudaMemcpyDeviceToHost);
     double ops = (double)ITERS * 4 * ILP * warps_per_smsp;  // op<> calls per SMSP
     printf("%-34s warps/SMSP=%d  %.3f cyc per op  (%.3f cyc per SASS instr if %d instr/op)\n", name, warps_per_smsp,
