@@ -60,6 +60,57 @@ struct SketchDst {
     int n;
 };
 
+// ---- per-row pieces of the sketch kernels (sketch_fill.cu, sketch_select.cu, sketch_select_large.cu) ----
+// Row `row` of a batch is bytes [beg, beg + len) of the bases and has n = max(len - k, 0) k-mers (mash.go:73).
+struct RowSpan {
+    uint64_t beg, len, n;
+};
+__device__ __forceinline__ RowSpan row_span(const uint64_t *offsets, uint32_t uniform_len, uint64_t row, uint32_t k) {
+    RowSpan r;
+    if (offsets) {
+        r.beg = offsets[row];
+        r.len = offsets[row + 1] - r.beg;
+    } else {
+        r.beg = row * (uint64_t)uniform_len;
+        r.len = uniform_len;
+    }
+    r.n = r.len > k ? r.len - k : 0;
+    return r;
+}
+// the select regime of mash.go:87-102 (s == 0 included: it panics there); other rows are filled positionally
+__host__ __device__ __forceinline__ bool select_regime(uint64_t n, uint64_t s) { return n >= s && n > 0; }
+
+// Thread 0 writes the status and count of a finished select-regime row.  `panic`: the row reaches the
+// reference's Sketches[-1] index (mash.go:96-98); each kernel tests that its own way.
+__device__ __forceinline__ void put_row_status(int32_t *status, uint32_t *count, uint64_t row, uint32_t cnt, bool panic) {
+    if (threadIdx.x != 0) return;
+    if (status) status[row] = panic ? PG_ITEM_PANIC : PG_ITEM_OK;
+    if (count) count[row] = cnt;
+}
+// s == 0: mash.go:96 reads Sketches[-1] on the first k-mer of a select-regime row.  True when that settled the row.
+__device__ __forceinline__ bool empty_sketch_panics(uint32_t s, int32_t *status, uint32_t *count, uint64_t row) {
+    if (s != 0) return false;
+    put_row_status(status, count, row, 0, true);
+    return true;
+}
+
+// Fused all-gather: the CTA copies the finished row src[0, s) to the row of every destination except
+// dst, which already holds it.  Static indices keep `extra` in parameter space.
+template <int NT>
+__device__ __forceinline__ void replicate_row(const SketchDst &extra, uint64_t row, uint64_t row_stride, const uint32_t *src,
+                                              const uint32_t *dst, uint32_t s) {
+    if (extra.n > 0) {
+        __syncthreads();  // src is complete
+#pragma unroll
+        for (int pr = 0; pr < PG_MAX_PEERS; ++pr) {
+            if (pr >= extra.n) continue;
+            uint32_t *peer = extra.ptr[pr] + row * row_stride;
+            if (peer == dst) continue;
+            for (uint32_t i = threadIdx.x; i < s; i += NT) peer[i] = src[i];
+        }
+    }
+}
+
 // ---- kernel launchers (one per .cu) -------------------------------------------
 // sketch_fill.cu
 int launch_sketch_uniform(const uint8_t *d_bases, uint64_t n_reads, uint32_t read_len, int k, int s,
@@ -70,7 +121,7 @@ int launch_sketch_ragged(const uint8_t *d_bases, const uint64_t *d_offsets, uint
                          uint64_t row_stride, uint32_t *d_count, int32_t *d_status, cudaStream_t st);
 // sketch_select.cu  (reads with n >= s; uniform: read_len != 0 and d_offsets == nullptr)
 int launch_sketch_select(const uint8_t *d_bases, const uint64_t *d_offsets, uint32_t read_len,
-                         uint64_t n_reads, int k, int s, uint32_t flags, uint32_t *d_out,
+                         uint64_t n_reads, int k, int s, uint32_t *d_out,
                          uint64_t row_stride, uint32_t *d_count, int32_t *d_status, cudaStream_t st,
                          const SketchDst *extra = nullptr, uint64_t max_read_len = 0);
 // sketch_select_large.cu: the select regime for s > 16384 or k > 1024 (hashes through global memory)

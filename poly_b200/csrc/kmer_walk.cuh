@@ -3,28 +3,32 @@
 // shared memory, 4 bytes (= 4 k-mers) per step.  The murmur3 block pre-mix K(p) of the 4 bytes at
 // position p is computed once and kept in a register ring shared by the k/4 k-mers that use it.
 //
-// PG_KMER_STEP(U, CHECKED, EMIT) is one word step (ring slot U); PG_K1_STEP is the same with the
-// positional store.  It uses these locals of the enclosing
-// scope (K, NB = K/4, TAIL = K%4, TAILMASK, LUT = (TAIL == 1) are compile-time):
-//   w_cur, w_nxt          the realigned words at the current / next word position
-//   raw_a, raw_b, swp, sh  raw staged words one step ahead of their use, funnel-shift amount
-//   ring[4][NB]            pre-mixes of the last NB word steps
+// A walk kernel is a template on K that opens with PG_WALK_CONSTANTS (K, NB = K/4, TAIL = K%4,
+// TAILMASK, LUT = (TAIL == 1), all compile-time), loads the tail table with load_kmix_table when LUT,
+// and starts each walk with PG_WALK_PROLOGUE.  PG_KMER_STEP(U, CHECKED, EMIT) is then one word step
+// (ring slot U); PG_K1_STEP is the same with the positional store.  They use these locals of the
+// enclosing scope:
+//   sw, sh                 staged words of the walk (the first at or before its first byte), funnel-shift amount
+//   w_cur, w_nxt          the realigned words at the current / next word position      (PG_WALK_PROLOGUE)
+//   raw_a, raw_b, swp      raw staged words one step ahead of their use                 (PG_WALK_PROLOGUE)
+//   ring[4][NB]            pre-mixes of the last NB word steps                          (PG_WALK_PROLOGUE)
 //   sb                     byte pointer: the tail byte of k-mer i is sb[i]      (LUT only)
 //   lut_stride, lut_base   shared-memory tail table (256 x kmix(byte)); the stride (4) is a
 //                          runtime value so byte*4 + base stays an IMAD on the FMA pipe
-//   ROTF, rotmul           number of leading body rounds whose rotate runs on the FMA pipe (0 = none) and the
-//                          runtime multiplier 8192 they use (murmur3.cuh, mm3_round_fma)
 //   my_out, i, nk          hashes of k-mers i .. i+3 go to my_out[i ..]; CHECKED guards i+r < nk
 #pragma once
 #include <stdint.h>
 
 #include "murmur3.cuh"
+#include "tma.cuh"
 
 namespace pg {
 
+// Shared-space load from a 32-bit shared address.  volatile: the rank loop of sketch_thresh_select_kernel
+// reads what other threads scattered before a barrier, and the load must stay behind that barrier.
 __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) {
     uint32_t v;
-    asm("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(saddr));
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(saddr));
     return v;
 }
 
@@ -40,6 +44,41 @@ constexpr KmixTable make_kmix_table() {
 }
 static __device__ __align__(16) const KmixTable g_kmix_byte = make_kmix_table();
 
+// The tail table into shared memory by one bulk copy that completes on `bar`; called by the thread that
+// initialised the barrier.
+__device__ __forceinline__ void load_kmix_table(uint32_t *s_lut, uint64_t *bar) {
+    mbar_expect_tx(bar, sizeof(KmixTable));
+    bulk_g2s(s_lut, &g_kmix_byte, sizeof(KmixTable), bar);
+}
+
+#define PG_WALK_CONSTANTS                                                                      \
+    constexpr int NB = K / 4;    /* 4-byte body blocks per k-mer */                            \
+    constexpr int TAIL = K % 4;  /* tail bytes per k-mer */                                    \
+    constexpr uint32_t TAILMASK = TAIL == 1 ? 0xffu : TAIL == 2 ? 0xffffu : 0xffffffu;         \
+    constexpr bool LUT = TAIL == 1;                                                            \
+    static_assert(NB >= 1 && K <= 32, "walk path: 4 <= k <= 32")
+
+// The first two realigned words, the raw words one step ahead of them, and word steps 0 .. NB-1,
+// which only fill the ring.
+#define PG_WALK_PROLOGUE                                                                       \
+    uint32_t raw_a = sw[0], raw_b = sw[1];                                                     \
+    uint32_t w_cur = __funnelshift_r(raw_a, raw_b, sh); /* bytes 4Q .. 4Q+3 of the walk */     \
+    raw_a = raw_b; raw_b = sw[2];                                                              \
+    uint32_t w_nxt = __funnelshift_r(raw_a, raw_b, sh); /* bytes 4Q+4 .. 4Q+7 */               \
+    raw_a = raw_b; raw_b = sw[3];                                                              \
+    const uint32_t *swp = sw + 4;                                                              \
+    uint32_t ring[4][NB]; /* ring[r][*]: pre-mixes K(4q+r) of the last NB word steps */        \
+    _Pragma("unroll") for (int q = 0; q < NB; ++q) {                                           \
+        ring[0][q] = mm3_kmix(w_cur);                                                          \
+        ring[1][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 8));                               \
+        ring[2][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 16));                              \
+        ring[3][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 24));                              \
+        w_cur = w_nxt;                                                                         \
+        w_nxt = __funnelshift_r(raw_a, raw_b, sh);                                             \
+        raw_a = raw_b;                                                                         \
+        raw_b = *swp++;                                                                        \
+    }
+
 // One word step = 4 k-mers (ring slot U).  EMIT(r, value) consumes the hash of k-mer i + r.
 #define PG_KMER_STEP(U, CHECKED, EMIT)                                                         \
     {                                                                                          \
@@ -50,9 +89,9 @@ static __device__ __align__(16) const KmixTable g_kmix_byte = make_kmix_table();
         w[3] = __funnelshift_r(w_cur, w_nxt, 24);                                              \
         uint32_t h[4];                                                                         \
         _Pragma("unroll") for (int r = 0; r < 4; ++r) {                                        \
-            uint32_t x = ROTF > 0 ? mm3_round_fma(0u, ring[r][U], rotmul) : mm3_round0(ring[r][U]); \
+            uint32_t x = mm3_round0(ring[r][U]);                                               \
             _Pragma("unroll") for (int j = 1; j < NB; ++j)                                     \
-                x = j < ROTF ? mm3_round_fma(x, ring[r][((U) + j) % NB], rotmul) : mm3_round(x, ring[r][((U) + j) % NB]); \
+                x = mm3_round(x, ring[r][((U) + j) % NB]);                                     \
             if (LUT) x ^= lds_u32(sb[i + r] * lut_stride + lut_base);                          \
             else if (TAIL) x ^= mm3_kmix(w[r] & TAILMASK);                                     \
             x ^= (uint32_t)K;                                                                  \

@@ -46,7 +46,8 @@ constexpr int SEL_MAX_S = 16384;    // largest sketch size of the shared-memory 
 constexpr int SEL_LOOKAHEAD = 1024; // max k supported by the staged path (bytes beyond chunk)
 constexpr int SEL_NBK = 2048;       // value buckets of the final sort-select (v >> 21)
 constexpr int SEL_BSHIFT = 21;
-constexpr int SEL_STAGE_WORDS = (SEL_CHUNK + SEL_LOOKAHEAD + 16 + 16) / 4;  // 15 B head + 8 B slack, 16-B multiple
+constexpr uint32_t STAGE_PAD = 32;  // zero bytes behind a staged chunk: the walks read up to a word step beyond it
+constexpr int SEL_STAGE_WORDS = (15 + SEL_CHUNK + SEL_LOOKAHEAD + STAGE_PAD + 15) / 16 * 4;  // head + chunk + k + pad, 16-B multiple
 
 struct SelSmem {
     uint32_t *cand;   // [cap]
@@ -67,11 +68,6 @@ __device__ __forceinline__ uint32_t smem_fetch_inc(uint32_t *p) {
     return old;
 }
 
-__device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) {  // shared-space load from a 32-bit shared address
-    uint32_t v;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(saddr));
-    return v;
-}
 __device__ __forceinline__ void stg_u32(uint32_t *p, uint32_t v) {
     asm volatile("st.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
@@ -247,10 +243,47 @@ __device__ bool final_bucket_sort(const SelSmem &m, uint32_t cnt, uint32_t s, ui
     return true;
 }
 
+// Final stage of a row: cand[0..cnt) holds a superset of the bottom-s multiset (cnt >= s); writes the ascending
+// bottom-s to dst.  The bucket sort-select, or, for degenerate value distributions, exact radix select to s and a
+// bitonic sort of the P (power of two >= s) words.  All threads must call.
+template <int NT>
+__device__ void finish_bottom_s(const SelSmem &m, uint32_t cnt, uint32_t s, uint32_t P, uint32_t *__restrict__ dst) {
+    if (final_bucket_sort<NT>(m, cnt, s, dst)) return;
+    const uint32_t tid = threadIdx.x;
+    if (cnt > s) prune_to_s<NT>(m, cnt, s);
+    for (uint32_t i = s + tid; i < P; i += NT) m.cand[i] = 0xffffffffu;
+    __syncthreads();
+    bitonic_sort<NT>(m.cand, P);
+    for (uint32_t i = tid; i < s; i += NT) dst[i] = m.cand[i];
+}
+
+// Stages the nbytes bytes at src (one chunk plus the k - 1 bytes its last k-mers reach into) at sb + (src & 15),
+// sb 16-byte aligned: the 16-byte aligned body by one bulk copy that completes on `bar` (thread 0 arms it), the
+// tail by plain loads, then STAGE_PAD zero bytes.  whole: at least 16 bytes behind the chunk still belong to the
+// sequence, so the body is rounded up, over-reads them and is the whole stage.  Otherwise the caller needs a
+// barrier between the plain stores and their readers.
+template <int NT>
+__device__ __forceinline__ void stage_chunk(uint8_t *sb, const uint8_t *src, uint32_t nbytes, bool whole, uint64_t *bar) {
+    const uint32_t head = (uint32_t)((uintptr_t)src & 15u);
+    const uint32_t body = whole ? (head + nbytes + 15u) & ~15u : (head + nbytes) & ~15u;
+    if (threadIdx.x == 0) {
+        mbar_expect_tx(bar, body);
+        if (body) bulk_g2s(sb, src - head, body, bar);
+    }
+    if (!whole)
+        for (uint32_t i = body + threadIdx.x; i < head + nbytes + STAGE_PAD; i += NT)
+            sb[i] = i < head + nbytes ? __ldg(src - head + i) : (uint8_t)0;
+}
+// Waits for the stage of chunk c, counted from the barriers' initialisation: chunk c lives in buffer c & 1, whose
+// barrier completes once per use, so the phase to wait for is (c >> 1) & 1.
+__device__ __forceinline__ void stage_wait(uint64_t *bars, uint32_t c) {
+    mbar_wait(&bars[c & 1u], (c >> 1) & 1u);
+}
+
 __global__ void __launch_bounds__(SEL_THREADS)
 sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ offsets,
                      uint32_t uniform_len, uint64_t n_reads, uint32_t k, uint32_t s, uint32_t P,
-                     uint32_t cap, uint32_t flags, uint32_t *__restrict__ out, uint64_t row_stride,
+                     uint32_t cap, uint32_t *__restrict__ out, uint64_t row_stride,
                      uint32_t *__restrict__ count, int32_t *__restrict__ status, const SketchDst extra) {
     extern __shared__ __align__(16) uint32_t smem_w[];
     SelSmem m;
@@ -263,7 +296,7 @@ sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restri
     m.tmpcap = (uint32_t)(m.hist - m.keep);
 
     __shared__ __align__(8) uint64_t s_bar[2];
-    uint32_t par0 = 0u, par1 = 0u;  // barrier parities (uniform across the CTA)
+    uint32_t chunk_idx = 0;  // chunks this CTA has staged (over all its rows): chunk c uses stage buffer c & 1
     const uint32_t tid = threadIdx.x;
     if (tid == 0) {
         mbar_init(&s_bar[0], 1);
@@ -275,25 +308,12 @@ sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restri
     const uint32_t tailmask = tail == 1 ? 0xffu : tail == 2 ? 0xffffu : 0xffffffu;
 
     for (uint64_t row = blockIdx.x; row < n_reads; row += gridDim.x) {
-        uint64_t beg, len;
-        if (offsets) {
-            beg = offsets[row];
-            len = offsets[row + 1] - beg;
-        } else {
-            beg = row * (uint64_t)uniform_len;
-            len = uniform_len;
-        }
-        const uint64_t n = len > k ? len - k : 0;
-        if (n < s || n == 0) continue;  // fill regime: other kernel
-        const uint8_t *seq = bases + beg;
+        const RowSpan sp = row_span(offsets, uniform_len, row, k);
+        const uint64_t n = sp.n;
+        if (!select_regime(n, s)) continue;  // fill regime: other kernel
+        const uint8_t *seq = bases + sp.beg;
         uint32_t *dst = out + row * row_stride;
-        if (s == 0) {  // mash.go:96 reads Sketches[-1] on the first k-mer
-            if (tid == 0) {
-                if (status) status[row] = PG_ITEM_PANIC;
-                if (count) count[row] = 0;
-            }
-            continue;
-        }
+        if (empty_sketch_panics(s, status, count, row)) continue;
 
         if (tid == 0) { m.misc[0] = 0; m.misc[5] = 0xffffffffu; }
         __syncthreads();
@@ -301,36 +321,19 @@ sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restri
         uint32_t h_first = 0;
 
         // chunk c lives in stage buffer c & 1; its copy is issued one iteration ahead
+        // bytes [c0, c0 + ch + k) of the read; the plain-stored tail is covered by the barrier after the wait
         auto issue_stage = [&](uint64_t c0, uint32_t buf) {
-            // bytes [c0, c0 + ch + k) of the read -> sb[head ..): 16-byte aligned body by TMA,
-            // the (< 16) trailing bytes and 8 bytes of zero slack by plain stores
-            const uint32_t ch = (uint32_t)min((uint64_t)SEL_CHUNK, n - c0);
-            const uint32_t nbytes = ch + k;
-            const uint8_t *src = seq + c0;
-            const uint32_t head = (uint32_t)((uintptr_t)src & 15u);
-            const uint32_t body = (head + nbytes) & ~15u;
-            uint8_t *sb = reinterpret_cast<uint8_t *>(m.bytes + buf * SEL_STAGE_WORDS);
-            if (tid == 0) {
-                if (body) {
-                    mbar_expect_tx(&s_bar[buf], body);
-                    bulk_g2s(sb, src - head, body, &s_bar[buf]);
-                } else {
-                    mbar_expect_tx(&s_bar[buf], 0);
-                }
-            }
-            for (uint32_t i = body + tid; i < head + nbytes + 8; i += SEL_THREADS)
-                sb[i] = i < head + nbytes ? __ldg(src - head + i) : (uint8_t)0;
+            stage_chunk<SEL_THREADS>(reinterpret_cast<uint8_t *>(m.bytes + buf * SEL_STAGE_WORDS), seq + c0,
+                                     (uint32_t)min((uint64_t)SEL_CHUNK, n - c0) + k, false, &s_bar[buf]);
         };
-        issue_stage(0, 0);
-        uint32_t chunk_idx = 0;
+        issue_stage(0, chunk_idx & 1u);
         for (uint64_t c0 = 0; c0 < n; c0 += SEL_CHUNK, ++chunk_idx) {
             const uint32_t ch = (uint32_t)min((uint64_t)SEL_CHUNK, n - c0);
             const uint32_t buf = chunk_idx & 1u;
             if (c0 + SEL_CHUNK < n) issue_stage(c0 + SEL_CHUNK, buf ^ 1u);  // previous user of that buffer finished last iteration
             const uint32_t head = (uint32_t)((uintptr_t)(seq + c0) & 15u);
             const uint32_t *stage = m.bytes + buf * SEL_STAGE_WORDS;
-            if (buf == 0) { mbar_wait(&s_bar[0], par0); par0 ^= 1u; }
-            else          { mbar_wait(&s_bar[1], par1); par1 ^= 1u; }
+            stage_wait(s_bar, chunk_idx);
             // make room: candidates after this chunk must fit
             uint32_t cnt = m.misc[0];
             __syncthreads();
@@ -378,30 +381,11 @@ sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restri
 
         uint32_t cnt = m.misc[0];
         __syncthreads();
-        if (!final_bucket_sort<SEL_THREADS>(m, cnt, s, dst)) {
-            if (cnt > s) prune_to_s<SEL_THREADS>(m, cnt, s);
-            for (uint32_t i = s + tid; i < P; i += SEL_THREADS) m.cand[i] = 0xffffffffu;
-            __syncthreads();
-            bitonic_sort<SEL_THREADS>(m.cand, P);
-            for (uint32_t i = tid; i < s; i += SEL_THREADS) dst[i] = m.cand[i];
-        }
-        // fused all-gather: replicate the finished row into the gathered buffer of every rank
-        if (extra.n > 0) {
-            __syncthreads();
-            for (int pr = 0; pr < extra.n; ++pr) {
-                uint32_t *peer = extra.ptr[pr] + row * row_stride;
-                if (peer == dst) continue;
-                for (uint32_t i = tid; i < s; i += SEL_THREADS) peer[i] = dst[i];
-            }
-        }
-        if (tid == 0) {
-            int32_t st = PG_ITEM_OK;
-            // s == 1: mash.go:96-98 indexes Sketches[-1] as soon as a later hash is
-            // strictly below Sketches[0]
-            if (s == 1 && m.misc[5] < h_first) st = PG_ITEM_PANIC;
-            if (status) status[row] = st;
-            if (count) count[row] = s;
-        }
+        finish_bottom_s<SEL_THREADS>(m, cnt, s, P, dst);
+        replicate_row<SEL_THREADS>(extra, row, row_stride, dst, dst, s);
+        // s == 1: mash.go:96-98 indexes Sketches[-1] as soon as a later hash is strictly below Sketches[0]
+        // (h_first is thread 0's, which alone writes the status)
+        put_row_status(status, count, row, s, s == 1 && m.misc[5] < h_first);
         __syncthreads();
     }
 }
@@ -443,14 +427,8 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
                           const uint64_t *__restrict__ slice_beg, const uint32_t *__restrict__ slice_n,
                           unsigned long long *__restrict__ next_row, const uint32_t *__restrict__ row_list,
                           const uint32_t *__restrict__ n_list) {
-    constexpr int NB = K / 4;
-    constexpr int TAIL = K % 4;
-    constexpr uint32_t TAILMASK = TAIL == 1 ? 0xffu : TAIL == 2 ? 0xffffu : 0xffffffu;
-    constexpr bool LUT = TAIL == 1;
+    PG_WALK_CONSTANTS;
     constexpr uint32_t k = K;
-    constexpr int ROTF = 0;
-    const uint32_t rotmul = 0;
-    static_assert(NB >= 1 && K <= 32, "walk path: 4 <= k <= 32");
     static_assert(SELW_SEG % 4 == 0, "a segment is a whole number of word steps");
 
     extern __shared__ __align__(16) uint32_t smem_w[];
@@ -464,18 +442,15 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
     m.tmpcap = (uint32_t)(m.hist - m.keep);
 
     __shared__ __align__(16) uint32_t s_lut[LUT ? 256 : 4];
-    __shared__ __align__(8) uint64_t s_bar[3];
-    uint32_t par0 = 0u, par1 = 0u;
+    __shared__ __align__(8) uint64_t s_bar[3];  // [0], [1]: stage buffers, [2]: the table
+    uint32_t chunk_idx = 0;  // chunks this CTA has staged (over all its rows): chunk c uses stage buffer c & 1
     const uint32_t tid = threadIdx.x;
     if (tid == 0) {
         mbar_init(&s_bar[0], 1);
         mbar_init(&s_bar[1], 1);
         mbar_init(&s_bar[2], 1);
         fence_mbar_init();
-        if (LUT) {
-            mbar_expect_tx(&s_bar[2], 1024u);
-            bulk_g2s(s_lut, &g_kmix_byte, 1024u, &s_bar[2]);
-        }
+        if (LUT) load_kmix_table(s_lut, &s_bar[2]);
     }
     __syncthreads();
     if (LUT) mbar_wait(&s_bar[2], 0);
@@ -499,26 +474,14 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
             beg = slice_beg[row];
             n = slice_n[row];
         } else {
-            uint64_t len;
-            if (offsets) {
-                beg = offsets[row];
-                len = offsets[row + 1] - beg;
-            } else {
-                beg = row * (uint64_t)uniform_len;
-                len = uniform_len;
-            }
-            n = len > k ? len - k : 0;
+            const RowSpan sp = row_span(offsets, uniform_len, row, k);
+            beg = sp.beg;
+            n = sp.n;
         }
-        if (n < s || n == 0) continue;  // fill regime: other kernel
+        if (!select_regime(n, s)) continue;  // fill regime: other kernel
         const uint8_t *seq = bases + beg;
         uint32_t *dst = out + row * row_stride;
-        if (s == 0) {  // mash.go:96 reads Sketches[-1] on the first k-mer
-            if (tid == 0) {
-                if (status) status[row] = PG_ITEM_PANIC;
-                if (count) count[row] = 0;
-            }
-            continue;
-        }
+        if (empty_sketch_panics(s, status, count, row)) continue;
         if (tid == 0) { m.misc[5] = 0xffffffffu; m.misc[8] = 0; m.misc[9] = 0; m.misc[10] = 0; }
         __syncthreads();
         uint64_t limit = 1ull << 32;  // admit h < limit
@@ -531,34 +494,17 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
         auto tail_by_tma = [&](uint64_t c0, uint32_t ch) { return n - (c0 + ch) >= 16; };
         auto issue_stage = [&](uint64_t c0, uint32_t buf) {
             const uint32_t ch = (uint32_t)min((uint64_t)SELW_CHUNK, n - c0);
-            const uint32_t nbytes = ch + k;
-            const uint8_t *src = seq + c0;
-            const uint32_t head = (uint32_t)((uintptr_t)src & 15u);
-            const bool all_tma = tail_by_tma(c0, ch);
-            const uint32_t body = all_tma ? (head + nbytes + 15u) & ~15u : (head + nbytes) & ~15u;
-            uint8_t *sb8 = reinterpret_cast<uint8_t *>(m.bytes + buf * SELW_STAGE_WORDS);
-            if (tid == 0) {
-                if (body) {
-                    mbar_expect_tx(&s_bar[buf], body);
-                    bulk_g2s(sb8, src - head, body, &s_bar[buf]);
-                } else {
-                    mbar_expect_tx(&s_bar[buf], 0);
-                }
-            }
-            if (!all_tma)
-                for (uint32_t i = body + tid; i < head + nbytes + 32; i += SELW_THREADS)  // tail + over-read pad
-                    sb8[i] = i < head + nbytes ? __ldg(src - head + i) : (uint8_t)0;
+            stage_chunk<SELW_THREADS>(reinterpret_cast<uint8_t *>(m.bytes + buf * SELW_STAGE_WORDS), seq + c0, ch + k,
+                                      tail_by_tma(c0, ch), &s_bar[buf]);
         };
-        issue_stage(0, 0);
-        uint32_t chunk_idx = 0;
+        issue_stage(0, chunk_idx & 1u);
         for (uint64_t c0 = 0; c0 < n; c0 += SELW_CHUNK, ++chunk_idx) {
             const uint32_t ch = (uint32_t)min((uint64_t)SELW_CHUNK, n - c0);
             const uint32_t buf = chunk_idx & 1u;
             if (c0 + SELW_CHUNK < n) issue_stage(c0 + SELW_CHUNK, buf ^ 1u);  // its last readers passed the barrier below
             const uint32_t head = (uint32_t)((uintptr_t)(seq + c0) & 15u);
             const uint8_t *stage = reinterpret_cast<const uint8_t *>(m.bytes + buf * SELW_STAGE_WORDS);
-            if (buf == 0) { mbar_wait(&s_bar[0], par0); par0 ^= 1u; }
-            else          { mbar_wait(&s_bar[1], par1); par1 ^= 1u; }
+            stage_wait(s_bar, chunk_idx);
             if (!tail_by_tma(c0, ch)) __syncthreads();  // plain-store part of this stage
             if (cnt + ch > cap) {  // worst case every hash of the chunk is admitted
                 limit = prune_to_s<SELW_THREADS>(m, cnt, s);
@@ -579,24 +525,7 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
                 const uint32_t sh = (b0 & 3u) * 8u;
                 uint32_t *my_out = m.cand + cnt + tid;  // transposed target (full chunk, unfiltered)
                 uint32_t *my_pos = m.cand + cnt + seg;  // positional target (partial chunk, unfiltered)
-                uint32_t raw_a = sw[0], raw_b = sw[1];
-                uint32_t w_cur = __funnelshift_r(raw_a, raw_b, sh);
-                raw_a = raw_b; raw_b = sw[2];
-                uint32_t w_nxt = __funnelshift_r(raw_a, raw_b, sh);
-                raw_a = raw_b; raw_b = sw[3];
-                const uint32_t *swp = sw + 4;
-                uint32_t ring[4][NB];
-#pragma unroll
-                for (int q = 0; q < NB; ++q) {
-                    ring[0][q] = mm3_kmix(w_cur);
-                    ring[1][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 8));
-                    ring[2][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 16));
-                    ring[3][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 24));
-                    w_cur = w_nxt;
-                    w_nxt = __funnelshift_r(raw_a, raw_b, sh);
-                    raw_a = raw_b;
-                    raw_b = *swp++;
-                }
+                PG_WALK_PROLOGUE
                 uint32_t i = 0;
     // a full segment is SELW_SEG / 4 word steps with no bounds tests; the last segment of a chunk is checked
 #define PG_WALK_SEGMENT(EMIT)                                                          \
@@ -626,29 +555,9 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
             if (tid == 0) m.misc[8 + (chunk_idx + 2) % 3u] = 0;  // next use: chunk_idx + 2, after the next barrier
         }
         __syncthreads();
-        if (!final_bucket_sort<SELW_THREADS>(m, cnt, s, dst)) {
-            if (cnt > s) prune_to_s<SELW_THREADS>(m, cnt, s);
-            for (uint32_t i = s + tid; i < P; i += SELW_THREADS) m.cand[i] = 0xffffffffu;
-            __syncthreads();
-            bitonic_sort<SELW_THREADS>(m.cand, P);
-            for (uint32_t i = tid; i < s; i += SELW_THREADS) dst[i] = m.cand[i];
-        }
-        if (extra.n > 0) {  // fused all-gather: replicate the finished row into every rank's buffer
-            __syncthreads();
-#pragma unroll
-            for (int pr = 0; pr < PG_MAX_PEERS; ++pr) {  // static indices: the struct stays in parameter space
-                if (pr >= extra.n) continue;
-                uint32_t *peer = extra.ptr[pr] + row * row_stride;
-                if (peer == dst) continue;
-                for (uint32_t i = tid; i < s; i += SELW_THREADS) peer[i] = dst[i];
-            }
-        }
-        if (tid == 0) {
-            int32_t st = PG_ITEM_OK;
-            if (s == 1 && m.misc[5] < h_first) st = PG_ITEM_PANIC;
-            if (status) status[row] = st;
-            if (count) count[row] = s;
-        }
+        finish_bottom_s<SELW_THREADS>(m, cnt, s, P, dst);
+        replicate_row<SELW_THREADS>(extra, row, row_stride, dst, dst, s);
+        put_row_status(status, count, row, s, s == 1 && m.misc[5] < h_first);  // as in sketch_select_kernel
         __syncthreads();
     }
 }
@@ -715,18 +624,9 @@ select_merge_kernel(const uint32_t *__restrict__ part, const uint32_t *__restric
             }
             const uint32_t cnt = m.misc[0];
             __syncthreads();
-            if (!final_bucket_sort<SELM_THREADS>(m, cnt, s, dst)) {
-                if (cnt > s) prune_to_s<SELM_THREADS>(m, cnt, s);
-                for (uint32_t i = s + tid; i < P; i += SELM_THREADS) m.cand[i] = 0xffffffffu;
-                __syncthreads();
-                bitonic_sort<SELM_THREADS>(m.cand, P);
-                for (uint32_t i = tid; i < s; i += SELM_THREADS) dst[i] = m.cand[i];
-            }
+            finish_bottom_s<SELM_THREADS>(m, cnt, s, P, dst);
         }
-        if (tid == 0) {
-            if (status) status[row] = PG_ITEM_OK;
-            if (count) count[row] = s;
-        }
+        put_row_status(status, count, row, s, false);
         __syncthreads();
     }
 }
@@ -738,7 +638,7 @@ select_merge_kernel(const uint32_t *__restrict__ part, const uint32_t *__restric
 // the mean -- and whether it did is CHECKED, never assumed: a row whose admitted count is < s (few
 // distinct k-mers) or exceeds its buffer (heavy duplication below T) is redone by the exact streaming
 // kernel above (retry list built on the device, no host round trip).  So:
-//   A. sketch_thresh_walk_kernel<K, RARE, ROLLED>: one WARP per work item (<= 8 chunks of 32 x SEG
+//   A. sketch_thresh_walk_kernel<K, RARE>: one WARP per work item (<= 8 chunks of 32 x SEG
 //      positions of one row, SeltGeom<K>; long sequences become many items, so there is no host-side
 //      slicing and no merge pass).  Chunks arrive by double-buffered 1-D TMA bulk copies; lane l walks SEG
 //      consecutive k-mers with the register ring of kmer_walk.cuh (one ring prologue per SEG k-mers
@@ -764,9 +664,6 @@ struct SeltGeom {
     static_assert(STEPS % 2 == 1 && (NB % 2 == 0 || STEPS % NB == 0), "segment geometry");
 };
 constexpr int SELT_ITEM_CHUNKS = 8;
-// rolled body (groups of 3 steps, then a ring rotation) from NB = 6 (k >= 24) on; k = 21 (NB = 5) keeps the unrolled 5-step
-// body, which is short enough not to stall on instruction fetch
-#define SELT_ROLLED_DEFAULT(K_) ((K_) / 4 >= 6)
 constexpr int SELT_SEL_THREADS = 256;
 
 __host__ __device__ __forceinline__ uint32_t selt_threshold_m1(uint64_t n, uint32_t mu) {
@@ -800,19 +697,17 @@ __device__ __forceinline__ void strip_advance_if_le(uint32_t &saddr, uint32_t h,
         }                                                                                \
     }
 
-template <int K, bool RARE, bool ROLLED>
+template <int K, bool RARE>
 __global__ void __launch_bounds__(32)
 sketch_thresh_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ offsets, uint32_t uniform_len,
                           uint64_t row0, uint64_t n_rows, uint32_t items_per_row, uint32_t s, uint32_t mu, uint32_t cap,
                           uint32_t *__restrict__ gcand, uint32_t *__restrict__ gcnt, uint32_t lut_stride, uint32_t tm1_uniform) {
-    constexpr int NB = K / 4;
-    constexpr int TAIL = K % 4;
-    constexpr uint32_t TAILMASK = TAIL == 1 ? 0xffu : TAIL == 2 ? 0xffffu : 0xffffffu;
-    constexpr bool LUT = TAIL == 1;
+    PG_WALK_CONSTANTS;
     constexpr uint32_t k = K;
-    constexpr int ROTF = 0;
-    const uint32_t rotmul = 0;
-    static_assert(NB >= 1 && K <= 32, "walk path: 4 <= k <= 32");
+    // Loop shape: from NB = 6 (k >= 24) on, groups of 3 steps of code with the ring rotated after each group, so the
+    // body fits the instruction cache; below, the unrolled NB-step body (k = 21: 5 steps), short enough not to
+    // stall on instruction fetch.
+    constexpr bool ROLLED = NB >= 6;
     constexpr int SELT_SEG = SeltGeom<K>::SEG, SELT_CHUNK = SeltGeom<K>::CHUNK, SELT_STAGE_BYTES = SeltGeom<K>::STAGE;
 
     extern __shared__ __align__(128) uint8_t smem[];  // 2 stage buffers | strip [SELT_SEG][32]
@@ -823,20 +718,13 @@ sketch_thresh_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
     const uint64_t lrow = item / items_per_row;  // row within this launch group
     if (lrow >= n_rows) return;
     const uint64_t row = row0 + lrow;
-    uint64_t beg, len;
-    if (offsets) {
-        beg = offsets[row];
-        len = offsets[row + 1] - beg;
-    } else {
-        beg = row * (uint64_t)uniform_len;
-        len = uniform_len;
-    }
-    const uint64_t n = len > k ? len - k : 0;
-    if (n < s || n == 0) return;  // fill regime: other kernel
+    const RowSpan sp = row_span(offsets, uniform_len, row, k);
+    const uint64_t n = sp.n;
+    if (!select_regime(n, s)) return;  // fill regime: other kernel
     const uint64_t p0 = (uint64_t)(item % items_per_row) * (uint64_t)(SELT_ITEM_CHUNKS * SELT_CHUNK);
     if (p0 >= n) return;
     const uint64_t p1 = min(n, p0 + (uint64_t)(SELT_ITEM_CHUNKS * SELT_CHUNK));
-    const uint8_t *seq = bases + beg;
+    const uint8_t *seq = bases + sp.beg;
     const uint32_t tm1 = offsets ? selt_threshold_m1(n, mu) : tm1_uniform;  // fixed-length reads: computed once on the host
     uint32_t *my_cand = gcand + lrow * (uint64_t)cap;
     uint32_t *strip = reinterpret_cast<uint32_t *>(smem + 2 * SELT_STAGE_BYTES);
@@ -848,37 +736,22 @@ sketch_thresh_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
         mbar_init(&s_bar[1], 1);
         mbar_init(&s_bar[2], 1);
         fence_mbar_init();
-        if (LUT) {
-            mbar_expect_tx(&s_bar[2], 1024u);
-            bulk_g2s(s_lut, &g_kmix_byte, 1024u, &s_bar[2]);
-        }
+        if (LUT) load_kmix_table(s_lut, &s_bar[2]);
     }
     __syncwarp();
     const uint32_t lut_base = smem_u32(s_lut);
 
-    // A chunk that is not the last of its row may over-read up to 15 bytes (they belong to the same
-    // sequence): the whole stage is then one TMA copy.  Otherwise the 16-byte aligned body comes by
-    // TMA and the tail by plain loads.
+    // A chunk may over-read up to 15 bytes when they still belong to the sequence (even beyond the item end p1):
+    // the whole stage is then one TMA copy.  Otherwise the 16-byte aligned body comes by TMA and the tail by
+    // plain loads.
     auto tail_by_tma = [&](uint64_t c0, uint32_t ch) { return n - (c0 + ch) >= 16; };
     auto issue_stage = [&](uint64_t c0, uint32_t buf) {
         const uint32_t ch = (uint32_t)min((uint64_t)SELT_CHUNK, p1 - c0);
-        const uint32_t nbytes = ch + k;
-        const uint8_t *src = seq + c0;
-        const uint32_t head = (uint32_t)((uintptr_t)src & 15u);
-        const bool all_tma = tail_by_tma(c0, ch);
-        const uint32_t body = all_tma ? (head + nbytes + 15u) & ~15u : (head + nbytes) & ~15u;
-        uint8_t *sb8 = smem + buf * SELT_STAGE_BYTES;
-        if (lane == 0) {
-            mbar_expect_tx(&s_bar[buf], body);
-            if (body) bulk_g2s(sb8, src - head, body, &s_bar[buf]);
-        }
-        if (!all_tma)
-            for (uint32_t i = body + lane; i < head + nbytes + 32; i += 32)  // tail + over-read pad
-                sb8[i] = i < head + nbytes ? __ldg(src - head + i) : (uint8_t)0;
+        stage_chunk<32>(smem + buf * SELT_STAGE_BYTES, seq + c0, ch + k, tail_by_tma(c0, ch), &s_bar[buf]);
     };
     issue_stage(p0, 0);
     if (LUT) mbar_wait(&s_bar[2], 0);
-    uint32_t par0 = 0u, par1 = 0u, chunk_idx = 0;
+    uint32_t chunk_idx = 0;
     for (uint64_t c0 = p0; c0 < p1; c0 += SELT_CHUNK, ++chunk_idx) {
         const uint32_t ch = (uint32_t)min((uint64_t)SELT_CHUNK, p1 - c0);
         const uint32_t buf = chunk_idx & 1u;
@@ -886,8 +759,7 @@ sketch_thresh_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
         if (c0 + SELT_CHUNK < p1) issue_stage(c0 + SELT_CHUNK, buf ^ 1u);
         const uint32_t head = (uint32_t)((uintptr_t)(seq + c0) & 15u);
         const uint8_t *stage = smem + buf * SELT_STAGE_BYTES;
-        if (buf == 0) { mbar_wait(&s_bar[0], par0); par0 ^= 1u; }
-        else          { mbar_wait(&s_bar[1], par1); par1 ^= 1u; }
+        stage_wait(s_bar, chunk_idx);
         if (!tail_by_tma(c0, ch)) __syncwarp();  // plain-store part of this stage
 
         uint32_t sa = sa0;  // shared address of the lane's next strip slot: (sa - sa0) / 128 hashes admitted in this chunk
@@ -907,31 +779,14 @@ sketch_thresh_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
             const uint32_t *sw = reinterpret_cast<const uint32_t *>(stage) + (b0 >> 2);
             const uint8_t *sb = stage + b0 + 4 * NB;
             const uint32_t sh = (b0 & 3u) * 8u;
-            uint32_t raw_a = sw[0], raw_b = sw[1];
-            uint32_t w_cur = __funnelshift_r(raw_a, raw_b, sh);
-            raw_a = raw_b; raw_b = sw[2];
-            uint32_t w_nxt = __funnelshift_r(raw_a, raw_b, sh);
-            raw_a = raw_b; raw_b = sw[3];
-            const uint32_t *swp = sw + 4;
-            uint32_t ring[4][NB];
-#pragma unroll
-            for (int q = 0; q < NB; ++q) {
-                ring[0][q] = mm3_kmix(w_cur);
-                ring[1][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 8));
-                ring[2][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 16));
-                ring[3][q] = mm3_kmix(__funnelshift_r(w_cur, w_nxt, 24));
-                w_cur = w_nxt;
-                w_nxt = __funnelshift_r(raw_a, raw_b, sh);
-                raw_a = raw_b;
-                raw_b = *swp++;
-            }
+            PG_WALK_PROLOGUE
             // whole groups of NB word steps without bounds tests, then < NB checked steps: the loop body is
             // NB steps of code (it stays in the instruction cache) instead of a fully unrolled segment
             uint32_t i = 0;
-            if (ROLLED) {  // groups of 3 steps of code with the ring rotated after each group: the body fits the instruction cache
+            if constexpr (ROLLED) {
                 const uint32_t n_full = nk & ~3u;
                 const uint32_t n_grp = (nk / 12u) * 12u;
-                if (RARE) {
+                if constexpr (RARE) {
 #pragma unroll 1
                     while (i < n_grp) {
                         PG_KMER_STEP(0, false, PG_EMIT_STRIP_RARE)
@@ -953,7 +808,7 @@ sketch_thresh_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
                 if (i < nk) PG_KMER_STEP_ROLLED(true, PG_EMIT_STRIP)
             } else {
                 const uint32_t n_main = (nk / (4 * NB)) * (4 * NB);
-                if (RARE) {
+                if constexpr (RARE) {
 #pragma unroll 1
                     while (i < n_main) {
 #pragma unroll
@@ -1032,11 +887,8 @@ sketch_thresh_select_kernel(const uint64_t *__restrict__ offsets, uint32_t unifo
     const uint32_t tid = threadIdx.x;
     for (uint64_t lrow = blockIdx.x; lrow < n_rows; lrow += gridDim.x) {
         const uint64_t row = row0 + lrow;
-        uint64_t len;
-        if (offsets) len = offsets[row + 1] - offsets[row];
-        else len = uniform_len;
-        const uint64_t n = len > k ? len - k : 0;
-        if (n < s || n == 0) continue;  // fill regime: other kernel
+        const uint64_t n = row_span(offsets, uniform_len, row, k).n;
+        if (!select_regime(n, s)) continue;  // fill regime: other kernel
         const uint32_t cnt = gcnt[lrow];
         if (cnt < s || cnt > cap) {  // the estimate did not hold for this row: exact streaming kernel redoes it
             if (tid == 0) retry_rows[atomicAdd(n_retry, 1u)] = (uint32_t)row;
@@ -1133,22 +985,18 @@ sketch_thresh_select_kernel(const uint64_t *__restrict__ offsets, uint32_t unifo
                 }
             }
         }
-        if (extra.n > 0) {  // fused all-gather: replicate the finished row into every rank's buffer
-            __syncthreads();
-#pragma unroll
-            for (int pr = 0; pr < PG_MAX_PEERS; ++pr) {
-                if (pr >= extra.n) continue;
-                uint32_t *peer = extra.ptr[pr] + row * row_stride;
-                if (peer == dst) continue;
-                for (uint32_t i = tid; i < s; i += SELT_SEL_THREADS) peer[i] = dst[i];
-            }
-        }
-        if (tid == 0) {
-            if (status) status[row] = PG_ITEM_OK;
-            if (count) count[row] = s;
-        }
+        replicate_row<SELT_SEL_THREADS>(extra, row, row_stride, dst, dst, s);
+        put_row_status(status, count, row, s, false);
         __syncthreads();
     }
+}
+
+// the stage B instantiation for select batch width U (one of 3, 4, 5, 6, 8)
+template <bool MUL>
+static auto thresh_select_fn(int u) {
+    return u == 3 ? sketch_thresh_select_kernel<3, MUL> : u == 4 ? sketch_thresh_select_kernel<4, MUL>
+         : u == 5 ? sketch_thresh_select_kernel<5, MUL> : u == 6 ? sketch_thresh_select_kernel<6, MUL>
+                  : sketch_thresh_select_kernel<8, MUL>;
 }
 
 template <int K>
@@ -1269,12 +1117,8 @@ static int launch_select_thresh(const uint8_t *d_bases, const uint64_t *d_offset
     // admission probability of the longest rows: below 1/512 a warp step (128 hashes) admits something a quarter of the time
     const uint32_t tm1_u = d_offsets ? 0u : selt_threshold_m1(nmax, mu);  // every row of a fixed-length batch has n == nmax
     const bool rare = (uint64_t)mu * 512 < nmax;
-    // PG_K2T_ROLLED=1: 3-step loop body with the ring rotated by register moves, =0: NB-step body (A/B and test knob)
-    const int rolled_env = [] { const char *e = getenv("PG_K2T_ROLLED"); return e ? atoi(e) : -1; }();
-    const bool rolled = K / 4 >= 3 && (rolled_env >= 0 ? rolled_env != 0 : SELT_ROLLED_DEFAULT(K));  // the 3-step group needs NB >= 3
-    const void *walk_fn = rare ? (rolled ? (const void *)sketch_thresh_walk_kernel<K, true, true> : (const void *)sketch_thresh_walk_kernel<K, true, false>)
-                               : (rolled ? (const void *)sketch_thresh_walk_kernel<K, false, true> : (const void *)sketch_thresh_walk_kernel<K, false, false>);
-    { const int rc_ = func_smem(walk_fn, smem_a); if (rc_ != PG_OK) return rc_; }
+    const auto walk_fn = rare ? sketch_thresh_walk_kernel<K, true> : sketch_thresh_walk_kernel<K, false>;
+    { const int rc_ = func_smem((const void *)walk_fn, smem_a); if (rc_ != PG_OK) return rc_; }
     // batch width of the select: fewest load slots for a typical row (mu + 2.5 sigma candidates), ties to the wider batch
     const uint32_t typ = mu + (uint32_t)(2.5 * sqrt((double)mu));
     int sel_u = 8;
@@ -1285,20 +1129,14 @@ static int launch_select_thresh(const uint8_t *d_bases, const uint64_t *d_offset
             if (slots <= best) { best = slots; sel_u = u; }
         }
     }
-    const int sel_u_env = [] { const char *e = getenv("PG_K2T_SEL_U"); return e ? atoi(e) : 0; }();      // A/B and test knobs, read per call
-    const int sel_mul_env = [] { const char *e = getenv("PG_K2T_SEL_MUL"); return e ? atoi(e) : -1; }();
-    if (sel_u_env == 3 || sel_u_env == 4 || sel_u_env == 5 || sel_u_env == 6 || sel_u_env == 8) sel_u = sel_u_env;
     // bucket function: the plain shift when it uses >= 3/4 of the 2048 buckets (fixed-length batch: T known here)
     bool sel_mul = true;
     if (!d_offsets) {
         const uint32_t tb = 32u - (uint32_t)__builtin_clz(tm1_u | 1u);
         sel_mul = ((tm1_u >> (tb > 11u ? tb - 11u : 0u)) + 1u) < 1536u;
     }
-    if (sel_mul_env >= 0) sel_mul = sel_mul_env != 0;
-#define PG_SEL_FN(U_) (sel_mul ? (const void *)sketch_thresh_select_kernel<U_, true> : (const void *)sketch_thresh_select_kernel<U_, false>)
-    const void *sel_fn = sel_u == 3 ? PG_SEL_FN(3) : sel_u == 4 ? PG_SEL_FN(4) : sel_u == 5 ? PG_SEL_FN(5) : sel_u == 6 ? PG_SEL_FN(6) : PG_SEL_FN(8);
-#undef PG_SEL_FN
-    { const int rc_ = func_smem(sel_fn, smem_b); if (rc_ != PG_OK) return rc_; }
+    const auto sel_fn = sel_mul ? thresh_select_fn<true>(sel_u) : thresh_select_fn<false>(sel_u);
+    { const int rc_ = func_smem((const void *)sel_fn, smem_b); if (rc_ != PG_OK) return rc_; }
     int per_sm = 1;
     PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sel_fn, SELT_SEL_THREADS, smem_b));
     // candidate lists: cap words per row, rows in groups of <= 1.5 GiB of temporaries
@@ -1316,30 +1154,12 @@ static int launch_select_thresh(const uint8_t *d_bases, const uint64_t *d_offset
     for (uint64_t r0 = 0; r0 < n_reads; r0 += group) {
         const uint64_t rows = std::min(group, n_reads - r0);
         PG_CUDA(cudaMemsetAsync(d_cnt, 0, rows * 4, st));
-#define PG_LAUNCH_WALK(RARE_, ROLLED_)                                                                                     \
-    sketch_thresh_walk_kernel<K, RARE_, ROLLED_><<<(unsigned)(rows * ipr), 32, smem_a, st>>>(d_bases, d_offsets, read_len, r0, rows, \
-                                                                                            (uint32_t)ipr, (uint32_t)s, mu, cap, d_cand, d_cnt, 4u, tm1_u)
-        if (rare && rolled) PG_LAUNCH_WALK(true, true);
-        else if (rare) PG_LAUNCH_WALK(true, false);
-        else if (rolled) PG_LAUNCH_WALK(false, true);
-        else PG_LAUNCH_WALK(false, false);
-#undef PG_LAUNCH_WALK
+        walk_fn<<<(unsigned)(rows * ipr), 32, smem_a, st>>>(d_bases, d_offsets, read_len, r0, rows, (uint32_t)ipr, (uint32_t)s, mu, cap,
+                                                            d_cand, d_cnt, 4u, tm1_u);
         PG_LAUNCH_CHECK("sketch_thresh_walk_kernel");
         const uint64_t blocks = std::min<uint64_t>(rows, (uint64_t)sm_count() * std::max(per_sm, 1));
-#define PG_LAUNCH_SEL_(U_, M_)                                                                                                 \
-    sketch_thresh_select_kernel<U_, M_><<<(unsigned)blocks, SELT_SEL_THREADS, smem_b, st>>>(d_offsets, read_len, r0, rows, (uint32_t)K, (uint32_t)s, \
-                                                                                             mu, cap, d_cand, d_cnt, d_out, row_stride, d_count,     \
-                                                                                             d_status, ex, d_retry, d_nretry, tm1_u)
-#define PG_LAUNCH_SEL(U_) do { if (sel_mul) PG_LAUNCH_SEL_(U_, true); else PG_LAUNCH_SEL_(U_, false); } while (0)
-        switch (sel_u) {
-            case 3: PG_LAUNCH_SEL(3); break;
-            case 4: PG_LAUNCH_SEL(4); break;
-            case 5: PG_LAUNCH_SEL(5); break;
-            case 6: PG_LAUNCH_SEL(6); break;
-            default: PG_LAUNCH_SEL(8); break;
-        }
-#undef PG_LAUNCH_SEL
-#undef PG_LAUNCH_SEL_
+        sel_fn<<<(unsigned)blocks, SELT_SEL_THREADS, smem_b, st>>>(d_offsets, read_len, r0, rows, (uint32_t)K, (uint32_t)s, mu, cap, d_cand,
+                                                                    d_cnt, d_out, row_stride, d_count, d_status, ex, d_retry, d_nretry, tm1_u);
         PG_LAUNCH_CHECK("sketch_thresh_select_kernel");
     }
     // rows the estimate failed on (few distinct k-mers, heavy duplication): exact streaming kernel, device-side list
@@ -1354,15 +1174,11 @@ template <int K>
 static int launch_select_auto(const uint8_t *d_bases, const uint64_t *d_offsets, uint32_t read_len, uint64_t max_read_len, uint64_t n_reads, int s,
                               uint32_t P, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, int32_t *d_status,
                               cudaStream_t st, const SketchDst &ex) {
-    static const bool no_slices = [] { const char *e = getenv("PG_K2_NO_SLICES"); return e && atoi(e) != 0; }();
-    static const bool no_thresh = [] { const char *e = getenv("PG_K2_NO_THRESH"); return e && atoi(e) != 0; }();  // A/B knob
-    if (!no_thresh) {
-        bool handled = false;
-        const int rc = launch_select_thresh<K>(d_bases, d_offsets, read_len, max_read_len, n_reads, s, P, d_out, row_stride, d_count, d_status, st,
-                                               ex, &handled);
-        if (rc != PG_OK || handled) return rc;
-    }
-    if (ex.n == 0 && !no_slices) {
+    bool handled = false;
+    const int rc = launch_select_thresh<K>(d_bases, d_offsets, read_len, max_read_len, n_reads, s, P, d_out, row_stride, d_count, d_status, st,
+                                           ex, &handled);
+    if (rc != PG_OK || handled) return rc;
+    if (ex.n == 0) {
         bool sliced = false;
         const int rc = try_select_sliced<K>(d_bases, d_offsets, read_len, n_reads, s, P, d_out, row_stride, d_count, d_status, st, &sliced);
         if (rc != PG_OK || sliced) return rc;
@@ -1373,7 +1189,7 @@ static int launch_select_auto(const uint8_t *d_bases, const uint64_t *d_offsets,
 }  // namespace
 
 int launch_sketch_select(const uint8_t *d_bases, const uint64_t *d_offsets, uint32_t read_len,
-                         uint64_t n_reads, int k, int s, uint32_t flags, uint32_t *d_out,
+                         uint64_t n_reads, int k, int s, uint32_t *d_out,
                          uint64_t row_stride, uint32_t *d_count, int32_t *d_status,
                          cudaStream_t st, const SketchDst *extra, uint64_t max_read_len) {
     if (n_reads == 0) return PG_OK;
@@ -1390,18 +1206,15 @@ int launch_sketch_select(const uint8_t *d_bases, const uint64_t *d_offsets, uint
     uint32_t P = 1;
     while (P < (uint32_t)std::max(s, 1)) P <<= 1;
     if (P < 2) P = 2;
-    // K2w (register-ring walk) for the instantiated k; PG_K2_GENERIC=1 forces the generic kernel (A/B knob)
-    static const bool force_generic = [] { const char *e = getenv("PG_K2_GENERIC"); return e && atoi(e) != 0; }();
-    if (!force_generic && (size_t)s * 8 + 56 * 1024 <= 227 * 1024) {  // shared memory of the walk kernel
-        switch (k) {
+    // the walk kernels (K2t, K2w) for the instantiated k
+    switch (k) {
 #define PG_K2W_CASE(KK) \
     case KK: return launch_select_auto<KK>(d_bases, d_offsets, read_len, max_read_len, n_reads, s, P, d_out, row_stride, d_count, d_status, st, ex);
-            PG_K2W_CASE(11) PG_K2W_CASE(13) PG_K2W_CASE(15) PG_K2W_CASE(16) PG_K2W_CASE(17) PG_K2W_CASE(19)
-            PG_K2W_CASE(21) PG_K2W_CASE(23) PG_K2W_CASE(24) PG_K2W_CASE(25) PG_K2W_CASE(27) PG_K2W_CASE(29)
-            PG_K2W_CASE(31) PG_K2W_CASE(32)
+        PG_K2W_CASE(11) PG_K2W_CASE(13) PG_K2W_CASE(15) PG_K2W_CASE(16) PG_K2W_CASE(17) PG_K2W_CASE(19)
+        PG_K2W_CASE(21) PG_K2W_CASE(23) PG_K2W_CASE(24) PG_K2W_CASE(25) PG_K2W_CASE(27) PG_K2W_CASE(29)
+        PG_K2W_CASE(31) PG_K2W_CASE(32)
 #undef PG_K2W_CASE
-            default: break;
-        }
+        default: break;
     }
     uint32_t cap = (std::max<uint32_t>(P, (uint32_t)s + 4 * SEL_CHUNK) + 3u) & ~3u;
     const size_t words = (size_t)cap + (((size_t)s + 3) & ~(size_t)3) + 4 + (SEL_CHUNK + SEL_LOOKAHEAD) +
@@ -1412,7 +1225,7 @@ int launch_sketch_select(const uint8_t *d_bases, const uint64_t *d_offsets, uint
     PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sketch_select_kernel, SEL_THREADS, smem));
     const uint64_t blocks = std::min<uint64_t>(n_reads, (uint64_t)sm_count() * std::max(per_sm, 1));  // one wave, grid-stride over rows
     sketch_select_kernel<<<(unsigned)blocks, SEL_THREADS, smem, st>>>(
-        d_bases, d_offsets, read_len, n_reads, (uint32_t)k, (uint32_t)s, P, cap, flags, d_out,
+        d_bases, d_offsets, read_len, n_reads, (uint32_t)k, (uint32_t)s, P, cap, d_out,
         row_stride, d_count, d_status, ex);
     PG_LAUNCH_CHECK("sketch_select_kernel");
     return PG_OK;

@@ -26,28 +26,17 @@ constexpr uint32_t LG_CHUNK = 8192;   // k-mer positions per hashing work item
 constexpr int LG_THREADS = 1024;
 constexpr uint32_t LG_TILE = 8192;    // words of the sort buffer one shared-memory tile holds
 
-__device__ __forceinline__ void row_span(const uint64_t *offsets, uint32_t uniform_len, uint64_t row, uint64_t *beg, uint64_t *len) {
-    if (offsets) {
-        *beg = offsets[row];
-        *len = offsets[row + 1] - *beg;
-    } else {
-        *beg = row * (uint64_t)uniform_len;
-        *len = uniform_len;
-    }
-}
-
 __global__ void __launch_bounds__(LG_HASH_THREADS)
 large_hash_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ offsets, uint32_t uniform_len, uint64_t row0,
                   uint64_t n_items, uint32_t chunks_per_row, uint32_t k, uint32_t s, uint64_t base_off, uint32_t *__restrict__ tmp) {
     for (uint64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
         const uint64_t row = row0 + item / chunks_per_row;
         const uint64_t i0 = (item % chunks_per_row) * (uint64_t)LG_CHUNK;
-        uint64_t beg, len;
-        row_span(offsets, uniform_len, row, &beg, &len);
-        const uint64_t n = len > k ? len - k : 0;
-        if (n < s || n == 0 || i0 >= n) continue;  // fill regime rows belong to the other kernel
-        const uint8_t *seq = bases + beg;
-        uint32_t *dst = tmp + (beg - base_off);
+        const RowSpan sp = row_span(offsets, uniform_len, row, k);
+        const uint64_t n = sp.n;
+        if (!select_regime(n, s) || i0 >= n) continue;  // fill regime rows belong to the other kernel
+        const uint8_t *seq = bases + sp.beg;
+        uint32_t *dst = tmp + (sp.beg - base_off);
         const uint64_t i1 = min(n, i0 + (uint64_t)LG_CHUNK);
         for (uint64_t i = i0 + threadIdx.x; i < i1; i += LG_HASH_THREADS) {
             const uint8_t *p = seq + i;
@@ -71,7 +60,8 @@ __device__ __forceinline__ void bitonic_tile(uint32_t *tile, uint32_t words, uin
     }
 }
 
-__global__ void __launch_bounds__(LG_THREADS)
+// Two CTAs per SM, as the launcher's grid assumes (left to itself ptxas takes 56 registers: one CTA per SM).
+__global__ void __launch_bounds__(LG_THREADS, 2)
 large_select_kernel(const uint64_t *__restrict__ offsets, uint32_t uniform_len, uint64_t row0, uint64_t n_rows, uint32_t k, uint32_t s,
                     uint64_t P, uint64_t base_off, const uint32_t *__restrict__ tmp, uint32_t *__restrict__ sortbuf,
                     uint32_t *__restrict__ out, uint64_t row_stride, uint32_t *__restrict__ count, int32_t *__restrict__ status,
@@ -83,18 +73,11 @@ large_select_kernel(const uint64_t *__restrict__ offsets, uint32_t uniform_len, 
     const uint32_t tid = threadIdx.x, lane = tid & 31u;
     for (uint64_t lrow = blockIdx.x; lrow < n_rows; lrow += gridDim.x) {
         const uint64_t row = row0 + lrow;
-        uint64_t beg, len;
-        row_span(offsets, uniform_len, row, &beg, &len);
-        const uint64_t n = len > k ? len - k : 0;
-        if (n < s || n == 0) continue;
-        if (s == 0) {  // mash.go:96 reads Sketches[-1] on the first k-mer
-            if (tid == 0) {
-                if (status) status[row] = PG_ITEM_PANIC;
-                if (count) count[row] = 0;
-            }
-            continue;
-        }
-        const uint32_t *src = tmp + (beg - base_off);
+        const RowSpan sp = row_span(offsets, uniform_len, row, k);
+        const uint64_t n = sp.n;
+        if (!select_regime(n, s)) continue;
+        if (empty_sketch_panics(s, status, count, row)) continue;
+        const uint32_t *src = tmp + (sp.beg - base_off);
         uint32_t *sb = sortbuf + lrow * P;
         uint32_t *dst = out + row * row_stride;
         // ---- exact radix select: v* = the s-th smallest hash, need_eq = copies of v* among the s smallest ----
@@ -181,16 +164,9 @@ large_select_kernel(const uint64_t *__restrict__ offsets, uint32_t uniform_len, 
         }
         // ---- output: ascending bottom-s to every destination ----
         for (uint32_t i = tid; i < s; i += LG_THREADS) dst[i] = sb[i];
-        for (int pr = 0; pr < extra.n; ++pr) {
-            uint32_t *peer = extra.ptr[pr] + row * row_stride;
-            if (peer == dst) continue;
-            for (uint32_t i = tid; i < s; i += LG_THREADS) peer[i] = sb[i];
-        }
-        if (tid == 0) {
-            // s == 1: mash.go:96-98 indexes Sketches[-1] as soon as a later hash is strictly below Sketches[0]
-            if (status) status[row] = (s == 1 && sb[0] < src[0]) ? PG_ITEM_PANIC : PG_ITEM_OK;
-            if (count) count[row] = s;
-        }
+        replicate_row<LG_THREADS>(extra, row, row_stride, sb, dst, s);
+        // s == 1: mash.go:96-98 indexes Sketches[-1] as soon as a later hash is strictly below Sketches[0]
+        put_row_status(status, count, row, s, s == 1 && sb[0] < src[0]);
         __syncthreads();
     }
 }

@@ -136,7 +136,7 @@ def test_select_regime_long_reads_with_pruning(gpu, oracle):
         seqs = [bytes(rng.choice(list(b"ACGT"), size=l).astype(np.uint8)) for l in lens]
         seqs.append(bytes(rng.choice(list(b"AC"), size=70_001).astype(np.uint8)))
         seqs.append(b"ACG" * 20_000)
-        if s == 1000:  # a genome-sized sequence: cut into slices, sketched in parallel, merged
+        if s == 1000:  # a 2.5 Mbp sequence: many K2t work items in one row
             seqs.append(bytes(rng.choice(list(b"ACGT"), size=2_500_003).astype(np.uint8)))
             seqs += [bytes(rng.choice(list(b"ACGT"), size=int(l)).astype(np.uint8)) for l in rng.integers(0, 3000, 40)]
         bases, offsets = mash.flatten(seqs)
@@ -150,6 +150,41 @@ def test_select_regime_long_reads_with_pruning(gpu, oracle):
             cnt = min(max(len(q) - k, 0), s)
             assert status[i] == 0 and count[i] == cnt, (k, s, i)
             assert np.array_equal(out[i, :cnt], o.Sketches[:cnt]), (k, s, i, len(q))
+    # A ragged batch that K2t declines (rows x work items of its longest row > 4 Mi) with few select-regime rows among at
+    # most 4 x 3 x SMs rows: the select-regime rows are cut into slices, sketched in parallel and merged
+    # (try_select_sliced + select_merge_kernel).  K2t's item: 8 x 32 x SEG positions, SEG = 60 for k = 21.  The batch
+    # goes through the device entry point in one call: the host entry point would cut it into chunks of fewer rows.
+    import ctypes
+    import torch
+    from poly_b200 import _lib
+    L_ = _lib.lib()
+    sms = ctypes.c_int(0)
+    _lib.check(L_.pg_device_sm_count(ctypes.byref(sms)))
+    k, s = 21, 1000
+    n_rows = 4 * 3 * sms.value - 1
+    items = (4 << 20) // n_rows + 1  # K2t work items of the longest row: n_rows x items > 4 Mi
+    long_len = items * 8 * 32 * 60 + k  # about 41 Mbp on 132 SMs
+    lens = [long_len] + [int(x) for x in rng.integers(2_000, 60_000, 10)] + [int(x) for x in rng.integers(0, s + k, n_rows - 11)]
+    rng.shuffle(lens)
+    assert sum(l - k >= s for l in lens) < 3 * sms.value
+    seqs = [bytes(rng.choice(list(b"ACGT"), size=l).astype(np.uint8)) for l in lens]
+    bases, offsets = mash.flatten(seqs)
+    dev = torch.device("cuda", 0)
+    st = torch.cuda.current_stream(dev).cuda_stream
+    d_bases = torch.from_numpy(bases).to(dev)
+    d_off = torch.from_numpy(offsets.astype(np.int64)).to(dev)
+    d_out = torch.empty((n_rows, s), dtype=torch.int32, device=dev)
+    d_count = torch.empty(n_rows, dtype=torch.int32, device=dev)
+    d_status = torch.empty(n_rows, dtype=torch.int32, device=dev)
+    _lib.check(L_.pg_mash_sketch_batch_dev(d_bases.data_ptr(), d_off.data_ptr(), n_rows, max(lens), k, s, _lib.PG_SKETCH_PAD_ZERO,
+                                           d_out.data_ptr(), s, d_count.data_ptr(), d_status.data_ptr(), st))
+    assert L_.pg_last_kernel() == b"select_merge_kernel"  # the batch did take the slicing path
+    torch.cuda.synchronize(dev)
+    out, count, status = d_out.cpu().numpy().view(np.uint32), d_count.cpu().numpy(), d_status.cpu().numpy()
+    rc, want = oracle.sketch_batch(bases, offsets, k, s, variant=1, nthreads=os.cpu_count() or 1)
+    assert rc == 0 and not status.any()
+    assert np.array_equal(count, np.minimum(np.maximum(np.array(lens) - k, 0), s))
+    assert np.array_equal(out, want)
 
 
 def test_cfg3_shape_sample_golden(gpu, oracle):
@@ -435,28 +470,32 @@ def test_select_threshold_path(gpu, oracle, monkeypatch):
     retry list hands to the exact streaming kernel.  Everything bit-exact against the oracle."""
     rng = np.random.default_rng(77)
     monkeypatch.setenv("PG_K2T_GROUP_ROWS", "7")
-    cases = [(21, 1000, 40_000, 20), (31, 2000, 10_000, 40), (16, 64, 5_000, 33), (21, 1000, 1021 + 21, 9), (21, 1000, 1300, 9),
-             (24, 5000, 30_000, 5), (32, 3, 9_000, 12), (11, 500, 2176 * 8 + 11 + 1, 6), (28, 300, 7_013, 8)]
-    # both bucket functions of the select stage and both loop shapes of the walk, on every case
-    for knobs in ({}, {"PG_K2T_SEL_MUL": "0", "PG_K2T_ROLLED": "0", "PG_K2T_SEL_U": "3"}, {"PG_K2T_SEL_MUL": "1", "PG_K2T_ROLLED": "1", "PG_K2T_SEL_U": "8"}):
-        for name in ("PG_K2T_SEL_MUL", "PG_K2T_ROLLED", "PG_K2T_SEL_U"):
-            monkeypatch.delenv(name, raising=False)
-        for name, v in knobs.items():
-            monkeypatch.setenv(name, v)
-        for k, s, L, n in cases:
-            reads = rng.choice(list(b"ACGT"), size=n * L).astype(np.uint8).reshape(n, L)
-            reads[1] = ord("A")                                                   # homopolymer: one distinct hash
-            reads[2] = np.frombuffer((b"ACG" * (L // 3 + 1))[:L], dtype=np.uint8)  # period 3: three distinct hashes
-            reads[3] = rng.choice(list(b"AC"), size=L).astype(np.uint8)           # low complexity
-            reads[4, : L // 2] = reads[4, L // 2: 2 * (L // 2)]                    # every k-mer of one half twice
-            got = mash.sketch_uniform(reads.reshape(-1), n, L, k, s)
-            rc, want = oracle.sketch_batch(reads.reshape(-1), synth.uniform_offsets(n, L), k, s, variant=1)
-            assert rc == 0
-            cnt = min(L - k, s)
-            assert np.array_equal(got, want[:, :cnt]), (knobs, k, s, L, n, [i for i in range(n) if not np.array_equal(got[i], want[i, :cnt])])
-    for name in ("PG_K2T_SEL_MUL", "PG_K2T_ROLLED", "PG_K2T_SEL_U"):
-        monkeypatch.delenv(name, raising=False)
-    # ragged batch whose longest read spans several items: row x item mapping with empty items
+    # (k, s, L, n) and what launch_select_thresh picks for it: the select batch width U (fitted to mu = s + 6 sqrt(s) + 48),
+    # the bucket function of stage B (plain shift, or scaled when the shift would use < 3/4 of the buckets) and the
+    # loop shape of the walk (unrolled for k < 24, rolled from k = 24 on).  Together every variant is reached.
+    cases = [(21, 1000, 40_000, 20),        # U 6, shift,  unrolled
+             (31, 2000, 10_000, 40),        # U 5, shift,  rolled
+             (16, 64, 5_000, 33),           # U 3, scaled, unrolled
+             (21, 1000, 1021 + 21, 9),      # U 6, shift,  unrolled (T = 2^32: every hash is a candidate)
+             (21, 1000, 1300, 9),           # U 6, shift,  unrolled
+             (24, 5000, 30_000, 5),         # U 8, scaled, rolled
+             (32, 3, 9_000, 12),            # U 3, shift,  rolled
+             (11, 500, 2176 * 8 + 11 + 1, 6),  # U 3, scaled, unrolled (rows of several work items)
+             (28, 300, 7_013, 8),           # k = 28 has no walk instantiation: the generic select kernel
+             (19, 700, 20_000, 8)]          # U 4, scaled, unrolled
+    for k, s, L, n in cases:
+        reads = rng.choice(list(b"ACGT"), size=n * L).astype(np.uint8).reshape(n, L)
+        reads[1] = ord("A")                                                   # homopolymer: one distinct hash
+        reads[2] = np.frombuffer((b"ACG" * (L // 3 + 1))[:L], dtype=np.uint8)  # period 3: three distinct hashes
+        reads[3] = rng.choice(list(b"AC"), size=L).astype(np.uint8)           # low complexity
+        reads[4, : L // 2] = reads[4, L // 2: 2 * (L // 2)]                    # every k-mer of one half twice
+        got = mash.sketch_uniform(reads.reshape(-1), n, L, k, s)
+        rc, want = oracle.sketch_batch(reads.reshape(-1), synth.uniform_offsets(n, L), k, s, variant=1)
+        assert rc == 0
+        cnt = min(L - k, s)
+        assert np.array_equal(got, want[:, :cnt]), (k, s, L, n, [i for i in range(n) if not np.array_equal(got[i], want[i, :cnt])])
+    # ragged batch (scaled buckets, a different T per row) whose longest read spans several items: row x item mapping
+    # with empty items
     lens = [int(x) for x in rng.integers(1200, 50_000, 30)] + [0, 5, 1021, 1022, 1023]
     seqs = [bytes(rng.choice(list(b"ACGT"), size=l).astype(np.uint8)) for l in lens] + [b"T" * 30_000]
     bases, offsets = mash.flatten(seqs)
