@@ -454,3 +454,54 @@ func FastqIngestRecords(text []byte) (bases []byte, offsets []uint64, spans []ui
 	})
 	return bases[:total], offsets[:n+1], spans[:4*n], int32(code), uint64(line), err
 }
+
+// Index wraps a pg_mash_index: a reference sketch set copied to the device of the calling thread
+// (pg_thread_device / pg_init) and indexed there once.  It is read-only after NewIndex: any number of
+// goroutines may call Query at once.  Close must not run while a Query is in flight.
+type Index struct {
+	h *C.pg_mash_index
+}
+
+// MaxTopK is the largest k Query accepts (PG_INDEX_MAX_TOP_K).
+const MaxTopK = int(C.PG_INDEX_MAX_TOP_K)
+
+// NewIndex wraps pg_mash_index_create over n sketches of s words each (full arrays, zero tails included).
+func NewIndex(sketches []uint32, n, s int) (*Index, error) {
+	var h *C.pg_mash_index
+	var p *C.uint32_t
+	if len(sketches) > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
+	}
+	if err := locked(func() C.int { return C.pg_mash_index_create(p, C.uint64_t(n), C.int32_t(s), &h) }); err != nil {
+		return nil, err
+	}
+	return &Index{h: h}, nil
+}
+
+// Query wraps pg_mash_index_query: for each of nq query sketches of sq words, up to k references with
+// same >= minSame, ordered by same descending and then reference index ascending.  Row q of ref / same /
+// dist holds nHits[q] entries.
+func (ix *Index) Query(queries []uint32, nq, sq, k, minSame int) (ref, same []uint32, dist []float64, nHits []uint32, err error) {
+	slots := nq * k
+	ref, same, dist, nHits = make([]uint32, slots+1), make([]uint32, slots+1), make([]float64, slots+1), make([]uint32, nq+1)
+	var p *C.uint32_t
+	if len(queries) > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&queries[0]))
+	}
+	err = locked(func() C.int {
+		return C.pg_mash_index_query(ix.h, p, C.uint64_t(nq), C.int32_t(sq), C.uint32_t(k), C.uint32_t(minSame),
+			(*C.uint32_t)(unsafe.Pointer(&ref[0])), (*C.uint32_t)(unsafe.Pointer(&same[0])), (*C.double)(unsafe.Pointer(&dist[0])),
+			(*C.uint32_t)(unsafe.Pointer(&nHits[0])))
+	})
+	return ref[:slots], same[:slots], dist[:slots], nHits[:nq], err
+}
+
+// Close wraps pg_mash_index_free.
+func (ix *Index) Close() error {
+	if ix.h == nil {
+		return nil
+	}
+	h := ix.h
+	ix.h = nil
+	return locked(func() C.int { return C.pg_mash_index_free(h) })
+}

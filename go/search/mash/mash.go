@@ -140,3 +140,73 @@ func RelatedPairs(sketches []*Mash) []RelatedPair {
 	}
 	return out
 }
+
+// Neighbor is one reference of a Nearest result.
+type Neighbor struct {
+	Index    int     // position in the reference list given to NewIndex
+	Same     int     // matching hashes as query.Similarity(reference) counts them (mash.go:121-132)
+	Distance float64 // query.Distance(reference) (mash.go:134,139)
+}
+
+// Index holds a reference sketch set on the GPU for repeated nearest-neighbour queries (the sketches are
+// copied; the references may be changed or dropped afterwards).  Safe for concurrent use; call Close when done.
+type Index struct {
+	ix *polyb200.Index
+	s  int
+}
+
+// NewIndex copies references of one common SketchSize to the GPU and indexes them.
+func NewIndex(references []*Mash) (*Index, error) {
+	s := 0
+	if len(references) > 0 {
+		s = references[0].SketchSize
+	}
+	flat := make([]uint32, 0, len(references)*s)
+	for _, m := range references {
+		if m.SketchSize != s {
+			return nil, errors.New("mash: every reference of an index must have the same SketchSize")
+		}
+		flat = append(flat, m.Sketches[:s]...)
+	}
+	ix, err := polyb200.NewIndex(flat, len(references), s)
+	if errors.Is(err, polyb200.ErrPanic) {
+		panic("runtime error: index out of range [-1]") // Similarity on a sketch of size 0 would
+	} else if err != nil {
+		return nil, err
+	}
+	return &Index{ix: ix, s: s}, nil
+}
+
+// Nearest returns, for each query (all of one SketchSize), the k references with the largest matching counts
+// (query.Similarity(reference), the query as receiver) that share at least one hash, ordered by count
+// descending and then by reference position.  1 <= k <= 1024.
+func (ix *Index) Nearest(queries []*Mash, k int) [][]Neighbor {
+	sq := 0
+	if len(queries) > 0 {
+		sq = queries[0].SketchSize
+	}
+	flat := make([]uint32, 0, len(queries)*sq)
+	for _, m := range queries {
+		if m.SketchSize != sq {
+			panic("mash: every query of a batch must have the same SketchSize")
+		}
+		flat = append(flat, m.Sketches[:sq]...)
+	}
+	ref, same, dist, nHits, err := ix.ix.Query(flat, len(queries), sq, k, 1)
+	if errors.Is(err, polyb200.ErrPanic) {
+		panic("runtime error: index out of range [-1]")
+	} else if err != nil {
+		panic(err)
+	}
+	res := make([][]Neighbor, len(queries))
+	for q := range res {
+		res[q] = make([]Neighbor, nHits[q])
+		for t := range res[q] {
+			res[q][t] = Neighbor{Index: int(ref[q*k+t]), Same: int(same[q*k+t]), Distance: dist[q*k+t]}
+		}
+	}
+	return res
+}
+
+// Close releases the index's device memory.
+func (ix *Index) Close() error { return ix.ix.Close() }

@@ -307,6 +307,56 @@ inline std::vector<Mash> MashesOf(const SketchSet &set) {
     return out;
 }
 
+// ---- sketch index: top-k nearest references (pg_mash_index_*) ----------------------------------------
+// One reference of a query's result: refs[Ref], its matching count as queries[q].Similarity(refs[Ref]) counts it
+// (the query is the receiver, mash.go:107-135), and queries[q].Distance(refs[Ref]).
+struct Neighbor {
+    uint32_t Ref;
+    uint32_t Same;
+    double Distance;
+};
+// RAII owner of a device-resident index over a reference set of one SketchSize (the library copies the sketches).
+class Index {
+    pg_mash_index *h_ = nullptr;
+    int s_ = 0;
+
+public:
+    explicit Index(const std::vector<Mash> &refs) {
+        s_ = refs.empty() ? 0 : refs[0].SketchSize;
+        std::vector<uint32_t> flat;
+        flat.reserve(refs.size() * (size_t)std::max(s_, 0));
+        for (auto &m : refs) {
+            if (m.SketchSize != s_ || (int)m.Sketches.size() < s_) throw std::invalid_argument("references must share one SketchSize");
+            flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + s_);
+        }
+        int rc = pg_mash_index_create(flat.data(), refs.size(), s_, &h_);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+    }
+    Index(const Index &) = delete;
+    Index &operator=(const Index &) = delete;
+    ~Index() { pg_mash_index_free(h_); }
+    // For each query, up to k references with Same >= minSame, by Same descending and then Ref ascending.
+    std::vector<std::vector<Neighbor>> Nearest(const std::vector<Mash> &queries, uint32_t k, uint32_t minSame = 1) const {
+        const int sq = queries.empty() ? 0 : queries[0].SketchSize;
+        std::vector<uint32_t> flat;
+        for (auto &m : queries) {
+            if (m.SketchSize != sq || (int)m.Sketches.size() < sq) throw std::invalid_argument("queries must share one SketchSize");
+            flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + sq);
+        }
+        const size_t nq = queries.size();
+        std::vector<uint32_t> ref(nq * k), same(nq * k), nh(nq);
+        std::vector<double> dist(nq * k);
+        int rc = pg_mash_index_query(h_, flat.data(), nq, sq, k, minSame, ref.data(), same.data(), dist.data(), nh.data());
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+        std::vector<std::vector<Neighbor>> out(nq);
+        for (size_t q = 0; q < nq; ++q)
+            for (uint32_t t = 0; t < nh[q]; ++t) out[q].push_back(Neighbor{ref[q * k + t], same[q * k + t], dist[q * k + t]});
+        return out;
+    }
+};
+
 }  // namespace mash
 
 namespace align {

@@ -222,6 +222,48 @@ int pg_mash_distance_sparse_dev(const uint32_t *d_sketches, uint64_t n, int32_t 
                                 uint32_t *d_pair_same, uint64_t pairs_cap, uint64_t *d_n_pairs,
                                 void *stream);
 
+/* ---- sketch index: top-k nearest references of query sketches -------------------------------------
+ * A reference set of n sketches of size s (n x s full Go arrays, zero tail included, as
+ * pg_mash_distance_block takes them) is copied to the device once and indexed there; batches of
+ * query sketches are then ranked against it.  For query q and reference j, same[q][j] is what
+ * queries[q].Similarity(refs[j]) counts -- the QUERY is the receiver (mash.go:107-135): larger/smaller
+ * by SketchSize with the receiver winning ties, the range early-out, the two-pointer walk (exact also
+ * for unsorted n < s sketches).  KmerSize is not compared, as in the reference.  distance =
+ * 1 - same/min(sq, s) in double, bit-identical to (*Mash).Distance (mash.go:134,139).
+ *
+ * Result for query q (row q of the nq x top_k outputs): the references with same >= min_same, ordered
+ * by same descending, then by reference index ascending (ties at the cut are broken the same way),
+ * cut to the first top_k; n_hits[q] (<= top_k) of them are listed.  The denominator is the same for
+ * every reference of a query, so this is also distance ascending.  Unused slots hold ref 0xFFFFFFFF,
+ * same 0 and distance 1.0.  min_same = 0 also lists references that share nothing, in index order.
+ * 1 <= top_k <= PG_INDEX_MAX_TOP_K, else PG_ERR_ARG.  Any of the four outputs may be NULL.  nq == 0
+ * is valid.  A sketch of size 0 (s or sq) is PG_ERR_PANIC, as in the distance calls above.
+ * PG_ERR_UNSUPPORTED when a query must be compared pairwise (an unsorted query or reference, or a set
+ * too skewed for the inverted index) and 8 * (sq + s) words exceed the kernel's shared-memory tile.
+ *
+ * Ownership, device and threads:
+ *   - create copies the reference sketches into device memory the index owns; no caller pointer is
+ *     retained.  pg_mash_index_free releases it;
+ *   - the index lives on the device current for the calling thread at creation (pg_thread_device /
+ *     pg_init); queries run on that device whatever thread calls them (the calling thread's current
+ *     CUDA device is set to it).  _dev queries take device pointers on that device;
+ *   - the index is read-only after creation: any number of threads may query one index at once.
+ *     Freeing an index while a query on it is running, or while a _dev query is still enqueued on a
+ *     stream that has not been synchronised, is the caller's error;
+ *   - create, create_dev and both query calls synchronise (the host chooses the kernels from the data);
+ *     query_dev leaves its outputs on the device, ordered on `stream`.
+ */
+#define PG_INDEX_MAX_TOP_K 1024u
+typedef struct pg_mash_index pg_mash_index;
+int pg_mash_index_create(const uint32_t *sketches, uint64_t n, int32_t s, pg_mash_index **out);
+int pg_mash_index_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, void *stream, pg_mash_index **out);
+int pg_mash_index_query(const pg_mash_index *ix, const uint32_t *queries, uint64_t nq, int32_t sq, uint32_t top_k,
+                        uint32_t min_same, uint32_t *hit_ref, uint32_t *hit_same, double *hit_distance, uint32_t *n_hits);
+int pg_mash_index_query_dev(const pg_mash_index *ix, const uint32_t *d_queries, uint64_t nq, int32_t sq, uint32_t top_k,
+                            uint32_t min_same, uint32_t *d_hit_ref, uint32_t *d_hit_same, double *d_hit_distance,
+                            uint32_t *d_n_hits, void *stream);
+int pg_mash_index_free(pg_mash_index *ix);
+
 /* ---- align.SmithWaterman score -- search/align/align.go:171-203 -------------------
  * One template against n queries.  query_is_a != 0: stringA = query (outer loop),
  * stringB = template; else swapped.  lut_a/lut_b: byte -> index into the first /

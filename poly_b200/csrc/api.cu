@@ -1170,6 +1170,113 @@ int pg_mash_distance_sparse(const uint32_t *sketches, uint64_t n, int32_t s, uin
 }
 
 // ---------------------------------------------------------------------------------
+// Sketch index: top-k nearest references
+// ---------------------------------------------------------------------------------
+}  // extern "C"
+
+struct pg_mash_index {
+    int device;
+    uint32_t *d_sk;        // the index's own copy of the n x s reference sketches
+    DistancePlan plan;     // sortedness flags + join index over d_sk
+};
+
+static int index_create(const uint32_t *src, bool src_dev, uint64_t n, int32_t s, cudaStream_t st, pg_mash_index **out) {
+    if (n && s <= 0) { set_error("index over sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
+    pg_mash_index *ix = new pg_mash_index{t_ctx->device, nullptr, DistancePlan()};
+    const uint64_t words = n * (uint64_t)std::max(s, 0);
+    int rc = PG_OK;
+    cudaError_t e = cudaMallocAsync(&ix->d_sk, words ? words * 4 : 4, st);
+    if (e != cudaSuccess) { cudaGetLastError(); ix->d_sk = nullptr; set_error("cudaMallocAsync(%llu) for the index failed", (unsigned long long)(words * 4)); rc = PG_ERR_NOMEM; }
+    if (rc == PG_OK && words) {
+        e = cudaMemcpyAsync(ix->d_sk, src, words * 4, src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) rc = cuda_fail(e, "index copy", __FILE__, __LINE__);
+    }
+    if (rc == PG_OK) rc = distance_plan_create(ix->d_sk, n, s, st, &ix->plan);
+    if (rc == PG_OK) { e = cudaStreamSynchronize(st); if (e != cudaSuccess) rc = cuda_fail(e, "index build", __FILE__, __LINE__); }
+    if (rc != PG_OK) {
+        distance_plan_destroy(ix->plan, st);
+        if (ix->d_sk) cudaFreeAsync(ix->d_sk, st);
+        cudaStreamSynchronize(st);
+        delete ix;
+        return rc;
+    }
+    *out = ix;
+    return PG_OK;
+}
+
+extern "C" {
+
+int pg_mash_index_create(const uint32_t *sketches, uint64_t n, int32_t s, pg_mash_index **out) {
+    if (!out) { set_error("null index pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n && s > 0 && !sketches) { set_error("null buffer"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(t_ctx->mu);
+    return index_create(sketches, false, n, s, t_ctx->streams[0], out);
+}
+
+int pg_mash_index_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, void *stream, pg_mash_index **out) {
+    if (!out) { set_error("null index pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n && s > 0 && !d_sketches) { set_error("null buffer"); return PG_ERR_ARG; }
+    return index_create(d_sketches, true, n, s, (cudaStream_t)stream, out);
+}
+
+int pg_mash_index_query_dev(const pg_mash_index *ix, const uint32_t *d_queries, uint64_t nq, int32_t sq, uint32_t top_k,
+                            uint32_t min_same, uint32_t *d_hit_ref, uint32_t *d_hit_same, double *d_hit_distance,
+                            uint32_t *d_n_hits, void *stream) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    return launch_index_query(ix->plan, d_queries, nq, sq, top_k, min_same, d_hit_ref, d_hit_same, d_hit_distance, d_n_hits,
+                              (cudaStream_t)stream);
+}
+
+int pg_mash_index_query(const pg_mash_index *ix, const uint32_t *queries, uint64_t nq, int32_t sq, uint32_t top_k,
+                        uint32_t min_same, uint32_t *hit_ref, uint32_t *hit_same, double *hit_distance, uint32_t *n_hits) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    if (top_k == 0 || top_k > PG_INDEX_MAX_TOP_K) { set_error("top_k %u outside [1, %u]", top_k, PG_INDEX_MAX_TOP_K); return PG_ERR_ARG; }
+    if (nq == 0) return PG_OK;
+    if (sq <= 0) { set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq); return PG_ERR_PANIC; }
+    if (!queries) { set_error("null buffer"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(t_ctx->mu);
+    cudaStream_t st = t_ctx->streams[0];
+    const uint64_t slots = nq * (uint64_t)top_k;
+    Tmp d_q(st), d_ref(st), d_same(st), d_dist(st), d_nh(st);
+    if ((rc = d_q.alloc(nq * (uint64_t)sq * 4)) || (hit_ref && (rc = d_ref.alloc(slots * 4))) || (hit_same && (rc = d_same.alloc(slots * 4))) ||
+        (hit_distance && (rc = d_dist.alloc(slots * 8))) || (n_hits && (rc = d_nh.alloc(nq * 4))))
+        return rc;
+    PG_CUDA(cudaMemcpyAsync(d_q.p, queries, nq * (uint64_t)sq * 4, cudaMemcpyHostToDevice, st));
+    rc = launch_index_query(ix->plan, d_q.as<uint32_t>(), nq, sq, top_k, min_same, d_ref.as<uint32_t>(), d_same.as<uint32_t>(),
+                            d_dist.as<double>(), d_nh.as<uint32_t>(), st);
+    if (rc != PG_OK) return rc;
+    if (hit_ref) PG_CUDA(cudaMemcpyAsync(hit_ref, d_ref.p, slots * 4, cudaMemcpyDeviceToHost, st));
+    if (hit_same) PG_CUDA(cudaMemcpyAsync(hit_same, d_same.p, slots * 4, cudaMemcpyDeviceToHost, st));
+    if (hit_distance) PG_CUDA(cudaMemcpyAsync(hit_distance, d_dist.p, slots * 8, cudaMemcpyDeviceToHost, st));
+    if (n_hits) PG_CUDA(cudaMemcpyAsync(n_hits, d_nh.p, nq * 4, cudaMemcpyDeviceToHost, st));
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
+}
+
+int pg_mash_index_free(pg_mash_index *ix) {
+    if (!ix) return PG_OK;
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(t_ctx->mu);
+    cudaStream_t st = t_ctx->streams[0];
+    distance_plan_destroy(ix->plan, st);
+    if (ix->d_sk) cudaFreeAsync(ix->d_sk, st);
+    delete ix;
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
+}
+
+// ---------------------------------------------------------------------------------
 // Smith-Waterman score
 // ---------------------------------------------------------------------------------
 static int align_score_dev(int global, const uint8_t *d_queries, const uint64_t *d_q_offsets, uint64_t n_queries,

@@ -142,6 +142,7 @@ int launch_distance_sparse(const uint32_t *d_sk, uint64_t n, int s, uint64_t row
 // set and reused for every row block
 struct JoinIndex {
     uint64_t *entries = nullptr, *start = nullptr;
+    uint32_t *vmax = nullptr;  // device word: the largest value, which sets the bucket scale (hist_kernel)
     uint64_t nb = 0, n = 0;
     int s = 0;
     bool ok = false;
@@ -160,6 +161,13 @@ struct DistancePlan {
 int distance_plan_create(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, DistancePlan *plan);
 int distance_plan_rows(const DistancePlan &plan, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st);
 void distance_plan_destroy(DistancePlan &plan, cudaStream_t st);
+// distance.cu: flag[r] = 1 if sketch r is non-decreasing; *d_n_unsorted = number of other sketches
+int launch_sorted_flags(const uint32_t *d_sk, uint64_t n, int s, uint8_t *d_flag, uint32_t *d_n_unsorted, cudaStream_t st);
+// mash_index.cu: the top_k most similar sketches of plan's set for each of nq query sketches of size sq
+// (receiver = query); outputs nq x top_k on the device, any may be NULL
+constexpr uint32_t INDEX_MAX_TOP_K = 1024;
+int launch_index_query(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t top_k, uint32_t min_same,
+                       uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint32_t *d_n_hits, cudaStream_t st);
 // sw_score.cu
 int launch_sw_score(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen,
                     const uint8_t *d_t, uint64_t tlen, int query_is_a, const int16_t *lut_a,

@@ -274,6 +274,14 @@ int launch_similarity_pairs(const uint32_t *d_sk, const uint64_t *d_off, uint64_
     return PG_OK;
 }
 
+int launch_sorted_flags(const uint32_t *d_sk, uint64_t n, int s, uint8_t *d_flag, uint32_t *d_n_unsorted, cudaStream_t st) {
+    PG_CUDA(cudaMemsetAsync(d_n_unsorted, 0, 4, st));
+    if (n == 0) return PG_OK;
+    sorted_flag_kernel<<<(unsigned)std::min<uint64_t>((n + 7) / 8, 4096), 256, 0, st>>>(d_sk, n, (uint32_t)s, d_flag, d_n_unsorted);
+    PG_LAUNCH_CHECK("sorted_flag_kernel");
+    return PG_OK;
+}
+
 int distance_plan_create(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, DistancePlan *plan) {
     plan->d_sk = d_sk; plan->n = n; plan->s = s; plan->d_flag = nullptr; plan->join = JoinIndex();
     if (n == 0) return PG_OK;
@@ -283,9 +291,7 @@ int distance_plan_create(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t s
     }
     PG_CUDA(cudaMallocAsync(&plan->d_flag, n + 8, st));
     uint32_t *d_unsorted = reinterpret_cast<uint32_t *>(plan->d_flag + ((n + 3) & ~3ull));
-    PG_CUDA(cudaMemsetAsync(d_unsorted, 0, 4, st));
-    sorted_flag_kernel<<<(unsigned)std::min<uint64_t>((n + 7) / 8, 4096), 256, 0, st>>>(d_sk, n, s, plan->d_flag, d_unsorted);
-    PG_LAUNCH_CHECK("sorted_flag_kernel");
+    { const int rc_ = launch_sorted_flags(d_sk, n, s, plan->d_flag, d_unsorted, st); if (rc_ != PG_OK) return rc_; }
     // every sketch ascending (the select regime, L-k >= s): inverted-index join, output-sensitive
     uint32_t n_unsorted = 1;
     PG_CUDA(cudaMemcpyAsync(&n_unsorted, d_unsorted, 4, cudaMemcpyDeviceToHost, st));

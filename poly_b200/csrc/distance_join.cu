@@ -278,7 +278,7 @@ __global__ void same_to_distance_kernel(const uint32_t *__restrict__ same, uint6
 // applicable" (skewed data: a bucket would not fit shared memory) and the caller must use the
 // pairwise kernel.
 int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinIndex *ix) {
-    ix->ok = false; ix->entries = nullptr; ix->start = nullptr; ix->nb = 0; ix->n = n; ix->s = s;
+    ix->ok = false; ix->entries = nullptr; ix->start = nullptr; ix->vmax = nullptr; ix->nb = 0; ix->n = n; ix->s = s;
     const uint64_t total = n * (uint64_t)s;
     if (total == 0 || n > 0xffffffffull) return PG_OK;
     uint32_t *d_scalars = nullptr;  // [0] vmax, [1] largest bucket
@@ -324,7 +324,8 @@ int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinInd
             nb = std::min<uint64_t>(nb * 8, 1u << 22);
         }
     }
-    cudaFreeAsync(d_scalars, st);
+    if (ix->ok) ix->vmax = d_scalars;  // the bucket scale, for lookups of values that are not in the set
+    else cudaFreeAsync(d_scalars, st);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "distance join build", __FILE__, __LINE__);
     return PG_OK;
@@ -351,7 +352,8 @@ int join_emit(const JoinIndex &ix, uint64_t row_begin, uint64_t row_end, uint32_
 void join_free(JoinIndex &ix, cudaStream_t st) {
     if (ix.entries) cudaFreeAsync(ix.entries, st);
     if (ix.start) cudaFreeAsync(ix.start, st);
-    ix.entries = nullptr; ix.start = nullptr; ix.ok = false;
+    if (ix.vmax) cudaFreeAsync(ix.vmax, st);
+    ix.entries = nullptr; ix.start = nullptr; ix.vmax = nullptr; ix.ok = false;
 }
 
 }  // namespace pg

@@ -241,6 +241,138 @@ def DistanceMatrix(mashes: Sequence[Mash]) -> np.ndarray:
     return distance_block(sk)[1]
 
 
+# ---- sketch index: top-k nearest references (pg_mash_index_*) --------------------------------------------
+INDEX_MAX_TOP_K = 1024  # PG_INDEX_MAX_TOP_K
+NO_REF = 0xFFFFFFFF
+
+
+def min_same_for_distance(max_distance: float, den: int) -> int:
+    """Smallest matching count whose Distance is <= max_distance, evaluating the reference's own f64
+    expression 1 - same/den (mash.go:134,139) for every same in [0, den]; den + 1 when none qualifies.
+    The expression is non-increasing in same, so filtering by the returned count is exact."""
+    same = np.arange(den + 1, dtype=np.float64)
+    ok = np.nonzero(1.0 - same / np.float64(max(den, 1)) <= max_distance)[0]
+    return int(ok[0]) if len(ok) else den + 1
+
+
+def _sketch_rows(sketches):
+    """[n, s] uint32 array (host) or CUDA tensor (device), or a list of Mash of one SketchSize."""
+    if hasattr(sketches, "data_ptr"):
+        if sketches.dim() != 2 or sketches.element_size() != 4 or not sketches.is_contiguous():
+            raise ValueError("sketch tensors must be contiguous 32-bit [n, s]")
+        return sketches
+    if isinstance(sketches, (list, tuple)):
+        if not sketches:
+            return np.zeros((0, 0), dtype=np.uint32)
+        s = sketches[0].SketchSize
+        if any(m.SketchSize != s for m in sketches):
+            raise ValueError("every sketch of a set must have the same SketchSize")
+        return np.stack([np.ascontiguousarray(m.Sketches[:s], dtype=np.uint32) for m in sketches]).reshape(len(sketches), s)
+    arr = np.ascontiguousarray(sketches, dtype=np.uint32)
+    if arr.ndim != 2:
+        raise ValueError("sketches must be [n, s]")
+    return arr
+
+
+def _index_rc(rc: int) -> None:
+    if rc == _lib.PG_ERR_PANIC:
+        raise GoPanic("index out of range [-1]")  # Sketches[SketchSize-1] with SketchSize 0
+    _lib.check(rc)
+
+
+class SketchIndex:
+    """A reference sketch set held on the GPU for top-k queries: `nearest` ranks every reference j for
+    query q by queries[q].Similarity(refs[j]) (the query is the receiver, mash.go:107-135).
+
+    sketches: [n, s] uint32 (full Go arrays, zero tail included), a CUDA tensor of that shape, or a list of
+    Mash of one SketchSize.  The index copies them; it lives on the device current at creation."""
+
+    def __init__(self, sketches):
+        rows = _sketch_rows(sketches)
+        n, s = int(rows.shape[0]), int(rows.shape[1])
+        h = C.c_void_p()
+        if hasattr(rows, "data_ptr"):
+            import torch
+
+            rc = _lib.lib().pg_mash_index_create_dev(rows.data_ptr(), n, s, torch.cuda.current_stream(rows.device).cuda_stream, C.byref(h))
+        else:
+            rc = _lib.lib().pg_mash_index_create(rows.ctypes.data, n, s, C.byref(h))
+        _index_rc(rc)
+        self._h = h
+        self._dev_queried = None
+        self.n, self.s = n, s
+
+    @classmethod
+    def load(cls, path: str) -> "SketchIndex":
+        """An index over the sketch set of a PGSKETCH file (rows re-materialised with their zero tails)."""
+        from . import sketchfile
+
+        sk, _, _, s = sketchfile.load(path, pad_zero=True)
+        return cls(sk[:, :s])
+
+    def nearest(self, queries, k: int, min_same: Optional[int] = None, max_distance: Optional[float] = None):
+        """For each query sketch, the k references with the largest matching counts (same descending, then
+        reference index ascending), keeping only same >= min_same (default 1) -- or, alternatively, only
+        Distance <= max_distance.  Returns (ref [nq, k] uint32, same [nq, k] uint32, distance [nq, k] float64,
+        n_hits [nq] uint32); slots past n_hits[q] hold ref 0xFFFFFFFF, same 0, distance 1.0.  CUDA tensor
+        queries give CUDA tensor results (int32 tensors carry the uint32 bits), ordered on the current stream."""
+        if self._h is None:
+            raise ValueError("the index is closed")
+        if min_same is not None and max_distance is not None:
+            raise ValueError("give min_same or max_distance, not both")
+        rows = _sketch_rows(queries)
+        nq, sq = int(rows.shape[0]), int(rows.shape[1])
+        if max_distance is not None:
+            min_same = min_same_for_distance(max_distance, min(sq, self.s))
+        min_same = 1 if min_same is None else int(min_same)
+        if not 0 <= min_same <= 0xFFFFFFFF:
+            raise ValueError("min_same must fit 32 bits")
+        if k < 0 or k > 0xFFFFFFFF:
+            raise PolyError(_lib.PG_ERR_ARG, f"top_k {k} outside [1, {INDEX_MAX_TOP_K}]")
+        if hasattr(rows, "data_ptr"):
+            import torch
+
+            dev = rows.device
+            ref = torch.empty((nq, max(k, 1)), dtype=torch.int32, device=dev)
+            same = torch.empty((nq, max(k, 1)), dtype=torch.int32, device=dev)
+            dist = torch.empty((nq, max(k, 1)), dtype=torch.float64, device=dev)
+            nh = torch.empty(nq, dtype=torch.int32, device=dev)
+            rc = _lib.lib().pg_mash_index_query_dev(self._h, rows.data_ptr(), nq, sq, k, min_same, ref.data_ptr(), same.data_ptr(),
+                                                    dist.data_ptr(), nh.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+            self._dev_queried = dev
+        else:
+            ref = np.empty((nq, max(k, 1)), dtype=np.uint32)
+            same = np.empty((nq, max(k, 1)), dtype=np.uint32)
+            dist = np.empty((nq, max(k, 1)), dtype=np.float64)
+            nh = np.empty(nq, dtype=np.uint32)
+            rc = _lib.lib().pg_mash_index_query(self._h, rows.ctypes.data, nq, sq, k, min_same, ref.ctypes.data, same.ctypes.data,
+                                                dist.ctypes.data, nh.ctypes.data)
+        _index_rc(rc)
+        return ref[:, :k], same[:, :k], dist[:, :k], nh
+
+    def close(self) -> None:
+        if self._h is not None:
+            if self._dev_queried is not None:  # results of device queries may still be in flight on torch's streams
+                import torch
+
+                torch.cuda.synchronize(self._dev_queried)
+            h, self._h = self._h, None
+            _lib.check(_lib.lib().pg_mash_index_free(h))
+
+    def __enter__(self) -> "SketchIndex":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        if getattr(self, "_h", None) is not None:
+            try:
+                self.close()
+            except Exception:
+                pass
+
+
 # ---- single-process multi-GPU additions (pg_*_multi; SURVEY.md 8b / 8e) ----------------------------
 def _device_list(devices):
     if devices is None:
