@@ -290,6 +290,25 @@ struct Tmp {
     ~Tmp() { if (p) cudaFreeAsync(p, st); }
     template <typename T> T *as() { return (T *)p; }
 };
+
+// Rows [rb, re) of a plan's matching counts and/or distances into host arrays that start at row rb, in row
+// blocks of <= 64 Mi pairs per pass
+int plan_rows_to_host(const DistancePlan &plan, uint64_t rb, uint64_t re, uint32_t *same, double *distance, cudaStream_t st) {
+    const uint64_t n = plan.n, rows_per = std::max<uint64_t>(8, ((64ull << 20) / n) & ~7ull);
+    for (uint64_t b = rb; b < re; b += rows_per) {
+        const uint64_t e = std::min(re, b + rows_per), cells = (e - b) * n;
+        Tmp d_same(st), d_dist(st);
+        int rc;
+        if (same && (rc = d_same.alloc(cells * 4))) return rc;
+        if (distance && (rc = d_dist.alloc(cells * 8))) return rc;
+        rc = distance_plan_rows(plan, b, e, same ? d_same.as<uint32_t>() : nullptr, distance ? d_dist.as<double>() : nullptr, st);
+        if (rc != PG_OK) return rc;
+        if (same) PG_CUDA(cudaMemcpyAsync(same + (b - rb) * n, d_same.p, cells * 4, cudaMemcpyDeviceToHost, st));
+        if (distance) PG_CUDA(cudaMemcpyAsync(distance + (b - rb) * n, d_dist.p, cells * 8, cudaMemcpyDeviceToHost, st));
+        PG_CUDA(cudaStreamSynchronize(st));
+    }
+    return PG_OK;
+}
 }  // namespace
 }  // namespace pg
 
@@ -990,20 +1009,7 @@ extern "C" int pg_mash_sketch_distance_multi(const uint8_t *bases, uint64_t n_re
             if ((same || distance) && nl) {
                 DistancePlan plan;
                 int c = distance_plan_create(d_full, n, s, st, &plan);
-                const uint64_t rows_per = std::max<uint64_t>(8, ((64ull << 20) / n) & ~7ull);
-                for (uint64_t rb = lo; rb < hi && c == PG_OK; rb += rows_per) {
-                    const uint64_t re = std::min(hi, rb + rows_per);
-                    Tmp d_same(st), d_dist(st);
-                    if (same && (c = d_same.alloc((re - rb) * n * 4))) break;
-                    if (distance && (c = d_dist.alloc((re - rb) * n * 8))) break;
-                    c = distance_plan_rows(plan, rb, re, same ? d_same.as<uint32_t>() : nullptr, distance ? d_dist.as<double>() : nullptr, st);
-                    if (c != PG_OK) break;
-                    cudaError_t e = cudaSuccess;
-                    if (same) e = cudaMemcpyAsync(same + rb * n, d_same.p, (re - rb) * n * 4, cudaMemcpyDeviceToHost, st);
-                    if (e == cudaSuccess && distance) e = cudaMemcpyAsync(distance + rb * n, d_dist.p, (re - rb) * n * 8, cudaMemcpyDeviceToHost, st);
-                    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-                    if (e != cudaSuccess) c = cuda_fail(e, "distance block copy", __FILE__, __LINE__);
-                }
+                if (c == PG_OK) c = plan_rows_to_host(plan, lo, hi, same ? same + lo * n : nullptr, distance ? distance + lo * n : nullptr, st);
                 distance_plan_destroy(plan, st);
                 if (c != PG_OK) return c;
             }
@@ -1101,24 +1107,10 @@ int pg_mash_distance_block(const uint32_t *sketches, uint64_t n, int32_t s, uint
     Tmp d_sk(st);
     if ((rc = d_sk.alloc(n * (uint64_t)s * 4))) return rc;
     PG_CUDA(cudaMemcpyAsync(d_sk.p, sketches, n * (uint64_t)s * 4, cudaMemcpyHostToDevice, st));
-    // one plan (sortedness + join index) for the whole call; row blocks of <= 64 Mi pairs per pass
+    // one plan (sortedness + join index) for the whole call
     DistancePlan plan;
     rc = distance_plan_create(d_sk.as<uint32_t>(), n, s, st, &plan);
-    const uint64_t rows_per = std::max<uint64_t>(8, ((64ull << 20) / n) & ~7ull);
-    for (uint64_t rb = row_begin; rb < row_end && rc == PG_OK; rb += rows_per) {
-        const uint64_t re = std::min(row_end, rb + rows_per);
-        Tmp d_same(st), d_dist(st);
-        if (same && (rc = d_same.alloc((re - rb) * n * 4))) break;
-        if (distance && (rc = d_dist.alloc((re - rb) * n * 8))) break;
-        rc = distance_plan_rows(plan, rb, re, same ? d_same.as<uint32_t>() : nullptr, distance ? d_dist.as<double>() : nullptr, st);
-        if (rc != PG_OK) break;
-        cudaError_t e = cudaSuccess;
-        if (same) e = cudaMemcpyAsync(same + (rb - row_begin) * n, d_same.p, (re - rb) * n * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && distance)
-            e = cudaMemcpyAsync(distance + (rb - row_begin) * n, d_dist.p, (re - rb) * n * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) rc = cuda_fail(e, "distance block copy", __FILE__, __LINE__);
-    }
+    if (rc == PG_OK) rc = plan_rows_to_host(plan, row_begin, row_end, same, distance, st);
     distance_plan_destroy(plan, st);
     return rc;
 }

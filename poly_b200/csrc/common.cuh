@@ -111,6 +111,29 @@ __device__ __forceinline__ void replicate_row(const SketchDst &extra, uint64_t r
     }
 }
 
+// Ascending bitonic sort of key[0, P) in shared memory by the NT threads of the CTA, P a power of two.  The
+// keys must be in place before the call (a CTA barrier behind their stores); all threads call, and the
+// sorted keys are visible to the whole CTA on return.
+template <typename T, int NT>
+__device__ void block_bitonic_sort(T *key, uint32_t P) {
+    // Pair t of a stage with distance j touches elements inside the 64-element block [64 * (t / 32), +64)
+    // whenever j <= 32, and a warp owns 32 consecutive pairs t: those stages only need a warp barrier.
+    static_assert(NT % 32 == 0, "a warp must own 32 consecutive pairs of every stage");
+    for (uint32_t k2 = 2; k2 <= P; k2 <<= 1) {
+        for (uint32_t j = k2 >> 1; j > 0; j >>= 1) {
+            for (uint32_t t = threadIdx.x; t < (P >> 1); t += NT) {
+                const uint32_t i = ((t & ~(j - 1)) << 1) | (t & (j - 1)), ixj = i | j;
+                const bool up = (i & k2) == 0;
+                const T a = key[i], c = key[ixj];
+                if ((a > c) == up) { key[i] = c; key[ixj] = a; }
+            }
+            if (j > 32) __syncthreads();  // this stage wrote outside the warp's own 64-element block
+            else __syncwarp();            // stages with distance <= 32 read and write inside it
+        }
+        __syncthreads();  // the next k2 starts with a distance that may cross warps
+    }
+}
+
 // ---- kernel launchers (one per .cu) -------------------------------------------
 // sketch_fill.cu
 int launch_sketch_uniform(const uint8_t *d_bases, uint64_t n_reads, uint32_t read_len, int k, int s,
@@ -147,6 +170,14 @@ struct JoinIndex {
     int s = 0;
     bool ok = false;
 };
+// The bucket of value v: values scaled to [0, nb) by the set's largest value vmax.  The index is built
+// (hist_kernel, scatter_kernel) and probed (index_probe_kernel) with this one mapping.
+__device__ __forceinline__ uint64_t join_bucket_scale(uint32_t nb, uint32_t vmax) {
+    return (((uint64_t)nb) << 32) / ((uint64_t)vmax + 1);
+}
+__device__ __forceinline__ uint32_t join_bucket(uint32_t v, uint64_t scale, uint32_t nb) {
+    return min((uint32_t)(((uint64_t)v * scale) >> 32), nb - 1);
+}
 int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinIndex *ix);
 int join_emit(const JoinIndex &ix, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st);
 void join_free(JoinIndex &ix, cudaStream_t st);

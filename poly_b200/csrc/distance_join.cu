@@ -28,10 +28,6 @@ constexpr int JOIN_CAP = 4096;      // entries a bucket CTA can hold (32 KB of k
 constexpr int JOIN_SMEM = JOIN_CAP * (8 + 3 * 2);
 constexpr int JOIN_THREADS = 256;
 
-__device__ __forceinline__ uint32_t bucket_of(uint32_t v, uint64_t scale /* = B * 2^32 / (vmax+1) */) {
-    return (uint32_t)(((uint64_t)v * scale) >> 32);
-}
-
 __global__ void max_value_kernel(const uint32_t *__restrict__ sk, uint64_t n, uint32_t s,
                                  uint32_t *__restrict__ vmax) {
     // ascending rows: the maximum of a row is its last element
@@ -44,9 +40,9 @@ __global__ void max_value_kernel(const uint32_t *__restrict__ sk, uint64_t n, ui
 
 __global__ void hist_kernel(const uint32_t *__restrict__ sk, uint64_t total, const uint32_t *__restrict__ vmax,
                             uint32_t nbuckets, uint32_t *__restrict__ hist) {
-    const uint64_t scale = (((uint64_t)nbuckets) << 32) / ((uint64_t)(*vmax) + 1);
+    const uint64_t scale = join_bucket_scale(nbuckets, *vmax);
     for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
-        const uint32_t b = min(bucket_of(__ldg(sk + e), scale), nbuckets - 1);
+        const uint32_t b = join_bucket(__ldg(sk + e), scale, nbuckets);
         // consecutive elements of an ascending row mostly share a bucket: aggregate per warp
         const uint32_t peers = __match_any_sync(__activemask(), b);
         if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&hist[b], __popc(peers));
@@ -82,11 +78,11 @@ __global__ void scatter_kernel(const uint32_t *__restrict__ sk, uint64_t total, 
                                const uint32_t *__restrict__ vmax, uint32_t nbuckets,
                                const uint64_t *__restrict__ start, uint32_t *__restrict__ cursor,
                                uint64_t *__restrict__ entries) {
-    const uint64_t scale = (((uint64_t)nbuckets) << 32) / ((uint64_t)(*vmax) + 1);
+    const uint64_t scale = join_bucket_scale(nbuckets, *vmax);
     for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
         const uint32_t v = __ldg(sk + e);
         const uint32_t id = (uint32_t)(e / s);
-        const uint32_t b = min(bucket_of(v, scale), nbuckets - 1);
+        const uint32_t b = join_bucket(v, scale, nbuckets);
         const uint32_t peers = __match_any_sync(__activemask(), b);
         const int leader = __ffs(peers) - 1;
         uint32_t base = 0;
@@ -110,21 +106,7 @@ bucket_sort_kernel(uint64_t *__restrict__ entries, const uint64_t *__restrict__ 
         while (P < m) P <<= 1;
         for (uint32_t i = threadIdx.x; i < P; i += JOIN_THREADS) key[i] = i < m ? entries[lo + i] : ~0ull;
         __syncthreads();
-        // Pair t of a stage with distance j touches elements inside the 64-element block [64 * (t / 32), +64)
-        // whenever j <= 32, and a warp owns 32 consecutive pairs t: those stages only need a warp barrier.
-        for (uint32_t k2 = 2; k2 <= P; k2 <<= 1) {
-            for (uint32_t j = k2 >> 1; j > 0; j >>= 1) {
-                for (uint32_t t = threadIdx.x; t < (P >> 1); t += JOIN_THREADS) {
-                    const uint32_t i = ((t & ~(j - 1)) << 1) | (t & (j - 1)), ixj = i | j;
-                    const bool up = (i & k2) == 0;
-                    const uint64_t a = key[i], c = key[ixj];
-                    if ((a > c) == up) { key[i] = c; key[ixj] = a; }
-                }
-                if (j > 32) __syncthreads();  // this stage wrote outside the warp's own 64-element block
-                else __syncwarp();            // stages with distance <= 32 read and write inside it
-            }
-            __syncthreads();  // the next k2 starts with a distance that may cross warps
-        }
+        block_bitonic_sort<uint64_t, JOIN_THREADS>(key, P);
         for (uint32_t i = threadIdx.x; i < m; i += JOIN_THREADS) entries[lo + i] = key[i];
         __syncthreads();
     }

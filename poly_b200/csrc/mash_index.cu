@@ -29,8 +29,6 @@ constexpr int SEL_BITS = 12;          // histogram digit: counts are selected 12
 constexpr int SEL_BINS = 1 << SEL_BITS;
 constexpr uint32_t NO_REF = 0xffffffffu;
 
-__device__ __forceinline__ uint32_t bucket_of(uint32_t v, uint64_t scale) { return (uint32_t)(((uint64_t)v * scale) >> 32); }
-
 // One CTA per query row of the block; rows whose query is not ascending are left to the pairwise kernel.
 // Lanes search 32 distinct query values at once, then the warp walks each found run with its lanes along the
 // run, so the reductions of one instruction go to neighbouring words of the accumulator row.
@@ -43,7 +41,7 @@ index_probe_kernel(const uint32_t *__restrict__ q, uint32_t sq, uint64_t row0, c
     const uint32_t *Q = q + row * sq;
     uint32_t *A = acc + (uint64_t)blockIdx.x * n;
     const uint32_t vmax = *vmax_p;
-    const uint64_t scale = (((uint64_t)nb) << 32) / ((uint64_t)vmax + 1);  // as hist_kernel / scatter_kernel
+    const uint64_t scale = join_bucket_scale(nb, vmax);
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     for (uint32_t base = warp * 32; base < sq; base += PROBE_THREADS) {
         const uint32_t i = base + lane;
@@ -55,7 +53,7 @@ index_probe_kernel(const uint32_t *__restrict__ q, uint32_t sq, uint64_t row0, c
             if ((i == 0 || __ldg(Q + i - 1) != v) && v <= vmax) {  // head of a value; larger values match nothing
                 cq = 1;
                 while (i + cq < sq && __ldg(Q + i + cq) == v) ++cq;
-                const uint32_t b = min(bucket_of(v, scale), nb - 1);
+                const uint32_t b = join_bucket(v, scale, nb);
                 uint64_t lo = start[b];
                 hi = start[b + 1];
                 const uint64_t key = (uint64_t)v << 32;
@@ -248,17 +246,7 @@ index_select_kernel(const uint32_t *__restrict__ acc, uint64_t n, uint64_t row0,
     while (P < m) P <<= 1;
     for (uint32_t i = m + threadIdx.x; i < P; i += SEL_THREADS) key[i] = ~0ull;
     __syncthreads();
-    for (uint32_t k2 = 2; k2 <= P; k2 <<= 1) {
-        for (uint32_t jd = k2 >> 1; jd > 0; jd >>= 1) {
-            for (uint32_t tt = threadIdx.x; tt < (P >> 1); tt += SEL_THREADS) {
-                const uint32_t i = ((tt & ~(jd - 1)) << 1) | (tt & (jd - 1)), ixj = i | jd;
-                const bool up = (i & k2) == 0;
-                const uint64_t a = key[i], b = key[ixj];
-                if ((a > b) == up) { key[i] = b; key[ixj] = a; }
-            }
-            __syncthreads();
-        }
-    }
+    block_bitonic_sort<uint64_t, SEL_THREADS>(key, P);
     for (uint32_t i = threadIdx.x; i < top_k; i += SEL_THREADS) {
         const uint64_t o = row * top_k + i;
         const uint32_t same = i < m ? 0xffffffffu - (uint32_t)(key[i] >> 32) : 0;

@@ -297,6 +297,25 @@ def test_distance_block_matches_pairs_and_oracle(gpu, oracle):
     assert np.array_equal(s2, same[5:11]) and np.array_equal(d2, dist[5:11])
 
 
+def test_distance_block_tile_shared_memory_limit(gpu):
+    """Unsorted sketches take the pairwise tile kernel, which stages two tiles of 8 sketches (2 * 8 * s words) in
+    at most 200 KB of shared memory: s = 3300 is refused with PG_ERR_UNSUPPORTED, and no output is written."""
+    import torch
+    from poly_b200 import _lib
+
+    n, s = 12, 3300
+    sk = np.random.default_rng(13).integers(0, 1 << 32, size=(n, s), dtype=np.uint32)
+    with pytest.raises(_lib.PolyError) as e:
+        mash.distance_block(sk)
+    assert e.value.code == _lib.PG_ERR_UNSUPPORTED
+    dev = torch.device("cuda", torch.cuda.current_device())
+    d_sk = torch.from_numpy(sk.view(np.int32)).to(dev)
+    d_same = torch.full((n, n), -1, dtype=torch.int32, device=dev)
+    rc = _lib.lib().pg_mash_distance_block_dev(d_sk.data_ptr(), n, s, 0, n, d_same.data_ptr(), None, torch.cuda.current_stream(dev).cuda_stream)
+    torch.cuda.synchronize(dev)
+    assert rc == _lib.PG_ERR_UNSUPPORTED and bool((d_same == -1).all())
+
+
 def test_full_size_properties_cfg2_slice(gpu, oracle):
     """BASELINE cfg2 shape at 2M reads (device path via host API): spot-check rows against
     the oracle, and a checksum-of-checksums that is independent of chunking."""

@@ -219,6 +219,11 @@ def test_errors_and_empty_batches(family):
         ref, same, dist, nh = ix.nearest(queries[:3], 5, min_same=10**6)  # nothing qualifies
         assert (nh == 0).all() and (ref == mash.NO_REF).all() and (same == 0).all() and (dist == 1.0).all()
         assert_same_result(ix.nearest(queries[:50], 10, max_distance=0.9), index_oracle.nearest(refs, queries[:50], 10, mash.min_same_for_distance(0.9, 500)))
+        # unsorted queries take the pairwise tile kernel: 8 * (6000 + 500) words of tiles exceed its 200 KB
+        unsorted = np.random.default_rng(9).integers(0, 1 << 32, size=(4, 6000), dtype=np.uint32)
+        with pytest.raises(_lib.PolyError) as e:
+            ix.nearest(unsorted, 5)
+        assert e.value.code == _lib.PG_ERR_UNSUPPORTED
 
 
 def test_sketch_file_index_equals_array_index(family, fill_sets):
