@@ -2,8 +2,9 @@
 // written positionally (/root/reference/search/mash/mash.go:73-84).
 //
 // Fast path (fixed-length reads, k in the instantiated set, compact output):
-//   * one CTA = one warp = one tile of 32 reads; the 32*L input bytes are contiguous in HBM and
-//     are brought in by ONE 1-D TMA bulk copy (cp.async.bulk + mbarrier; SASS UBLKCP);
+//   * one CTA = one persistent warp that loops over tiles of 32 reads; a tile's 32*L input
+//     bytes are contiguous in HBM and are brought in by ONE 1-D TMA bulk copy (cp.async.bulk +
+//     mbarrier; SASS UBLKCP), issued while the warp hashes its previous tile;
 //   * one THREAD per read walks the read 4 bytes per step.  The murmur3 block pre-mix
 //     K(p) = rotl(w(p)*c1,15)*c2 of the 4 bytes at position p is computed ONCE and kept
 //     in a register ring shared by the k/4 k-mers that consume it, so the cost per
@@ -31,77 +32,96 @@
 namespace pg {
 
 // ---- K1 fast path ----------------------------------------------------------------
-// smem: in tile (32*L bytes + 16 B over-read pad, 16-B rounded) | out tile (+ 1 KB static table when k % 4 == 1)
+// smem: 2 input stages (32*L bytes + 16 B over-read pad, 16-B rounded, each) | out tile
+// (+ 1 KB static table when k % 4 == 1)
 __host__ __device__ inline uint32_t k1_in_bytes(uint32_t L) {
     return (32u * L + 16u + 15u) & ~15u;
 }
+__host__ __device__ inline size_t k1_smem_bytes(uint32_t L, uint32_t nk) {
+    return 2 * (size_t)k1_in_bytes(L) + (size_t)32 * nk * 4;
+}
 
-// One CTA = one warp = one tile of 32 reads.
+// One CTA = one warp, persistent: it hashes tiles blockIdx.x, blockIdx.x + gridDim.x, ... of 32
+// reads (the host launches no more CTAs than there are tiles).  The barriers and the tail table
+// are set up once per CTA; the load of the next tile is in flight while this one is hashed, and
+// the single output tile is only waited for (its previous store has read it) just before reuse.
 // lut_stride == 4 arrives as a kernel argument so that the table address byte*4 + base
 // stays an IMAD (FMA pipe) instead of being strength-reduced to LEA (ALU pipe).
 template <int K>
 __global__ void __launch_bounds__(32)
 sketch_fill_uniform_kernel(const uint8_t *__restrict__ bases, const SketchDst dst,
-                           uint32_t L, uint32_t nk, uint32_t lut_stride) {
+                           uint32_t L, uint32_t nk, uint64_t n_tiles, uint32_t lut_stride) {
     PG_WALK_CONSTANTS;
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ __align__(16) uint32_t s_lut[LUT ? 256 : 4];
-    __shared__ __align__(8) uint64_t s_bar[2];  // [0]: the tile, [1]: the table
+    __shared__ __align__(8) uint64_t s_bar[3];  // [0], [1]: the input stages, [2]: the table
     const uint32_t tid = threadIdx.x;  // lane == read within the tile
-    uint8_t *s_in = smem;
-    uint32_t *s_out = reinterpret_cast<uint32_t *>(s_in + k1_in_bytes(L));
-
-    const uint64_t tile = blockIdx.x;
+    const uint32_t in_stage = k1_in_bytes(L);
+    uint32_t *s_out = reinterpret_cast<uint32_t *>(smem + 2 * in_stage);
     const uint32_t in_bytes = 32u * L;  // multiple of 16 (host guarantees)
+    const uint64_t stride = gridDim.x;
+    uint64_t tile = blockIdx.x;
 
     if (tid == 0) {
-        mbar_init(&s_bar[0], 1);
-        mbar_init(&s_bar[1], 1);
+        for (int b = 0; b < 3; ++b) mbar_init(&s_bar[b], 1);
         fence_mbar_init();
-        if (LUT) load_kmix_table(s_lut, &s_bar[1]);
+        if (LUT) load_kmix_table(s_lut, &s_bar[2]);
+        mbar_expect_tx(&s_bar[0], in_bytes);
+        bulk_g2s(smem, bases + tile * in_bytes, in_bytes, &s_bar[0]);
     }
     __syncthreads();  // barrier init visible to everyone
-    if (tid == 0) {
-        mbar_expect_tx(&s_bar[0], in_bytes);
-        bulk_g2s(s_in, bases + tile * in_bytes, in_bytes, &s_bar[0]);
-    }
-    mbar_wait(&s_bar[0], 0);
-    if (LUT) mbar_wait(&s_bar[1], 0);
+    if (LUT) mbar_wait(&s_bar[2], 0);
 
     // my read: bytes [tid*L, tid*L+L) of the tile, realigned to words on the fly
     const uint32_t b0 = tid * L;
-    const uint32_t *sw = reinterpret_cast<const uint32_t *>(s_in) + (b0 >> 2);
-    const uint8_t *sb = s_in + b0 + 4 * NB;  // tail byte of k-mer i is sb[i]
     const uint32_t sh = (b0 & 3u) * 8u;
     uint32_t *my_out = s_out + tid * nk;
     const uint32_t lut_base = smem_u32(s_lut);
 
-    PG_WALK_PROLOGUE
+    for (uint32_t c = 0; tile < n_tiles; tile += stride, ++c) {  // c: this CTA's tile counter
+        if (tid == 0) {
+            // prefetch into the other stage; its previous tile was consumed before the last __syncwarp
+            if (tile + stride < n_tiles) {
+                const uint32_t o = (c + 1) & 1u;
+                mbar_expect_tx(&s_bar[o], in_bytes);
+                bulk_g2s(smem + o * in_stage, bases + (tile + stride) * in_bytes, in_bytes, &s_bar[o]);
+            }
+            bulk_wait_read0();  // the previous tile's store has read the output tile
+        }
+        mbar_wait(&s_bar[c & 1u], (c >> 1) & 1u);
+        __syncwarp();
 
-    // At word step Q = NB + i/4 the k-mers i+r (r = 0..3) complete: their body blocks are
-    // ring[r][oldest .. newest], their tail bytes start at position i + r + 4*NB.
-    uint32_t i = 0;
-    const uint32_t n_main = (nk / (4 * NB)) * (4 * NB);
-    while (i < n_main) {  // full groups of NB word steps: no bounds tests
-#pragma unroll
-        for (int u = 0; u < NB; ++u) PG_K1_STEP(u, false)
-    }
-#pragma unroll
-    for (int u = 0; u < NB; ++u) {  // remainder: < NB full steps plus possibly a partial one
-        if (i < nk) PG_K1_STEP(u, true)
-    }
+        const uint8_t *s_in = smem + (c & 1u) * in_stage;
+        const uint32_t *sw = reinterpret_cast<const uint32_t *>(s_in) + (b0 >> 2);
+        const uint8_t *sb = s_in + b0 + 4 * NB;  // tail byte of k-mer i is sb[i]
 
-    // hand the staged tile to the async proxy and bulk-store it (positional, mash.go:81-84)
-    fence_async_smem();
-    __syncwarp();
-    if (tid == 0) {
-        // one bulk store per destination: the local buffer, or (fused all-gather) the gathered
-        // buffer of every rank, peers reached through their NVLink-mapped addresses
+        PG_WALK_PROLOGUE
+
+        // At word step Q = NB + i/4 the k-mers i+r (r = 0..3) complete: their body blocks are
+        // ring[r][oldest .. newest], their tail bytes start at position i + r + 4*NB.
+        uint32_t i = 0;
+        const uint32_t n_main = (nk / (4 * NB)) * (4 * NB);
+        while (i < n_main) {  // full groups of NB word steps: no bounds tests
 #pragma unroll
-        for (int p = 0; p < PG_MAX_PEERS; ++p)  // static indices: the struct stays in parameter space
-            if (p < dst.n) bulk_s2g(dst.ptr[p] + tile * (uint64_t)(32u * nk), s_out, 32u * nk * 4u);  // multiple of 16
-        bulk_wait_read0();
+            for (int u = 0; u < NB; ++u) PG_K1_STEP(u, false)
+        }
+#pragma unroll
+        for (int u = 0; u < NB; ++u) {  // remainder: < NB full steps plus possibly a partial one
+            if (i < nk) PG_K1_STEP(u, true)
+        }
+
+        // hand the staged tile to the async proxy and bulk-store it (positional, mash.go:81-84)
+        fence_async_smem();
+        __syncwarp();
+        if (tid == 0) {
+            // one bulk store per destination: the local buffer, or (fused all-gather) the gathered
+            // buffer of every rank, peers reached through their NVLink-mapped addresses
+#pragma unroll
+            for (int p = 0; p < PG_MAX_PEERS; ++p)  // static indices: the struct stays in parameter space
+                if (p < dst.n) bulk_s2g(dst.ptr[p] + tile * (uint64_t)(32u * nk), s_out, 32u * nk * 4u);  // multiple of 16
+        }
     }
+    if (tid == 0) bulk_wait_read0();
 }
 
 // ---- K1r: the same walk for RAGGED reads (every read in the fill regime) --------------------
@@ -224,9 +244,14 @@ sketch_fill_generic_kernel(const uint8_t *__restrict__ bases, const uint64_t *__
 template <int K>
 static int launch_k1(const uint8_t *d_bases, uint64_t n_tiles, uint32_t L, uint32_t nk,
                      const SketchDst &dst, cudaStream_t st) {
-    const size_t smem = k1_in_bytes(L) + (size_t)32 * nk * 4;
-    { const int rc_ = func_smem((const void *)sketch_fill_uniform_kernel<K>, smem); if (rc_ != PG_OK) return rc_; }
-    sketch_fill_uniform_kernel<K><<<(unsigned)n_tiles, 32, smem, st>>>(d_bases, dst, L, nk, 4u);
+    const void *fn = (const void *)sketch_fill_uniform_kernel<K>;
+    const size_t smem = k1_smem_bytes(L, nk);
+    { const int rc_ = func_smem(fn, smem); if (rc_ != PG_OK) return rc_; }
+    int per_sm = 0;
+    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 32, smem));
+    // persistent: the CTAs that are resident at once, and none without a tile
+    const uint64_t grid = std::min<uint64_t>(n_tiles, (uint64_t)sm_count() * std::max(per_sm, 1));
+    sketch_fill_uniform_kernel<K><<<(unsigned)grid, 32, smem, st>>>(d_bases, dst, L, nk, n_tiles, 4u);
     PG_LAUNCH_CHECK("sketch_fill_uniform_kernel");
     return PG_OK;
 }
@@ -276,22 +301,15 @@ int launch_sketch_uniform(const uint8_t *d_bases, uint64_t n_reads, uint32_t L, 
     bool aligned = ((uintptr_t)d_bases % 16 == 0) && ((uintptr_t)d_out % 16 == 0);
     if (extra)
         for (int p = 0; p < extra->n; ++p) aligned = aligned && ((uintptr_t)extra->ptr[p] % 16 == 0);
-    const size_t smem1 = k1_in_bytes(L) + (size_t)32 * nk * 4;
-    if (compact && aligned && nk > 0 && (32 * (uint64_t)L) % 16 == 0 && smem1 <= 100 * 1024 && n_reads >= 32) {
-        const uint64_t tiles = n_reads / 32;  // one CTA per tile of 32 reads
+    const size_t tile_bytes = k1_in_bytes(L) + (size_t)32 * nk * 4;  // one input stage + the output tile
+    if (compact && aligned && nk > 0 && (32 * (uint64_t)L) % 16 == 0 && tile_bytes <= 100 * 1024 && n_reads >= 32) {
+        const uint64_t tiles = n_reads / 32;
+        SketchDst dst;
+        dst.n = extra ? extra->n : 1;
+        for (int p = 0; p < dst.n; ++p) dst.ptr[p] = extra ? extra->ptr[p] : d_out;
         bool handled = false;
-        uint64_t t0 = 0;
-        while (t0 < tiles) {
-            const uint64_t nt = std::min<uint64_t>(tiles - t0, 0x7fffffffull);  // grid.x limit
-            SketchDst dst;
-            dst.n = extra ? extra->n : 1;
-            for (int p = 0; p < dst.n; ++p)
-                dst.ptr[p] = (extra ? extra->ptr[p] : d_out) + t0 * 32 * (uint64_t)nk;
-            int rc = dispatch_k1(k, d_bases + t0 * 32 * (uint64_t)L, nt, L, nk, dst, st, &handled);
-            if (rc != PG_OK) return rc;
-            if (!handled) break;
-            t0 += nt;
-        }
+        const int rc = dispatch_k1(k, d_bases, tiles, L, nk, dst, st, &handled);
+        if (rc != PG_OK) return rc;
         if (handled) {
             done = tiles * 32;
             if (d_status) PG_CUDA(cudaMemsetAsync(d_status, 0, done * sizeof(int32_t), st));
