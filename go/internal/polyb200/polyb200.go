@@ -505,3 +505,34 @@ func (ix *Index) Close() error {
 	ix.h = nil
 	return locked(func() C.int { return C.pg_mash_index_free(h) })
 }
+
+// SeqhashBatch wraps pg_seqhash_batch: digest[32*i:32*i+32], errCode[i] and errPos[i] for each of the
+// sequences bases[offsets[i]:offsets[i+1]], all of one seqType (0 DNA, 1 RNA, 2 PROTEIN) and flags
+// (1 circular | 2 double-stranded).
+func SeqhashBatch(bases []byte, offsets []uint64, seqType int32, flags uint32) (digest []byte, errCode []int32, errPos []uint64, err error) {
+	n := len(offsets) - 1
+	digest, errCode, errPos = make([]byte, 32*n+32), make([]int32, n+1), make([]uint64, n+1)
+	var p *C.uint8_t
+	if len(bases) > 0 {
+		p = (*C.uint8_t)(unsafe.Pointer(&bases[0]))
+	}
+	err = locked(func() C.int {
+		return C.pg_seqhash_batch(p, (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n), C.int32_t(seqType), C.uint32_t(flags),
+			(*C.uint8_t)(unsafe.Pointer(&digest[0])), (*C.int32_t)(unsafe.Pointer(&errCode[0])), (*C.uint64_t)(unsafe.Pointer(&errPos[0])))
+	})
+	return digest[:32*n], errCode[:n], errPos[:n], err
+}
+
+// LeastRotationBatch wraps pg_least_rotation_batch: the smallest start of the least rotation of each sequence.
+func LeastRotationBatch(bases []byte, offsets []uint64) ([]uint64, error) {
+	n := len(offsets) - 1
+	rot := make([]uint64, n+1)
+	var p *C.uint8_t
+	if len(bases) > 0 {
+		p = (*C.uint8_t)(unsafe.Pointer(&bases[0]))
+	}
+	err := locked(func() C.int {
+		return C.pg_least_rotation_batch(p, (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n), (*C.uint64_t)(unsafe.Pointer(&rot[0])))
+	})
+	return rot[:n], err
+}

@@ -13,6 +13,7 @@
 //   poly::fasta::Parse / ParseAll            <- io/fasta/fasta.go:72-77,89-118,149-243
 //   poly::pcr::DesignPrimers* / SimulateSimple / Simulate <- primers/pcr/pcr.go:44-186
 //   poly::mash::ToJSON / FromJSON (the encoding/json shape of mash.Mash) and the PGSKETCH container
+//   poly::seqhash::Hash / HashBatch / RotateSequence <- seqhash/seqhash.go:78-223
 // A Go panic surfaces as poly::GoPanic; align's alphabet.Error as poly::align::AlphabetError.
 // The Go package in go/ (cgo) is the real drop-in; this header is what the tests in this
 // repository can compile and run (tests/test_gpu_hostcpp.py).  No compute happens here.
@@ -814,4 +815,71 @@ inline ParseResult Parse(const std::string &text) {
 }
 
 }  // namespace fastq
+
+namespace seqhash {
+// seqhash.go:64-68
+inline const std::string DNA = "DNA", RNA = "RNA", PROTEIN = "PROTEIN";
+
+// (seqhash, error message) per sequence; the message is empty on success.  A byte >= 0x80 ahead of any
+// letter outside the alphabet is reported as unsupported rather than guessed at (DESIGN.md §7).
+inline std::vector<std::pair<std::string, std::string>> HashBatch(const std::vector<std::string> &seqs, const std::string &sequenceType,
+                                                                  bool circular, bool doubleStranded) {
+    std::vector<std::pair<std::string, std::string>> out(seqs.size());
+    const int32_t type = sequenceType == DNA ? PG_SEQHASH_DNA : sequenceType == RNA ? PG_SEQHASH_RNA : sequenceType == PROTEIN ? PG_SEQHASH_PROTEIN : -1;
+    if (type < 0) {  // seqhash.go:151-153, before any GPU call
+        for (auto &o : out) o.second = "Only sequenceTypes of DNA, RNA, or PROTEIN allowed. Got sequenceType: " + sequenceType;
+        return out;
+    }
+    if (seqs.empty()) return out;
+    Flat f(seqs);
+    std::vector<uint8_t> digest(32 * seqs.size());
+    std::vector<int32_t> code(seqs.size());
+    std::vector<uint64_t> pos(seqs.size());
+    check(pg_seqhash_batch(f.bases.data(), f.offsets.data(), seqs.size(), type,
+                           (circular ? PG_SEQHASH_CIRCULAR : 0u) | (doubleStranded ? PG_SEQHASH_DOUBLE_STRANDED : 0u), digest.data(), code.data(),
+                           pos.data()));
+    static const char hex[] = "0123456789abcdef";
+    for (size_t i = 0; i < seqs.size(); ++i) {
+        if (code[i] == 1) {
+            char c = seqs[i][pos[i]];
+            if (c >= 'a' && c <= 'z') c -= 32;
+            out[i].second = (type == PG_SEQHASH_PROTEIN ? "Only letters ACDEFGHIKLMNPQRSTVWYUO*BXZ are allowed for Proteins. Got letter: "
+                                                        : "Only letters ATUGCYRSWKMBDHVNZ are allowed for DNA/RNA. Got letter: ") + std::string(1, c);
+        } else if (code[i] == 2) {
+            out[i].second = "Proteins cannot be double stranded";
+        } else if (code[i] == 3) {
+            out[i].second = "unsupported: byte >= 0x80 at " + std::to_string(pos[i]) + " (strings.ToUpper would re-encode it)";
+        } else {
+            std::string h = "v1_";
+            h += sequenceType[0];
+            h += circular ? 'C' : 'L';
+            h += doubleStranded ? 'D' : 'S';
+            h += '_';
+            for (int k = 0; k < 32; ++k) {
+                h += hex[digest[32 * i + k] >> 4];
+                h += hex[digest[32 * i + k] & 15];
+            }
+            out[i].first = h;
+        }
+    }
+    return out;
+}
+
+// seqhash.Hash (seqhash.go:141): (seqhash, error message)
+inline std::pair<std::string, std::string> Hash(const std::string &sequence, const std::string &sequenceType, bool circular, bool doubleStranded) {
+    return HashBatch({sequence}, sequenceType, circular, doubleStranded)[0];
+}
+
+// seqhash.RotateSequence (seqhash.go:127) of every sequence, in one call
+inline std::vector<std::string> RotateSequences(const std::vector<std::string> &seqs) {
+    std::vector<std::string> out(seqs.size());
+    if (seqs.empty()) return out;
+    Flat f(seqs);
+    std::vector<uint64_t> rot(seqs.size());
+    check(pg_least_rotation_batch(f.bases.data(), f.offsets.data(), seqs.size(), rot.data()));
+    for (size_t i = 0; i < seqs.size(); ++i) out[i] = seqs[i].substr(rot[i]) + seqs[i].substr(0, rot[i]);
+    return out;
+}
+inline std::string RotateSequence(const std::string &sequence) { return RotateSequences({sequence})[0]; }
+}  // namespace seqhash
 }  // namespace poly

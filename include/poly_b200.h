@@ -23,7 +23,9 @@
  *     synchronise the given stream before returning because a host decision depends
  *     on a device result: pg_mash_distance_block_dev / pg_mash_distance_sparse_dev
  *     (sortedness and bucket sizes choose the algorithm), pg_fastq_ingest_dev /
- *     pg_fasta_ingest_dev (they return counts and the error position by value), and
+ *     pg_fasta_ingest_dev (they return counts and the error position by value),
+ *     pg_seqhash_batch_dev (waits for earlier work on the stream to read the total length, but not
+ *     for its own kernels), and
  *     pg_mash_sketch_batch_dev for ragged batches the threshold path does not take
  *     (s < 2, or more than 4 Mi row x item slots) when they hold few long sequences;
  *   - there is NO CPU fallback: without a usable sm_90 device every compute entry
@@ -423,6 +425,40 @@ int pg_fasta_ingest_dev(const uint8_t *d_text, uint64_t nbytes, uint32_t max_lin
                         uint64_t names_cap, uint64_t *d_name_offsets, uint64_t records_cap,
                         uint64_t *n_records, uint64_t *total_bases, uint64_t *total_name_bytes,
                         int32_t *err_code, uint64_t *err_line, void *stream);
+
+/* ---- seqhash.Hash -- seqhash/seqhash.go:141-223 ----------------------------------------------------
+ * One call hashes sequences [offsets[i], offsets[i+1]) of `seqs` (n + 1 offsets), all of one
+ * seq_type (PG_SEQHASH_DNA / _RNA / _PROTEIN) and with one set of flags (PG_SEQHASH_CIRCULAR |
+ * PG_SEQHASH_DOUBLE_STRANDED); another seq_type or flag bit is PG_ERR_ARG.  Per sequence, as Hash:
+ * ASCII upper-case, U -> T for RNA, the alphabet check in order (DNA/RNA "ATUGCYRSWKMBDHVNZ", protein
+ * "ACDEFGHIKLMNPQRSTVWYUO*BXZ"), then "Proteins cannot be double stranded"; the deterministic
+ * sequence (least rotation when circular, the smaller of s and transform.ReverseComplement(s) -- or of
+ * their least rotations -- when double-stranded; the complement of the DNA letters U and Z is the
+ * byte 0x00, as in the reference) and digest[32 i .. 32 i + 31] = BLAKE3-256 of it.  The Seqhash
+ * string is "v1_" + {D,R,P} + {C,L} + {D,S} + "_" + hex(digest).
+ * err_code[i]: 0 ok; 1 a letter outside the alphabet, err_pos[i] = its byte index; 2 "Proteins cannot
+ * be double stranded"; 3 a byte >= 0x80 comes before any letter outside the alphabet (strings.ToUpper
+ * would re-encode it: unsupported, not hashed; err_pos[i] = its byte index).  Failed sequences get a
+ * zero digest; err_code and err_pos may be NULL.  Sequences may be of any length: the host entry point
+ * hashes them in groups under a device-memory budget (a single sequence needs about twice its length
+ * of device memory; PG_ERR_NOMEM when that does not fit).
+ * pg_seqhash_batch_dev: device pointers, max_len >= every sequence length, digest 4-byte aligned.  It
+ * reads offsets[0] and offsets[n] back to the host to size its scratch (so it waits for earlier work on
+ * the stream), then only enqueues: it returns before the hashes are computed. */
+#define PG_SEQHASH_DNA 0
+#define PG_SEQHASH_RNA 1
+#define PG_SEQHASH_PROTEIN 2
+#define PG_SEQHASH_CIRCULAR 1u
+#define PG_SEQHASH_DOUBLE_STRANDED 2u
+int pg_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, int32_t seq_type,
+                     uint32_t flags, uint8_t *digest, int32_t *err_code, uint64_t *err_pos);
+int pg_seqhash_batch_dev(const uint8_t *d_seqs, const uint64_t *d_offsets, uint64_t n, int32_t seq_type,
+                         uint32_t flags, uint8_t *d_digest, int32_t *d_err_code, uint64_t *d_err_pos,
+                         uint64_t max_len, void *stream);
+/* seqhash.RotateSequence / boothLeastRotation (seqhash.go:78-138) on the raw bytes (no case folding):
+ * rotation[i] = the smallest start of the lexicographically least rotation of sequence i (0 when
+ * empty); RotateSequence(s) = s[r:] + s[:r]. */
+int pg_least_rotation_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, uint64_t *rotation);
 
 /* ---- synthetic workloads (SURVEY.md 8d; bench/test tooling, not a reference API) ---
  * kind 0: independent reads  base(i,j) = code(seed, i*L + j)

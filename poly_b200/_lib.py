@@ -90,6 +90,9 @@ _SIGS = {
                                   C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(C.c_uint64)]),
     "pg_fasta_ingest_dev": (C.c_int, [_u8p, C.c_uint64, C.c_uint32, C.c_uint32, _u8p, C.c_uint64, _u64p, _u8p, C.c_uint64, _u64p, C.c_uint64,
                                       C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.c_void_p]),
+    "pg_seqhash_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_int32, C.c_uint32, _u8p, _i32p, _u64p]),
+    "pg_seqhash_batch_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_int32, C.c_uint32, _u8p, _i32p, _u64p, C.c_uint64, C.c_void_p]),
+    "pg_least_rotation_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p]),
     "pg_synth_reads_dev": (C.c_int, [_u8p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_int32, C.c_uint32, C.c_void_p]),
 }
 EXPORTS = tuple(_SIGS)

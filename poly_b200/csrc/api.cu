@@ -1665,6 +1665,105 @@ int pg_fasta_ingest(const uint8_t *text, uint64_t nbytes, uint32_t max_line_size
 }
 
 // ---------------------------------------------------------------------------------
+static int seqhash_check(int32_t seq_type, uint32_t flags) {
+    if (seq_type < PG_SEQHASH_DNA || seq_type > PG_SEQHASH_PROTEIN) {
+        set_error("seq_type %d is not PG_SEQHASH_DNA, _RNA or _PROTEIN", seq_type);
+        return PG_ERR_ARG;
+    }
+    if (flags & ~(PG_SEQHASH_CIRCULAR | PG_SEQHASH_DOUBLE_STRANDED)) {
+        set_error("unknown seqhash flag bits 0x%x", flags);
+        return PG_ERR_ARG;
+    }
+    return PG_OK;
+}
+
+static int check_offsets(const uint64_t *offsets, uint64_t n) {
+    if (!offsets) { set_error("null offsets"); return PG_ERR_ARG; }
+    for (uint64_t i = 0; i < n; ++i)
+        if (offsets[i + 1] < offsets[i]) { set_error("offsets decrease at %llu", (unsigned long long)i); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+int pg_seqhash_batch_dev(const uint8_t *d_seqs, const uint64_t *d_offsets, uint64_t n, int32_t seq_type, uint32_t flags,
+                         uint8_t *d_digest, int32_t *d_err_code, uint64_t *d_err_pos, uint64_t max_len, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK || (rc = seqhash_check(seq_type, flags)) != PG_OK) return rc;
+    if (n == 0) return PG_OK;
+    if (!d_offsets || !d_digest) { set_error("null offsets or digest"); return PG_ERR_ARG; }
+    cudaStream_t st = (cudaStream_t)stream;
+    uint64_t first = 0, last = 0;  // the scratch is sized by the total length
+    PG_CUDA(cudaMemcpyAsync(&first, d_offsets, 8, cudaMemcpyDeviceToHost, st));
+    PG_CUDA(cudaMemcpyAsync(&last, d_offsets + n, 8, cudaMemcpyDeviceToHost, st));
+    PG_CUDA(cudaStreamSynchronize(st));
+    if (last < first) { set_error("offsets[n] < offsets[0]"); return PG_ERR_ARG; }
+    return launch_seqhash(d_seqs, d_offsets, n, max_len, last - first, seq_type, flags, d_digest, d_err_code, d_err_pos, st);
+}
+
+int pg_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, int32_t seq_type, uint32_t flags, uint8_t *digest,
+                     int32_t *err_code, uint64_t *err_pos) {
+    int rc = ensure_device();
+    if (rc != PG_OK || (rc = seqhash_check(seq_type, flags)) != PG_OK) return rc;
+    if (n == 0) return PG_OK;
+    if ((rc = check_offsets(offsets, n)) != PG_OK) return rc;
+    if (!digest) { set_error("null digest"); return PG_ERR_ARG; }
+    // Sequences go to the device in groups whose device memory stays within the budget (a single longer
+    // sequence is a group of its own): input and canonical copy, one 32-byte chaining value per KiB and
+    // per sequence, offsets, orientation, error and digest words per sequence.
+    uint64_t budget = 2ull << 30;
+    if (const char *e = getenv("PG_SEQHASH_GROUP_BYTES")) budget = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
+    auto cost = [&](uint64_t g, uint64_t e) {
+        const uint64_t bytes = offsets[e] - offsets[g], cnt = e - g;
+        return 2 * bytes + 64 + 32 * (bytes / 1024 + cnt) + 101 * cnt;
+    };
+    std::lock_guard<std::mutex> lk(t_ctx->mu);
+    cudaStream_t st = t_ctx->streams[0];
+    for (uint64_t g = 0; g < n;) {
+        uint64_t e = g + 1, max_len = offsets[g + 1] - offsets[g];
+        while (e < n && cost(g, e + 1) <= budget) {
+            max_len = std::max<uint64_t>(max_len, offsets[e + 1] - offsets[e]);
+            ++e;
+        }
+        const uint64_t cnt = e - g, b0 = offsets[g], bytes = offsets[e] - b0;
+        Tmp d_b(st), d_off(st), d_dig(st), d_err(st), d_pos(st);
+        if ((rc = d_b.alloc(bytes)) || (rc = d_off.alloc((cnt + 1) * 8)) || (rc = d_dig.alloc(cnt * 32)) || (rc = d_err.alloc(cnt * 4)) ||
+            (rc = d_pos.alloc(cnt * 8)))
+            return rc;
+        if (bytes) PG_CUDA(cudaMemcpyAsync(d_b.p, seqs + b0, bytes, cudaMemcpyHostToDevice, st));
+        PG_CUDA(cudaMemcpyAsync(d_off.p, offsets + g, (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
+        rc = launch_seqhash(d_b.as<uint8_t>() - b0, d_off.as<uint64_t>(), cnt, max_len, bytes, seq_type, flags, d_dig.as<uint8_t>(),
+                            d_err.as<int32_t>(), d_pos.as<uint64_t>(), st);
+        if (rc != PG_OK) return rc;
+        PG_CUDA(cudaMemcpyAsync(digest + 32 * g, d_dig.p, cnt * 32, cudaMemcpyDeviceToHost, st));
+        if (err_code) PG_CUDA(cudaMemcpyAsync(err_code + g, d_err.p, cnt * 4, cudaMemcpyDeviceToHost, st));
+        if (err_pos) PG_CUDA(cudaMemcpyAsync(err_pos + g, d_pos.p, cnt * 8, cudaMemcpyDeviceToHost, st));
+        PG_CUDA(cudaStreamSynchronize(st));
+        g = e;
+    }
+    return PG_OK;
+}
+
+int pg_least_rotation_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, uint64_t *rotation) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n == 0) return PG_OK;
+    if ((rc = check_offsets(offsets, n)) != PG_OK) return rc;
+    if (!rotation) { set_error("null rotation"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(t_ctx->mu);
+    cudaStream_t st = t_ctx->streams[0];
+    const uint64_t b0 = offsets[0], bytes = offsets[n] - b0;
+    uint64_t max_len = 0;
+    for (uint64_t i = 0; i < n; ++i) max_len = std::max<uint64_t>(max_len, offsets[i + 1] - offsets[i]);
+    Tmp d_b(st), d_off(st), d_rot(st);
+    if ((rc = d_b.alloc(bytes)) || (rc = d_off.alloc((n + 1) * 8)) || (rc = d_rot.alloc(n * 8))) return rc;
+    if (bytes) PG_CUDA(cudaMemcpyAsync(d_b.p, seqs + b0, bytes, cudaMemcpyHostToDevice, st));
+    PG_CUDA(cudaMemcpyAsync(d_off.p, offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
+    if ((rc = launch_least_rotation(d_b.as<uint8_t>() - b0, d_off.as<uint64_t>(), n, max_len, d_rot.as<uint64_t>(), st)) != PG_OK) return rc;
+    PG_CUDA(cudaMemcpyAsync(rotation, d_rot.p, n * 8, cudaMemcpyDeviceToHost, st));
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
+}
+
+// ---------------------------------------------------------------------------------
 int pg_synth_reads_dev(uint8_t *d_bases, uint64_t first_read, uint64_t n_reads, uint32_t read_len,
                        uint64_t seed, int32_t kind, uint32_t family, void *stream) {
     int rc = ensure_device();

@@ -241,6 +241,12 @@ int launch_fasta_ingest(const uint8_t *d_text, uint64_t nbytes, uint32_t max_lin
                         uint64_t names_cap, uint64_t *d_name_offsets, uint64_t records_cap, uint64_t *n_records,
                         uint64_t *total_bases, uint64_t *total_name_bytes, int32_t *err_code, uint64_t *err_line,
                         cudaStream_t st);
+// seqhash.cu: digests (n x 32 bytes), error codes and positions of pg_seqhash_batch for sequences of at most
+// max_len bytes, total = off[n] - off[0]
+int launch_seqhash(const uint8_t *d_in, const uint64_t *d_off, uint64_t n, uint64_t max_len, uint64_t total, int seq_type,
+                   uint32_t flags, uint8_t *d_digest, int32_t *d_err, uint64_t *d_pos, cudaStream_t st);
+int launch_least_rotation(const uint8_t *d_in, const uint64_t *d_off, uint64_t n, uint64_t max_len, uint64_t *d_rotation,
+                          cudaStream_t st);
 // synth.cu
 int launch_synth_reads(uint8_t *d_bases, uint64_t first_read, uint64_t n_reads, uint32_t read_len,
                        uint64_t seed, int kind, uint32_t family, cudaStream_t st);
