@@ -28,6 +28,10 @@
  *     for its own kernels), and
  *     pg_mash_sketch_batch_dev for ragged batches the threshold path does not take
  *     (s < 2, or more than 4 Mi row x item slots) when they hold few long sequences;
+ *   - a ragged batch of n items passes n + 1 offsets, item i being [offsets[i], offsets[i+1]).
+ *     Offsets must not decrease: the host-pointer entry points return PG_ERR_ARG if they do,
+ *     without launching anything (pg_mash_sketch_batch and its _multi form check each chunk
+ *     as they stage it, so earlier chunks may have run);
  *   - there is NO CPU fallback: without a usable sm_90 device every compute entry
  *     point fails with PG_ERR_NO_DEVICE.
  */

@@ -275,21 +275,144 @@ static inline uint64_t kmers_of(uint64_t len, int k) { return len > (uint64_t)k 
 
 }  // namespace pg
 
-// small RAII helper for temporary device buffers of the non-pipelined host paths
+// Staging for the one-shot host-pointer entry points: every step of such a call goes through a HostCall.
 namespace pg {
 namespace {
-struct Tmp {
-    void *p = nullptr;
-    cudaStream_t st;
-    explicit Tmp(cudaStream_t s) : st(s) {}
-    int alloc(size_t bytes) {
-        cudaError_t e = cudaMallocAsync(&p, bytes ? bytes : 16, st);
-        if (e != cudaSuccess) { set_error("cudaMallocAsync(%zu): %s", bytes, cudaGetErrorString(e)); cudaGetLastError(); return PG_ERR_NOMEM; }
-        return PG_OK;
+// `count` elements of T from `tmp`, at least 16 bytes
+template <typename T>
+int scratch_alloc(StreamScratch &tmp, T **p, uint64_t count) {
+    const uint64_t bytes = count * sizeof(T);
+    uint8_t *b = nullptr;
+    cudaError_t e = tmp.alloc(&b, std::max<uint64_t>(bytes, 16));
+    if (e != cudaSuccess) { set_error("cudaMallocAsync(%zu): %s", (size_t)bytes, cudaGetErrorString(e)); cudaGetLastError(); return PG_ERR_NOMEM; }
+    *p = (T *)b;
+    return PG_OK;
+}
+
+// Host ragged batches: item i is [offsets[i], offsets[i+1]) and offsets never decrease (a decrease would
+// hand a kernel a length near 2^64).  *max_len = the longest item.
+int check_ragged(const uint64_t *offsets, uint64_t n, uint64_t *max_len) {
+    uint64_t m = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        if (offsets[i + 1] < offsets[i]) { set_error("offsets decrease at %llu", (unsigned long long)i); return PG_ERR_ARG; }
+        m = std::max(m, offsets[i + 1] - offsets[i]);
     }
-    ~Tmp() { if (p) cudaFreeAsync(p, st); }
-    template <typename T> T *as() { return (T *)p; }
+    *max_len = m;
+    return PG_OK;
+}
+
+// a ragged batch on the device: item i is base[off[i] .. off[i+1]) with the caller's own offsets
+template <typename T>
+struct Ragged {
+    const T *base;
+    const uint64_t *off;
+    uint64_t max_len;
 };
+
+// One call of a host-pointer entry point on the current device: holds the device's lock, runs on its
+// first stream and owns the call's device temporaries.  The first error sticks: later steps do nothing
+// and finish() returns it.  Unless finish() ran, the destructor waits for the stream, so that no copy
+// into or out of the caller's memory is still running when the entry point returns.
+class HostCall {
+    std::lock_guard<std::mutex> lock_;
+    StreamScratch tmp_;
+    int rc_ = PG_OK;
+    bool finished_ = false;
+    void copy(void *dst, const void *src, uint64_t bytes, cudaMemcpyKind kind) {
+        if (rc_ != PG_OK) return;
+        cudaError_t e = cudaMemcpyAsync(dst, src, bytes, kind, st);
+        if (e != cudaSuccess) rc_ = cuda_fail(e, "cudaMemcpyAsync", __FILE__, __LINE__);
+    }
+
+public:
+    const cudaStream_t st;
+    HostCall() : lock_(t_ctx->mu), tmp_(t_ctx->streams[0]), st(t_ctx->streams[0]) {}
+    ~HostCall() {
+        if (finished_) return;
+        cudaStreamSynchronize(st);
+        cudaGetLastError();
+    }
+    int error() const { return rc_; }
+    // nullptr once an error has occurred
+    template <typename T>
+    T *alloc(uint64_t count, bool zero = false) {
+        T *p = nullptr;
+        if (rc_ != PG_OK || (rc_ = scratch_alloc(tmp_, &p, count)) != PG_OK) return nullptr;
+        if (zero) {
+            cudaError_t e = cudaMemsetAsync(p, 0, count * sizeof(T), st);
+            if (e != cudaSuccess) { rc_ = cuda_fail(e, "cudaMemsetAsync", __FILE__, __LINE__); return nullptr; }
+        }
+        return p;
+    }
+    // h[0 .. count) on the device, in a buffer with room for `extra` more elements
+    template <typename T>
+    T *upload(const T *h, uint64_t count, uint64_t extra = 0) {
+        T *d = alloc<T>(count + extra);
+        if (count) copy(d, h, count * sizeof(T), cudaMemcpyHostToDevice);
+        return rc_ == PG_OK ? d : nullptr;
+    }
+    template <typename T>
+    void download(T *h, const T *d, uint64_t count) {
+        if (h && count) copy(h, d, count * sizeof(T), cudaMemcpyDeviceToHost);
+    }
+    // check_ragged, then items [offsets[0], offsets[n]) and the n + 1 offsets to the device
+    template <typename T>
+    Ragged<T> ragged(const T *items, const uint64_t *offsets, uint64_t n) {
+        Ragged<T> r{nullptr, nullptr, 0};
+        if (rc_ != PG_OK || (rc_ = check_ragged(offsets, n, &r.max_len)) != PG_OK) return r;
+        const uint64_t b0 = offsets[0];
+        const T *d = upload(items + b0, offsets[n] - b0);
+        r.off = upload(offsets, n + 1);
+        if (rc_ == PG_OK) r.base = d - b0;  // the kernels index with the absolute offsets
+        return r;
+    }
+    int sync() {
+        cudaError_t e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess && rc_ == PG_OK) rc_ = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+        return rc_;
+    }
+    int finish() {
+        finished_ = true;
+        return sync();
+    }
+};
+
+// Per-item statuses -> `status` (may be NULL) and the call's code: PG_ERR_PANIC if any item panics, else
+// PG_ERR_UNSUPPORTED if any is unsupported, with that code's message
+int fold_item_status(const std::vector<int32_t> &hst, int32_t *status, const char *panic_msg, const char *unsupported_msg) {
+    int worst = PG_OK;
+    for (size_t i = 0; i < hst.size(); ++i) {
+        if (status) status[i] = hst[i];
+        if (hst[i] == PG_ITEM_PANIC) worst = PG_ERR_PANIC;
+        else if (hst[i] == PG_ITEM_UNSUPPORTED && worst == PG_OK) worst = PG_ERR_UNSUPPORTED;
+    }
+    if (worst == PG_ERR_PANIC) set_error("%s", panic_msg);
+    if (worst == PG_ERR_UNSUPPORTED) set_error("%s", unsupported_msg);
+    return worst;
+}
+
+// a device output list whose first entries come back to the caller's array
+struct CappedList {
+    void *host;
+    const void *dev;
+    size_t elem_bytes;
+};
+
+// Ends a call whose kernel stored its entry count at d_n: *n_out = that count, and the first min(count, cap)
+// entries of every list come back.  More entries than cap is PG_ERR_ARG.
+int finish_capped(HostCall &c, const unsigned long long *d_n, uint64_t cap, uint64_t *n_out, std::initializer_list<CappedList> lists,
+                  const char *cap_name, const char *entries) {
+    unsigned long long found = 0;
+    c.download(&found, d_n, 1);
+    int rc = c.sync();
+    if (rc != PG_OK) return rc;
+    *n_out = found;
+    const uint64_t kept = std::min<uint64_t>(found, cap);
+    for (const CappedList &l : lists) c.download((uint8_t *)l.host, (const uint8_t *)l.dev, kept * l.elem_bytes);
+    if ((rc = c.finish()) != PG_OK) return rc;
+    if (found > cap) { set_error("%s %llu < %llu %s", cap_name, (unsigned long long)cap, found, entries); return PG_ERR_ARG; }
+    return PG_OK;
+}
 
 // Rows [rb, re) of a plan's matching counts and/or distances into host arrays that start at row rb, in row
 // blocks of <= 64 Mi pairs per pass
@@ -297,14 +420,15 @@ int plan_rows_to_host(const DistancePlan &plan, uint64_t rb, uint64_t re, uint32
     const uint64_t n = plan.n, rows_per = std::max<uint64_t>(8, ((64ull << 20) / n) & ~7ull);
     for (uint64_t b = rb; b < re; b += rows_per) {
         const uint64_t e = std::min(re, b + rows_per), cells = (e - b) * n;
-        Tmp d_same(st), d_dist(st);
+        StreamScratch tmp(st);
+        uint32_t *d_same = nullptr;
+        double *d_dist = nullptr;
         int rc;
-        if (same && (rc = d_same.alloc(cells * 4))) return rc;
-        if (distance && (rc = d_dist.alloc(cells * 8))) return rc;
-        rc = distance_plan_rows(plan, b, e, same ? d_same.as<uint32_t>() : nullptr, distance ? d_dist.as<double>() : nullptr, st);
-        if (rc != PG_OK) return rc;
-        if (same) PG_CUDA(cudaMemcpyAsync(same + (b - rb) * n, d_same.p, cells * 4, cudaMemcpyDeviceToHost, st));
-        if (distance) PG_CUDA(cudaMemcpyAsync(distance + (b - rb) * n, d_dist.p, cells * 8, cudaMemcpyDeviceToHost, st));
+        if (same && (rc = scratch_alloc(tmp, &d_same, cells))) return rc;
+        if (distance && (rc = scratch_alloc(tmp, &d_dist, cells))) return rc;
+        if ((rc = distance_plan_rows(plan, b, e, d_same, d_dist, st)) != PG_OK) return rc;
+        if (same) PG_CUDA(cudaMemcpyAsync(same + (b - rb) * n, d_same, cells * 4, cudaMemcpyDeviceToHost, st));
+        if (distance) PG_CUDA(cudaMemcpyAsync(distance + (b - rb) * n, d_dist, cells * 8, cudaMemcpyDeviceToHost, st));
         PG_CUDA(cudaStreamSynchronize(st));
     }
     return PG_OK;
@@ -1054,37 +1178,22 @@ int pg_mash_similarity_pairs(const uint32_t *sketches, const uint64_t *sk_offset
     if (rc != PG_OK) return rc;
     if (n_pairs == 0) return PG_OK;
     if (!sk_offsets || !pair_a || !pair_b) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t words = sk_offsets[n_sketches];
-    Tmp d_sk(st), d_off(st), d_a(st), d_b(st), d_same(st), d_sim(st), d_dist(st), d_st(st);
-    if ((rc = d_sk.alloc(words * 4)) || (rc = d_off.alloc((n_sketches + 1) * 8)) ||
-        (rc = d_a.alloc(n_pairs * 4)) || (rc = d_b.alloc(n_pairs * 4)) ||
-        (rc = d_same.alloc(n_pairs * 8)) || (rc = d_sim.alloc(n_pairs * 8)) ||
-        (rc = d_dist.alloc(n_pairs * 8)) || (rc = d_st.alloc(n_pairs * 4)))
+    HostCall c;
+    const Ragged<uint32_t> sk = c.ragged(sketches, sk_offsets, n_sketches);
+    const uint32_t *d_a = c.upload(pair_a, n_pairs), *d_b = c.upload(pair_b, n_pairs);
+    int64_t *d_same = c.alloc<int64_t>(n_pairs);
+    double *d_sim = c.alloc<double>(n_pairs), *d_dist = c.alloc<double>(n_pairs);
+    int32_t *d_st = c.alloc<int32_t>(n_pairs, true);
+    if ((rc = c.error()) || (rc = launch_similarity_pairs(sk.base, sk.off, n_sketches, d_a, d_b, n_pairs, d_same, d_sim, d_dist, d_st, c.st)))
         return rc;
-    if (words) PG_CUDA(cudaMemcpyAsync(d_sk.p, sketches, words * 4, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_off.p, sk_offsets, (n_sketches + 1) * 8, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_a.p, pair_a, n_pairs * 4, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_b.p, pair_b, n_pairs * 4, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemsetAsync(d_st.p, 0, n_pairs * 4, st));
-    rc = launch_similarity_pairs(d_sk.as<uint32_t>(), d_off.as<uint64_t>(), n_sketches, d_a.as<uint32_t>(),
-                                 d_b.as<uint32_t>(), n_pairs, d_same.as<int64_t>(), d_sim.as<double>(),
-                                 d_dist.as<double>(), d_st.as<int32_t>(), st);
-    if (rc != PG_OK) return rc;
     std::vector<int32_t> hst(n_pairs);
-    if (same) PG_CUDA(cudaMemcpyAsync(same, d_same.p, n_pairs * 8, cudaMemcpyDeviceToHost, st));
-    if (similarity) PG_CUDA(cudaMemcpyAsync(similarity, d_sim.p, n_pairs * 8, cudaMemcpyDeviceToHost, st));
-    if (distance) PG_CUDA(cudaMemcpyAsync(distance, d_dist.p, n_pairs * 8, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(hst.data(), d_st.p, n_pairs * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    bool panic = false;
-    for (uint64_t i = 0; i < n_pairs; ++i) {
-        if (status) status[i] = hst[i];
-        panic |= hst[i] != PG_ITEM_OK;
-    }
-    if (panic) { set_error("at least one pair involves an empty sketch or an invalid index (reference panics)"); return PG_ERR_PANIC; }
-    return PG_OK;
+    c.download(same, d_same, n_pairs);
+    c.download(similarity, d_sim, n_pairs);
+    c.download(distance, d_dist, n_pairs);
+    c.download(hst.data(), d_st, n_pairs);
+    if ((rc = c.finish())) return rc;
+    // the pair kernel reports no unsupported items
+    return fold_item_status(hst, status, "at least one pair involves an empty sketch or an invalid index (reference panics)", nullptr);
 }
 
 int pg_mash_distance_block_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint64_t row_begin,
@@ -1102,17 +1211,15 @@ int pg_mash_distance_block(const uint32_t *sketches, uint64_t n, int32_t s, uint
     if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
     if (row_end == row_begin || n == 0) return PG_OK;
     if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    Tmp d_sk(st);
-    if ((rc = d_sk.alloc(n * (uint64_t)s * 4))) return rc;
-    PG_CUDA(cudaMemcpyAsync(d_sk.p, sketches, n * (uint64_t)s * 4, cudaMemcpyHostToDevice, st));
+    HostCall c;
+    const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)s);
+    if ((rc = c.error())) return rc;
     // one plan (sortedness + join index) for the whole call
     DistancePlan plan;
-    rc = distance_plan_create(d_sk.as<uint32_t>(), n, s, st, &plan);
-    if (rc == PG_OK) rc = plan_rows_to_host(plan, row_begin, row_end, same, distance, st);
-    distance_plan_destroy(plan, st);
-    return rc;
+    rc = distance_plan_create(d_sk, n, s, c.st, &plan);
+    if (rc == PG_OK) rc = plan_rows_to_host(plan, row_begin, row_end, same, distance, c.st);
+    distance_plan_destroy(plan, c.st);
+    return rc != PG_OK ? rc : c.finish();
 }
 
 int pg_mash_distance_sparse_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint64_t row_begin, uint64_t row_end, uint32_t flags,
@@ -1136,29 +1243,13 @@ int pg_mash_distance_sparse(const uint32_t *sketches, uint64_t n, int32_t s, uin
     if (row_end == row_begin || n == 0) return PG_OK;
     if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
     if (pairs_cap && (!pair_i || !pair_j || !pair_same)) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    Tmp d_sk(st), d_i(st), d_j(st), d_c(st), d_n(st);
-    if ((rc = d_sk.alloc(n * (uint64_t)s * 4)) || (rc = d_i.alloc(pairs_cap * 4)) || (rc = d_j.alloc(pairs_cap * 4)) ||
-        (rc = d_c.alloc(pairs_cap * 4)) || (rc = d_n.alloc(8)))
+    HostCall c;
+    const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)s);
+    uint32_t *d_i = c.alloc<uint32_t>(pairs_cap), *d_j = c.alloc<uint32_t>(pairs_cap), *d_c = c.alloc<uint32_t>(pairs_cap);
+    unsigned long long *d_n = c.alloc<unsigned long long>(1);
+    if ((rc = c.error()) || (rc = launch_distance_sparse(d_sk, n, s, row_begin, row_end, flags, d_i, d_j, d_c, pairs_cap, d_n, c.st)))
         return rc;
-    PG_CUDA(cudaMemcpyAsync(d_sk.p, sketches, n * (uint64_t)s * 4, cudaMemcpyHostToDevice, st));
-    rc = launch_distance_sparse(d_sk.as<uint32_t>(), n, s, row_begin, row_end, flags, d_i.as<uint32_t>(), d_j.as<uint32_t>(), d_c.as<uint32_t>(),
-                                pairs_cap, d_n.as<unsigned long long>(), st);
-    if (rc != PG_OK) return rc;
-    unsigned long long found = 0;
-    PG_CUDA(cudaMemcpyAsync(&found, d_n.p, 8, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    *n_pairs = found;
-    const uint64_t kept = std::min<uint64_t>(found, pairs_cap);
-    if (kept) {
-        PG_CUDA(cudaMemcpyAsync(pair_i, d_i.p, kept * 4, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaMemcpyAsync(pair_j, d_j.p, kept * 4, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaMemcpyAsync(pair_same, d_c.p, kept * 4, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaStreamSynchronize(st));
-    }
-    if (found > pairs_cap) { set_error("pairs_cap %llu < %llu pairs", (unsigned long long)pairs_cap, found); return PG_ERR_ARG; }
-    return PG_OK;
+    return finish_capped(c, d_n, pairs_cap, n_pairs, {{pair_i, d_i, 4}, {pair_j, d_j, 4}, {pair_same, d_c, 4}}, "pairs_cap", "pairs");
 }
 
 // ---------------------------------------------------------------------------------
@@ -1236,23 +1327,18 @@ int pg_mash_index_query(const pg_mash_index *ix, const uint32_t *queries, uint64
     if (nq == 0) return PG_OK;
     if (sq <= 0) { set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq); return PG_ERR_PANIC; }
     if (!queries) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
+    HostCall c;
     const uint64_t slots = nq * (uint64_t)top_k;
-    Tmp d_q(st), d_ref(st), d_same(st), d_dist(st), d_nh(st);
-    if ((rc = d_q.alloc(nq * (uint64_t)sq * 4)) || (hit_ref && (rc = d_ref.alloc(slots * 4))) || (hit_same && (rc = d_same.alloc(slots * 4))) ||
-        (hit_distance && (rc = d_dist.alloc(slots * 8))) || (n_hits && (rc = d_nh.alloc(nq * 4))))
-        return rc;
-    PG_CUDA(cudaMemcpyAsync(d_q.p, queries, nq * (uint64_t)sq * 4, cudaMemcpyHostToDevice, st));
-    rc = launch_index_query(ix->plan, d_q.as<uint32_t>(), nq, sq, top_k, min_same, d_ref.as<uint32_t>(), d_same.as<uint32_t>(),
-                            d_dist.as<double>(), d_nh.as<uint32_t>(), st);
-    if (rc != PG_OK) return rc;
-    if (hit_ref) PG_CUDA(cudaMemcpyAsync(hit_ref, d_ref.p, slots * 4, cudaMemcpyDeviceToHost, st));
-    if (hit_same) PG_CUDA(cudaMemcpyAsync(hit_same, d_same.p, slots * 4, cudaMemcpyDeviceToHost, st));
-    if (hit_distance) PG_CUDA(cudaMemcpyAsync(hit_distance, d_dist.p, slots * 8, cudaMemcpyDeviceToHost, st));
-    if (n_hits) PG_CUDA(cudaMemcpyAsync(n_hits, d_nh.p, nq * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    return PG_OK;
+    const uint32_t *d_q = c.upload(queries, nq * (uint64_t)sq);
+    uint32_t *d_ref = hit_ref ? c.alloc<uint32_t>(slots) : nullptr, *d_same = hit_same ? c.alloc<uint32_t>(slots) : nullptr;
+    double *d_dist = hit_distance ? c.alloc<double>(slots) : nullptr;
+    uint32_t *d_nh = n_hits ? c.alloc<uint32_t>(nq) : nullptr;
+    if ((rc = c.error()) || (rc = launch_index_query(ix->plan, d_q, nq, sq, top_k, min_same, d_ref, d_same, d_dist, d_nh, c.st))) return rc;
+    c.download(hit_ref, d_ref, slots);
+    c.download(hit_same, d_same, slots);
+    c.download(hit_distance, d_dist, slots);
+    c.download(n_hits, d_nh, nq);
+    return c.finish();
 }
 
 int pg_mash_index_free(pg_mash_index *ix) {
@@ -1292,27 +1378,18 @@ static int align_score_host(int global, const uint8_t *queries, const uint64_t *
     if (rc != PG_OK) return rc;
     if (n_queries == 0) return PG_OK;
     if (!q_offsets || !score || !lut_a || !lut_b || !table) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t q0 = q_offsets[0], qbytes = q_offsets[n_queries] - q0;
-    uint64_t maxq = 0;
-    for (uint64_t i = 0; i < n_queries; ++i) maxq = std::max(maxq, q_offsets[i + 1] - q_offsets[i]);
-    Tmp d_q(st), d_off(st), d_t(st), d_sc(st), d_ec(st), d_ep(st);
-    if ((rc = d_q.alloc(qbytes)) || (rc = d_off.alloc((n_queries + 1) * 8)) || (rc = d_t.alloc(templ_len)) ||
-        (rc = d_sc.alloc(n_queries * 8)) || (rc = d_ec.alloc(n_queries * 4)) || (rc = d_ep.alloc(n_queries * 8)))
+    HostCall c;
+    const Ragged<uint8_t> q = c.ragged(queries, q_offsets, n_queries);
+    const uint8_t *d_t = c.upload(templ, templ_len);
+    int64_t *d_sc = c.alloc<int64_t>(n_queries), *d_ep = c.alloc<int64_t>(n_queries);
+    int32_t *d_ec = c.alloc<int32_t>(n_queries);
+    if ((rc = c.error()) || (rc = launch_sw_score(q.base, q.off, n_queries, q.max_len, d_t, templ_len, query_is_a, lut_a, lut_b, table, n_a, n_b,
+                                                  gap, d_sc, d_ec, d_ep, c.st, global)))
         return rc;
-    if (qbytes) PG_CUDA(cudaMemcpyAsync(d_q.p, queries + q0, qbytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_off.p, q_offsets, (n_queries + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (templ_len) PG_CUDA(cudaMemcpyAsync(d_t.p, templ, templ_len, cudaMemcpyHostToDevice, st));
-    rc = launch_sw_score(d_q.as<uint8_t>() - q0, d_off.as<uint64_t>(), n_queries, maxq, d_t.as<uint8_t>(), templ_len,
-                         query_is_a, lut_a, lut_b, table, n_a, n_b, gap, d_sc.as<int64_t>(), d_ec.as<int32_t>(),
-                         d_ep.as<int64_t>(), st, global);
-    if (rc != PG_OK) return rc;
-    PG_CUDA(cudaMemcpyAsync(score, d_sc.p, n_queries * 8, cudaMemcpyDeviceToHost, st));
-    if (err_code) PG_CUDA(cudaMemcpyAsync(err_code, d_ec.p, n_queries * 4, cudaMemcpyDeviceToHost, st));
-    if (err_pos) PG_CUDA(cudaMemcpyAsync(err_pos, d_ep.p, n_queries * 8, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    return PG_OK;
+    c.download(score, d_sc, n_queries);
+    c.download(err_code, d_ec, n_queries);
+    c.download(err_pos, d_ep, n_queries);
+    return c.finish();
 }
 
 int pg_sw_score_batch_dev(const uint8_t *d_queries, const uint64_t *d_q_offsets, uint64_t n_queries,
@@ -1359,35 +1436,25 @@ static int align_strings_host(int global, const uint8_t *queries, const uint64_t
         set_error("null buffer");
         return PG_ERR_ARG;
     }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t q0 = q_offsets[0], qbytes = q_offsets[n_queries] - q0;
-    uint64_t maxq = 0;
-    for (uint64_t i = 0; i < n_queries; ++i) maxq = std::max(maxq, q_offsets[i + 1] - q_offsets[i]);
-    Tmp d_q(st), d_off(st), d_t(st), d_sc(st), d_ec(st), d_ep(st), d_a(st), d_b(st), d_len(st), d_st(st);
-    if ((rc = d_q.alloc(qbytes)) || (rc = d_off.alloc((n_queries + 1) * 8)) || (rc = d_t.alloc(templ_len)) ||
-        (rc = d_sc.alloc(n_queries * 8)) || (rc = d_ec.alloc(n_queries * 4)) || (rc = d_ep.alloc(n_queries * 8)) ||
-        (rc = d_a.alloc(n_queries * out_stride)) || (rc = d_b.alloc(n_queries * out_stride)) ||
-        (rc = d_len.alloc(n_queries * 4)) || (rc = d_st.alloc(n_queries * 4)))
+    HostCall c;
+    const Ragged<uint8_t> q = c.ragged(queries, q_offsets, n_queries);
+    const uint8_t *d_t = c.upload(templ, templ_len);
+    int64_t *d_sc = c.alloc<int64_t>(n_queries), *d_ep = c.alloc<int64_t>(n_queries);
+    int32_t *d_ec = c.alloc<int32_t>(n_queries);
+    uint8_t *d_a = c.alloc<uint8_t>(n_queries * out_stride), *d_b = c.alloc<uint8_t>(n_queries * out_stride);
+    uint32_t *d_len = c.alloc<uint32_t>(n_queries, true);
+    int32_t *d_st = c.alloc<int32_t>(n_queries, true);
+    if ((rc = c.error()) || (rc = launch_sw_align(q.base, q.off, n_queries, q.max_len, d_t, templ_len, query_is_a, lut_a, lut_b, table, n_a, n_b,
+                                                  gap, d_sc, d_ec, d_ep, d_a, d_b, out_stride, d_len, d_st, c.st, global)))
         return rc;
-    if (qbytes) PG_CUDA(cudaMemcpyAsync(d_q.p, queries + q0, qbytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_off.p, q_offsets, (n_queries + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (templ_len) PG_CUDA(cudaMemcpyAsync(d_t.p, templ, templ_len, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemsetAsync(d_len.p, 0, n_queries * 4, st));
-    PG_CUDA(cudaMemsetAsync(d_st.p, 0, n_queries * 4, st));
-    rc = launch_sw_align(d_q.as<uint8_t>() - q0, d_off.as<uint64_t>(), n_queries, maxq, d_t.as<uint8_t>(), templ_len, query_is_a,
-                         lut_a, lut_b, table, n_a, n_b, gap, d_sc.as<int64_t>(), d_ec.as<int32_t>(), d_ep.as<int64_t>(),
-                         d_a.as<uint8_t>(), d_b.as<uint8_t>(), out_stride, d_len.as<uint32_t>(), d_st.as<int32_t>(), st, global);
-    if (rc != PG_OK) return rc;
-    PG_CUDA(cudaMemcpyAsync(score, d_sc.p, n_queries * 8, cudaMemcpyDeviceToHost, st));
-    if (err_code) PG_CUDA(cudaMemcpyAsync(err_code, d_ec.p, n_queries * 4, cudaMemcpyDeviceToHost, st));
-    if (err_pos) PG_CUDA(cudaMemcpyAsync(err_pos, d_ep.p, n_queries * 8, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(align_a, d_a.p, n_queries * out_stride, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(align_b, d_b.p, n_queries * out_stride, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(align_len, d_len.p, n_queries * 4, cudaMemcpyDeviceToHost, st));
-    if (status) PG_CUDA(cudaMemcpyAsync(status, d_st.p, n_queries * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    return PG_OK;
+    c.download(score, d_sc, n_queries);
+    c.download(err_code, d_ec, n_queries);
+    c.download(err_pos, d_ep, n_queries);
+    c.download(align_a, d_a, n_queries * out_stride);
+    c.download(align_b, d_b, n_queries * out_stride);
+    c.download(align_len, d_len, n_queries);
+    c.download(status, d_st, n_queries);
+    return c.finish();
 }
 
 int pg_sw_align_batch(const uint8_t *queries, const uint64_t *q_offsets, uint64_t n_queries,
@@ -1426,36 +1493,19 @@ int pg_tm_batch(const uint8_t *bases, const uint64_t *offsets, uint64_t n, doubl
     if (rc != PG_OK) return rc;
     if (n == 0) return PG_OK;
     if (!offsets) { set_error("null offsets"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t b0 = offsets[0], nbytes = offsets[n] - b0;
-    Tmp d_b(st), d_off(st), d_tm(st), d_dh(st), d_ds(st), d_st(st);
-    if ((rc = d_b.alloc(nbytes)) || (rc = d_off.alloc((n + 1) * 8)) || (rc = d_tm.alloc(n * 8)) ||
-        (rc = d_dh.alloc(n * 8)) || (rc = d_ds.alloc(n * 8)) || (rc = d_st.alloc(n * 4)))
-        return rc;
-    if (nbytes) PG_CUDA(cudaMemcpyAsync(d_b.p, bases + b0, nbytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_off.p, offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemsetAsync(d_tm.p, 0, n * 8, st));
-    PG_CUDA(cudaMemsetAsync(d_dh.p, 0, n * 8, st));
-    PG_CUDA(cudaMemsetAsync(d_ds.p, 0, n * 8, st));
-    rc = launch_tm(d_b.as<uint8_t>() - b0, d_off.as<uint64_t>(), n, cp, na, mg, d_tm.as<double>(), d_dh.as<double>(),
-                   d_ds.as<double>(), d_st.as<int32_t>(), st);
-    if (rc != PG_OK) return rc;
+    HostCall c;
+    const Ragged<uint8_t> b = c.ragged(bases, offsets, n);
+    double *d_tm = c.alloc<double>(n, true), *d_dh = c.alloc<double>(n, true), *d_ds = c.alloc<double>(n, true);
+    int32_t *d_st = c.alloc<int32_t>(n);
+    if ((rc = c.error()) || (rc = launch_tm(b.base, b.off, n, cp, na, mg, d_tm, d_dh, d_ds, d_st, c.st))) return rc;
     std::vector<int32_t> hst(n);
-    if (tm) PG_CUDA(cudaMemcpyAsync(tm, d_tm.p, n * 8, cudaMemcpyDeviceToHost, st));
-    if (dh) PG_CUDA(cudaMemcpyAsync(dh, d_dh.p, n * 8, cudaMemcpyDeviceToHost, st));
-    if (ds) PG_CUDA(cudaMemcpyAsync(ds, d_ds.p, n * 8, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(hst.data(), d_st.p, n * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    int worst = PG_OK;
-    for (uint64_t i = 0; i < n; ++i) {
-        if (status) status[i] = hst[i];
-        if (hst[i] == PG_ITEM_PANIC) worst = PG_ERR_PANIC;
-        else if (hst[i] == PG_ITEM_UNSUPPORTED && worst == PG_OK) worst = PG_ERR_UNSUPPORTED;
-    }
-    if (worst == PG_ERR_PANIC) set_error("at least one primer is empty: primers.SantaLucia panics (index out of range)");
-    if (worst == PG_ERR_UNSUPPORTED) set_error("at least one primer holds a byte >= 0x80 (unsupported: strings.ToUpper would re-encode it)");
-    return worst;
+    c.download(tm, d_tm, n);
+    c.download(dh, d_dh, n);
+    c.download(ds, d_ds, n);
+    c.download(hst.data(), d_st, n);
+    if ((rc = c.finish())) return rc;
+    return fold_item_status(hst, status, "at least one primer is empty: primers.SantaLucia panics (index out of range)",
+                            "at least one primer holds a byte >= 0x80 (unsupported: strings.ToUpper would re-encode it)");
 }
 
 int pg_design_primers_batch(const uint8_t *bases, const uint64_t *offsets, uint64_t n,
@@ -1464,32 +1514,18 @@ int pg_design_primers_batch(const uint8_t *bases, const uint64_t *offsets, uint6
     if (rc != PG_OK) return rc;
     if (n == 0) return PG_OK;
     if (!offsets || !fwd_len || !rev_len) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t b0 = offsets[0], nbytes = offsets[n] - b0;
-    Tmp d_b(st), d_off(st), d_f(st), d_r(st), d_st(st);
-    if ((rc = d_b.alloc(nbytes)) || (rc = d_off.alloc((n + 1) * 8)) || (rc = d_f.alloc(n * 4)) ||
-        (rc = d_r.alloc(n * 4)) || (rc = d_st.alloc(n * 4)))
-        return rc;
-    if (nbytes) PG_CUDA(cudaMemcpyAsync(d_b.p, bases + b0, nbytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_off.p, offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    rc = launch_design_primers(d_b.as<uint8_t>() - b0, d_off.as<uint64_t>(), n, target_tm, d_f.as<uint32_t>(),
-                               d_r.as<uint32_t>(), d_st.as<int32_t>(), st);
-    if (rc != PG_OK) return rc;
+    HostCall c;
+    const Ragged<uint8_t> b = c.ragged(bases, offsets, n);
+    uint32_t *d_f = c.alloc<uint32_t>(n), *d_r = c.alloc<uint32_t>(n);
+    int32_t *d_st = c.alloc<int32_t>(n);
+    if ((rc = c.error()) || (rc = launch_design_primers(b.base, b.off, n, target_tm, d_f, d_r, d_st, c.st))) return rc;
     std::vector<int32_t> hst(n);
-    PG_CUDA(cudaMemcpyAsync(fwd_len, d_f.p, n * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(rev_len, d_r.p, n * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(hst.data(), d_st.p, n * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    int worst = PG_OK;
-    for (uint64_t i = 0; i < n; ++i) {
-        if (status) status[i] = hst[i];
-        if (hst[i] == PG_ITEM_PANIC) worst = PG_ERR_PANIC;
-        else if (hst[i] == PG_ITEM_UNSUPPORTED && worst == PG_OK) worst = PG_ERR_UNSUPPORTED;
-    }
-    if (worst == PG_ERR_PANIC) set_error("at least one sequence is exhausted before the target Tm: pcr.DesignPrimers panics (slice bounds out of range)");
-    if (worst == PG_ERR_UNSUPPORTED) set_error("at least one sequence holds a byte >= 0x80 (unsupported)");
-    return worst;
+    c.download(fwd_len, d_f, n);
+    c.download(rev_len, d_r, n);
+    c.download(hst.data(), d_st, n);
+    if ((rc = c.finish())) return rc;
+    return fold_item_status(hst, status, "at least one sequence is exhausted before the target Tm: pcr.DesignPrimers panics (slice bounds out of range)",
+                            "at least one sequence holds a byte >= 0x80 (unsupported)");
 }
 
 int pg_pcr_minimal_primer_batch(const uint8_t *bases, const uint64_t *offsets, uint64_t n, double target_tm,
@@ -1498,28 +1534,17 @@ int pg_pcr_minimal_primer_batch(const uint8_t *bases, const uint64_t *offsets, u
     if (rc != PG_OK) return rc;
     if (n == 0) return PG_OK;
     if (!offsets || !min_len) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t b0 = offsets[0], nbytes = offsets[n] - b0;
-    Tmp d_b(st), d_off(st), d_m(st), d_st(st);
-    if ((rc = d_b.alloc(nbytes)) || (rc = d_off.alloc((n + 1) * 8)) || (rc = d_m.alloc(n * 4)) || (rc = d_st.alloc(n * 4))) return rc;
-    if (nbytes) PG_CUDA(cudaMemcpyAsync(d_b.p, bases + b0, nbytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_off.p, offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    rc = launch_minimal_primer(d_b.as<uint8_t>() - b0, d_off.as<uint64_t>(), n, target_tm, d_m.as<uint32_t>(), d_st.as<int32_t>(), st);
-    if (rc != PG_OK) return rc;
+    HostCall c;
+    const Ragged<uint8_t> b = c.ragged(bases, offsets, n);
+    uint32_t *d_m = c.alloc<uint32_t>(n);
+    int32_t *d_st = c.alloc<int32_t>(n);
+    if ((rc = c.error()) || (rc = launch_minimal_primer(b.base, b.off, n, target_tm, d_m, d_st, c.st))) return rc;
     std::vector<int32_t> hst(n);
-    PG_CUDA(cudaMemcpyAsync(min_len, d_m.p, n * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(hst.data(), d_st.p, n * 4, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    int worst = PG_OK;
-    for (uint64_t i = 0; i < n; ++i) {
-        if (status) status[i] = hst[i];
-        if (hst[i] == PG_ITEM_PANIC) worst = PG_ERR_PANIC;
-        else if (hst[i] == PG_ITEM_UNSUPPORTED && worst == PG_OK) worst = PG_ERR_UNSUPPORTED;
-    }
-    if (worst == PG_ERR_PANIC) set_error("at least one primer is shorter than 7 nt: pcr.SimulateSimple panics (slice bounds out of range)");
-    if (worst == PG_ERR_UNSUPPORTED) set_error("at least one primer holds a byte >= 0x80 (unsupported)");
-    return worst;
+    c.download(min_len, d_m, n);
+    c.download(hst.data(), d_st, n);
+    if ((rc = c.finish())) return rc;
+    return fold_item_status(hst, status, "at least one primer is shorter than 7 nt: pcr.SimulateSimple panics (slice bounds out of range)",
+                            "at least one primer holds a byte >= 0x80 (unsupported)");
 }
 
 int pg_find_sites_batch(const uint8_t *seqs, const uint64_t *seq_offsets, uint64_t n_seq, const uint8_t *patterns,
@@ -1531,39 +1556,22 @@ int pg_find_sites_batch(const uint8_t *seqs, const uint64_t *seq_offsets, uint64
     *n_hits = 0;
     if (n_seq == 0 || n_pat == 0) return PG_OK;
     if (!seq_offsets || !pat_offsets || (hits_cap && (!hit_seq || !hit_pos || !hit_pat))) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t s0 = seq_offsets[0], sbytes = seq_offsets[n_seq] - s0, p0 = pat_offsets[0], pbytes = pat_offsets[n_pat] - p0;
+    HostCall c;
+    const Ragged<uint8_t> sq = c.ragged(seqs, seq_offsets, n_seq);
+    uint64_t max_pat_len;
+    if ((rc = c.error()) || (rc = check_ragged(pat_offsets, n_pat, &max_pat_len))) return rc;
+    const uint64_t sbytes = seq_offsets[n_seq] - seq_offsets[0], p0 = pat_offsets[0], pbytes = pat_offsets[n_pat] - p0;
     std::vector<uint64_t> poff(n_pat + 1);
     for (uint32_t q = 0; q <= n_pat; ++q) poff[q] = pat_offsets[q] - p0;  // the kernel stages patterns from offset 0
-    Tmp d_s(st), d_soff(st), d_p(st), d_poff(st), d_hs(st), d_hp(st), d_hq(st), d_n(st);
-    if ((rc = d_s.alloc(sbytes)) || (rc = d_soff.alloc((n_seq + 1) * 8)) || (rc = d_p.alloc(pbytes)) || (rc = d_poff.alloc((n_pat + 1) * 8)) ||
-        (rc = d_hs.alloc(hits_cap * 4)) || (rc = d_hp.alloc(hits_cap * 8)) || (rc = d_hq.alloc(hits_cap * 4)) || (rc = d_n.alloc(8)))
+    const uint8_t *d_p = c.upload(patterns + p0, pbytes);
+    const uint64_t *d_poff = c.upload(poff.data(), n_pat + 1);
+    uint32_t *d_hs = c.alloc<uint32_t>(hits_cap), *d_hq = c.alloc<uint32_t>(hits_cap);
+    uint64_t *d_hp = c.alloc<uint64_t>(hits_cap);
+    unsigned long long *d_n = c.alloc<unsigned long long>(1, true);
+    if ((rc = c.error()) || (rc = launch_find_sites(sq.base, sq.off, n_seq, sbytes, d_p, d_poff, n_pat, pbytes, flags, d_hs, d_hp, d_hq, hits_cap,
+                                                    d_n, c.st)))
         return rc;
-    if (sbytes) PG_CUDA(cudaMemcpyAsync(d_s.p, seqs + s0, sbytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_soff.p, seq_offsets, (n_seq + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (pbytes) PG_CUDA(cudaMemcpyAsync(d_p.p, patterns + p0, pbytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_poff.p, poff.data(), (n_pat + 1) * 8, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemsetAsync(d_n.p, 0, 8, st));
-    rc = launch_find_sites(d_s.as<uint8_t>() - s0, d_soff.as<uint64_t>(), n_seq, sbytes, d_p.as<uint8_t>(), d_poff.as<uint64_t>(), n_pat, pbytes,
-                           flags, d_hs.as<uint32_t>(), d_hp.as<uint64_t>(), d_hq.as<uint32_t>(), hits_cap, d_n.as<unsigned long long>(), st);
-    if (rc != PG_OK) return rc;
-    unsigned long long found = 0;
-    PG_CUDA(cudaMemcpyAsync(&found, d_n.p, 8, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    *n_hits = found;
-    const uint64_t kept = std::min<uint64_t>(found, hits_cap);
-    if (kept) {
-        PG_CUDA(cudaMemcpyAsync(hit_seq, d_hs.p, kept * 4, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaMemcpyAsync(hit_pos, d_hp.p, kept * 8, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaMemcpyAsync(hit_pat, d_hq.p, kept * 4, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaStreamSynchronize(st));
-    }
-    if (found > hits_cap) {
-        set_error("hits_cap %llu < %llu occurrences", (unsigned long long)hits_cap, found);
-        return PG_ERR_ARG;
-    }
-    return PG_OK;
+    return finish_capped(c, d_n, hits_cap, n_hits, {{hit_seq, d_hs, 4}, {hit_pos, d_hp, 8}, {hit_pat, d_hq, 4}}, "hits_cap", "occurrences");
 }
 
 static int fastq_ingest_dev_impl(const uint8_t *d_text, uint64_t nbytes, uint8_t *d_bases, uint64_t bases_cap,
@@ -1582,21 +1590,17 @@ static int fastq_ingest_host_impl(const uint8_t *text, uint64_t nbytes, uint8_t 
     int rc = ensure_device();
     if (rc != PG_OK) return rc;
     if (!n_records || !total_bases || !err_code || !err_line || !offsets) { set_error("null buffer"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    Tmp d_text(st), d_bases(st), d_off(st), d_spans(st);
-    if ((rc = d_text.alloc(nbytes + 16)) || (rc = d_bases.alloc(bases_cap + 16)) || (rc = d_off.alloc((records_cap + 1) * 8)))
+    HostCall c;
+    const uint8_t *d_text = c.upload(text, nbytes, 16);
+    uint8_t *d_bases = c.alloc<uint8_t>(bases_cap + 16);
+    uint64_t *d_off = c.alloc<uint64_t>(records_cap + 1), *d_spans = spans ? c.alloc<uint64_t>((records_cap + 1) * 4) : nullptr;
+    if ((rc = c.error()) || (rc = launch_fastq_ingest(d_text, nbytes, d_bases, bases_cap, d_off, records_cap, n_records, total_bases, err_code,
+                                                      err_line, c.st, d_spans)))
         return rc;
-    if (spans && (rc = d_spans.alloc((records_cap + 1) * 32))) return rc;
-    if (nbytes) PG_CUDA(cudaMemcpyAsync(d_text.p, text, nbytes, cudaMemcpyHostToDevice, st));
-    rc = launch_fastq_ingest(d_text.as<uint8_t>(), nbytes, d_bases.as<uint8_t>(), bases_cap, d_off.as<uint64_t>(), records_cap,
-                             n_records, total_bases, err_code, err_line, st, spans ? d_spans.as<uint64_t>() : nullptr);
-    if (rc != PG_OK) return rc;
-    if (*total_bases) PG_CUDA(cudaMemcpyAsync(bases, d_bases.p, *total_bases, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(offsets, d_off.p, (*n_records + 1) * 8, cudaMemcpyDeviceToHost, st));
-    if (spans && *n_records) PG_CUDA(cudaMemcpyAsync(spans, d_spans.p, *n_records * 32, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    return PG_OK;
+    c.download(bases, d_bases, *total_bases);
+    c.download(offsets, d_off, *n_records + 1);
+    c.download(spans, d_spans, *n_records * 4);
+    return c.finish();
 }
 
 int pg_fastq_ingest_dev(const uint8_t *d_text, uint64_t nbytes, uint8_t *d_bases, uint64_t bases_cap,
@@ -1643,25 +1647,18 @@ int pg_fasta_ingest(const uint8_t *text, uint64_t nbytes, uint32_t max_line_size
     if (!n_records || !total_bases || !total_name_bytes || !err_code || !err_line || !offsets) { set_error("null buffer"); return PG_ERR_ARG; }
     const bool want_names = names != nullptr || name_offsets != nullptr;
     if (want_names && (!names || !name_offsets)) { set_error("names and name_offsets must be given together"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    Tmp d_text(st), d_bases(st), d_off(st), d_names(st), d_noff(st);
-    if ((rc = d_text.alloc(nbytes + 16)) || (rc = d_bases.alloc(bases_cap + 16)) || (rc = d_off.alloc((records_cap + 1) * 8)))
+    HostCall c;
+    const uint8_t *d_text = c.upload(text, nbytes, 16);
+    uint8_t *d_bases = c.alloc<uint8_t>(bases_cap + 16), *d_names = want_names ? c.alloc<uint8_t>(names_cap + 16) : nullptr;
+    uint64_t *d_off = c.alloc<uint64_t>(records_cap + 1), *d_noff = want_names ? c.alloc<uint64_t>(records_cap + 1) : nullptr;
+    if ((rc = c.error()) || (rc = launch_fasta_ingest(d_text, nbytes, max_line_size, flags, d_bases, bases_cap, d_off, d_names, names_cap, d_noff,
+                                                      records_cap, n_records, total_bases, total_name_bytes, err_code, err_line, c.st)))
         return rc;
-    if (want_names && ((rc = d_names.alloc(names_cap + 16)) || (rc = d_noff.alloc((records_cap + 1) * 8)))) return rc;
-    if (nbytes) PG_CUDA(cudaMemcpyAsync(d_text.p, text, nbytes, cudaMemcpyHostToDevice, st));
-    rc = launch_fasta_ingest(d_text.as<uint8_t>(), nbytes, max_line_size, flags, d_bases.as<uint8_t>(), bases_cap, d_off.as<uint64_t>(),
-                             want_names ? d_names.as<uint8_t>() : nullptr, names_cap, want_names ? d_noff.as<uint64_t>() : nullptr,
-                             records_cap, n_records, total_bases, total_name_bytes, err_code, err_line, st);
-    if (rc != PG_OK) return rc;
-    if (*total_bases) PG_CUDA(cudaMemcpyAsync(bases, d_bases.p, *total_bases, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaMemcpyAsync(offsets, d_off.p, (*n_records + 1) * 8, cudaMemcpyDeviceToHost, st));
-    if (want_names) {
-        if (*total_name_bytes) PG_CUDA(cudaMemcpyAsync(names, d_names.p, *total_name_bytes, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaMemcpyAsync(name_offsets, d_noff.p, (*n_records + 1) * 8, cudaMemcpyDeviceToHost, st));
-    }
-    PG_CUDA(cudaStreamSynchronize(st));
-    return PG_OK;
+    c.download(bases, d_bases, *total_bases);
+    c.download(offsets, d_off, *n_records + 1);
+    c.download(names, d_names, *total_name_bytes);
+    c.download(name_offsets, d_noff, *n_records + 1);
+    return c.finish();
 }
 
 // ---------------------------------------------------------------------------------
@@ -1674,13 +1671,6 @@ static int seqhash_check(int32_t seq_type, uint32_t flags) {
         set_error("unknown seqhash flag bits 0x%x", flags);
         return PG_ERR_ARG;
     }
-    return PG_OK;
-}
-
-static int check_offsets(const uint64_t *offsets, uint64_t n) {
-    if (!offsets) { set_error("null offsets"); return PG_ERR_ARG; }
-    for (uint64_t i = 0; i < n; ++i)
-        if (offsets[i + 1] < offsets[i]) { set_error("offsets decrease at %llu", (unsigned long long)i); return PG_ERR_ARG; }
     return PG_OK;
 }
 
@@ -1704,7 +1694,9 @@ int pg_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, i
     int rc = ensure_device();
     if (rc != PG_OK || (rc = seqhash_check(seq_type, flags)) != PG_OK) return rc;
     if (n == 0) return PG_OK;
-    if ((rc = check_offsets(offsets, n)) != PG_OK) return rc;
+    if (!offsets) { set_error("null offsets"); return PG_ERR_ARG; }
+    uint64_t max_len;  // the whole batch is checked before the first group is launched
+    if ((rc = check_ragged(offsets, n, &max_len)) != PG_OK) return rc;
     if (!digest) { set_error("null digest"); return PG_ERR_ARG; }
     // Sequences go to the device in groups whose device memory stays within the budget (a single longer
     // sequence is a group of its own): input and canonical copy, one 32-byte chaining value per KiB and
@@ -1715,28 +1707,22 @@ int pg_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, i
         const uint64_t bytes = offsets[e] - offsets[g], cnt = e - g;
         return 2 * bytes + 64 + 32 * (bytes / 1024 + cnt) + 101 * cnt;
     };
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
     for (uint64_t g = 0; g < n;) {
-        uint64_t e = g + 1, max_len = offsets[g + 1] - offsets[g];
-        while (e < n && cost(g, e + 1) <= budget) {
-            max_len = std::max<uint64_t>(max_len, offsets[e + 1] - offsets[e]);
-            ++e;
-        }
-        const uint64_t cnt = e - g, b0 = offsets[g], bytes = offsets[e] - b0;
-        Tmp d_b(st), d_off(st), d_dig(st), d_err(st), d_pos(st);
-        if ((rc = d_b.alloc(bytes)) || (rc = d_off.alloc((cnt + 1) * 8)) || (rc = d_dig.alloc(cnt * 32)) || (rc = d_err.alloc(cnt * 4)) ||
-            (rc = d_pos.alloc(cnt * 8)))
+        uint64_t e = g + 1;
+        while (e < n && cost(g, e + 1) <= budget) ++e;
+        const uint64_t cnt = e - g;
+        HostCall c;
+        const Ragged<uint8_t> in = c.ragged(seqs, offsets + g, cnt);
+        uint8_t *d_dig = c.alloc<uint8_t>(cnt * 32);
+        int32_t *d_err = c.alloc<int32_t>(cnt);
+        uint64_t *d_pos = c.alloc<uint64_t>(cnt);
+        if ((rc = c.error()) || (rc = launch_seqhash(in.base, in.off, cnt, in.max_len, offsets[e] - offsets[g], seq_type, flags, d_dig, d_err, d_pos,
+                                                     c.st)))
             return rc;
-        if (bytes) PG_CUDA(cudaMemcpyAsync(d_b.p, seqs + b0, bytes, cudaMemcpyHostToDevice, st));
-        PG_CUDA(cudaMemcpyAsync(d_off.p, offsets + g, (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
-        rc = launch_seqhash(d_b.as<uint8_t>() - b0, d_off.as<uint64_t>(), cnt, max_len, bytes, seq_type, flags, d_dig.as<uint8_t>(),
-                            d_err.as<int32_t>(), d_pos.as<uint64_t>(), st);
-        if (rc != PG_OK) return rc;
-        PG_CUDA(cudaMemcpyAsync(digest + 32 * g, d_dig.p, cnt * 32, cudaMemcpyDeviceToHost, st));
-        if (err_code) PG_CUDA(cudaMemcpyAsync(err_code + g, d_err.p, cnt * 4, cudaMemcpyDeviceToHost, st));
-        if (err_pos) PG_CUDA(cudaMemcpyAsync(err_pos + g, d_pos.p, cnt * 8, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaStreamSynchronize(st));
+        c.download(digest + 32 * g, d_dig, cnt * 32);
+        c.download(err_code ? err_code + g : nullptr, d_err, cnt);
+        c.download(err_pos ? err_pos + g : nullptr, d_pos, cnt);
+        if ((rc = c.finish()) != PG_OK) return rc;
         g = e;
     }
     return PG_OK;
@@ -1746,21 +1732,14 @@ int pg_least_rotation_batch(const uint8_t *seqs, const uint64_t *offsets, uint64
     int rc = ensure_device();
     if (rc != PG_OK) return rc;
     if (n == 0) return PG_OK;
-    if ((rc = check_offsets(offsets, n)) != PG_OK) return rc;
+    if (!offsets) { set_error("null offsets"); return PG_ERR_ARG; }
     if (!rotation) { set_error("null rotation"); return PG_ERR_ARG; }
-    std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
-    const uint64_t b0 = offsets[0], bytes = offsets[n] - b0;
-    uint64_t max_len = 0;
-    for (uint64_t i = 0; i < n; ++i) max_len = std::max<uint64_t>(max_len, offsets[i + 1] - offsets[i]);
-    Tmp d_b(st), d_off(st), d_rot(st);
-    if ((rc = d_b.alloc(bytes)) || (rc = d_off.alloc((n + 1) * 8)) || (rc = d_rot.alloc(n * 8))) return rc;
-    if (bytes) PG_CUDA(cudaMemcpyAsync(d_b.p, seqs + b0, bytes, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d_off.p, offsets, (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    if ((rc = launch_least_rotation(d_b.as<uint8_t>() - b0, d_off.as<uint64_t>(), n, max_len, d_rot.as<uint64_t>(), st)) != PG_OK) return rc;
-    PG_CUDA(cudaMemcpyAsync(rotation, d_rot.p, n * 8, cudaMemcpyDeviceToHost, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    return PG_OK;
+    HostCall c;
+    const Ragged<uint8_t> in = c.ragged(seqs, offsets, n);
+    uint64_t *d_rot = c.alloc<uint64_t>(n);
+    if ((rc = c.error()) || (rc = launch_least_rotation(in.base, in.off, n, in.max_len, d_rot, c.st))) return rc;
+    c.download(rotation, d_rot, n);
+    return c.finish();
 }
 
 // ---------------------------------------------------------------------------------
