@@ -30,8 +30,7 @@
  *     (s < 2, or more than 4 Mi row x item slots) when they hold few long sequences;
  *   - a ragged batch of n items passes n + 1 offsets, item i being [offsets[i], offsets[i+1]).
  *     Offsets must not decrease: the host-pointer entry points return PG_ERR_ARG if they do,
- *     without launching anything (pg_mash_sketch_batch and its _multi form check each chunk
- *     as they stage it, so earlier chunks may have run);
+ *     without launching anything;
  *   - there is NO CPU fallback: without a usable sm_90 device every compute entry
  *     point fails with PG_ERR_NO_DEVICE.
  */
@@ -98,7 +97,8 @@ int pg_stream_sync(void *stream);
  *   n_i <  s : out row i = the n_i hashes in positional order   (mash.go:81-84)
  *   n_i >= s : out row i = ascending bottom-s multiset          (mash.go:87-102)
  * count[i] = min(n_i, s) informative words; row i starts at out + i*row_stride.
- * row_stride must be >= the largest count of the batch (>= s with PG_SKETCH_PAD_ZERO); words
+ * row_stride must be >= the largest count of the batch (>= s with PG_SKETCH_PAD_ZERO; the host
+ * entry points check this for the whole batch before launching anything); words
  * [count[i], row_stride) of a row are written as zeros -- the zero tail a fresh Mash holds,
  * as far as the row reaches.  With PG_SKETCH_PAD_ZERO every row is a full Go array of s words.
  * status[i] (may be NULL) reports per-read PG_ITEM_PANIC for s in {0,1} inputs on

@@ -27,18 +27,19 @@ static thread_local char t_err[512] = "";
 static thread_local const char *t_last_kernel = "";
 static std::atomic<uint64_t> g_launches{0};
 
-// grow-only device scratch used by the host-pointer entry points (under the context's mutex)
-struct Scratch {
+// Grow-only buffer of the pipelined host path (under the context's mutex): device memory, or portable
+// pinned host memory for staging pageable caller buffers.
+template <bool Pinned>
+struct GrowBuf {
     void *p = nullptr;
     size_t cap = 0;
     int reserve(size_t bytes) {
         if (bytes <= cap) return PG_OK;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        cudaError_t e = cudaMalloc(&p, bytes);
+        release();
+        cudaError_t e = Pinned ? cudaHostAlloc(&p, bytes, cudaHostAllocPortable) : cudaMalloc(&p, bytes);
         if (e != cudaSuccess) {
-            set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+            p = nullptr;
+            set_error("%s(%zu) failed: %s", Pinned ? "cudaHostAlloc" : "cudaMalloc", bytes, cudaGetErrorString(e));
             cudaGetLastError();
             return PG_ERR_NOMEM;
         }
@@ -46,32 +47,7 @@ struct Scratch {
         return PG_OK;
     }
     void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
-
-// grow-only pinned host staging (pageable caller buffers go through these; under the context's mutex)
-struct PinnedScratch {
-    void *p = nullptr;
-    size_t cap = 0;
-    int reserve(size_t bytes) {
-        if (bytes <= cap) return PG_OK;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        cudaError_t e = cudaHostAlloc(&p, bytes, cudaHostAllocPortable);
-        if (e != cudaSuccess) {
-            set_error("cudaHostAlloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-            cudaGetLastError();
-            return PG_ERR_NOMEM;
-        }
-        cap = bytes;
-        return PG_OK;
-    }
-    void release() {
-        if (p) cudaFreeHost(p);
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
         p = nullptr;
         cap = 0;
     }
@@ -144,13 +120,29 @@ public:
 // the one-process-per-GPU layout (pg_init(device) picks the process default).
 constexpr int MAX_DEVICES = 32;
 constexpr int N_SLOTS = 3;  // stream/buffer slots of the pipelined host path
+
+// One stream/buffer slot of the pipelined host path and the chunk it has in flight.  Slot 0's stream
+// also serves the one-shot host-pointer entry points.
+struct Slot {
+    cudaStream_t stream = nullptr;
+    GrowBuf<false> in, out, aux, st;  // device: input bytes, rows, offsets + counts, statuses
+    GrowBuf<true> pin_in, pin_out;    // pinned staging of pageable caller buffers
+    uint64_t r0 = 0, nr = 0, dstride = 0;  // in flight: rows [r0, r0 + nr), dstride words per device row
+    bool used = false;
+    std::vector<int32_t> status;  // the chunk's statuses, copied back on the stream
+    void release() {
+        in.release(); out.release(); aux.release(); st.release();
+        pin_in.release(); pin_out.release();
+        if (stream) cudaStreamDestroy(stream);
+        stream = nullptr;
+    }
+};
+
 struct DevCtx {
     int device = -1;
     int sms = 0;
     std::atomic<bool> ready{false};
-    cudaStream_t streams[N_SLOTS] = {nullptr, nullptr, nullptr};
-    Scratch in[N_SLOTS], out[N_SLOTS], aux[N_SLOTS], st[N_SLOTS];
-    PinnedScratch pin_in[N_SLOTS], pin_out[N_SLOTS];
+    Slot slots[N_SLOTS];
     CopyPool pool;
     std::mutex mu;   // serialises the host-pointer entry points on this device
     std::mutex fmu;  // guards func_smem
@@ -204,8 +196,8 @@ static int ctx_create_locked(int device) {
         return PG_ERR_NO_DEVICE;
     }
     PG_CUDA(cudaSetDevice(device));
-    for (int i = 0; i < N_SLOTS; ++i)
-        if (!c.streams[i]) PG_CUDA(cudaStreamCreateWithFlags(&c.streams[i], cudaStreamNonBlocking));
+    for (Slot &sl : c.slots)
+        if (!sl.stream) PG_CUDA(cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking));
     {   // Stream-ordered temporaries (cudaMallocAsync) are freed at the end of every call and most calls
         // synchronise: with the default release threshold of 0 the pool would hand its memory back to the
         // driver each time.  Keep up to 12 GiB cached (the 8 GiB pair tiles of the sparse distance path included) so that small calls do not pay a driver allocation.
@@ -272,6 +264,8 @@ static int ensure_device() {
 }
 
 static inline uint64_t kmers_of(uint64_t len, int k) { return len > (uint64_t)k ? len - (uint64_t)k : 0; }
+// informative words of the sketch of a read of `len` bytes
+static inline uint64_t sketch_words(uint64_t len, int k, int s) { return std::min<uint64_t>(kmers_of(len, k), (uint64_t)s); }
 
 }  // namespace pg
 
@@ -326,7 +320,7 @@ class HostCall {
 
 public:
     const cudaStream_t st;
-    HostCall() : lock_(t_ctx->mu), tmp_(t_ctx->streams[0]), st(t_ctx->streams[0]) {}
+    HostCall() : lock_(t_ctx->mu), tmp_(t_ctx->slots[0].stream), st(t_ctx->slots[0].stream) {}
     ~HostCall() {
         if (finished_) return;
         cudaStreamSynchronize(st);
@@ -467,11 +461,7 @@ int pg_shutdown(void) {
         std::lock_guard<std::mutex> lk2(c.mu);
         cudaSetDevice(d);
         cudaDeviceSynchronize();
-        for (int i = 0; i < N_SLOTS; ++i) {
-            c.in[i].release(); c.out[i].release(); c.aux[i].release(); c.st[i].release();
-            c.pin_in[i].release(); c.pin_out[i].release();
-            if (c.streams[i]) { cudaStreamDestroy(c.streams[i]); c.streams[i] = nullptr; }
-        }
+        for (Slot &sl : c.slots) sl.release();
         c.pool.stop();
         {
             std::lock_guard<std::mutex> lk3(c.fmu);
@@ -603,6 +593,15 @@ static int check_dev_flags(uint32_t flags) {
     if (flags & PG_SKETCH_TAIL_KEEP) { set_error("PG_SKETCH_TAIL_KEEP applies to host buffers only"); return PG_ERR_ARG; }
     return PG_OK;
 }
+// the least row stride of a batch whose longest read has max_len bytes: its count, or s with PAD_ZERO
+static uint64_t need_row_stride(uint64_t max_len, int32_t k, int32_t s, uint32_t flags) {
+    return (flags & PG_SKETCH_PAD_ZERO) ? (uint64_t)s : sketch_words(max_len, k, s);
+}
+static int check_row_stride(uint64_t row_stride, uint64_t max_len, int32_t k, int32_t s, uint32_t flags) {
+    const uint64_t need = need_row_stride(max_len, k, s, flags);
+    if (row_stride < need) { set_error("row_stride %llu < %llu", (unsigned long long)row_stride, (unsigned long long)need); return PG_ERR_ARG; }
+    return PG_OK;
+}
 
 int pg_mash_sketch_uniform_dev(const uint8_t *d_bases, uint64_t n_reads, uint32_t read_len,
                                int32_t k, int32_t s, uint32_t flags, uint32_t *d_out,
@@ -612,9 +611,7 @@ int pg_mash_sketch_uniform_dev(const uint8_t *d_bases, uint64_t n_reads, uint32_
     if ((rc = check_ks(k, s)) != PG_OK) return rc;
     if ((rc = check_dev_flags(flags)) != PG_OK) return rc;
     if (n_reads && (!d_bases || !d_out)) { set_error("null buffer"); return PG_ERR_ARG; }
-    const uint64_t cnt = std::min<uint64_t>(kmers_of(read_len, k), (uint64_t)s);
-    const uint64_t need = (flags & PG_SKETCH_PAD_ZERO) ? (uint64_t)s : cnt;
-    if (row_stride < need) { set_error("row_stride %llu < %llu", (unsigned long long)row_stride, (unsigned long long)need); return PG_ERR_ARG; }
+    if ((rc = check_row_stride(row_stride, read_len, k, s, flags)) != PG_OK) return rc;
     return launch_sketch_uniform(d_bases, n_reads, read_len, k, s, flags, d_out, row_stride,
                                  d_status, (cudaStream_t)stream);
 }
@@ -628,9 +625,7 @@ int pg_mash_sketch_batch_dev(const uint8_t *d_bases, const uint64_t *d_offsets, 
     if ((rc = check_ks(k, s)) != PG_OK) return rc;
     if ((rc = check_dev_flags(flags)) != PG_OK) return rc;
     if (n_reads && (!d_offsets || !d_out)) { set_error("null buffer"); return PG_ERR_ARG; }
-    const uint64_t cnt = std::min<uint64_t>(kmers_of(max_read_len, k), (uint64_t)s);
-    const uint64_t need = (flags & PG_SKETCH_PAD_ZERO) ? (uint64_t)s : cnt;
-    if (row_stride < need) { set_error("row_stride %llu < %llu", (unsigned long long)row_stride, (unsigned long long)need); return PG_ERR_ARG; }
+    if ((rc = check_row_stride(row_stride, max_read_len, k, s, flags)) != PG_OK) return rc;
     return launch_sketch_ragged(d_bases, d_offsets, n_reads, max_read_len, k, s, flags, d_out,
                                 row_stride, d_count, d_status, (cudaStream_t)stream);
 }
@@ -666,7 +661,7 @@ static int sketch_scatter_dev(const uint8_t *d_bases, uint64_t n_local, uint32_t
         set_error("bad destination set (%d buffers, own index %d; at most %d)", n_dst, self, PG_MAX_PEERS);
         return PG_ERR_ARG;
     }
-    const uint64_t cnt = std::min<uint64_t>(kmers_of(read_len, k), (uint64_t)s);
+    const uint64_t cnt = sketch_words(read_len, k, s);
     SketchDst dst;
     dst.n = n_dst;
     for (int p = 0; p < n_dst; ++p) {
@@ -693,7 +688,7 @@ int pg_mash_sketch_uniform_scatter_dev(const uint8_t *d_bases, uint64_t n_local,
 }
 
 // Pipelined host path shared by the uniform and ragged entry points: chunks of reads
-// cycle through 3 stream/buffer slots (H2D, kernel, D2H overlap across slots).
+// cycle through the N_SLOTS stream/buffer slots (H2D, kernel, D2H overlap across slots).
 static bool is_pageable(const void *p) {
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return true; }
@@ -708,16 +703,50 @@ static int host_copy_helpers() {
     return std::max(0, std::min(8, cores / 2) - 1);
 }
 
-static int sketch_host(const uint8_t *bases, const uint64_t *offsets, uint32_t ulen, uint64_t n_reads,
-                       int32_t k, int32_t s, uint32_t flags, uint32_t *out, uint64_t row_stride,
-                       uint32_t *count, int32_t *status) {
-    int rc = ensure_device();
-    if (rc != PG_OK) return rc;
-    if ((rc = check_ks(k, s)) != PG_OK) return rc;
-    if (n_reads == 0) return PG_OK;
-    if (!bases || !out) { set_error("null buffer"); return PG_ERR_ARG; }
-    DevCtx *cx = t_ctx;
-    std::lock_guard<std::mutex> lk(cx->mu);
+namespace pg {
+namespace {
+
+// One host sketch call: reads [0, n) of a ragged batch (offsets) or of fixed-length reads (ulen bytes
+// each, offsets == nullptr), the sketch of read i at out + i * row_stride
+struct SketchCall {
+    const uint8_t *bases;
+    const uint64_t *offsets;
+    uint32_t ulen;
+    uint64_t n;
+    int32_t k, s;
+    uint32_t flags;
+    uint32_t *out;
+    uint64_t row_stride;
+    uint32_t *count;
+    int32_t *status;
+};
+
+// Every argument check of a host sketch call, made before anything is launched or written: k and s,
+// the buffers, the offsets of the whole batch and the row stride its longest read needs.
+static int sketch_check(const SketchCall &q) {
+    int rc;
+    if ((rc = check_ks(q.k, q.s)) != PG_OK || q.n == 0) return rc;
+    if (!q.bases || !q.out) { set_error("null buffer"); return PG_ERR_ARG; }
+    uint64_t max_len = q.ulen;
+    if (q.offsets && (rc = check_ragged(q.offsets, q.n, &max_len)) != PG_OK) return rc;
+    return check_row_stride(q.row_stride, max_len, q.k, q.s, q.flags);
+}
+
+// reads [r0, r1) of the batch, bytes [beg, end) of bases
+struct Chunk {
+    uint64_t r0, r1, beg, end, maxlen, minlen;
+    bool uniform;  // all reads of one length below 2^32: the uniform kernel takes the chunk
+};
+
+// One pipelined host sketch call on the current device, over a batch sketch_check accepted; holds the
+// device's lock.  Chunk i goes to slot i % N_SLOTS once the slot's previous chunk is drained.  Unless
+// run() completes, the destructor waits for every slot's stream, so that no copy into or out of the
+// caller's memory is still running when the entry point returns.
+class SketchPipe {
+    static constexpr uint64_t TARGET_OUT_BYTES = 128ull << 20;  // staged output bytes per chunk
+    DevCtx &cx_;
+    std::lock_guard<std::mutex> lock_;
+    SketchCall q_;  // flags without PG_SKETCH_TAIL_KEEP
     // Pinned caller buffers (pg_host_alloc, cudaHostRegister) are DMA'd directly.  Pageable ones (a Go
     // []byte / []uint32) would be bounced by the driver at ~14 GB/s: they go through pinned staging
     // buffers instead, filled / emptied by a few host threads while the other slots' DMA runs; the
@@ -725,188 +754,214 @@ static int sketch_host(const uint8_t *bases, const uint64_t *offsets, uint32_t u
     // written by the host threads, not shipped over PCIe.
     // PG_SKETCH_TAIL_KEEP: only the informative words of a row are written.  Ragged batches then always go through
     // the staging buffers, whose rows are copied out count[i] words at a time.
-    const bool keep_tail = (flags & PG_SKETCH_TAIL_KEEP) != 0;
-    flags &= ~PG_SKETCH_TAIL_KEEP;
-    const bool stage_in = is_pageable(bases), stage_out = is_pageable(out) || (keep_tail && offsets != nullptr);
-    if (stage_in || stage_out) cx->pool.start(host_copy_helpers(), cx->device);
-    const int nthr = cx->pool.threads();
-    const bool want_status = status != nullptr || s <= 1;
-    const uint64_t target_bytes = (stage_in || stage_out) ? (32ull << 20) : (192ull << 20);  // input bytes per chunk
-    const uint64_t target_out_bytes = 128ull << 20;                                          // staged output bytes per chunk
-    bool any_panic = false;
-    uint64_t r0 = 0;
-    int slot = 0;
-    struct Pending { uint64_t r0, nr, dstride; bool used; } pend[N_SLOTS] = {};
-    std::vector<int32_t> st_slot[N_SLOTS];
-    auto par_rows = [&](uint64_t nrows, const std::function<void(uint64_t, uint64_t)> &f) {
-        const int parts = (int)std::min<uint64_t>((uint64_t)nthr, std::max<uint64_t>(1, nrows));
-        cx->pool.run(parts, [&](int i) { f(nrows * (uint64_t)i / parts, nrows * (uint64_t)(i + 1) / parts); });
-    };
-    auto drain = [&](int sl) -> int {
-        if (!pend[sl].used) return PG_OK;
-        PG_CUDA(cudaStreamSynchronize(cx->streams[sl]));
-        const Pending &pd = pend[sl];
-        if (stage_out && pd.dstride) {  // staged rows -> caller rows (+ zero tail up to the caller's stride)
-            const uint32_t *src = (const uint32_t *)cx->pin_out[sl].p;
-            par_rows(pd.nr, [&](uint64_t a, uint64_t b) {
-                if (pd.dstride == row_stride && !(keep_tail && offsets)) {
-                    memcpy(out + (pd.r0 + a) * row_stride, src + a * pd.dstride, (b - a) * pd.dstride * 4);
+    const bool keep_tail_, stage_in_, stage_out_, want_status_;
+    const uint64_t target_bytes_;  // input bytes per chunk
+    bool any_panic_ = false, finished_ = false;
+
+    // f(a, b) over min(threads, nrows) parts of rows [0, nrows), on the copy pool
+    void par_rows(uint64_t nrows, const std::function<void(uint64_t, uint64_t)> &f) {
+        const int parts = (int)std::min<uint64_t>((uint64_t)cx_.pool.threads(), std::max<uint64_t>(1, nrows));
+        cx_.pool.run(parts, [&](int i) { f(nrows * (uint64_t)i / parts, nrows * (uint64_t)(i + 1) / parts); });
+    }
+
+    // the chunk that starts at read r0
+    Chunk next_chunk(uint64_t r0) const {
+        Chunk c{r0, r0, 0, 0, 0, ~0ull, false};
+        if (q_.offsets) {
+            const uint64_t *off = q_.offsets;
+            c.beg = off[r0];
+            while (c.r1 < q_.n && (c.r1 == r0 || off[c.r1 + 1] - c.beg <= target_bytes_)) {
+                const uint64_t len = off[c.r1 + 1] - off[c.r1];
+                c.maxlen = std::max(c.maxlen, len);
+                c.minlen = std::min(c.minlen, len);
+                ++c.r1;
+                if (stage_out_ && (c.r1 - r0) * sketch_words(c.maxlen, q_.k, q_.s) * 4 >= TARGET_OUT_BYTES) break;
+            }
+            c.end = off[c.r1];
+        } else {
+            uint64_t per = std::max<uint64_t>(1, target_bytes_ / std::max<uint32_t>(q_.ulen, 1));
+            const uint64_t row_bytes = sketch_words(q_.ulen, q_.k, q_.s) * 4;
+            if (stage_out_ && row_bytes) per = std::min(per, std::max<uint64_t>(32, TARGET_OUT_BYTES / row_bytes));
+            per = (per + 31) & ~31ull;  // keep chunk starts on K1 tile boundaries
+            c.r1 = std::min(q_.n, r0 + per);
+            c.beg = r0 * (uint64_t)q_.ulen;
+            c.end = c.r1 * (uint64_t)q_.ulen;
+            c.maxlen = c.minlen = q_.ulen;
+        }
+        c.uniform = c.maxlen == c.minlen && c.maxlen <= 0xffffffffull;
+        return c;
+    }
+
+    // *src = the chunk's input bytes as the H2D copy reads them: pageable input is first copied into the
+    // slot's pinned buffer, in 1 MiB granules over the copy pool
+    int stage_in(Slot &sl, const Chunk &c, const uint8_t **src) {
+        const uint8_t *h = q_.bases + c.beg;
+        const uint64_t bytes = c.end - c.beg;
+        *src = h;
+        if (!stage_in_ || !bytes) return PG_OK;
+        const int rc = sl.pin_in.reserve(bytes);
+        if (rc != PG_OK) return rc;
+        uint8_t *pin = (uint8_t *)sl.pin_in.p;
+        par_rows((bytes + (1u << 20) - 1) >> 20, [&](uint64_t a, uint64_t b) {
+            const uint64_t lo = a << 20, hi = std::min<uint64_t>(bytes, b << 20);
+            if (hi > lo) memcpy(pin + lo, h + lo, hi - lo);
+        });
+        *src = pin;
+        return PG_OK;
+    }
+
+    // the chunk's copies in, kernel and copies out on the slot's stream; the slot is drained
+    int enqueue(Slot &sl, const Chunk &c) {
+        const int32_t k = q_.k, s = q_.s;
+        const uint64_t nr = c.r1 - c.r0, in_bytes = c.end - c.beg, cnt_max = sketch_words(c.maxlen, k, s);
+        // staged output: compact device rows, the host threads pad; direct output: the device pads
+        const bool compact = stage_out_ || keep_tail_;
+        const uint32_t dev_flags = compact ? (q_.flags & ~PG_SKETCH_PAD_ZERO) : q_.flags;
+        const uint64_t dev_stride = compact ? cnt_max : need_row_stride(c.maxlen, k, s, q_.flags);
+        const cudaStream_t st = sl.stream;
+        int rc;
+        if ((rc = sl.in.reserve(in_bytes + 64)) != PG_OK) return rc;
+        if ((rc = sl.out.reserve(std::max<uint64_t>(nr * dev_stride * 4, 16))) != PG_OK) return rc;
+        uint8_t *d_in = (uint8_t *)sl.in.p;
+        uint32_t *d_out = (uint32_t *)sl.out.p;
+        int32_t *d_status = nullptr;
+        uint32_t *d_count = nullptr;
+        if (want_status_) {
+            if ((rc = sl.st.reserve(nr * 4)) != PG_OK) return rc;
+            d_status = (int32_t *)sl.st.p;
+            PG_CUDA(cudaMemsetAsync(d_status, 0, nr * 4, st));
+            sl.status.assign(nr, 0);
+        }
+        const uint8_t *h_src;
+        if ((rc = stage_in(sl, c, &h_src)) != PG_OK) return rc;
+        if (in_bytes) PG_CUDA(cudaMemcpyAsync(d_in, h_src, in_bytes, cudaMemcpyHostToDevice, st));
+        if (c.uniform) {
+            rc = launch_sketch_uniform(d_in, nr, (uint32_t)c.maxlen, k, s, dev_flags, d_out, dev_stride, d_status, st);
+        } else {
+            if ((rc = sl.aux.reserve((nr + 1) * 8 + nr * 4)) != PG_OK) return rc;
+            uint64_t *d_off = (uint64_t *)sl.aux.p;
+            d_count = (uint32_t *)(d_off + nr + 1);
+            PG_CUDA(cudaMemcpyAsync(d_off, q_.offsets + c.r0, (nr + 1) * 8, cudaMemcpyHostToDevice, st));
+            // kernels index bases with absolute offsets: shift the base pointer
+            rc = launch_sketch_ragged(d_in - c.beg, d_off, nr, c.maxlen, k, s, dev_flags, d_out, dev_stride, d_count, d_status, st);
+        }
+        if (rc != PG_OK) return rc;
+        uint32_t *out = q_.out + c.r0 * q_.row_stride;
+        if (dev_stride) {
+            if (stage_out_) {
+                if ((rc = sl.pin_out.reserve(nr * dev_stride * 4)) != PG_OK) return rc;
+                PG_CUDA(cudaMemcpyAsync(sl.pin_out.p, d_out, nr * dev_stride * 4, cudaMemcpyDeviceToHost, st));
+            } else if (q_.row_stride == dev_stride) {
+                PG_CUDA(cudaMemcpyAsync(out, d_out, nr * dev_stride * 4, cudaMemcpyDeviceToHost, st));
+            } else {
+                PG_CUDA(cudaMemcpy2DAsync(out, q_.row_stride * 4, d_out, dev_stride * 4, dev_stride * 4, nr, cudaMemcpyDeviceToHost, st));
+            }
+        }
+        if (q_.count) {
+            if (c.uniform) std::fill(q_.count + c.r0, q_.count + c.r1, (uint32_t)cnt_max);
+            else PG_CUDA(cudaMemcpyAsync(q_.count + c.r0, d_count, nr * 4, cudaMemcpyDeviceToHost, st));
+        }
+        if (want_status_) PG_CUDA(cudaMemcpyAsync(sl.status.data(), d_status, nr * 4, cudaMemcpyDeviceToHost, st));
+        sl.r0 = c.r0;
+        sl.nr = nr;
+        sl.dstride = dev_stride;
+        sl.used = true;
+        return PG_OK;
+    }
+
+    // waits for the slot's chunk, then unstages its rows (or zeroes their tails) and folds its statuses
+    int drain(Slot &sl) {
+        if (!sl.used) return PG_OK;
+        PG_CUDA(cudaStreamSynchronize(sl.stream));
+        const uint64_t rs = q_.row_stride, ds = sl.dstride;
+        uint32_t *out = q_.out + sl.r0 * rs;
+        if (stage_out_ && ds) {  // staged rows -> caller rows (+ zero tail up to the caller's stride)
+            const uint32_t *src = (const uint32_t *)sl.pin_out.p;
+            par_rows(sl.nr, [&](uint64_t a, uint64_t b) {
+                if (ds == rs && !(keep_tail_ && q_.offsets)) {
+                    memcpy(out + a * rs, src + a * ds, (b - a) * ds * 4);
                     return;
                 }
                 for (uint64_t i = a; i < b; ++i) {
-                    uint32_t *dst = out + (pd.r0 + i) * row_stride;
-                    if (keep_tail) {  // exactly the informative words of this row
-                        const uint64_t r = pd.r0 + i;
-                        const uint64_t ci = offsets ? std::min<uint64_t>(kmers_of(offsets[r + 1] - offsets[r], k), (uint64_t)s) : pd.dstride;
-                        memcpy(dst, src + i * pd.dstride, ci * 4);
+                    if (keep_tail_) {  // exactly the informative words of this row
+                        const uint64_t r = sl.r0 + i;
+                        const uint64_t ci = q_.offsets ? sketch_words(q_.offsets[r + 1] - q_.offsets[r], q_.k, q_.s) : ds;
+                        memcpy(out + i * rs, src + i * ds, ci * 4);
                         continue;
                     }
-                    memcpy(dst, src + i * pd.dstride, pd.dstride * 4);
-                    memset(dst + pd.dstride, 0, (row_stride - pd.dstride) * 4);
+                    memcpy(out + i * rs, src + i * ds, ds * 4);
+                    memset(out + i * rs + ds, 0, (rs - ds) * 4);
                 }
             });
-        } else if (row_stride > pd.dstride && !keep_tail) {  // direct DMA wrote dstride words per row: zero the rest of each row
-            par_rows(pd.nr, [&](uint64_t a, uint64_t b) {
-                for (uint64_t i = a; i < b; ++i) memset(out + (pd.r0 + i) * row_stride + pd.dstride, 0, (row_stride - pd.dstride) * 4);
+        } else if (rs > ds && !keep_tail_) {  // direct DMA wrote ds words per row: zero the rest of each row
+            par_rows(sl.nr, [&](uint64_t a, uint64_t b) {
+                for (uint64_t i = a; i < b; ++i) memset(out + i * rs + ds, 0, (rs - ds) * 4);
             });
         }
-        if (want_status) {
-            for (uint64_t i = 0; i < pd.nr; ++i) {
-                if (st_slot[sl][i] != PG_ITEM_OK) any_panic = true;
-                if (status) status[pd.r0 + i] = st_slot[sl][i];
+        if (want_status_) {
+            for (uint64_t i = 0; i < sl.nr; ++i) {
+                if (sl.status[i] != PG_ITEM_OK) any_panic_ = true;
+                if (q_.status) q_.status[sl.r0 + i] = sl.status[i];
             }
         }
-        pend[sl].used = false;
+        sl.used = false;
         return PG_OK;
-    };
-    auto body = [&]() -> int {
-        while (r0 < n_reads) {
-            // chunk [r0, r1)
-            uint64_t r1, beg, end, maxlen, minlen;
-            if (offsets) {
-                beg = offsets[r0];
-                r1 = r0;
-                maxlen = 0;
-                minlen = ~0ull;
-                while (r1 < n_reads && (r1 == r0 || offsets[r1 + 1] - beg <= target_bytes)) {
-                    if (offsets[r1 + 1] < offsets[r1]) { set_error("offsets not monotone at %llu", (unsigned long long)r1); return PG_ERR_ARG; }
-                    const uint64_t len = offsets[r1 + 1] - offsets[r1];
-                    maxlen = std::max(maxlen, len);
-                    minlen = std::min(minlen, len);
-                    ++r1;
-                    if (stage_out && (r1 - r0) * std::min<uint64_t>(kmers_of(maxlen, k), (uint64_t)s) * 4 >= target_out_bytes) break;
-                }
-                end = offsets[r1];
-            } else {
-                uint64_t per = std::max<uint64_t>(1, target_bytes / std::max<uint32_t>(ulen, 1));
-                const uint64_t row_bytes = std::min<uint64_t>(kmers_of(ulen, k), (uint64_t)s) * 4;
-                if (stage_out && row_bytes) per = std::min(per, std::max<uint64_t>(32, target_out_bytes / row_bytes));
-                per = (per + 31) & ~31ull;  // keep chunk starts on K1 tile boundaries
-                r1 = std::min(n_reads, r0 + per);
-                beg = r0 * (uint64_t)ulen;
-                end = r1 * (uint64_t)ulen;
-                maxlen = minlen = ulen;
-            }
-            const uint64_t nr = r1 - r0;
-            const bool uniform = maxlen == minlen && maxlen <= 0xffffffffull;
-            const uint64_t cnt_max = std::min<uint64_t>(kmers_of(maxlen, k), (uint64_t)s);
-            const uint64_t need_stride = (flags & PG_SKETCH_PAD_ZERO) ? (uint64_t)s : cnt_max;
-            if (row_stride < need_stride) { set_error("row_stride %llu < %llu", (unsigned long long)row_stride, (unsigned long long)need_stride); return PG_ERR_ARG; }
-            // staged output: compact device rows, the host threads pad; direct output: the device pads
-            const uint32_t dev_flags = (stage_out || keep_tail) ? (flags & ~PG_SKETCH_PAD_ZERO) : flags;
-            const uint64_t dev_stride = (stage_out || keep_tail) ? cnt_max : need_stride;
+    }
 
-            int rc2;
-            if ((rc2 = drain(slot)) != PG_OK) return rc2;
-            cudaStream_t stx = cx->streams[slot];
-            const uint64_t in_bytes = end - beg;
-            if ((rc2 = cx->in[slot].reserve(in_bytes + 64)) != PG_OK) return rc2;
-            if ((rc2 = cx->out[slot].reserve(std::max<uint64_t>(nr * dev_stride * 4, 16))) != PG_OK) return rc2;
-            uint8_t *d_in = (uint8_t *)cx->in[slot].p;
-            uint32_t *d_out = (uint32_t *)cx->out[slot].p;
-            int32_t *d_status = nullptr;
-            uint32_t *d_count = nullptr;
-            uint64_t *d_off = nullptr;
-            if (want_status) {
-                if ((rc2 = cx->st[slot].reserve(nr * 4)) != PG_OK) return rc2;
-                d_status = (int32_t *)cx->st[slot].p;
-                PG_CUDA(cudaMemsetAsync(d_status, 0, nr * 4, stx));
-                st_slot[slot].assign(nr, 0);
-            }
-            const uint8_t *h_src = bases + beg;
-            if (stage_in && in_bytes) {
-                if ((rc2 = cx->pin_in[slot].reserve(in_bytes)) != PG_OK) return rc2;
-                uint8_t *pin = (uint8_t *)cx->pin_in[slot].p;
-                par_rows((in_bytes + (1u << 20) - 1) >> 20, [&](uint64_t a, uint64_t b) {  // 1 MiB granules
-                    const uint64_t lo = a << 20, hi = std::min<uint64_t>(in_bytes, b << 20);
-                    if (hi > lo) memcpy(pin + lo, h_src + lo, hi - lo);
-                });
-                h_src = pin;
-            }
-            if (in_bytes) PG_CUDA(cudaMemcpyAsync(d_in, h_src, in_bytes, cudaMemcpyHostToDevice, stx));
-            if (uniform) {
-                rc2 = launch_sketch_uniform(d_in, nr, (uint32_t)maxlen, k, s, dev_flags, d_out, dev_stride, d_status, stx);
-            } else {
-                if ((rc2 = cx->aux[slot].reserve((nr + 1) * 8 + nr * 4)) != PG_OK) return rc2;
-                d_off = (uint64_t *)cx->aux[slot].p;
-                d_count = (uint32_t *)(d_off + nr + 1);
-                PG_CUDA(cudaMemcpyAsync(d_off, offsets + r0, (nr + 1) * 8, cudaMemcpyHostToDevice, stx));
-                // kernels index bases with absolute offsets: shift the base pointer
-                rc2 = launch_sketch_ragged(d_in - beg, d_off, nr, maxlen, k, s, dev_flags, d_out, dev_stride, d_count, d_status, stx);
-            }
-            if (rc2 != PG_OK) return rc2;
-            if (dev_stride) {
-                if (stage_out) {
-                    if ((rc2 = cx->pin_out[slot].reserve(nr * dev_stride * 4)) != PG_OK) return rc2;
-                    PG_CUDA(cudaMemcpyAsync(cx->pin_out[slot].p, d_out, nr * dev_stride * 4, cudaMemcpyDeviceToHost, stx));
-                } else if (row_stride == dev_stride) {
-                    PG_CUDA(cudaMemcpyAsync(out + r0 * row_stride, d_out, nr * dev_stride * 4, cudaMemcpyDeviceToHost, stx));
-                } else {
-                    PG_CUDA(cudaMemcpy2DAsync(out + r0 * row_stride, row_stride * 4, d_out, dev_stride * 4, dev_stride * 4, nr, cudaMemcpyDeviceToHost, stx));
-                }
-            }
-            if (count) {
-                if (uniform) {
-                    for (uint64_t i = 0; i < nr; ++i) count[r0 + i] = (uint32_t)cnt_max;
-                } else {
-                    PG_CUDA(cudaMemcpyAsync(count + r0, d_count, nr * 4, cudaMemcpyDeviceToHost, stx));
-                }
-            }
-            if (want_status) PG_CUDA(cudaMemcpyAsync(st_slot[slot].data(), d_status, nr * 4, cudaMemcpyDeviceToHost, stx));
-            pend[slot] = {r0, nr, dev_stride, true};
-            slot = (slot + 1) % N_SLOTS;
-            r0 = r1;
+public:
+    explicit SketchPipe(const SketchCall &q)
+        : cx_(*t_ctx), lock_(cx_.mu), q_(q), keep_tail_((q.flags & PG_SKETCH_TAIL_KEEP) != 0), stage_in_(is_pageable(q.bases)),
+          stage_out_(is_pageable(q.out) || (keep_tail_ && q.offsets)), want_status_(q.status != nullptr || q.s <= 1),
+          target_bytes_((stage_in_ || stage_out_) ? (32ull << 20) : (192ull << 20)) {
+        q_.flags &= ~PG_SKETCH_TAIL_KEEP;
+        if (stage_in_ || stage_out_) cx_.pool.start(host_copy_helpers(), cx_.device);
+    }
+    ~SketchPipe() {
+        if (finished_) return;
+        for (Slot &sl : cx_.slots) {
+            cudaStreamSynchronize(sl.stream);
+            sl.used = false;
         }
-        for (int i = 0; i < N_SLOTS; ++i) {
-            const int rc2 = drain((slot + i) % N_SLOTS);  // oldest first
-            if (rc2 != PG_OK) return rc2;
+        cudaGetLastError();
+    }
+    int run() {
+        int rc, slot = 0;
+        for (uint64_t r0 = 0; r0 < q_.n; slot = (slot + 1) % N_SLOTS) {
+            const Chunk c = next_chunk(r0);
+            if ((rc = drain(cx_.slots[slot])) != PG_OK || (rc = enqueue(cx_.slots[slot], c)) != PG_OK) return rc;
+            r0 = c.r1;
+        }
+        for (int i = 0; i < N_SLOTS; ++i)
+            if ((rc = drain(cx_.slots[(slot + i) % N_SLOTS])) != PG_OK) return rc;  // oldest first
+        finished_ = true;
+        if (any_panic_) {
+            set_error("at least one read hits an input on which mash.Sketch panics (sketchSize <= 1)");
+            return PG_ERR_PANIC;
         }
         return PG_OK;
-    };
-    rc = body();
-    if (rc != PG_OK) {  // nothing may still be copying into the caller's (or this frame's) buffers when we return
-        for (int i = 0; i < N_SLOTS; ++i) cudaStreamSynchronize(cx->streams[i]);
-        cudaGetLastError();
-        return rc;
     }
-    if (any_panic) {
-        set_error("at least one read hits an input on which mash.Sketch panics (sketchSize <= 1)");
-        return PG_ERR_PANIC;
-    }
-    return PG_OK;
+};
+
+static int sketch_host(const SketchCall &q) {
+    int rc = ensure_device();
+    if (rc != PG_OK || (rc = sketch_check(q)) != PG_OK || q.n == 0) return rc;
+    return SketchPipe(q).run();
 }
+
+}  // namespace
+}  // namespace pg
 
 int pg_mash_sketch_batch(const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads, int32_t k,
                          int32_t s, uint32_t flags, uint32_t *out, uint64_t row_stride,
                          uint32_t *count, int32_t *status) {
     if (n_reads && !offsets) { set_error("null offsets"); return PG_ERR_ARG; }
-    return sketch_host(bases, offsets, 0, n_reads, k, s, flags, out, row_stride, count, status);
+    return sketch_host({bases, offsets, 0, n_reads, k, s, flags, out, row_stride, count, status});
 }
 
 int pg_mash_sketch_uniform(const uint8_t *bases, uint64_t n_reads, uint32_t read_len, int32_t k,
                            int32_t s, uint32_t flags, uint32_t *out, uint64_t row_stride,
                            int32_t *status) {
-    return sketch_host(bases, nullptr, read_len, n_reads, k, s, flags, out, row_stride, nullptr, status);
+    return sketch_host({bases, nullptr, read_len, n_reads, k, s, flags, out, row_stride, nullptr, status});
 }
 
 // ---------------------------------------------------------------------------------
@@ -973,32 +1028,28 @@ public:
     }
 };
 
-}  // namespace
-}  // namespace pg
-
-static int sketch_multi(const uint8_t *bases, const uint64_t *offsets, uint32_t ulen, uint64_t n_reads, int32_t k, int32_t s,
-                        uint32_t flags, uint32_t *out, uint64_t row_stride, uint32_t *count, int32_t *status,
-                        const int32_t *devices, int32_t n_devices) {
-    int rc;
-    if ((rc = check_ks(k, s)) != PG_OK) return rc;
-    std::vector<int> dev;
-    if ((rc = resolve_devices(devices, n_devices, &dev)) != PG_OK) return rc;
-    if (n_reads == 0) return PG_OK;
-    if (!bases || !out) { set_error("null buffer"); return PG_ERR_ARG; }
-    const int P = (int)dev.size();
-    // contiguous shards; boundaries on K1 tile boundaries (32 reads).  Ragged batches balance bytes.
-    std::vector<uint64_t> cut(P + 1, n_reads);
+// P contiguous shards of n reads, cut on K1 tile boundaries (32 reads): shard r is [cut[r], cut[r + 1])
+std::vector<uint64_t> uniform_cuts(uint64_t n, int P) {
+    std::vector<uint64_t> cut(P + 1, n);
     cut[0] = 0;
-    if (!offsets) {
-        uint64_t per = (n_reads + P - 1) / P;
-        per = (per + 31) & ~31ull;
-        for (int r = 1; r < P; ++r) cut[r] = std::min(n_reads, (uint64_t)r * per);
-    } else {
-        const uint64_t b0 = offsets[0], total = offsets[n_reads] - b0;
+    const uint64_t per = ((n + P - 1) / P + 31) & ~31ull;
+    for (int r = 1; r < P; ++r) cut[r] = std::min(n, (uint64_t)r * per);
+    return cut;
+}
+
+// The batch is checked once, here, before it is cut; each shard then runs the pipeline on its device's thread.
+int sketch_multi(const SketchCall &q, const int32_t *devices, int32_t n_devices) {
+    std::vector<int> dev;
+    int rc;
+    if ((rc = resolve_devices(devices, n_devices, &dev)) != PG_OK || (rc = sketch_check(q)) != PG_OK || q.n == 0) return rc;
+    const int P = (int)dev.size();
+    std::vector<uint64_t> cut = uniform_cuts(q.n, P);
+    if (q.offsets) {  // ragged batches balance bytes instead
+        const uint64_t b0 = q.offsets[0], total = q.offsets[q.n] - b0;
         for (int r = 1; r < P; ++r) {
             const uint64_t want = b0 + total / P * r;
-            uint64_t i = std::lower_bound(offsets, offsets + n_reads + 1, want) - offsets;
-            i = std::min<uint64_t>((i + 31) & ~31ull, n_reads);
+            uint64_t i = std::lower_bound(q.offsets, q.offsets + q.n + 1, want) - q.offsets;
+            i = std::min<uint64_t>((i + 31) & ~31ull, q.n);
             cut[r] = std::max(i, cut[r - 1]);
         }
     }
@@ -1007,13 +1058,18 @@ static int sketch_multi(const uint8_t *bases, const uint64_t *offsets, uint32_t 
     for (int r = 0; r < P; ++r) {
         const uint64_t lo = cut[r], hi = cut[r + 1];
         if (hi <= lo) continue;
-        th.emplace_back([=, &res] {
+        SketchCall shard = q;
+        shard.n = hi - lo;
+        if (q.offsets) shard.offsets += lo;
+        else shard.bases += lo * (uint64_t)q.ulen;
+        shard.out += lo * q.row_stride;
+        if (q.count) shard.count += lo;
+        if (q.status) shard.status += lo;
+        th.emplace_back([&res, &dev, r, shard] {
             t_bound_device = dev[r];  // this worker's entry points run on its device
             pg_numa_bind_thread(dev[r], nullptr);  // best effort: staging copies from the GPU's NUMA node
-            const int wrc = offsets ? sketch_host(bases, offsets + lo, 0, hi - lo, k, s, flags, out + lo * row_stride, row_stride,
-                                                  count ? count + lo : nullptr, status ? status + lo : nullptr)
-                                    : sketch_host(bases + lo * (uint64_t)ulen, nullptr, ulen, hi - lo, k, s, flags, out + lo * row_stride,
-                                                  row_stride, nullptr, status ? status + lo : nullptr);
+            int wrc = ensure_device();
+            if (wrc == PG_OK) wrc = SketchPipe(shard).run();
             res[r].rc = wrc;
             if (wrc != PG_OK) res[r].msg = t_err;
         });
@@ -1022,17 +1078,20 @@ static int sketch_multi(const uint8_t *bases, const uint64_t *offsets, uint32_t 
     return fold_results(res);
 }
 
+}  // namespace
+}  // namespace pg
+
 extern "C" int pg_mash_sketch_uniform_multi(const uint8_t *bases, uint64_t n_reads, uint32_t read_len, int32_t k, int32_t s,
                                             uint32_t flags, uint32_t *out, uint64_t row_stride, int32_t *status,
                                             const int32_t *devices, int32_t n_devices) {
-    return sketch_multi(bases, nullptr, read_len, n_reads, k, s, flags, out, row_stride, nullptr, status, devices, n_devices);
+    return sketch_multi({bases, nullptr, read_len, n_reads, k, s, flags, out, row_stride, nullptr, status}, devices, n_devices);
 }
 
 extern "C" int pg_mash_sketch_batch_multi(const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads, int32_t k, int32_t s,
                                           uint32_t flags, uint32_t *out, uint64_t row_stride, uint32_t *count, int32_t *status,
                                           const int32_t *devices, int32_t n_devices) {
     if (n_reads && !offsets) { set_error("null offsets"); return PG_ERR_ARG; }
-    return sketch_multi(bases, offsets, 0, n_reads, k, s, flags, out, row_stride, count, status, devices, n_devices);
+    return sketch_multi({bases, offsets, 0, n_reads, k, s, flags, out, row_stride, count, status}, devices, n_devices);
 }
 
 // Sketch + all-pairs distance over several devices of this process (cfg3 / cfg4 pipeline, SURVEY 8e):
@@ -1053,16 +1112,10 @@ extern "C" int pg_mash_sketch_distance_multi(const uint8_t *bases, uint64_t n_re
     if (!bases) { set_error("null buffer"); return PG_ERR_ARG; }
     if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
     const uint64_t n = n_reads, L = read_len;
-    const uint64_t cnt = std::min<uint64_t>(kmers_of(L, k), (uint64_t)s);
-    int P = (int)std::min<uint64_t>(dev.size(), (n + 31) / 32);
+    const uint64_t cnt = sketch_words(L, k, s);
+    const int P = (int)std::min<uint64_t>(dev.size(), (n + 31) / 32);
     dev.resize(P);
-    std::vector<uint64_t> cut(P + 1, n);
-    cut[0] = 0;
-    {
-        uint64_t per = (n + P - 1) / P;
-        per = (per + 31) & ~31ull;
-        for (int r = 1; r < P; ++r) cut[r] = std::min(n, (uint64_t)r * per);
-    }
+    const std::vector<uint64_t> cut = uniform_cuts(n, P);
     // peer access available between every pair?
     bool fused = true;
     for (int a = 0; a < P && fused; ++a)
@@ -1089,7 +1142,7 @@ extern "C" int pg_mash_sketch_distance_multi(const uint8_t *bases, uint64_t n_re
         step([&]() -> int {
             int c = ensure_device();
             if (c != PG_OK) return c;
-            st = t_ctx->streams[0];
+            st = t_ctx->slots[0].stream;
             if (fused)
                 for (int p = 0; p < P; ++p)
                     if (p != r) {
@@ -1296,7 +1349,7 @@ int pg_mash_index_create(const uint32_t *sketches, uint64_t n, int32_t s, pg_mas
     if (rc != PG_OK) return rc;
     if (n && s > 0 && !sketches) { set_error("null buffer"); return PG_ERR_ARG; }
     std::lock_guard<std::mutex> lk(t_ctx->mu);
-    return index_create(sketches, false, n, s, t_ctx->streams[0], out);
+    return index_create(sketches, false, n, s, t_ctx->slots[0].stream, out);
 }
 
 int pg_mash_index_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, void *stream, pg_mash_index **out) {
@@ -1346,7 +1399,7 @@ int pg_mash_index_free(pg_mash_index *ix) {
     int rc = use_device(ix->device);
     if (rc != PG_OK) return rc;
     std::lock_guard<std::mutex> lk(t_ctx->mu);
-    cudaStream_t st = t_ctx->streams[0];
+    cudaStream_t st = t_ctx->slots[0].stream;
     distance_plan_destroy(ix->plan, st);
     if (ix->d_sk) cudaFreeAsync(ix->d_sk, st);
     delete ix;

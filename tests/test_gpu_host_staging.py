@@ -83,7 +83,15 @@ def _least_rotation(L):
     return L.pg_least_rotation_batch(_p(SEQS), _p(BAD), N, o(np.uint64))
 
 
+def _sketch(L, multi):
+    o, k, s = Out(), 3, 4
+    args = (_p(SEQS), _p(BAD), N, k, s, 0, o(np.uint32, N * s), s, o(np.uint32), o(np.int32))
+    return L.pg_mash_sketch_batch_multi(*args, None, 0) if multi else L.pg_mash_sketch_batch(*args)
+
+
 CALLS = {
+    "pg_mash_sketch_batch": lambda L: _sketch(L, False),
+    "pg_mash_sketch_batch_multi": lambda L: _sketch(L, True),
     "pg_mash_similarity_pairs": _similarity_pairs,
     "pg_sw_score_batch": lambda L: _score(L, "pg_sw_score_batch"),
     "pg_nw_score_batch": lambda L: _score(L, "pg_nw_score_batch"),
