@@ -312,6 +312,84 @@ func alignBatch(global bool, queries []byte, qOffsets []uint64, template string,
 	}
 }
 
+// ScorePairs wraps pg_sw_score_pairs (global = false) / pg_nw_score_pairs (global = true): pair p scores
+// A[pairA[p]] against B[pairB[p]] of the two flattened sets.
+func ScorePairs(global bool, aBases []byte, aOff []uint64, bBases []byte, bOff []uint64, pairA, pairB []uint32,
+	lutA, lutB *[256]int16, table []int64, nA, nB int, gap int64) (score []int64, errCode []int32, errPos []int64, err error) {
+	n := len(pairA)
+	score, errCode, errPos = make([]int64, n+1), make([]int32, n+1), make([]int64, n+1)
+	pa, pb := append(pairA[:n:n], 0), append(pairB[:n:n], 0) // copies with room for &pa[0] when n == 0
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread() // pg_last_error() is thread-local: read it on the calling thread
+	var rc C.int
+	if global {
+		rc = C.pg_nw_score_pairs((*C.uint8_t)(unsafe.Pointer(&aBases[0])), (*C.uint64_t)(unsafe.Pointer(&aOff[0])), C.uint64_t(len(aOff)-1),
+			(*C.uint8_t)(unsafe.Pointer(&bBases[0])), (*C.uint64_t)(unsafe.Pointer(&bOff[0])), C.uint64_t(len(bOff)-1),
+			(*C.uint32_t)(unsafe.Pointer(&pa[0])), (*C.uint32_t)(unsafe.Pointer(&pb[0])), C.uint64_t(n),
+			(*C.int16_t)(unsafe.Pointer(&lutA[0])), (*C.int16_t)(unsafe.Pointer(&lutB[0])), (*C.int64_t)(unsafe.Pointer(&table[0])),
+			C.int32_t(nA), C.int32_t(nB), C.int64_t(gap),
+			(*C.int64_t)(unsafe.Pointer(&score[0])), (*C.int32_t)(unsafe.Pointer(&errCode[0])), (*C.int64_t)(unsafe.Pointer(&errPos[0])))
+	} else {
+		rc = C.pg_sw_score_pairs((*C.uint8_t)(unsafe.Pointer(&aBases[0])), (*C.uint64_t)(unsafe.Pointer(&aOff[0])), C.uint64_t(len(aOff)-1),
+			(*C.uint8_t)(unsafe.Pointer(&bBases[0])), (*C.uint64_t)(unsafe.Pointer(&bOff[0])), C.uint64_t(len(bOff)-1),
+			(*C.uint32_t)(unsafe.Pointer(&pa[0])), (*C.uint32_t)(unsafe.Pointer(&pb[0])), C.uint64_t(n),
+			(*C.int16_t)(unsafe.Pointer(&lutA[0])), (*C.int16_t)(unsafe.Pointer(&lutB[0])), (*C.int64_t)(unsafe.Pointer(&table[0])),
+			C.int32_t(nA), C.int32_t(nB), C.int64_t(gap),
+			(*C.int64_t)(unsafe.Pointer(&score[0])), (*C.int32_t)(unsafe.Pointer(&errCode[0])), (*C.int64_t)(unsafe.Pointer(&errPos[0])))
+	}
+	return score[:n], errCode[:n], errPos[:n], check(rc)
+}
+
+// AlignPairs wraps pg_sw_align_pairs / pg_nw_align_pairs: ScorePairs plus the two aligned strings of
+// every pair.  Rows are len(a) + len(b) bytes wide, which no alignment exceeds.
+func AlignPairs(global bool, aBases []byte, aOff []uint64, bBases []byte, bOff []uint64, pairA, pairB []uint32,
+	lutA, lutB *[256]int16, table []int64, nA, nB int, gap int64) (score []int64, errCode []int32, errPos []int64, alignA, alignB []string, err error) {
+	n := len(pairA)
+	stride := 1
+	for p := 0; p < n; p++ {
+		if int(pairA[p]) < len(aOff)-1 && int(pairB[p]) < len(bOff)-1 {
+			if w := int(aOff[pairA[p]+1]-aOff[pairA[p]]) + int(bOff[pairB[p]+1]-bOff[pairB[p]]); w > stride {
+				stride = w
+			}
+		}
+	}
+	score, errCode, errPos = make([]int64, n+1), make([]int32, n+1), make([]int64, n+1)
+	oa, ob := make([]byte, n*stride+1), make([]byte, n*stride+1)
+	ln, st := make([]uint32, n+1), make([]int32, n+1)
+	pa, pb := append(pairA[:n:n], 0), append(pairB[:n:n], 0)
+	runtime.LockOSThread()
+	defer runtime.UnlockOSThread() // pg_last_error() is thread-local: read it on the calling thread
+	var rc C.int
+	if global {
+		rc = C.pg_nw_align_pairs((*C.uint8_t)(unsafe.Pointer(&aBases[0])), (*C.uint64_t)(unsafe.Pointer(&aOff[0])), C.uint64_t(len(aOff)-1),
+			(*C.uint8_t)(unsafe.Pointer(&bBases[0])), (*C.uint64_t)(unsafe.Pointer(&bOff[0])), C.uint64_t(len(bOff)-1),
+			(*C.uint32_t)(unsafe.Pointer(&pa[0])), (*C.uint32_t)(unsafe.Pointer(&pb[0])), C.uint64_t(n),
+			(*C.int16_t)(unsafe.Pointer(&lutA[0])), (*C.int16_t)(unsafe.Pointer(&lutB[0])), (*C.int64_t)(unsafe.Pointer(&table[0])),
+			C.int32_t(nA), C.int32_t(nB), C.int64_t(gap),
+			(*C.int64_t)(unsafe.Pointer(&score[0])), (*C.int32_t)(unsafe.Pointer(&errCode[0])), (*C.int64_t)(unsafe.Pointer(&errPos[0])),
+			(*C.uint8_t)(unsafe.Pointer(&oa[0])), (*C.uint8_t)(unsafe.Pointer(&ob[0])), C.uint64_t(stride),
+			(*C.uint32_t)(unsafe.Pointer(&ln[0])), (*C.int32_t)(unsafe.Pointer(&st[0])))
+	} else {
+		rc = C.pg_sw_align_pairs((*C.uint8_t)(unsafe.Pointer(&aBases[0])), (*C.uint64_t)(unsafe.Pointer(&aOff[0])), C.uint64_t(len(aOff)-1),
+			(*C.uint8_t)(unsafe.Pointer(&bBases[0])), (*C.uint64_t)(unsafe.Pointer(&bOff[0])), C.uint64_t(len(bOff)-1),
+			(*C.uint32_t)(unsafe.Pointer(&pa[0])), (*C.uint32_t)(unsafe.Pointer(&pb[0])), C.uint64_t(n),
+			(*C.int16_t)(unsafe.Pointer(&lutA[0])), (*C.int16_t)(unsafe.Pointer(&lutB[0])), (*C.int64_t)(unsafe.Pointer(&table[0])),
+			C.int32_t(nA), C.int32_t(nB), C.int64_t(gap),
+			(*C.int64_t)(unsafe.Pointer(&score[0])), (*C.int32_t)(unsafe.Pointer(&errCode[0])), (*C.int64_t)(unsafe.Pointer(&errPos[0])),
+			(*C.uint8_t)(unsafe.Pointer(&oa[0])), (*C.uint8_t)(unsafe.Pointer(&ob[0])), C.uint64_t(stride),
+			(*C.uint32_t)(unsafe.Pointer(&ln[0])), (*C.int32_t)(unsafe.Pointer(&st[0])))
+	}
+	if e := check(rc); e != nil {
+		return nil, nil, nil, nil, nil, e
+	}
+	alignA, alignB = make([]string, n), make([]string, n)
+	for p := 0; p < n; p++ {
+		alignA[p] = string(oa[p*stride : p*stride+int(ln[p])])
+		alignB[p] = string(ob[p*stride : p*stride+int(ln[p])])
+	}
+	return score[:n], errCode[:n], errPos[:n], alignA, alignB, nil
+}
+
 // TmBatch wraps pg_tm_batch.
 func TmBatch(bases []byte, offsets []uint64, cp, na, mg float64) (tm, dH, dS []float64, status []int32, err error) {
 	n := len(offsets) - 1

@@ -1,7 +1,8 @@
 // Package align: drop-in for github.com/bebop/poly/search/align.SmithWaterman
 // (search/align/align.go:171-232: score, aligned strings, error) and for the score of
 // NeedlemanWunsch (align.go:100-134,166), backed by libpolyb200.so.  NOT COMPILED HERE.
-// Both need the shorter string to have <= 64 symbols; longer pairs keep the pure-Go path.
+// SmithWaterman / NeedlemanWunsch need the shorter string to have <= 64 symbols; longer pairs keep the
+// pure-Go path.  The *Pair* functions take lists of pairs of strings of any length.
 package align
 
 import (
@@ -144,6 +145,91 @@ func NeedlemanWunschScore(stringA, stringB string, scoring Scoring) (int, error)
 		return 0, e
 	}
 	return int(score[0]), nil
+}
+
+// pairIndices checks every pair against the two sets -- out of range panics, as indexing as[i] / bs[j]
+// in the caller's loop would -- and converts the indices for the C ABI.
+func pairIndices(as, bs []string, pairA, pairB []int) ([]uint32, []uint32) {
+	if len(pairA) != len(pairB) {
+		panic(fmt.Sprintf("align: %d pairA indices but %d pairB indices", len(pairA), len(pairB)))
+	}
+	pa, pb := make([]uint32, len(pairA)), make([]uint32, len(pairB))
+	for p := range pairA {
+		_, _ = as[pairA[p]], bs[pairB[p]]
+		pa[p], pb[p] = uint32(pairA[p]), uint32(pairB[p])
+	}
+	return pa, pb
+}
+
+// pairError rebuilds the reference's *alphabet.Error of a pair from its error code and position.
+func pairError(scoring Scoring, ec int32, ep int64, a, b string) error {
+	var e error
+	if ec == 1 {
+		_, e = scoring.SubstitutionMatrix.FirstAlphabet.Encode(string(a[ep]))
+	} else if ec == 2 {
+		_, e = scoring.SubstitutionMatrix.SecondAlphabet.Encode(string(b[ep]))
+	}
+	return e
+}
+
+func pairScores(global bool, as, bs []string, pairA, pairB []int, scoring Scoring) ([]int, []error) {
+	pa, pb := pairIndices(as, bs, pairA, pairB)
+	lutA, lutB, table, nA, nB := flatten(scoring.SubstitutionMatrix)
+	aBases, aOff := polyb200.Flatten(as)
+	bBases, bOff := polyb200.Flatten(bs)
+	score, ec, ep, err := polyb200.ScorePairs(global, aBases, aOff, bBases, bOff, pa, pb, &lutA, &lutB, table, nA, nB, int64(scoring.GapPenalty))
+	if err != nil {
+		panic(err)
+	}
+	scores, errs := make([]int, len(pa)), make([]error, len(pa))
+	for p := range pa {
+		scores[p] = int(score[p])
+		errs[p] = pairError(scoring, ec[p], ep[p], as[pairA[p]], bs[pairB[p]])
+	}
+	return scores, errs
+}
+
+// SmithWatermanPairScores scores SmithWaterman(as[pairA[p]], bs[pairB[p]], scoring) for every pair p in one
+// GPU pass, with each pair's error as SmithWaterman returns it.  A string may have any length.
+func SmithWatermanPairScores(as, bs []string, pairA, pairB []int, scoring Scoring) ([]int, []error) {
+	return pairScores(false, as, bs, pairA, pairB, scoring)
+}
+
+// NeedlemanWunschPairScores scores NeedlemanWunsch(as[pairA[p]], bs[pairB[p]], scoring) for every pair p.
+func NeedlemanWunschPairScores(as, bs []string, pairA, pairB []int, scoring Scoring) ([]int, []error) {
+	return pairScores(true, as, bs, pairA, pairB, scoring)
+}
+
+func pairAligns(global bool, as, bs []string, pairA, pairB []int, scoring Scoring) ([]int, []string, []string, []error) {
+	pa, pb := pairIndices(as, bs, pairA, pairB)
+	lutA, lutB, table, nA, nB := flatten(scoring.SubstitutionMatrix)
+	aBases, aOff := polyb200.Flatten(as)
+	bBases, bOff := polyb200.Flatten(bs)
+	score, ec, ep, alignA, alignB, err := polyb200.AlignPairs(global, aBases, aOff, bBases, bOff, pa, pb, &lutA, &lutB, table, nA, nB,
+		int64(scoring.GapPenalty))
+	if err != nil {
+		panic(err)
+	}
+	scores, errs := make([]int, len(pa)), make([]error, len(pa))
+	for p := range pa {
+		if errs[p] = pairError(scoring, ec[p], ep[p], as[pairA[p]], bs[pairB[p]]); errs[p] != nil {
+			alignA[p], alignB[p] = "", "" // (0, "", "", err), as the reference returns
+			continue
+		}
+		scores[p] = int(score[p])
+	}
+	return scores, alignA, alignB, errs
+}
+
+// SmithWatermanPairAligns is SmithWaterman(as[pairA[p]], bs[pairB[p]], scoring) for every pair p: scores,
+// aligned strings and errors, in one call.
+func SmithWatermanPairAligns(as, bs []string, pairA, pairB []int, scoring Scoring) ([]int, []string, []string, []error) {
+	return pairAligns(false, as, bs, pairA, pairB, scoring)
+}
+
+// NeedlemanWunschPairAligns is NeedlemanWunsch(as[pairA[p]], bs[pairB[p]], scoring) for every pair p.
+func NeedlemanWunschPairAligns(as, bs []string, pairA, pairB []int, scoring Scoring) ([]int, []string, []string, []error) {
+	return pairAligns(true, as, bs, pairA, pairB, scoring)
 }
 
 var _ = alphabet.DNA

@@ -520,6 +520,95 @@ inline int64_t NeedlemanWunschScore(const std::string &a, const std::string &b, 
     return score;
 }
 
+// Pair lists: pair p aligns stringA = as[pairA[p]] against stringB = bs[pairB[p]] in one call.  Indices must
+// lie in [0, as.size()) / [0, bs.size()) (Error PG_ERR_ARG otherwise); errors[p] is "" or the
+// reference's alphabet error of that pair.
+inline std::vector<int64_t> table_of(const Scoring &sc) {
+    const int na = (int)sc.Matrix.scores.size(), nb = (int)sc.Matrix.scores[0].size();
+    std::vector<int64_t> table((size_t)na * nb);
+    for (int i = 0; i < na; ++i)
+        for (int j = 0; j < nb; ++j) table[(size_t)i * nb + j] = sc.Matrix.scores[i][j];
+    return table;
+}
+inline std::string pair_error(int32_t ecode, int64_t epos, const std::string &a, const std::string &b) {
+    if (!ecode) return "";
+    return "Symbol " + go_string_of_byte(ecode == 1 ? (uint8_t)a[epos] : (uint8_t)b[epos]) + " not in alphabet";
+}
+inline std::vector<int64_t> pair_scores(bool global, const std::vector<std::string> &as, const std::vector<std::string> &bs,
+                                        const std::vector<uint32_t> &pairA, const std::vector<uint32_t> &pairB, const Scoring &sc,
+                                        std::vector<std::string> *errors) {
+    if (pairA.size() != pairB.size()) throw std::invalid_argument("pairA and pairB differ in length");
+    Flat fa(as), fb(bs);
+    auto lut_a = sc.Matrix.FirstAlphabet.byte_lut(), lut_b = sc.Matrix.SecondAlphabet.byte_lut();
+    auto table = table_of(sc);
+    const size_t n = pairA.size();
+    std::vector<int64_t> score(n), epos(n);
+    std::vector<int32_t> ecode(n);
+    check((global ? pg_nw_score_pairs : pg_sw_score_pairs)(fa.bases.data(), fa.offsets.data(), as.size(), fb.bases.data(), fb.offsets.data(),
+                                                           bs.size(), pairA.data(), pairB.data(), n, lut_a.data(), lut_b.data(), table.data(),
+                                                           (int)sc.Matrix.scores.size(), (int)sc.Matrix.scores[0].size(), sc.GapPenalty,
+                                                           score.data(), ecode.data(), epos.data()));
+    if (errors) {
+        errors->assign(n, "");
+        for (size_t k = 0; k < n; ++k) (*errors)[k] = pair_error(ecode[k], epos[k], as[pairA[k]], bs[pairB[k]]);
+    }
+    return score;
+}
+inline std::vector<int64_t> SmithWatermanPairScores(const std::vector<std::string> &as, const std::vector<std::string> &bs,
+                                                    const std::vector<uint32_t> &pairA, const std::vector<uint32_t> &pairB,
+                                                    const Scoring &sc, std::vector<std::string> *errors = nullptr) {
+    return pair_scores(false, as, bs, pairA, pairB, sc, errors);
+}
+inline std::vector<int64_t> NeedlemanWunschPairScores(const std::vector<std::string> &as, const std::vector<std::string> &bs,
+                                                      const std::vector<uint32_t> &pairA, const std::vector<uint32_t> &pairB,
+                                                      const Scoring &sc, std::vector<std::string> *errors = nullptr) {
+    return pair_scores(true, as, bs, pairA, pairB, sc, errors);
+}
+// aligned strings per pair ({0, "", ""} where errors[p] is set)
+inline std::vector<Alignment> pair_aligns(bool global, const std::vector<std::string> &as, const std::vector<std::string> &bs,
+                                          const std::vector<uint32_t> &pairA, const std::vector<uint32_t> &pairB, const Scoring &sc,
+                                          std::vector<std::string> *errors) {
+    if (pairA.size() != pairB.size()) throw std::invalid_argument("pairA and pairB differ in length");
+    Flat fa(as), fb(bs);
+    auto lut_a = sc.Matrix.FirstAlphabet.byte_lut(), lut_b = sc.Matrix.SecondAlphabet.byte_lut();
+    auto table = table_of(sc);
+    const size_t n = pairA.size();
+    uint64_t stride = 1;  // an alignment has at most len(a) + len(b) columns
+    for (size_t k = 0; k < n; ++k)
+        if (pairA[k] < as.size() && pairB[k] < bs.size()) stride = std::max<uint64_t>(stride, as[pairA[k]].size() + bs[pairB[k]].size());
+    std::vector<int64_t> score(n), epos(n);
+    std::vector<int32_t> ecode(n), status(n);
+    std::vector<uint32_t> len(n);
+    std::vector<uint8_t> oa(std::max<size_t>(n, 1) * stride), ob(std::max<size_t>(n, 1) * stride);
+    check((global ? pg_nw_align_pairs : pg_sw_align_pairs)(fa.bases.data(), fa.offsets.data(), as.size(), fb.bases.data(), fb.offsets.data(),
+                                                           bs.size(), pairA.data(), pairB.data(), n, lut_a.data(), lut_b.data(), table.data(),
+                                                           (int)sc.Matrix.scores.size(), (int)sc.Matrix.scores[0].size(), sc.GapPenalty,
+                                                           score.data(), ecode.data(), epos.data(), oa.data(), ob.data(), stride, len.data(),
+                                                           status.data()));
+    std::vector<Alignment> out(n);
+    if (errors) errors->assign(n, "");
+    for (size_t k = 0; k < n; ++k) {
+        if (ecode[k]) {
+            if (errors) (*errors)[k] = pair_error(ecode[k], epos[k], as[pairA[k]], bs[pairB[k]]);
+            out[k] = Alignment{0, "", ""};
+            continue;
+        }
+        const char *pa = reinterpret_cast<const char *>(oa.data() + k * stride), *pb = reinterpret_cast<const char *>(ob.data() + k * stride);
+        out[k] = Alignment{score[k], std::string(pa, len[k]), std::string(pb, len[k])};
+    }
+    return out;
+}
+inline std::vector<Alignment> SmithWatermanPairAligns(const std::vector<std::string> &as, const std::vector<std::string> &bs,
+                                                      const std::vector<uint32_t> &pairA, const std::vector<uint32_t> &pairB,
+                                                      const Scoring &sc, std::vector<std::string> *errors = nullptr) {
+    return pair_aligns(false, as, bs, pairA, pairB, sc, errors);
+}
+inline std::vector<Alignment> NeedlemanWunschPairAligns(const std::vector<std::string> &as, const std::vector<std::string> &bs,
+                                                        const std::vector<uint32_t> &pairA, const std::vector<uint32_t> &pairB,
+                                                        const Scoring &sc, std::vector<std::string> *errors = nullptr) {
+    return pair_aligns(true, as, bs, pairA, pairB, sc, errors);
+}
+
 }  // namespace align
 
 namespace primers {

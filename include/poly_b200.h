@@ -315,6 +315,70 @@ int pg_nw_align_batch(const uint8_t *queries, const uint64_t *q_offsets, uint64_
                       int64_t *err_pos, uint8_t *align_a, uint8_t *align_b, uint64_t out_stride,
                       uint32_t *align_len, int32_t *status);
 
+/* ---- align.SmithWaterman / align.NeedlemanWunsch over a list of pairs ----------------------
+ * Pair p aligns stringA = A[pair_a[p]] (the reference's outer loop, the rows) against
+ * stringB = B[pair_b[p]], where A (seqs_a, offsets_a, n_seqs_a) and B are ragged sets as in the
+ * one-template calls.  A and B may be the same buffers; a pair list never copies a sequence.  Per
+ * pair, score / err_code / err_pos are bit-identical to pg_sw_score_batch (pg_nw_score_batch) on
+ * that (a, b): the first failing cell in row-major order, score 0 on error.  Alphabet limits and
+ * the int32 / int64 score-width rule are those of the one-template calls, with the longest a and
+ * the longest b of the call.
+ * Host entry points: both sets are checked as ragged batches and every pair index against
+ * n_seqs_a / n_seqs_b before anything is launched (PG_ERR_ARG, no output written).  n_pairs == 0
+ * is PG_OK.  Both sets are uploaded once; pairs, outputs and scratch go in groups sized from the
+ * device memory left free by the sets (at most 1 GiB of pairs and outputs per group), and the
+ * long-pair scratch shrinks to what fits; PG_ERR_NOMEM only when the two sets plus one pair's
+ * scratch do not fit.  Score width and scratch follow the longest a and b the pairs reference.
+ * _dev score variants take device sets, pairs and outputs and host max_len_a / max_len_b, LUTs and
+ * table; they only enqueue work on `stream` and never wait for the device.  A pair whose index is
+ * out of range, or whose sequence is longer than max_len_a / max_len_b, gets
+ * err_code = PG_PAIR_OUT_OF_RANGE, score 0 and err_pos -1; nothing out of bounds is read.
+ * pg_sw_align_pairs / pg_nw_align_pairs add the aligned strings exactly as pg_sw_align_batch /
+ * pg_nw_align_batch (align_a / align_b rows of out_stride bytes, align_len, status, with
+ * PG_ITEM_UNSUPPORTED and the needed length when out_stride is too short).  Every pair of a group
+ * keeps a whole (la + 1) x (lb + 1) matrix of 32-bit cells, la / lb the group's longest referenced
+ * a / b: scores must fit 32 bits over la + lb cells, and one pair's matrix is limited to 16 Gi cells
+ * (PG_ERR_UNSUPPORTED otherwise). */
+#define PG_PAIR_OUT_OF_RANGE 3
+int pg_sw_score_pairs(const uint8_t *seqs_a, const uint64_t *offsets_a, uint64_t n_seqs_a,
+                      const uint8_t *seqs_b, const uint64_t *offsets_b, uint64_t n_seqs_b,
+                      const uint32_t *pair_a, const uint32_t *pair_b, uint64_t n_pairs,
+                      const int16_t *lut_a, const int16_t *lut_b, const int64_t *table,
+                      int32_t n_a, int32_t n_b, int64_t gap,
+                      int64_t *score, int32_t *err_code, int64_t *err_pos);
+int pg_nw_score_pairs(const uint8_t *seqs_a, const uint64_t *offsets_a, uint64_t n_seqs_a,
+                      const uint8_t *seqs_b, const uint64_t *offsets_b, uint64_t n_seqs_b,
+                      const uint32_t *pair_a, const uint32_t *pair_b, uint64_t n_pairs,
+                      const int16_t *lut_a, const int16_t *lut_b, const int64_t *table,
+                      int32_t n_a, int32_t n_b, int64_t gap,
+                      int64_t *score, int32_t *err_code, int64_t *err_pos);
+int pg_sw_score_pairs_dev(const uint8_t *d_seqs_a, const uint64_t *d_offsets_a, uint64_t n_seqs_a, uint64_t max_len_a,
+                          const uint8_t *d_seqs_b, const uint64_t *d_offsets_b, uint64_t n_seqs_b, uint64_t max_len_b,
+                          const uint32_t *d_pair_a, const uint32_t *d_pair_b, uint64_t n_pairs,
+                          const int16_t *lut_a_host, const int16_t *lut_b_host, const int64_t *table_host,
+                          int32_t n_a, int32_t n_b, int64_t gap,
+                          int64_t *d_score, int32_t *d_err_code, int64_t *d_err_pos, void *stream);
+int pg_nw_score_pairs_dev(const uint8_t *d_seqs_a, const uint64_t *d_offsets_a, uint64_t n_seqs_a, uint64_t max_len_a,
+                          const uint8_t *d_seqs_b, const uint64_t *d_offsets_b, uint64_t n_seqs_b, uint64_t max_len_b,
+                          const uint32_t *d_pair_a, const uint32_t *d_pair_b, uint64_t n_pairs,
+                          const int16_t *lut_a_host, const int16_t *lut_b_host, const int64_t *table_host,
+                          int32_t n_a, int32_t n_b, int64_t gap,
+                          int64_t *d_score, int32_t *d_err_code, int64_t *d_err_pos, void *stream);
+int pg_sw_align_pairs(const uint8_t *seqs_a, const uint64_t *offsets_a, uint64_t n_seqs_a,
+                      const uint8_t *seqs_b, const uint64_t *offsets_b, uint64_t n_seqs_b,
+                      const uint32_t *pair_a, const uint32_t *pair_b, uint64_t n_pairs,
+                      const int16_t *lut_a, const int16_t *lut_b, const int64_t *table,
+                      int32_t n_a, int32_t n_b, int64_t gap,
+                      int64_t *score, int32_t *err_code, int64_t *err_pos,
+                      uint8_t *align_a, uint8_t *align_b, uint64_t out_stride, uint32_t *align_len, int32_t *status);
+int pg_nw_align_pairs(const uint8_t *seqs_a, const uint64_t *offsets_a, uint64_t n_seqs_a,
+                      const uint8_t *seqs_b, const uint64_t *offsets_b, uint64_t n_seqs_b,
+                      const uint32_t *pair_a, const uint32_t *pair_b, uint64_t n_pairs,
+                      const int16_t *lut_a, const int16_t *lut_b, const int64_t *table,
+                      int32_t n_a, int32_t n_b, int64_t gap,
+                      int64_t *score, int32_t *err_code, int64_t *err_pos,
+                      uint8_t *align_a, uint8_t *align_b, uint64_t out_stride, uint32_t *align_len, int32_t *status);
+
 /* ---- align.NeedlemanWunsch score -- search/align/align.go:100-134 (fill) and :166 --------
  * (a "next" row of SURVEY.md 8f).  Same arguments and error semantics as the Smith-Waterman
  * entry points; score = matrix[len(a)][len(b)] of the global alignment (gap ramps on the first

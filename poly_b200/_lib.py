@@ -77,6 +77,12 @@ _SIGS = {
     "pg_nw_align_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, _u8p, C.c_uint64, C.c_int32, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p, _u8p, _u8p, C.c_uint64, _u32p, _i32p]),
     "pg_nw_score_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, _u8p, C.c_uint64, C.c_int32, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p]),
     "pg_nw_score_batch_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_uint64, _u8p, C.c_uint64, C.c_int32, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p, C.c_void_p]),
+    "pg_sw_score_pairs": (C.c_int, [_u8p, _u64p, C.c_uint64, _u8p, _u64p, C.c_uint64, _u32p, _u32p, C.c_uint64, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p]),
+    "pg_nw_score_pairs": (C.c_int, [_u8p, _u64p, C.c_uint64, _u8p, _u64p, C.c_uint64, _u32p, _u32p, C.c_uint64, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p]),
+    "pg_sw_score_pairs_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_uint64, _u8p, _u64p, C.c_uint64, C.c_uint64, _u32p, _u32p, C.c_uint64, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p, C.c_void_p]),
+    "pg_nw_score_pairs_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_uint64, _u8p, _u64p, C.c_uint64, C.c_uint64, _u32p, _u32p, C.c_uint64, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p, C.c_void_p]),
+    "pg_sw_align_pairs": (C.c_int, [_u8p, _u64p, C.c_uint64, _u8p, _u64p, C.c_uint64, _u32p, _u32p, C.c_uint64, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p, _u8p, _u8p, C.c_uint64, _u32p, _i32p]),
+    "pg_nw_align_pairs": (C.c_int, [_u8p, _u64p, C.c_uint64, _u8p, _u64p, C.c_uint64, _u32p, _u32p, C.c_uint64, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p, _u8p, _u8p, C.c_uint64, _u32p, _i32p]),
     "pg_tm_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_double, C.c_double, C.c_double, _f64p, _f64p, _f64p, _i32p]),
     "pg_tm_batch_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_double, C.c_double, C.c_double, _f64p, _f64p, _f64p, _i32p, C.c_void_p]),
     "pg_design_primers_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_double, _u32p, _u32p, _i32p]),

@@ -13,6 +13,8 @@ from __future__ import annotations
 
 from typing import List, Optional, Sequence, Tuple
 
+import ctypes as C
+
 import numpy as np
 
 from . import _lib
@@ -229,3 +231,125 @@ def NeedlemanWunsch(stringA: BytesLike, stringB: BytesLike, scoring: Scoring):
         return NeedlemanWunschAlign(stringA, stringB, scoring) + (None,)
     except AlphabetError as e:
         return 0, "", "", e
+
+
+# ---- pair lists: pair p aligns stringA = seqs_a[pairs[p, 0]] against stringB = seqs_b[pairs[p, 1]] ----
+
+def _pair_inputs(seqs_a, seqs_b, pairs, scoring: Scoring):
+    """Flattened sets, the two index columns of the (n, 2) pair array, LUTs and table."""
+    m = scoring.SubstitutionMatrix
+    lut_a, lut_b = m.FirstAlphabet.byte_lut(), m.SecondAlphabet.byte_lut()
+    table = np.ascontiguousarray(m.scores, dtype=np.int64)
+    ba, oa = seqs_a if isinstance(seqs_a, tuple) else flatten(seqs_a)
+    bb, ob = seqs_b if isinstance(seqs_b, tuple) else flatten(seqs_b)
+    pairs = np.asarray(pairs)
+    if pairs.size == 0:
+        pairs = pairs.reshape(0, 2)
+    if pairs.ndim != 2 or pairs.shape[1] != 2:
+        raise ValueError(f"pairs must be an (n, 2) array, got shape {pairs.shape}")
+    if pairs.size and (pairs.min() < 0 or pairs.max() > 0xFFFFFFFF):
+        raise ValueError("pair indices must lie in [0, 2^32)")
+    pa = np.ascontiguousarray(pairs[:, 0], dtype=np.uint32)
+    pb = np.ascontiguousarray(pairs[:, 1], dtype=np.uint32)
+    return (np.ascontiguousarray(ba, np.uint8), np.ascontiguousarray(oa, np.uint64), np.ascontiguousarray(bb, np.uint8),
+            np.ascontiguousarray(ob, np.uint64), pa, pb, lut_a, lut_b, table)
+
+
+def pair_scores_arrays(seqs_a, seqs_b, pairs, scoring: Scoring, global_alignment: bool = False):
+    """(score, err_code, err_pos) NumPy arrays for every pair (pg_sw_score_pairs / pg_nw_score_pairs).
+    seqs_a / seqs_b: lists of sequences or (bases, offsets) arrays; pairs: (n, 2) integer array."""
+    ba, oa, bb, ob, pa, pb, lut_a, lut_b, table = _pair_inputs(seqs_a, seqs_b, pairs, scoring)
+    n = len(pa)
+    score, ec, ep = np.zeros(n, np.int64), np.zeros(n, np.int32), np.zeros(n, np.int64)
+    fn = _lib.lib().pg_nw_score_pairs if global_alignment else _lib.lib().pg_sw_score_pairs
+    _lib.check(fn(ba.ctypes.data, oa.ctypes.data, len(oa) - 1, bb.ctypes.data, ob.ctypes.data, len(ob) - 1, pa.ctypes.data, pb.ctypes.data, n,
+                  lut_a.ctypes.data, lut_b.ctypes.data, table.ctypes.data, table.shape[0], table.shape[1], scoring.GapPenalty,
+                  score.ctypes.data, ec.ctypes.data, ep.ctypes.data))
+    return score, ec, ep
+
+
+def _pair_errors(ec, ep, ba, oa, bb, ob, pa, pb) -> List[Optional[AlphabetError]]:
+    errs: List[Optional[AlphabetError]] = []
+    for k in range(len(ec)):
+        if ec[k]:
+            i, j = int(pa[k]), int(pb[k])
+            errs.append(_error_for(int(ec[k]), int(ep[k]), ba[int(oa[i]): int(oa[i + 1])], bb[int(ob[j]): int(ob[j + 1])]))
+        else:
+            errs.append(None)
+    return errs
+
+
+def SmithWatermanPairScores(seqs_a, seqs_b, pairs, scoring: Scoring, global_alignment: bool = False):
+    """Batched align.SmithWaterman(seqs_a[i], seqs_b[j], scoring) score for every (i, j) row of `pairs`:
+    (scores, errors) as SmithWatermanScores returns them."""
+    ba, oa, bb, ob, pa, pb, _, _, _ = _pair_inputs(seqs_a, seqs_b, pairs, scoring)
+    score, ec, ep = pair_scores_arrays((ba, oa), (bb, ob), np.stack([pa, pb], 1), scoring, global_alignment)
+    return [int(x) for x in score], _pair_errors(ec, ep, ba, oa, bb, ob, pa, pb)
+
+
+def NeedlemanWunschPairScores(seqs_a, seqs_b, pairs, scoring: Scoring):
+    """Batched align.NeedlemanWunsch(seqs_a[i], seqs_b[j], scoring) score for every (i, j) row of `pairs`."""
+    return SmithWatermanPairScores(seqs_a, seqs_b, pairs, scoring, global_alignment=True)
+
+
+def SmithWatermanPairAligns(seqs_a, seqs_b, pairs, scoring: Scoring, global_alignment: bool = False):
+    """Full align.SmithWaterman (NeedlemanWunsch with global_alignment=True) for every (i, j) row of
+    `pairs`: [(score, alignA, alignB, err)], as SmithWatermanAligns returns them."""
+    ba, oa, bb, ob, pa, pb, lut_a, lut_b, table = _pair_inputs(seqs_a, seqs_b, pairs, scoring)
+    n = len(pa)
+    la, lb = np.diff(oa.astype(np.int64)), np.diff(ob.astype(np.int64))
+    longest = int((la[pa] + lb[pb]).max()) if n else 0
+    stride = max(longest, 1)  # an alignment never has more columns than len(a) + len(b)
+    fn = _lib.lib().pg_nw_align_pairs if global_alignment else _lib.lib().pg_sw_align_pairs
+    score, ec, ep = np.zeros(n, np.int64), np.zeros(n, np.int32), np.zeros(n, np.int64)
+    out_a, out_b = np.zeros((max(n, 1), stride), np.uint8), np.zeros((max(n, 1), stride), np.uint8)
+    ln, st = np.zeros(n, np.uint32), np.zeros(n, np.int32)
+    _lib.check(fn(ba.ctypes.data, oa.ctypes.data, len(oa) - 1, bb.ctypes.data, ob.ctypes.data, len(ob) - 1, pa.ctypes.data, pb.ctypes.data, n,
+                  lut_a.ctypes.data, lut_b.ctypes.data, table.ctypes.data, table.shape[0], table.shape[1], scoring.GapPenalty,
+                  score.ctypes.data, ec.ctypes.data, ep.ctypes.data, out_a.ctypes.data, out_b.ctypes.data, stride, ln.ctypes.data,
+                  st.ctypes.data))
+    errs = _pair_errors(ec, ep, ba, oa, bb, ob, pa, pb)
+    return [(0, "", "", errs[k]) if errs[k] is not None else
+            (int(score[k]), bytes(out_a[k, : ln[k]]).decode("latin-1"), bytes(out_b[k, : ln[k]]).decode("latin-1"), None)
+            for k in range(n)]
+
+
+def NeedlemanWunschPairAligns(seqs_a, seqs_b, pairs, scoring: Scoring):
+    """Full align.NeedlemanWunsch for every (i, j) row of `pairs`: [(score, alignA, alignB, err)]."""
+    return SmithWatermanPairAligns(seqs_a, seqs_b, pairs, scoring, global_alignment=True)
+
+
+def pair_scores_device(d_seqs_a, d_offsets_a, max_len_a: int, d_seqs_b, d_offsets_b, max_len_b: int, d_pairs, scoring: Scoring,
+                       global_alignment: bool = False, stream=None):
+    """pg_sw_score_pairs_dev / pg_nw_score_pairs_dev on torch CUDA tensors: d_offsets_* int64 [n + 1], d_pairs an
+    integer [n, 2] tensor (int32 is taken as the uint32 bits of the index; wider indices outside [0, 2^32) are
+    flagged, never truncated to a valid one).  Returns (score int64[n],
+    err_code int32[n], err_pos int64[n]) on the device; err_code PG_PAIR_OUT_OF_RANGE (3) marks a pair
+    whose index or length is out of range.  Only enqueues work on the stream."""
+    import torch
+
+    m = scoring.SubstitutionMatrix
+    lut_a, lut_b = m.FirstAlphabet.byte_lut(), m.SecondAlphabet.byte_lut()
+    table = np.ascontiguousarray(m.scores, dtype=np.int64)
+    dev = d_offsets_a.device
+    if d_pairs.dim() != 2 or d_pairs.shape[1] != 2:
+        raise ValueError(f"d_pairs must be an (n, 2) tensor, got shape {tuple(d_pairs.shape)}")
+
+    def column(x):  # uint32 bits; an index outside [0, 2^32) becomes 2^32 - 1, which the kernel flags (no host sync)
+        if x.dtype == torch.int32:
+            return x.contiguous()
+        x = x.to(torch.int64)
+        return torch.where((x < 0) | (x > 0xFFFFFFFF), torch.full_like(x, 0xFFFFFFFF), x).to(torch.int32).contiguous()
+
+    pa, pb = column(d_pairs[:, 0]), column(d_pairs[:, 1])
+    n = pa.numel()
+    score = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    code = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    pos = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    st = stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream
+    fn = _lib.lib().pg_nw_score_pairs_dev if global_alignment else _lib.lib().pg_sw_score_pairs_dev
+    _lib.check(fn(d_seqs_a.data_ptr(), d_offsets_a.data_ptr(), d_offsets_a.numel() - 1, max_len_a, d_seqs_b.data_ptr(), d_offsets_b.data_ptr(),
+                  d_offsets_b.numel() - 1, max_len_b, pa.data_ptr(), pb.data_ptr(), n, lut_a.ctypes.data, lut_b.ctypes.data,
+                  table.ctypes.data, table.shape[0], table.shape[1], scoring.GapPenalty, score.data_ptr(), code.data_ptr(),
+                  pos.data_ptr(), C.c_void_p(st)))
+    return score[:n], code[:n], pos[:n]

@@ -30,6 +30,8 @@ struct LongParams {
     int query_is_a, n_b, gap;
     uint64_t out_stride;
     uint64_t cells_per_pair;  // (max_qlen + 1) * (tlen + 1): stride of a pair's matrix
+    const uint64_t *toff;     // non-null: item k is query pq[k] against template pt[k] of (t, toff)
+    const uint32_t *pq, *pt;
 };
 
 template <bool GLOBAL>
@@ -39,12 +41,15 @@ align_long_kernel(LongParams p, const int16_t *__restrict__ lut_a, const int16_t
                   int *__restrict__ matrices, uint8_t *__restrict__ out_a, uint8_t *__restrict__ out_b,
                   uint32_t *__restrict__ out_len, int32_t *__restrict__ status) {
     __shared__ unsigned long long s_first;  // SW: smallest (i << 32 | j) with H[i][j] == B
-    const uint64_t qi = p.q_first + blockIdx.x;
-    const uint64_t qbeg = p.qoff[qi];
-    const uint64_t qlen = p.qoff[qi + 1] - qbeg;
+    const uint64_t qi = p.q_first + blockIdx.x;  // the item: index of every output
+    const uint64_t qs = p.toff ? p.pq[qi] : qi;
+    const uint64_t qbeg = p.qoff[qs];
+    const uint64_t qlen = p.qoff[qs + 1] - qbeg;
+    const uint8_t *tp = p.toff ? p.t + p.toff[p.pt[qi]] : p.t;
+    const uint64_t tlen = p.toff ? p.toff[p.pt[qi] + 1] - p.toff[p.pt[qi]] : p.tlen;
     // stringA indexes the rows (outer loop of the reference), stringB the columns
-    const uint8_t *A = p.query_is_a ? p.q + qbeg : p.t, *B = p.query_is_a ? p.t : p.q + qbeg;
-    const uint64_t la = p.query_is_a ? qlen : p.tlen, lb = p.query_is_a ? p.tlen : qlen;
+    const uint8_t *A = p.query_is_a ? p.q + qbeg : tp, *B = p.query_is_a ? tp : p.q + qbeg;
+    const uint64_t la = p.query_is_a ? qlen : tlen, lb = p.query_is_a ? tlen : qlen;
     const int best = err[qi] ? 0 : (int)score[qi];
     const bool active = GLOBAL ? (!err[qi] && la > 0 && lb > 0) : best > 0;
     if (!active) {  // SW: maxScore never updated, the loop does not run; NW: a string is empty
@@ -108,7 +113,7 @@ int launch_sw_align_long(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq
                          uint64_t tlen, int query_is_a, const int16_t *lut_a, const int16_t *lut_b, const int64_t *table,
                          int n_a, int n_b, int64_t gap, const int64_t *d_score, const int32_t *d_err, uint8_t *d_align_a,
                          uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status, cudaStream_t st,
-                         int global) {
+                         int global, const uint64_t *d_toff, const uint32_t *d_pq, const uint32_t *d_pt) {
     if (nq == 0) return PG_OK;
     int64_t amax = 0;
     for (int i = 0; i < n_a * n_b; ++i) amax = std::max<int64_t>(amax, table[i] < 0 ? -table[i] : table[i]);
@@ -138,6 +143,7 @@ int launch_sw_align_long(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq
     LongParams p;
     p.q = d_q; p.qoff = d_qoff; p.t = d_t; p.tlen = tlen; p.query_is_a = query_is_a; p.n_b = n_b; p.gap = (int)gap;
     p.out_stride = out_stride; p.cells_per_pair = cells;
+    p.toff = d_toff; p.pq = d_pq; p.pt = d_pt;
     for (uint64_t q0 = 0; q0 < nq; q0 += per) {
         p.q_first = q0;
         p.n = std::min(per, nq - q0);
