@@ -22,6 +22,18 @@ import (
 // ErrPanic is returned where the pure-Go reference would panic (index out of range).
 var ErrPanic = errors.New("poly: reference panics on this input (index out of range)")
 
+// ErrCloneUnsupported is returned by the clone wrappers for PG_ERR_UNSUPPORTED: a part or fragment with a
+// byte >= 0x80 (strings.ToUpper would re-encode it), or an enzyme site that is not a plain literal.
+var ErrCloneUnsupported = errors.New("clone: unsupported input (non-literal enzyme site or non-ASCII byte)")
+
+// cloneCheck is check with PG_ERR_UNSUPPORTED mapped to ErrCloneUnsupported.
+func cloneCheck(rc C.int) error {
+	if rc == C.PG_ERR_UNSUPPORTED {
+		return ErrCloneUnsupported
+	}
+	return check(rc)
+}
+
 // locked runs one C ABI call with the goroutine pinned to its OS thread, so that pg_last_error()
 // (a thread-local string) is read on the thread that produced it.
 func locked(call func() C.int) error {
@@ -613,4 +625,147 @@ func LeastRotationBatch(bases []byte, offsets []uint64) ([]uint64, error) {
 		return C.pg_least_rotation_batch(p, (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n), (*C.uint64_t)(unsafe.Pointer(&rot[0])))
 	})
 	return rot[:n], err
+}
+
+// CloneEnzyme is an enzyme for the clone entry points: the two sites are literals (clone.go:77-84).
+type CloneEnzyme struct {
+	ForwardSite, ReverseSite, RecognitionSite string
+	Skip, OverheadLength                      int
+}
+
+// cEnzymes copies enzymes into C memory (the struct holds pointers, which may not point into Go memory);
+// free releases it.
+func cEnzymes(enzymes []CloneEnzyme) (p *C.pg_clone_enzyme, free func()) {
+	n := len(enzymes)
+	arr := (*[1 << 20]C.pg_clone_enzyme)(C.malloc(C.size_t(n+1) * C.size_t(unsafe.Sizeof(C.pg_clone_enzyme{}))))[: n+1 : n+1]
+	var strs []unsafe.Pointer
+	cstr := func(s string) *C.uint8_t {
+		b := C.CBytes([]byte(s + "\x00"))
+		strs = append(strs, b)
+		return (*C.uint8_t)(b)
+	}
+	for i, e := range enzymes {
+		arr[i] = C.pg_clone_enzyme{forward_site: cstr(e.ForwardSite), forward_len: C.uint32_t(len(e.ForwardSite)),
+			reverse_site: cstr(e.ReverseSite), reverse_len: C.uint32_t(len(e.ReverseSite)),
+			recognition_site: cstr(e.RecognitionSite), recognition_len: C.uint32_t(len(e.RecognitionSite)),
+			skip: C.int32_t(e.Skip), overhang_length: C.int32_t(e.OverheadLength)}
+	}
+	return &arr[0], func() {
+		for _, s := range strs {
+			C.free(s)
+		}
+		C.free(unsafe.Pointer(&arr[0]))
+	}
+}
+
+// CloneFragments is pg_clone_digest_batch's output: fragment f is Seq[SeqOff[f]:SeqOff[f+1]] with overhangs
+// OH[OHOff[2f]:OHOff[2f+1]] and OH[OHOff[2f+1]:OHOff[2f+2]]; Count[i] fragments for item i.
+type CloneFragments struct {
+	Count         []uint32
+	Status        []int32
+	Seq, OH       []byte
+	SeqOff, OHOff []uint64
+}
+
+// CloneDigest wraps pg_clone_digest_batch: CutWithEnzyme of every part x enzyme (item = part*len(enzymes)+enzyme).
+// ErrPanic when an item panics in the reference; the other items' fragments are still returned.
+func CloneDigest(bases []byte, offsets []uint64, circular []bool, enzymes []CloneEnzyme, directional bool) (*CloneFragments, error) {
+	n := len(offsets) - 1
+	circ := make([]uint8, n+1)
+	for i, c := range circular {
+		if c {
+			circ[i] = 1
+		}
+	}
+	enz, free := cEnzymes(enzymes)
+	defer free()
+	dir := C.int32_t(0)
+	if directional {
+		dir = 1
+	}
+	items := n*len(enzymes) + 1
+	out := &CloneFragments{Count: make([]uint32, items), Status: make([]int32, items)}
+	var caps, need [3]C.uint64_t
+	for {
+		out.Seq, out.OH = make([]byte, caps[1]+1), make([]byte, caps[2]+1)
+		out.SeqOff, out.OHOff = make([]uint64, caps[0]+1), make([]uint64, 2*caps[0]+1)
+		rc := C.int(0)
+		_ = locked(func() C.int {
+			rc = C.pg_clone_digest_batch((*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])),
+				(*C.uint8_t)(unsafe.Pointer(&circ[0])), C.uint64_t(n), enz, C.uint32_t(len(enzymes)), dir,
+				(*C.uint32_t)(unsafe.Pointer(&out.Count[0])), (*C.int32_t)(unsafe.Pointer(&out.Status[0])),
+				(*C.uint8_t)(unsafe.Pointer(&out.Seq[0])), caps[1], (*C.uint64_t)(unsafe.Pointer(&out.SeqOff[0])),
+				(*C.uint8_t)(unsafe.Pointer(&out.OH[0])), caps[2], (*C.uint64_t)(unsafe.Pointer(&out.OHOff[0])), caps[0],
+				&need[0], &need[1], &need[2])
+			return rc
+		})
+		if rc == C.PG_ERR_ARG && (need[0] > caps[0] || need[1] > caps[1] || need[2] > caps[2]) {
+			caps = need
+			continue
+		}
+		out.Count, out.Status = out.Count[:items-1], out.Status[:items-1]
+		return out, cloneCheck(rc)
+	}
+}
+
+// CloneConstructs is the output of the ligation entry points: construct k is Bytes[Off[k]:Off[k+1]],
+// Kind[k] 0 a clone or 1 a looping construct; Counts[2r], Counts[2r+1] per reaction; Status[r] per reaction.
+type CloneConstructs struct {
+	Bytes  []byte
+	Off    []uint64
+	Kind   []uint8
+	Counts []uint64
+	Status []int32
+}
+
+// cloneLigation runs one ligation entry point with buffers grown to the reported need.
+func cloneLigation(nReactions int, call func(bcap, ccap C.uint64_t, o *CloneConstructs, nb, nc *C.uint64_t) C.int) (*CloneConstructs, error) {
+	bcap, ccap := C.uint64_t(1<<20), C.uint64_t(1<<12)
+	for {
+		o := &CloneConstructs{Bytes: make([]byte, bcap+1), Off: make([]uint64, ccap+1), Kind: make([]uint8, ccap+1),
+			Counts: make([]uint64, 2*nReactions+2), Status: make([]int32, nReactions+1)}
+		var nb, nc C.uint64_t
+		rc := C.int(0)
+		_ = locked(func() C.int { rc = call(bcap, ccap, o, &nb, &nc); return rc })
+		if rc == C.PG_ERR_ARG && (nb > bcap || nc > ccap) {
+			if nb > bcap {
+				bcap = nb
+			}
+			if nc > ccap {
+				ccap = nc
+			}
+			continue
+		}
+		return o, cloneCheck(rc)
+	}
+}
+
+// CloneGoldenGate wraps pg_clone_golden_gate_batch: reaction r is parts [reactionOffsets[r], reactionOffsets[r+1]).
+func CloneGoldenGate(bases []byte, offsets []uint64, circular []bool, reactionOffsets []uint64, enzyme CloneEnzyme) (*CloneConstructs, error) {
+	n, R := len(offsets)-1, len(reactionOffsets)-1
+	circ := make([]uint8, n+1)
+	for i, c := range circular {
+		if c {
+			circ[i] = 1
+		}
+	}
+	enz, free := cEnzymes([]CloneEnzyme{enzyme})
+	defer free()
+	return cloneLigation(R, func(bcap, ccap C.uint64_t, o *CloneConstructs, nb, nc *C.uint64_t) C.int {
+		return C.pg_clone_golden_gate_batch((*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])),
+			(*C.uint8_t)(unsafe.Pointer(&circ[0])), C.uint64_t(n), (*C.uint64_t)(unsafe.Pointer(&reactionOffsets[0])), C.uint64_t(R), enz,
+			bcap, ccap, (*C.uint8_t)(unsafe.Pointer(&o.Bytes[0])), (*C.uint64_t)(unsafe.Pointer(&o.Off[0])), (*C.uint8_t)(unsafe.Pointer(&o.Kind[0])),
+			nil, (*C.uint64_t)(unsafe.Pointer(&o.Counts[0])), (*C.int32_t)(unsafe.Pointer(&o.Status[0])), nb, nc)
+	})
+}
+
+// CloneCircularLigate wraps pg_clone_circular_ligate_batch on fragments in CloneFragments' layout.
+func CloneCircularLigate(seq []byte, seqOff []uint64, oh []byte, ohOff []uint64, reactionOffsets []uint64) (*CloneConstructs, error) {
+	nf, R := len(seqOff)-1, len(reactionOffsets)-1
+	return cloneLigation(R, func(bcap, ccap C.uint64_t, o *CloneConstructs, nb, nc *C.uint64_t) C.int {
+		return C.pg_clone_circular_ligate_batch((*C.uint8_t)(unsafe.Pointer(&seq[0])), (*C.uint64_t)(unsafe.Pointer(&seqOff[0])),
+			(*C.uint8_t)(unsafe.Pointer(&oh[0])), (*C.uint64_t)(unsafe.Pointer(&ohOff[0])), C.uint64_t(nf),
+			(*C.uint64_t)(unsafe.Pointer(&reactionOffsets[0])), C.uint64_t(R), bcap, ccap, (*C.uint8_t)(unsafe.Pointer(&o.Bytes[0])),
+			(*C.uint64_t)(unsafe.Pointer(&o.Off[0])), (*C.uint8_t)(unsafe.Pointer(&o.Kind[0])), nil, (*C.uint64_t)(unsafe.Pointer(&o.Counts[0])), nb, nc)
+	})
 }

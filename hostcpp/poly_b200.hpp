@@ -971,4 +971,162 @@ inline std::vector<std::string> RotateSequences(const std::vector<std::string> &
 }
 inline std::string RotateSequence(const std::string &sequence) { return RotateSequences({sequence})[0]; }
 }  // namespace seqhash
+// ---- clone (clone/clone.go:138-355) over pg_clone_digest_batch / pg_clone_golden_gate_batch /
+// pg_clone_circular_ligate_batch.  Enzyme patterns must be literals (UnsupportedError otherwise).
+namespace clone {
+struct UnsupportedError : std::runtime_error {
+    using std::runtime_error::runtime_error;
+};
+struct Part {
+    std::string Sequence;
+    bool Circular = false;
+};
+struct Fragment {
+    std::string Sequence, ForwardOverhang, ReverseOverhang;
+};
+struct Enzyme {
+    std::string Name, RegexpFor, RegexpRev;
+    int Skip = 0, OverheadLength = 0;
+    std::string RecognitionSite;
+};
+inline pg_clone_enzyme to_pg(const Enzyme &e) {
+    for (const std::string *p : {&e.RegexpFor, &e.RegexpRev})
+        if (p->empty() || p->size() > 32 || p->find_first_of("\\.+*?()|[]{}^$") != std::string::npos)
+            throw UnsupportedError("enzyme " + e.Name + ": pattern " + *p + " is not a literal (only literal sites are supported)");
+    return pg_clone_enzyme{(const uint8_t *)e.RegexpFor.data(), (uint32_t)e.RegexpFor.size(), (const uint8_t *)e.RegexpRev.data(),
+                           (uint32_t)e.RegexpRev.size(), (const uint8_t *)e.RecognitionSite.data(), (uint32_t)e.RecognitionSite.size(), e.Skip,
+                           e.OverheadLength};
+}
+inline std::vector<Enzyme> GetBaseRestrictionEnzymes() {  // clone.go:358-364
+    return {{"BsaI", "GGTCTC", "GAGACC", 1, 4, "GGTCTC"}, {"BbsI", "GAAGAC", "GTCTTC", 2, 4, "GAAGAC"}, {"BtgZI", "GCGATG", "CATCGC", 10, 4, "GCGATG"}};
+}
+inline void item_status(int32_t st) {
+    if (st == PG_ITEM_PANIC) throw GoPanic("slice bounds out of range");
+    if (st == PG_ITEM_UNSUPPORTED) throw UnsupportedError("a byte >= 0x80: strings.ToUpper would re-encode it (unsupported)");
+}
+// CutWithEnzyme of every part x enzyme: out[p][e]; an item that panics throws GoPanic
+inline std::vector<std::vector<std::vector<Fragment>>> CutWithEnzymeBatch(const std::vector<Part> &parts, bool directional,
+                                                                          const std::vector<Enzyme> &enzymes) {
+    std::vector<std::vector<std::vector<Fragment>>> out(parts.size(), std::vector<std::vector<Fragment>>(enzymes.size()));
+    if (parts.empty() || enzymes.empty()) return out;
+    std::vector<std::string> seqs;
+    std::vector<uint8_t> circ;
+    for (const Part &p : parts) { seqs.push_back(p.Sequence); circ.push_back(p.Circular); }
+    std::vector<pg_clone_enzyme> enz;
+    for (const Enzyme &e : enzymes) enz.push_back(to_pg(e));
+    Flat f(seqs);
+    const size_t n = parts.size() * enzymes.size();
+    std::vector<uint32_t> cnt(n);
+    std::vector<int32_t> st(n);
+    uint64_t caps[3] = {0, 0, 0}, need[3];
+    std::vector<uint8_t> sb, ob;
+    std::vector<uint64_t> so, oo;
+    for (;;) {
+        sb.assign(caps[1] + 1, 0); ob.assign(caps[2] + 1, 0); so.assign(caps[0] + 1, 0); oo.assign(2 * caps[0] + 1, 0);
+        const int rc = pg_clone_digest_batch(f.bases.data(), f.offsets.data(), circ.data(), parts.size(), enz.data(), (uint32_t)enz.size(), directional,
+                                             cnt.data(), st.data(), sb.data(), caps[1], so.data(), ob.data(), caps[2], oo.data(), caps[0], &need[0],
+                                             &need[1], &need[2]);
+        if (rc == PG_ERR_ARG && (need[0] > caps[0] || need[1] > caps[1] || need[2] > caps[2])) {
+            for (int k = 0; k < 3; ++k) caps[k] = need[k];
+            continue;
+        }
+        if (rc != PG_ERR_PANIC && rc != PG_ERR_UNSUPPORTED) check(rc);
+        break;
+    }
+    size_t fr = 0;
+    for (size_t i = 0; i < n; ++i)
+        for (uint32_t k = 0; k < cnt[i]; ++k, ++fr)
+            out[i / enzymes.size()][i % enzymes.size()].push_back(
+                Fragment{std::string((const char *)sb.data() + so[fr], so[fr + 1] - so[fr]), std::string((const char *)ob.data() + oo[2 * fr], oo[2 * fr + 1] - oo[2 * fr]),
+                         std::string((const char *)ob.data() + oo[2 * fr + 1], oo[2 * fr + 2] - oo[2 * fr + 1])});
+    for (size_t i = 0; i < n; ++i)
+        if (st[i] == PG_ITEM_PANIC) item_status(st[i]);
+    for (size_t i = 0; i < n; ++i) item_status(st[i]);
+    return out;
+}
+inline std::vector<Fragment> CutWithEnzyme(const Part &part, bool directional, const Enzyme &enzyme) {
+    return CutWithEnzymeBatch({part}, directional, {enzyme})[0][0];
+}
+class EnzymeManager {
+    std::map<std::string, Enzyme> enzymeMap;
+
+public:
+    explicit EnzymeManager(const std::vector<Enzyme> &enzymes) {
+        for (const Enzyme &e : enzymes) enzymeMap[e.Name] = e;
+    }
+    // (enzyme, error message); the message is "Enzyme X not found" when it is missing (clone.go:134)
+    std::pair<Enzyme, std::string> GetEnzymeByName(const std::string &name) const {
+        auto it = enzymeMap.find(name);
+        if (it == enzymeMap.end()) return {Enzyme{}, "Enzyme " + name + " not found"};
+        return {it->second, ""};
+    }
+    std::pair<std::vector<Fragment>, std::string> CutWithEnzymeByName(const Part &part, bool directional, const std::string &name) const {
+        auto e = GetEnzymeByName(name);
+        if (!e.second.empty()) return {{}, e.second};
+        return {CutWithEnzyme(part, directional, e.first), ""};
+    }
+};
+inline EnzymeManager NewEnzymeManager(const std::vector<Enzyme> &enzymes) { return EnzymeManager(enzymes); }
+
+using Constructs = std::pair<std::vector<std::string>, std::vector<std::string>>;  // (clones, looping constructs)
+// call(bytes_cap, constructs_cap, out, offsets, kinds, counts, status, need_bytes, need_constructs)
+// per_reaction: the call reports unsupported input per reaction (GoldenGate); otherwise it refuses the call
+template <typename Call>
+std::vector<Constructs> ligation_outputs(size_t n_reactions, Call call, bool per_reaction = true) {
+    uint64_t bcap = 1 << 20, ccap = 1 << 12, nb = 0, nc = 0;
+    std::vector<uint8_t> out, kinds;
+    std::vector<uint64_t> off, counts(2 * n_reactions + 2);
+    std::vector<int32_t> st(n_reactions + 1);
+    for (;;) {
+        out.assign(bcap + 1, 0); off.assign(ccap + 1, 0); kinds.assign(ccap + 1, 0);
+        const int rc = call(bcap, ccap, out.data(), off.data(), kinds.data(), counts.data(), st.data(), &nb, &nc);
+        if (rc == PG_ERR_ARG && (nb > bcap || nc > ccap)) {
+            bcap = std::max(bcap, nb);
+            ccap = std::max(ccap, nc);
+            continue;
+        }
+        if (rc == PG_ERR_UNSUPPORTED && !per_reaction) throw UnsupportedError(pg_last_error());
+        if (rc != PG_ERR_PANIC && rc != PG_ERR_UNSUPPORTED) check(rc);
+        break;
+    }
+    std::vector<Constructs> res(n_reactions);
+    size_t k = 0;
+    for (size_t r = 0; r < n_reactions; ++r) {
+        item_status(st[r]);
+        for (uint64_t j = 0; j < counts[2 * r] + counts[2 * r + 1]; ++j, ++k)
+            (kinds[k] == 0 ? res[r].first : res[r].second).emplace_back((const char *)out.data() + off[k], off[k + 1] - off[k]);
+    }
+    return res;
+}
+inline std::vector<Constructs> GoldenGateBatch(const std::vector<std::vector<Part>> &reactions, const Enzyme &enzyme) {
+    std::vector<std::string> seqs;
+    std::vector<uint8_t> circ;
+    std::vector<uint64_t> roff{0};
+    for (const auto &r : reactions) {
+        for (const Part &p : r) { seqs.push_back(p.Sequence); circ.push_back(p.Circular); }
+        roff.push_back(seqs.size());
+    }
+    circ.push_back(0);
+    Flat f(seqs);
+    const pg_clone_enzyme e = to_pg(enzyme);
+    return ligation_outputs(reactions.size(), [&](uint64_t bcap, uint64_t ccap, uint8_t *out, uint64_t *off, uint8_t *kinds, uint64_t *counts,
+                                                  int32_t *st, uint64_t *nb, uint64_t *nc) {
+        return pg_clone_golden_gate_batch(f.bases.data(), f.offsets.data(), circ.data(), seqs.size(), roff.data(), reactions.size(), &e, bcap, ccap, out,
+                                          off, kinds, nullptr, counts, st, nb, nc);
+    });
+}
+inline Constructs GoldenGate(const std::vector<Part> &sequences, const Enzyme &cuttingEnzyme) { return GoldenGateBatch({sequences}, cuttingEnzyme)[0]; }
+inline Constructs CircularLigate(const std::vector<Fragment> &fragments) {
+    std::vector<std::string> seqs, ohs;
+    for (const Fragment &f : fragments) { seqs.push_back(f.Sequence); ohs.push_back(f.ForwardOverhang); ohs.push_back(f.ReverseOverhang); }
+    Flat s(seqs), o(ohs);
+    const uint64_t roff[2] = {0, fragments.size()};
+    return ligation_outputs(1, [&](uint64_t bcap, uint64_t ccap, uint8_t *out, uint64_t *off, uint8_t *kinds, uint64_t *counts, int32_t *st,
+                                   uint64_t *nb, uint64_t *nc) {
+        st[0] = PG_ITEM_OK;
+        return pg_clone_circular_ligate_batch(s.bases.data(), s.offsets.data(), o.bases.data(), o.offsets.data(), fragments.size(), roff, 1, bcap, ccap,
+                                              out, off, kinds, nullptr, counts, nb, nc);
+    }, false)[0];
+}
+}  // namespace clone
 }  // namespace poly

@@ -528,6 +528,67 @@ int pg_seqhash_batch_dev(const uint8_t *d_seqs, const uint64_t *d_offsets, uint6
  * empty); RotateSequence(s) = s[r:] + s[:r]. */
 int pg_least_rotation_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, uint64_t *rotation);
 
+/* ---- clone.CutWithEnzyme / CircularLigate / GoldenGate -- clone/clone.go:138-355 --------------------
+ * An enzyme: RegexpFor and RegexpRev as literal sites (1..32 bytes of 0x01..0x7f; anything else is
+ * PG_ERR_UNSUPPORTED: the library does not implement Go's regexp language), Skip, OverheadLength and
+ * RecognitionSite.  Palindromic = RecognitionSite equals its reverse complement (checks.IsPalindromic). */
+typedef struct {
+    const uint8_t *forward_site;
+    uint32_t forward_len;
+    const uint8_t *reverse_site;
+    uint32_t reverse_len;
+    const uint8_t *recognition_site;
+    uint32_t recognition_len;
+    int32_t skip;
+    int32_t overhang_length;
+} pg_clone_enzyme;
+/* CutWithEnzyme(part p, directional, enzyme e) for every item i = p * n_enzymes + e, exactly as the
+ * reference (quirks included): ToUpper(part) or ToUpper(part + part) when circular[p] != 0, leftmost
+ * non-overlapping matches of each site, the linear drop of the last overhang of a set, the stable sort,
+ * the four fragment branches and the len > 8 filter.  Per item: frag_count[i] and status[i] (may be
+ * NULL): PG_ITEM_PANIC where a slice of the reference is out of range (no fragments; the call returns
+ * PG_ERR_PANIC after writing everything else), PG_ITEM_UNSUPPORTED for a byte >= 0x80 (strings.ToUpper
+ * would re-encode it).  Fragments in item order: Sequence f = seq_bytes[seq_offsets[f], seq_offsets[f+1]),
+ * ForwardOverhang = oh_bytes[oh_offsets[2f], oh_offsets[2f+1]), ReverseOverhang = oh_bytes[oh_offsets[2f+1],
+ * oh_offsets[2f+2]); seq_offsets has frag_cap + 1 entries, oh_offsets 2 * frag_cap + 1.  *n_frags,
+ * *n_seq_bytes and *n_oh_bytes are always written; more than frag_cap, seq_cap or oh_cap is PG_ERR_ARG
+ * (frag_count and status are written, the fragments are not).  A batch in which a part could hold 2^32 or
+ * more matches of a site (2 L / site length for a circular part) is PG_ERR_ARG before any launch. */
+int pg_clone_digest_batch(const uint8_t *parts, const uint64_t *part_offsets, const uint8_t *circular, uint64_t n_parts,
+                          const pg_clone_enzyme *enzymes, uint32_t n_enzymes, int32_t directional, uint32_t *frag_count,
+                          int32_t *status, uint8_t *seq_bytes, uint64_t seq_cap, uint64_t *seq_offsets, uint8_t *oh_bytes,
+                          uint64_t oh_cap, uint64_t *oh_offsets, uint64_t frag_cap, uint64_t *n_frags, uint64_t *n_seq_bytes,
+                          uint64_t *n_oh_bytes);
+/* GoldenGate(parts of reaction r, enzyme) for n_reactions independent reactions: reaction r is parts
+ * [reaction_offsets[r], reaction_offsets[r+1]) (reaction_offsets runs from 0 to n_parts).  All parts are
+ * digested (directional) in one launch; recurseLigate runs on the host over fragment ids; every
+ * construct it would hash is built and seqhashed on the device, in groups under a device-memory budget.
+ * Per reaction the output keeps, in the reference's order, the first construct of each seqhash, as
+ * CircularLigate's existingSeqhashes does.  Outputs: constructs of reaction 0, then 1, ..., each reaction's
+ * in the reference's hashing order; construct k = out[construct_offsets[k], construct_offsets[k+1]),
+ * kinds[k] 0 a clone (openConstructs) or 1 a looping construct (infiniteLoops), digests[32 k ..] its seqhash
+ * digest (kinds and digests may be NULL); counts[2 r], counts[2 r + 1] = clones and loops of reaction r.
+ * The work is bounded by the caller: *need_bytes and *need_constructs (always written) are the bytes and
+ * the number of all constructs the ligations hash, duplicates included; more than bytes_cap or
+ * constructs_cap is PG_ERR_ARG before anything is built.  Sized at the need, out holds bytes_cap bytes and
+ * construct_offsets constructs_cap + 1 entries.  status[r] (may be NULL): PG_ITEM_PANIC / _UNSUPPORTED
+ * when a part of the reaction cuts that way (the reaction has no constructs; the call returns
+ * PG_ERR_PANIC / PG_ERR_UNSUPPORTED after writing everything else). */
+int pg_clone_golden_gate_batch(const uint8_t *parts, const uint64_t *part_offsets, const uint8_t *circular, uint64_t n_parts,
+                               const uint64_t *reaction_offsets, uint64_t n_reactions, const pg_clone_enzyme *enzyme,
+                               uint64_t bytes_cap, uint64_t constructs_cap, uint8_t *out, uint64_t *construct_offsets,
+                               uint8_t *kinds, uint8_t *digests, uint64_t *counts, int32_t *status, uint64_t *need_bytes,
+                               uint64_t *need_constructs);
+/* CircularLigate on caller-given fragments, in pg_clone_digest_batch's layout (n_frags fragments),
+ * grouped into reactions by reaction_offsets (from 0 to n_frags); outputs as pg_clone_golden_gate_batch.
+ * A fragment byte >= 0x80 is PG_ERR_UNSUPPORTED before anything is launched: seqhash.Hash's
+ * strings.ToUpper would re-encode it (and maps some such letters into the alphabet). */
+int pg_clone_circular_ligate_batch(const uint8_t *seq_bytes, const uint64_t *seq_offsets, const uint8_t *oh_bytes,
+                                   const uint64_t *oh_offsets, uint64_t n_frags, const uint64_t *reaction_offsets,
+                                   uint64_t n_reactions, uint64_t bytes_cap, uint64_t constructs_cap, uint8_t *out,
+                                   uint64_t *construct_offsets, uint8_t *kinds, uint8_t *digests, uint64_t *counts,
+                                   uint64_t *need_bytes, uint64_t *need_constructs);
+
 /* ---- synthetic workloads (SURVEY.md 8d; bench/test tooling, not a reference API) ---
  * kind 0: independent reads  base(i,j) = code(seed, i*L + j)
  * kind 1: family reads       (family = reads per template, 1/64 substitutions)

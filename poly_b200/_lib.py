@@ -99,6 +99,12 @@ _SIGS = {
     "pg_seqhash_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_int32, C.c_uint32, _u8p, _i32p, _u64p]),
     "pg_seqhash_batch_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_int32, C.c_uint32, _u8p, _i32p, _u64p, C.c_uint64, C.c_void_p]),
     "pg_least_rotation_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p]),
+    "pg_clone_digest_batch": (C.c_int, [_u8p, _u64p, _u8p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_int32, _u32p, _i32p, _u8p, C.c_uint64, _u64p, _u8p,
+                                        C.c_uint64, _u64p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "pg_clone_golden_gate_batch": (C.c_int, [_u8p, _u64p, _u8p, C.c_uint64, _u64p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint64, _u8p, _u64p, _u8p,
+                                             _u8p, _u64p, _i32p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "pg_clone_circular_ligate_batch": (C.c_int, [_u8p, _u64p, _u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_uint64, C.c_uint64, _u8p, _u64p, _u8p,
+                                                 _u8p, _u64p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "pg_synth_reads_dev": (C.c_int, [_u8p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_int32, C.c_uint32, C.c_void_p]),
 }
 EXPORTS = tuple(_SIGS)

@@ -30,6 +30,22 @@ int sm_count();
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) cached per (device, kernel); thread-safe (api.cu)
 int func_smem(const void *kernel, size_t bytes);
 
+// transform.complementTable (transform.go:78-109): every unlisted byte maps to 0, including the DNA
+// letters U and Z.  Seqhash reads it on upper-cased bytes; the clone ligation on fragments as given.
+__host__ __device__ __forceinline__ uint8_t complement(uint8_t c) {
+    switch (c) {
+        case 'A': return 'T'; case 'B': return 'V'; case 'C': return 'G'; case 'D': return 'H';
+        case 'G': return 'C'; case 'H': return 'D'; case 'K': return 'M'; case 'M': return 'K';
+        case 'N': return 'N'; case 'R': return 'Y'; case 'S': return 'S'; case 'T': return 'A';
+        case 'V': return 'B'; case 'W': return 'W'; case 'Y': return 'R';
+        case 'a': return 't'; case 'b': return 'v'; case 'c': return 'g'; case 'd': return 'h';
+        case 'g': return 'c'; case 'h': return 'd'; case 'k': return 'm'; case 'm': return 'k';
+        case 'n': return 'n'; case 'r': return 'y'; case 's': return 's'; case 't': return 'a';
+        case 'v': return 'b'; case 'w': return 'w'; case 'y': return 'r';
+        default: return 0;
+    }
+}
+
 // Stream-ordered temporaries that are released together when the scope ends -- also on the early
 // returns of PG_CUDA -- with cudaFreeAsync on the stream they were allocated on.
 struct StreamScratch {

@@ -30,18 +30,6 @@ __device__ __forceinline__ uint8_t fold(uint8_t c, int mode) {
     return c;
 }
 
-// transform.complementTable (transform.go:78-109) on upper-case bytes: every other byte maps to 0,
-// including the DNA letters U and Z
-__device__ __forceinline__ uint8_t complement(uint8_t c) {
-    switch (c) {
-        case 'A': return 'T'; case 'B': return 'V'; case 'C': return 'G'; case 'D': return 'H';
-        case 'G': return 'C'; case 'H': return 'D'; case 'K': return 'M'; case 'M': return 'K';
-        case 'N': return 'N'; case 'R': return 'Y'; case 'S': return 'S'; case 'T': return 'A';
-        case 'V': return 'B'; case 'W': return 'W'; case 'Y': return 'R';
-        default: return 0;
-    }
-}
-
 // Byte maps of one call in shared memory: map[0][c] = fold(c), map[1][c] = complement(fold(c)).  Every CTA
 // fills them once; a lookup replaces the compare chains on every read.
 __device__ __forceinline__ void fill_maps(uint8_t (*map)[256], int mode) {
