@@ -627,6 +627,34 @@ func LeastRotationBatch(bases []byte, offsets []uint64) ([]uint64, error) {
 	return rot[:n], err
 }
 
+// FoldZukerBatch wraps pg_fold_zuker_batch: per sequence the minimum free energy, the dot-bracket and the
+// item status (PG_ITEM_*).  PG_ERR_PANIC / PG_ERR_UNSUPPORTED are per-item outcomes here, not call errors.
+func FoldZukerBatch(bases []byte, offsets []uint64, temp float64) (mfe []float64, dotBracket []string, status []int32, err error) {
+	n := len(offsets) - 1
+	mfe, status = make([]float64, n+1), make([]int32, n+1)
+	dbLen := make([]uint64, n+1)
+	db := make([]byte, len(bases)+1)
+	var p *C.uint8_t
+	if len(bases) > 0 {
+		p = (*C.uint8_t)(unsafe.Pointer(&bases[0]))
+	}
+	err = locked(func() C.int {
+		rc := C.pg_fold_zuker_batch(p, (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n), C.double(temp),
+			(*C.double)(unsafe.Pointer(&mfe[0])), (*C.uint8_t)(unsafe.Pointer(&db[0])), (*C.uint64_t)(unsafe.Pointer(&dbLen[0])),
+			(*C.int32_t)(unsafe.Pointer(&status[0])))
+		if rc == C.PG_ERR_PANIC || rc == C.PG_ERR_UNSUPPORTED {
+			return C.PG_OK
+		}
+		return rc
+	})
+	dotBracket = make([]string, n)
+	for i := 0; i < n; i++ {
+		b := offsets[i] - offsets[0]
+		dotBracket[i] = string(db[b : b+dbLen[i]])
+	}
+	return mfe[:n], dotBracket, status[:n], err
+}
+
 // CloneEnzyme is an enzyme for the clone entry points: the two sites are literals (clone.go:77-84).
 type CloneEnzyme struct {
 	ForwardSite, ReverseSite, RecognitionSite string

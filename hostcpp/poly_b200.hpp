@@ -22,6 +22,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <limits>
 #include <map>
 #include <stdexcept>
 #include <string>
@@ -1129,4 +1130,59 @@ inline Constructs CircularLigate(const std::vector<Fragment> &fragments) {
     }, false)[0];
 }
 }  // namespace clone
+// ---- fold (fold/fold.go, fold/seqfold.go) over pg_fold_zuker_batch --------------------------------------
+namespace fold {
+struct UnsupportedError : std::runtime_error {
+    using std::runtime_error::runtime_error;
+};
+// fold.Result: the minimum free energy and dot-bracket of the folded structure (Result{} gives +inf and "")
+struct Result {
+    double mfe = std::numeric_limits<double>::infinity();
+    std::string dot_bracket;
+    double MinimumFreeEnergy() const { return mfe; }
+    std::string DotBracket() const { return dot_bracket; }
+};
+// one item of ZukerBatch: status is PG_ITEM_OK, PG_ITEM_FOLD_NOT_NUCLEIC (error holds the reference's message),
+// PG_ITEM_PANIC, PG_ITEM_UNSUPPORTED or PG_ITEM_FOLD_INTERNAL
+struct Item {
+    Result result;
+    std::string error;
+    int32_t status = PG_ITEM_OK;
+};
+// Zuker of every sequence in one GPU call
+inline std::vector<Item> ZukerBatch(const std::vector<std::string> &seqs, double temp) {
+    std::vector<Item> out(seqs.size());
+    if (seqs.empty()) return out;
+    Flat f(seqs);
+    std::vector<double> mfe(seqs.size());
+    std::vector<uint8_t> db(std::max<size_t>(f.bases.size(), 1));
+    std::vector<uint64_t> len(seqs.size());
+    std::vector<int32_t> st(seqs.size());
+    const int rc = pg_fold_zuker_batch(f.bases.data(), f.offsets.data(), seqs.size(), temp, mfe.data(), db.data(), len.data(), st.data());
+    if (rc != PG_ERR_PANIC && rc != PG_ERR_UNSUPPORTED) check(rc);
+    for (size_t i = 0; i < seqs.size(); ++i) {
+        out[i].status = st[i];
+        if (st[i] == PG_ITEM_OK) {
+            out[i].result.mfe = mfe[i];
+            out[i].result.dot_bracket.assign((const char *)db.data() + f.offsets[i], len[i]);
+        } else if (st[i] == PG_ITEM_FOLD_NOT_NUCLEIC) {
+            std::string up = seqs[i];
+            for (auto &c : up)
+                if (c >= 'a' && c <= 'z') c -= 32;
+            out[i].error = "error creating folding context: the sequence " + up + " is not RNA or DNA";
+        } else if (st[i] == PG_ITEM_FOLD_INTERNAL) {
+            out[i].error = "fold.Zuker: an internal error of the reference fired on this sequence";
+        }
+    }
+    return out;
+}
+// fold.Zuker (fold.go:56): (Result, error message, empty on success); throws GoPanic where the reference
+// panics and UnsupportedError for a byte >= 0x80 or more than PG_FOLD_MAX_LEN nt
+inline std::pair<Result, std::string> Zuker(const std::string &seq, double temp) {
+    Item it = ZukerBatch({seq}, temp)[0];
+    if (it.status == PG_ITEM_PANIC) throw GoPanic("index out of range");
+    if (it.status == PG_ITEM_UNSUPPORTED) throw UnsupportedError("a byte >= 0x80 or more than PG_FOLD_MAX_LEN nt (unsupported)");
+    return {it.result, it.error};
+}
+}  // namespace fold
 }  // namespace poly

@@ -56,6 +56,8 @@ extern "C" {
 #define PG_ITEM_OK 0
 #define PG_ITEM_PANIC 1       /* reference panics (index out of range) on this item     */
 #define PG_ITEM_UNSUPPORTED 2 /* e.g. byte >= 0x80 passed to SantaLucia (ToUpper)       */
+#define PG_ITEM_FOLD_NOT_NUCLEIC 3 /* fold: "the sequence %s is not RNA or DNA"           */
+#define PG_ITEM_FOLD_INTERNAL 4    /* fold: one of the reference's internal errors fired  */
 
 /* ---- library / device management -------------------------------------------- */
 int pg_version(void);
@@ -527,6 +529,23 @@ int pg_seqhash_batch_dev(const uint8_t *d_seqs, const uint64_t *d_offsets, uint6
  * rotation[i] = the smallest start of the lexicographically least rotation of sequence i (0 when
  * empty); RotateSequence(s) = s[r:] + s[:r]. */
 int pg_least_rotation_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, uint64_t *rotation);
+
+/* ---- fold.Zuker -- fold/fold.go, fold/seqfold.go ----------------------------------------------------
+ * Folds sequences [offsets[i], offsets[i+1]) of `seqs` (n + 1 offsets) at temp degrees Celsius, as
+ * Zuker(seq, temp) followed by Result.MinimumFreeEnergy() and Result.DotBracket():
+ * mfe[i] (float64, bit for bit the reference's sum), the dot-bracket at dot_bracket[offsets[i] -
+ * offsets[0] ..] (laid out like seqs; it is never longer than the sequence) and its length db_len[i].
+ * status[i] (may be NULL): PG_ITEM_OK; PG_ITEM_FOLD_NOT_NUCLEIC where the upper-cased sequence is
+ * neither DNA (ACGT) nor RNA (ACGU), the reference's error "the sequence %s is not RNA or DNA";
+ * PG_ITEM_PANIC where the reference panics (0 or 1 nt, or a traceback shift out of range);
+ * PG_ITEM_UNSUPPORTED for a byte >= 0x80 (strings.ToUpper would re-encode it) or more than
+ * PG_FOLD_MAX_LEN nt; PG_ITEM_FOLD_INTERNAL if one of the reference's internal errors fired.  Items
+ * that are not OK get mfe 0, db_len 0 and '.' over their region of dot_bracket.  Returns PG_ERR_PANIC if any item panics, else
+ * PG_ERR_UNSUPPORTED if any is unsupported, with every output written.  Items go to the device in
+ * groups under a device-memory budget (about 34 n^2 + 0.13 n^3 bytes of scratch per n-nt item). */
+#define PG_FOLD_MAX_LEN 1024
+int pg_fold_zuker_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, double temp, double *mfe,
+                        uint8_t *dot_bracket, uint64_t *db_len, int32_t *status);
 
 /* ---- clone.CutWithEnzyme / CircularLigate / GoldenGate -- clone/clone.go:138-355 --------------------
  * An enzyme: RegexpFor and RegexpRev as literal sites (1..32 bytes of 0x01..0x7f; anything else is

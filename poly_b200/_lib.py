@@ -105,6 +105,7 @@ _SIGS = {
                                              _u8p, _u64p, _i32p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "pg_clone_circular_ligate_batch": (C.c_int, [_u8p, _u64p, _u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_uint64, C.c_uint64, _u8p, _u64p, _u8p,
                                                  _u8p, _u64p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "pg_fold_zuker_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_double, _f64p, _u8p, _u64p, _i32p]),
     "pg_synth_reads_dev": (C.c_int, [_u8p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_int32, C.c_uint32, C.c_void_p]),
 }
 EXPORTS = tuple(_SIGS)

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "../../include/poly_b200.h"
 
 namespace pg {
@@ -271,6 +273,12 @@ int launch_seqhash(const uint8_t *d_in, const uint64_t *d_off, uint64_t n, uint6
                    uint32_t flags, uint8_t *d_digest, int32_t *d_err, uint64_t *d_pos, cudaStream_t st);
 int launch_least_rotation(const uint8_t *d_in, const uint64_t *d_off, uint64_t n, uint64_t max_len, uint64_t *d_rotation,
                           cudaStream_t st);
+// fold.cu: per-item device scratch of pg_fold_zuker_batch (0 for items that are not folded), the DNA and RNA
+// energy tables at temp degrees Celsius (uploaded as is), and the kernel over items [0, n)
+uint64_t fold_scratch_bytes(uint64_t len);
+std::vector<uint8_t> fold_tables(double temp);
+int launch_fold_zuker(const uint8_t *d_seqs, const uint64_t *d_off, uint64_t n, const uint8_t *d_tables, uint8_t *d_scratch,
+                      const uint64_t *d_scr_off, double *d_mfe, uint8_t *d_db, uint64_t *d_db_len, int32_t *d_status, cudaStream_t st);
 // synth.cu
 int launch_synth_reads(uint8_t *d_bases, uint64_t first_read, uint64_t n_reads, uint32_t read_len,
                        uint64_t seed, int kind, uint32_t family, cudaStream_t st);
