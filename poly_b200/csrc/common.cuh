@@ -217,32 +217,29 @@ int launch_sorted_flags(const uint32_t *d_sk, uint64_t n, int s, uint8_t *d_flag
 constexpr uint32_t INDEX_MAX_TOP_K = 1024;
 int launch_index_query(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t top_k, uint32_t min_same,
                        uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint32_t *d_n_hits, cudaStream_t st);
+// Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
+// pointers (align_core.cuh).
+struct AlignScoring;
 // sw_score.cu
-int launch_sw_score(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen,
-                    const uint8_t *d_t, uint64_t tlen, int query_is_a, const int16_t *lut_a,
-                    const int16_t *lut_b, const int64_t *table, int n_a, int n_b, int64_t gap,
-                    int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st, int global = 0);
+int launch_sw_score(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen, const uint8_t *d_t, uint64_t tlen,
+                    int query_is_a, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st);
 // sw_align.cu (score + aligned strings; queries <= 64 symbols, 32-bit scores)
-int launch_sw_align(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen,
-                    const uint8_t *d_t, uint64_t tlen, int query_is_a, const int16_t *lut_a,
-                    const int16_t *lut_b, const int64_t *table, int n_a, int n_b, int64_t gap,
-                    int64_t *d_score, int32_t *d_err, int64_t *d_errpos, uint8_t *d_align_a,
-                    uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status,
-                    cudaStream_t st, int global = 0);
+int launch_sw_align(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen, const uint8_t *d_t, uint64_t tlen,
+                    int query_is_a, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos, uint8_t *d_align_a,
+                    uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status, cudaStream_t st);
 // sw_align_long.cu (both strings longer than 64 symbols: full matrix in HBM).  With d_toff, item k
 // aligns query d_pq[k] against template d_pt[k] of the ragged set (d_t, d_toff) and tlen is the
 // longest template; without it every query meets the one template d_t[0, tlen).
 int launch_sw_align_long(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen, const uint8_t *d_t,
-                         uint64_t tlen, int query_is_a, const int16_t *lut_a, const int16_t *lut_b, const int64_t *table,
-                         int n_a, int n_b, int64_t gap, const int64_t *d_score, const int32_t *d_err, uint8_t *d_align_a,
-                         uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status, cudaStream_t st,
-                         int global, const uint64_t *d_toff = nullptr, const uint32_t *d_pq = nullptr,
+                         uint64_t tlen, int query_is_a, const AlignScoring &s, const int64_t *d_score, const int32_t *d_err,
+                         uint8_t *d_align_a, uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status,
+                         cudaStream_t st, const uint64_t *d_toff = nullptr, const uint32_t *d_pq = nullptr,
                          const uint32_t *d_pt = nullptr);
 // sw_pairs.cu: scores of n_pairs (A[d_pa[k]], B[d_pb[k]]) pairs; only enqueues work on st
 int launch_sw_score_pairs(const uint8_t *d_a, const uint64_t *d_aoff, uint64_t na, uint64_t max_la, const uint8_t *d_b,
                           const uint64_t *d_boff, uint64_t nb, uint64_t max_lb, const uint32_t *d_pa, const uint32_t *d_pb,
-                          uint64_t n_pairs, const int16_t *lut_a, const int16_t *lut_b, const int64_t *table, int n_a, int n_b,
-                          int64_t gap, int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st, int global);
+                          uint64_t n_pairs, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos,
+                          cudaStream_t st);
 // tm.cu
 int launch_tm(const uint8_t *d_bases, const uint64_t *d_off, uint64_t n, double cp, double na,
               double mg, double *d_tm, double *d_dh, double *d_ds, int32_t *d_status,

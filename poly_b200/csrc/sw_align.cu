@@ -15,10 +15,9 @@
 // A path that leaves the W-column window is reported (status 2) and the host re-runs that query
 // with W = template length.
 #include <algorithm>
-#include <cstring>
 #include <vector>
 
-#include "common.cuh"
+#include "align_core.cuh"
 
 namespace pg {
 
@@ -107,9 +106,7 @@ sw_align_kernel(AlignParams p, const int16_t *__restrict__ lut_q, const int16_t 
                 for (int i = 0; i < ROWS; ++i) {
                     if (i < (int)qlen) {
                         const int old = col[i];
-                        int v = __viaddmax_s32(diag, s_tab[qrow[i] + tj], 0);
-                        v = __viaddmax_s32(old, gap, v);
-                        v = __viaddmax_s32(up, gap, v);
+                        const int v = sw_cell<int, false>(diag, s_tab[qrow[i] + tj], old, up, gap);
                         if (v == B) {
                             const uint32_t cq = i + 1, ct = (uint32_t)(t0 + j) + 1;
                             // stringA outer: query_is_a -> (query, template) lexicographic, else (template, query)
@@ -153,15 +150,7 @@ sw_align_kernel(AlignParams p, const int16_t *__restrict__ lut_q, const int16_t 
                 for (int i = 0; i < ROWS; ++i) {
                     if (i < (int)qlen) {
                         const int old = col[i];
-                        int v;
-                        if (GLOBAL) {
-                            v = __viaddmax_s32(diag, s_tab[qrow[i] + tj], old + gap);  // align.go:132-135
-                            v = __viaddmax_s32(up, gap, v);
-                        } else {
-                            v = __viaddmax_s32(diag, s_tab[qrow[i] + tj], 0);
-                            v = __viaddmax_s32(old, gap, v);
-                            v = __viaddmax_s32(up, gap, v);
-                        }
+                        const int v = sw_cell<int, GLOBAL>(diag, s_tab[qrow[i] + tj], old, up, gap);
                         if (keep) slot[(uint64_t)i * p.n] = v;
                         diag = old;
                         up = v;
@@ -193,6 +182,7 @@ sw_align_kernel(AlignParams p, const int16_t *__restrict__ lut_q, const int16_t 
         const int h_left = p.query_is_a ? H(cq, ct - 1, outside) : H(cq - 1, ct, outside);
         if (outside) break;
         uint8_t ca, cb;
+        // trace_step's choice, written out: calling trace_step and trace_finish changes this kernel's machine code
         if (h == hd + sc) {                 // align.go:215-219
             ca = p.query_is_a ? qc : tc_;
             cb = p.query_is_a ? tc_ : qc;
@@ -208,17 +198,15 @@ sw_align_kernel(AlignParams p, const int16_t *__restrict__ lut_q, const int16_t 
         } else {
             break;  // unreachable for a max of the three (the reference would not terminate)
         }
-        if (len < p.out_stride) { oa[len] = ca; ob[len] = cb; }
-        else overflow = true;
-        ++len;
+        trace_put(oa, ob, p.out_stride, ca, cb, len, overflow);
         h = H(cq, ct, outside);
     }
     if (outside) {
         status[qi] = 2;  // window too small: host retries with W = template length
         return;
     }
-    const uint32_t n_written = min(len, (uint32_t)p.out_stride);
-    for (uint32_t x = 0; x < n_written / 2; ++x) {  // built by prepending == reversed
+    const uint32_t n_written = min(len, (uint32_t)p.out_stride);  // trace_finish, written out as above
+    for (uint32_t x = 0; x < n_written / 2; ++x) {
         uint8_t t1 = oa[x]; oa[x] = oa[n_written - 1 - x]; oa[n_written - 1 - x] = t1;
         t1 = ob[x]; ob[x] = ob[n_written - 1 - x]; ob[n_written - 1 - x] = t1;
     }
@@ -227,87 +215,67 @@ sw_align_kernel(AlignParams p, const int16_t *__restrict__ lut_q, const int16_t 
 }
 
 template <int ROWS, bool GLOBAL>
-int run_align(AlignParams p, const int16_t *d_lut_q, const int16_t *d_lut_t, const int *d_tab, const int64_t *d_score,
-              const int32_t *d_err, uint8_t *d_a, uint8_t *d_b, uint32_t *d_len, int32_t *d_status, cudaStream_t st) {
+int run_align(const AlignParams &p, const AlignTables<int> &d, const int64_t *d_score, const int32_t *d_err, uint8_t *d_a,
+              uint8_t *d_b, uint32_t *d_len, int32_t *d_status, cudaStream_t st) {
     if (p.n == 0) return PG_OK;
+    StreamScratch tmp(st);
     int *d_ring = nullptr;
-    PG_CUDA(cudaMallocAsync(&d_ring, (size_t)p.W * ROWS * p.n * sizeof(int), st));
+    PG_CUDA(tmp.alloc(&d_ring, (size_t)p.W * ROWS * p.n));
     const size_t smem = AL_TCHUNK + 512 + (size_t)p.n_q * p.n_t * sizeof(int);
-    PG_CUDA(cudaFuncSetAttribute(sw_align_kernel<ROWS, GLOBAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sw_align_kernel<ROWS, GLOBAL><<<(unsigned)((p.n + AL_THREADS - 1) / AL_THREADS), AL_THREADS, smem, st>>>(
-        p, d_lut_q, d_lut_t, d_tab, d_score, d_err, d_ring, d_a, d_b, d_len, d_status);
-    note_launch(GLOBAL ? "nw_align_kernel" : "sw_align_kernel");
-    cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(d_ring, st);
-    if (e != cudaSuccess) return cuda_fail(e, "sw_align_kernel", __FILE__, __LINE__);
-    return PG_OK;
+    return launch_smem(sw_align_kernel<ROWS, GLOBAL>, (unsigned)((p.n + AL_THREADS - 1) / AL_THREADS), AL_THREADS, smem, st,
+                       GLOBAL ? "nw_align_kernel" : "sw_align_kernel", p, d.lut_row, d.lut_col, d.tab, d_score, d_err, d_ring, d_a,
+                       d_b, d_len, d_status);
 }
 
 }  // namespace
 
 // Device-resident driver: scores (K4) first, then the traceback kernel in batches; queries whose
 // path leaves the default window are re-run with a full-length window.
-int launch_sw_align(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen,
-                    const uint8_t *d_t, uint64_t tlen, int query_is_a, const int16_t *lut_a,
-                    const int16_t *lut_b, const int64_t *table, int n_a, int n_b, int64_t gap,
-                    int64_t *d_score, int32_t *d_err, int64_t *d_errpos, uint8_t *d_align_a,
-                    uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status,
-                    cudaStream_t st, int global) {
+int launch_sw_align(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen, const uint8_t *d_t, uint64_t tlen,
+                    int query_is_a, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos, uint8_t *d_align_a,
+                    uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status, cudaStream_t st) {
     if (nq == 0) return PG_OK;
     if (max_qlen > 64) {  // both strings may be long: whole matrix in HBM, literal traceback (sw_align_long.cu)
-        int rc = launch_sw_score(d_q, d_qoff, nq, max_qlen, d_t, tlen, query_is_a, lut_a, lut_b, table, n_a, n_b, gap,
-                                 d_score, d_err, d_errpos, st, global);
+        int rc = launch_sw_score(d_q, d_qoff, nq, max_qlen, d_t, tlen, query_is_a, s, d_score, d_err, d_errpos, st);
         if (rc != PG_OK) return rc;
-        return launch_sw_align_long(d_q, d_qoff, nq, max_qlen, d_t, tlen, query_is_a, lut_a, lut_b, table, n_a, n_b, gap, d_score,
-                                    d_err, d_align_a, d_align_b, out_stride, d_len, d_status, st, global);
+        return launch_sw_align_long(d_q, d_qoff, nq, max_qlen, d_t, tlen, query_is_a, s, d_score, d_err, d_align_a, d_align_b,
+                                    out_stride, d_len, d_status, st);
     }
-    int64_t amax = 0;
-    for (int i = 0; i < n_a * n_b; ++i) amax = std::max<int64_t>(amax, table[i] < 0 ? -table[i] : table[i]);
-    const int64_t agap = gap < 0 ? -gap : gap;
-    if ((global ? (long double)std::max(amax, agap) * (long double)(tlen + 66) : (long double)amax * 64 + (long double)std::max(amax, agap)) >= 2.0e9L) {
+    if (score_bound(s.global, s.abs_max(), s.abs_gap(), 64, 64 + tlen) >= SCORE32_LIMIT) {
         set_error("aligned strings need scores that fit 32 bits");
         return PG_ERR_UNSUPPORTED;
     }
-    int rc = launch_sw_score(d_q, d_qoff, nq, max_qlen, d_t, tlen, query_is_a, lut_a, lut_b, table, n_a, n_b, gap,
-                             d_score, d_err, d_errpos, st, global);
+    int rc = launch_sw_score(d_q, d_qoff, nq, max_qlen, d_t, tlen, query_is_a, s, d_score, d_err, d_errpos, st);
     if (rc != PG_OK) return rc;
 
     AlignParams p;
     p.q = d_q; p.qoff = d_qoff; p.qlist = nullptr; p.t = d_t; p.tlen = tlen; p.query_is_a = query_is_a;
-    p.n_q = query_is_a ? n_a : n_b;
-    p.n_t = query_is_a ? n_b : n_a;
-    p.gap = (int)gap;
-    p.global = global;
+    p.n_q = query_is_a ? s.n_a : s.n_b;
+    p.n_t = query_is_a ? s.n_b : s.n_a;
+    p.gap = (int)s.gap;
+    p.global = s.global;
     p.out_stride = out_stride;
-    const int16_t *lut_q = query_is_a ? lut_a : lut_b, *lut_t = query_is_a ? lut_b : lut_a;
-    std::vector<uint8_t> blob(1024 + (size_t)p.n_q * p.n_t * sizeof(int));
-    memcpy(blob.data(), lut_q, 512);
-    memcpy(blob.data() + 512, lut_t, 512);
-    int *ht = reinterpret_cast<int *>(blob.data() + 1024);
-    for (int q = 0; q < p.n_q; ++q)
-        for (int t = 0; t < p.n_t; ++t)
-            ht[q * p.n_t + t] = (int)(query_is_a ? table[(size_t)q * n_b + t] : table[(size_t)t * n_b + q]);
-    uint8_t *d_blob = nullptr;
-    PG_CUDA(cudaMallocAsync(&d_blob, blob.size(), st));
-    PG_CUDA(cudaMemcpyAsync(d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaStreamSynchronize(st));
-    const int16_t *d_lut_q = reinterpret_cast<const int16_t *>(d_blob), *d_lut_t = d_lut_q + 256;
-    const int *d_tab = reinterpret_cast<const int *>(d_blob + 1024);
+    StreamScratch tmp(st);
+    AlignTables<int> d;  // the query symbol on the table's rows
+    if ((rc = upload_tables<int>(s, {query_is_a != 0}, false, tmp, st, &d)) != PG_OK) return rc;
 
     const int rows = max_qlen <= 32 ? 32 : 64;
+    auto run = [&]() {
+        return s.global ? (rows == 32 ? run_align<32, true>(p, d, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st)
+                                      : run_align<64, true>(p, d, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st))
+                        : (rows == 32 ? run_align<32, false>(p, d, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st)
+                                      : run_align<64, false>(p, d, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st));
+    };
     // NW walks the whole matrix: keep every column
-    const uint32_t W0 = global ? (uint32_t)std::max<uint64_t>(tlen, 1) : (uint32_t)std::min<uint64_t>(std::max<uint64_t>(tlen, 1), 2 * rows + 32);
+    const uint32_t W0 = s.global ? (uint32_t)std::max<uint64_t>(tlen, 1) : (uint32_t)std::min<uint64_t>(std::max<uint64_t>(tlen, 1), 2 * rows + 32);
     // batches bounded by ~1 GiB of ring
     const uint64_t per = std::max<uint64_t>(1, ((1ull << 30) / ((uint64_t)W0 * rows * 4)));
     for (uint64_t q0 = 0; q0 < nq && rc == PG_OK; q0 += per) {
         p.q_first = q0; p.n = std::min<uint64_t>(per, nq - q0); p.W = W0;
-        rc = global ? (rows == 32 ? run_align<32, true>(p, d_lut_q, d_lut_t, d_tab, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st)
-                                  : run_align<64, true>(p, d_lut_q, d_lut_t, d_tab, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st))
-                    : (rows == 32 ? run_align<32, false>(p, d_lut_q, d_lut_t, d_tab, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st)
-                                  : run_align<64, false>(p, d_lut_q, d_lut_t, d_tab, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st));
+        rc = run();
     }
     // retries with a full-length window (rare: long gap runs)
-    if (rc == PG_OK && !global && W0 < tlen) {
+    if (rc == PG_OK && !s.global && W0 < tlen) {
         std::vector<int32_t> hst(nq);
         PG_CUDA(cudaMemcpyAsync(hst.data(), d_status, nq * 4, cudaMemcpyDeviceToHost, st));
         PG_CUDA(cudaStreamSynchronize(st));
@@ -316,19 +284,15 @@ int launch_sw_align(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uin
             if (hst[i] == 2) redo.push_back((uint32_t)i);
         if (!redo.empty()) {
             uint32_t *d_list = nullptr;
-            PG_CUDA(cudaMallocAsync(&d_list, redo.size() * 4, st));
+            PG_CUDA(tmp.alloc(&d_list, redo.size()));
             PG_CUDA(cudaMemcpyAsync(d_list, redo.data(), redo.size() * 4, cudaMemcpyHostToDevice, st));
             const uint64_t per2 = std::max<uint64_t>(1, (1ull << 30) / (tlen * rows * 4));
             for (uint64_t r0 = 0; r0 < redo.size() && rc == PG_OK; r0 += per2) {
                 p.qlist = d_list + r0; p.q_first = 0; p.n = std::min<uint64_t>(per2, redo.size() - r0); p.W = (uint32_t)tlen;
-                rc = rows == 32 ? run_align<32, false>(p, d_lut_q, d_lut_t, d_tab, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st)
-                                : run_align<64, false>(p, d_lut_q, d_lut_t, d_tab, d_score, d_err, d_align_a, d_align_b, d_len, d_status, st);
+                rc = run();
             }
-            PG_CUDA(cudaStreamSynchronize(st));
-            cudaFreeAsync(d_list, st);
         }
     }
-    cudaFreeAsync(d_blob, st);
     return rc;
 }
 

@@ -10,10 +10,8 @@
 //          reversed and flips them.
 // Generality path (memory-bound on the matrix, 4 bytes per cell); scores must fit 32 bits.
 #include <algorithm>
-#include <cstring>
-#include <vector>
 
-#include "common.cuh"
+#include "align_core.cuh"
 
 namespace pg {
 
@@ -69,11 +67,8 @@ align_long_kernel(LongParams p, const int16_t *__restrict__ lut_a, const int16_t
             const uint64_t j = d - i;
             const int ia = lut_a[A[i - 1]], ib = lut_b[B[j - 1]];
             const int sc = (ia < 0 || ib < 0) ? 0 : tab[ia * p.n_b + ib];  // bad symbols were reported by the score kernel
-            int v = max(M[(i - 1) * W + j - 1] + sc, max(M[(i - 1) * W + j] + gap, M[i * W + j - 1] + gap));
-            if (!GLOBAL) {
-                v = max(v, 0);                                                                           // align.go:192-196
-                if (v == best) atomicMin(&s_first, ((unsigned long long)i << 32) | (unsigned long long)j);  // align.go:197-201
-            }
+            const int v = sw_cell<int, GLOBAL>(M[(i - 1) * W + j - 1], sc, M[i * W + j - 1], M[(i - 1) * W + j], gap);
+            if (!GLOBAL && v == best) atomicMin(&s_first, ((unsigned long long)i << 32) | (unsigned long long)j);  // align.go:197-201
             M[i * W + j] = v;
         }
         __syncthreads();
@@ -87,38 +82,24 @@ align_long_kernel(LongParams p, const int16_t *__restrict__ lut_a, const int16_t
     while (GLOBAL ? (i > 0 && j > 0) : M[i * W + j] > 0) {
         const int ia = lut_a[A[i - 1]], ib = lut_b[B[j - 1]];
         const int sc = (ia < 0 || ib < 0) ? 0 : tab[ia * p.n_b + ib];
-        const int h = M[i * W + j];
-        uint8_t ca, cb;
-        if (h == M[(i - 1) * W + j - 1] + sc) { ca = A[i - 1]; cb = B[j - 1]; --i; --j; }   // align.go:146-150 / 215-219
-        else if (h == M[(i - 1) * W + j] + gap) { ca = A[i - 1]; cb = '-'; --i; }           // align.go:151-154 / 220-223
-        else if (GLOBAL || h == M[i * W + j - 1] + gap) { ca = '-'; cb = B[j - 1]; --j; }   // align.go:155-159 / 224-228
-        else break;  // unreachable for a max of the three
-        if (len < p.out_stride) { oa[len] = ca; ob[len] = cb; }
-        else overflow = true;
-        ++len;
+        const TraceStep step = trace_step<GLOBAL>(M[i * W + j], M[(i - 1) * W + j - 1], M[(i - 1) * W + j], M[i * W + j - 1], sc, gap);
+        if (step == STEP_DIAG) { trace_put(oa, ob, p.out_stride, A[i - 1], B[j - 1], len, overflow); --i; --j; }
+        else if (step == STEP_UP) { trace_put(oa, ob, p.out_stride, A[i - 1], '-', len, overflow); --i; }
+        else if (step == STEP_LEFT) { trace_put(oa, ob, p.out_stride, '-', B[j - 1], len, overflow); --j; }
+        else break;
     }
-    const uint32_t n_written = min(len, (uint32_t)p.out_stride);
-    for (uint32_t x = 0; x < n_written / 2; ++x) {  // built by prepending / reversed at the end
-        uint8_t t1 = oa[x]; oa[x] = oa[n_written - 1 - x]; oa[n_written - 1 - x] = t1;
-        t1 = ob[x]; ob[x] = ob[n_written - 1 - x]; ob[n_written - 1 - x] = t1;
-    }
-    out_len[qi] = len;
-    status[qi] = overflow ? PG_ITEM_UNSUPPORTED : PG_ITEM_OK;
+    trace_finish(oa, ob, p.out_stride, len, overflow, out_len, status, qi);
 }
 
 }  // namespace
 
 // scores (and the reference's first error) come from launch_sw_score; this adds the strings
 int launch_sw_align_long(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen, const uint8_t *d_t,
-                         uint64_t tlen, int query_is_a, const int16_t *lut_a, const int16_t *lut_b, const int64_t *table,
-                         int n_a, int n_b, int64_t gap, const int64_t *d_score, const int32_t *d_err, uint8_t *d_align_a,
-                         uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status, cudaStream_t st,
-                         int global, const uint64_t *d_toff, const uint32_t *d_pq, const uint32_t *d_pt) {
+                         uint64_t tlen, int query_is_a, const AlignScoring &s, const int64_t *d_score, const int32_t *d_err,
+                         uint8_t *d_align_a, uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status,
+                         cudaStream_t st, const uint64_t *d_toff, const uint32_t *d_pq, const uint32_t *d_pt) {
     if (nq == 0) return PG_OK;
-    int64_t amax = 0;
-    for (int i = 0; i < n_a * n_b; ++i) amax = std::max<int64_t>(amax, table[i] < 0 ? -table[i] : table[i]);
-    const int64_t agap = gap < 0 ? -gap : gap;
-    if ((long double)std::max(amax, agap) * (long double)(max_qlen + tlen + 2) >= 2.0e9L) {
+    if (score_bound(1, s.abs_max(), s.abs_gap(), 0, max_qlen + tlen) >= SCORE32_LIMIT) {  // the NW bound for SW too
         set_error("aligned strings need scores that fit 32 bits");
         return PG_ERR_UNSUPPORTED;
     }
@@ -127,32 +108,22 @@ int launch_sw_align_long(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq
         set_error("alignment matrix of %llu x %llu cells does not fit", (unsigned long long)max_qlen, (unsigned long long)tlen);
         return PG_ERR_UNSUPPORTED;
     }
-    std::vector<uint8_t> blob(1024 + (size_t)n_a * n_b * sizeof(int));
-    memcpy(blob.data(), lut_a, 512);
-    memcpy(blob.data() + 512, lut_b, 512);
-    int *ht = reinterpret_cast<int *>(blob.data() + 1024);
-    for (int i = 0; i < n_a * n_b; ++i) ht[i] = (int)table[i];
     StreamScratch tmp(st);
-    uint8_t *d_blob = nullptr;
-    PG_CUDA(tmp.alloc(&d_blob, blob.size()));
-    PG_CUDA(cudaMemcpyAsync(d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaStreamSynchronize(st));  // blob is a local
+    AlignTables<int> d;  // a's symbol on the table's rows
+    int rc = upload_tables<int>(s, {true}, false, tmp, st, &d);
+    if (rc != PG_OK) return rc;
     const uint64_t per = std::max<uint64_t>(1, std::min<uint64_t>((512ull << 20) / cells, 65535));  // <= 2 GiB of matrices per launch
     int *d_m = nullptr;
     PG_CUDA(tmp.alloc(&d_m, std::min(per, nq) * cells));
     LongParams p;
-    p.q = d_q; p.qoff = d_qoff; p.t = d_t; p.tlen = tlen; p.query_is_a = query_is_a; p.n_b = n_b; p.gap = (int)gap;
+    p.q = d_q; p.qoff = d_qoff; p.t = d_t; p.tlen = tlen; p.query_is_a = query_is_a; p.n_b = s.n_b; p.gap = (int)s.gap;
     p.out_stride = out_stride; p.cells_per_pair = cells;
     p.toff = d_toff; p.pq = d_pq; p.pt = d_pt;
     for (uint64_t q0 = 0; q0 < nq; q0 += per) {
         p.q_first = q0;
         p.n = std::min(per, nq - q0);
-        if (global)
-            align_long_kernel<true><<<(unsigned)p.n, ALL_THREADS, 0, st>>>(p, (const int16_t *)d_blob, (const int16_t *)(d_blob + 512), (const int *)(d_blob + 1024),
-                                                                          d_score, d_err, d_m, d_align_a, d_align_b, d_len, d_status);
-        else
-            align_long_kernel<false><<<(unsigned)p.n, ALL_THREADS, 0, st>>>(p, (const int16_t *)d_blob, (const int16_t *)(d_blob + 512), (const int *)(d_blob + 1024),
-                                                                           d_score, d_err, d_m, d_align_a, d_align_b, d_len, d_status);
+        (s.global ? align_long_kernel<true> : align_long_kernel<false>)<<<(unsigned)p.n, ALL_THREADS, 0, st>>>(
+            p, d.lut_row, d.lut_col, d.tab, d_score, d_err, d_m, d_align_a, d_align_b, d_len, d_status);
         PG_LAUNCH_CHECK("align_long_kernel");
     }
     return PG_OK;

@@ -16,11 +16,9 @@
 // biggest-first by log2(cells); the long kernel takes them from an atomic work counter.  No host
 // round trip, so the _dev entry points only enqueue work.
 #include <algorithm>
-#include <cstring>
 #include <type_traits>
-#include <vector>
 
-#include "common.cuh"
+#include "align_core.cuh"
 
 namespace pg {
 
@@ -36,21 +34,6 @@ constexpr int RING = 64;
 
 __host__ __device__ constexpr int short_rows(int c) { return c == 0 ? 1 : c == 1 ? 2 : c == 2 ? 4 : c == 3 ? 5 : 8; }
 
-template <typename T>
-struct Big {
-    static constexpr T value = (T)1 << (sizeof(T) * 8 - 3);
-};
-
-template <typename T>
-__device__ __forceinline__ T addmax(T a, T b, T c) {  // max(a + b, c)
-    const T x = a + b;
-    return x > c ? x : c;
-}
-template <>
-__device__ __forceinline__ int addmax<int>(int a, int b, int c) {
-    return __viaddmax_s32(a, b, c);
-}
-
 struct PairParams {
     const uint8_t *a;
     const uint64_t *aoff;
@@ -65,7 +48,7 @@ struct PairParams {
 };
 
 // Device parameter block: the two byte LUTs, then the table twice: [n_a + 1][n_b] (rows = a) and
-// [n_b + 1][n_a] (rows = b), each with a last row of -Big for rows beyond the shorter string.
+// [n_b + 1][n_a] (rows = b), each with a last row of NegBig for rows beyond the shorter string.
 template <typename T>
 struct Blob {
     const int16_t *lut_a, *lut_b;
@@ -121,11 +104,8 @@ pair_classify_kernel(PairParams p, const int16_t *__restrict__ g_lut_a, const in
             if (la > p.max_la || lb > p.max_lb) {
                 ec = PG_PAIR_OUT_OF_RANGE;
             } else if (la > 0 && lb > 0) {
-                // first failing cell in row-major order, stringA outer (align.go:186-191); Encode(a) before Encode(b)
                 const int64_t bad_a = warp_first_bad(p.a + a0, la, lut_a), bad_b = warp_first_bad(p.b + b0, lb, lut_b);
-                if (bad_a == 0) { ec = 1; ep = 0; }
-                else if (bad_b >= 0) { ec = 2; ep = bad_b; }
-                else if (bad_a > 0) { ec = 1; ep = bad_a; }
+                first_error(bad_a, bad_b, ec, ep);
                 if (!ec) c = (uint8_t)class_of(min(la, lb), la * lb, p.min_class);
             } else if (global) {
                 sc = (int64_t)(la + lb) * gap;  // a pure gap ramp (align.go:115-122,166)
@@ -168,7 +148,7 @@ struct PairView {
     const uint8_t *S, *L;
     uint32_t m, n;
     const int16_t *lut_row, *lut_col;
-    const T *tab;  // [rows: S symbol or the -Big row][n_col]
+    const T *tab;  // [rows: S symbol or the NegBig row][n_col]
     int n_row, n_col;
 };
 
@@ -243,17 +223,8 @@ __device__ __forceinline__ void sweep(const PairView<T> &v, uint32_t row0, T gap
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 const T old = H[r];  // H[i][j-1]
-                const T sc = v.tab[rowoff[r] + cv];
-                T x;
-                if (GLOBAL) {
-                    x = addmax<T>(diag, sc, old + gap);  // align.go:132-135
-                    x = addmax<T>(up, gap, x);
-                } else {
-                    x = addmax<T>(diag, sc, (T)0);       // align.go:192-196
-                    x = addmax<T>(old, gap, x);
-                    x = addmax<T>(up, gap, x);
-                    if (!MASK || r < nvalid) best = x > best ? x : best;  // align.go:197-201
-                }
+                const T x = sw_cell<T, GLOBAL>(diag, v.tab[rowoff[r] + cv], old, up, gap);
+                if (!GLOBAL && (!MASK || r < nvalid)) best = x > best ? x : best;  // align.go:197-201
                 diag = old;
                 up = x;
                 H[r] = x;
@@ -365,39 +336,28 @@ pair_long_kernel(PairParams p, Blob<T> g, bool smem_tab, T gap, Ctl *__restrict_
 }
 
 template <typename T>
-int run_pairs(const PairParams &p0, const int16_t *lut_a, const int16_t *lut_b, const int64_t *table, int64_t gap, int global,
-              int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st) {
+int run_pairs(const PairParams &p0, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st) {
     PairParams p = p0;
     p.min_class = sizeof(T) == 4 ? 0 : N_SHORT - 1;
-    const int n_a = p.n_a, n_b = p.n_b;
-    const size_t nab = (size_t)(n_a + 1) * n_b, nba = (size_t)(n_b + 1) * n_a;
-    // parameter block: LUTs, the table with a rows and with b rows; built here and copied from pageable
-    // memory, which the driver stages before cudaMemcpyAsync returns
-    std::vector<uint8_t> blob(1024 + (nab + nba) * sizeof(T));
-    memcpy(blob.data(), lut_a, 512);
-    memcpy(blob.data() + 512, lut_b, 512);
-    T *tab_ab = reinterpret_cast<T *>(blob.data() + 1024), *tab_ba = tab_ab + nab;
-    const T NEG = (T)0 - Big<T>::value;
-    for (int i = 0; i <= n_a; ++i)
-        for (int j = 0; j < n_b; ++j) tab_ab[(size_t)i * n_b + j] = i < n_a ? (T)table[(size_t)i * n_b + j] : NEG;
-    for (int j = 0; j <= n_b; ++j)
-        for (int i = 0; i < n_a; ++i) tab_ba[(size_t)j * n_a + i] = j < n_b ? (T)table[(size_t)i * n_b + j] : NEG;
-
+    const int64_t gap = s.gap;
+    const int global = s.global;
+    const size_t nab = (size_t)(s.n_a + 1) * s.n_b, nba = (size_t)(s.n_b + 1) * s.n_a;
     StreamScratch tmp(st);
-    uint8_t *d_blob = nullptr, *d_cls = nullptr;
+    AlignTables<T> d;  // the LUTs, then the table with a rows and with b rows
+    int rc = upload_tables<T>(s, {true, false}, true, tmp, st, &d);
+    if (rc != PG_OK) return rc;
+    uint8_t *d_cls = nullptr;
     Ctl *d_ctl = nullptr;
     uint32_t *d_list = nullptr;
-    PG_CUDA(tmp.alloc(&d_blob, blob.size()));
     PG_CUDA(tmp.alloc(&d_ctl, 1));
     PG_CUDA(tmp.alloc(&d_cls, p.n));
     PG_CUDA(tmp.alloc(&d_list, p.n));
-    PG_CUDA(cudaMemcpyAsync(d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
     PG_CUDA(cudaMemsetAsync(d_ctl, 0, sizeof(Ctl), st));
     Blob<T> g;
-    g.lut_a = reinterpret_cast<const int16_t *>(d_blob);
-    g.lut_b = g.lut_a + 256;
-    g.tab_ab = reinterpret_cast<const T *>(d_blob + 1024);
-    g.tab_ba = g.tab_ab + nab;
+    g.lut_a = d.lut_row;
+    g.lut_b = d.lut_col;
+    g.tab_ab = d.tab;
+    g.tab_ba = d.tab + nab;
     const size_t tab_bytes = (nab + nba) * sizeof(T);
     const bool smem_tab = tab_bytes <= 48 * 1024;
     const size_t smem = smem_tab ? tab_bytes : 0;
@@ -433,7 +393,6 @@ int run_pairs(const PairParams &p0, const int16_t *lut_a, const int16_t *lut_b, 
         return PG_OK;
         }
     };
-    int rc;
     if ((rc = launch_short(std::integral_constant<int, 1>{}, 0)) != PG_OK) return rc;
     if ((rc = launch_short(std::integral_constant<int, 2>{}, 1)) != PG_OK) return rc;
     if ((rc = launch_short(std::integral_constant<int, 4>{}, 2)) != PG_OK) return rc;
@@ -474,12 +433,10 @@ int run_pairs(const PairParams &p0, const int16_t *lut_a, const int16_t *lut_b, 
 
 int launch_sw_score_pairs(const uint8_t *d_a, const uint64_t *d_aoff, uint64_t na, uint64_t max_la, const uint8_t *d_b,
                           const uint64_t *d_boff, uint64_t nb, uint64_t max_lb, const uint32_t *d_pa, const uint32_t *d_pb,
-                          uint64_t n_pairs, const int16_t *lut_a, const int16_t *lut_b, const int64_t *table, int n_a, int n_b,
-                          int64_t gap, int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st, int global) {
-    if (n_a <= 0 || n_b <= 0 || n_a > 255 || n_b > 255) {
-        set_error("alphabet sizes must be in 1..255 (got %d, %d)", n_a, n_b);
-        return PG_ERR_ARG;
-    }
+                          uint64_t n_pairs, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos,
+                          cudaStream_t st) {
+    int rc = s.check();
+    if (rc != PG_OK) return rc;
     if (n_pairs == 0) return PG_OK;
     if (n_pairs > 0xffffffffull || max_la > 0xffffffffull || max_lb > 0xffffffffull) {
         set_error("pair lists are limited to 2^32 - 1 pairs and sequences to 2^32 - 1 symbols");
@@ -488,15 +445,11 @@ int launch_sw_score_pairs(const uint8_t *d_a, const uint64_t *d_aoff, uint64_t n
     PairParams p;
     p.a = d_a; p.aoff = d_aoff; p.na = na; p.max_la = max_la;
     p.b = d_b; p.boff = d_boff; p.nb = nb; p.max_lb = max_lb;
-    p.pa = d_pa; p.pb = d_pb; p.n = n_pairs; p.n_a = n_a; p.n_b = n_b; p.min_class = 0;
-    int64_t amax = 0;
-    for (int i = 0; i < n_a * n_b; ++i) amax = std::max<int64_t>(amax, table[i] < 0 ? -table[i] : table[i]);
-    const int64_t agap = gap < 0 ? -gap : gap;
-    // the score-width rule of launch_sw_score with the longest a and b of the call
-    const long double bound = global ? (long double)std::max(amax, agap) * (long double)(max_la + max_lb + 2)
-                                     : (long double)amax * (long double)std::min(max_la, max_lb) + (long double)std::max(amax, agap);
-    if (bound < 2.0e9L) return run_pairs<int>(p, lut_a, lut_b, table, gap, global, d_score, d_err, d_errpos, st);
-    return run_pairs<long long>(p, lut_a, lut_b, table, gap, global, d_score, d_err, d_errpos, st);
+    p.pa = d_pa; p.pb = d_pb; p.n = n_pairs; p.n_a = s.n_a; p.n_b = s.n_b; p.min_class = 0;
+    // the longest a and b of the call
+    if (score_bound(s.global, s.abs_max(), s.abs_gap(), std::min(max_la, max_lb), max_la + max_lb) < SCORE32_LIMIT)
+        return run_pairs<int>(p, s, d_score, d_err, d_errpos, st);
+    return run_pairs<long long>(p, s, d_score, d_err, d_errpos, st);
 }
 
 }  // namespace pg

@@ -13,13 +13,9 @@
 // the outer loop; the reported error (first failing cell in row-major order,
 // align.go:188-191) does, and is resolved per orientation at the end.
 #include <algorithm>
-#include <cstdlib>
-#include <cstring>
-#include <limits>
 #include <type_traits>
-#include <vector>
 
-#include "common.cuh"
+#include "align_core.cuh"
 
 namespace pg {
 
@@ -27,16 +23,6 @@ namespace {
 
 constexpr int SW_THREADS = 128;
 constexpr int SW_TCHUNK = 8192;  // template symbols staged per pass
-
-template <typename T>
-__device__ __forceinline__ T addmax(T a, T b, T c) {  // max(a + b, c)
-    const T x = a + b;
-    return x > c ? x : c;
-}
-template <>
-__device__ __forceinline__ int addmax<int>(int a, int b, int c) {
-    return __viaddmax_s32(a, b, c);
-}
 
 struct SwParams {
     const uint8_t *q;
@@ -56,10 +42,6 @@ struct SwParams {
 // shared memory ([n_t][ROWS][threads], conflict-free, immediate offsets) so a cell is
 // 1 LDS + 3 add-max + 1 max; otherwise (large alphabets) the score comes from the shared
 // table through a per-row offset.
-template <typename T>
-struct SwBig {
-    static constexpr T value = (T)1 << (sizeof(T) * 8 - 3);  // 2^29 / 2^61: no overflow in diag + sc
-};
 
 template <typename T, int ROWS, bool PROFILE, bool MASK, bool GLOBAL>
 __global__ void __launch_bounds__(SW_THREADS)
@@ -75,9 +57,8 @@ sw_score_kernel(SwParams p, const int16_t *__restrict__ lut_q, const int16_t *__
     __shared__ unsigned long long s_first_bad_t;
 
     const uint32_t tid = threadIdx.x;
-    const T NEG = (T)0 - SwBig<T>::value;
     for (int i = tid; i < p.n_q * p.n_t; i += SW_THREADS) s_tab[i] = tab[i];
-    for (int i = tid; i < p.n_t; i += SW_THREADS) s_tab[p.n_q * p.n_t + i] = NEG;  // row n_q: "beyond the query"
+    for (int i = tid; i < p.n_t; i += SW_THREADS) s_tab[p.n_q * p.n_t + i] = NegBig<T>::value;  // row n_q: "beyond the query"
     for (int i = tid; i < 256; i += SW_THREADS) s_lut_t[i] = lut_t[i];
     if (tid == 0) s_first_bad_t = ~0ull;
     __syncthreads();
@@ -137,14 +118,8 @@ sw_score_kernel(SwParams p, const int16_t *__restrict__ lut_q, const int16_t *__
                 for (int i = 0; i < ROWS; ++i) {
                     const T old = col[i];                                    // H[i][j-1]
                     const T sc = PROFILE ? pcol[i * SW_THREADS] : s_tab[qrow[i] + tj];  // align.go:188 / :126
-                    T v;
-                    if (GLOBAL) {
-                        v = addmax<T>(diag, sc, old + gap);                  // align.go:132-135 (no zero floor)
-                        v = addmax<T>(up, gap, v);
-                    } else {
-                        v = addmax<T>(diag, sc, (T)0);                       // align.go:192,195
-                        v = addmax<T>(old, gap, v);                          // left / up by orientation
-                        v = addmax<T>(up, gap, v);
+                    const T v = sw_cell<T, GLOBAL>(diag, sc, old, up, gap);
+                    if (!GLOBAL) {
                         if (MASK) { if (i < (int)qlen) best = v > best ? v : best; }
                         else best = v > best ? v : best;                     // align.go:197-201
                     }
@@ -167,13 +142,9 @@ sw_score_kernel(SwParams p, const int16_t *__restrict__ lut_q, const int16_t *__
     int32_t ec = 0;
     int64_t ep = -1;
     if (qlen > 0 && p.tlen > 0) {
-        // first failing cell in row-major order, stringA outer (align.go:186-191);
-        // Encode(a) is tried before Encode(b) (matrix.go:29-36)
         const int64_t bad_a = p.query_is_a ? first_bad_q : bad_t;
         const int64_t bad_b = p.query_is_a ? bad_t : first_bad_q;
-        if (bad_a == 0) { ec = 1; ep = 0; }
-        else if (bad_b >= 0) { ec = 2; ep = bad_b; }
-        else if (bad_a > 0) { ec = 1; ep = bad_a; }
+        first_error(bad_a, bad_b, ec, ep);
     }
     score[qi] = ec ? 0 : (int64_t)best;
     if (err) err[qi] = ec;
@@ -279,9 +250,7 @@ sw_score_x2_kernel(SwParams p, const int16_t *__restrict__ lut_q, const int16_t 
         if (qlen[h] > 0 && p.tlen > 0) {
             const int64_t bad_a = p.query_is_a ? first_bad_q[h] : bad_t;
             const int64_t bad_b = p.query_is_a ? bad_t : first_bad_q[h];
-            if (bad_a == 0) { ec = 1; ep = 0; }
-            else if (bad_b >= 0) { ec = 2; ep = bad_b; }
-            else if (bad_a > 0) { ec = 1; ep = bad_a; }
+            first_error(bad_a, bad_b, ec, ep);
         }
         const int b16 = (int)(int16_t)(h ? (best >> 16) : (best & 0xffffu));
         score[q0 + h] = ec ? 0 : (int64_t)b16;
@@ -320,12 +289,9 @@ sw_score_long_kernel(SwParams p, uint64_t q_first, const int16_t *__restrict__ l
             const T sc = (qx < 0 || tj < 0) ? (T)0 : tab[qx * p.n_t + tj];
             T v;
             if (p.global) {
-                v = addmax<T>(diag, sc, old + gap);
-                v = addmax<T>(up, gap, v);
+                v = sw_cell<T, true>(diag, sc, old, up, gap);
             } else {
-                v = addmax<T>(diag, sc, (T)0);
-                v = addmax<T>(old, gap, v);
-                v = addmax<T>(up, gap, v);
+                v = sw_cell<T, false>(diag, sc, old, up, gap);
                 best = v > best ? v : best;
             }
             diag = old;
@@ -339,9 +305,7 @@ sw_score_long_kernel(SwParams p, uint64_t q_first, const int16_t *__restrict__ l
     if (qlen > 0 && p.tlen > 0) {
         const int64_t bad_a = p.query_is_a ? first_bad_q : bad_t;
         const int64_t bad_b = p.query_is_a ? bad_t : first_bad_q;
-        if (bad_a == 0) { ec = 1; ep = 0; }
-        else if (bad_b >= 0) { ec = 2; ep = bad_b; }
-        else if (bad_a > 0) { ec = 1; ep = bad_a; }
+        first_error(bad_a, bad_b, ec, ep);
     }
     score[qi] = ec ? 0 : (int64_t)best;
     if (err) err[qi] = ec;
@@ -349,64 +313,43 @@ sw_score_long_kernel(SwParams p, uint64_t q_first, const int16_t *__restrict__ l
 }
 
 template <typename T>
-int run_sw(const SwParams &p, uint64_t max_qlen, const int16_t *h_lut_q, const int16_t *h_lut_t,
-           const std::vector<int64_t> &tab_qt, int64_t gap, int64_t *d_score, int32_t *d_err,
-           int64_t *d_errpos, cudaStream_t st, bool x2_ok = false) {
-    // small parameter block: LUTs + table (query symbol major)
+int run_sw(const SwParams &p, uint64_t max_qlen, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos,
+           cudaStream_t st, bool x2_ok = false) {
+    StreamScratch tmp(st);
+    AlignTables<T> d;  // the query symbol on the table's rows
+    int rc = upload_tables<T>(s, {p.query_is_a != 0}, false, tmp, st, &d);
+    if (rc != PG_OK) return rc;
+    const int64_t gap = s.gap;
     const size_t ntab = (size_t)p.n_q * p.n_t;
-    std::vector<uint8_t> blob(512 * 2 + ntab * sizeof(T));
-    memcpy(blob.data(), h_lut_q, 512);
-    memcpy(blob.data() + 512, h_lut_t, 512);
-    T *ht = reinterpret_cast<T *>(blob.data() + 1024);
-    for (size_t i = 0; i < ntab; ++i) ht[i] = (T)tab_qt[i];
-    uint8_t *d_blob = nullptr;
-    PG_CUDA(cudaMallocAsync(&d_blob, blob.size(), st));
-    PG_CUDA(cudaMemcpyAsync(d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaStreamSynchronize(st));  // blob is a stack-lifetime host buffer
-    const int16_t *d_lut_q = reinterpret_cast<const int16_t *>(d_blob);
-    const int16_t *d_lut_t = d_lut_q + 256;
-    const T *d_tab = reinterpret_cast<const T *>(d_blob + 1024);
-
     const size_t base_smem = SW_TCHUNK + 512 + (ntab + p.n_t) * sizeof(T);
     const unsigned blocks = (unsigned)((p.nq + SW_THREADS - 1) / SW_THREADS);
-    int rc = PG_OK;
     const bool mask = gap > 0;
     bool launched = false;
     // smallest instantiated row count that covers the longest query
-    auto try_rows = [&](auto rows_tag) -> bool {
+    auto try_rows = [&](auto rows_tag) {
         constexpr int ROWS = decltype(rows_tag)::value;
-        if (launched || max_qlen > (uint64_t)ROWS) return false;
+        if (launched || max_qlen > (uint64_t)ROWS) return;
         const size_t prof = (size_t)p.n_t * ROWS * SW_THREADS * sizeof(T);
         const bool profile = base_smem + prof <= 100 * 1024;
         const size_t smem = base_smem + (profile ? prof : 0);
-        if (smem > 200 * 1024) return false;
-#define PG_SW_LAUNCH(PROF, MSK, GLB)                                                                     \
-        do {                                                                                                 \
-            cudaFuncSetAttribute(sw_score_kernel<T, ROWS, PROF, MSK, GLB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            sw_score_kernel<T, ROWS, PROF, MSK, GLB><<<blocks, SW_THREADS, smem, st>>>(p, d_lut_q, d_lut_t, d_tab, (T)gap, d_score, d_err, d_errpos); \
-        } while (0)
-        if (p.global) { if (profile) PG_SW_LAUNCH(true, false, true); else PG_SW_LAUNCH(false, false, true); }
-        else if (profile && !mask) PG_SW_LAUNCH(true, false, false);
-        else if (profile && mask) PG_SW_LAUNCH(true, true, false);
-        else if (!profile && !mask) PG_SW_LAUNCH(false, false, false);
-        else PG_SW_LAUNCH(false, true, false);
-#undef PG_SW_LAUNCH
-        note_launch(p.global ? "nw_score_kernel" : "sw_score_kernel");
+        if (smem > 200 * 1024) return;
+        auto k = p.global ? (profile ? sw_score_kernel<T, ROWS, true, false, true> : sw_score_kernel<T, ROWS, false, false, true>)
+                 : profile ? (mask ? sw_score_kernel<T, ROWS, true, true, false> : sw_score_kernel<T, ROWS, true, false, false>)
+                           : (mask ? sw_score_kernel<T, ROWS, false, true, false> : sw_score_kernel<T, ROWS, false, false, false>);
+        rc = launch_smem(k, blocks, SW_THREADS, smem, st, p.global ? "nw_score_kernel" : "sw_score_kernel", p, d.lut_row, d.lut_col,
+                         d.tab, (T)gap, d_score, d_err, d_errpos);
         launched = true;
-        return true;
     };
     // packed 2 x int16 kernel: local alignment, gap <= 0, every DP value < 2^14 (checked by the caller: x2_ok)
-    auto try_x2 = [&](auto rows_tag) -> bool {
+    auto try_x2 = [&](auto rows_tag) {
         constexpr int ROWS = decltype(rows_tag)::value;
-        if (launched || max_qlen > (uint64_t)ROWS) return false;
+        if (launched || max_qlen > (uint64_t)ROWS) return;
         const size_t smem = SW_TCHUNK + 512 + ntab * sizeof(int) + (size_t)p.n_t * ROWS * SW_THREADS * sizeof(uint32_t);
-        if (smem > 100 * 1024) return false;
-        cudaFuncSetAttribute(sw_score_x2_kernel<ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        sw_score_x2_kernel<ROWS><<<(unsigned)((p.nq + 2 * SW_THREADS - 1) / (2 * SW_THREADS)), SW_THREADS, smem, st>>>(
-            p, d_lut_q, d_lut_t, reinterpret_cast<const int *>(d_tab), (int)gap, d_score, d_err, d_errpos);
-        note_launch("sw_score_x2_kernel");
+        if (smem > 100 * 1024) return;
+        rc = launch_smem(sw_score_x2_kernel<ROWS>, (unsigned)((p.nq + 2 * SW_THREADS - 1) / (2 * SW_THREADS)), SW_THREADS, smem, st,
+                         "sw_score_x2_kernel", p, d.lut_row, d.lut_col, reinterpret_cast<const int *>(d.tab), (int)gap, d_score, d_err,
+                         d_errpos);
         launched = true;
-        return true;
     };
     if (sizeof(T) == 4 && x2_ok) {
         try_x2(std::integral_constant<int, 8>{});
@@ -429,68 +372,41 @@ int run_sw(const SwParams &p, uint64_t max_qlen, const int16_t *h_lut_q, const i
         try_rows(std::integral_constant<int, 32>{});
         try_rows(std::integral_constant<int, 64>{});
     }
-    if (launched) {
-    } else {
-        // batches bounded by a 1 GiB scratch column store
-        uint64_t per = std::max<uint64_t>(1, (1ull << 30) / (std::max<uint64_t>(max_qlen, 1) * sizeof(T)));
-        per = std::min<uint64_t>(per, p.nq);
-        T *d_scr = nullptr;
-        PG_CUDA(cudaMallocAsync(&d_scr, per * std::max<uint64_t>(max_qlen, 1) * sizeof(T), st));
-        for (uint64_t q0 = 0; q0 < p.nq; q0 += per) {
-            const uint64_t nb = std::min<uint64_t>(per, p.nq - q0);
-            sw_score_long_kernel<T><<<(unsigned)((nb + SW_THREADS - 1) / SW_THREADS), SW_THREADS, 0, st>>>(
-                p, q0, d_lut_q, d_lut_t, d_tab, (T)gap, d_scr, nb, d_score, d_err, d_errpos);
-            note_launch("sw_score_long_kernel");
-        }
-        cudaFreeAsync(d_scr, st);
+    if (launched) return rc;
+    // batches bounded by a 1 GiB scratch column store
+    uint64_t per = std::max<uint64_t>(1, (1ull << 30) / (std::max<uint64_t>(max_qlen, 1) * sizeof(T)));
+    per = std::min<uint64_t>(per, p.nq);
+    T *d_scr = nullptr;
+    PG_CUDA(tmp.alloc(&d_scr, per * std::max<uint64_t>(max_qlen, 1)));
+    for (uint64_t q0 = 0; q0 < p.nq; q0 += per) {
+        const uint64_t nb = std::min<uint64_t>(per, p.nq - q0);
+        sw_score_long_kernel<T><<<(unsigned)((nb + SW_THREADS - 1) / SW_THREADS), SW_THREADS, 0, st>>>(
+            p, q0, d.lut_row, d.lut_col, d.tab, (T)gap, d_scr, nb, d_score, d_err, d_errpos);
+        PG_LAUNCH_CHECK("sw_score_long_kernel");
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = cuda_fail(e, "sw_score launch", __FILE__, __LINE__);
-    cudaFreeAsync(d_blob, st);
-    return rc;
+    return PG_OK;
 }
 
 }  // namespace
 
-int launch_sw_score(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen,
-                    const uint8_t *d_t, uint64_t tlen, int query_is_a, const int16_t *lut_a,
-                    const int16_t *lut_b, const int64_t *table, int n_a, int n_b, int64_t gap,
-                    int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st, int global) {
+int launch_sw_score(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uint64_t max_qlen, const uint8_t *d_t, uint64_t tlen,
+                    int query_is_a, const AlignScoring &s, int64_t *d_score, int32_t *d_err, int64_t *d_errpos, cudaStream_t st) {
     if (nq == 0) return PG_OK;
-    if (n_a <= 0 || n_b <= 0 || n_a > 255 || n_b > 255) {
-        set_error("alphabet sizes must be in 1..255 (got %d, %d)", n_a, n_b);
-        return PG_ERR_ARG;
-    }
+    int rc = s.check();
+    if (rc != PG_OK) return rc;
     SwParams p;
     p.q = d_q; p.qoff = d_qoff; p.nq = nq; p.t = d_t; p.tlen = tlen; p.query_is_a = query_is_a;
-    p.global = global;
-    p.n_q = query_is_a ? n_a : n_b;
-    p.n_t = query_is_a ? n_b : n_a;
-    const int16_t *lut_q = query_is_a ? lut_a : lut_b;
-    const int16_t *lut_t = query_is_a ? lut_b : lut_a;
-    // table with the query symbol as the row: tab_qt[q][t] = S(a, b) in either orientation
-    std::vector<int64_t> tab_qt((size_t)p.n_q * p.n_t);
-    int64_t amax = 0;
-    for (int q = 0; q < p.n_q; ++q)
-        for (int t = 0; t < p.n_t; ++t) {
-            const int64_t v = query_is_a ? table[(size_t)q * n_b + t] : table[(size_t)t * n_b + q];
-            tab_qt[(size_t)q * p.n_t + t] = v;
-            amax = std::max<int64_t>(amax, v < 0 ? -v : v);
-        }
-    const int64_t agap = gap < 0 ? -gap : gap;
-    // every DP value lies in [0, min(la,lb) * max S]; operands of one add stay below
-    // that plus max(|S|,|gap|): use 32-bit DPX arithmetic when this provably fits
-    // (NW: every value lies within (la + lb) * max(|S|, |gap|))
-    const long double bound = global ? (long double)std::max(amax, agap) * (long double)(max_qlen + tlen + 2)
-                                     : (long double)amax * (long double)std::min<uint64_t>(max_qlen, tlen) +
-                                           (long double)std::max(amax, agap);
-    if (bound < 2.0e9L) {
+    p.global = s.global;
+    p.n_q = query_is_a ? s.n_a : s.n_b;
+    p.n_t = query_is_a ? s.n_b : s.n_a;
+    const int64_t agap = s.abs_gap();
+    const long double bound = score_bound(s.global, s.abs_max(), agap, std::min<uint64_t>(max_qlen, tlen), max_qlen + tlen);
+    if (bound < SCORE32_LIMIT) {
         // two queries per register (2 x int16) when a local alignment's values stay below 2^14 and gap <= 0
-        static const bool no_x2 = [] { const char *e = getenv("PG_SW_NO_X2"); return e && atoi(e) != 0; }();  // A/B knob
-        const bool x2_ok = !global && gap <= 0 && bound < 16000.0L && agap < 16000 && nq >= 2 && !no_x2;
-        return run_sw<int>(p, max_qlen, lut_q, lut_t, tab_qt, gap, d_score, d_err, d_errpos, st, x2_ok);
+        const bool x2_ok = !s.global && s.gap <= 0 && bound < 16000.0L && agap < 16000 && nq >= 2;
+        return run_sw<int>(p, max_qlen, s, d_score, d_err, d_errpos, st, x2_ok);
     }
-    return run_sw<long long>(p, max_qlen, lut_q, lut_t, tab_qt, gap, d_score, d_err, d_errpos, st);
+    return run_sw<long long>(p, max_qlen, s, d_score, d_err, d_errpos, st);
 }
 
 }  // namespace pg

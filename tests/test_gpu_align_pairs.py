@@ -99,6 +99,8 @@ def test_long_pair_vs_oracle(gpu, oracle):
     A, B = [a, rand_seqs(rng, [7000])[0]], [bytes(b), a[:6999]]
     check_vs_oracle(oracle, A, B, np.array([[0, 0], [1, 1], [1, 0], [0, 1]]), scoring(-2))
     check_vs_oracle(oracle, B, A, np.array([[0, 0], [1, 1]]), scoring(-1))
+    align.pair_scores_arrays(A, B, np.array([[0, 0], [1, 1]]), scoring(-2), False)
+    assert _lib.lib().pg_last_kernel() == b"sw_pair_long_kernel"
 
 
 def test_default_matrix_and_int64_table(gpu, oracle):

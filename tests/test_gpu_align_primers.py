@@ -6,7 +6,7 @@ import os
 import numpy as np
 import pytest
 
-from poly_b200 import align, mash, primers, synth
+from poly_b200 import _lib, align, mash, primers, synth
 from test_oracle_align_primers import GENE, NUC_4, TEST_LUT, TEST_MAT, design_primers, lut
 
 pytestmark = pytest.mark.gpu
@@ -19,6 +19,10 @@ def _make_scoring():
 
 
 SC = _make_scoring()
+
+
+def last_kernel():
+    return _lib.lib().pg_last_kernel().decode()
 
 
 def test_reference_TestSmithWaterman(gpu):
@@ -69,6 +73,7 @@ def test_sw_batch_vs_oracle(gpu, oracle, maxq, tlen):
     t = bytes(rng.choice(list(b"ACGT"), size=tlen).astype(np.uint8))
     for query_is_a in (True, False):
         scores, errs = align.SmithWatermanScores(qs, t, SC, query_is_a=query_is_a)
+        assert last_kernel() in (("sw_score_kernel", "sw_score_x2_kernel") if maxq <= 64 else ("sw_score_long_kernel",))
         for i in range(0, nq, 7):
             a, b = (qs[i], t) if query_is_a else (t, qs[i])
             w = oracle.sw_score(a, b, TEST_LUT, TEST_LUT, TEST_MAT, -2)
@@ -173,6 +178,7 @@ def test_nw_batch_vs_oracle(gpu, oracle, maxq, tlen):
     t = bytes(rng.choice(list(b"ACGT"), size=tlen).astype(np.uint8))
     for query_is_a in (True, False):
         scores, errs = align.NeedlemanWunschScores(qs, t, SC, query_is_a=query_is_a)
+        assert last_kernel() == ("nw_score_kernel" if maxq <= 64 else "sw_score_long_kernel")
         for i in range(0, nq, 5):
             a, b = (qs[i], t) if query_is_a else (t, qs[i])
             w = oracle.nw_score(a, b, TEST_LUT, TEST_LUT, TEST_MAT, -2)
@@ -244,6 +250,7 @@ def test_sw_align_batch_vs_oracle(gpu, oracle, maxq, tlen, gap):
     sc = align.NewScoring(SC.SubstitutionMatrix, gap)
     for query_is_a in (True, False):
         res = align.SmithWatermanAligns(qs, t, sc, query_is_a=query_is_a)
+        assert last_kernel() == "sw_align_kernel"
         step = 1 if tlen <= 1000 else 3
         for i in range(0, nq, step):
             a, b = (qs[i], t) if query_is_a else (t, qs[i])
@@ -369,6 +376,7 @@ def test_sw_packed_int16_kernel(gpu, oracle):
         t = bytes(rng.choice(list(b"ACGT"), size=tlen).astype(np.uint8))
         for query_is_a in (True, False):
             scores, errs = align.SmithWatermanScores(qs, t, sc, query_is_a=query_is_a)
+            assert last_kernel() == "sw_score_x2_kernel"
             for i in range(nq):
                 x, y = (qs[i], t) if query_is_a else (t, qs[i])
                 w = oracle.sw_score(x, y, lut5, lut5, mat, gap)
@@ -379,4 +387,5 @@ def test_sw_packed_int16_kernel(gpu, oracle):
     q = [bytes(rng.choice(list(b"ACGT"), size=25).astype(np.uint8)) for _ in range(10)]
     t = q[3] + bytes(rng.choice(list(b"ACGT"), size=300).astype(np.uint8))
     scores, _ = align.SmithWatermanScores(q, t, sc)
+    assert last_kernel() == "sw_score_kernel"
     assert scores[3] == 25 * 3 * 700 and all(scores[i] == oracle.sw_score(q[i], t, lut5, lut5, mat, -2)[0] for i in range(10))
