@@ -655,6 +655,101 @@ func FoldZukerBatch(bases []byte, offsets []uint64, temp float64) (mfe []float64
 	return mfe[:n], dotBracket, status[:n], err
 }
 
+// FragmentBatch wraps pg_fragment_batch: per sequence the item status (PG_ITEM_*), the efficiency, the failing
+// step's min and max and the fragment ends (fragment j of item i is [start, ends[i][j]) with start 0 for j = 0,
+// else ends[i][j-1] - 4).  An empty include list is Fragment.  PG_ERR_PANIC / PG_ERR_UNSUPPORTED are per-item
+// outcomes here, not call errors.
+func FragmentBatch(seqs []string, minSize, maxSize int, exclude, include []string) (status []int32, eff []float64, errMin, errMax []int64,
+	ends [][]uint64, err error) {
+	n := len(seqs)
+	bases, offsets := Flatten(seqs)
+	ex, exOff := Flatten(exclude)
+	inc, incOff := Flatten(include)
+	status, eff = make([]int32, n+1), make([]float64, n+1)
+	errMin, errMax = make([]int64, n+1), make([]int64, n+1)
+	fragOff := make([]uint64, n+1)
+	flat := make([]uint64, len(bases)/8+2*n+1)
+	var total C.uint64_t
+	for attempt := 0; attempt < 2; attempt++ {
+		err = locked(func() C.int {
+			rc := C.pg_fragment_batch((*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n),
+				C.int64_t(minSize), C.int64_t(maxSize), (*C.uint8_t)(unsafe.Pointer(&ex[0])), (*C.uint64_t)(unsafe.Pointer(&exOff[0])),
+				C.uint64_t(len(exclude)), (*C.uint8_t)(unsafe.Pointer(&inc[0])), (*C.uint64_t)(unsafe.Pointer(&incOff[0])), C.uint64_t(len(include)),
+				(*C.int32_t)(unsafe.Pointer(&status[0])), (*C.double)(unsafe.Pointer(&eff[0])), (*C.int64_t)(unsafe.Pointer(&errMin[0])),
+				(*C.int64_t)(unsafe.Pointer(&errMax[0])), (*C.uint64_t)(unsafe.Pointer(&fragOff[0])), (*C.uint64_t)(unsafe.Pointer(&flat[0])),
+				C.uint64_t(len(flat)), &total)
+			if rc == C.PG_ERR_PANIC || rc == C.PG_ERR_UNSUPPORTED {
+				return C.PG_OK
+			}
+			if rc == C.PG_ERR_ARG && uint64(total) > uint64(len(flat)) {
+				return C.PG_OK // too small a guess: once more with the exact count
+			}
+			return rc
+		})
+		if err != nil || uint64(total) <= uint64(len(flat)) {
+			break
+		}
+		flat = make([]uint64, uint64(total))
+	}
+	if err != nil {
+		return nil, nil, nil, nil, nil, err
+	}
+	ends = make([][]uint64, n)
+	for i := 0; i < n; i++ {
+		ends[i] = flat[fragOff[i]:fragOff[i+1]]
+	}
+	return status[:n], eff[:n], errMin[:n], errMax[:n], ends, nil
+}
+
+// fragmentSets flattens a list of overhang sets for the set entry points.
+func fragmentSets(sets [][]string) ([]byte, []uint64, []uint64) {
+	var all []string
+	setOff := make([]uint64, len(sets)+1)
+	for i, s := range sets {
+		all = append(all, s...)
+		setOff[i+1] = uint64(len(all))
+	}
+	b, off := Flatten(all)
+	return b, off, setOff
+}
+
+// FragmentSetEfficiencyBatch wraps pg_fragment_set_efficiency_batch: SetEfficiency of every set.
+func FragmentSetEfficiencyBatch(sets [][]string) ([]float64, error) {
+	n := len(sets)
+	b, off, setOff := fragmentSets(sets)
+	eff := make([]float64, n+1)
+	err := locked(func() C.int {
+		return C.pg_fragment_set_efficiency_batch((*C.uint8_t)(unsafe.Pointer(&b[0])), (*C.uint64_t)(unsafe.Pointer(&off[0])),
+			(*C.uint64_t)(unsafe.Pointer(&setOff[0])), C.uint64_t(n), (*C.double)(unsafe.Pointer(&eff[0])))
+	})
+	return eff[:n], err
+}
+
+// FragmentNextOverhangsBatch wraps pg_fragment_next_overhangs_batch: NextOverhangs of every set.
+func FragmentNextOverhangsBatch(sets [][]string) (cands [][]string, effs [][]float64, err error) {
+	n := len(sets)
+	b, off, setOff := fragmentSets(sets)
+	raw := make([]byte, 1024*n+1)
+	nc := make([]uint32, n+1)
+	eff := make([]float64, 256*n+1)
+	err = locked(func() C.int {
+		return C.pg_fragment_next_overhangs_batch((*C.uint8_t)(unsafe.Pointer(&b[0])), (*C.uint64_t)(unsafe.Pointer(&off[0])),
+			(*C.uint64_t)(unsafe.Pointer(&setOff[0])), C.uint64_t(n), (*C.uint8_t)(unsafe.Pointer(&raw[0])), (*C.uint32_t)(unsafe.Pointer(&nc[0])),
+			(*C.double)(unsafe.Pointer(&eff[0])))
+	})
+	if err != nil {
+		return nil, nil, err
+	}
+	cands, effs = make([][]string, n), make([][]float64, n)
+	for i := 0; i < n; i++ {
+		for j := 0; j < int(nc[i]); j++ {
+			cands[i] = append(cands[i], string(raw[1024*i+4*j:1024*i+4*j+4]))
+		}
+		effs[i] = eff[256*i : 256*i+int(nc[i])]
+	}
+	return cands, effs, nil
+}
+
 // CloneEnzyme is an enzyme for the clone entry points: the two sites are literals (clone.go:77-84).
 type CloneEnzyme struct {
 	ForwardSite, ReverseSite, RecognitionSite string

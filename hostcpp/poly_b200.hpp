@@ -1185,4 +1185,146 @@ inline std::pair<Result, std::string> Zuker(const std::string &seq, double temp)
     return {it.result, it.error};
 }
 }  // namespace fold
+// ---- synthesis/fragment (synthesis/fragment/fragment.go) over pg_fragment_batch and the set entry points ----
+namespace fragment {
+struct UnsupportedError : std::runtime_error {
+    using std::runtime_error::runtime_error;
+};
+// one item of FragmentWithOverhangsBatch: status is PG_ITEM_OK, PG_ITEM_FRAGMENT_* (error holds the reference's
+// message and fragments is empty), PG_ITEM_PANIC or PG_ITEM_UNSUPPORTED
+struct Item {
+    std::vector<std::string> fragments;
+    double efficiency = 0;
+    std::string error;
+    int32_t status = PG_ITEM_OK;
+};
+// FragmentWithOverhangs of every sequence in one GPU call (an empty include list is Fragment)
+inline std::vector<Item> FragmentWithOverhangsBatch(const std::vector<std::string> &seqs, int64_t minFragmentSize, int64_t maxFragmentSize,
+                                                    const std::vector<std::string> &excludeOverhangs,
+                                                    const std::vector<std::string> &includeOverhangs) {
+    const size_t n = seqs.size();
+    std::vector<Item> out(n);
+    if (n == 0) return out;
+    Flat f(seqs), ex(excludeOverhangs), inc(includeOverhangs);
+    ex.bases.push_back(0);
+    inc.bases.push_back(0);
+    std::vector<int32_t> st(n);
+    std::vector<double> eff(n);
+    std::vector<int64_t> emin(n), emax(n);
+    std::vector<uint64_t> foff(n + 1), ends(f.bases.size() / 8 + 2 * n);
+    uint64_t total = 0;
+    int rc;
+    for (;;) {
+        rc = pg_fragment_batch(f.bases.data(), f.offsets.data(), n, minFragmentSize, maxFragmentSize, ex.bases.data(), ex.offsets.data(),
+                               excludeOverhangs.size(), inc.bases.data(), inc.offsets.data(), includeOverhangs.size(), st.data(), eff.data(),
+                               emin.data(), emax.data(), foff.data(), ends.data(), ends.size(), &total);
+        if (rc != PG_ERR_ARG || total <= ends.size()) break;
+        ends.resize(total);  // the first guess was too small: once more with the exact count
+    }
+    if (rc != PG_ERR_PANIC && rc != PG_ERR_UNSUPPORTED) check(rc);
+    for (size_t i = 0; i < n; ++i) {
+        Item &it = out[i];
+        it.status = st[i];
+        it.efficiency = eff[i];
+        if (st[i] == PG_ITEM_OK) {
+            std::string up = seqs[i];
+            for (auto &c : up)
+                if (c >= 'a' && c <= 'z') c -= 32;
+            for (uint64_t j = foff[i]; j < foff[i + 1]; ++j) {
+                const uint64_t b = j == foff[i] ? 0 : ends[j - 1] - 4;
+                it.fragments.push_back(up.substr(b, ends[j] - b));
+            }
+        } else if (st[i] == PG_ITEM_FRAGMENT_MIN_GT_MAX) {
+            it.error = "minFragmentSize (" + std::to_string(emin[i]) + ") larger than maxFragmentSize (" + std::to_string(emax[i]) + ")";
+        } else if (st[i] == PG_ITEM_FRAGMENT_MIN_LT_12) {
+            it.error = "minFragmentSize must be equal to or greater than 12 . Got size of " + std::to_string(emin[i]);
+        } else if (st[i] == PG_ITEM_FRAGMENT_NO_POSITION) {
+            it.error = "bestOverhangPosition failed by equaling zero";
+        }
+    }
+    return out;
+}
+inline std::vector<Item> FragmentBatch(const std::vector<std::string> &seqs, int64_t minFragmentSize, int64_t maxFragmentSize,
+                                       const std::vector<std::string> &excludeOverhangs) {
+    return FragmentWithOverhangsBatch(seqs, minFragmentSize, maxFragmentSize, excludeOverhangs, {});
+}
+// fragment.FragmentWithOverhangs (fragment.go:199): (fragments, efficiency, error message, empty on success);
+// throws GoPanic where the reference panics (fewer than 4 bytes) and UnsupportedError for a byte >= 0x80
+struct Fragments {
+    std::vector<std::string> fragments;
+    double efficiency;
+    std::string error;
+};
+inline Fragments FragmentWithOverhangs(const std::string &sequence, int64_t minFragmentSize, int64_t maxFragmentSize,
+                                       const std::vector<std::string> &excludeOverhangs, const std::vector<std::string> &includeOverhangs) {
+    Item it = FragmentWithOverhangsBatch({sequence}, minFragmentSize, maxFragmentSize, excludeOverhangs, includeOverhangs)[0];
+    if (it.status == PG_ITEM_PANIC) throw GoPanic("slice bounds out of range");
+    if (it.status == PG_ITEM_UNSUPPORTED) throw UnsupportedError("a byte >= 0x80 (unsupported)");
+    return {it.fragments, it.efficiency, it.error};
+}
+// fragment.Fragment (fragment.go:191)
+inline Fragments Fragment(const std::string &sequence, int64_t minFragmentSize, int64_t maxFragmentSize,
+                          const std::vector<std::string> &excludeOverhangs) {
+    return FragmentWithOverhangs(sequence, minFragmentSize, maxFragmentSize, excludeOverhangs, {});
+}
+namespace detail {
+struct Sets {
+    std::vector<uint8_t> bases;
+    std::vector<uint64_t> offsets, set_offsets{0};
+    explicit Sets(const std::vector<std::vector<std::string>> &sets) {
+        std::vector<std::string> all;
+        for (auto &s : sets) {
+            all.insert(all.end(), s.begin(), s.end());
+            set_offsets.push_back(all.size());
+        }
+        Flat f(all);
+        bases = std::move(f.bases);
+        bases.push_back(0);
+        offsets = std::move(f.offsets);
+    }
+};
+}  // namespace detail
+// SetEfficiency of every set in one GPU call
+inline std::vector<double> SetEfficiencyBatch(const std::vector<std::vector<std::string>> &sets) {
+    std::vector<double> eff(sets.size());
+    if (sets.empty()) return eff;
+    detail::Sets s(sets);
+    check(pg_fragment_set_efficiency_batch(s.bases.data(), s.offsets.data(), s.set_offsets.data(), sets.size(), eff.data()));
+    return eff;
+}
+// fragment.SetEfficiency (fragment.go:24)
+inline double SetEfficiency(const std::vector<std::string> &overhangs) { return SetEfficiencyBatch({overhangs})[0]; }
+// NextOverhangs of every set in one GPU call: (candidates, efficiencies) per set
+inline std::vector<std::pair<std::vector<std::string>, std::vector<double>>> NextOverhangsBatch(const std::vector<std::vector<std::string>> &sets) {
+    std::vector<std::pair<std::vector<std::string>, std::vector<double>>> out(sets.size());
+    if (sets.empty()) return out;
+    detail::Sets s(sets);
+    std::vector<uint8_t> cands(1024 * sets.size());
+    std::vector<uint32_t> nc(sets.size());
+    std::vector<double> eff(256 * sets.size());
+    check(pg_fragment_next_overhangs_batch(s.bases.data(), s.offsets.data(), s.set_offsets.data(), sets.size(), cands.data(), nc.data(), eff.data()));
+    for (size_t i = 0; i < sets.size(); ++i)
+        for (uint32_t j = 0; j < nc[i]; ++j) {
+            out[i].first.emplace_back((const char *)cands.data() + 1024 * i + 4 * j, 4);
+            out[i].second.push_back(eff[256 * i + j]);
+        }
+    return out;
+}
+// fragment.NextOverhangs (fragment.go:43)
+inline std::pair<std::vector<std::string>, std::vector<double>> NextOverhangs(const std::vector<std::string> &currentOverhangs) {
+    return NextOverhangsBatch({currentOverhangs})[0];
+}
+// fragment.NextOverhang (fragment.go:85): the first strict maximum above 0, or ""
+inline std::string NextOverhang(const std::vector<std::string> &currentOverhangs) {
+    const auto r = NextOverhangs(currentOverhangs);
+    double best = 0;
+    std::string pick;
+    for (size_t i = 0; i < r.first.size(); ++i)
+        if (r.second[i] > best) {
+            best = r.second[i];
+            pick = r.first[i];
+        }
+    return pick;
+}
+}  // namespace fragment
 }  // namespace poly

@@ -58,6 +58,9 @@ extern "C" {
 #define PG_ITEM_UNSUPPORTED 2 /* e.g. byte >= 0x80 passed to SantaLucia (ToUpper)       */
 #define PG_ITEM_FOLD_NOT_NUCLEIC 3 /* fold: "the sequence %s is not RNA or DNA"           */
 #define PG_ITEM_FOLD_INTERNAL 4    /* fold: one of the reference's internal errors fired  */
+#define PG_ITEM_FRAGMENT_MIN_GT_MAX 5  /* fragment: "minFragmentSize (%d) larger than maxFragmentSize (%d)" */
+#define PG_ITEM_FRAGMENT_MIN_LT_12 6   /* fragment: "minFragmentSize must be equal to or greater than 12 . Got size of %d" */
+#define PG_ITEM_FRAGMENT_NO_POSITION 7 /* fragment: "bestOverhangPosition failed by equaling zero" */
 
 /* ---- library / device management -------------------------------------------- */
 int pg_version(void);
@@ -546,6 +549,35 @@ int pg_least_rotation_batch(const uint8_t *seqs, const uint64_t *offsets, uint64
 #define PG_FOLD_MAX_LEN 1024
 int pg_fold_zuker_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, double temp, double *mfe,
                         uint8_t *dot_bracket, uint64_t *db_len, int32_t *status);
+
+/* ---- synthesis/fragment: Fragment, FragmentWithOverhangs, SetEfficiency, NextOverhangs ----------------
+ * pg_fragment_batch: Fragment(seq, min_size, max_size, exclude) of every sequence [offsets[i], offsets[i+1])
+ * of `seqs`, or FragmentWithOverhangs(..., exclude, include) when n_include > 0.  The exclude and include
+ * lists (ragged, n_exclude + 1 and n_include + 1 offsets) are shared by the whole batch; overhangs are any
+ * bytes of any length and are used exactly as given (only the sequence is upper-cased).  Per item:
+ * status[i] (may be NULL) PG_ITEM_OK; PG_ITEM_FRAGMENT_MIN_GT_MAX / _MIN_LT_12 with the failing step's
+ * values in err_min[i] / err_max[i] (after an end-game adjustment these are the adjusted values);
+ * PG_ITEM_FRAGMENT_NO_POSITION; PG_ITEM_PANIC for fewer than 4 bytes; PG_ITEM_UNSUPPORTED for a byte >= 0x80.
+ * efficiency[i] is the reference's float64, bit for bit (0 unless OK).  The fragments are given by their
+ * ends: item i has frag_offsets[i+1] - frag_offsets[i] of them (0 unless OK) at ends[frag_offsets[i] ..];
+ * fragment j is [start_j, end_j) of the item with start_0 = 0 and start_j = end_{j-1} - 4, and the last end
+ * is the item's length.  *n_ends (the total) and frag_offsets (n + 1 entries) are always written; more ends
+ * than ends_cap is PG_ERR_ARG with every other output written, and nothing written past ends[ends_cap]
+ * (ends may hold the ends of the leading items, which went to the device first).  Otherwise returns
+ * PG_ERR_PANIC if any item panics, else PG_ERR_UNSUPPORTED if any is unsupported, with every output
+ * written.  Items go to the device in groups under a device-memory budget. */
+int pg_fragment_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, int64_t min_size, int64_t max_size, const uint8_t *exclude,
+                      const uint64_t *exclude_offsets, uint64_t n_exclude, const uint8_t *include, const uint64_t *include_offsets,
+                      uint64_t n_include, int32_t *status, double *efficiency, int64_t *err_min, int64_t *err_max, uint64_t *frag_offsets,
+                      uint64_t *ends, uint64_t ends_cap, uint64_t *n_ends);
+/* Set i is the overhangs [set_offsets[i], set_offsets[i+1]) of the ragged list (overhangs, overhang_offsets),
+ * in order (duplicates count).  pg_fragment_set_efficiency_batch: efficiency[i] = SetEfficiency(set i).
+ * pg_fragment_next_overhangs_batch: NextOverhangs(set i): n_cands[i] candidates at cands[1024 i ..]
+ * (4 bytes each, in the reference's order) and their efficiencies at efficiency[256 i ..]. */
+int pg_fragment_set_efficiency_batch(const uint8_t *overhangs, const uint64_t *overhang_offsets, const uint64_t *set_offsets, uint64_t n_sets,
+                                     double *efficiency);
+int pg_fragment_next_overhangs_batch(const uint8_t *overhangs, const uint64_t *overhang_offsets, const uint64_t *set_offsets, uint64_t n_sets,
+                                     uint8_t *cands, uint32_t *n_cands, double *efficiency);
 
 /* ---- clone.CutWithEnzyme / CircularLigate / GoldenGate -- clone/clone.go:138-355 --------------------
  * An enzyme: RegexpFor and RegexpRev as literal sites (1..32 bytes of 0x01..0x7f; anything else is

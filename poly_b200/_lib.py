@@ -106,6 +106,10 @@ _SIGS = {
     "pg_clone_circular_ligate_batch": (C.c_int, [_u8p, _u64p, _u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_uint64, C.c_uint64, _u8p, _u64p, _u8p,
                                                  _u8p, _u64p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "pg_fold_zuker_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_double, _f64p, _u8p, _u64p, _i32p]),
+    "pg_fragment_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_int64, C.c_int64, _u8p, _u64p, C.c_uint64, _u8p, _u64p, C.c_uint64, _i32p, _f64p,
+                                    _i64p, _i64p, _u64p, _u64p, C.c_uint64, _u64p]),
+    "pg_fragment_set_efficiency_batch": (C.c_int, [_u8p, _u64p, _u64p, C.c_uint64, _f64p]),
+    "pg_fragment_next_overhangs_batch": (C.c_int, [_u8p, _u64p, _u64p, C.c_uint64, _u8p, _u32p, _f64p]),
     "pg_synth_reads_dev": (C.c_int, [_u8p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64, C.c_int32, C.c_uint32, C.c_void_p]),
 }
 EXPORTS = tuple(_SIGS)

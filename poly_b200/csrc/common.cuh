@@ -276,6 +276,55 @@ uint64_t fold_scratch_bytes(uint64_t len);
 std::vector<uint8_t> fold_tables(double temp);
 int launch_fold_zuker(const uint8_t *d_seqs, const uint64_t *d_off, uint64_t n, const uint8_t *d_tables, uint8_t *d_scratch,
                       const uint64_t *d_scr_off, double *d_mfe, uint8_t *d_db, uint64_t *d_db_len, int32_t *d_status, cudaStream_t st);
+// fragment.cu: poly's synthesis/fragment.  fragment_host turns the batch-wide exclude and include lists
+// into what the kernel reads (the fidelity table, R and the keys of the excludes, the A/C/G/T masks and the
+// other 4-byte words with their reverse complements); fragment_max_ends bounds an item's fragment count.
+struct FragmentHost {
+    std::vector<uint8_t> fid;  // the kernel's table: 120 x 120 counts, then the code -> key map
+    std::vector<long long> r_ex;
+    std::vector<uint32_t> ex_mask, inc_mask, ex_other, inc_other;
+    std::vector<uint8_t> ex_keys;
+};
+struct FragmentArgs {
+    const uint8_t *seqs;
+    const uint64_t *off;
+    uint64_t n;
+    int64_t min_size, max_size;
+    const uint8_t *fid;
+    const long long *r_ex;
+    const uint32_t *ex_mask, *inc_mask;
+    const uint8_t *ex_keys;
+    uint64_t n_ex_keys;
+    const uint32_t *ex_other, *inc_other;
+    uint64_t n_ex_other, n_inc_other;
+    int has_include;
+    uint32_t *scratch;  // set by launch_fragment
+    uint64_t slot_words;
+    int32_t *status;
+    double *eff;
+    int64_t *err_min, *err_max;
+    uint64_t *n_ends, *ends;    // item i's ends at ends[ends_off[i] ..], room for fragment_max_ends(L_i)
+    const uint64_t *ends_off;
+};
+struct SetArgs {
+    const uint8_t *fid;
+    const uint8_t *ov;          // overhang bytes, indexed with ov_off
+    const uint64_t *ov_off, *set_off;
+    uint64_t first, n_sets;     // sets first .. first + n_sets; outputs are indexed from 0
+    int next;                   // 0: SetEfficiency, 1: NextOverhangs
+    uint8_t *scratch;           // set by launch_overhang_sets
+    uint64_t slot_bytes;
+    double *eff;                // n_sets (SetEfficiency) or n_sets x 256 (NextOverhangs)
+    uint8_t *cands;             // n_sets x 256 x 4
+    uint32_t *n_cands;
+};
+uint64_t fragment_max_ends(uint64_t len);
+FragmentHost fragment_host(const uint8_t *ex, const uint64_t *ex_off, uint64_t n_ex, const uint8_t *inc, const uint64_t *inc_off, uint64_t n_inc);
+int launch_fragment(FragmentArgs a, uint64_t max_len, uint64_t scratch_budget, StreamScratch &tmp, cudaStream_t st);
+int launch_fragment_compact(const uint64_t *d_region, const uint64_t *d_region_off, const uint64_t *d_n_ends, const uint64_t *d_out_off, uint64_t n,
+                            uint64_t *d_out, cudaStream_t st);
+// max_keys: the most keyed members of any set in the launch
+int launch_overhang_sets(SetArgs a, uint64_t max_keys, uint64_t scratch_budget, StreamScratch &tmp, cudaStream_t st);
 // synth.cu
 int launch_synth_reads(uint8_t *d_bases, uint64_t first_read, uint64_t n_reads, uint32_t read_len,
                        uint64_t seed, int kind, uint32_t family, cudaStream_t st);
