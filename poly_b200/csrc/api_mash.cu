@@ -1,0 +1,835 @@
+// api_mash.cu -- the C ABI of poly's mash: Sketch on device and host buffers (the pipelined host path),
+// the single-process multi-GPU entry points, Similarity / Distance and the sketch index.
+#include <algorithm>
+#include <atomic>
+#include <cstring>
+#include <functional>
+#include <sched.h>
+#include <string>
+#include <thread>
+#include <vector>
+
+#include "runtime.cuh"
+
+struct pg_mash_index {
+    int device;
+    uint32_t *d_sk;        // the index's own copy of the n x s reference sketches
+    pg::DistancePlan plan;  // sortedness flags + join index over d_sk
+};
+
+namespace pg {
+namespace {
+
+static inline uint64_t kmers_of(uint64_t len, int k) { return len > (uint64_t)k ? len - (uint64_t)k : 0; }
+// informative words of the sketch of a read of `len` bytes
+static inline uint64_t sketch_words(uint64_t len, int k, int s) { return std::min<uint64_t>(kmers_of(len, k), (uint64_t)s); }
+
+// Rows [rb, re) of a plan's matching counts and/or distances into host arrays that start at row rb, in row
+// blocks of <= 64 Mi pairs per pass
+int plan_rows_to_host(const DistancePlan &plan, uint64_t rb, uint64_t re, uint32_t *same, double *distance, cudaStream_t st) {
+    const uint64_t n = plan.n, rows_per = std::max<uint64_t>(8, ((64ull << 20) / n) & ~7ull);
+    for (uint64_t b = rb; b < re; b += rows_per) {
+        const uint64_t e = std::min(re, b + rows_per), cells = (e - b) * n;
+        StreamScratch tmp(st);
+        uint32_t *d_same = nullptr;
+        double *d_dist = nullptr;
+        int rc;
+        if (same && (rc = scratch_alloc(tmp, &d_same, cells))) return rc;
+        if (distance && (rc = scratch_alloc(tmp, &d_dist, cells))) return rc;
+        if ((rc = distance_plan_rows(plan, b, e, d_same, d_dist, st)) != PG_OK) return rc;
+        if (same) PG_CUDA(cudaMemcpyAsync(same + (b - rb) * n, d_same, cells * 4, cudaMemcpyDeviceToHost, st));
+        if (distance) PG_CUDA(cudaMemcpyAsync(distance + (b - rb) * n, d_dist, cells * 8, cudaMemcpyDeviceToHost, st));
+        PG_CUDA(cudaStreamSynchronize(st));
+    }
+    return PG_OK;
+}
+
+static int check_ks(int32_t k, int32_t s) {
+    if (k < 0) { set_error("kmerSize %d < 0: the reference panics (slice bounds)", k); return PG_ERR_ARG; }
+    if (s < 0) { set_error("sketchSize %d < 0: the reference panics (makeslice)", s); return PG_ERR_ARG; }
+    return PG_OK;
+}
+static int check_dev_flags(uint32_t flags) {
+    if (flags & PG_SKETCH_TAIL_KEEP) { set_error("PG_SKETCH_TAIL_KEEP applies to host buffers only"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+// the least row stride of a batch whose longest read has max_len bytes: its count, or s with PAD_ZERO
+static uint64_t need_row_stride(uint64_t max_len, int32_t k, int32_t s, uint32_t flags) {
+    return (flags & PG_SKETCH_PAD_ZERO) ? (uint64_t)s : sketch_words(max_len, k, s);
+}
+static int check_row_stride(uint64_t row_stride, uint64_t max_len, int32_t k, int32_t s, uint32_t flags) {
+    const uint64_t need = need_row_stride(max_len, k, s, flags);
+    if (row_stride < need) { set_error("row_stride %llu < %llu", (unsigned long long)row_stride, (unsigned long long)need); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+// rows [row_offset, row_offset + n_local) of every destination buffer (compact rows of cnt words)
+static int sketch_scatter_dev(const uint8_t *d_bases, uint64_t n_local, uint32_t read_len, int32_t k, int32_t s,
+                              void *const *dst_ptrs, int32_t n_dst, int32_t self, uint64_t row_offset, cudaStream_t st) {
+    int rc;
+    if ((rc = check_ks(k, s)) != PG_OK) return rc;
+    if (n_dst < 1 || n_dst > PG_MAX_PEERS || self < 0 || self >= n_dst || !dst_ptrs) {
+        set_error("bad destination set (%d buffers, own index %d; at most %d)", n_dst, self, PG_MAX_PEERS);
+        return PG_ERR_ARG;
+    }
+    const uint64_t cnt = sketch_words(read_len, k, s);
+    SketchDst dst;
+    dst.n = n_dst;
+    for (int p = 0; p < n_dst; ++p) {
+        if (!dst_ptrs[p]) { set_error("null gathered pointer for rank %d", p); return PG_ERR_ARG; }
+        dst.ptr[p] = (uint32_t *)dst_ptrs[p] + row_offset * cnt;  // this rank's row block
+    }
+    return launch_sketch_uniform(d_bases, n_local, read_len, k, s, 0, dst.ptr[self], cnt, nullptr, st, &dst);
+}
+
+// Pipelined host path shared by the uniform and ragged entry points: chunks of reads
+// cycle through the N_SLOTS stream/buffer slots (H2D, kernel, D2H overlap across slots).
+static bool is_pageable(const void *p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return true; }
+    return a.type == cudaMemoryTypeUnregistered;
+}
+
+static int host_copy_helpers() {
+    if (const char *e = getenv("PG_HOST_COPY_THREADS")) return std::max(0, atoi(e) - 1);
+    cpu_set_t cur;
+    int cores = (int)std::thread::hardware_concurrency();
+    if (sched_getaffinity(0, sizeof cur, &cur) == 0) cores = std::min(cores, CPU_COUNT(&cur));
+    return std::max(0, std::min(8, cores / 2) - 1);
+}
+
+// One host sketch call: reads [0, n) of a ragged batch (offsets) or of fixed-length reads (ulen bytes
+// each, offsets == nullptr), the sketch of read i at out + i * row_stride
+struct SketchCall {
+    const uint8_t *bases;
+    const uint64_t *offsets;
+    uint32_t ulen;
+    uint64_t n;
+    int32_t k, s;
+    uint32_t flags;
+    uint32_t *out;
+    uint64_t row_stride;
+    uint32_t *count;
+    int32_t *status;
+};
+
+// Every argument check of a host sketch call, made before anything is launched or written: k and s,
+// the buffers, the offsets of the whole batch and the row stride its longest read needs.
+static int sketch_check(const SketchCall &q) {
+    int rc;
+    if ((rc = check_ks(q.k, q.s)) != PG_OK || q.n == 0) return rc;
+    if (!q.bases || !q.out) { set_error("null buffer"); return PG_ERR_ARG; }
+    uint64_t max_len = q.ulen;
+    if (q.offsets && (rc = check_ragged(q.offsets, q.n, &max_len)) != PG_OK) return rc;
+    return check_row_stride(q.row_stride, max_len, q.k, q.s, q.flags);
+}
+
+// reads [r0, r1) of the batch, bytes [beg, end) of bases
+struct Chunk {
+    uint64_t r0, r1, beg, end, maxlen, minlen;
+    bool uniform;  // all reads of one length below 2^32: the uniform kernel takes the chunk
+};
+
+// One pipelined host sketch call on the current device, over a batch sketch_check accepted; holds the
+// device's lock.  Chunk i goes to slot i % N_SLOTS once the slot's previous chunk is drained.  Unless
+// run() completes, the destructor waits for every slot's stream, so that no copy into or out of the
+// caller's memory is still running when the entry point returns.
+class SketchPipe {
+    static constexpr uint64_t TARGET_OUT_BYTES = 128ull << 20;  // staged output bytes per chunk
+    DevCtx &cx_;
+    std::lock_guard<std::mutex> lock_;
+    SketchCall q_;  // flags without PG_SKETCH_TAIL_KEEP
+    // Pinned caller buffers (pg_host_alloc, cudaHostRegister) are DMA'd directly.  Pageable ones (a Go
+    // []byte / []uint32) would be bounced by the driver at ~14 GB/s: they go through pinned staging
+    // buffers instead, filled / emptied by a few host threads while the other slots' DMA runs; the
+    // device then always produces compact rows and the zero tail of PG_SKETCH_PAD_ZERO rows is
+    // written by the host threads, not shipped over PCIe.
+    // PG_SKETCH_TAIL_KEEP: only the informative words of a row are written.  Ragged batches then always go through
+    // the staging buffers, whose rows are copied out count[i] words at a time.
+    const bool keep_tail_, stage_in_, stage_out_, want_status_;
+    const uint64_t target_bytes_;  // input bytes per chunk
+    bool any_panic_ = false, finished_ = false;
+
+    // f(a, b) over min(threads, nrows) parts of rows [0, nrows), on the copy pool
+    void par_rows(uint64_t nrows, const std::function<void(uint64_t, uint64_t)> &f) {
+        const int parts = (int)std::min<uint64_t>((uint64_t)cx_.pool.threads(), std::max<uint64_t>(1, nrows));
+        cx_.pool.run(parts, [&](int i) { f(nrows * (uint64_t)i / parts, nrows * (uint64_t)(i + 1) / parts); });
+    }
+
+    // the chunk that starts at read r0
+    Chunk next_chunk(uint64_t r0) const {
+        Chunk c{r0, r0, 0, 0, 0, ~0ull, false};
+        if (q_.offsets) {
+            const uint64_t *off = q_.offsets;
+            c.beg = off[r0];
+            while (c.r1 < q_.n && (c.r1 == r0 || off[c.r1 + 1] - c.beg <= target_bytes_)) {
+                const uint64_t len = off[c.r1 + 1] - off[c.r1];
+                c.maxlen = std::max(c.maxlen, len);
+                c.minlen = std::min(c.minlen, len);
+                ++c.r1;
+                if (stage_out_ && (c.r1 - r0) * sketch_words(c.maxlen, q_.k, q_.s) * 4 >= TARGET_OUT_BYTES) break;
+            }
+            c.end = off[c.r1];
+        } else {
+            uint64_t per = std::max<uint64_t>(1, target_bytes_ / std::max<uint32_t>(q_.ulen, 1));
+            const uint64_t row_bytes = sketch_words(q_.ulen, q_.k, q_.s) * 4;
+            if (stage_out_ && row_bytes) per = std::min(per, std::max<uint64_t>(32, TARGET_OUT_BYTES / row_bytes));
+            per = (per + 31) & ~31ull;  // keep chunk starts on K1 tile boundaries
+            c.r1 = std::min(q_.n, r0 + per);
+            c.beg = r0 * (uint64_t)q_.ulen;
+            c.end = c.r1 * (uint64_t)q_.ulen;
+            c.maxlen = c.minlen = q_.ulen;
+        }
+        c.uniform = c.maxlen == c.minlen && c.maxlen <= 0xffffffffull;
+        return c;
+    }
+
+    // *src = the chunk's input bytes as the H2D copy reads them: pageable input is first copied into the
+    // slot's pinned buffer, in 1 MiB granules over the copy pool
+    int stage_in(Slot &sl, const Chunk &c, const uint8_t **src) {
+        const uint8_t *h = q_.bases + c.beg;
+        const uint64_t bytes = c.end - c.beg;
+        *src = h;
+        if (!stage_in_ || !bytes) return PG_OK;
+        const int rc = sl.pin_in.reserve(bytes);
+        if (rc != PG_OK) return rc;
+        uint8_t *pin = (uint8_t *)sl.pin_in.p;
+        par_rows((bytes + (1u << 20) - 1) >> 20, [&](uint64_t a, uint64_t b) {
+            const uint64_t lo = a << 20, hi = std::min<uint64_t>(bytes, b << 20);
+            if (hi > lo) memcpy(pin + lo, h + lo, hi - lo);
+        });
+        *src = pin;
+        return PG_OK;
+    }
+
+    // the chunk's copies in, kernel and copies out on the slot's stream; the slot is drained
+    int enqueue(Slot &sl, const Chunk &c) {
+        const int32_t k = q_.k, s = q_.s;
+        const uint64_t nr = c.r1 - c.r0, in_bytes = c.end - c.beg, cnt_max = sketch_words(c.maxlen, k, s);
+        // staged output: compact device rows, the host threads pad; direct output: the device pads
+        const bool compact = stage_out_ || keep_tail_;
+        const uint32_t dev_flags = compact ? (q_.flags & ~PG_SKETCH_PAD_ZERO) : q_.flags;
+        const uint64_t dev_stride = compact ? cnt_max : need_row_stride(c.maxlen, k, s, q_.flags);
+        const cudaStream_t st = sl.stream;
+        int rc;
+        if ((rc = sl.in.reserve(in_bytes + 64)) != PG_OK) return rc;
+        if ((rc = sl.out.reserve(std::max<uint64_t>(nr * dev_stride * 4, 16))) != PG_OK) return rc;
+        uint8_t *d_in = (uint8_t *)sl.in.p;
+        uint32_t *d_out = (uint32_t *)sl.out.p;
+        int32_t *d_status = nullptr;
+        uint32_t *d_count = nullptr;
+        if (want_status_) {
+            if ((rc = sl.st.reserve(nr * 4)) != PG_OK) return rc;
+            d_status = (int32_t *)sl.st.p;
+            PG_CUDA(cudaMemsetAsync(d_status, 0, nr * 4, st));
+            sl.status.assign(nr, 0);
+        }
+        const uint8_t *h_src;
+        if ((rc = stage_in(sl, c, &h_src)) != PG_OK) return rc;
+        if (in_bytes) PG_CUDA(cudaMemcpyAsync(d_in, h_src, in_bytes, cudaMemcpyHostToDevice, st));
+        if (c.uniform) {
+            rc = launch_sketch_uniform(d_in, nr, (uint32_t)c.maxlen, k, s, dev_flags, d_out, dev_stride, d_status, st);
+        } else {
+            if ((rc = sl.aux.reserve((nr + 1) * 8 + nr * 4)) != PG_OK) return rc;
+            uint64_t *d_off = (uint64_t *)sl.aux.p;
+            d_count = (uint32_t *)(d_off + nr + 1);
+            PG_CUDA(cudaMemcpyAsync(d_off, q_.offsets + c.r0, (nr + 1) * 8, cudaMemcpyHostToDevice, st));
+            // kernels index bases with absolute offsets: shift the base pointer
+            rc = launch_sketch_ragged(d_in - c.beg, d_off, nr, c.maxlen, k, s, dev_flags, d_out, dev_stride, d_count, d_status, st);
+        }
+        if (rc != PG_OK) return rc;
+        uint32_t *out = q_.out + c.r0 * q_.row_stride;
+        if (dev_stride) {
+            if (stage_out_) {
+                if ((rc = sl.pin_out.reserve(nr * dev_stride * 4)) != PG_OK) return rc;
+                PG_CUDA(cudaMemcpyAsync(sl.pin_out.p, d_out, nr * dev_stride * 4, cudaMemcpyDeviceToHost, st));
+            } else if (q_.row_stride == dev_stride) {
+                PG_CUDA(cudaMemcpyAsync(out, d_out, nr * dev_stride * 4, cudaMemcpyDeviceToHost, st));
+            } else {
+                PG_CUDA(cudaMemcpy2DAsync(out, q_.row_stride * 4, d_out, dev_stride * 4, dev_stride * 4, nr, cudaMemcpyDeviceToHost, st));
+            }
+        }
+        if (q_.count) {
+            if (c.uniform) std::fill(q_.count + c.r0, q_.count + c.r1, (uint32_t)cnt_max);
+            else PG_CUDA(cudaMemcpyAsync(q_.count + c.r0, d_count, nr * 4, cudaMemcpyDeviceToHost, st));
+        }
+        if (want_status_) PG_CUDA(cudaMemcpyAsync(sl.status.data(), d_status, nr * 4, cudaMemcpyDeviceToHost, st));
+        sl.r0 = c.r0;
+        sl.nr = nr;
+        sl.dstride = dev_stride;
+        sl.used = true;
+        return PG_OK;
+    }
+
+    // waits for the slot's chunk, then unstages its rows (or zeroes their tails) and folds its statuses
+    int drain(Slot &sl) {
+        if (!sl.used) return PG_OK;
+        PG_CUDA(cudaStreamSynchronize(sl.stream));
+        const uint64_t rs = q_.row_stride, ds = sl.dstride;
+        uint32_t *out = q_.out + sl.r0 * rs;
+        if (stage_out_ && ds) {  // staged rows -> caller rows (+ zero tail up to the caller's stride)
+            const uint32_t *src = (const uint32_t *)sl.pin_out.p;
+            par_rows(sl.nr, [&](uint64_t a, uint64_t b) {
+                if (ds == rs && !(keep_tail_ && q_.offsets)) {
+                    memcpy(out + a * rs, src + a * ds, (b - a) * ds * 4);
+                    return;
+                }
+                for (uint64_t i = a; i < b; ++i) {
+                    if (keep_tail_) {  // exactly the informative words of this row
+                        const uint64_t r = sl.r0 + i;
+                        const uint64_t ci = q_.offsets ? sketch_words(q_.offsets[r + 1] - q_.offsets[r], q_.k, q_.s) : ds;
+                        memcpy(out + i * rs, src + i * ds, ci * 4);
+                        continue;
+                    }
+                    memcpy(out + i * rs, src + i * ds, ds * 4);
+                    memset(out + i * rs + ds, 0, (rs - ds) * 4);
+                }
+            });
+        } else if (rs > ds && !keep_tail_) {  // direct DMA wrote ds words per row: zero the rest of each row
+            par_rows(sl.nr, [&](uint64_t a, uint64_t b) {
+                for (uint64_t i = a; i < b; ++i) memset(out + i * rs + ds, 0, (rs - ds) * 4);
+            });
+        }
+        if (want_status_) {
+            for (uint64_t i = 0; i < sl.nr; ++i) {
+                if (sl.status[i] != PG_ITEM_OK) any_panic_ = true;
+                if (q_.status) q_.status[sl.r0 + i] = sl.status[i];
+            }
+        }
+        sl.used = false;
+        return PG_OK;
+    }
+
+public:
+    explicit SketchPipe(const SketchCall &q)
+        : cx_(*cur_ctx()), lock_(cx_.mu), q_(q), keep_tail_((q.flags & PG_SKETCH_TAIL_KEEP) != 0), stage_in_(is_pageable(q.bases)),
+          stage_out_(is_pageable(q.out) || (keep_tail_ && q.offsets)), want_status_(q.status != nullptr || q.s <= 1),
+          target_bytes_((stage_in_ || stage_out_) ? (32ull << 20) : (192ull << 20)) {
+        q_.flags &= ~PG_SKETCH_TAIL_KEEP;
+        if (stage_in_ || stage_out_) cx_.pool.start(host_copy_helpers(), cx_.device);
+    }
+    ~SketchPipe() {
+        if (finished_) return;
+        for (Slot &sl : cx_.slots) {
+            cudaStreamSynchronize(sl.stream);
+            sl.used = false;
+        }
+        cudaGetLastError();
+    }
+    int run() {
+        int rc, slot = 0;
+        for (uint64_t r0 = 0; r0 < q_.n; slot = (slot + 1) % N_SLOTS) {
+            const Chunk c = next_chunk(r0);
+            if ((rc = drain(cx_.slots[slot])) != PG_OK || (rc = enqueue(cx_.slots[slot], c)) != PG_OK) return rc;
+            r0 = c.r1;
+        }
+        for (int i = 0; i < N_SLOTS; ++i)
+            if ((rc = drain(cx_.slots[(slot + i) % N_SLOTS])) != PG_OK) return rc;  // oldest first
+        finished_ = true;
+        if (any_panic_) {
+            set_error("at least one read hits an input on which mash.Sketch panics (sketchSize <= 1)");
+            return PG_ERR_PANIC;
+        }
+        return PG_OK;
+    }
+};
+
+static int sketch_host(const SketchCall &q) {
+    int rc = ensure_device();
+    if (rc != PG_OK || (rc = sketch_check(q)) != PG_OK || q.n == 0) return rc;
+    return SketchPipe(q).run();
+}
+
+struct WorkerResult {
+    int rc = PG_OK;
+    std::string msg;
+};
+
+// worst result of the workers, message copied to the caller's thread-local slot.  A reference panic
+// (PG_ERR_PANIC: per-item statuses are still complete) ranks below real failures.
+static int fold_results(const std::vector<WorkerResult> &res) {
+    int worst = PG_OK;
+    const std::string *msg = nullptr;
+    for (const WorkerResult &r : res) {
+        if (r.rc == PG_OK) continue;
+        const bool soft = r.rc == PG_ERR_PANIC, worst_soft = worst == PG_ERR_PANIC || worst == PG_OK;
+        if (worst == PG_OK || (!soft && worst_soft)) { worst = r.rc; msg = &r.msg; }
+    }
+    if (msg) set_error("%s", msg->c_str());
+    return worst;
+}
+
+static int resolve_devices(const int32_t *devices, int32_t n_devices, std::vector<int> *out) {
+    int n = 0, rc = device_count_checked(&n);
+    if (rc != PG_OK) return rc;
+    out->clear();
+    if (!devices) {
+        const int cnt = n_devices > 0 ? std::min<int>(n_devices, n) : n;
+        for (int i = 0; i < cnt; ++i) out->push_back(i);
+    } else {
+        if (n_devices <= 0) { set_error("device list given with n_devices = %d", n_devices); return PG_ERR_ARG; }
+        for (int i = 0; i < n_devices; ++i) {
+            if (devices[i] < 0 || devices[i] >= n) { set_error("device %d out of range (count %d)", devices[i], n); return PG_ERR_ARG; }
+            for (int j = 0; j < i; ++j)
+                if (devices[j] == devices[i]) { set_error("device %d listed twice", devices[i]); return PG_ERR_ARG; }
+            out->push_back(devices[i]);
+        }
+    }
+    if (out->size() > (size_t)PG_MAX_PEERS) out->resize(PG_MAX_PEERS);
+    return PG_OK;
+}
+
+// reusable barrier for the device threads of one call
+class Rendezvous {
+    std::mutex mu_;
+    std::condition_variable cv_;
+    int n_, waiting_ = 0;
+    uint64_t gen_ = 0;
+public:
+    explicit Rendezvous(int n) : n_(n) {}
+    void wait() {
+        std::unique_lock<std::mutex> lk(mu_);
+        const uint64_t g = gen_;
+        if (++waiting_ == n_) { waiting_ = 0; ++gen_; cv_.notify_all(); }
+        else cv_.wait(lk, [&] { return gen_ != g; });
+    }
+};
+
+// P contiguous shards of n reads, cut on K1 tile boundaries (32 reads): shard r is [cut[r], cut[r + 1])
+std::vector<uint64_t> uniform_cuts(uint64_t n, int P) {
+    std::vector<uint64_t> cut(P + 1, n);
+    cut[0] = 0;
+    const uint64_t per = ((n + P - 1) / P + 31) & ~31ull;
+    for (int r = 1; r < P; ++r) cut[r] = std::min(n, (uint64_t)r * per);
+    return cut;
+}
+
+// The batch is checked once, here, before it is cut; each shard then runs the pipeline on its device's thread.
+int sketch_multi(const SketchCall &q, const int32_t *devices, int32_t n_devices) {
+    std::vector<int> dev;
+    int rc;
+    if ((rc = resolve_devices(devices, n_devices, &dev)) != PG_OK || (rc = sketch_check(q)) != PG_OK || q.n == 0) return rc;
+    const int P = (int)dev.size();
+    std::vector<uint64_t> cut = uniform_cuts(q.n, P);
+    if (q.offsets) {  // ragged batches balance bytes instead
+        const uint64_t b0 = q.offsets[0], total = q.offsets[q.n] - b0;
+        for (int r = 1; r < P; ++r) {
+            const uint64_t want = b0 + total / P * r;
+            uint64_t i = std::lower_bound(q.offsets, q.offsets + q.n + 1, want) - q.offsets;
+            i = std::min<uint64_t>((i + 31) & ~31ull, q.n);
+            cut[r] = std::max(i, cut[r - 1]);
+        }
+    }
+    std::vector<WorkerResult> res(P);
+    std::vector<std::thread> th;
+    for (int r = 0; r < P; ++r) {
+        const uint64_t lo = cut[r], hi = cut[r + 1];
+        if (hi <= lo) continue;
+        SketchCall shard = q;
+        shard.n = hi - lo;
+        if (q.offsets) shard.offsets += lo;
+        else shard.bases += lo * (uint64_t)q.ulen;
+        shard.out += lo * q.row_stride;
+        if (q.count) shard.count += lo;
+        if (q.status) shard.status += lo;
+        th.emplace_back([&res, &dev, r, shard] {
+            bind_thread_device(dev[r]);  // this worker's entry points run on its device
+            pg_numa_bind_thread(dev[r], nullptr);  // best effort: staging copies from the GPU's NUMA node
+            int wrc = ensure_device();
+            if (wrc == PG_OK) wrc = SketchPipe(shard).run();
+            res[r].rc = wrc;
+            if (wrc != PG_OK) res[r].msg = pg_last_error();
+        });
+    }
+    for (std::thread &t : th) t.join();
+    return fold_results(res);
+}
+
+static int index_create(const uint32_t *src, bool src_dev, uint64_t n, int32_t s, cudaStream_t st, pg_mash_index **out) {
+    if (n && s <= 0) { set_error("index over sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
+    pg_mash_index *ix = new pg_mash_index{cur_ctx()->device, nullptr, DistancePlan()};
+    const uint64_t words = n * (uint64_t)std::max(s, 0);
+    int rc = PG_OK;
+    cudaError_t e = cudaMallocAsync(&ix->d_sk, words ? words * 4 : 4, st);
+    if (e != cudaSuccess) { cudaGetLastError(); ix->d_sk = nullptr; set_error("cudaMallocAsync(%llu) for the index failed", (unsigned long long)(words * 4)); rc = PG_ERR_NOMEM; }
+    if (rc == PG_OK && words) {
+        e = cudaMemcpyAsync(ix->d_sk, src, words * 4, src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) rc = cuda_fail(e, "index copy", __FILE__, __LINE__);
+    }
+    if (rc == PG_OK) rc = distance_plan_create(ix->d_sk, n, s, st, &ix->plan);
+    if (rc == PG_OK) { e = cudaStreamSynchronize(st); if (e != cudaSuccess) rc = cuda_fail(e, "index build", __FILE__, __LINE__); }
+    if (rc != PG_OK) {
+        distance_plan_destroy(ix->plan, st);
+        if (ix->d_sk) cudaFreeAsync(ix->d_sk, st);
+        cudaStreamSynchronize(st);
+        delete ix;
+        return rc;
+    }
+    *out = ix;
+    return PG_OK;
+}
+
+}  // namespace
+}  // namespace pg
+
+using namespace pg;
+
+extern "C" {
+
+// ---------------------------------------------------------------------------------
+// mash.Sketch
+// ---------------------------------------------------------------------------------
+int pg_mash_sketch_uniform_dev(const uint8_t *d_bases, uint64_t n_reads, uint32_t read_len,
+                               int32_t k, int32_t s, uint32_t flags, uint32_t *d_out,
+                               uint64_t row_stride, int32_t *d_status, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if ((rc = check_ks(k, s)) != PG_OK) return rc;
+    if ((rc = check_dev_flags(flags)) != PG_OK) return rc;
+    if (n_reads && (!d_bases || !d_out)) { set_error("null buffer"); return PG_ERR_ARG; }
+    if ((rc = check_row_stride(row_stride, read_len, k, s, flags)) != PG_OK) return rc;
+    return launch_sketch_uniform(d_bases, n_reads, read_len, k, s, flags, d_out, row_stride,
+                                 d_status, (cudaStream_t)stream);
+}
+
+int pg_mash_sketch_batch_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_reads,
+                             uint64_t max_read_len, int32_t k, int32_t s, uint32_t flags,
+                             uint32_t *d_out, uint64_t row_stride, uint32_t *d_count,
+                             int32_t *d_status, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if ((rc = check_ks(k, s)) != PG_OK) return rc;
+    if ((rc = check_dev_flags(flags)) != PG_OK) return rc;
+    if (n_reads && (!d_offsets || !d_out)) { set_error("null buffer"); return PG_ERR_ARG; }
+    if ((rc = check_row_stride(row_stride, max_read_len, k, s, flags)) != PG_OK) return rc;
+    return launch_sketch_ragged(d_bases, d_offsets, n_reads, max_read_len, k, s, flags, d_out,
+                                row_stride, d_count, d_status, (cudaStream_t)stream);
+}
+
+int pg_mash_sketch_uniform_gather_dev(const uint8_t *d_bases, uint64_t n_local, uint32_t read_len,
+                                      int32_t k, int32_t s, void *const *gathered_ptrs,
+                                      int32_t world, int32_t rank, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    return sketch_scatter_dev(d_bases, n_local, read_len, k, s, gathered_ptrs, world, rank, (uint64_t)(rank < 0 ? 0 : rank) * n_local,
+                              (cudaStream_t)stream);
+}
+
+int pg_mash_sketch_uniform_scatter_dev(const uint8_t *d_bases, uint64_t n_local, uint32_t read_len, int32_t k, int32_t s,
+                                       void *const *dst_ptrs, int32_t n_dst, int32_t self, uint64_t row_offset, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    return sketch_scatter_dev(d_bases, n_local, read_len, k, s, dst_ptrs, n_dst, self, row_offset, (cudaStream_t)stream);
+}
+
+int pg_mash_sketch_batch(const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads, int32_t k,
+                         int32_t s, uint32_t flags, uint32_t *out, uint64_t row_stride,
+                         uint32_t *count, int32_t *status) {
+    if (n_reads && !offsets) { set_error("null offsets"); return PG_ERR_ARG; }
+    return sketch_host({bases, offsets, 0, n_reads, k, s, flags, out, row_stride, count, status});
+}
+
+int pg_mash_sketch_uniform(const uint8_t *bases, uint64_t n_reads, uint32_t read_len, int32_t k,
+                           int32_t s, uint32_t flags, uint32_t *out, uint64_t row_stride,
+                           int32_t *status) {
+    return sketch_host({bases, nullptr, read_len, n_reads, k, s, flags, out, row_stride, nullptr, status});
+}
+
+// ---------------------------------------------------------------------------------
+// Single-process multi-GPU entry points (SURVEY.md 8b "multi-GPU variants taking a device
+// count", 8e): one host thread per device, reads sharded in contiguous blocks, no data-path
+// collective for Sketch; Sketch+Distance exchanges the finished sketches by peer stores issued
+// from the sketch kernels themselves (in-process peer access, no IPC).
+// ---------------------------------------------------------------------------------
+int pg_mash_sketch_uniform_multi(const uint8_t *bases, uint64_t n_reads, uint32_t read_len, int32_t k, int32_t s,
+                                            uint32_t flags, uint32_t *out, uint64_t row_stride, int32_t *status,
+                                            const int32_t *devices, int32_t n_devices) {
+    return sketch_multi({bases, nullptr, read_len, n_reads, k, s, flags, out, row_stride, nullptr, status}, devices, n_devices);
+}
+
+int pg_mash_sketch_batch_multi(const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads, int32_t k, int32_t s,
+                                          uint32_t flags, uint32_t *out, uint64_t row_stride, uint32_t *count, int32_t *status,
+                                          const int32_t *devices, int32_t n_devices) {
+    if (n_reads && !offsets) { set_error("null offsets"); return PG_ERR_ARG; }
+    return sketch_multi({bases, offsets, 0, n_reads, k, s, flags, out, row_stride, count, status}, devices, n_devices);
+}
+
+// Sketch + all-pairs distance over several devices of this process (cfg3 / cfg4 pipeline, SURVEY 8e):
+//   1. device r takes reads [lo_r, hi_r), copies them in and runs the sketch kernel, whose finished
+//      tiles / rows are stored straight into the gathered buffer of EVERY device (peer access
+//      enabled in-process): sketching and the all-gather are one kernel;
+//   2. after a rendezvous every device holds all n sketches and computes row block r of the pair
+//      matrix (receiver = row) with the same kernels as pg_mash_distance_block.
+// Without peer access between two of the devices the exchange falls back to cudaMemcpyPeerAsync pulls.
+int pg_mash_sketch_distance_multi(const uint8_t *bases, uint64_t n_reads, uint32_t read_len, int32_t k, int32_t s,
+                                             const int32_t *devices, int32_t n_devices, uint32_t *sketches, uint32_t *same,
+                                             double *distance) {
+    int rc;
+    if ((rc = check_ks(k, s)) != PG_OK) return rc;
+    std::vector<int> dev;
+    if ((rc = resolve_devices(devices, n_devices, &dev)) != PG_OK) return rc;
+    if (n_reads == 0) return PG_OK;
+    if (!bases) { set_error("null buffer"); return PG_ERR_ARG; }
+    if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
+    const uint64_t n = n_reads, L = read_len;
+    const uint64_t cnt = sketch_words(L, k, s);
+    const int P = (int)std::min<uint64_t>(dev.size(), (n + 31) / 32);
+    dev.resize(P);
+    const std::vector<uint64_t> cut = uniform_cuts(n, P);
+    // peer access available between every pair?
+    bool fused = true;
+    for (int a = 0; a < P && fused; ++a)
+        for (int b = 0; b < P && fused; ++b) {
+            int can = 1;
+            if (a != b && cudaDeviceCanAccessPeer(&can, dev[a], dev[b]) != cudaSuccess) can = 0;
+            fused = fused && can;
+        }
+    cudaGetLastError();
+    std::vector<void *> gathered(P, nullptr);  // [n][cnt] compact rows on every device
+    std::vector<WorkerResult> res(P);
+    std::atomic<bool> failed{false};
+    Rendezvous meet(P);
+    auto worker = [&](int r) {
+        WorkerResult &my = res[r];
+        auto fail = [&](int code) { my.rc = code; my.msg = pg_last_error(); failed.store(true); };
+        auto step = [&](auto &&fn) { if (!failed.load()) { const int c = fn(); if (c != PG_OK) fail(c); } };
+        bind_thread_device(dev[r]);
+        pg_numa_bind_thread(dev[r], nullptr);
+        const uint64_t lo = cut[r], hi = cut[r + 1], nl = hi - lo;
+        uint8_t *d_reads = nullptr;
+        uint32_t *d_full = nullptr;  // [n][s] full Go arrays (== gathered when cnt == s)
+        cudaStream_t st = nullptr;
+        step([&]() -> int {
+            int c = ensure_device();
+            if (c != PG_OK) return c;
+            st = cur_ctx()->slots[0].stream;
+            if (fused)
+                for (int p = 0; p < P; ++p)
+                    if (p != r) {
+                        cudaError_t e = cudaDeviceEnablePeerAccess(dev[p], 0);
+                        if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return cuda_fail(e, "cudaDeviceEnablePeerAccess", __FILE__, __LINE__);
+                        cudaGetLastError();
+                    }
+            PG_CUDA(cudaMalloc(&gathered[r], std::max<uint64_t>(n * cnt * 4, 16)));
+            PG_CUDA(cudaMalloc(&d_reads, std::max<uint64_t>(nl * L, 16) + 64));
+            return PG_OK;
+        });
+        meet.wait();  // every buffer exists, peer access is on
+        step([&]() -> int {
+            if (nl) PG_CUDA(cudaMemcpyAsync(d_reads, bases + lo * L, nl * L, cudaMemcpyHostToDevice, st));
+            int c;
+            if (fused) {
+                c = sketch_scatter_dev(d_reads, nl, read_len, k, s, gathered.data(), P, r, lo, st);
+            } else {
+                void *own = gathered[r];
+                c = sketch_scatter_dev(d_reads, nl, read_len, k, s, &own, 1, 0, lo, st);
+            }
+            if (c != PG_OK) return c;
+            PG_CUDA(cudaStreamSynchronize(st));
+            return PG_OK;
+        });
+        meet.wait();  // all sketches computed (fused: and stored everywhere)
+        step([&]() -> int {
+            if (!fused)  // pull the other devices' row blocks
+                for (int p = 0; p < P; ++p)
+                    if (p != r && cut[p + 1] > cut[p])
+                        PG_CUDA(cudaMemcpyPeerAsync((uint32_t *)gathered[r] + cut[p] * cnt, dev[r], (uint32_t *)gathered[p] + cut[p] * cnt, dev[p],
+                                                    (cut[p + 1] - cut[p]) * cnt * 4, st));
+            if (cnt == (uint64_t)s) {
+                d_full = (uint32_t *)gathered[r];
+            } else {  // the zero tail of a fresh Mash is materialised after the exchange
+                PG_CUDA(cudaMalloc(&d_full, n * (uint64_t)s * 4));
+                PG_CUDA(cudaMemsetAsync(d_full, 0, n * (uint64_t)s * 4, st));
+                if (cnt) PG_CUDA(cudaMemcpy2DAsync(d_full, (size_t)s * 4, gathered[r], cnt * 4, cnt * 4, n, cudaMemcpyDeviceToDevice, st));
+            }
+            if (sketches && nl) PG_CUDA(cudaMemcpyAsync(sketches + lo * (uint64_t)s, d_full + lo * (uint64_t)s, nl * (uint64_t)s * 4, cudaMemcpyDeviceToHost, st));
+            if ((same || distance) && nl) {
+                DistancePlan plan;
+                int c = distance_plan_create(d_full, n, s, st, &plan);
+                if (c == PG_OK) c = plan_rows_to_host(plan, lo, hi, same ? same + lo * n : nullptr, distance ? distance + lo * n : nullptr, st);
+                distance_plan_destroy(plan, st);
+                if (c != PG_OK) return c;
+            }
+            PG_CUDA(cudaStreamSynchronize(st));
+            return PG_OK;
+        });
+        meet.wait();  // nobody reads a peer buffer any more
+        if (cur_ctx()) {
+            cudaSetDevice(dev[r]);
+            if (d_full && d_full != gathered[r]) cudaFree(d_full);
+            if (d_reads) cudaFree(d_reads);
+            if (gathered[r]) cudaFree(gathered[r]);
+            cudaGetLastError();
+        }
+    };
+    std::vector<std::thread> th;
+    for (int r = 0; r < P; ++r) th.emplace_back(worker, r);
+    for (std::thread &t : th) t.join();
+    return fold_results(res);
+}
+
+// ---------------------------------------------------------------------------------
+// Similarity / Distance
+// ---------------------------------------------------------------------------------
+int pg_mash_similarity_pairs_dev(const uint32_t *d_sketches, const uint64_t *d_sk_offsets,
+                                 uint64_t n_sketches, const uint32_t *d_pair_a,
+                                 const uint32_t *d_pair_b, uint64_t n_pairs, int64_t *d_same,
+                                 double *d_similarity, double *d_distance, int32_t *d_status,
+                                 void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    return launch_similarity_pairs(d_sketches, d_sk_offsets, n_sketches, d_pair_a, d_pair_b, n_pairs,
+                                   d_same, d_similarity, d_distance, d_status, (cudaStream_t)stream);
+}
+
+int pg_mash_similarity_pairs(const uint32_t *sketches, const uint64_t *sk_offsets,
+                             uint64_t n_sketches, const uint32_t *pair_a, const uint32_t *pair_b,
+                             uint64_t n_pairs, int64_t *same, double *similarity, double *distance,
+                             int32_t *status) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n_pairs == 0) return PG_OK;
+    if (!sk_offsets || !pair_a || !pair_b) { set_error("null buffer"); return PG_ERR_ARG; }
+    HostCall c;
+    const Ragged<uint32_t> sk = c.ragged(sketches, sk_offsets, n_sketches);
+    const uint32_t *d_a = c.upload(pair_a, n_pairs), *d_b = c.upload(pair_b, n_pairs);
+    int64_t *d_same = c.alloc<int64_t>(n_pairs);
+    double *d_sim = c.alloc<double>(n_pairs), *d_dist = c.alloc<double>(n_pairs);
+    int32_t *d_st = c.alloc<int32_t>(n_pairs, true);
+    if ((rc = c.error()) || (rc = launch_similarity_pairs(sk.base, sk.off, n_sketches, d_a, d_b, n_pairs, d_same, d_sim, d_dist, d_st, c.st)))
+        return rc;
+    std::vector<int32_t> hst(n_pairs);
+    c.download(same, d_same, n_pairs);
+    c.download(similarity, d_sim, n_pairs);
+    c.download(distance, d_dist, n_pairs);
+    c.download(hst.data(), d_st, n_pairs);
+    if ((rc = c.finish())) return rc;
+    // the pair kernel reports no unsupported items
+    return fold_item_status(hst, status, "at least one pair involves an empty sketch or an invalid index (reference panics)", nullptr);
+}
+
+int pg_mash_distance_block_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint64_t row_begin,
+                               uint64_t row_end, uint32_t *d_same, double *d_distance, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    return launch_distance_block(d_sketches, n, s, row_begin, row_end, d_same, d_distance, (cudaStream_t)stream);
+}
+
+int pg_mash_distance_block(const uint32_t *sketches, uint64_t n, int32_t s, uint64_t row_begin,
+                           uint64_t row_end, uint32_t *same, double *distance) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    if (row_end == row_begin || n == 0) return PG_OK;
+    if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
+    HostCall c;
+    const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)s);
+    if ((rc = c.error())) return rc;
+    // one plan (sortedness + join index) for the whole call
+    DistancePlan plan;
+    rc = distance_plan_create(d_sk, n, s, c.st, &plan);
+    if (rc == PG_OK) rc = plan_rows_to_host(plan, row_begin, row_end, same, distance, c.st);
+    distance_plan_destroy(plan, c.st);
+    return rc != PG_OK ? rc : c.finish();
+}
+
+int pg_mash_distance_sparse_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint64_t row_begin, uint64_t row_end, uint32_t flags,
+                                uint32_t *d_pair_i, uint32_t *d_pair_j, uint32_t *d_pair_same, uint64_t pairs_cap, uint64_t *d_n_pairs,
+                                void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    if (!d_n_pairs || (pairs_cap && (!d_pair_i || !d_pair_j || !d_pair_same))) { set_error("null buffer"); return PG_ERR_ARG; }
+    return launch_distance_sparse(d_sketches, n, s, row_begin, row_end, flags, d_pair_i, d_pair_j, d_pair_same, pairs_cap,
+                                  (unsigned long long *)d_n_pairs, (cudaStream_t)stream);
+}
+
+int pg_mash_distance_sparse(const uint32_t *sketches, uint64_t n, int32_t s, uint64_t row_begin, uint64_t row_end, uint32_t flags,
+                            uint32_t *pair_i, uint32_t *pair_j, uint32_t *pair_same, uint64_t pairs_cap, uint64_t *n_pairs) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (!n_pairs) { set_error("null buffer"); return PG_ERR_ARG; }
+    *n_pairs = 0;
+    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    if (row_end == row_begin || n == 0) return PG_OK;
+    if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
+    if (pairs_cap && (!pair_i || !pair_j || !pair_same)) { set_error("null buffer"); return PG_ERR_ARG; }
+    HostCall c;
+    const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)s);
+    uint32_t *d_i = c.alloc<uint32_t>(pairs_cap), *d_j = c.alloc<uint32_t>(pairs_cap), *d_c = c.alloc<uint32_t>(pairs_cap);
+    unsigned long long *d_n = c.alloc<unsigned long long>(1);
+    if ((rc = c.error()) || (rc = launch_distance_sparse(d_sk, n, s, row_begin, row_end, flags, d_i, d_j, d_c, pairs_cap, d_n, c.st)))
+        return rc;
+    return finish_capped(c, d_n, pairs_cap, n_pairs, {{pair_i, d_i, 4}, {pair_j, d_j, 4}, {pair_same, d_c, 4}}, "pairs_cap", "pairs");
+}
+
+// ---------------------------------------------------------------------------------
+// Sketch index: top-k nearest references
+// ---------------------------------------------------------------------------------
+int pg_mash_index_create(const uint32_t *sketches, uint64_t n, int32_t s, pg_mash_index **out) {
+    if (!out) { set_error("null index pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n && s > 0 && !sketches) { set_error("null buffer"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+    return index_create(sketches, false, n, s, cur_ctx()->slots[0].stream, out);
+}
+
+int pg_mash_index_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, void *stream, pg_mash_index **out) {
+    if (!out) { set_error("null index pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n && s > 0 && !d_sketches) { set_error("null buffer"); return PG_ERR_ARG; }
+    return index_create(d_sketches, true, n, s, (cudaStream_t)stream, out);
+}
+
+int pg_mash_index_query_dev(const pg_mash_index *ix, const uint32_t *d_queries, uint64_t nq, int32_t sq, uint32_t top_k,
+                            uint32_t min_same, uint32_t *d_hit_ref, uint32_t *d_hit_same, double *d_hit_distance,
+                            uint32_t *d_n_hits, void *stream) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    return launch_index_query(ix->plan, d_queries, nq, sq, top_k, min_same, d_hit_ref, d_hit_same, d_hit_distance, d_n_hits,
+                              (cudaStream_t)stream);
+}
+
+int pg_mash_index_query(const pg_mash_index *ix, const uint32_t *queries, uint64_t nq, int32_t sq, uint32_t top_k,
+                        uint32_t min_same, uint32_t *hit_ref, uint32_t *hit_same, double *hit_distance, uint32_t *n_hits) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    if (top_k == 0 || top_k > PG_INDEX_MAX_TOP_K) { set_error("top_k %u outside [1, %u]", top_k, PG_INDEX_MAX_TOP_K); return PG_ERR_ARG; }
+    if (nq == 0) return PG_OK;
+    if (sq <= 0) { set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq); return PG_ERR_PANIC; }
+    if (!queries) { set_error("null buffer"); return PG_ERR_ARG; }
+    HostCall c;
+    const uint64_t slots = nq * (uint64_t)top_k;
+    const uint32_t *d_q = c.upload(queries, nq * (uint64_t)sq);
+    uint32_t *d_ref = hit_ref ? c.alloc<uint32_t>(slots) : nullptr, *d_same = hit_same ? c.alloc<uint32_t>(slots) : nullptr;
+    double *d_dist = hit_distance ? c.alloc<double>(slots) : nullptr;
+    uint32_t *d_nh = n_hits ? c.alloc<uint32_t>(nq) : nullptr;
+    if ((rc = c.error()) || (rc = launch_index_query(ix->plan, d_q, nq, sq, top_k, min_same, d_ref, d_same, d_dist, d_nh, c.st))) return rc;
+    c.download(hit_ref, d_ref, slots);
+    c.download(hit_same, d_same, slots);
+    c.download(hit_distance, d_dist, slots);
+    c.download(n_hits, d_nh, nq);
+    return c.finish();
+}
+
+int pg_mash_index_free(pg_mash_index *ix) {
+    if (!ix) return PG_OK;
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+    cudaStream_t st = cur_ctx()->slots[0].stream;
+    distance_plan_destroy(ix->plan, st);
+    if (ix->d_sk) cudaFreeAsync(ix->d_sk, st);
+    delete ix;
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
+}
+
+}  // extern "C"

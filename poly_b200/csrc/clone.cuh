@@ -1,4 +1,4 @@
-// clone.cuh -- internal types of the clone digest and ligation (clone.cu, clone_host.cpp, api.cu)
+// clone.cuh -- internal types of the clone digest and ligation (clone.cu, clone_host.cpp, api_clone.cu)
 #pragma once
 #include <string>
 #include <vector>

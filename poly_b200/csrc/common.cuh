@@ -10,7 +10,7 @@
 
 namespace pg {
 
-// thread-local error string + helpers (api.cu)
+// thread-local error string + helpers (runtime.cu)
 void set_error(const char *fmt, ...);
 int cuda_fail(cudaError_t e, const char *what, const char *file, int line);
 void note_launch(const char *kernel_name);
@@ -29,7 +29,7 @@ void note_launch(const char *kernel_name);
     } while (0)
 
 int sm_count();
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) cached per (device, kernel); thread-safe (api.cu)
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) cached per (device, kernel); thread-safe (runtime.cu)
 int func_smem(const void *kernel, size_t bytes);
 
 // transform.complementTable (transform.go:78-109): every unlisted byte maps to 0, including the DNA
@@ -52,23 +52,23 @@ __host__ __device__ __forceinline__ uint8_t complement(uint8_t c) {
 // returns of PG_CUDA -- with cudaFreeAsync on the stream they were allocated on.
 struct StreamScratch {
     cudaStream_t st;
-    void *ptr[24];
-    int n = 0;
+    std::vector<void *> ptr;
     explicit StreamScratch(cudaStream_t s) : st(s) {}
     StreamScratch(const StreamScratch &) = delete;
     StreamScratch &operator=(const StreamScratch &) = delete;
     ~StreamScratch() {
-        for (int i = 0; i < n; ++i) cudaFreeAsync(ptr[i], st);
+        for (void *p : ptr) cudaFreeAsync(p, st);
     }
     template <typename T>
     cudaError_t alloc(T **p, uint64_t count) {  // at least one element, so the pointer is always valid
-        if (n >= 24) return cudaErrorMemoryAllocation;
-        cudaError_t e = cudaMallocAsync((void **)p, (count ? count : 1) * sizeof(T), st);
-        if (e == cudaSuccess) ptr[n++] = *p;
+        ptr.push_back(nullptr);  // the slot first, so that keeping the buffer cannot throw and leak it
+        cudaError_t e = cudaMallocAsync(&ptr.back(), (count ? count : 1) * sizeof(T), st);
+        if (e != cudaSuccess) ptr.pop_back();
+        else *p = (T *)ptr.back();
         return e;
     }
     void adopt(void *p) {  // take ownership of a buffer allocated elsewhere on the same stream
-        if (p && n < 24) ptr[n++] = p;
+        if (p) ptr.push_back(p);
     }
 };
 

@@ -237,7 +237,7 @@ int launch_distance_sparse(const uint32_t *d_sk, uint64_t n, int s, uint64_t row
     DistancePlan plan;
     int rc = distance_plan_create(d_sk, n, s, st, &plan);
     // tiles of <= 8 GiB: every pass over the index costs one read of all its entries and the run tables of every
-    // bucket, but a tile that outgrows the memory pool's cache (12 GiB, api.cu) is mapped and unmapped by the
+    // bucket, but a tile that outgrows the memory pool's cache (12 GiB, runtime.cu) is mapped and unmapped by the
     // driver on every call
     const uint64_t budget_words = 2ull << 30;
     const uint64_t rows_per = std::max<uint64_t>(8, std::min<uint64_t>(row_end - row_begin, (budget_words / n) & ~7ull));

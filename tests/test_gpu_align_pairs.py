@@ -142,6 +142,33 @@ def test_pair_list_shapes(gpu, oracle):
     assert [len(x) for x in align.pair_scores_arrays(A, B, np.zeros((0, 2), np.int64), scoring())] == [0, 0, 0]
 
 
+def test_pair_groups_match_one_group(gpu, monkeypatch):
+    """A small group budget cuts one call into many pair groups; every output matches the one-group call."""
+    rng = np.random.default_rng(13)
+    A = rand_seqs(rng, rng.integers(0, 200, 60))
+    B = rand_seqs(rng, rng.integers(0, 200, 40))
+    A[3], B[5] = b"ACXGT", b"GGTXA"  # errors, with their positions, in several groups
+    pairs = np.stack([rng.integers(0, len(A), 2000), rng.integers(0, len(B), 2000)], 1)
+
+    def run():
+        before = _lib.lib().pg_launch_count()
+        out = ([align.pair_scores_arrays(A, B, pairs, scoring(-2), g) for g in (False, True)],
+               align.SmithWatermanPairAligns(A, B, pairs, scoring(-2)), align.NeedlemanWunschPairAligns(A, B, pairs, scoring(-2)))
+        return out, _lib.lib().pg_launch_count() - before
+
+    def key(aligns):  # errors compare by their text
+        return [(s, a, b, str(e)) for s, a, b, e in aligns]
+
+    (scores, sw, nw), launches = run()
+    monkeypatch.setenv("PG_GROUP_BYTES", str(8_000))  # about 240 pairs per score group, 9 per string group
+    (g_scores, g_sw, g_nw), g_launches = run()
+    assert g_launches > launches
+    for w, x in zip(scores, g_scores):
+        for a, b in zip(w, x):
+            assert np.array_equal(a, b)
+    assert key(g_sw) == key(sw) and key(g_nw) == key(nw)
+
+
 def test_host_out_of_range_index_writes_nothing(gpu):
     A, B = [b"ACGT", b"GG"], [b"ACG"]
     ba, oa = flatten(A)

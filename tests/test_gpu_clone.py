@@ -114,17 +114,17 @@ def test_golden_gate_combinatorial_library(clone):
     _, wc, wl = co.golden_gate(parts, "BsaI")
     assert len(wc) == want == 4096
     bsai = clone.GetBaseRestrictionEnzymes()[0]
-    old = os.environ.get("PG_CLONE_GROUP_BYTES")
+    old = os.environ.get("PG_GROUP_BYTES")
     for budget in (None, str(3 << 20)):  # one group, then many groups across the emits
         if budget:
-            os.environ["PG_CLONE_GROUP_BYTES"] = budget
+            os.environ["PG_GROUP_BYTES"] = budget
         try:
             (clones, loops, cd, ld), = clone.GoldenGateBatch([gg_parts(clone, parts)], bsai, digests=True)
         finally:
             if old is None:
-                os.environ.pop("PG_CLONE_GROUP_BYTES", None)
+                os.environ.pop("PG_GROUP_BYTES", None)
             else:
-                os.environ["PG_CLONE_GROUP_BYTES"] = old
+                os.environ["PG_GROUP_BYTES"] = old
         assert [c.encode() for c in clones] == wc and [l.encode() for l in loops] == wl
         for k in range(0, len(clones), 97):
             assert seqhash_oracle.seqhash(wc[k], "DNA", True, True)[1] == cd[k]

@@ -182,5 +182,5 @@ def test_several_groups(monkeypatch):
     rnd = random.Random(11)
     seqs = ["".join(rnd.choice("ACGT") for _ in range(rnd.randint(20, 60))) for _ in range(64)] + ["", "ACGN"]
     rnd.shuffle(seqs)
-    monkeypatch.setenv("PG_FOLD_GROUP_BYTES", str(300_000))  # a few items per group
+    monkeypatch.setenv("PG_GROUP_BYTES", str(300_000))  # a few items per group
     check(seqs)

@@ -137,7 +137,7 @@ def test_empty_batch_and_capacity():
 
 
 def test_several_groups(monkeypatch):
-    monkeypatch.setenv("PG_FRAGMENT_GROUP_BYTES", str(40_000))
+    monkeypatch.setenv("PG_GROUP_BYTES", str(40_000))
     check(seeded_genes(120, 7), 40, 60, ["AAAA"])
 
 

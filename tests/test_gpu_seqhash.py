@@ -180,7 +180,7 @@ def test_forced_small_groups(gpu, monkeypatch):
     seqs = [s.encode() for s in _random_batch(rng, "ACGTZ", 200, 6000)] + [b"ACGT" * 5000]
     flat, off, _ = seqhash._flatten(seqs)
     base = [seqhash.hash_arrays(flat, off, "DNA", c, d) for c, d in FLAGS]
-    monkeypatch.setenv("PG_SEQHASH_GROUP_BYTES", "4096")
+    monkeypatch.setenv("PG_GROUP_BYTES", "4096")
     for (c, d), (dig, code, pos) in zip(FLAGS, base):
         g_dig, g_code, g_pos = seqhash.hash_arrays(flat, off, "DNA", c, d)
         assert np.array_equal(g_dig, dig) and np.array_equal(g_code, code) and np.array_equal(g_pos, pos)
