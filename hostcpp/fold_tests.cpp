@@ -1,7 +1,7 @@
 // fold_tests.cpp -- fold_test.go, seqfold_test.go and example_test.go (fold/) restated against the C++ host
 // mirror, plus exact parity with the C restatement on a fixture list.
 // Usage: fold_tests EXPECTED.tsv -- one "sequence<TAB>temp<TAB>status<TAB>mfe as %a<TAB>dot-bracket" line per
-// item, written by tests/test_gpu_fold.py from tests/fold_oracle.c.  Prints "fold_tests: all passed" when every
+// item, written by tests/test_gpu_fold.py from oracle/fold_oracle.c.  Prints "fold_tests: all passed" when every
 // check holds.
 #include <cmath>
 #include <cstdio>

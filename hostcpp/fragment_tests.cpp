@@ -1,6 +1,6 @@
 // fragment_tests.cpp -- fragment_test.go and example_test.go (synthesis/fragment/) restated against the C++ host
 // mirror, plus exact parity with the C restatement on a fixture list.
-// Usage: fragment_tests EXPECTED.tsv -- written by tests/test_gpu_fragment.py from tests/fragment_oracle.c and
+// Usage: fragment_tests EXPECTED.tsv -- written by tests/test_gpu_fragment.py from oracle/fragment_oracle.c and
 // tests/golden/fragment/pins.json.  Lines:
 //   F <name> seq min max excludes includes status efficiency(%a) fragments error     (lists joined with ',')
 //   S set efficiency(%a)

@@ -1,5 +1,5 @@
 /*
- * oracle/poly_oracle.h -- CPU restatement of the bebop/poly hot path.
+ * oracle/poly_oracle.h -- CPU restatement of the bebop/poly hot path: every function liboracle.so exports.
  *
  * TEST INFRASTRUCTURE ONLY.  Nothing under oracle/ is part of the product: it
  * may be imported/linked/executed only by tests/, __graft_entry__.smoke() and
@@ -28,6 +28,7 @@ extern "C" {
 #define PO_OK 0
 #define PO_PANIC (-1)       /* the Go reference would panic on this input        */
 #define PO_UNSUPPORTED (-2) /* outside the restated domain (non-ASCII ToUpper)   */
+#define PO_NOMEM (-100)     /* a batch driver could not allocate its worker pool */
 
 /* github.com/spaolacci/murmur3 v1.1.0 Sum32WithSeed == MurmurHash3_x86_32. */
 uint32_t po_murmur3_32(const uint8_t *data, size_t len, uint32_t seed);
@@ -111,6 +112,53 @@ int po_sw_score_batch(const uint8_t *queries, const uint64_t *offsets, uint64_t 
 int po_melting_temp_batch(const uint8_t *bases, const uint64_t *offsets, uint64_t n, int nthreads, double *tm, uint64_t *checksum);
 int po_mash_similarity_block(const uint32_t *sk, uint64_t n, int s, uint64_t row_lo, uint64_t row_hi, uint64_t col_lo,
                              uint64_t col_hi, int nthreads, uint32_t *same, uint64_t *checksum);
+
+/* ---- seqhash_oracle.c: seqhash/seqhash.go:78-223 and BLAKE3 (hash mode, 32-byte output) */
+void po_blake3(const uint8_t *in, uint64_t len, uint8_t out[32]);
+int64_t po_booth_least_rotation(const uint8_t *seq, int64_t n);
+void po_rotate_sequence(const uint8_t *seq, int64_t n, uint8_t *out);
+int po_seqhash(const uint8_t *seq, int64_t n, int seq_type, int circular, int double_stranded, uint8_t digest[32], int64_t *err_pos);
+int po_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, int seq_type, int circular, int double_stranded,
+                     int nthreads, uint8_t *digest, int32_t *err_code, int64_t *err_pos);
+
+/* ---- pair_oracle.c: po_sw_score / po_nw_score over a list of (a, b) index pairs */
+int po_pair_scores(int global, const uint8_t *a, const uint64_t *off_a, const uint8_t *b, const uint64_t *off_b, const uint32_t *pair_a,
+                   const uint32_t *pair_b, uint64_t n, const int16_t *lut_a, const int16_t *lut_b, const int64_t *table, int n_b,
+                   int64_t gap, int nthreads, int64_t *score, int32_t *err_code, int64_t *err_pos);
+
+/* ---- clone_oracle.c: clone/clone.go:138-355 (CutWithEnzyme, CircularLigate) */
+void co_free(void *p);
+int co_cut(const uint8_t *part, int64_t L, int circular, int directional, const uint8_t *fsite, int64_t fl, const uint8_t *rsite,
+           int64_t rl, const uint8_t *recog, int64_t recl, int64_t skip, int64_t ohl, uint8_t **out, uint64_t *out_bytes, int64_t *n_frag);
+int co_cut_batch(const uint8_t *parts, const uint64_t *offsets, const uint8_t *circular, uint64_t n_parts, const uint8_t *const *sites,
+                 const int64_t *site_lens, const int64_t *skip_ohl, int n_enz, int directional, int nthreads, int64_t *n_frag, int32_t *status);
+void co_circular_ligate(const uint8_t *frags, int64_t n, uint8_t **clones, uint64_t *clone_bytes, int64_t *n_clones, uint8_t **loops,
+                        uint64_t *loop_bytes, int64_t *n_loops);
+
+/* ---- fold_oracle.c: fold.go and seqfold.go (Zuker) */
+void fo_set_table(int kind, int t, int count, const char *keys, const double *h, const double *s);
+void fo_set_multibranch(int kind, const double *mb);
+int fo_fold(const char *raw, int64_t n, double temp, double *mfe, char *db, int64_t *db_len, char **structs);
+int fo_probe(const char *raw, int64_t n, double temp, int which, int a, int b, int cc, int d, double *out);
+void fo_pair(const char *s, int a, int b, int c, int d, char *out);
+void fo_free(void *p);
+int fo_fold_batch(const uint8_t *seqs, const uint64_t *off, uint64_t n, double temp, double *mfe, uint8_t *db, uint64_t *db_len,
+                  int32_t *status, int threads);
+
+/* ---- fragment_oracle.c: synthesis/fragment/fragment.go */
+void fr_set_table(const uint8_t *keys, const int32_t *counts);
+double fr_set_efficiency(const uint8_t *bytes, const uint64_t *off, uint64_t n);
+int fr_next_overhangs(const uint8_t *bytes, const uint64_t *off, uint64_t n, uint8_t *cands, double *eff);
+int fr_fragment(const uint8_t *seq_in, int64_t len_in, int64_t minFragmentSize, int64_t maxFragmentSize, const uint8_t *ex,
+                const uint64_t *ex_off, uint64_t n_ex, const uint8_t *inc, const uint64_t *inc_off, uint64_t n_inc, double *eff,
+                int64_t *err_min, int64_t *err_max, uint64_t *ends, uint64_t *n_ends);
+int fr_fragment_batch(const uint8_t *seqs, const uint64_t *off, uint64_t n, int64_t min, int64_t max, const uint8_t *ex,
+                      const uint64_t *ex_off, uint64_t n_ex, const uint8_t *inc, const uint64_t *inc_off, uint64_t n_inc, int32_t *status,
+                      double *eff, int64_t *err_min, int64_t *err_max, uint64_t *ends, const uint64_t *ends_off, uint64_t *n_ends,
+                      int threads);
+int fr_set_efficiency_batch(const uint8_t *bytes, const uint64_t *off, const uint64_t *set_off, uint64_t n_sets, double *eff, int threads);
+int fr_next_overhangs_batch(const uint8_t *bytes, const uint64_t *off, const uint64_t *set_off, uint64_t n_sets, uint8_t *cands,
+                            uint32_t *n_cands, double *eff, int threads);
 
 #ifdef __cplusplus
 }

@@ -3,23 +3,17 @@
  * (hash mode, 32-byte output, written from the BLAKE3 specification).
  *
  * TEST INFRASTRUCTURE ONLY (as everything under oracle/): the checker of the CUDA seqhash path and the
- * timed CPU arm of tools/bench_seqhash.py ("C restatement, not Go").  Built on its own into
- * oracle/libseqhash_oracle.so and loaded by tests/seqhash_oracle.py.
+ * timed CPU arm of tools/bench_seqhash.py ("C restatement, not Go").  Loaded by tests/seqhash_oracle.py.
  *
  * Non-ASCII input: the first byte that is >= 0x80 or outside the alphabet decides, as the library
  * does (DESIGN.md §7): a byte >= 0x80 there is reported as unsupported (3), not hashed.
  */
-#include <pthread.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
 
-void po_blake3(const uint8_t *in, uint64_t len, uint8_t out[32]);
-int64_t po_booth_least_rotation(const uint8_t *seq, int64_t n);
-void po_rotate_sequence(const uint8_t *seq, int64_t n, uint8_t *out);
-int po_seqhash(const uint8_t *seq, int64_t n, int seq_type, int circular, int double_stranded, uint8_t digest[32], int64_t *err_pos);
-void po_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, int seq_type, int circular, int double_stranded,
-                      int nthreads, uint8_t *digest, int32_t *err_code, int64_t *err_pos);
+#include "parallel.h"
+#include "poly_oracle.h"
 
 /* ---- BLAKE3 ------------------------------------------------------------------------------------ */
 #define B3_CHUNK_START 1u
@@ -217,34 +211,24 @@ int po_seqhash(const uint8_t *seq, int64_t n, int seq_type, int circular, int do
 typedef struct {
     const uint8_t *seqs;
     const uint64_t *offsets;
-    uint64_t n, next;
     int seq_type, circular, ds;
     uint8_t *digest;
     int32_t *err_code;
     int64_t *err_pos;
 } sh_batch;
 
-static void *sh_worker(void *arg) {
+static void sh_one(void *arg, uint64_t i) {
     sh_batch *b = arg;
-    for (;;) {
-        uint64_t i = __atomic_fetch_add(&b->next, 1, __ATOMIC_RELAXED);
-        if (i >= b->n) return NULL;
-        int64_t pos = 0;
-        int code = po_seqhash(b->seqs + b->offsets[i], (int64_t)(b->offsets[i + 1] - b->offsets[i]), b->seq_type, b->circular, b->ds,
-                              b->digest + 32 * i, &pos);
-        if (code) memset(b->digest + 32 * i, 0, 32);
-        b->err_code[i] = code;
-        b->err_pos[i] = pos;
-    }
+    int64_t pos = 0;
+    int code = po_seqhash(b->seqs + b->offsets[i], (int64_t)(b->offsets[i + 1] - b->offsets[i]), b->seq_type, b->circular, b->ds,
+                          b->digest + 32 * i, &pos);
+    if (code) memset(b->digest + 32 * i, 0, 32);
+    b->err_code[i] = code;
+    b->err_pos[i] = pos;
 }
 
-void po_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, int seq_type, int circular, int double_stranded,
-                      int nthreads, uint8_t *digest, int32_t *err_code, int64_t *err_pos) {
-    sh_batch b = {seqs, offsets, n, 0, seq_type, circular, double_stranded, digest, err_code, err_pos};
-    if (nthreads < 1) nthreads = 1;
-    pthread_t *th = malloc(sizeof(pthread_t) * (size_t)nthreads);
-    for (int t = 1; t < nthreads; t++) pthread_create(&th[t], NULL, sh_worker, &b);
-    sh_worker(&b);
-    for (int t = 1; t < nthreads; t++) pthread_join(th[t], NULL);
-    free(th);
+int po_seqhash_batch(const uint8_t *seqs, const uint64_t *offsets, uint64_t n, int seq_type, int circular, int double_stranded,
+                     int nthreads, uint8_t *digest, int32_t *err_code, int64_t *err_pos) {
+    sh_batch b = {seqs, offsets, seq_type, circular, double_stranded, digest, err_code, err_pos};
+    return po_parallel_for(n, nthreads, 1, sh_one, &b);
 }

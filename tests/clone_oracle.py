@@ -1,23 +1,29 @@
-"""ctypes binding of tests/clone_oracle.c, the CPU restatement of clone.go (CutWithEnzyme, CircularLigate,
-GoldenGate), and a Python restatement of the deferred-hash ligation that libpolyb200 runs (DESIGN.md "Clone").
+"""ctypes binding of oracle/clone_oracle.c, the CPU restatement of clone.go (CutWithEnzyme, CircularLigate,
+GoldenGate), in oracle/liboracle.so, and a Python restatement of the deferred-hash ligation that libpolyb200
+runs (DESIGN.md "Clone").
 
-TEST INFRASTRUCTURE ONLY (tests/ and tools/bench_clone.py).  The C file is compiled on first use into a
-temporary directory and linked against oracle/libseqhash_oracle.so, so nothing is written into the tree."""
+TEST INFRASTRUCTURE ONLY (tests/ and tools/bench_clone.py)."""
 from __future__ import annotations
 
 import ctypes as C
-import os
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 
+import oracle_ffi
 import seqhash_oracle
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 OK, PANIC, UNSUPPORTED = 0, 1, 2
+_vpp, _u64p, _i64p = C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_int64)
+SIGS = {
+    "co_free": (None, [C.c_void_p]),
+    "co_cut": (C.c_int, [C.c_char_p, C.c_int64, C.c_int, C.c_int, C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_char_p, C.c_int64,
+                         C.c_int64, C.c_int64, _vpp, _u64p, _i64p]),
+    "co_cut_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                               C.c_int, C.c_void_p, C.c_void_p]),
+    "co_circular_ligate": (None, [C.c_char_p, C.c_int64, _vpp, _u64p, _i64p, _vpp, _u64p, _i64p]),
+}
 
 # clone.GetBaseRestrictionEnzymes (clone.go:358-364): name -> (forward site, reverse site, skip, overhang length,
 # recognition site)
@@ -31,24 +37,7 @@ BASE_ENZYMES = {
 def lib():
     global _LIB
     if _LIB is None:
-        so = seqhash_oracle.build()
-        seqhash_oracle.lib()  # resolves po_seqhash for the clone oracle
-        out = os.path.join(tempfile.mkdtemp(prefix="clone_oracle_"), "libclone_oracle.so")
-        subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-pthread", "-Wall", os.path.join(_HERE, "clone_oracle.c"), so,
-                               "-Wl,-rpath," + os.path.dirname(so), "-o", out])
-        L = C.CDLL(out)
-        L.co_free.restype = None
-        L.co_free.argtypes = [C.c_void_p]
-        L.co_cut.restype = C.c_int
-        L.co_cut.argtypes = [C.c_char_p, C.c_int64, C.c_int, C.c_int, C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_char_p, C.c_int64,
-                             C.c_int64, C.c_int64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_int64)]
-        L.co_cut_batch.restype = None
-        L.co_cut_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
-                                   C.c_int, C.c_void_p, C.c_void_p]
-        L.co_circular_ligate.restype = None
-        L.co_circular_ligate.argtypes = [C.c_char_p, C.c_int64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_int64),
-                                         C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_int64)]
-        _LIB = L
+        _LIB = oracle_ffi.bind(SIGS)
     return _LIB
 
 
@@ -93,8 +82,9 @@ def cut_counts(parts: np.ndarray, offsets: np.ndarray, circular: np.ndarray, enz
     parts = np.ascontiguousarray(parts, np.uint8)
     offsets = np.ascontiguousarray(offsets, np.uint64)
     circ = np.ascontiguousarray(circular, np.uint8)
-    lib().co_cut_batch(parts.ctypes.data, offsets.ctypes.data, circ.ctypes.data, len(offsets) - 1, sites, lens.ctypes.data, so.ctypes.data,
-                       len(enz), int(directional), nthreads, nfrag.ctypes.data, status.ctypes.data)
+    rc = lib().co_cut_batch(parts.ctypes.data, offsets.ctypes.data, circ.ctypes.data, len(offsets) - 1, sites, lens.ctypes.data,
+                            so.ctypes.data, len(enz), int(directional), nthreads, nfrag.ctypes.data, status.ctypes.data)
+    assert rc == oracle_ffi.PO_OK, rc
     return nfrag, status
 
 

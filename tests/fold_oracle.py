@@ -1,23 +1,32 @@
-"""ctypes binding of tests/fold_oracle.c, the CPU restatement of poly's fold package (Zuker).
+"""ctypes binding of oracle/fold_oracle.c, the CPU restatement of poly's fold package (Zuker), in
+oracle/liboracle.so.
 
-TEST INFRASTRUCTURE ONLY (tests/ and tools/bench_fold.py).  The C file is compiled on first use into a
-temporary directory, so nothing is written into the tree.  Its energy tables are read from
-tests/golden/fold/energies.json."""
+TEST INFRASTRUCTURE ONLY (tests/ and tools/bench_fold.py).  Its energy tables are read from
+tests/golden/fold/energies.json and handed to the library on first use."""
 from __future__ import annotations
 
 import ctypes as C
 import json
 import os
-import subprocess
-import tempfile
 
 import numpy as np
+
+import oracle_ffi
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 ENERGIES = os.path.join(_HERE, "golden", "fold", "energies.json")
 OK, PANIC, UNSUPPORTED, NOT_NUCLEIC, INTERNAL = 0, 1, 2, 3, 4
 TABLES = ("nearestNeighbors", "internalMismatches", "terminalMismatches", "danglingEnds", "triTetraLoops", "internalLoops", "bulgeLoops",
           "hairpinLoops")
+SIGS = {
+    "fo_set_table": (None, [C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_void_p, C.c_void_p]),
+    "fo_set_multibranch": (None, [C.c_int, C.c_void_p]),
+    "fo_fold": (C.c_int, [C.c_char_p, C.c_int64, C.c_double, C.POINTER(C.c_double), C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_void_p)]),
+    "fo_probe": (C.c_int, [C.c_char_p, C.c_int64, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double)]),
+    "fo_pair": (None, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_char_p]),
+    "fo_free": (None, [C.c_void_p]),
+    "fo_fold_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+}
 _LIB = None
 
 
@@ -29,25 +38,7 @@ def energies() -> dict:
 def lib():
     global _LIB
     if _LIB is None:
-        out = os.path.join(tempfile.mkdtemp(prefix="fold_oracle_"), "libfold_oracle.so")
-        subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-Wall",
-                               os.path.join(_HERE, "fold_oracle.c"), "-o", out, "-lm"])
-        L = C.CDLL(out)
-        L.fo_set_table.restype = None
-        L.fo_set_table.argtypes = [C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_void_p, C.c_void_p]
-        L.fo_set_multibranch.restype = None
-        L.fo_set_multibranch.argtypes = [C.c_int, C.c_void_p]
-        L.fo_fold.restype = C.c_int
-        L.fo_fold.argtypes = [C.c_char_p, C.c_int64, C.c_double, C.POINTER(C.c_double), C.c_char_p, C.POINTER(C.c_int64),
-                              C.POINTER(C.c_void_p)]
-        L.fo_probe.restype = C.c_int
-        L.fo_probe.argtypes = [C.c_char_p, C.c_int64, C.c_double, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double)]
-        L.fo_pair.restype = None
-        L.fo_pair.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_char_p]
-        L.fo_free.restype = None
-        L.fo_free.argtypes = [C.c_void_p]
-        L.fo_fold_batch.restype = None
-        L.fo_fold_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+        L = oracle_ffi.bind(SIGS)
         tabs = energies()
         for kind, name in enumerate(("dna", "rna")):
             t = tabs[name]
@@ -100,14 +91,13 @@ def pair(seq: bytes, a: int, b: int, c: int, d: int) -> str:
 
 def fold_batch(seqs, temp: float, threads: int = 16):
     """(mfe float64[n], dot-brackets [bytes], status int32[n]) over `threads` host threads."""
-    raw = [bytes(s) for s in seqs]
-    off = np.zeros(len(raw) + 1, dtype=np.uint64)
-    np.cumsum([len(r) for r in raw], out=off[1:])
-    flat = np.frombuffer(b"".join(raw) or b"\0", dtype=np.uint8)
-    mfe = np.zeros(max(len(raw), 1), dtype=np.float64)
+    flat, off = oracle_ffi.ragged(seqs)
+    n = len(off) - 1
+    mfe = np.zeros(max(n, 1), dtype=np.float64)
     db = np.zeros(max(int(off[-1]), 1), dtype=np.uint8)
-    dbl = np.zeros(max(len(raw), 1), dtype=np.uint64)
-    st = np.zeros(max(len(raw), 1), dtype=np.int32)
-    lib().fo_fold_batch(flat.ctypes.data, off.ctypes.data, len(raw), temp, mfe.ctypes.data, db.ctypes.data, dbl.ctypes.data, st.ctypes.data, threads)
-    dbs = [db[int(off[i]): int(off[i]) + int(dbl[i])].tobytes() for i in range(len(raw))]
-    return mfe[: len(raw)], dbs, st[: len(raw)]
+    dbl = np.zeros(max(n, 1), dtype=np.uint64)
+    st = np.zeros(max(n, 1), dtype=np.int32)
+    rc = lib().fo_fold_batch(flat.ctypes.data, off.ctypes.data, n, temp, mfe.ctypes.data, db.ctypes.data, dbl.ctypes.data, st.ctypes.data, threads)
+    assert rc == oracle_ffi.PO_OK, rc
+    dbs = [db[int(off[i]): int(off[i]) + int(dbl[i])].tobytes() for i in range(n)]
+    return mfe[:n], dbs, st[:n]

@@ -1,22 +1,33 @@
-"""ctypes binding of tests/fragment_oracle.c, the CPU restatement of poly's synthesis/fragment.
+"""ctypes binding of oracle/fragment_oracle.c, the CPU restatement of poly's synthesis/fragment, in
+oracle/liboracle.so.
 
-TEST INFRASTRUCTURE ONLY (tests/, smoke() and tools/bench_fragment.py).  The C file is compiled on first
-use into a temporary directory, so nothing is written into the tree.  Its fidelity table is read from
-tests/golden/fragment/ligation_fidelity.json."""
+TEST INFRASTRUCTURE ONLY (tests/, smoke() and tools/bench_fragment.py).  Its fidelity table is read from
+tests/golden/fragment/ligation_fidelity.json and handed to the library on first use."""
 from __future__ import annotations
 
 import ctypes as C
 import json
 import os
-import subprocess
-import tempfile
 
 import numpy as np
+
+import oracle_ffi
+from oracle_ffi import ragged
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 FIDELITY = os.path.join(_HERE, "golden", "fragment", "ligation_fidelity.json")
 PINS = os.path.join(_HERE, "golden", "fragment", "pins.json")
 OK, PANIC, UNSUPPORTED, MIN_GT_MAX, MIN_LT_12, NO_POSITION = 0, 1, 2, 3, 4, 5
+_vp, _u64, _i64 = C.c_void_p, C.c_uint64, C.c_int64
+SIGS = {
+    "fr_set_table": (None, [_vp, _vp]),
+    "fr_set_efficiency": (C.c_double, [_vp, _vp, _u64]),
+    "fr_next_overhangs": (C.c_int, [_vp, _vp, _u64, _vp, _vp]),
+    "fr_fragment": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp]),
+    "fr_fragment_batch": (C.c_int, [_vp, _vp, _u64, _i64, _i64, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int]),
+    "fr_set_efficiency_batch": (C.c_int, [_vp, _vp, _vp, _u64, _vp, C.c_int]),
+    "fr_next_overhangs_batch": (C.c_int, [_vp, _vp, _vp, _u64, _vp, _vp, _vp, C.c_int]),
+}
 _LIB = None
 
 
@@ -33,39 +44,13 @@ def pins() -> dict:
 def lib():
     global _LIB
     if _LIB is None:
-        out = os.path.join(tempfile.mkdtemp(prefix="fragment_oracle_"), "libfragment_oracle.so")
-        subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-Wall",
-                               os.path.join(_HERE, "fragment_oracle.c"), "-o", out])
-        L = C.CDLL(out)
-        vp, u64, i64 = C.c_void_p, C.c_uint64, C.c_int64
-        L.fr_set_table.restype = None
-        L.fr_set_table.argtypes = [vp, vp]
-        L.fr_set_efficiency.restype = C.c_double
-        L.fr_set_efficiency.argtypes = [vp, vp, u64]
-        L.fr_next_overhangs.restype = C.c_int
-        L.fr_next_overhangs.argtypes = [vp, vp, u64, vp, vp]
-        L.fr_fragment.restype = C.c_int
-        L.fr_fragment.argtypes = [vp, i64, i64, i64, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp]
-        L.fr_fragment_batch.restype = None
-        L.fr_fragment_batch.argtypes = [vp, vp, u64, i64, i64, vp, vp, u64, vp, vp, u64, vp, vp, vp, vp, vp, vp, vp, C.c_int]
-        L.fr_set_efficiency_batch.restype = None
-        L.fr_set_efficiency_batch.argtypes = [vp, vp, vp, u64, vp, C.c_int]
-        L.fr_next_overhangs_batch.restype = None
-        L.fr_next_overhangs_batch.argtypes = [vp, vp, vp, u64, vp, vp, vp, C.c_int]
+        L = oracle_ffi.bind(SIGS)
         t = fidelity()
         keys = np.frombuffer("".join(t["keys"]).encode(), dtype=np.uint8).copy()
         counts = np.array(t["counts"], dtype=np.int32)
         L.fr_set_table(keys.ctypes.data, counts.ctypes.data)
         _LIB = L
     return _LIB
-
-
-def ragged(items):
-    """(flat uint8, offsets uint64[n + 1]) of a list of str / bytes"""
-    raw = [s.encode("latin-1") if isinstance(s, str) else bytes(s) for s in items]
-    off = np.zeros(len(raw) + 1, dtype=np.uint64)
-    np.cumsum([len(r) for r in raw], out=off[1:])
-    return np.frombuffer(b"".join(raw) + b"\0", dtype=np.uint8).copy(), off
 
 
 def max_ends(length: int) -> int:
@@ -115,9 +100,10 @@ def fragment_batch(seqs, mn: int, mx: int, exclude=(), include=(), threads: int 
     ends = np.zeros(max(int(eoff[-1]), 1), dtype=np.uint64)
     st, ne = np.zeros(max(n, 1), dtype=np.int32), np.zeros(max(n, 1), dtype=np.uint64)
     eff, emin, emax = np.zeros(max(n, 1)), np.zeros(max(n, 1), dtype=np.int64), np.zeros(max(n, 1), dtype=np.int64)
-    lib().fr_fragment_batch(flat.ctypes.data, off.ctypes.data, n, mn, mx, ex.ctypes.data, exo.ctypes.data, len(exclude), inc.ctypes.data,
-                            inco.ctypes.data, len(include), st.ctypes.data, eff.ctypes.data, emin.ctypes.data, emax.ctypes.data, ends.ctypes.data,
-                            eoff.ctypes.data, ne.ctypes.data, threads)
+    rc = lib().fr_fragment_batch(flat.ctypes.data, off.ctypes.data, n, mn, mx, ex.ctypes.data, exo.ctypes.data, len(exclude), inc.ctypes.data,
+                                 inco.ctypes.data, len(include), st.ctypes.data, eff.ctypes.data, emin.ctypes.data, emax.ctypes.data,
+                                 ends.ctypes.data, eoff.ctypes.data, ne.ctypes.data, threads)
+    assert rc == oracle_ffi.PO_OK, rc
     return st[:n], eff[:n], emin[:n], emax[:n], [[int(x) for x in ends[int(eoff[i]): int(eoff[i]) + int(ne[i])]] for i in range(n)]
 
 
@@ -131,7 +117,8 @@ def _sets(sets):
 def set_efficiency_batch(sets, threads: int = 16) -> np.ndarray:
     flat, off, soff = _sets(sets)
     eff = np.zeros(max(len(sets), 1))
-    lib().fr_set_efficiency_batch(flat.ctypes.data, off.ctypes.data, soff.ctypes.data, len(sets), eff.ctypes.data, threads)
+    rc = lib().fr_set_efficiency_batch(flat.ctypes.data, off.ctypes.data, soff.ctypes.data, len(sets), eff.ctypes.data, threads)
+    assert rc == oracle_ffi.PO_OK, rc
     return eff[: len(sets)]
 
 
@@ -142,5 +129,7 @@ def next_overhangs_batch(sets, threads: int = 16):
     cands = np.zeros((max(n, 1), 256, 4), dtype=np.uint8)
     nc = np.zeros(max(n, 1), dtype=np.uint32)
     eff = np.zeros((max(n, 1), 256))
-    lib().fr_next_overhangs_batch(flat.ctypes.data, off.ctypes.data, soff.ctypes.data, n, cands.ctypes.data, nc.ctypes.data, eff.ctypes.data, threads)
+    rc = lib().fr_next_overhangs_batch(flat.ctypes.data, off.ctypes.data, soff.ctypes.data, n, cands.ctypes.data, nc.ctypes.data,
+                                       eff.ctypes.data, threads)
+    assert rc == oracle_ffi.PO_OK, rc
     return cands[:n], nc[:n], eff[:n]

@@ -1,11 +1,15 @@
-"""ctypes binding for oracle/liboracle.so -- the CPU restatement of the reference.
+"""ctypes binding for oracle/liboracle.so -- the CPU restatement of the reference -- and the one place
+that builds and loads it.  The other binding modules (seqhash_oracle, clone_oracle, fold_oracle,
+fragment_oracle, pair_oracle) keep their own signature tables and apply them to the same handle with bind().
 
-TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__.smoke() and bench.py's
+TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__ (build and smoke) and bench.py's
 cpu_baseline / --impl reference legs.  Never imported by poly_b200/.
 """
 from __future__ import annotations
 
 import ctypes as C
+import glob
+import importlib
 import os
 import subprocess
 
@@ -13,83 +17,101 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 ORACLE_DIR = os.path.join(os.path.dirname(_HERE), "oracle")
+LIB_PATH = os.path.join(ORACLE_DIR, "liboracle.so")
+BINDINGS = ("oracle_ffi", "seqhash_oracle", "clone_oracle", "fold_oracle", "fragment_oracle", "pair_oracle")
 _LIB = None
 
 PO_OK, PO_PANIC, PO_UNSUPPORTED = 0, -1, -2
 
+_i32p, _i64p, _u64p, _f64p = C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_uint64), C.POINTER(C.c_double)
+_ALIGN = [C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, _i64p]
+
+SIGS = {
+    "po_murmur3_32": (C.c_uint32, [C.c_char_p, C.c_size_t, C.c_uint32]),
+    "po_mash_sketch_faithful": (C.c_int, [C.c_char_p, C.c_int64, C.c_int, C.c_int, C.c_void_p]),
+    "po_mash_sketch_closed": (C.c_int, [C.c_char_p, C.c_int64, C.c_int, C.c_int, C.c_void_p]),
+    "po_mash_similarity": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, _i64p, _f64p]),
+    "po_mash_distance": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, _f64p]),
+    "po_mash_sketch_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, _u64p]),
+    "po_sw_score": (C.c_int, _ALIGN + [_i64p, _i64p, _i32p, _i64p]),
+    "po_sw_align": (C.c_int, _ALIGN + [C.c_char_p, C.c_char_p, C.c_int64, _i64p, _i32p, _i64p]),
+    "po_nw_align": (C.c_int, _ALIGN + [C.c_char_p, C.c_char_p, C.c_int64, _i64p, _i32p, _i64p]),
+    "po_nw_score": (C.c_int, _ALIGN + [_i32p, _i64p]),
+    "po_fastq_parse": (C.c_int, [C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, _u64p, _i32p, _u64p]),
+    "po_fasta_parse": (C.c_int, [C.c_char_p, C.c_uint64, C.c_uint32, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
+                                 C.c_void_p, C.c_uint64, _u64p, _i32p, _u64p]),
+    "po_reverse_complement": (None, [C.c_char_p, C.c_int64, C.c_char_p]),
+    "po_santalucia": (C.c_int, [C.c_char_p, C.c_int64, C.c_double, C.c_double, C.c_double, _f64p, _f64p, _f64p]),
+    "po_melting_temp": (C.c_int, [C.c_char_p, C.c_int64, _f64p]),
+    "po_sw_score_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                    C.c_int64, C.c_int, C.c_void_p, _u64p]),
+    "po_melting_temp_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, _u64p]),
+    "po_mash_similarity_block": (C.c_int, [C.c_void_p, C.c_uint64, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int,
+                                           C.c_void_p, _u64p]),
+}
+
 
 def build(force: bool = False) -> str:
-    """Compile oracle/liboracle.so when missing or stale.  Several ranks of a torchrun job may get here
-    at once: the build runs under an exclusive file lock and replaces the library atomically."""
+    """Compile oracle/liboracle.so (oracle/Makefile) when it is missing or older than any oracle/*.c, *.h or the
+    Makefile.  Several ranks of a torchrun job may get here at once: the build runs under an exclusive file lock
+    and replaces the library atomically."""
     import fcntl
 
-    so = os.path.join(ORACLE_DIR, "liboracle.so")
-    srcs = [os.path.join(ORACLE_DIR, f) for f in ("mash_oracle.c", "align_primers_oracle.c", "fasta_oracle.c", "batch_drivers.c", "poly_oracle.h")]
+    deps = glob.glob(os.path.join(ORACLE_DIR, "*.[ch]")) + [os.path.join(ORACLE_DIR, "Makefile")]
 
     def stale():
-        return force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
+        return force or not os.path.exists(LIB_PATH) or any(os.path.getmtime(d) > os.path.getmtime(LIB_PATH) for d in deps)
 
     if stale():
         with open(os.path.join(ORACLE_DIR, ".build.lock"), "w") as lk:
             fcntl.flock(lk, fcntl.LOCK_EX)
             if stale():  # nobody built it while we waited
                 tmp = f"liboracle.{os.getpid()}.tmp.so"
-                subprocess.check_call(["make", "-C", ORACLE_DIR, "-s", "-B", "CC=gcc", f"OUT={tmp}"])
-                os.replace(os.path.join(ORACLE_DIR, tmp), so)
-    return so
+                subprocess.check_call(["make", "-C", ORACLE_DIR, "-s", "-B", f"OUT={tmp}"])
+                os.replace(os.path.join(ORACLE_DIR, tmp), LIB_PATH)
+    return LIB_PATH
 
 
 def lib():
+    """The one handle on liboracle.so (built first when missing or stale), with this module's table bound."""
     global _LIB
     if _LIB is None:
-        L = C.CDLL(build())
-        u8p, u32p, u64p, i64p = (C.POINTER(C.c_uint8), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_int64))
-        L.po_murmur3_32.restype = C.c_uint32
-        L.po_murmur3_32.argtypes = [C.c_char_p, C.c_size_t, C.c_uint32]
-        for f in (L.po_mash_sketch_faithful, L.po_mash_sketch_closed):
-            f.restype = C.c_int
-            f.argtypes = [C.c_char_p, C.c_int64, C.c_int, C.c_int, C.c_void_p]
-        L.po_mash_similarity.restype = C.c_int
-        L.po_mash_similarity.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, i64p, C.POINTER(C.c_double)]
-        L.po_mash_distance.restype = C.c_int
-        L.po_mash_distance.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double)]
-        L.po_mash_sketch_batch.restype = C.c_int
-        L.po_mash_sketch_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, u64p]
-        L.po_sw_score.restype = C.c_int
-        L.po_sw_score.argtypes = [C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                  C.c_int64, i64p, i64p, i64p, C.POINTER(C.c_int32), i64p]
-        L.po_sw_align.restype = C.c_int
-        L.po_sw_align.argtypes = [C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                  C.c_int64, i64p, C.c_char_p, C.c_char_p, C.c_int64, i64p, C.POINTER(C.c_int32), i64p]
-        L.po_fastq_parse.restype = C.c_int
-        L.po_fastq_parse.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, u64p, C.POINTER(C.c_int32), u64p]
-        L.po_fasta_parse.restype = C.c_int
-        L.po_fasta_parse.argtypes = [C.c_char_p, C.c_uint64, C.c_uint32, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p,
-                                     C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, u64p, C.POINTER(C.c_int32), u64p]
-        L.po_nw_align.restype = C.c_int
-        L.po_nw_align.argtypes = L.po_sw_align.argtypes
-        L.po_nw_score.restype = C.c_int
-        L.po_nw_score.argtypes = [C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                  C.c_int64, i64p, C.POINTER(C.c_int32), i64p]
-        L.po_reverse_complement.restype = None
-        L.po_reverse_complement.argtypes = [C.c_char_p, C.c_int64, C.c_char_p]
-        L.po_santalucia.restype = C.c_int
-        L.po_santalucia.argtypes = [C.c_char_p, C.c_int64, C.c_double, C.c_double, C.c_double] + [C.POINTER(C.c_double)] * 3
-        L.po_melting_temp.restype = C.c_int
-        L.po_melting_temp.argtypes = [C.c_char_p, C.c_int64, C.POINTER(C.c_double)]
-        L.po_sw_score_batch.restype = C.c_int
-        L.po_sw_score_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                        C.c_int64, C.c_int, C.c_void_p, u64p]
-        L.po_melting_temp_batch.restype = C.c_int
-        L.po_melting_temp_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, u64p]
-        L.po_mash_similarity_block.restype = C.c_int
-        L.po_mash_similarity_block.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int, C.c_void_p, u64p]
-        _LIB = L
+        _LIB = C.CDLL(build())
+        bind(SIGS)
     return _LIB
+
+
+def bind(sigs: dict):
+    """Apply a {name: (restype, argtypes)} table to the shared handle and return the handle."""
+    L = lib()
+    for name, (res, args) in sigs.items():
+        f = getattr(L, name)
+        f.restype = res
+        f.argtypes = args
+    return L
+
+
+def signatures() -> dict:
+    """The signature tables of every binding module, merged: every oracle function bound in Python."""
+    out = {}
+    for m in BINDINGS:
+        out.update(importlib.import_module(m).SIGS)
+    return out
 
 
 def _b(s) -> bytes:
     return s.encode("latin-1") if isinstance(s, str) else bytes(s)
+
+
+def ragged(items):
+    """(flat uint8, offsets uint64[n + 1]) of a sequence of str / bytes, with a NUL after the last item so that
+    the pointer is valid for an empty list.  A (bases, offsets) tuple of arrays is returned as contiguous arrays."""
+    if isinstance(items, tuple) and len(items) == 2 and isinstance(items[0], np.ndarray):
+        return np.ascontiguousarray(items[0], np.uint8), np.ascontiguousarray(items[1], np.uint64)
+    raw = [_b(s) for s in items]
+    off = np.zeros(len(raw) + 1, dtype=np.uint64)
+    np.cumsum([len(r) for r in raw], out=off[1:])
+    return np.frombuffer(b"".join(raw) + b"\0", dtype=np.uint8).copy(), off
 
 
 def murmur3_32(data, seed: int = 0) -> int:

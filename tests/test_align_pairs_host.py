@@ -51,7 +51,7 @@ def test_pair_calls_fail_without_a_device():
 
 @pytest.mark.parametrize("gap", [-3, -2, 0, 1])
 def test_pair_driver_matches_per_pair_oracle(gap):
-    """The C pair driver (tests/pair_oracle.c) equals po_sw_score / po_nw_score called pair by pair, errors
+    """The C pair driver (oracle/pair_oracle.c) equals po_sw_score / po_nw_score called pair by pair, errors
     and empty strings included, on random pairs of two ragged sets."""
     rng = np.random.default_rng(40 + gap)
     A = [bytes(rng.choice(list(b"ACGT"), size=int(n)).astype(np.uint8)) for n in rng.integers(0, 300, 120)]

@@ -1,4 +1,4 @@
-"""GPU tier: clone digests and Golden Gate assemblies, bit-exact against the clone oracle (tests/clone_oracle.c)."""
+"""GPU tier: clone digests and Golden Gate assemblies, bit-exact against the clone oracle (oracle/clone_oracle.c)."""
 from __future__ import annotations
 
 import ctypes as C

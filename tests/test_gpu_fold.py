@@ -1,4 +1,4 @@
-"""GPU tier for fold: pg_fold_zuker_batch against the C restatement (tests/fold_oracle.c), bit for bit:
+"""GPU tier for fold: pg_fold_zuker_batch against the C restatement (oracle/fold_oracle.c), bit for bit:
 MFE float64 bits, dot-bracket bytes and status on every item."""
 import os
 import random

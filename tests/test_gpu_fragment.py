@@ -1,5 +1,5 @@
 """GPU tier for synthesis/fragment: pg_fragment_batch, pg_fragment_set_efficiency_batch and
-pg_fragment_next_overhangs_batch against the C restatement (tests/fragment_oracle.c), bit for bit: status,
+pg_fragment_next_overhangs_batch against the C restatement (oracle/fragment_oracle.c), bit for bit: status,
 fragment ends, error numbers and the float64 efficiency bytes of every item."""
 import os
 import random

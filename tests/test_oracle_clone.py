@@ -1,4 +1,4 @@
-"""CPU tier: the clone oracle (tests/clone_oracle.c) against the reference's own pins (clone/clone_test.go,
+"""CPU tier: the clone oracle (oracle/clone_oracle.c) against the reference's own pins (clone/clone_test.go,
 clone/example_test.go), and the deferred-hash ligation design against the oracle's eager hashing."""
 from __future__ import annotations
 

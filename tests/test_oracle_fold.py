@@ -1,4 +1,4 @@
-"""CPU tier for fold: the C restatement (tests/fold_oracle.c) reproduces every pin of poly's fold tests
+"""CPU tier for fold: the C restatement (oracle/fold_oracle.c) reproduces every pin of poly's fold tests
 (fold_test.go, seqfold_test.go, example_test.go), and the library's energy tables equal
 tests/golden/fold/energies.json entry by entry."""
 import math

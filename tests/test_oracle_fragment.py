@@ -1,5 +1,5 @@
 """CPU tier for synthesis/fragment: the library's fidelity table equals tests/golden/fragment/ligation_fidelity.json
-entry for entry; the C restatement (tests/fragment_oracle.c) reproduces every pin of poly's fragment_test.go
+entry for entry; the C restatement (oracle/fragment_oracle.c) reproduces every pin of poly's fragment_test.go
 and example_test.go; and an independent Python restatement of the GPU's incremental formulation (R over the
 120 keys, one pass over the keyed members per candidate) gives the oracle's bits on seeded cases."""
 import os

@@ -15,7 +15,7 @@ Workloads (inputs generated from seeds; scoring +3 / -3, gap -2 over {-, A, C, G
                           (reported only)
 Per workload: cells = sum of len(a) * len(b), the median wall time of `--runs` calls after warm-up (each
 ends in a device synchronise) and GCUPS; parity of a sample against the C restatement (oracle/, driven pair by pair
-by tests/pair_oracle.c); and a CPU arm: that C driver on all schedulable cores over a P1 / P3 sample
+by oracle/pair_oracle.c); and a CPU arm: that C driver on all schedulable cores over a P1 / P3 sample
 ("C restatement, not Go").
 The card's name, power limit and SM clock are read in the same run."""
 import argparse
@@ -86,7 +86,7 @@ def timed(fn, runs, warmup=2):
 
 
 def oracle_scores(A, B, pairs, global_alignment, threads):
-    """Scores from the C pair driver over the restated po_sw_score / po_nw_score (tests/pair_oracle.c)."""
+    """Scores from the C pair driver over the restated po_sw_score / po_nw_score (oracle/pair_oracle.c)."""
     return pair_oracle.scores((A.h_seqs, A.h_off), (B.h_seqs, B.h_off), pairs, LUT, LUT, MAT, -2, global_alignment, threads)[0].tolist()
 
 

@@ -6,7 +6,7 @@
           base enzymes (directional), through pg_clone_digest_batch in batches of --batch parts.  Reported:
           input GB/s of the whole host call (upload, kernels, copy-back) and of the digest kernels alone
           (torch.profiler, separate untimed pass) against the 3.35 TB/s HBM3 data-sheet bound.  CPU arm: the C
-          restatement (tests/clone_oracle.c) on every schedulable core over a prefix of the parts.
+          restatement (oracle/clone_oracle.c) on every schedulable core over a prefix of the parts.
   golden  a backbone + --positions x --variants parts (tests/clone_util.combinatorial_library): variants **
           positions clones.  Timed: digest (pg_clone_digest_batch on the same parts); digest + enumeration that
           only counts (a call with zero caps stops there: it stores no recipes); and the full call.  The rest of
@@ -129,7 +129,7 @@ def bench_digest(args, dev):
         "kernel_ms": ks, "input_gbps_kernels": total_bytes / (kernel_total / 1e3) / 1e9,
         "kernel_fraction_of_hbm_bound": (total_bytes / (kernel_total / 1e3)) / (HBM_TBPS * 1e12),
         "fragments_per_batch": caps[0][0], "parity_items": len(sample), "parity_fragments": frags_seen,
-        "cpu_arm": {"impl": "C restatement (tests/clone_oracle.c), not Go", "threads": cores, "parts": n_cpu,
+        "cpu_arm": {"impl": "C restatement (oracle/clone_oracle.c), not Go", "threads": cores, "parts": n_cpu,
                     "input_gbps": n_cpu * L / cpu_s / 1e9},
     }
 

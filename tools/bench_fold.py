@@ -13,7 +13,7 @@ Per workload: the median wall time of `--runs` calls after one warm-up call (eac
 synchronise, so the time includes the host-device copies) as items/s and V-loop candidate checks/s
 (the count of (rightOfStart, leftOfEnd) candidates is computed from the shapes: sum over diagonals d >= 5
 of (n - d)(d - 5)(d - 4) / 2 per item); parity (MFE bits, dot-bracket, status) of a sample against the
-C restatement (tests/fold_oracle.c); and a CPU arm, that C restatement on 16 host threads over a slice
+C restatement (oracle/fold_oracle.c); and a CPU arm, that C restatement on 16 host threads over a slice
 ("C restatement, not Go").  The card's name and power limit are read in the same run."""
 import argparse
 import json

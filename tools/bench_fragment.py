@@ -11,7 +11,7 @@ Per workload: the median wall time of `--runs` calls after one warm-up call (eac
 synchronise, so the time includes the host-device copies) as items/s and bases/s (sets/s for `next`, whose
 sets are flattened into the C ABI's arrays before the timed calls);
 parity (status, ends, error numbers, float64 bytes) of a sample against the C restatement
-(tests/fragment_oracle.c); and that restatement on 16 host threads over the sample ("C restatement, not
+(oracle/fragment_oracle.c); and that restatement on 16 host threads over the sample ("C restatement, not
 Go").  The card's name, power limit and SM clock are read in the same run.  This is integer and FP64
 latency-bound work: no share of a bandwidth or FLOP roof is claimed."""
 import argparse
