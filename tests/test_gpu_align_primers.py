@@ -8,6 +8,7 @@ import pytest
 
 from poly_b200 import _lib, align, mash, primers, synth
 from test_oracle_align_primers import GENE, NUC_4, TEST_LUT, TEST_MAT, design_primers, lut
+from test_oracle_tm_restatement import same_bits
 
 pytestmark = pytest.mark.gpu
 GOLD = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "survey_goldens.json")))
@@ -117,7 +118,7 @@ def test_cfg5_goldens_and_sample(gpu, oracle):
     assert tm[:6] == pytest.approx(GOLD["cfg5"]["tm"], rel=1e-6)  # north_star tolerance: 1e-6 relative
     for i in range(n):
         rc, wt, wh, ws = oracle.santalucia(bytes(pr[25 * i:25 * i + 25]), primers.DEFAULT_CP, primers.DEFAULT_NA, primers.DEFAULT_MG)
-        assert abs(tm[i] - wt) <= 1e-6 * abs(wt) and abs(dh[i] - wh) <= 1e-9 * abs(wh) and abs(ds[i] - ws) <= 1e-6 * abs(ws)
+        assert rc == 0 and same_bits([tm[i], dh[i], ds[i]], [wt, wh, ws]).all(), i
 
 
 def test_reference_tm_tests(gpu):
@@ -148,8 +149,7 @@ def test_tm_edge_symbols_vs_oracle(gpu, oracle):
         for i, q in enumerate(seqs):
             rc, wt, wh, ws = oracle.santalucia(q, cp, na, mg)
             assert rc == 0 and st[i] == 0
-            assert dh[i] == pytest.approx(wh, rel=1e-12, abs=1e-12) and ds[i] == pytest.approx(ws, rel=1e-9)
-            assert tm[i] == pytest.approx(wt, rel=1e-6), q
+            assert same_bits([tm[i], dh[i], ds[i]], [wt, wh, ws]).all(), q
 
 
 def test_reference_design_primers_through_gpu(gpu):
@@ -207,7 +207,7 @@ def test_cfg5_full_size_properties(gpu, oracle):
     tm, dh, ds, st = primers.santalucia_arrays(pr, off, primers.DEFAULT_CP, primers.DEFAULT_NA, primers.DEFAULT_MG)
     assert not st.any() and np.isfinite(tm).all() and 20 < tm.min() and tm.max() < 90
     for i in idx:
-        assert tm[i] == pytest.approx(oracle.melting_temp(bytes(pr[25 * i:25 * i + 25])), rel=1e-6)
+        assert same_bits(tm[i], oracle.melting_temp(bytes(pr[25 * i:25 * i + 25]))), i
 
 
 def test_reference_alignment_strings(gpu):
