@@ -214,6 +214,25 @@ func DistanceSparse(sketches []uint32, n, s int, rowBegin, rowEnd int, upper boo
 	}
 }
 
+// Cluster wraps pg_mash_cluster: single-linkage groups of n sketches of size s, sketches i < j being linked when
+// sketches[i].Similarity(sketches[j]) counts at least minSame matching hashes (the lower index is the receiver).
+// label[i] is the smallest index of i's group; nGroups counts the groups and nLinks the linked pairs.
+func Cluster(sketches []uint32, n, s, minSame int) (label []uint32, nGroups, nLinks uint64, err error) {
+	label = make([]uint32, n+1)
+	var sk *C.uint32_t
+	if len(sketches) > 0 {
+		sk = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
+	}
+	var groups, links C.uint64_t
+	err = locked(func() C.int {
+		return C.pg_mash_cluster(sk, C.uint64_t(n), C.int32_t(s), C.uint32_t(minSame), (*C.uint32_t)(unsafe.Pointer(&label[0])), &groups, &links)
+	})
+	if err != nil {
+		return nil, 0, 0, err
+	}
+	return label[:n], uint64(groups), uint64(links), nil
+}
+
 // SWScoreBatch wraps pg_sw_score_batch.
 func SWScoreBatch(queries []byte, qOffsets []uint64, template string, queryIsA bool, lutA, lutB *[256]int16, table []int64,
 	nA, nB int, gap int64) (score []int64, errCode []int32, errPos []int64, err error) {

@@ -5,6 +5,7 @@ package mash
 
 import (
 	"errors"
+	"fmt"
 
 	"github.com/bebop/poly/internal/polyb200"
 )
@@ -139,6 +140,49 @@ func RelatedPairs(sketches []*Mash) []RelatedPair {
 		out[t] = RelatedPair{I: int(pi[t]), J: int(pj[t]), Same: int(same[t]), Distance: 1 - float64(same[t])/float64(s)}
 	}
 	return out
+}
+
+// Cluster groups sketches of one common SketchSize by single linkage: sketches i < j are linked when
+// sketches[i].Distance(sketches[j]) <= maxDistance (the lower index is the receiver), and the groups are the connected
+// components.  labels[i] is the smallest index in i's group, so labels[i] == i marks one representative per group.
+// The threshold is turned into a matching count by evaluating Distance's own expression 1 - same/SketchSize
+// (mash.go:134,139), so a maxDistance that sits exactly on a pair's Distance includes the pair.  A maxDistance that
+// every pair satisfies (>= 1) is an error; one that none can satisfy labels every sketch with itself.
+func Cluster(sketches []*Mash, maxDistance float64) ([]int, error) {
+	n := len(sketches)
+	if n == 0 {
+		return nil, nil
+	}
+	s := sketches[0].SketchSize
+	minSame := 0
+	for minSame <= s && !(1-float64(minSame)/float64(s) <= maxDistance) {
+		minSame++
+	}
+	if minSame == 0 && s > 0 {
+		return nil, fmt.Errorf("mash: maxDistance %v links every pair", maxDistance)
+	}
+	labels := make([]int, n)
+	if minSame > s && s > 0 {
+		for i := range labels {
+			labels[i] = i
+		}
+		return labels, nil
+	}
+	flat := make([]uint32, 0, n*s)
+	for _, m := range sketches {
+		if m.SketchSize != s {
+			return nil, errors.New("mash: Cluster needs one common SketchSize")
+		}
+		flat = append(flat, m.Sketches[:s]...)
+	}
+	label, _, _, err := polyb200.Cluster(flat, n, s, minSame)
+	if err != nil {
+		return nil, err
+	}
+	for i, l := range label {
+		labels[i] = int(l)
+	}
+	return labels, nil
 }
 
 // Neighbor is one reference of a Nearest result.

@@ -359,6 +359,37 @@ public:
     }
 };
 
+// ---- cluster: single-linkage groups of a sketch set (pg_mash_cluster) --------------------------------
+// Labels[i] = the smallest index in i's group; Groups = number of groups; Links = number of linked pairs i < j.
+struct Clusters {
+    std::vector<uint32_t> Labels;
+    uint64_t Groups = 0, Links = 0;
+};
+// The smallest matching count whose Distance over sketches of size `den` is <= maxDistance, by Distance's own
+// expression 1 - same/den (mash.go:134,139); den + 1 when no count qualifies.
+inline uint32_t MinSameForDistance(double maxDistance, int den) {
+    uint32_t same = 0;
+    while ((int64_t)same <= den && !(1 - (double)same / (double)std::max(den, 1) <= maxDistance)) ++same;
+    return same;
+}
+// Sketches i < j of one SketchSize are linked when mashes[i].Similarity(mashes[j]) counts at least minSame matching
+// hashes (the lower index is the receiver); the groups are the connected components.
+inline Clusters Cluster(const std::vector<Mash> &mashes, uint32_t minSame) {
+    const int s = mashes.empty() ? 0 : mashes[0].SketchSize;
+    std::vector<uint32_t> flat;
+    flat.reserve(mashes.size() * (size_t)std::max(s, 0));
+    for (auto &m : mashes) {
+        if (m.SketchSize != s || (int)m.Sketches.size() < s) throw std::invalid_argument("sketches must share one SketchSize");
+        flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + s);
+    }
+    Clusters out;
+    out.Labels.resize(mashes.size());
+    int rc = pg_mash_cluster(flat.data(), mashes.size(), s, minSame, out.Labels.data(), &out.Groups, &out.Links);
+    if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+    check(rc);
+    return out;
+}
+
 }  // namespace mash
 
 namespace align {

@@ -21,8 +21,8 @@
  *     only enqueue work: the sketch, Smith-Waterman / Needleman-Wunsch score, Tm and
  *     synth *_dev entry points never wait for the device.  Exceptions, which
  *     synchronise the given stream before returning because a host decision depends
- *     on a device result: pg_mash_distance_block_dev / pg_mash_distance_sparse_dev
- *     (sortedness and bucket sizes choose the algorithm), pg_fastq_ingest_dev /
+ *     on a device result: pg_mash_distance_block_dev / pg_mash_distance_sparse_dev /
+ *     pg_mash_cluster_dev (sortedness and bucket sizes choose the algorithm), pg_fastq_ingest_dev /
  *     pg_fasta_ingest_dev (they return counts and the error position by value),
  *     pg_seqhash_batch_dev (waits for earlier work on the stream to read the total length, but not
  *     for its own kernels), and
@@ -232,6 +232,35 @@ int pg_mash_distance_sparse_dev(const uint32_t *d_sketches, uint64_t n, int32_t 
                                 uint64_t row_end, uint32_t flags, uint32_t *d_pair_i, uint32_t *d_pair_j,
                                 uint32_t *d_pair_same, uint64_t pairs_cap, uint64_t *d_n_pairs,
                                 void *stream);
+
+/* ---- cluster: single-linkage groups of a sketch set at a matching-count threshold --------------------
+ * sketches is n x s (full Go arrays, zero tail included, as pg_mash_distance_block takes them).
+ *   - Link rule: sketches i < j are linked iff same(i, j) >= min_same, where same(i, j) is what
+ *     sketches[i].Similarity(sketches[j]) counts with the LOWER index as the receiver (mash.go:107-135): the
+ *     value pg_mash_distance_block writes at row i, column j, and pg_mash_distance_sparse lists under
+ *     PG_PAIRS_UPPER.  Unsorted (L - k < s) sketches are counted by that literal walk, not as sets.  Between
+ *     sketches of one size the walk advances whichever side holds the smaller value, so column i of row j holds
+ *     the same count: the receiver is stated to name the entry that is read, not because the choice matters.
+ *   - Groups are the connected components of the link graph (single linkage: members need not be linked
+ *     directly).
+ *   - Label rule: label[i] = the smallest sketch index in i's group, so label[i] == i marks one representative
+ *     per group and the output depends on the input only.
+ *   - *n_groups = number of i with label[i] == i; *n_links = number of linked pairs i < j (the count of
+ *     PG_PAIRS_UPPER triples with same >= min_same).  Either may be NULL.
+ *   - Errors, checked in this order: n > 2^32 - 1 is PG_ERR_ARG; n == 0 is valid (nothing is read or written
+ *     but the two counts, which are 0); s <= 0 is PG_ERR_PANIC as in the distance calls (Sketches[-1]);
+ *     min_same == 0 (every pair would link) or min_same > s (none could) is PG_ERR_ARG.  PG_ERR_UNSUPPORTED
+ *     as pg_mash_distance_block when unsorted sketches exceed the pairwise kernel's shared-memory tile.
+ * A matching count for a Distance cut: the smallest c with 1 - (double)c / s <= max_distance.
+ * The pairs are never materialised: dense row-block tiles are scanned on the device as they are produced.
+ * Device memory beyond the sketches: one tile of <= 8 GiB, 4 n bytes and the distance plan.
+ * The _dev variant synchronises `stream` in one place, while it builds the distance plan before the first tile
+ * (sortedness and bucket sizes choose the algorithm, as in pg_mash_distance_block_dev); it then only enqueues,
+ * and leaves d_label and the two DEVICE counters ordered on `stream` without waiting for them. */
+int pg_mash_cluster(const uint32_t *sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t *label,
+                    uint64_t *n_groups, uint64_t *n_links);
+int pg_mash_cluster_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t *d_label,
+                        uint64_t *d_n_groups, uint64_t *d_n_links, void *stream);
 
 /* ---- sketch index: top-k nearest references of query sketches -------------------------------------
  * A reference set of n sketches of size s (n x s full Go arrays, zero tail included, as

@@ -1,5 +1,5 @@
 // api_mash.cu -- the C ABI of poly's mash: Sketch on device and host buffers (the pipelined host path),
-// the single-process multi-GPU entry points, Similarity / Distance and the sketch index.
+// the single-process multi-GPU entry points, Similarity / Distance, the groups of a sketch set and the sketch index.
 #include <algorithm>
 #include <atomic>
 #include <cstring>
@@ -762,6 +762,37 @@ int pg_mash_distance_sparse(const uint32_t *sketches, uint64_t n, int32_t s, uin
     if ((rc = c.error()) || (rc = launch_distance_sparse(d_sk, n, s, row_begin, row_end, flags, d_i, d_j, d_c, pairs_cap, d_n, c.st)))
         return rc;
     return finish_capped(c, d_n, pairs_cap, n_pairs, {{pair_i, d_i, 4}, {pair_j, d_j, 4}, {pair_same, d_c, 4}}, "pairs_cap", "pairs");
+}
+
+// ---------------------------------------------------------------------------------
+// Single-linkage groups of a sketch set
+// ---------------------------------------------------------------------------------
+int pg_mash_cluster_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t *d_label,
+                        uint64_t *d_n_groups, uint64_t *d_n_links, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n && s > 0 && (!d_sketches || !d_label)) { set_error("null buffer"); return PG_ERR_ARG; }
+    return launch_mash_cluster(d_sketches, n, s, min_same, d_label, (unsigned long long *)d_n_groups, (unsigned long long *)d_n_links,
+                               (cudaStream_t)stream);
+}
+
+int pg_mash_cluster(const uint32_t *sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t *label, uint64_t *n_groups,
+                    uint64_t *n_links) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n_groups) *n_groups = 0;
+    if (n_links) *n_links = 0;
+    if ((rc = mash_cluster_check(n, s, min_same)) != PG_OK || n == 0) return rc;
+    if (!sketches || !label) { set_error("null buffer"); return PG_ERR_ARG; }
+    HostCall c;
+    const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)s);
+    uint32_t *d_label = c.alloc<uint32_t>(n);
+    unsigned long long *d_cnt = c.alloc<unsigned long long>(2);
+    if ((rc = c.error()) || (rc = launch_mash_cluster(d_sk, n, s, min_same, d_label, d_cnt, d_cnt + 1, c.st))) return rc;
+    c.download(label, d_label, n);
+    c.download((unsigned long long *)n_groups, d_cnt, 1);
+    c.download((unsigned long long *)n_links, d_cnt + 1, 1);
+    return c.finish();
 }
 
 // ---------------------------------------------------------------------------------

@@ -210,6 +210,14 @@ struct DistancePlan {
 int distance_plan_create(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, DistancePlan *plan);
 int distance_plan_rows(const DistancePlan &plan, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st);
 void distance_plan_destroy(DistancePlan &plan, cudaStream_t st);
+// distance.cu: rows per dense tile of the passes that consume a plan's tiles on the device (sparse pairs, cluster); n > 0
+uint64_t distance_tile_rows(uint64_t n, uint64_t rows);
+// mash_cluster.cu: single-linkage groups at same >= min_same; label[i] = smallest index of i's group, the
+// counters (either may be NULL) = number of groups and of linked pairs i < j.  mash_cluster_check is the
+// argument rule of pg_mash_cluster, which the host entry point applies before it copies anything.
+int mash_cluster_check(uint64_t n, int s, uint32_t min_same);
+int launch_mash_cluster(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t *d_label,
+                        unsigned long long *d_n_groups, unsigned long long *d_n_links, cudaStream_t st);
 // distance.cu: flag[r] = 1 if sketch r is non-decreasing; *d_n_unsorted = number of other sketches
 int launch_sorted_flags(const uint32_t *d_sk, uint64_t n, int s, uint8_t *d_flag, uint32_t *d_n_unsorted, cudaStream_t st);
 // mash_index.cu: the top_k most similar sketches of plan's set for each of nq query sketches of size sq

@@ -225,6 +225,15 @@ compact_pairs_kernel(const uint32_t *__restrict__ tile, uint64_t rows, uint64_t 
 
 }  // namespace
 
+// Rows per dense tile of a pass over `rows` rows of n columns that consumes the tiles on the device.
+// Tiles of <= 8 GiB: every pass over the index costs one read of all its entries and the run tables of every
+// bucket, but a tile that outgrows the memory pool's cache (12 GiB, runtime.cu) is mapped and unmapped by the
+// driver on every call.
+uint64_t distance_tile_rows(uint64_t n, uint64_t rows) {
+    const uint64_t budget_words = 2ull << 30;
+    return std::max<uint64_t>(8, std::min<uint64_t>(rows, (budget_words / n) & ~7ull));
+}
+
 // Non-zero off-diagonal matching counts of rows [row_begin, row_end) as (i, j, same) triples: dense tiles of
 // the row block (same kernels as the dense entry point) compacted on the device, so only the informative
 // pairs ever leave the GPU.  *d_n_pairs counts every qualifying pair, also beyond pairs_cap.
@@ -236,11 +245,7 @@ int launch_distance_sparse(const uint32_t *d_sk, uint64_t n, int s, uint64_t row
     if (n > 0xffffffffull) { set_error("too many sketches for 32-bit pair indices"); return PG_ERR_ARG; }
     DistancePlan plan;
     int rc = distance_plan_create(d_sk, n, s, st, &plan);
-    // tiles of <= 8 GiB: every pass over the index costs one read of all its entries and the run tables of every
-    // bucket, but a tile that outgrows the memory pool's cache (12 GiB, runtime.cu) is mapped and unmapped by the
-    // driver on every call
-    const uint64_t budget_words = 2ull << 30;
-    const uint64_t rows_per = std::max<uint64_t>(8, std::min<uint64_t>(row_end - row_begin, (budget_words / n) & ~7ull));
+    const uint64_t rows_per = distance_tile_rows(n, row_end - row_begin);
     uint32_t *d_tile = nullptr;
     if (rc == PG_OK) {
         cudaError_t e = cudaMallocAsync(&d_tile, rows_per * n * 4, st);

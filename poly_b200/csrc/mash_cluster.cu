@@ -1,0 +1,173 @@
+// mash_cluster.cu -- single-linkage groups of a sketch set at a matching-count threshold.
+//
+// Sketches i < j are linked iff same(i, j) >= min_same, same(i, j) being what
+// sketches[i].Similarity(sketches[j]) counts with the LOWER index as the receiver (the entry the dense
+// pass of distance.cu writes at row i, column j).  Groups are the connected components of that graph and
+// label[i] is the smallest index of i's group.
+//
+// The dense row-block tiles of distance.cu are scanned on the device as they are produced and every
+// qualifying entry is merged into a union-find forest over parent[n]; no pair list exists anywhere.
+//
+// cluster_link_kernel    : upper-triangle entries of one tile -> lock-free unions + the link count
+// cluster_flatten_kernel : label[i] = root(i) and the number of roots, after the last tile
+//
+// The union rule: a root is only ever re-parented, by atomicCAS, to a SMALLER root.  parent[x] <= x then holds
+// for every x at every moment, so the root of a finished component is its smallest member whatever order the
+// atomics landed in: the labels are a function of the input alone (not of tile size, grid or timing).
+#include <algorithm>
+
+#include "common.cuh"
+
+namespace pg {
+
+namespace {
+
+// Loads of parent[] while other CTAs are linking go to L2 (volatile): a root seen through a stale L1 line
+// would fail its CAS, be read as a root again and never make progress.
+__device__ __forceinline__ uint32_t parent_of(const uint32_t *parent, uint32_t x) {
+    return *reinterpret_cast<const volatile uint32_t *>(parent + x);
+}
+
+// Root of x with path halving.  x's new parent is one of its ancestors, and ancestors stay ancestors (links
+// only re-parent roots), so the plain store races only with stores of other valid ancestors.  A node that is
+// already a child of its root is not written, so a settled forest is found read-only.
+__device__ __forceinline__ uint32_t find_root(uint32_t *parent, uint32_t x) {
+    for (;;) {
+        const uint32_t p = parent_of(parent, x);
+        if (p == x) return x;
+        const uint32_t g = parent_of(parent, p);
+        if (g == p) return p;
+        parent[x] = g;
+        x = g;
+    }
+}
+
+__device__ __forceinline__ void unite(uint32_t *parent, uint32_t a, uint32_t b) {
+    for (;;) {
+        a = find_root(parent, a);
+        b = find_root(parent, b);
+        if (a == b) return;  // members of one family meet here: ~R^2 links, ~R CAS
+        const uint32_t lo = min(a, b), hi = max(a, b);
+        const uint32_t seen = atomicCAS(parent + hi, hi, lo);
+        if (seen == hi) return;
+        a = seen;  // hi was linked elsewhere meanwhile: go on from its new parent
+        b = lo;
+    }
+}
+
+// One warp covers 128 consecutive words of the (rows x n) tile per step, as compact_pairs_kernel does.
+__global__ void __launch_bounds__(256)
+cluster_link_kernel(const uint32_t *__restrict__ tile, uint64_t rows, uint64_t n, uint64_t row0, uint32_t min_same,
+                    uint32_t *parent, unsigned long long *__restrict__ n_links) {
+    const uint64_t total = rows * n;
+    const uint32_t lane = threadIdx.x & 31u;
+    const bool vec = (n & 3) == 0;  // rows are 16-byte aligned
+    uint32_t links = 0;
+    // the loop bound is warp-uniform: the warp reduction behind the loop needs every lane
+    for (uint64_t w0 = ((uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) * 4; w0 < total; w0 += (uint64_t)gridDim.x * blockDim.x * 4) {
+        const uint64_t e0 = w0 + lane * 4;
+        uint32_t v[4] = {0, 0, 0, 0};
+        if (e0 + 3 < total && vec) {
+            const uint4 q = *reinterpret_cast<const uint4 *>(tile + e0);
+            v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+        } else {
+            for (int t = 0; t < 4; ++t) if (e0 + t < total) v[t] = tile[e0 + t];
+        }
+        // most of a tile is zeros: nothing below this line runs for them (min_same >= 1)
+        if (max(max(v[0], v[1]), max(v[2], v[3])) < min_same) continue;
+        uint64_t i = row0 + e0 / n, j = e0 % n;
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            if (v[t] >= min_same && j > i) {
+                ++links;
+                unite(parent, (uint32_t)i, (uint32_t)j);
+            }
+            if (++j == n) { j = 0; ++i; }
+        }
+    }
+    links = __reduce_add_sync(0xffffffffu, links);
+    if (lane == 0 && links) atomicAdd(n_links, (unsigned long long)links);
+}
+
+__global__ void __launch_bounds__(256)
+cluster_init_kernel(uint32_t *__restrict__ parent, uint64_t n) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) parent[i] = (uint32_t)i;
+}
+
+__global__ void __launch_bounds__(256)
+cluster_flatten_kernel(const uint32_t *__restrict__ parent, uint64_t n, uint32_t *__restrict__ label,
+                       unsigned long long *__restrict__ n_groups) {
+    const uint32_t lane = threadIdx.x & 31u;
+    uint32_t roots = 0;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n; i0 += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t i = i0 + lane;
+        if (i >= n) continue;
+        uint32_t r = (uint32_t)i;
+        for (uint32_t p = parent[r]; p != r; p = parent[r]) r = p;
+        label[i] = r;
+        roots += r == (uint32_t)i;
+    }
+    roots = __reduce_add_sync(0xffffffffu, roots);
+    if (lane == 0 && roots) atomicAdd(n_groups, (unsigned long long)roots);
+}
+
+}  // namespace
+
+int mash_cluster_check(uint64_t n, int s, uint32_t min_same) {
+    if (n > 0xffffffffull) { set_error("too many sketches for 32-bit labels"); return PG_ERR_ARG; }
+    if (n == 0) return PG_OK;
+    if (s <= 0) { set_error("cluster over sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
+    if (min_same == 0 || min_same > (uint32_t)s) {
+        set_error("min_same %u outside [1, %d]: 0 links every pair, more than the sketch size links none", min_same, s);
+        return PG_ERR_ARG;
+    }
+    return PG_OK;
+}
+
+int launch_mash_cluster(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t *d_label,
+                        unsigned long long *d_n_groups, unsigned long long *d_n_links, cudaStream_t st) {
+    if (d_n_groups) PG_CUDA(cudaMemsetAsync(d_n_groups, 0, 8, st));
+    if (d_n_links) PG_CUDA(cudaMemsetAsync(d_n_links, 0, 8, st));
+    int rc = mash_cluster_check(n, s, min_same);
+    if (rc != PG_OK || n == 0) return rc;
+    StreamScratch tmp(st);  // parent[n], then the two counters: freed on every way out
+    uint32_t *d_parent = nullptr;
+    const uint64_t parent_words = (n + 1) & ~1ull;
+    cudaError_t e = tmp.alloc(&d_parent, parent_words + 4);
+    if (e != cudaSuccess) { cudaGetLastError(); set_error("cudaMallocAsync(%llu) for the cluster forest failed", (unsigned long long)((parent_words + 4) * 4)); return PG_ERR_NOMEM; }
+    unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(d_parent + parent_words);  // [0] links, [1] groups
+    PG_CUDA(cudaMemsetAsync(d_cnt, 0, 16, st));
+    const unsigned row_blocks = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)sm_count() * 16);
+    cluster_init_kernel<<<row_blocks, 256, 0, st>>>(d_parent, n);
+    PG_LAUNCH_CHECK("cluster_init_kernel");
+
+    DistancePlan plan;
+    rc = distance_plan_create(d_sk, n, s, st, &plan);
+    const uint64_t rows_per = distance_tile_rows(n, n);
+    uint32_t *d_tile = nullptr;
+    if (rc == PG_OK) {
+        e = cudaMallocAsync(&d_tile, rows_per * n * 4, st);
+        if (e != cudaSuccess) { cudaGetLastError(); set_error("cudaMallocAsync(%llu) for the pair tile failed", (unsigned long long)(rows_per * n * 4)); rc = PG_ERR_NOMEM; }
+        else tmp.adopt(d_tile);
+    }
+    for (uint64_t rb = 0; rb < n && rc == PG_OK; rb += rows_per) {
+        const uint64_t re = std::min(n, rb + rows_per);
+        rc = distance_plan_rows(plan, rb, re, d_tile, nullptr, st);
+        if (rc != PG_OK) break;
+        const uint64_t quads = ((re - rb) * n + 3) / 4;
+        cluster_link_kernel<<<(unsigned)std::min<uint64_t>((quads + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(
+            d_tile, re - rb, n, rb, min_same, d_parent, d_cnt);
+        note_launch("cluster_link_kernel");
+        e = cudaGetLastError();
+        if (e != cudaSuccess) rc = cuda_fail(e, "cluster_link_kernel", __FILE__, __LINE__);
+    }
+    distance_plan_destroy(plan, st);
+    if (rc != PG_OK) return rc;
+    cluster_flatten_kernel<<<row_blocks, 256, 0, st>>>(d_parent, n, d_label, d_cnt + 1);
+    PG_LAUNCH_CHECK("cluster_flatten_kernel");
+    if (d_n_links) PG_CUDA(cudaMemcpyAsync(d_n_links, d_cnt, 8, cudaMemcpyDeviceToDevice, st));
+    if (d_n_groups) PG_CUDA(cudaMemcpyAsync(d_n_groups, d_cnt + 1, 8, cudaMemcpyDeviceToDevice, st));
+    return PG_OK;
+}
+
+}  // namespace pg

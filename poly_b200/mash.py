@@ -373,6 +373,48 @@ class SketchIndex:
                 pass
 
 
+# ---- cluster: single-linkage groups of a sketch set (pg_mash_cluster) -------------------------------------
+def cluster(sketches, min_same: Optional[int] = None, max_distance: Optional[float] = None):
+    """Groups of a sketch set: sketches i < j are linked when sketches[i].Similarity(sketches[j]) counts at
+    least min_same matching hashes (the lower index is the receiver) -- or, alternatively, when their Distance
+    is <= max_distance -- and the groups are the connected components (single linkage).
+
+    sketches: what SketchIndex takes.  Returns (labels [n] uint32, n_groups, n_links): labels[i] is the smallest
+    index in i's group, so labels[i] == i marks one representative per group; n_links counts the linked pairs.
+    CUDA tensor sketches give a CUDA int32 label tensor (carrying the uint32 bits) and 0-dim int64 count
+    tensors, ordered on the current stream.  The pairs themselves are never materialised."""
+    if (min_same is None) == (max_distance is None):
+        raise ValueError("give exactly one of min_same and max_distance")
+    rows = _sketch_rows(sketches)
+    n, s = int(rows.shape[0]), int(rows.shape[1])
+    on_device = hasattr(rows, "data_ptr")
+    if on_device:
+        import torch
+    if max_distance is not None and s > 0:  # s == 0: the library reports the reference's panic
+        min_same = min_same_for_distance(max_distance, s)
+        if min_same == 0:
+            raise ValueError(f"max_distance {max_distance!r} links every pair: every Distance is <= it")
+        if min_same == s + 1:  # no matching count reaches the cut: every sketch is its own group
+            if on_device:
+                return torch.arange(n, dtype=torch.int32, device=rows.device), torch.tensor(n, device=rows.device), torch.tensor(0, device=rows.device)
+            return np.arange(n, dtype=np.uint32), n, 0
+    min_same = 1 if min_same is None else int(min_same)
+    if not 0 <= min_same <= 0xFFFFFFFF:
+        raise ValueError("min_same must fit 32 bits")
+    if on_device:
+        dev = rows.device
+        labels = torch.empty(n, dtype=torch.int32, device=dev)
+        counts = torch.zeros(2, dtype=torch.int64, device=dev)
+        rc = _lib.lib().pg_mash_cluster_dev(rows.data_ptr(), n, s, min_same, labels.data_ptr(), counts.data_ptr(),
+                                            counts.data_ptr() + 8, torch.cuda.current_stream(dev).cuda_stream)
+        _index_rc(rc)
+        return labels, counts[0], counts[1]
+    labels = np.empty(n, dtype=np.uint32)
+    ng, nl = C.c_uint64(0), C.c_uint64(0)
+    _index_rc(_lib.lib().pg_mash_cluster(rows.ctypes.data, n, s, min_same, labels.ctypes.data, C.byref(ng), C.byref(nl)))
+    return labels, int(ng.value), int(nl.value)
+
+
 # ---- single-process multi-GPU additions (pg_*_multi; SURVEY.md 8b / 8e) ----------------------------
 def _device_list(devices):
     if devices is None:
