@@ -233,6 +233,29 @@ func Cluster(sketches []uint32, n, s, minSame int) (label []uint32, nGroups, nLi
 	return label[:n], uint64(groups), uint64(links), nil
 }
 
+// Dereplicate wraps pg_mash_dereplicate: greedy representatives of n sketches of size s, linked as in Cluster.
+// In index order, i is a representative iff no representative r < i is linked to i; rep[i] = i for one, else the
+// smallest linked representative, or with nearest the one with the largest count (ties to the smaller index).
+func Dereplicate(sketches []uint32, n, s, minSame int, nearest bool) (rep []uint32, nReps uint64, err error) {
+	rep = make([]uint32, n+1)
+	var sk *C.uint32_t
+	if len(sketches) > 0 {
+		sk = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
+	}
+	flags := C.uint32_t(0)
+	if nearest {
+		flags = C.PG_DEREP_NEAREST
+	}
+	var reps C.uint64_t
+	err = locked(func() C.int {
+		return C.pg_mash_dereplicate(sk, C.uint64_t(n), C.int32_t(s), C.uint32_t(minSame), flags, (*C.uint32_t)(unsafe.Pointer(&rep[0])), &reps)
+	})
+	if err != nil {
+		return nil, 0, err
+	}
+	return rep[:n], uint64(reps), nil
+}
+
 // SWScoreBatch wraps pg_sw_score_batch.
 func SWScoreBatch(queries []byte, qOffsets []uint64, template string, queryIsA bool, lutA, lutB *[256]int16, table []int64,
 	nA, nB int, gap int64) (score []int64, errCode []int32, errPos []int64, err error) {

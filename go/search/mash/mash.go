@@ -185,6 +185,56 @@ func Cluster(sketches []*Mash, maxDistance float64) ([]int, error) {
 	return labels, nil
 }
 
+// Dereplicate picks representatives of sketches of one common SketchSize, in index order: sketch i is a
+// representative iff no representative r < i has sketches[r].Distance(sketches[i]) <= maxDistance.  It returns
+// rep, with rep[i] == i for a representative; any other sketch gets the first representative within the cut, or
+// with nearest the one at the smallest Distance (the earlier one on a tie).  That is the result of
+//
+//	for i := range sketches {
+//		for _, r := range reps { if sketches[r].Distance(sketches[i]) <= maxDistance { rep[i] = r; continue outer } }
+//		reps = append(reps, i); rep[i] = i
+//	}
+//
+// computed in one GPU pass.  Permute sketches first to give some of them priority.  The threshold becomes a matching
+// count as in Cluster; a maxDistance that every pair satisfies (>= 1) is an error, one that none can satisfy makes
+// every sketch its own representative.
+func Dereplicate(sketches []*Mash, maxDistance float64, nearest bool) ([]int, error) {
+	n := len(sketches)
+	if n == 0 {
+		return nil, nil
+	}
+	s := sketches[0].SketchSize
+	minSame := 0
+	for minSame <= s && !(1-float64(minSame)/float64(s) <= maxDistance) {
+		minSame++
+	}
+	if minSame == 0 && s > 0 {
+		return nil, fmt.Errorf("mash: maxDistance %v links every pair", maxDistance)
+	}
+	reps := make([]int, n)
+	if minSame > s && s > 0 {
+		for i := range reps {
+			reps[i] = i
+		}
+		return reps, nil
+	}
+	flat := make([]uint32, 0, n*s)
+	for _, m := range sketches {
+		if m.SketchSize != s {
+			return nil, errors.New("mash: Dereplicate needs one common SketchSize")
+		}
+		flat = append(flat, m.Sketches[:s]...)
+	}
+	rep, _, err := polyb200.Dereplicate(flat, n, s, minSame, nearest)
+	if err != nil {
+		return nil, err
+	}
+	for i, r := range rep {
+		reps[i] = int(r)
+	}
+	return reps, nil
+}
+
 // Neighbor is one reference of a Nearest result.
 type Neighbor struct {
 	Index    int     // position in the reference list given to NewIndex

@@ -390,6 +390,31 @@ inline Clusters Cluster(const std::vector<Mash> &mashes, uint32_t minSame) {
     return out;
 }
 
+// ---- dereplicate: greedy representatives of a sketch set (pg_mash_dereplicate) ---------------------------
+// Rep[i] = i for a representative, otherwise i's representative; NReps = number of representatives.
+struct Representatives {
+    std::vector<uint32_t> Rep;
+    uint64_t NReps = 0;
+};
+// Links as in Cluster.  In index order, i is a representative iff no representative r < i is linked to i; any
+// other i gets the smallest linked representative, or with `nearest` the one with the largest count (ties to the
+// smaller index).
+inline Representatives Dereplicate(const std::vector<Mash> &mashes, uint32_t minSame, bool nearest = false) {
+    const int s = mashes.empty() ? 0 : mashes[0].SketchSize;
+    std::vector<uint32_t> flat;
+    flat.reserve(mashes.size() * (size_t)std::max(s, 0));
+    for (auto &m : mashes) {
+        if (m.SketchSize != s || (int)m.Sketches.size() < s) throw std::invalid_argument("sketches must share one SketchSize");
+        flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + s);
+    }
+    Representatives out;
+    out.Rep.resize(mashes.size());
+    int rc = pg_mash_dereplicate(flat.data(), mashes.size(), s, minSame, nearest ? PG_DEREP_NEAREST : 0u, out.Rep.data(), &out.NReps);
+    if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+    check(rc);
+    return out;
+}
+
 }  // namespace mash
 
 namespace align {

@@ -22,7 +22,8 @@
  *     synth *_dev entry points never wait for the device.  Exceptions, which
  *     synchronise the given stream before returning because a host decision depends
  *     on a device result: pg_mash_distance_block_dev / pg_mash_distance_sparse_dev /
- *     pg_mash_cluster_dev (sortedness and bucket sizes choose the algorithm), pg_fastq_ingest_dev /
+ *     pg_mash_cluster_dev / pg_mash_dereplicate_dev (sortedness and bucket sizes choose the
+ *     algorithm), pg_fastq_ingest_dev /
  *     pg_fasta_ingest_dev (they return counts and the error position by value),
  *     pg_seqhash_batch_dev (waits for earlier work on the stream to read the total length, but not
  *     for its own kernels), and
@@ -261,6 +262,38 @@ int pg_mash_cluster(const uint32_t *sketches, uint64_t n, int32_t s, uint32_t mi
                     uint64_t *n_groups, uint64_t *n_links);
 int pg_mash_cluster_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t *d_label,
                         uint64_t *d_n_groups, uint64_t *d_n_links, void *stream);
+
+/* ---- dereplicate: greedy representatives of a sketch set at a matching-count threshold ----------------
+ * sketches is n x s (full Go arrays, zero tail included, as pg_mash_cluster takes them).
+ *   - Link rule: that of pg_mash_cluster.  Sketches r < i are linked iff same(r, i) >= min_same, same(r, i)
+ *     being what sketches[r].Similarity(sketches[i]) counts with the LOWER index as the receiver; unsorted
+ *     (L - k < s) sketches are counted by that literal walk.
+ *   - Representatives, in index order: i is a representative iff no representative r < i is linked to i (a
+ *     caller's greedy loop over the set: every sketch within the cut of one kept so far joins the first such,
+ *     any other is kept).  Callers who want another priority (length, quality) permute the set first.
+ *   - Assignment: rep[i] = i for a representative.  Otherwise, by default, rep[i] = the smallest representative
+ *     linked to i; with PG_DEREP_NEAREST, the linked earlier representative with the largest same (for one
+ *     sketch size, the smallest Distance), ties to the smaller index.  Both modes pick the same representatives.
+ *   - *n_reps = number of i with rep[i] == i.  It may be NULL.
+ *   - The output depends on the input only: not on tile or sub-block size, grid or the order of atomics.
+ *   - Errors, checked in this order: a flags bit other than PG_DEREP_NEAREST is PG_ERR_ARG; then the rules of
+ *     pg_mash_cluster: n > 2^32 - 1 is PG_ERR_ARG; n == 0 is valid (nothing is read or written but *n_reps,
+ *     which is 0); s <= 0 is PG_ERR_PANIC; min_same == 0 or min_same > s is PG_ERR_ARG.  PG_ERR_UNSUPPORTED as
+ *     pg_mash_distance_block when unsorted sketches exceed the pairwise kernel's shared-memory tile.
+ * A matching count for a Distance cut: the smallest c with 1 - (double)c / s <= max_distance.
+ * The pairs are never materialised: dense row-block tiles are consumed on the device as they are produced, and
+ * only the representatives' rows are read beyond the 1024-row diagonal blocks.
+ * Device memory beyond the sketches: one tile of <= 8 GiB, the distance plan, the 4 n bytes of rep (the first
+ * assignment is built there in place; PG_DEREP_NEAREST adds 8 n bytes, a 64-bit key per sketch), a 128 KiB link
+ * bitmap and a 4 KiB list.
+ * The _dev variant synchronises `stream` in one place, while it builds the distance plan before the first tile,
+ * as pg_mash_cluster_dev does; it then only enqueues, with no host round trip per tile or sub-block, and leaves
+ * d_rep and the DEVICE counter ordered on `stream` without waiting for them. */
+#define PG_DEREP_NEAREST 1u
+int pg_mash_dereplicate(const uint32_t *sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t flags,
+                        uint32_t *rep, uint64_t *n_reps);
+int pg_mash_dereplicate_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t flags,
+                            uint32_t *d_rep, uint64_t *d_n_reps, void *stream);
 
 /* ---- sketch index: top-k nearest references of query sketches -------------------------------------
  * A reference set of n sketches of size s (n x s full Go arrays, zero tail included, as

@@ -68,6 +68,8 @@ _SIGS = {
     "pg_mash_distance_sparse_dev": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_uint64, C.c_uint64, C.c_uint32, _u32p, _u32p, _u32p, C.c_uint64, C.c_void_p, C.c_void_p]),
     "pg_mash_cluster": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_uint32, _u32p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "pg_mash_cluster_dev": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_uint32, _u32p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pg_mash_dereplicate": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_uint32, C.c_uint32, _u32p, C.POINTER(C.c_uint64)]),
+    "pg_mash_dereplicate_dev": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_uint32, C.c_uint32, _u32p, C.c_void_p, C.c_void_p]),
     "pg_mash_index_create": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.POINTER(C.c_void_p)]),
     "pg_mash_index_create_dev": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p)]),
     "pg_mash_index_query": (C.c_int, [C.c_void_p, _u32p, C.c_uint64, C.c_int32, C.c_uint32, C.c_uint32, _u32p, _u32p, _f64p, _u32p]),

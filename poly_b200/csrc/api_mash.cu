@@ -1,5 +1,6 @@
 // api_mash.cu -- the C ABI of poly's mash: Sketch on device and host buffers (the pipelined host path),
-// the single-process multi-GPU entry points, Similarity / Distance, the groups of a sketch set and the sketch index.
+// the single-process multi-GPU entry points, Similarity / Distance, the groups and the representatives of a
+// sketch set and the sketch index.
 #include <algorithm>
 #include <atomic>
 #include <cstring>
@@ -792,6 +793,34 @@ int pg_mash_cluster(const uint32_t *sketches, uint64_t n, int32_t s, uint32_t mi
     c.download(label, d_label, n);
     c.download((unsigned long long *)n_groups, d_cnt, 1);
     c.download((unsigned long long *)n_links, d_cnt + 1, 1);
+    return c.finish();
+}
+
+// ---------------------------------------------------------------------------------
+// Greedy representatives of a sketch set
+// ---------------------------------------------------------------------------------
+int pg_mash_dereplicate_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t flags, uint32_t *d_rep,
+                            uint64_t *d_n_reps, void *stream) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n && s > 0 && (!d_sketches || !d_rep)) { set_error("null buffer"); return PG_ERR_ARG; }
+    return launch_mash_derep(d_sketches, n, s, min_same, flags, d_rep, (unsigned long long *)d_n_reps, (cudaStream_t)stream);
+}
+
+int pg_mash_dereplicate(const uint32_t *sketches, uint64_t n, int32_t s, uint32_t min_same, uint32_t flags, uint32_t *rep,
+                        uint64_t *n_reps) {
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    if (n_reps) *n_reps = 0;
+    if ((rc = mash_derep_check(n, s, min_same, flags)) != PG_OK || n == 0) return rc;
+    if (!sketches || !rep) { set_error("null buffer"); return PG_ERR_ARG; }
+    HostCall c;
+    const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)s);
+    uint32_t *d_rep = c.alloc<uint32_t>(n);
+    unsigned long long *d_cnt = c.alloc<unsigned long long>(1);
+    if ((rc = c.error()) || (rc = launch_mash_derep(d_sk, n, s, min_same, flags, d_rep, d_cnt, c.st))) return rc;
+    c.download(rep, d_rep, n);
+    c.download((unsigned long long *)n_reps, d_cnt, 1);
     return c.finish();
 }
 

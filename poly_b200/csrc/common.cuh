@@ -218,6 +218,12 @@ uint64_t distance_tile_rows(uint64_t n, uint64_t rows);
 int mash_cluster_check(uint64_t n, int s, uint32_t min_same);
 int launch_mash_cluster(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t *d_label,
                         unsigned long long *d_n_groups, unsigned long long *d_n_links, cudaStream_t st);
+// mash_derep.cu: greedy representatives at same >= min_same; rep[i] = i's representative (first or, with
+// PG_DEREP_NEAREST, nearest), the counter (may be NULL) = number of representatives.  mash_derep_check is the
+// argument rule of pg_mash_dereplicate: the flags, then mash_cluster_check.
+int mash_derep_check(uint64_t n, int s, uint32_t min_same, uint32_t flags);
+int launch_mash_derep(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t flags, uint32_t *d_rep,
+                      unsigned long long *d_n_reps, cudaStream_t st);
 // distance.cu: flag[r] = 1 if sketch r is non-decreasing; *d_n_unsorted = number of other sketches
 int launch_sorted_flags(const uint32_t *d_sk, uint64_t n, int s, uint8_t *d_flag, uint32_t *d_n_unsorted, cudaStream_t st);
 // mash_index.cu: the top_k most similar sketches of plan's set for each of nq query sketches of size sq

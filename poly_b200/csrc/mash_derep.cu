@@ -1,0 +1,231 @@
+// mash_derep.cu -- greedy representatives of a sketch set at a matching-count threshold.
+//
+// Sketches r < i are linked iff same(r, i) >= min_same (the link rule of mash_cluster.cu: row r, column i of the
+// dense pass).  In index order, i is a representative iff no representative r < i is linked to i.  Every other
+// sketch is assigned the smallest linked representative (first) or the one with the largest count, ties to the
+// smaller index (PG_DEREP_NEAREST).
+//
+// The dense row-block tiles of distance.cu are consumed on the device in sub-blocks of kDerepRows consecutive rows
+// (never straddling a tile).  For sub-block [a, a + b):
+//
+// derep_links_kernel  : whole grid; the links among the sub-block's own rows as a b x kDerepRows bitmap
+// derep_walk_kernel   : one CTA; the serial part.  It reads which rows earlier marks already cover, then walks the
+//                       rows in order in shared memory: the next uncovered row is a representative and its link
+//                       bits cover the rows after it.  At most kDerepRows steps whatever the input; it writes the
+//                       sub-block's representatives as a list.
+// derep_mark_kernel   : whole grid; the representatives' tile rows at columns (r, n), and nothing else.  A linked
+//                       column j gets atomicMin(rep[j], r) (first) or atomicMax(key[j], same << 32 | ~r) (nearest),
+//                       both order-independent.  Columns inside the sub-block get their assignment here too.
+// derep_finish_kernel : after the last tile: rep[i] = i for representatives, keys to indices, the count.
+//
+// A representative's slot is never written (the marks only reach sketches linked to an earlier representative),
+// so "slot still unset" is exactly "representative" and no separate flag array is kept.  Stream order makes every
+// earlier mark visible to the next walk; the output depends on the input alone.
+#include <algorithm>
+
+#include "common.cuh"
+
+namespace pg {
+
+namespace {
+
+constexpr uint32_t kDerepRows = 1024;            // rows per sub-block: one bit per row in a warp's 32 x 32-bit words
+constexpr uint32_t kWords = kDerepRows / 32;
+constexpr uint32_t kNone = 0xffffffffu;          // first mode: rep[j] not yet assigned
+constexpr uint32_t kMarkCols = 4096;             // columns of one mark step: 256 threads x 4 quads
+
+// bits[t * kWords + w], bit x: sub-block row t is linked to sub-block row 32 w + x (only x above t, below b).
+// One warp per word: a coalesced 128-byte load and one ballot.
+__global__ void __launch_bounds__(256)
+derep_links_kernel(const uint32_t *__restrict__ tile, uint64_t n, uint64_t t0, uint64_t a, uint32_t b, uint32_t min_same,
+                   uint32_t *__restrict__ bits) {
+    const uint32_t lane = threadIdx.x & 31u;
+    for (uint32_t it = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; it < b * kWords; it += (gridDim.x * blockDim.x) >> 5) {
+        const uint32_t t = it / kWords, c = (it % kWords) * 32 + lane;
+        const uint32_t v = c > t && c < b ? tile[(t0 + t) * n + a + c] : 0;  // min_same >= 1: 0 never links
+        const uint32_t m = __ballot_sync(0xffffffffu, v >= min_same);
+        if (lane == 0) bits[it] = m;
+    }
+}
+
+// list[0] = number of representatives in [a, a + b), list[1..] = their indices in increasing order.
+template <bool Nearest>
+__global__ void __launch_bounds__(1024)
+derep_walk_kernel(const uint32_t *__restrict__ bits, uint64_t a, uint32_t b, const uint32_t *__restrict__ rep,
+                  const unsigned long long *__restrict__ key, uint32_t *__restrict__ list) {
+    extern __shared__ uint4 s_bits4[];
+    const uint32_t *s_bits = reinterpret_cast<const uint32_t *>(s_bits4);
+#pragma unroll 8
+    for (uint32_t i = threadIdx.x; i < b * kWords / 4; i += blockDim.x) s_bits4[i] = reinterpret_cast<const uint4 *>(bits)[i];
+    __syncthreads();
+    if (threadIdx.x >= 32) return;
+    const uint32_t lane = threadIdx.x;
+    // lane w holds rows 32 w .. 32 w + 31 of the sub-block: covered by an earlier mark (rows past b count as covered)
+    bool set[kWords];
+#pragma unroll
+    for (uint32_t w = 0; w < kWords; ++w) {  // all 32 loads in flight: every lane reads a row of the sub-block
+        const uint64_t row = a + min(w * 32 + lane, b - 1);
+        set[w] = Nearest ? key[row] != 0 : rep[row] != kNone;
+    }
+    uint32_t cov = 0;
+#pragma unroll
+    for (uint32_t w = 0; w < kWords; ++w) {
+        const uint32_t m = __ballot_sync(0xffffffffu, set[w] || w * 32 + lane >= b);
+        if (lane == w) cov = m;
+    }
+    // every step takes the first uncovered row: a ballot skips any run of covered rows at once
+    uint32_t reps = 0;
+    for (;;) {
+        const uint32_t open = __ballot_sync(0xffffffffu, cov != 0xffffffffu);
+        if (!open) break;
+        const uint32_t w = __ffs(open) - 1;
+        const uint32_t x = __ffs(~__shfl_sync(0xffffffffu, cov, w)) - 1;
+        cov |= s_bits[(w * 32 + x) * kWords + lane];
+        if (lane == w) {
+            cov |= 1u << x;
+            reps |= 1u << x;
+        }
+    }
+    const uint32_t cnt = __popc(reps);
+    uint32_t end = cnt;  // inclusive prefix sum over the lanes
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, end, d);
+        if (lane >= d) end += y;
+    }
+    uint32_t at = end - cnt;
+    for (uint32_t m = reps; m; m &= m - 1) list[1 + at++] = (uint32_t)a + lane * 32 + __ffs(m) - 1;
+    if (lane == 31) list[0] = end;
+}
+
+// The listed representatives' tile rows (tile row 0 is sketch row0), columns j > r.  One CTA step covers
+// kMarkCols columns of one representative with 16-byte loads, four per thread in flight.
+template <bool Nearest>
+__global__ void __launch_bounds__(256)
+derep_mark_kernel(const uint32_t *__restrict__ tile, uint64_t n, uint64_t row0, uint32_t min_same, const uint32_t *__restrict__ list,
+                  uint32_t *rep, unsigned long long *key) {
+    const uint64_t chunks = (n + kMarkCols - 1) / kMarkCols;
+    const uint64_t items = (uint64_t)list[0] * chunks;
+    const bool vec = (n & 3) == 0;  // rows are 16-byte aligned
+    for (uint64_t it = blockIdx.x; it < items; it += gridDim.x) {
+        const uint32_t r = list[1 + it / chunks];
+        const uint64_t c0 = (it % chunks) * kMarkCols;
+        if (c0 + kMarkCols <= (uint64_t)r + 1) continue;  // all at or left of the diagonal
+        const uint32_t *row = tile + (r - row0) * n;
+        uint32_t v[4][4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const uint64_t j0 = c0 + (q * 256 + threadIdx.x) * 4;
+            if (vec && j0 + 3 < n) {
+                const uint4 u = *reinterpret_cast<const uint4 *>(row + j0);
+                v[q][0] = u.x; v[q][1] = u.y; v[q][2] = u.z; v[q][3] = u.w;
+            } else {
+                for (int t = 0; t < 4; ++t) v[q][t] = j0 + t < n ? row[j0 + t] : 0;
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            if (max(max(v[q][0], v[q][1]), max(v[q][2], v[q][3])) < min_same) continue;
+            const uint64_t j0 = c0 + (q * 256 + threadIdx.x) * 4;
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const uint64_t j = j0 + t;
+                if (v[q][t] < min_same || j <= r) continue;
+                if (Nearest) atomicMax(key + j, (unsigned long long)v[q][t] << 32 | (uint32_t)~r);
+                else atomicMin(rep + j, r);
+            }
+        }
+    }
+}
+
+template <bool Nearest>
+__global__ void __launch_bounds__(256)
+derep_finish_kernel(uint32_t *__restrict__ rep, const unsigned long long *__restrict__ key, uint64_t n,
+                    unsigned long long *__restrict__ n_reps) {
+    const uint32_t lane = threadIdx.x & 31u;
+    uint32_t reps = 0;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n; i0 += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t i = i0 + lane;
+        if (i >= n) continue;
+        const bool self = Nearest ? key[i] == 0 : rep[i] == kNone;
+        if (self) rep[i] = (uint32_t)i;
+        else if (Nearest) rep[i] = ~(uint32_t)key[i];
+        reps += self;
+    }
+    reps = __reduce_add_sync(0xffffffffu, reps);
+    if (n_reps && lane == 0 && reps) atomicAdd(n_reps, (unsigned long long)reps);
+}
+
+template <bool Nearest>
+int derep_tiles(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t *d_rep, unsigned long long *d_key,
+                unsigned long long *d_n_reps, StreamScratch &tmp, cudaStream_t st) {
+    uint32_t *d_bits = nullptr, *d_list = nullptr;
+    if (tmp.alloc(&d_bits, kDerepRows * kWords + 1 + kDerepRows) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("cudaMallocAsync for the dereplication sub-block failed");
+        return PG_ERR_NOMEM;
+    }
+    d_list = d_bits + kDerepRows * kWords;
+    int rc = func_smem((const void *)derep_walk_kernel<Nearest>, kDerepRows * kWords * 4);
+    if (rc != PG_OK) return rc;
+
+    DistancePlan plan;
+    rc = distance_plan_create(d_sk, n, s, st, &plan);
+    const uint64_t rows_per = distance_tile_rows(n, n);
+    uint32_t *d_tile = nullptr;
+    if (rc == PG_OK) {
+        cudaError_t e = cudaMallocAsync(&d_tile, rows_per * n * 4, st);
+        if (e != cudaSuccess) { cudaGetLastError(); set_error("cudaMallocAsync(%llu) for the pair tile failed", (unsigned long long)(rows_per * n * 4)); rc = PG_ERR_NOMEM; }
+        else tmp.adopt(d_tile);
+    }
+    const unsigned grid = (unsigned)sm_count() * 8;
+    for (uint64_t rb = 0; rb < n && rc == PG_OK; rb += rows_per) {
+        const uint64_t re = std::min(n, rb + rows_per);
+        rc = distance_plan_rows(plan, rb, re, d_tile, nullptr, st);
+        if (rc != PG_OK) break;
+        for (uint64_t a = rb; a < re; a += kDerepRows) {
+            const uint32_t b = (uint32_t)std::min<uint64_t>(kDerepRows, re - a);
+            derep_links_kernel<<<(b * kWords + 7) / 8, 256, 0, st>>>(d_tile, n, a - rb, a, b, min_same, d_bits);
+            note_launch("derep_links_kernel");
+            derep_walk_kernel<Nearest><<<1, 1024, b * kWords * 4, st>>>(d_bits, a, b, d_rep, d_key, d_list);
+            note_launch("derep_walk_kernel");
+            derep_mark_kernel<Nearest><<<grid, 256, 0, st>>>(d_tile, n, rb, min_same, d_list, d_rep, d_key);
+            note_launch("derep_mark_kernel");
+        }
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) rc = cuda_fail(e, "dereplication sub-block kernels", __FILE__, __LINE__);
+    }
+    distance_plan_destroy(plan, st);
+    if (rc != PG_OK) return rc;
+    derep_finish_kernel<Nearest><<<(unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(d_rep, d_key, n, d_n_reps);
+    PG_LAUNCH_CHECK("derep_finish_kernel");
+    return PG_OK;
+}
+
+}  // namespace
+
+int mash_derep_check(uint64_t n, int s, uint32_t min_same, uint32_t flags) {
+    if (flags & ~PG_DEREP_NEAREST) { set_error("unknown dereplication flags 0x%x", flags); return PG_ERR_ARG; }
+    return mash_cluster_check(n, s, min_same);
+}
+
+int launch_mash_derep(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t flags, uint32_t *d_rep,
+                      unsigned long long *d_n_reps, cudaStream_t st) {
+    if (d_n_reps) PG_CUDA(cudaMemsetAsync(d_n_reps, 0, 8, st));
+    int rc = mash_derep_check(n, s, min_same, flags);
+    if (rc != PG_OK || n == 0) return rc;
+    StreamScratch tmp(st);  // keys (nearest), the sub-block's link bits and list, the tile: freed on every way out
+    if (!(flags & PG_DEREP_NEAREST)) {
+        PG_CUDA(cudaMemsetAsync(d_rep, 0xff, n * 4, st));  // kNone: the assignment is built in place
+        return derep_tiles<false>(d_sk, n, s, min_same, d_rep, nullptr, d_n_reps, tmp, st);
+    }
+    unsigned long long *d_key = nullptr;
+    if (tmp.alloc(&d_key, n) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("cudaMallocAsync(%llu) for the dereplication keys failed", (unsigned long long)(n * 8));
+        return PG_ERR_NOMEM;
+    }
+    PG_CUDA(cudaMemsetAsync(d_key, 0, n * 8, st));
+    return derep_tiles<true>(d_sk, n, s, min_same, d_rep, d_key, d_n_reps, tmp, st);
+}
+
+}  // namespace pg

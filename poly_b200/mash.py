@@ -415,6 +415,53 @@ def cluster(sketches, min_same: Optional[int] = None, max_distance: Optional[flo
     return labels, int(ng.value), int(nl.value)
 
 
+# ---- dereplicate: greedy representatives of a sketch set (pg_mash_dereplicate) ---------------------------
+PG_DEREP_NEAREST = 1
+
+
+def dereplicate(sketches, min_same: Optional[int] = None, max_distance: Optional[float] = None, nearest: bool = False):
+    """Representatives of a sketch set: sketches r < i are linked as in cluster (sketches[r].Similarity(sketches[i])
+    counts at least min_same matching hashes, or their Distance is <= max_distance).  In index order, i is a
+    representative iff no representative r < i is linked to i.  Every other sketch is assigned the smallest linked
+    representative, or with nearest=True the linked one with the largest count (smallest Distance), ties to the
+    smaller index.  Permute the set first for another priority.
+
+    sketches: what cluster takes.  Returns (rep [n] uint32, n_reps): rep[i] == i marks a representative.  CUDA
+    tensor sketches give a CUDA int32 tensor (carrying the uint32 bits) and a 0-dim int64 count tensor, ordered on
+    the current stream.  The pairs themselves are never materialised."""
+    if (min_same is None) == (max_distance is None):
+        raise ValueError("give exactly one of min_same and max_distance")
+    rows = _sketch_rows(sketches)
+    n, s = int(rows.shape[0]), int(rows.shape[1])
+    on_device = hasattr(rows, "data_ptr")
+    if on_device:
+        import torch
+    if max_distance is not None and s > 0:  # s == 0: the library reports the reference's panic
+        min_same = min_same_for_distance(max_distance, s)
+        if min_same == 0:
+            raise ValueError(f"max_distance {max_distance!r} links every pair: every Distance is <= it")
+        if min_same == s + 1:  # no matching count reaches the cut: every sketch represents itself
+            if on_device:
+                return torch.arange(n, dtype=torch.int32, device=rows.device), torch.tensor(n, device=rows.device)
+            return np.arange(n, dtype=np.uint32), n
+    min_same = 1 if min_same is None else int(min_same)
+    if not 0 <= min_same <= 0xFFFFFFFF:
+        raise ValueError("min_same must fit 32 bits")
+    flags = PG_DEREP_NEAREST if nearest else 0
+    if on_device:
+        dev = rows.device
+        rep = torch.empty(n, dtype=torch.int32, device=dev)
+        count = torch.zeros((), dtype=torch.int64, device=dev)
+        rc = _lib.lib().pg_mash_dereplicate_dev(rows.data_ptr(), n, s, min_same, flags, rep.data_ptr(), count.data_ptr(),
+                                                torch.cuda.current_stream(dev).cuda_stream)
+        _index_rc(rc)
+        return rep, count
+    rep = np.empty(n, dtype=np.uint32)
+    nr = C.c_uint64(0)
+    _index_rc(_lib.lib().pg_mash_dereplicate(rows.ctypes.data, n, s, min_same, flags, rep.ctypes.data, C.byref(nr)))
+    return rep, int(nr.value)
+
+
 # ---- single-process multi-GPU additions (pg_*_multi; SURVEY.md 8b / 8e) ----------------------------
 def _device_list(devices):
     if devices is None:
