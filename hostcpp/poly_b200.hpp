@@ -309,6 +309,20 @@ inline std::vector<Mash> MashesOf(const SketchSet &set) {
     return out;
 }
 
+namespace detail {
+// The n x s rows of mashes of one SketchSize s (0 for none) as the C ABI takes them; `what` names the set in the error.
+inline std::vector<uint32_t> FlatRows(const std::vector<Mash> &mashes, const char *what, int *s) {
+    *s = mashes.empty() ? 0 : mashes[0].SketchSize;
+    std::vector<uint32_t> flat;
+    flat.reserve(mashes.size() * (size_t)std::max(*s, 0));
+    for (auto &m : mashes) {
+        if (m.SketchSize != *s || (int)m.Sketches.size() < *s) throw std::invalid_argument(std::string(what) + " must share one SketchSize");
+        flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + *s);
+    }
+    return flat;
+}
+}  // namespace detail
+
 // ---- sketch index: top-k nearest references (pg_mash_index_*) ----------------------------------------
 // One reference of a query's result: refs[Ref], its matching count as queries[q].Similarity(refs[Ref]) counts it
 // (the query is the receiver, mash.go:107-135), and queries[q].Distance(refs[Ref]).
@@ -324,13 +338,7 @@ class Index {
 
 public:
     explicit Index(const std::vector<Mash> &refs) {
-        s_ = refs.empty() ? 0 : refs[0].SketchSize;
-        std::vector<uint32_t> flat;
-        flat.reserve(refs.size() * (size_t)std::max(s_, 0));
-        for (auto &m : refs) {
-            if (m.SketchSize != s_ || (int)m.Sketches.size() < s_) throw std::invalid_argument("references must share one SketchSize");
-            flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + s_);
-        }
+        const std::vector<uint32_t> flat = detail::FlatRows(refs, "references", &s_);
         int rc = pg_mash_index_create(flat.data(), refs.size(), s_, &h_);
         if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
         check(rc);
@@ -340,12 +348,8 @@ public:
     ~Index() { pg_mash_index_free(h_); }
     // For each query, up to k references with Same >= minSame, by Same descending and then Ref ascending.
     std::vector<std::vector<Neighbor>> Nearest(const std::vector<Mash> &queries, uint32_t k, uint32_t minSame = 1) const {
-        const int sq = queries.empty() ? 0 : queries[0].SketchSize;
-        std::vector<uint32_t> flat;
-        for (auto &m : queries) {
-            if (m.SketchSize != sq || (int)m.Sketches.size() < sq) throw std::invalid_argument("queries must share one SketchSize");
-            flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + sq);
-        }
+        int sq;
+        const std::vector<uint32_t> flat = detail::FlatRows(queries, "queries", &sq);
         const size_t nq = queries.size();
         std::vector<uint32_t> ref(nq * k), same(nq * k), nh(nq);
         std::vector<double> dist(nq * k);
@@ -375,13 +379,8 @@ inline uint32_t MinSameForDistance(double maxDistance, int den) {
 // Sketches i < j of one SketchSize are linked when mashes[i].Similarity(mashes[j]) counts at least minSame matching
 // hashes (the lower index is the receiver); the groups are the connected components.
 inline Clusters Cluster(const std::vector<Mash> &mashes, uint32_t minSame) {
-    const int s = mashes.empty() ? 0 : mashes[0].SketchSize;
-    std::vector<uint32_t> flat;
-    flat.reserve(mashes.size() * (size_t)std::max(s, 0));
-    for (auto &m : mashes) {
-        if (m.SketchSize != s || (int)m.Sketches.size() < s) throw std::invalid_argument("sketches must share one SketchSize");
-        flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + s);
-    }
+    int s;
+    const std::vector<uint32_t> flat = detail::FlatRows(mashes, "sketches", &s);
     Clusters out;
     out.Labels.resize(mashes.size());
     int rc = pg_mash_cluster(flat.data(), mashes.size(), s, minSame, out.Labels.data(), &out.Groups, &out.Links);
@@ -400,13 +399,8 @@ struct Representatives {
 // other i gets the smallest linked representative, or with `nearest` the one with the largest count (ties to the
 // smaller index).
 inline Representatives Dereplicate(const std::vector<Mash> &mashes, uint32_t minSame, bool nearest = false) {
-    const int s = mashes.empty() ? 0 : mashes[0].SketchSize;
-    std::vector<uint32_t> flat;
-    flat.reserve(mashes.size() * (size_t)std::max(s, 0));
-    for (auto &m : mashes) {
-        if (m.SketchSize != s || (int)m.Sketches.size() < s) throw std::invalid_argument("sketches must share one SketchSize");
-        flat.insert(flat.end(), m.Sketches.begin(), m.Sketches.begin() + s);
-    }
+    int s;
+    const std::vector<uint32_t> flat = detail::FlatRows(mashes, "sketches", &s);
     Representatives out;
     out.Rep.resize(mashes.size());
     int rc = pg_mash_dereplicate(flat.data(), mashes.size(), s, minSame, nearest ? PG_DEREP_NEAREST : 0u, out.Rep.data(), &out.NReps);

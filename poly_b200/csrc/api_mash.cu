@@ -25,26 +25,24 @@ static inline uint64_t kmers_of(uint64_t len, int k) { return len > (uint64_t)k 
 // informative words of the sketch of a read of `len` bytes
 static inline uint64_t sketch_words(uint64_t len, int k, int s) { return std::min<uint64_t>(kmers_of(len, k), (uint64_t)s); }
 
-// Rows [rb, re) of a plan's matching counts and/or distances into host arrays that start at row rb, in row
-// blocks of <= 64 Mi pairs per pass
-int plan_rows_to_host(const DistancePlan &plan, uint64_t rb, uint64_t re, uint32_t *same, double *distance, cudaStream_t st) {
-    const uint64_t n = plan.n, rows_per = std::max<uint64_t>(8, ((64ull << 20) / n) & ~7ull);
-    for (uint64_t b = rb; b < re; b += rows_per) {
-        const uint64_t e = std::min(re, b + rows_per), cells = (e - b) * n;
-        StreamScratch tmp(st);
-        uint32_t *d_same = nullptr;
-        double *d_dist = nullptr;
-        int rc;
-        if (same && (rc = scratch_alloc(tmp, &d_same, cells))) return rc;
-        if (distance && (rc = scratch_alloc(tmp, &d_dist, cells))) return rc;
-        if ((rc = distance_plan_rows(plan, b, e, d_same, d_dist, st)) != PG_OK) return rc;
+// Rows [rb, re) of the n x s sketches' matching counts and/or distances into host arrays that start at row rb, in
+// row blocks of <= 64 Mi pairs, each copied out and waited for before the next
+int rows_to_host(const uint32_t *d_sk, uint64_t n, int s, uint64_t rb, uint64_t re, uint32_t *same, double *distance, cudaStream_t st) {
+    const uint64_t rows_per = std::max<uint64_t>(8, ((64ull << 20) / n) & ~7ull);
+    return distance_plan_tiles(d_sk, n, s, rb, re, rows_per, same != nullptr, distance != nullptr, st,
+                               [&](const uint32_t *d_same, const double *d_dist, uint64_t b, uint64_t e) {
+        const uint64_t cells = (e - b) * n;
         if (same) PG_CUDA(cudaMemcpyAsync(same + (b - rb) * n, d_same, cells * 4, cudaMemcpyDeviceToHost, st));
         if (distance) PG_CUDA(cudaMemcpyAsync(distance + (b - rb) * n, d_dist, cells * 8, cudaMemcpyDeviceToHost, st));
         PG_CUDA(cudaStreamSynchronize(st));
-    }
-    return PG_OK;
+        return PG_OK;
+    });
 }
 
+static int check_rows(uint64_t n, uint64_t row_begin, uint64_t row_end) {
+    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    return PG_OK;
+}
 static int check_ks(int32_t k, int32_t s) {
     if (k < 0) { set_error("kmerSize %d < 0: the reference panics (slice bounds)", k); return PG_ERR_ARG; }
     if (s < 0) { set_error("sketchSize %d < 0: the reference panics (makeslice)", s); return PG_ERR_ARG; }
@@ -645,10 +643,7 @@ int pg_mash_sketch_distance_multi(const uint8_t *bases, uint64_t n_reads, uint32
             }
             if (sketches && nl) PG_CUDA(cudaMemcpyAsync(sketches + lo * (uint64_t)s, d_full + lo * (uint64_t)s, nl * (uint64_t)s * 4, cudaMemcpyDeviceToHost, st));
             if ((same || distance) && nl) {
-                DistancePlan plan;
-                int c = distance_plan_create(d_full, n, s, st, &plan);
-                if (c == PG_OK) c = plan_rows_to_host(plan, lo, hi, same ? same + lo * n : nullptr, distance ? distance + lo * n : nullptr, st);
-                distance_plan_destroy(plan, st);
+                const int c = rows_to_host(d_full, n, s, lo, hi, same ? same + lo * n : nullptr, distance ? distance + lo * n : nullptr, st);
                 if (c != PG_OK) return c;
             }
             PG_CUDA(cudaStreamSynchronize(st));
@@ -712,35 +707,27 @@ int pg_mash_similarity_pairs(const uint32_t *sketches, const uint64_t *sk_offset
 int pg_mash_distance_block_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint64_t row_begin,
                                uint64_t row_end, uint32_t *d_same, double *d_distance, void *stream) {
     int rc = ensure_device();
-    if (rc != PG_OK) return rc;
-    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    if (rc != PG_OK || (rc = check_rows(n, row_begin, row_end)) != PG_OK) return rc;
     return launch_distance_block(d_sketches, n, s, row_begin, row_end, d_same, d_distance, (cudaStream_t)stream);
 }
 
 int pg_mash_distance_block(const uint32_t *sketches, uint64_t n, int32_t s, uint64_t row_begin,
                            uint64_t row_end, uint32_t *same, double *distance) {
     int rc = ensure_device();
-    if (rc != PG_OK) return rc;
-    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    if (rc != PG_OK || (rc = check_rows(n, row_begin, row_end)) != PG_OK) return rc;
     if (row_end == row_begin || n == 0) return PG_OK;
     if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
     HostCall c;
     const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)s);
-    if ((rc = c.error())) return rc;
-    // one plan (sortedness + join index) for the whole call
-    DistancePlan plan;
-    rc = distance_plan_create(d_sk, n, s, c.st, &plan);
-    if (rc == PG_OK) rc = plan_rows_to_host(plan, row_begin, row_end, same, distance, c.st);
-    distance_plan_destroy(plan, c.st);
-    return rc != PG_OK ? rc : c.finish();
+    if ((rc = c.error()) || (rc = rows_to_host(d_sk, n, s, row_begin, row_end, same, distance, c.st))) return rc;
+    return c.finish();
 }
 
 int pg_mash_distance_sparse_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, uint64_t row_begin, uint64_t row_end, uint32_t flags,
                                 uint32_t *d_pair_i, uint32_t *d_pair_j, uint32_t *d_pair_same, uint64_t pairs_cap, uint64_t *d_n_pairs,
                                 void *stream) {
     int rc = ensure_device();
-    if (rc != PG_OK) return rc;
-    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    if (rc != PG_OK || (rc = check_rows(n, row_begin, row_end)) != PG_OK) return rc;
     if (!d_n_pairs || (pairs_cap && (!d_pair_i || !d_pair_j || !d_pair_same))) { set_error("null buffer"); return PG_ERR_ARG; }
     return launch_distance_sparse(d_sketches, n, s, row_begin, row_end, flags, d_pair_i, d_pair_j, d_pair_same, pairs_cap,
                                   (unsigned long long *)d_n_pairs, (cudaStream_t)stream);
@@ -752,7 +739,7 @@ int pg_mash_distance_sparse(const uint32_t *sketches, uint64_t n, int32_t s, uin
     if (rc != PG_OK) return rc;
     if (!n_pairs) { set_error("null buffer"); return PG_ERR_ARG; }
     *n_pairs = 0;
-    if (row_end > n || row_begin > row_end) { set_error("bad row range"); return PG_ERR_ARG; }
+    if ((rc = check_rows(n, row_begin, row_end)) != PG_OK) return rc;
     if (row_end == row_begin || n == 0) return PG_OK;
     if (s <= 0) { set_error("distance over sketches of size %d: the reference panics", s); return PG_ERR_PANIC; }
     if (pairs_cap && (!pair_i || !pair_j || !pair_same)) { set_error("null buffer"); return PG_ERR_ARG; }

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <functional>
 #include <vector>
 
 #include "../../include/poly_b200.h"
@@ -210,8 +211,26 @@ struct DistancePlan {
 int distance_plan_create(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, DistancePlan *plan);
 int distance_plan_rows(const DistancePlan &plan, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st);
 void distance_plan_destroy(DistancePlan &plan, cudaStream_t st);
-// distance.cu: rows per dense tile of the passes that consume a plan's tiles on the device (sparse pairs, cluster); n > 0
+// distance.cu: rows per dense tile of the passes that consume a plan's tiles on the device (sparse pairs, cluster,
+// dereplicate); n > 0
 uint64_t distance_tile_rows(uint64_t n, uint64_t rows);
+// distance.cu: rows [row_begin, row_end) (row_begin < row_end, n > 0) of n equal-size sketches as dense tiles of at most rows_per rows, over one
+// DistancePlan and one tile buffer (counts if want_same, distances if want_dist).  consume(same, dist, rb, re) runs
+// once each tile of rows [rb, re) is enqueued, with the unwanted buffer NULL; it may return early on an error.  The
+// plan and the tile are released on every way out; the result is the first code other than PG_OK.
+int distance_plan_tiles(const uint32_t *d_sk, uint64_t n, int s, uint64_t row_begin, uint64_t row_end, uint64_t rows_per,
+                        bool want_same, bool want_dist, cudaStream_t st,
+                        const std::function<int(const uint32_t *same, const double *dist, uint64_t rb, uint64_t re)> &consume);
+// Counts p[i .. i + 3] of an array of `end` counts: one 16-byte load when vec (rows of a multiple of 4 counts, so
+// every quad of a row-major tile is 16-byte aligned) and the quad is in range, else one by one with zeros past end.
+__device__ __forceinline__ void load_count_quad(const uint32_t *p, uint64_t i, uint64_t end, bool vec, uint32_t (&v)[4]) {
+    if (vec && i + 3 < end) {
+        const uint4 q = *reinterpret_cast<const uint4 *>(p + i);
+        v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+    } else {
+        for (int t = 0; t < 4; ++t) v[t] = i + t < end ? p[i + t] : 0;
+    }
+}
 // mash_cluster.cu: single-linkage groups at same >= min_same; label[i] = smallest index of i's group, the
 // counters (either may be NULL) = number of groups and of linked pairs i < j.  mash_cluster_check is the
 // argument rule of pg_mash_cluster, which the host entry point applies before it copies anything.

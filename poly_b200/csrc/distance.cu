@@ -200,13 +200,8 @@ compact_pairs_kernel(const uint32_t *__restrict__ tile, uint64_t rows, uint64_t 
     // the loop bound is warp-uniform (the ballots below need every lane): a warp covers 128 consecutive words
     for (uint64_t w0 = ((uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) * 4; w0 < total; w0 += (uint64_t)gridDim.x * blockDim.x * 4) {
         const uint64_t e0 = w0 + lane * 4;
-        uint32_t v[4] = {0, 0, 0, 0};
-        if (e0 + 3 < total && (n & 3) == 0) {
-            const uint4 q = *reinterpret_cast<const uint4 *>(tile + e0);  // rows are 16-byte aligned when n % 4 == 0
-            v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
-        } else {
-            for (int t = 0; t < 4; ++t) if (e0 + t < total) v[t] = tile[e0 + t];
-        }
+        uint32_t v[4];
+        load_count_quad(tile, e0, total, (n & 3) == 0, v);
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
             const uint64_t e = e0 + t;
@@ -243,28 +238,14 @@ int launch_distance_sparse(const uint32_t *d_sk, uint64_t n, int s, uint64_t row
     PG_CUDA(cudaMemsetAsync(d_n_pairs, 0, 8, st));
     if (row_end <= row_begin || n == 0) return PG_OK;
     if (n > 0xffffffffull) { set_error("too many sketches for 32-bit pair indices"); return PG_ERR_ARG; }
-    DistancePlan plan;
-    int rc = distance_plan_create(d_sk, n, s, st, &plan);
-    const uint64_t rows_per = distance_tile_rows(n, row_end - row_begin);
-    uint32_t *d_tile = nullptr;
-    if (rc == PG_OK) {
-        cudaError_t e = cudaMallocAsync(&d_tile, rows_per * n * 4, st);
-        if (e != cudaSuccess) { cudaGetLastError(); set_error("cudaMallocAsync(%llu) for the pair tile failed", (unsigned long long)(rows_per * n * 4)); rc = PG_ERR_NOMEM; }
-    }
-    for (uint64_t rb = row_begin; rb < row_end && rc == PG_OK; rb += rows_per) {
-        const uint64_t re = std::min(row_end, rb + rows_per);
-        rc = distance_plan_rows(plan, rb, re, d_tile, nullptr, st);
-        if (rc != PG_OK) break;
+    return distance_plan_tiles(d_sk, n, s, row_begin, row_end, distance_tile_rows(n, row_end - row_begin), true, false, st,
+                               [&](const uint32_t *tile, const double *, uint64_t rb, uint64_t re) {
         const uint64_t quads = ((re - rb) * n + 3) / 4;
         compact_pairs_kernel<<<(unsigned)std::min<uint64_t>((quads + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(
-            d_tile, re - rb, n, rb, flags & PG_PAIRS_UPPER, d_i, d_j, d_same, cap, d_n_pairs);
-        note_launch("compact_pairs_kernel");
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) rc = cuda_fail(e, "compact_pairs_kernel", __FILE__, __LINE__);
-    }
-    if (d_tile) cudaFreeAsync(d_tile, st);
-    distance_plan_destroy(plan, st);
-    return rc;
+            tile, re - rb, n, rb, flags & PG_PAIRS_UPPER, d_i, d_j, d_same, cap, d_n_pairs);
+        PG_LAUNCH_CHECK("compact_pairs_kernel");
+        return PG_OK;
+    });
 }
 
 int launch_similarity_pairs(const uint32_t *d_sk, const uint64_t *d_off, uint64_t n_sk,
@@ -344,6 +325,29 @@ int distance_plan_rows(const DistancePlan &plan, uint64_t row_begin, uint64_t ro
         PG_LAUNCH_CHECK("distance_block_kernel");
     }
     return PG_OK;
+}
+
+int distance_plan_tiles(const uint32_t *d_sk, uint64_t n, int s, uint64_t row_begin, uint64_t row_end, uint64_t rows_per,
+                        bool want_same, bool want_dist, cudaStream_t st,
+                        const std::function<int(const uint32_t *same, const double *dist, uint64_t rb, uint64_t re)> &consume) {
+    DistancePlan plan;
+    int rc = distance_plan_create(d_sk, n, s, st, &plan);
+    StreamScratch tmp(st);
+    const uint64_t cells = std::min(rows_per, row_end - row_begin) * n;
+    uint32_t *d_same = nullptr;
+    double *d_dist = nullptr;
+    if (rc == PG_OK && ((want_same && tmp.alloc(&d_same, cells) != cudaSuccess) || (want_dist && tmp.alloc(&d_dist, cells) != cudaSuccess))) {
+        cudaGetLastError();
+        set_error("cudaMallocAsync(%llu) for the pair tile failed", (unsigned long long)(cells * (want_same * 4 + want_dist * 8)));
+        rc = PG_ERR_NOMEM;
+    }
+    for (uint64_t rb = row_begin; rb < row_end && rc == PG_OK; rb += rows_per) {
+        const uint64_t re = std::min(row_end, rb + rows_per);
+        rc = distance_plan_rows(plan, rb, re, d_same, d_dist, st);
+        if (rc == PG_OK) rc = consume(d_same, d_dist, rb, re);
+    }
+    distance_plan_destroy(plan, st);
+    return rc;
 }
 
 int launch_distance_block(const uint32_t *d_sk, uint64_t n, int s, uint64_t row_begin,

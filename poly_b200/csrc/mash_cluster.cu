@@ -66,13 +66,8 @@ cluster_link_kernel(const uint32_t *__restrict__ tile, uint64_t rows, uint64_t n
     // the loop bound is warp-uniform: the warp reduction behind the loop needs every lane
     for (uint64_t w0 = ((uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) * 4; w0 < total; w0 += (uint64_t)gridDim.x * blockDim.x * 4) {
         const uint64_t e0 = w0 + lane * 4;
-        uint32_t v[4] = {0, 0, 0, 0};
-        if (e0 + 3 < total && vec) {
-            const uint4 q = *reinterpret_cast<const uint4 *>(tile + e0);
-            v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
-        } else {
-            for (int t = 0; t < 4; ++t) if (e0 + t < total) v[t] = tile[e0 + t];
-        }
+        uint32_t v[4];
+        load_count_quad(tile, e0, total, vec, v);
         // most of a tile is zeros: nothing below this line runs for them (min_same >= 1)
         if (max(max(v[0], v[1]), max(v[2], v[3])) < min_same) continue;
         uint64_t i = row0 + e0 / n, j = e0 % n;
@@ -141,27 +136,14 @@ int launch_mash_cluster(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_sa
     cluster_init_kernel<<<row_blocks, 256, 0, st>>>(d_parent, n);
     PG_LAUNCH_CHECK("cluster_init_kernel");
 
-    DistancePlan plan;
-    rc = distance_plan_create(d_sk, n, s, st, &plan);
-    const uint64_t rows_per = distance_tile_rows(n, n);
-    uint32_t *d_tile = nullptr;
-    if (rc == PG_OK) {
-        e = cudaMallocAsync(&d_tile, rows_per * n * 4, st);
-        if (e != cudaSuccess) { cudaGetLastError(); set_error("cudaMallocAsync(%llu) for the pair tile failed", (unsigned long long)(rows_per * n * 4)); rc = PG_ERR_NOMEM; }
-        else tmp.adopt(d_tile);
-    }
-    for (uint64_t rb = 0; rb < n && rc == PG_OK; rb += rows_per) {
-        const uint64_t re = std::min(n, rb + rows_per);
-        rc = distance_plan_rows(plan, rb, re, d_tile, nullptr, st);
-        if (rc != PG_OK) break;
+    rc = distance_plan_tiles(d_sk, n, s, 0, n, distance_tile_rows(n, n), true, false, st,
+                             [&](const uint32_t *tile, const double *, uint64_t rb, uint64_t re) {
         const uint64_t quads = ((re - rb) * n + 3) / 4;
         cluster_link_kernel<<<(unsigned)std::min<uint64_t>((quads + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(
-            d_tile, re - rb, n, rb, min_same, d_parent, d_cnt);
-        note_launch("cluster_link_kernel");
-        e = cudaGetLastError();
-        if (e != cudaSuccess) rc = cuda_fail(e, "cluster_link_kernel", __FILE__, __LINE__);
-    }
-    distance_plan_destroy(plan, st);
+            tile, re - rb, n, rb, min_same, d_parent, d_cnt);
+        PG_LAUNCH_CHECK("cluster_link_kernel");
+        return PG_OK;
+    });
     if (rc != PG_OK) return rc;
     cluster_flatten_kernel<<<row_blocks, 256, 0, st>>>(d_parent, n, d_label, d_cnt + 1);
     PG_LAUNCH_CHECK("cluster_flatten_kernel");

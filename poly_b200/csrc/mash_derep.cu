@@ -113,15 +113,7 @@ derep_mark_kernel(const uint32_t *__restrict__ tile, uint64_t n, uint64_t row0, 
         const uint32_t *row = tile + (r - row0) * n;
         uint32_t v[4][4];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const uint64_t j0 = c0 + (q * 256 + threadIdx.x) * 4;
-            if (vec && j0 + 3 < n) {
-                const uint4 u = *reinterpret_cast<const uint4 *>(row + j0);
-                v[q][0] = u.x; v[q][1] = u.y; v[q][2] = u.z; v[q][3] = u.w;
-            } else {
-                for (int t = 0; t < 4; ++t) v[q][t] = j0 + t < n ? row[j0 + t] : 0;
-            }
-        }
+        for (int q = 0; q < 4; ++q) load_count_quad(row, c0 + (q * 256 + threadIdx.x) * 4, n, vec, v[q]);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             if (max(max(v[q][0], v[q][1]), max(v[q][2], v[q][3])) < min_same) continue;
@@ -168,33 +160,20 @@ int derep_tiles(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint
     int rc = func_smem((const void *)derep_walk_kernel<Nearest>, kDerepRows * kWords * 4);
     if (rc != PG_OK) return rc;
 
-    DistancePlan plan;
-    rc = distance_plan_create(d_sk, n, s, st, &plan);
-    const uint64_t rows_per = distance_tile_rows(n, n);
-    uint32_t *d_tile = nullptr;
-    if (rc == PG_OK) {
-        cudaError_t e = cudaMallocAsync(&d_tile, rows_per * n * 4, st);
-        if (e != cudaSuccess) { cudaGetLastError(); set_error("cudaMallocAsync(%llu) for the pair tile failed", (unsigned long long)(rows_per * n * 4)); rc = PG_ERR_NOMEM; }
-        else tmp.adopt(d_tile);
-    }
     const unsigned grid = (unsigned)sm_count() * 8;
-    for (uint64_t rb = 0; rb < n && rc == PG_OK; rb += rows_per) {
-        const uint64_t re = std::min(n, rb + rows_per);
-        rc = distance_plan_rows(plan, rb, re, d_tile, nullptr, st);
-        if (rc != PG_OK) break;
+    rc = distance_plan_tiles(d_sk, n, s, 0, n, distance_tile_rows(n, n), true, false, st,
+                             [&](const uint32_t *tile, const double *, uint64_t rb, uint64_t re) {
         for (uint64_t a = rb; a < re; a += kDerepRows) {
             const uint32_t b = (uint32_t)std::min<uint64_t>(kDerepRows, re - a);
-            derep_links_kernel<<<(b * kWords + 7) / 8, 256, 0, st>>>(d_tile, n, a - rb, a, b, min_same, d_bits);
-            note_launch("derep_links_kernel");
+            derep_links_kernel<<<(b * kWords + 7) / 8, 256, 0, st>>>(tile, n, a - rb, a, b, min_same, d_bits);
+            PG_LAUNCH_CHECK("derep_links_kernel");
             derep_walk_kernel<Nearest><<<1, 1024, b * kWords * 4, st>>>(d_bits, a, b, d_rep, d_key, d_list);
-            note_launch("derep_walk_kernel");
-            derep_mark_kernel<Nearest><<<grid, 256, 0, st>>>(d_tile, n, rb, min_same, d_list, d_rep, d_key);
-            note_launch("derep_mark_kernel");
+            PG_LAUNCH_CHECK("derep_walk_kernel");
+            derep_mark_kernel<Nearest><<<grid, 256, 0, st>>>(tile, n, rb, min_same, d_list, d_rep, d_key);
+            PG_LAUNCH_CHECK("derep_mark_kernel");
         }
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) rc = cuda_fail(e, "dereplication sub-block kernels", __FILE__, __LINE__);
-    }
-    distance_plan_destroy(plan, st);
+        return PG_OK;
+    });
     if (rc != PG_OK) return rc;
     derep_finish_kernel<Nearest><<<(unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(d_rep, d_key, n, d_n_reps);
     PG_LAUNCH_CHECK("derep_finish_kernel");
@@ -213,7 +192,7 @@ int launch_mash_derep(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same
     if (d_n_reps) PG_CUDA(cudaMemsetAsync(d_n_reps, 0, 8, st));
     int rc = mash_derep_check(n, s, min_same, flags);
     if (rc != PG_OK || n == 0) return rc;
-    StreamScratch tmp(st);  // keys (nearest), the sub-block's link bits and list, the tile: freed on every way out
+    StreamScratch tmp(st);  // keys (nearest), the sub-block's link bits and list: freed on every way out
     if (!(flags & PG_DEREP_NEAREST)) {
         PG_CUDA(cudaMemsetAsync(d_rep, 0xff, n * 4, st));  // kNone: the assignment is built in place
         return derep_tiles<false>(d_sk, n, s, min_same, d_rep, nullptr, d_n_reps, tmp, st);

@@ -373,6 +373,25 @@ class SketchIndex:
                 pass
 
 
+def _link_rows(sketches, min_same: Optional[int], max_distance: Optional[float]):
+    """(rows, n, s, min_same) of a cluster or dereplicate call; min_same is None when no matching count reaches
+    max_distance, so that nothing links and the caller returns its trivial result without a launch."""
+    if (min_same is None) == (max_distance is None):
+        raise ValueError("give exactly one of min_same and max_distance")
+    rows = _sketch_rows(sketches)
+    n, s = int(rows.shape[0]), int(rows.shape[1])
+    if max_distance is not None and s > 0:  # s == 0: the library reports the reference's panic
+        min_same = min_same_for_distance(max_distance, s)
+        if min_same == 0:
+            raise ValueError(f"max_distance {max_distance!r} links every pair: every Distance is <= it")
+        if min_same == s + 1:
+            return rows, n, s, None
+    min_same = 1 if min_same is None else int(min_same)
+    if not 0 <= min_same <= 0xFFFFFFFF:
+        raise ValueError("min_same must fit 32 bits")
+    return rows, n, s, min_same
+
+
 # ---- cluster: single-linkage groups of a sketch set (pg_mash_cluster) -------------------------------------
 def cluster(sketches, min_same: Optional[int] = None, max_distance: Optional[float] = None):
     """Groups of a sketch set: sketches i < j are linked when sketches[i].Similarity(sketches[j]) counts at
@@ -383,24 +402,14 @@ def cluster(sketches, min_same: Optional[int] = None, max_distance: Optional[flo
     index in i's group, so labels[i] == i marks one representative per group; n_links counts the linked pairs.
     CUDA tensor sketches give a CUDA int32 label tensor (carrying the uint32 bits) and 0-dim int64 count
     tensors, ordered on the current stream.  The pairs themselves are never materialised."""
-    if (min_same is None) == (max_distance is None):
-        raise ValueError("give exactly one of min_same and max_distance")
-    rows = _sketch_rows(sketches)
-    n, s = int(rows.shape[0]), int(rows.shape[1])
+    rows, n, s, min_same = _link_rows(sketches, min_same, max_distance)
     on_device = hasattr(rows, "data_ptr")
     if on_device:
         import torch
-    if max_distance is not None and s > 0:  # s == 0: the library reports the reference's panic
-        min_same = min_same_for_distance(max_distance, s)
-        if min_same == 0:
-            raise ValueError(f"max_distance {max_distance!r} links every pair: every Distance is <= it")
-        if min_same == s + 1:  # no matching count reaches the cut: every sketch is its own group
-            if on_device:
-                return torch.arange(n, dtype=torch.int32, device=rows.device), torch.tensor(n, device=rows.device), torch.tensor(0, device=rows.device)
-            return np.arange(n, dtype=np.uint32), n, 0
-    min_same = 1 if min_same is None else int(min_same)
-    if not 0 <= min_same <= 0xFFFFFFFF:
-        raise ValueError("min_same must fit 32 bits")
+    if min_same is None:  # every sketch is its own group
+        if on_device:
+            return torch.arange(n, dtype=torch.int32, device=rows.device), torch.tensor(n, device=rows.device), torch.tensor(0, device=rows.device)
+        return np.arange(n, dtype=np.uint32), n, 0
     if on_device:
         dev = rows.device
         labels = torch.empty(n, dtype=torch.int32, device=dev)
@@ -429,24 +438,14 @@ def dereplicate(sketches, min_same: Optional[int] = None, max_distance: Optional
     sketches: what cluster takes.  Returns (rep [n] uint32, n_reps): rep[i] == i marks a representative.  CUDA
     tensor sketches give a CUDA int32 tensor (carrying the uint32 bits) and a 0-dim int64 count tensor, ordered on
     the current stream.  The pairs themselves are never materialised."""
-    if (min_same is None) == (max_distance is None):
-        raise ValueError("give exactly one of min_same and max_distance")
-    rows = _sketch_rows(sketches)
-    n, s = int(rows.shape[0]), int(rows.shape[1])
+    rows, n, s, min_same = _link_rows(sketches, min_same, max_distance)
     on_device = hasattr(rows, "data_ptr")
     if on_device:
         import torch
-    if max_distance is not None and s > 0:  # s == 0: the library reports the reference's panic
-        min_same = min_same_for_distance(max_distance, s)
-        if min_same == 0:
-            raise ValueError(f"max_distance {max_distance!r} links every pair: every Distance is <= it")
-        if min_same == s + 1:  # no matching count reaches the cut: every sketch represents itself
-            if on_device:
-                return torch.arange(n, dtype=torch.int32, device=rows.device), torch.tensor(n, device=rows.device)
-            return np.arange(n, dtype=np.uint32), n
-    min_same = 1 if min_same is None else int(min_same)
-    if not 0 <= min_same <= 0xFFFFFFFF:
-        raise ValueError("min_same must fit 32 bits")
+    if min_same is None:  # every sketch represents itself
+        if on_device:
+            return torch.arange(n, dtype=torch.int32, device=rows.device), torch.tensor(n, device=rows.device)
+        return np.arange(n, dtype=np.uint32), n
     flags = PG_DEREP_NEAREST if nearest else 0
     if on_device:
         dev = rows.device

@@ -18,12 +18,12 @@ import oracle_ffi
 _BLOCK_CELLS = 32 << 20  # counts per row block of the pair scan (128 MB)
 
 
-def links_of(sketches, min_same: int, nthreads=None) -> np.ndarray:
-    """The linked pairs i < j of the [n, s] sketches as an [m, 2] array in (i, j) order."""
+def links_of(sketches, min_same: int, nthreads=None):
+    """(i, j, same) of the linked pairs i < j of the [n, s] sketches, in (i, j) order."""
     sk = np.ascontiguousarray(sketches, np.uint32)
     n = len(sk)
     nthreads = nthreads or len(os.sched_getaffinity(0))
-    out = [np.zeros((0, 2), np.int64)]
+    out = [(np.zeros(0, np.int64),) * 3]
     rows = max(1, _BLOCK_CELLS // max(n, 1))
     for lo in range(0, n, rows):
         hi = min(n, lo + rows)
@@ -31,8 +31,8 @@ def links_of(sketches, min_same: int, nthreads=None) -> np.ndarray:
         assert rc == oracle_ffi.PO_OK, rc
         i, j = np.nonzero(same >= min_same)
         keep = j > i
-        out.append(np.stack([i[keep] + lo, j[keep] + lo], axis=1))
-    return np.concatenate(out)
+        out.append((i[keep] + lo, j[keep] + lo, same[i[keep], j[keep]].astype(np.int64)))
+    return tuple(np.concatenate(c) for c in zip(*out))
 
 
 def labels_of(n: int, link_i, link_j):
@@ -49,9 +49,9 @@ def labels_of(n: int, link_i, link_j):
 def cluster(sketches, min_same: int, nthreads=None, want_links: bool = False):
     """(label uint32[n], n_groups, n_links) of the [n, s] sketches at same >= min_same; with want_links also the
     [n_links, 2] array of linked pairs i < j in (i, j) order."""
-    links = links_of(sketches, min_same, nthreads)
-    label, n_groups = labels_of(len(sketches), links[:, 0], links[:, 1])
-    return (label, n_groups, len(links), links) if want_links else (label, n_groups, len(links))
+    i, j, _ = links_of(sketches, min_same, nthreads)
+    label, n_groups = labels_of(len(sketches), i, j)
+    return (label, n_groups, len(i), np.stack([i, j], axis=1)) if want_links else (label, n_groups, len(i))
 
 
 def cluster_pairs(pair_i, pair_j, pair_same, n: int, min_same: int):

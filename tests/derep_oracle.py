@@ -1,21 +1,17 @@
 """Greedy representatives of a sketch set on the CPU: the checker of pg_mash_dereplicate.
 
 The reference has no dereplication; the only reference arithmetic here is (*Mash).Similarity / Distance, through
-the oracle's po_mash_similarity_block (row = receiver) and OracleMash.Distance.  Sketches r < i are linked iff row
-r, column i counts at least min_same.  In index order, i is a representative iff no representative r < i is linked
-to i; any other i is assigned the smallest linked representative, or with nearest=True the linked representative
-with the largest count, ties to the smaller index.  A plain serial loop over the links, sharing nothing with the
-device's walk / mark split.
+the oracle's po_mash_similarity_block (row = receiver, scanned by cluster_oracle.links_of) and OracleMash.Distance.
+Sketches r < i are linked iff row r, column i counts at least min_same.  In index order, i is a representative iff
+no representative r < i is linked to i; any other i is assigned the smallest linked representative, or with
+nearest=True the linked representative with the largest count, ties to the smaller index.  A plain serial loop over
+the links, sharing nothing with the device's walk / mark split.
 TEST INFRASTRUCTURE ONLY (tests/, __graft_entry__.smoke() and tools/bench_derep.py)."""
 from __future__ import annotations
 
-import os
-
 import numpy as np
 
-import oracle_ffi
-
-_BLOCK_CELLS = 32 << 20  # counts per row block of the pair scan (128 MB)
+from cluster_oracle import links_of
 
 
 def _greedy(n: int, li, lj, ls, nearest: bool):
@@ -38,23 +34,6 @@ def _greedy(n: int, li, lj, ls, nearest: bool):
     alone = rep < 0
     rep[alone] = np.nonzero(alone)[0]
     return rep.astype(np.uint32), int((rep == np.arange(n)).sum())
-
-
-def links_of(sketches, min_same: int, nthreads=None):
-    """(i, j, same) of the linked pairs i < j of the [n, s] sketches."""
-    sk = np.ascontiguousarray(sketches, np.uint32)
-    n = len(sk)
-    nthreads = nthreads or len(os.sched_getaffinity(0))
-    out = [(np.zeros(0, np.int64),) * 3]
-    rows = max(1, _BLOCK_CELLS // max(n, 1))
-    for lo in range(0, n, rows):
-        hi = min(n, lo + rows)
-        rc, same = oracle_ffi.similarity_block(sk, lo, hi, lo, n, nthreads)  # columns below lo are never above the diagonal
-        assert rc == oracle_ffi.PO_OK, rc
-        i, j = np.nonzero(same >= min_same)
-        keep = j > i
-        out.append((i[keep] + lo, j[keep] + lo, same[i[keep], j[keep]].astype(np.int64)))
-    return tuple(np.concatenate(c) for c in zip(*out))
 
 
 def dereplicate(sketches, min_same: int, nearest: bool = False, nthreads=None):
