@@ -32,6 +32,9 @@ void note_launch(const char *kernel_name);
 int sm_count();
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) cached per (device, kernel); thread-safe (runtime.cu)
 int func_smem(const void *kernel, size_t bytes);
+// Grid of a kernel that loops over its work items: func_smem, then as many CTAs as are resident at once (at least
+// one per SM), but no more than `work` (runtime.cu)
+int resident_blocks(const void *kernel, int threads, size_t smem, uint64_t work, uint64_t *blocks);
 
 // transform.complementTable (transform.go:78-109): every unlisted byte maps to 0, including the DNA
 // letters U and Z.  Seqhash reads it on upper-cased bytes; the clone ligation on fragments as given.

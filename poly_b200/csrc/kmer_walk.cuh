@@ -18,6 +18,7 @@
 //   my_out, i, nk          hashes of k-mers i .. i+3 go to my_out[i ..]; CHECKED guards i+r < nk
 #pragma once
 #include <stdint.h>
+#include <utility>
 
 #include "murmur3.cuh"
 #include "tma.cuh"
@@ -57,6 +58,14 @@ __device__ __forceinline__ void load_kmix_table(uint32_t *s_lut, uint64_t *bar) 
     constexpr uint32_t TAILMASK = TAIL == 1 ? 0xffu : TAIL == 2 ? 0xffffu : 0xffffffu;         \
     constexpr bool LUT = TAIL == 1;                                                            \
     static_assert(NB >= 1 && K <= 32, "walk path: 4 <= k <= 32")
+
+// The k for which the walk kernels (K1, K1r, K2w, K2t) are instantiated.  with_walk_k(k, f) calls
+// f(std::integral_constant<int, K>{}) when k is one of them and returns whether it did.
+using WalkKs = std::integer_sequence<int, 11, 13, 15, 16, 17, 19, 21, 23, 24, 25, 27, 29, 31, 32>;
+template <class F, int... Ks>
+bool with_k_in(std::integer_sequence<int, Ks...>, int k, F &f) { return ((k == Ks && (f(std::integral_constant<int, Ks>{}), true)) || ...); }
+template <class F>
+bool with_walk_k(int k, F &&f) { return with_k_in(WalkKs{}, k, f); }
 
 // The first two realigned words, the raw words one step ahead of them, and word steps 0 .. NB-1,
 // which only fill the ring.

@@ -3,6 +3,7 @@
 // package (devices, memory, copies, IPC, synthetic reads).  The packages' entry points are the api_*.cu files.
 // No compute happens on the host: when no sm_90 device is usable every compute entry point fails with
 // PG_ERR_NO_DEVICE.
+#include <algorithm>
 #include <cctype>
 #include <cstdarg>
 #include <cstdio>
@@ -56,6 +57,14 @@ int func_smem(const void *fn, size_t bytes) {
         PG_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
         cur = bytes;
     }
+    return PG_OK;
+}
+
+int resident_blocks(const void *fn, int threads, size_t smem, uint64_t work, uint64_t *blocks) {
+    { const int rc_ = func_smem(fn, smem); if (rc_ != PG_OK) return rc_; }
+    int per_sm = 0;
+    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
+    *blocks = std::min<uint64_t>(work, (uint64_t)sm_count() * std::max(per_sm, 1));
     return PG_OK;
 }
 

@@ -28,19 +28,11 @@
 #include "murmur3.cuh"
 #include "tma.cuh"
 #include "kmer_walk.cuh"
+#include "sketch_smem.cuh"
 
 namespace pg {
 
-// ---- K1 fast path ----------------------------------------------------------------
-// smem: 2 input stages (32*L bytes + 16 B over-read pad, 16-B rounded, each) | out tile
-// (+ 1 KB static table when k % 4 == 1)
-__host__ __device__ inline uint32_t k1_in_bytes(uint32_t L) {
-    return (32u * L + 16u + 15u) & ~15u;
-}
-__host__ __device__ inline size_t k1_smem_bytes(uint32_t L, uint32_t nk) {
-    return 2 * (size_t)k1_in_bytes(L) + (size_t)32 * nk * 4;
-}
-
+// ---- K1 fast path (shared memory: k1_smem_bytes) -----------------------------------
 // One CTA = one warp, persistent: it hashes tiles blockIdx.x, blockIdx.x + gridDim.x, ... of 32
 // reads (the host launches no more CTAs than there are tiles).  The barriers and the tail table
 // are set up once per CTA; the load of the next tile is in flight while this one is hashed, and
@@ -140,7 +132,7 @@ sketch_fill_ragged_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ __align__(16) uint32_t s_lut[LUT ? 256 : 4];
     __shared__ __align__(8) uint64_t s_bar[2];
-    uint8_t *s_in = smem;                                        // [in_cap] (16-byte multiple, >= range + 47)
+    uint8_t *s_in = smem;                                        // [in_cap]: k1r_in_bytes, >= range + 47
     uint32_t *s_out = reinterpret_cast<uint32_t *>(smem + in_cap);  // [32][stride]
 
     const uint32_t tid = threadIdx.x;
@@ -244,30 +236,12 @@ sketch_fill_generic_kernel(const uint8_t *__restrict__ bases, const uint64_t *__
 template <int K>
 static int launch_k1(const uint8_t *d_bases, uint64_t n_tiles, uint32_t L, uint32_t nk,
                      const SketchDst &dst, cudaStream_t st) {
-    const void *fn = (const void *)sketch_fill_uniform_kernel<K>;
     const size_t smem = k1_smem_bytes(L, nk);
-    { const int rc_ = func_smem(fn, smem); if (rc_ != PG_OK) return rc_; }
-    int per_sm = 0;
-    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 32, smem));
-    // persistent: the CTAs that are resident at once, and none without a tile
-    const uint64_t grid = std::min<uint64_t>(n_tiles, (uint64_t)sm_count() * std::max(per_sm, 1));
+    uint64_t grid = 0;  // persistent: the CTAs that are resident at once, and none without a tile
+    { const int rc_ = resident_blocks((const void *)sketch_fill_uniform_kernel<K>, 32, smem, n_tiles, &grid); if (rc_ != PG_OK) return rc_; }
     sketch_fill_uniform_kernel<K><<<(unsigned)grid, 32, smem, st>>>(d_bases, dst, L, nk, n_tiles, 4u);
     PG_LAUNCH_CHECK("sketch_fill_uniform_kernel");
     return PG_OK;
-}
-
-static int dispatch_k1(int k, const uint8_t *d_bases, uint64_t n_tiles, uint32_t L, uint32_t nk,
-                       const SketchDst &dst, cudaStream_t st, bool *handled) {
-    *handled = true;
-    switch (k) {
-#define PG_K1_CASE(KK) \
-    case KK: return launch_k1<KK>(d_bases, n_tiles, L, nk, dst, st);
-        PG_K1_CASE(11) PG_K1_CASE(13) PG_K1_CASE(15) PG_K1_CASE(16) PG_K1_CASE(17) PG_K1_CASE(19)
-        PG_K1_CASE(21) PG_K1_CASE(23) PG_K1_CASE(24) PG_K1_CASE(25) PG_K1_CASE(27) PG_K1_CASE(29)
-        PG_K1_CASE(31) PG_K1_CASE(32)
-#undef PG_K1_CASE
-    default: *handled = false; return PG_OK;
-    }
 }
 
 static int launch_fill_generic(const uint8_t *d_bases, const uint64_t *d_offsets, uint32_t ulen,
@@ -307,10 +281,9 @@ int launch_sketch_uniform(const uint8_t *d_bases, uint64_t n_reads, uint32_t L, 
         SketchDst dst;
         dst.n = extra ? extra->n : 1;
         for (int p = 0; p < dst.n; ++p) dst.ptr[p] = extra ? extra->ptr[p] : d_out;
-        bool handled = false;
-        const int rc = dispatch_k1(k, d_bases, tiles, L, nk, dst, st, &handled);
-        if (rc != PG_OK) return rc;
-        if (handled) {
+        int rc = PG_OK;
+        if (with_walk_k(k, [&](auto kk) { rc = launch_k1<decltype(kk)::value>(d_bases, tiles, L, nk, dst, st); })) {
+            if (rc != PG_OK) return rc;
             done = tiles * 32;
             if (d_status) PG_CUDA(cudaMemsetAsync(d_status, 0, done * sizeof(int32_t), st));
         }
@@ -324,7 +297,7 @@ int launch_sketch_uniform(const uint8_t *d_bases, uint64_t n_reads, uint32_t L, 
 template <int K>
 static int launch_k1r(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_tiles, uint32_t stride,
                       uint32_t in_cap, uint32_t *d_out, uint32_t *d_count, int32_t *d_status, cudaStream_t st) {
-    const size_t smem = (size_t)in_cap + (size_t)32 * stride * 4;
+    const size_t smem = k1r_smem_bytes(in_cap, stride);
     { const int rc_ = func_smem((const void *)sketch_fill_ragged_kernel<K>, smem); if (rc_ != PG_OK) return rc_; }
     sketch_fill_ragged_kernel<K><<<(unsigned)n_tiles, 32, smem, st>>>(d_bases, d_offsets, d_out, stride, in_cap, d_count, d_status, 4u);
     PG_LAUNCH_CHECK("sketch_fill_ragged_kernel");
@@ -339,24 +312,17 @@ int launch_sketch_ragged(const uint8_t *d_bases, const uint64_t *d_offsets, uint
     const uint64_t nmax = max_read_len > (uint64_t)k ? max_read_len - (uint64_t)k : 0;
     uint64_t done = 0;
     // K1r: every read in the fill regime, rows not wider than the staging allows
-    const uint64_t in_cap = (32 * max_read_len + 48 + 15) & ~15ull;
+    const uint64_t in_cap = k1r_in_bytes(max_read_len);
     const uint64_t need_stride = (flags & PG_SKETCH_PAD_ZERO) ? (uint64_t)s : nmax;
     if (nmax > 0 && nmax < (uint64_t)s && row_stride >= need_stride && row_stride * 128 <= 96 * 1024 && in_cap <= 64 * 1024 &&
         (uintptr_t)d_out % 16 == 0 && n_reads >= 32 && (row_stride == need_stride || !(flags & PG_SKETCH_PAD_ZERO) || row_stride >= (uint64_t)s)) {
         const uint64_t tiles = n_reads / 32;
-        bool handled = true;
         int rc = PG_OK;
-        switch (k) {
-#define PG_K1R_CASE(KK) \
-    case KK: rc = launch_k1r<KK>(d_bases, d_offsets, tiles, (uint32_t)row_stride, (uint32_t)in_cap, d_out, d_count, d_status, st); break;
-            PG_K1R_CASE(11) PG_K1R_CASE(13) PG_K1R_CASE(15) PG_K1R_CASE(16) PG_K1R_CASE(17) PG_K1R_CASE(19)
-            PG_K1R_CASE(21) PG_K1R_CASE(23) PG_K1R_CASE(24) PG_K1R_CASE(25) PG_K1R_CASE(27) PG_K1R_CASE(29)
-            PG_K1R_CASE(31) PG_K1R_CASE(32)
-#undef PG_K1R_CASE
-            default: handled = false;
+        auto k1r = [&](auto kk) { rc = launch_k1r<decltype(kk)::value>(d_bases, d_offsets, tiles, (uint32_t)row_stride, (uint32_t)in_cap, d_out, d_count, d_status, st); };
+        if (with_walk_k(k, k1r)) {
+            if (rc != PG_OK) return rc;
+            done = tiles * 32;
         }
-        if (rc != PG_OK) return rc;
-        if (handled) done = tiles * 32;
     }
     if (done < n_reads) {
         int rc = launch_fill_generic(d_bases, d_offsets, 0, n_reads - done, done, k, s, d_out, row_stride,

@@ -35,29 +35,15 @@
 #include "murmur3.cuh"
 #include "tma.cuh"
 #include "kmer_walk.cuh"
+#include "sketch_smem.cuh"
 
 namespace pg {
 
 namespace {
 
 constexpr int SEL_THREADS = 512;
-constexpr int SEL_CHUNK = 2048;     // k-mer positions per chunk
 constexpr int SEL_MAX_S = 16384;    // largest sketch size of the shared-memory kernels (beyond: sketch_select_large.cu)
-constexpr int SEL_LOOKAHEAD = 1024; // max k supported by the staged path (bytes beyond chunk)
-constexpr int SEL_NBK = 2048;       // value buckets of the final sort-select (v >> 21)
 constexpr int SEL_BSHIFT = 21;
-constexpr uint32_t STAGE_PAD = 32;  // zero bytes behind a staged chunk: the walks read up to a word step beyond it
-constexpr int SEL_STAGE_WORDS = (15 + SEL_CHUNK + SEL_LOOKAHEAD + STAGE_PAD + 15) / 16 * 4;  // head + chunk + k + pad, 16-B multiple
-
-struct SelSmem {
-    uint32_t *cand;   // [cap]
-    uint32_t *keep;   // [s]
-    uint32_t *kv;     // [SEL_CHUNK + SEL_LOOKAHEAD]
-    uint32_t *bytes;  // 2 x [SEL_STAGE_WORDS] staged read bytes (word view), double-buffered
-    uint32_t *hist;   // [SEL_NBK + 1] (radix select uses the first 256 words)
-    uint32_t *misc;   // [8]: 0 cnt, 1 prefix, 2 want, 3 kept_lt, 4 kept_eq, 5 hmin_later, 6 bt, 7 need (K2w: 8..10 per-chunk counters)
-    uint32_t tmpcap;  // words available at keep[] for the final scatter (keep+kv+bytes are contiguous)
-};
 
 // atom.shared.add with the old value, as ONE instruction.  nvcc wraps atomicAdd(&shared[i], 1) whose result is
 // used into a leader-election loop over the distinct addresses of the warp (ncu: ~12 instructions x up to 32
@@ -286,14 +272,7 @@ sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restri
                      uint32_t cap, uint32_t *__restrict__ out, uint64_t row_stride,
                      uint32_t *__restrict__ count, int32_t *__restrict__ status, const SketchDst extra) {
     extern __shared__ __align__(16) uint32_t smem_w[];
-    SelSmem m;
-    m.cand = smem_w;
-    m.keep = m.cand + cap;
-    m.kv = m.keep + ((s + 3u) & ~3u) + 4u;  // 16-byte granules keep the TMA stage buffers aligned
-    m.bytes = m.kv + SEL_CHUNK + SEL_LOOKAHEAD;
-    m.hist = m.bytes + 2 * SEL_STAGE_WORDS;
-    m.misc = m.hist + SEL_NBK + 1;
-    m.tmpcap = (uint32_t)(m.hist - m.keep);
+    const SelSmem m = sel_generic_layout(cap, s).carve(smem_w);
 
     __shared__ __align__(8) uint64_t s_bar[2];
     uint32_t chunk_idx = 0;  // chunks this CTA has staged (over all its rows): chunk c uses stage buffer c & 1
@@ -402,11 +381,8 @@ sketch_select_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restri
 // against the admission limit and appends the few that pass (one shared-memory atomic each) --
 // for long sequences almost nothing passes, so the steady state is pure hashing.
 // About half the instructions of the generic kernel; 256 threads x 3 CTAs per SM keep the issue slots busy.
-constexpr int SELW_THREADS = 256;
-constexpr int SELW_SEG = 20;  // bytes between the segments of adjacent lanes = 5 words: conflict-free smem reads
-constexpr int SELW_CHUNK = SELW_THREADS * SELW_SEG;                      // 5120 k-mer positions
-constexpr int SELW_ROOM = 8192;                                          // candidate room beyond s
-constexpr int SELW_STAGE_WORDS = (15 + SELW_CHUNK + 32 + 48 + 15) / 16 * 4;  // head + chunk + k + over-read pad
+// Geometry: SELW_* in sketch_smem.cuh.
+constexpr int SELW_ROOM = 8192;  // candidate room beyond s
 
 #define PG_EMIT_ADMIT(R_, H_)                                              \
     if ((H_) < limit32) {                                                  \
@@ -432,14 +408,7 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
     static_assert(SELW_SEG % 4 == 0, "a segment is a whole number of word steps");
 
     extern __shared__ __align__(16) uint32_t smem_w[];
-    SelSmem m;
-    m.cand = smem_w;
-    m.keep = m.cand + cap;
-    m.kv = nullptr;
-    m.bytes = m.keep + ((s + 3u) & ~3u) + 4u;  // 16-byte granules keep the TMA stage buffers aligned
-    m.hist = m.bytes + 2 * SELW_STAGE_WORDS;
-    m.misc = m.hist + SEL_NBK + 1;
-    m.tmpcap = (uint32_t)(m.hist - m.keep);
+    const SelSmem m = sel_walk_layout(cap, s).carve(smem_w);
 
     __shared__ __align__(16) uint32_t s_lut[LUT ? 256 : 4];
     __shared__ __align__(8) uint64_t s_bar[3];  // [0], [1]: stage buffers, [2]: the table
@@ -482,7 +451,7 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
         const uint8_t *seq = bases + beg;
         uint32_t *dst = out + row * row_stride;
         if (empty_sketch_panics(s, status, count, row)) continue;
-        if (tid == 0) { m.misc[5] = 0xffffffffu; m.misc[8] = 0; m.misc[9] = 0; m.misc[10] = 0; }
+        if (tid == 0) { m.misc[5] = 0xffffffffu; for (int c = 0; c < 3; ++c) m.misc[SELW_CHUNK_CTR + c] = 0; }
         __syncthreads();
         uint64_t limit = 1ull << 32;  // admit h < limit
         uint32_t h_first = 0;
@@ -510,7 +479,7 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
                 limit = prune_to_s<SELW_THREADS>(m, cnt, s);
                 cnt = s;
             }
-            uint32_t *chunk_ctr = &m.misc[8 + chunk_idx % 3u];  // admitted by this chunk (zeroed two chunks ago)
+            uint32_t *chunk_ctr = &m.misc[SELW_CHUNK_CTR + chunk_idx % 3u];  // admitted by this chunk (zeroed two chunks ago)
             const bool unfiltered = limit == (1ull << 32);
             const bool full_chunk = ch == SELW_CHUNK;
             const uint32_t limit32 = (uint32_t)limit;
@@ -552,7 +521,7 @@ sketch_select_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
             } else {
                 cnt += *chunk_ctr;
             }
-            if (tid == 0) m.misc[8 + (chunk_idx + 2) % 3u] = 0;  // next use: chunk_idx + 2, after the next barrier
+            if (tid == 0) m.misc[SELW_CHUNK_CTR + (chunk_idx + 2) % 3u] = 0;  // next use: chunk_idx + 2, after the next barrier
         }
         __syncthreads();
         finish_bottom_s<SELW_THREADS>(m, cnt, s, P, dst);
@@ -578,14 +547,7 @@ select_merge_kernel(const uint32_t *__restrict__ part, const uint32_t *__restric
                     uint32_t s, uint32_t P, uint32_t cap, uint32_t *__restrict__ out, uint64_t row_stride,
                     uint32_t *__restrict__ count, int32_t *__restrict__ status) {
     extern __shared__ __align__(16) uint32_t smem_w[];
-    SelSmem m;
-    m.cand = smem_w;
-    m.keep = m.cand + cap;
-    m.kv = nullptr;
-    m.bytes = nullptr;
-    m.hist = m.keep + s + SEL_NBK + 64;  // scratch of the final stage: s + ties + one cursor per bucket
-    m.misc = m.hist + SEL_NBK + 1;
-    m.tmpcap = (uint32_t)(m.hist - m.keep);
+    const SelSmem m = sel_merge_layout(cap, s).carve(smem_w);
     const uint32_t tid = threadIdx.x;
     for (uint64_t row = blockIdx.x; row < n_rows; row += gridDim.x) {
         const uint32_t sl0 = row_slice0[row], sl1 = row_slice0[row + 1];
@@ -639,7 +601,7 @@ select_merge_kernel(const uint32_t *__restrict__ part, const uint32_t *__restric
 // distinct k-mers) or exceeds its buffer (heavy duplication below T) is redone by the exact streaming
 // kernel above (retry list built on the device, no host round trip).  So:
 //   A. sketch_thresh_walk_kernel<K, RARE>: one WARP per work item (<= 8 chunks of 32 x SEG
-//      positions of one row, SeltGeom<K>; long sequences become many items, so there is no host-side
+//      positions of one row, SeltGeom<K> in sketch_smem.cuh; long sequences become many items, so there is no host-side
 //      slicing and no merge pass).  Chunks arrive by double-buffered 1-D TMA bulk copies; lane l walks SEG
 //      consecutive k-mers with the register ring of kmer_walk.cuh (one ring prologue per SEG k-mers
 //      instead of per 20) and stores every hash into its private strip column, whose fill count advances
@@ -650,19 +612,6 @@ select_merge_kernel(const uint32_t *__restrict__ part, const uint32_t *__restric
 //      value buckets + exact rank inside each bucket (ties counted) -> ascending bottom-s, stored to
 //      every destination.
 // Extra HBM traffic: mu words per row written and read once (cfg3: 2 x 1 GB next to 1.8 GB algorithmic).
-// Positions per lane per chunk: 4 x an ODD number of word steps (lanes read their staged words an odd number
-// of words apart: bank-conflict free) that is a multiple of NB = K / 4 where NB is odd, so that a full
-// segment is whole groups of the NB-step loop body and never enters the bounds-checked tail; for even NB one
-// checked step remains.
-template <int K>
-struct SeltGeom {
-    static constexpr int NB = K / 4;
-    static constexpr int STEPS = NB == 2 ? 17 : NB == 3 ? 21 : NB == 4 ? 17 : NB == 5 ? 15 : 21;  // NB >= 6: whole groups of 3 steps
-    static constexpr int SEG = 4 * STEPS;      // 60 .. 84 k-mer positions
-    static constexpr int CHUNK = 32 * SEG;     // per warp chunk
-    static constexpr int STAGE = (15 + CHUNK + 32 + 48 + 15 + 255) / 256 * 256;  // head + chunk + k + over-read pad; also the dense flush buffer
-    static_assert(STEPS % 2 == 1 && (NB % 2 == 0 || STEPS % NB == 0), "segment geometry");
-};
 constexpr int SELT_ITEM_CHUNKS = 8;
 constexpr int SELT_SEL_THREADS = 256;
 
@@ -727,7 +676,7 @@ sketch_thresh_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__r
     const uint8_t *seq = bases + sp.beg;
     const uint32_t tm1 = offsets ? selt_threshold_m1(n, mu) : tm1_uniform;  // fixed-length reads: computed once on the host
     uint32_t *my_cand = gcand + lrow * (uint64_t)cap;
-    uint32_t *strip = reinterpret_cast<uint32_t *>(smem + 2 * SELT_STAGE_BYTES);
+    uint32_t *strip = reinterpret_cast<uint32_t *>(smem) + SeltGeom<K>::STRIP;
     uint32_t *my_strip = strip + lane;
     const uint32_t sa0 = smem_u32(my_strip);
 
@@ -881,8 +830,8 @@ sketch_thresh_select_kernel(const uint64_t *__restrict__ offsets, uint32_t unifo
                             const uint32_t *__restrict__ gcnt, uint32_t *__restrict__ out, uint64_t row_stride,
                             uint32_t *__restrict__ count, int32_t *__restrict__ status, const SketchDst extra,
                             uint32_t *__restrict__ retry_rows, uint32_t *__restrict__ n_retry, uint32_t tm1_uniform) {
-    extern __shared__ __align__(16) uint32_t smem_w[];  // tmp[cap] | cur[SEL_NBK] | flag
-    const uint32_t o_tmp = 0, o_cur = (cap + 3u) & ~3u, o_flag = o_cur + SEL_NBK;
+    extern __shared__ __align__(16) uint32_t smem_w[];
+    const SeltSelLayout lay(cap);
     __shared__ uint32_t s_wtot[SELT_SEL_THREADS / 32];
     const uint32_t tid = threadIdx.x;
     for (uint64_t lrow = blockIdx.x; lrow < n_rows; lrow += gridDim.x) {
@@ -905,8 +854,8 @@ sketch_thresh_select_kernel(const uint64_t *__restrict__ offsets, uint32_t unifo
         const uint32_t bshift = MUL ? (bits > 16u ? bits - 16u : 0u) : (bits > 11u ? bits - 11u : 0u);
         const uint32_t bscale = MUL ? ((uint32_t)SEL_NBK << 16) / ((tm1 >> bshift) + 1u) : 0u;
         auto bucket = [&](uint32_t e) -> uint32_t { return MUL ? ((e >> bshift) * bscale) >> 16 : e >> bshift; };
-        for (uint32_t i = tid; i < SEL_NBK; i += SELT_SEL_THREADS) smem_w[o_cur + i] = 0;
-        if (tid == 0) smem_w[o_flag] = 0;
+        for (uint32_t i = tid; i < SEL_NBK; i += SELT_SEL_THREADS) smem_w[lay.cur + i] = 0;
+        if (tid == 0) smem_w[lay.flag] = 0;
         __syncthreads();
         // histogram; loads in batches of U per thread so that a batch is one global round trip
         for (uint32_t base = 0; base < cnt; base += U * SELT_SEL_THREADS) {
@@ -918,14 +867,14 @@ sketch_thresh_select_kernel(const uint64_t *__restrict__ offsets, uint32_t unifo
             }
 #pragma unroll
             for (int u = 0; u < U; ++u)
-                if (base + u * SELT_SEL_THREADS + tid < cnt) atomicAdd(&smem_w[o_cur + bucket(v[u])], 1u);
+                if (base + u * SELT_SEL_THREADS + tid < cnt) atomicAdd(&smem_w[lay.cur + bucket(v[u])], 1u);
         }
         __syncthreads();
         {   // exclusive scan over the buckets: 8 per thread, warp scan, warp totals
             constexpr int PER = SEL_NBK / SELT_SEL_THREADS;
             uint32_t cb[PER], sum = 0, mx = 0;
 #pragma unroll
-            for (int j = 0; j < PER; ++j) { cb[j] = smem_w[o_cur + tid * PER + j]; sum += cb[j]; mx = max(mx, cb[j]); }
+            for (int j = 0; j < PER; ++j) { cb[j] = smem_w[lay.cur + tid * PER + j]; sum += cb[j]; mx = max(mx, cb[j]); }
             uint32_t incl = sum;
 #pragma unroll
             for (int d = 1; d < 32; d <<= 1) {
@@ -934,15 +883,15 @@ sketch_thresh_select_kernel(const uint64_t *__restrict__ offsets, uint32_t unifo
             }
             if ((tid & 31u) == 31u) s_wtot[tid >> 5] = incl;
             mx = __reduce_max_sync(0xffffffffu, mx);
-            if ((tid & 31u) == 0 && mx > 48u) atomicMax(&smem_w[o_flag], mx);
+            if ((tid & 31u) == 0 && mx > 48u) atomicMax(&smem_w[lay.flag], mx);
             __syncthreads();
             uint32_t run = incl - sum;
             for (uint32_t w = 0; w < (tid >> 5); ++w) run += s_wtot[w];
 #pragma unroll
-            for (int j = 0; j < PER; ++j) { smem_w[o_cur + tid * PER + j] = run; run += cb[j]; }
+            for (int j = 0; j < PER; ++j) { smem_w[lay.cur + tid * PER + j] = run; run += cb[j]; }
         }
         __syncthreads();
-        if (smem_w[o_flag] != 0) {  // crowded bucket: degenerate values, the exact streaming kernel takes the row
+        if (smem_w[lay.flag] != 0) {  // crowded bucket: degenerate values, the exact streaming kernel takes the row
             __syncthreads();
             if (tid == 0) retry_rows[atomicAdd(n_retry, 1u)] = (uint32_t)row;
             continue;
@@ -957,11 +906,11 @@ sketch_thresh_select_kernel(const uint64_t *__restrict__ offsets, uint32_t unifo
             }
 #pragma unroll
             for (int u = 0; u < U; ++u)
-                if (base + u * SELT_SEL_THREADS + tid < cnt) smem_w[o_tmp + smem_fetch_inc(&smem_w[o_cur + bucket(v[u])])] = v[u];
+                if (base + u * SELT_SEL_THREADS + tid < cnt) smem_w[lay.tmp + smem_fetch_inc(&smem_w[lay.cur + bucket(v[u])])] = v[u];
         }
         __syncthreads();
         {   // rank inside the bucket, through explicit shared-space addresses (kept in registers across the loop)
-            const uint32_t s_tmp = smem_u32(smem_w + o_tmp), s_cur = smem_u32(smem_w + o_cur);
+            const uint32_t s_tmp = smem_u32(smem_w + lay.tmp), s_cur = smem_u32(smem_w + lay.cur);
 #pragma unroll 2
             for (uint32_t p = tid; p < cnt; p += SELT_SEL_THREADS) {
                 const uint32_t e = lds_u32(s_tmp + 4u * p), b = bucket(e);
@@ -999,24 +948,30 @@ static auto thresh_select_fn(int u) {
                   : sketch_thresh_select_kernel<8, MUL>;
 }
 
+// cap: candidate words of a SelSmem kernel, max(P, s + room) in 16-byte granules so that what follows stays aligned
+static uint32_t sel_cap(uint32_t P, int s, uint32_t room) { return (std::max<uint32_t>(P, (uint32_t)s + room) + 3u) & ~3u; }
+// resident_blocks of a SelSmem kernel, whose stage buffers go to TMA bulk copies: they must start on 16-byte boundaries
+static int sel_blocks(const void *fn, int threads, const SelLayout &lay, uint64_t work, uint64_t *blocks) {
+    if (lay.stage() % 4 == 0) return resident_blocks(fn, threads, lay.bytes(), work, blocks);
+    set_error("internal: select stage buffers at word %llu are not 16-byte aligned", (unsigned long long)lay.stage());
+    return PG_ERR_ARG;
+}
+
 template <int K>
 static int launch_select_walk(const uint8_t *d_bases, const uint64_t *d_offsets, uint32_t read_len, uint64_t n_reads, int s,
                               uint32_t P, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, int32_t *d_status,
                               cudaStream_t st, const SketchDst &ex, const uint64_t *d_slice_beg = nullptr,
                               const uint32_t *d_slice_n = nullptr, const uint32_t *d_row_list = nullptr,
                               const uint32_t *d_n_list = nullptr) {
-    const uint32_t cap = (std::max<uint32_t>(P, (uint32_t)s + SELW_ROOM) + 3u) & ~3u;
-    const size_t words = (size_t)cap + (((size_t)s + 3) & ~(size_t)3) + 4 + 2 * SELW_STAGE_WORDS + (SEL_NBK + 1) + 16;
-    const size_t smem = words * 4;
-    { const int rc_ = func_smem((const void *)sketch_select_walk_kernel<K>, smem); if (rc_ != PG_OK) return rc_; }
-    int per_sm = 1;
-    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sketch_select_walk_kernel<K>, SELW_THREADS, smem));
-    const uint64_t blocks = std::min<uint64_t>(n_reads, (uint64_t)sm_count() * std::max(per_sm, 1));
+    const uint32_t cap = sel_cap(P, s, SELW_ROOM);
+    const SelLayout lay = sel_walk_layout(cap, s);
+    uint64_t blocks = 0;
+    { const int rc_ = sel_blocks((const void *)sketch_select_walk_kernel<K>, SELW_THREADS, lay, n_reads, &blocks); if (rc_ != PG_OK) return rc_; }
     StreamScratch tmp(st);
     unsigned long long *d_next = nullptr;
     PG_CUDA(tmp.alloc(&d_next, 1));
     PG_CUDA(cudaMemsetAsync(d_next, 0, 8, st));
-    sketch_select_walk_kernel<K><<<(unsigned)blocks, SELW_THREADS, smem, st>>>(d_bases, d_offsets, read_len, n_reads, (uint32_t)s, P, cap,
+    sketch_select_walk_kernel<K><<<(unsigned)blocks, SELW_THREADS, lay.bytes(), st>>>(d_bases, d_offsets, read_len, n_reads, (uint32_t)s, P, cap,
                                                                               d_out, row_stride, d_count, d_status, ex, 4u, d_slice_beg,
                                                                               d_slice_n, d_next, d_row_list, d_n_list);
     PG_LAUNCH_CHECK("sketch_select_walk_kernel");
@@ -1080,8 +1035,8 @@ static int try_select_sliced(const uint8_t *d_bases, const uint64_t *d_offsets, 
     none.n = 0;
     int rc = launch_select_walk<K>(d_bases, nullptr, 0, n_slices, s, P, d_part, (uint64_t)s, nullptr, nullptr, st, none, d_beg, d_cnt);
     if (rc == PG_OK) {
-        const uint32_t cap = (std::max<uint32_t>(P, (uint32_t)s + 2 * SELM_CHUNK) + 3u) & ~3u;
-        const size_t smem = ((size_t)cap + s + SEL_NBK + 64 + SEL_NBK + 1 + 8) * 4;
+        const uint32_t cap = sel_cap(P, s, 2 * SELM_CHUNK);
+        const size_t smem = sel_merge_layout(cap, s).bytes();
         { const int rc_ = func_smem((const void *)select_merge_kernel, smem); if (rc_ != PG_OK) return rc_; }
         const uint64_t blocks = std::min<uint64_t>(n_reads, (uint64_t)sm_count() * 2);
         select_merge_kernel<<<(unsigned)blocks, SELM_THREADS, smem, st>>>(d_part, d_row0, n_reads, (uint32_t)s, P, cap, d_out, row_stride,
@@ -1111,8 +1066,7 @@ static int launch_select_thresh(const uint8_t *d_bases, const uint64_t *d_offset
     const uint32_t mu = (uint32_t)s + 6u * (uint32_t)ceil(sqrt((double)s)) + 48u;
     uint32_t cap = mu + 8u * (uint32_t)ceil(sqrt((double)mu)) + 96u;
     cap = (cap + 3u) & ~3u;
-    const size_t smem_a = 2 * (size_t)SeltGeom<K>::STAGE + (size_t)SeltGeom<K>::SEG * 32 * 4;
-    const size_t smem_b = ((((size_t)cap + 3) & ~(size_t)3) + SEL_NBK + 16) * 4;  // tmp | cur | flag
+    const size_t smem_a = SeltGeom<K>::SMEM_BYTES, smem_b = SeltSelLayout(cap).bytes();
     if (smem_b > 220 * 1024) return PG_OK;
     // admission probability of the longest rows: below 1/512 a warp step (128 hashes) admits something a quarter of the time
     const uint32_t tm1_u = d_offsets ? 0u : selt_threshold_m1(nmax, mu);  // every row of a fixed-length batch has n == nmax
@@ -1136,14 +1090,13 @@ static int launch_select_thresh(const uint8_t *d_bases, const uint64_t *d_offset
         sel_mul = ((tm1_u >> (tb > 11u ? tb - 11u : 0u)) + 1u) < 1536u;
     }
     const auto sel_fn = sel_mul ? thresh_select_fn<true>(sel_u) : thresh_select_fn<false>(sel_u);
-    { const int rc_ = func_smem((const void *)sel_fn, smem_b); if (rc_ != PG_OK) return rc_; }
-    int per_sm = 1;
-    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sel_fn, SELT_SEL_THREADS, smem_b));
     // candidate lists: cap words per row, rows in groups of <= 1.5 GiB of temporaries
     uint64_t rows_per_group = std::max<uint64_t>(1, std::min<uint64_t>((3ull << 28) / cap, 0x7fffffffull / ipr));
     if (const char *e = getenv("PG_K2T_GROUP_ROWS"))  // test knob: force several launch groups
         if (atoll(e) > 0) rows_per_group = std::min<uint64_t>(rows_per_group, (uint64_t)atoll(e));
     const uint64_t group = std::min(n_reads, rows_per_group);
+    uint64_t sel_blocks = 0;  // resident CTAs for the largest group; a smaller last group takes min(rows, sel_blocks)
+    { const int rc_ = resident_blocks((const void *)sel_fn, SELT_SEL_THREADS, smem_b, group, &sel_blocks); if (rc_ != PG_OK) return rc_; }
     StreamScratch tmp(st);
     uint32_t *d_cand = nullptr, *d_cnt = nullptr, *d_retry = nullptr, *d_nretry = nullptr;
     PG_CUDA(tmp.alloc(&d_cand, group * cap));
@@ -1157,8 +1110,7 @@ static int launch_select_thresh(const uint8_t *d_bases, const uint64_t *d_offset
         walk_fn<<<(unsigned)(rows * ipr), 32, smem_a, st>>>(d_bases, d_offsets, read_len, r0, rows, (uint32_t)ipr, (uint32_t)s, mu, cap,
                                                             d_cand, d_cnt, 4u, tm1_u);
         PG_LAUNCH_CHECK("sketch_thresh_walk_kernel");
-        const uint64_t blocks = std::min<uint64_t>(rows, (uint64_t)sm_count() * std::max(per_sm, 1));
-        sel_fn<<<(unsigned)blocks, SELT_SEL_THREADS, smem_b, st>>>(d_offsets, read_len, r0, rows, (uint32_t)K, (uint32_t)s, mu, cap, d_cand,
+        sel_fn<<<(unsigned)std::min(rows, sel_blocks), SELT_SEL_THREADS, smem_b, st>>>(d_offsets, read_len, r0, rows, (uint32_t)K, (uint32_t)s, mu, cap, d_cand,
                                                                     d_cnt, d_out, row_stride, d_count, d_status, ex, d_retry, d_nretry, tm1_u);
         PG_LAUNCH_CHECK("sketch_thresh_select_kernel");
     }
@@ -1207,24 +1159,14 @@ int launch_sketch_select(const uint8_t *d_bases, const uint64_t *d_offsets, uint
     while (P < (uint32_t)std::max(s, 1)) P <<= 1;
     if (P < 2) P = 2;
     // the walk kernels (K2t, K2w) for the instantiated k
-    switch (k) {
-#define PG_K2W_CASE(KK) \
-    case KK: return launch_select_auto<KK>(d_bases, d_offsets, read_len, max_read_len, n_reads, s, P, d_out, row_stride, d_count, d_status, st, ex);
-        PG_K2W_CASE(11) PG_K2W_CASE(13) PG_K2W_CASE(15) PG_K2W_CASE(16) PG_K2W_CASE(17) PG_K2W_CASE(19)
-        PG_K2W_CASE(21) PG_K2W_CASE(23) PG_K2W_CASE(24) PG_K2W_CASE(25) PG_K2W_CASE(27) PG_K2W_CASE(29)
-        PG_K2W_CASE(31) PG_K2W_CASE(32)
-#undef PG_K2W_CASE
-        default: break;
-    }
-    uint32_t cap = (std::max<uint32_t>(P, (uint32_t)s + 4 * SEL_CHUNK) + 3u) & ~3u;
-    const size_t words = (size_t)cap + (((size_t)s + 3) & ~(size_t)3) + 4 + (SEL_CHUNK + SEL_LOOKAHEAD) +
-                         2 * SEL_STAGE_WORDS + (SEL_NBK + 1) + 8;
-    const size_t smem = words * 4;
-    { const int rc_ = func_smem((const void *)sketch_select_kernel, smem); if (rc_ != PG_OK) return rc_; }
-    int per_sm = 1;
-    PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sketch_select_kernel, SEL_THREADS, smem));
-    const uint64_t blocks = std::min<uint64_t>(n_reads, (uint64_t)sm_count() * std::max(per_sm, 1));  // one wave, grid-stride over rows
-    sketch_select_kernel<<<(unsigned)blocks, SEL_THREADS, smem, st>>>(
+    int rc = PG_OK;
+    auto walk = [&](auto kk) { rc = launch_select_auto<decltype(kk)::value>(d_bases, d_offsets, read_len, max_read_len, n_reads, s, P, d_out, row_stride, d_count, d_status, st, ex); };
+    if (with_walk_k(k, walk)) return rc;
+    const uint32_t cap = sel_cap(P, s, 4 * SEL_CHUNK);
+    const SelLayout lay = sel_generic_layout(cap, s);
+    uint64_t blocks = 0;  // one wave, grid-stride over rows
+    if ((rc = sel_blocks((const void *)sketch_select_kernel, SEL_THREADS, lay, n_reads, &blocks)) != PG_OK) return rc;
+    sketch_select_kernel<<<(unsigned)blocks, SEL_THREADS, lay.bytes(), st>>>(
         d_bases, d_offsets, read_len, n_reads, (uint32_t)k, (uint32_t)s, P, cap, d_out,
         row_stride, d_count, d_status, ex);
     PG_LAUNCH_CHECK("sketch_select_kernel");
