@@ -628,6 +628,33 @@ func (ix *Index) Query(queries []uint32, nq, sq, k, minSame int) (ref, same []ui
 	return ref[:slots], same[:slots], dist[:slots], nHits[:nq], err
 }
 
+// QueryWithin wraps pg_mash_index_query_within: for each of nq query sketches of sq words, every reference with
+// same >= minSame (>= 1), in reference order.  Query q's hits are entries offsets[q] .. offsets[q+1] of ref / same /
+// dist.  A counting call sizes the lists, a second call fills them.
+func (ix *Index) QueryWithin(queries []uint32, nq, sq, minSame int) (offsets []uint64, ref, same []uint32, dist []float64, err error) {
+	offsets = make([]uint64, nq+1)
+	var p *C.uint32_t
+	if len(queries) > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&queries[0]))
+	}
+	var total C.uint64_t
+	err = locked(func() C.int {
+		return C.pg_mash_index_query_within(ix.h, p, C.uint64_t(nq), C.int32_t(sq), C.uint32_t(minSame),
+			(*C.uint64_t)(unsafe.Pointer(&offsets[0])), nil, nil, nil, 0, &total)
+	})
+	if err != nil {
+		return nil, nil, nil, nil, err
+	}
+	m := int(total)
+	ref, same, dist = make([]uint32, m+1), make([]uint32, m+1), make([]float64, m+1)
+	err = locked(func() C.int {
+		return C.pg_mash_index_query_within(ix.h, p, C.uint64_t(nq), C.int32_t(sq), C.uint32_t(minSame),
+			(*C.uint64_t)(unsafe.Pointer(&offsets[0])), (*C.uint32_t)(unsafe.Pointer(&ref[0])), (*C.uint32_t)(unsafe.Pointer(&same[0])),
+			(*C.double)(unsafe.Pointer(&dist[0])), C.uint64_t(m), &total)
+	})
+	return offsets, ref[:m], same[:m], dist[:m], err
+}
+
 // Close wraps pg_mash_index_free.
 func (ix *Index) Close() error {
 	if ix.h == nil {

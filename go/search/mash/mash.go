@@ -302,5 +302,48 @@ func (ix *Index) Nearest(queries []*Mash, k int) [][]Neighbor {
 	return res
 }
 
+// Within returns, for each query (all of one SketchSize), every reference with query.Distance(reference) <=
+// maxDistance, however many there are, ordered by reference position.  The threshold becomes a matching count
+// as in Cluster, over min(query SketchSize, reference SketchSize); a maxDistance that every pair satisfies (>= 1)
+// is an error.
+func (ix *Index) Within(queries []*Mash, maxDistance float64) ([][]Neighbor, error) {
+	sq := 0
+	if len(queries) > 0 {
+		sq = queries[0].SketchSize
+	}
+	den := sq
+	if ix.s < den {
+		den = ix.s
+	}
+	minSame := 0
+	for minSame <= den && !(1-float64(minSame)/float64(den) <= maxDistance) {
+		minSame++
+	}
+	if minSame == 0 && den > 0 {
+		return nil, fmt.Errorf("mash: maxDistance %v lists every pair", maxDistance)
+	}
+	flat := make([]uint32, 0, len(queries)*sq)
+	for _, m := range queries {
+		if m.SketchSize != sq {
+			return nil, errors.New("mash: every query of a batch must have the same SketchSize")
+		}
+		flat = append(flat, m.Sketches[:sq]...)
+	}
+	off, ref, same, dist, err := ix.ix.QueryWithin(flat, len(queries), sq, minSame)
+	if errors.Is(err, polyb200.ErrPanic) {
+		panic("runtime error: index out of range [-1]")
+	} else if err != nil {
+		return nil, err
+	}
+	res := make([][]Neighbor, len(queries))
+	for q := range res {
+		res[q] = make([]Neighbor, 0, off[q+1]-off[q])
+		for h := off[q]; h < off[q+1]; h++ {
+			res[q] = append(res[q], Neighbor{Index: int(ref[h]), Same: int(same[h]), Distance: dist[h]})
+		}
+	}
+	return res, nil
+}
+
 // Close releases the index's device memory.
 func (ix *Index) Close() error { return ix.ix.Close() }

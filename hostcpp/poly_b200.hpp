@@ -361,6 +361,26 @@ public:
             for (uint32_t t = 0; t < nh[q]; ++t) out[q].push_back(Neighbor{ref[q * k + t], same[q * k + t], dist[q * k + t]});
         return out;
     }
+    // For each query, every reference with Same >= minSame (>= 1), however many, by Ref ascending.
+    std::vector<std::vector<Neighbor>> Within(const std::vector<Mash> &queries, uint32_t minSame = 1) const {
+        int sq;
+        const std::vector<uint32_t> flat = detail::FlatRows(queries, "queries", &sq);
+        const size_t nq = queries.size();
+        std::vector<uint64_t> off(nq + 1);
+        uint64_t total = 0;
+        // count first, then fill lists of the exact size
+        int rc = pg_mash_index_query_within(h_, flat.data(), nq, sq, minSame, off.data(), nullptr, nullptr, nullptr, 0, &total);
+        std::vector<uint32_t> ref(total + 1), same(total + 1);
+        std::vector<double> dist(total + 1);
+        if (rc == PG_OK)
+            rc = pg_mash_index_query_within(h_, flat.data(), nq, sq, minSame, off.data(), ref.data(), same.data(), dist.data(), total, &total);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+        std::vector<std::vector<Neighbor>> out(nq);
+        for (size_t q = 0; q < nq; ++q)
+            for (uint64_t h = off[q]; h < off[q + 1]; ++h) out[q].push_back(Neighbor{ref[h], same[h], dist[h]});
+        return out;
+    }
 };
 
 // ---- cluster: single-linkage groups of a sketch set (pg_mash_cluster) --------------------------------

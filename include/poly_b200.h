@@ -337,6 +337,43 @@ int pg_mash_index_query_dev(const pg_mash_index *ix, const uint32_t *d_queries, 
                             uint32_t *d_n_hits, void *stream);
 int pg_mash_index_free(pg_mash_index *ix);
 
+/* ---- sketch index: every reference within a matching-count cut (radius query) ----------------------
+ * The question "which references lie within Distance <= d of each query, however many there are", answered
+ * against a pg_mash_index without the top-k cap.
+ *   - Lists: query q's hits are the references j with same[q][j] >= min_same, in ascending reference index,
+ *     stored at positions [hit_offsets[q], hit_offsets[q+1]) of hit_ref / hit_same / hit_distance.  same[q][j]
+ *     is what queries[q].Similarity(refs[j]) counts, the QUERY being the receiver, exactly as in
+ *     pg_mash_index_query; hit_distance = 1 - same/min(sq, s) in double, bit-identical to (*Mash).Distance.
+ *     hit_offsets has nq + 1 entries; hit_offsets[nq] is the total.
+ *   - The output depends on the input alone: not on the row-block size, the grid or the order of atomics.
+ *   - Any of hit_ref / hit_same / hit_distance may be NULL.  With all three NULL (and hits_cap = 0) the call
+ *     only counts: it fills the offsets and the total and does not report an overflow.  n_hits (d_n_hits) may
+ *     be NULL too: the total is also hit_offsets[nq].
+ *   - A Distance cut becomes a count as for pg_mash_cluster: the smallest c with 1 - (double)c / min(sq, s) <=
+ *     max_distance.
+ *   - Errors, checked in this order: a null index is PG_ERR_ARG; min_same == 0 is PG_ERR_ARG (it would list all
+ *     nq x n pairs); nq == 0 is valid and writes hit_offsets[0] = 0 and a total of 0; sq <= 0 is PG_ERR_PANIC;
+ *     a null hit_offsets (or, for the host call, null queries) is PG_ERR_ARG; PG_ERR_UNSUPPORTED when a query
+ *     must be compared pairwise and the tile does not fit, as pg_mash_index_query reports it.
+ *   - min_same > min(sq, s) is valid and gives empty lists, as does an index of n == 0 references.
+ *   - Overflow: a total above hits_cap in a host call that asks for a list is PG_ERR_ARG; the offsets are then complete, the first
+ *     hits_cap hits are stored and *n_hits holds the total (as pg_mash_distance_sparse does).  The _dev call does
+ *     not fail on overflow: it never writes a list past hits_cap and leaves the total in d_n_hits.
+ *   - Each row block's dense counts are read twice, once to count and once to fill, so unlike the top-k query
+ *     there is no 2^24 limit on the sketch size.
+ * Synchronisation: the _dev call synchronises `stream` only where pg_mash_index_query_dev does, while it reads
+ * how many queries are unsorted; it then only enqueues (the offsets are scanned on the device, block after block)
+ * and leaves every output ordered on `stream` without waiting for it.  The host call synchronises.
+ * Threads and ownership: those of the index block above; any number of threads may mix pg_mash_index_query and
+ * pg_mash_index_query_within calls on one index. */
+int pg_mash_index_query_within(const pg_mash_index *ix, const uint32_t *queries, uint64_t nq, int32_t sq,
+                               uint32_t min_same, uint64_t *hit_offsets, uint32_t *hit_ref, uint32_t *hit_same,
+                               double *hit_distance, uint64_t hits_cap, uint64_t *n_hits);
+int pg_mash_index_query_within_dev(const pg_mash_index *ix, const uint32_t *d_queries, uint64_t nq, int32_t sq,
+                                   uint32_t min_same, uint64_t *d_hit_offsets, uint32_t *d_hit_ref,
+                                   uint32_t *d_hit_same, double *d_hit_distance, uint64_t hits_cap,
+                                   uint64_t *d_n_hits, void *stream);
+
 /* ---- align.SmithWaterman score -- search/align/align.go:171-203 -------------------
  * One template against n queries.  query_is_a != 0: stringA = query (outer loop),
  * stringB = template; else swapped.  lut_a/lut_b: byte -> index into the first /

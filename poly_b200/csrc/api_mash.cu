@@ -866,6 +866,49 @@ int pg_mash_index_query(const pg_mash_index *ix, const uint32_t *queries, uint64
     return c.finish();
 }
 
+// ---------------------------------------------------------------------------------
+// Sketch index: every reference within a matching-count cut
+// ---------------------------------------------------------------------------------
+int pg_mash_index_query_within_dev(const pg_mash_index *ix, const uint32_t *d_queries, uint64_t nq, int32_t sq, uint32_t min_same,
+                                   uint64_t *d_hit_offsets, uint32_t *d_hit_ref, uint32_t *d_hit_same, double *d_hit_distance,
+                                   uint64_t hits_cap, uint64_t *d_n_hits, void *stream) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    return launch_index_within(ix->plan, d_queries, nq, sq, min_same, d_hit_offsets, d_hit_ref, d_hit_same, d_hit_distance, hits_cap,
+                               d_n_hits, (cudaStream_t)stream);
+}
+
+int pg_mash_index_query_within(const pg_mash_index *ix, const uint32_t *queries, uint64_t nq, int32_t sq, uint32_t min_same,
+                               uint64_t *hit_offsets, uint32_t *hit_ref, uint32_t *hit_same, double *hit_distance, uint64_t hits_cap,
+                               uint64_t *n_hits) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    if (n_hits) *n_hits = 0;
+    if (min_same == 0) { set_error("min_same 0 would list all %llu x %llu pairs", (unsigned long long)nq, (unsigned long long)ix->plan.n); return PG_ERR_ARG; }
+    if (nq == 0) {
+        if (hit_offsets) hit_offsets[0] = 0;
+        return PG_OK;
+    }
+    if (sq <= 0) { set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq); return PG_ERR_PANIC; }
+    if (!hit_offsets || !queries) { set_error("null buffer"); return PG_ERR_ARG; }
+    HostCall c;
+    const uint32_t *d_q = c.upload(queries, nq * (uint64_t)sq);
+    uint64_t *d_off = c.alloc<uint64_t>(nq + 1);
+    uint32_t *d_ref = hit_ref ? c.alloc<uint32_t>(hits_cap) : nullptr, *d_same = hit_same ? c.alloc<uint32_t>(hits_cap) : nullptr;
+    double *d_dist = hit_distance ? c.alloc<double>(hits_cap) : nullptr;
+    unsigned long long *d_n = c.alloc<unsigned long long>(1);
+    if ((rc = c.error()) ||
+        (rc = launch_index_within(ix->plan, d_q, nq, sq, min_same, d_off, d_ref, d_same, d_dist, hits_cap, (uint64_t *)d_n, c.st)))
+        return rc;
+    c.download(hit_offsets, d_off, nq + 1);
+    uint64_t total = 0;
+    const bool counting = !hit_ref && !hit_same && !hit_distance;  // no list to overflow
+    return finish_capped(c, d_n, counting ? ~0ull : hits_cap, n_hits ? n_hits : &total,
+                         {{hit_ref, d_ref, 4}, {hit_same, d_same, 4}, {hit_distance, d_dist, 8}}, "hits_cap", "hits");
+}
+
 int pg_mash_index_free(pg_mash_index *ix) {
     if (!ix) return PG_OK;
     int rc = use_device(ix->device);

@@ -253,6 +253,11 @@ int launch_sorted_flags(const uint32_t *d_sk, uint64_t n, int s, uint8_t *d_flag
 constexpr uint32_t INDEX_MAX_TOP_K = 1024;
 int launch_index_query(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t top_k, uint32_t min_same,
                        uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint32_t *d_n_hits, cudaStream_t st);
+// mash_index.cu: every reference with same >= min_same for each query, as CSR lists in reference order: offsets
+// d_off[0 .. nq] (d_off[nq] = the total), entries at positions >= cap not stored, the lists and d_total may be NULL.
+// Argument rules and their order are those of pg_mash_index_query_within_dev.
+int launch_index_within(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, uint64_t *d_off,
+                        uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint64_t cap, uint64_t *d_total, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).
 struct AlignScoring;

@@ -13,8 +13,14 @@
 //                         rules of distance_block_kernel;
 //   index_select_kernel   one CTA per row: exact top_k by (same desc, reference index asc) with a count
 //                         histogram, a threshold count and an index-ordered pass over the ties.
+// Radius queries (launch_index_within) consume the same blocks with two other kernels:
+//   index_within_count_kernel  one CTA per row: the number of counts >= min_same, scanned in place into the
+//                              CSR offsets (the entry before the block already holds the earlier blocks' total);
+//   index_within_fill_kernel   one CTA per row: an index-ordered compaction of the row into its CSR slice.
 #include <algorithm>
 #include <cstdlib>
+
+#include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
 
@@ -257,22 +263,88 @@ index_select_kernel(const uint32_t *__restrict__ acc, uint64_t n, uint64_t row0,
     if (threadIdx.x == 0 && n_hits) n_hits[row] = m;
 }
 
-}  // namespace
+// One CTA per query row: off[row + 1] = the number of references with same >= min_same (min_same >= 1, so the
+// zeros load_count_quad returns past n never count).
+__global__ void __launch_bounds__(SEL_THREADS)
+index_within_count_kernel(const uint32_t *__restrict__ acc, uint64_t n, uint64_t row0, uint32_t min_same, uint64_t *__restrict__ off) {
+    __shared__ uint32_t s_part[SEL_THREADS / 32];
+    const uint32_t *A = acc + (uint64_t)blockIdx.x * n;
+    const bool vec = (n & 3) == 0;
+    uint32_t c = 0;
+    for (uint64_t j = 4ull * threadIdx.x; j < n; j += 4ull * SEL_THREADS) {
+        uint32_t v[4];
+        load_count_quad(A, j, n, vec, v);
+#pragma unroll
+        for (int t = 0; t < 4; ++t) c += v[t] >= min_same;
+    }
+    for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
+    if ((threadIdx.x & 31u) == 0) s_part[threadIdx.x >> 5] = c;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint64_t total = 0;
+        for (int w = 0; w < SEL_THREADS / 32; ++w) total += s_part[w];
+        off[row0 + blockIdx.x + 1] = total;
+    }
+}
 
-int launch_index_query(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t top_k, uint32_t min_same,
-                       uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint32_t *d_n_hits, cudaStream_t st) {
-    if (top_k == 0 || top_k > INDEX_MAX_TOP_K) {
-        set_error("top_k %u outside [1, %u]", top_k, INDEX_MAX_TOP_K);
-        return PG_ERR_ARG;
+// One CTA per query row: the references with same >= min_same in index order, stored from off[row] on; only
+// positions below cap are written.  Each thread takes four neighbouring counts of a chunk, so a thread's hits are
+// consecutive: a warp scan of the per-thread counts, the warps' totals in shared memory and a running base (the
+// same for every thread) give each hit its position.
+__global__ void __launch_bounds__(SEL_THREADS)
+index_within_fill_kernel(const uint32_t *__restrict__ acc, uint64_t n, uint64_t row0, uint32_t den, uint32_t min_same,
+                         const uint64_t *__restrict__ off, uint64_t cap, uint32_t *__restrict__ hit_ref, uint32_t *__restrict__ hit_same,
+                         double *__restrict__ hit_dist) {
+    __shared__ uint32_t s_part[SEL_THREADS / 32];
+    const uint32_t *A = acc + (uint64_t)blockIdx.x * n;
+    const uint64_t row = row0 + blockIdx.x;
+    const uint64_t end = min(off[row + 1], cap);
+    uint64_t base = off[row];
+    if (base >= end) return;  // an empty list, or one wholly past the cap
+    const bool vec = (n & 3) == 0;
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    for (uint64_t j0 = 0; j0 < n; j0 += 4ull * SEL_THREADS) {
+        const uint64_t j = j0 + 4ull * threadIdx.x;
+        uint32_t v[4];
+        load_count_quad(A, j, n, vec, v);
+        uint32_t mask = 0;
+#pragma unroll
+        for (int t = 0; t < 4; ++t) mask |= (uint32_t)(v[t] >= min_same) << t;
+        const uint32_t mine = __popc(mask);
+        uint32_t incl = mine;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= (uint32_t)d) incl += y;
+        }
+        if (lane == 31) s_part[warp] = incl;
+        __syncthreads();
+        uint64_t pos = base + incl - mine;
+        uint32_t total = 0;
+        for (uint32_t w = 0; w < SEL_THREADS / 32; ++w) { if (w < warp) pos += s_part[w]; total += s_part[w]; }
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            if (!((mask >> t) & 1u)) continue;
+            if (pos < end) {
+                if (hit_ref) hit_ref[pos] = (uint32_t)(j + t);
+                if (hit_same) hit_same[pos] = v[t];
+                if (hit_dist) hit_dist[pos] = 1 - (double)v[t] / (double)den;  // mash.go:134,139
+            }
+            ++pos;
+        }
+        base += total;
+        if (base >= end) break;  // the rest of the row lies past the cap (base is the same in every thread)
+        __syncthreads();         // s_part is read before the next chunk writes it
     }
-    if (nq == 0) return PG_OK;
-    if (sq <= 0) {
-        set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq);
-        return PG_ERR_PANIC;
-    }
+}
+
+// The accumulation loop of both query kinds (nq > 0, sq > 0): the queries' sortedness (the one host sync), the
+// probe / pairwise choice, and row blocks whose dense [rows][n] counts fit a 2 GiB budget.  consume(acc, rb, re)
+// runs once the counts of rows [rb, re) are enqueued into acc; the first code other than PG_OK is the result.
+int index_blocks(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, cudaStream_t st,
+                 const std::function<int(const uint32_t *acc, uint64_t rb, uint64_t re)> &consume) {
     const uint64_t n = plan.n;
-    const uint32_t sr = (uint32_t)plan.s, den = std::min<uint32_t>((uint32_t)sq, sr);
-    if (n && den >= (1u << 24)) { set_error("sketch size %u above the selection's 2^24 limit", den); return PG_ERR_UNSUPPORTED; }
+    const uint32_t sr = (uint32_t)plan.s;
     StreamScratch sc(st);
     uint8_t *d_qflag = nullptr;
     uint32_t *d_unsorted = nullptr;
@@ -318,10 +390,76 @@ int launch_index_query(const DistancePlan &plan, const uint32_t *d_q, uint64_t n
                                                                  plan.d_flag, d_acc);
             PG_LAUNCH_CHECK("index_pairwise_kernel");
         }
-        index_select_kernel<<<(unsigned)rows, SEL_THREADS, 0, st>>>(d_acc, n, rb, std::max<uint32_t>(den, 1), top_k, min_same, d_ref, d_same,
-                                                                    d_dist, d_n_hits);
-        PG_LAUNCH_CHECK("index_select_kernel");
+        const int rc_ = consume(d_acc, rb, re);
+        if (rc_ != PG_OK) return rc_;
     }
+    return PG_OK;
+}
+
+}  // namespace
+
+int launch_index_query(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t top_k, uint32_t min_same,
+                       uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint32_t *d_n_hits, cudaStream_t st) {
+    if (top_k == 0 || top_k > INDEX_MAX_TOP_K) {
+        set_error("top_k %u outside [1, %u]", top_k, INDEX_MAX_TOP_K);
+        return PG_ERR_ARG;
+    }
+    if (nq == 0) return PG_OK;
+    if (sq <= 0) {
+        set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq);
+        return PG_ERR_PANIC;
+    }
+    const uint64_t n = plan.n;
+    const uint32_t den = std::min<uint32_t>((uint32_t)sq, (uint32_t)plan.s);
+    if (n && den >= (1u << 24)) { set_error("sketch size %u above the selection's 2^24 limit", den); return PG_ERR_UNSUPPORTED; }
+    return index_blocks(plan, d_q, nq, sq, st, [&](const uint32_t *d_acc, uint64_t rb, uint64_t re) {
+        index_select_kernel<<<(unsigned)(re - rb), SEL_THREADS, 0, st>>>(d_acc, n, rb, std::max<uint32_t>(den, 1), top_k, min_same, d_ref,
+                                                                         d_same, d_dist, d_n_hits);
+        PG_LAUNCH_CHECK("index_select_kernel");
+        return PG_OK;
+    });
+}
+
+int launch_index_within(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, uint64_t *d_off,
+                        uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint64_t cap, uint64_t *d_total, cudaStream_t st) {
+    if (min_same == 0) {
+        set_error("min_same 0 would list all %llu x %llu pairs", (unsigned long long)nq, (unsigned long long)plan.n);
+        return PG_ERR_ARG;
+    }
+    if (nq == 0) {
+        if (d_off) PG_CUDA(cudaMemsetAsync(d_off, 0, 8, st));
+        if (d_total) PG_CUDA(cudaMemsetAsync(d_total, 0, 8, st));
+        return PG_OK;
+    }
+    if (sq <= 0) {
+        set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq);
+        return PG_ERR_PANIC;
+    }
+    if (!d_off) { set_error("null hit_offsets"); return PG_ERR_ARG; }
+    const uint64_t n = plan.n;
+    const uint32_t den = std::max<uint32_t>(std::min<uint32_t>((uint32_t)sq, (uint32_t)plan.s), 1);
+    StreamScratch sc(st);
+    uint8_t *d_scan = nullptr;  // CUB's scan storage, allocated for the first block (the largest)
+    size_t have = 0;
+    PG_CUDA(cudaMemsetAsync(d_off, 0, 8, st));
+    const int rc = index_blocks(plan, d_q, nq, sq, st, [&](const uint32_t *d_acc, uint64_t rb, uint64_t re) {
+        const unsigned rows = (unsigned)(re - rb);
+        index_within_count_kernel<<<rows, SEL_THREADS, 0, st>>>(d_acc, n, rb, min_same, d_off);
+        PG_LAUNCH_CHECK("index_within_count_kernel");
+        // d_off[rb] holds the total of the rows before the block: the inclusive scan makes the counts global offsets
+        size_t bytes = 0;
+        PG_CUDA(cub::DeviceScan::InclusiveSum(nullptr, bytes, d_off + rb, d_off + rb, (int64_t)rows + 1, st));
+        if (bytes > have) {
+            PG_CUDA(sc.alloc(&d_scan, bytes));
+            have = bytes;
+        }
+        PG_CUDA(cub::DeviceScan::InclusiveSum(d_scan, bytes, d_off + rb, d_off + rb, (int64_t)rows + 1, st));
+        index_within_fill_kernel<<<rows, SEL_THREADS, 0, st>>>(d_acc, n, rb, den, min_same, d_off, cap, d_ref, d_same, d_dist);
+        PG_LAUNCH_CHECK("index_within_fill_kernel");
+        return PG_OK;
+    });
+    if (rc != PG_OK) return rc;
+    if (d_total) PG_CUDA(cudaMemcpyAsync(d_total, d_off + nq, 8, cudaMemcpyDeviceToDevice, st));
     return PG_OK;
 }
 

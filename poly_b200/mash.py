@@ -350,6 +350,62 @@ class SketchIndex:
         _index_rc(rc)
         return ref[:, :k], same[:, :k], dist[:, :k], nh
 
+    def within(self, queries, min_same: Optional[int] = None, max_distance: Optional[float] = None):
+        """For each query sketch, every reference with at least min_same matching hashes (default 1) -- or,
+        alternatively, with Distance <= max_distance -- however many there are, in reference order.  Returns CSR
+        lists (offsets [nq + 1] uint64, ref [m] uint32, same [m] uint32, distance [m] float64): query q's hits are
+        entries [offsets[q], offsets[q + 1]).  A max_distance that every pair meets (>= 1) is a ValueError.
+
+        CUDA tensor queries give CUDA tensors (int64 offsets, int32 tensors carrying the uint32 bits).  The total
+        sizes the outputs, so this call waits for the device to count it, as torch.nonzero does."""
+        if self._h is None:
+            raise ValueError("the index is closed")
+        if min_same is not None and max_distance is not None:
+            raise ValueError("give min_same or max_distance, not both")
+        rows = _sketch_rows(queries)
+        nq, sq = int(rows.shape[0]), int(rows.shape[1])
+        if max_distance is not None:
+            min_same = min_same_for_distance(max_distance, min(sq, self.s))
+            if min_same == 0:
+                raise ValueError(f"max_distance {max_distance!r} lists every pair: every Distance is <= it")
+        min_same = 1 if min_same is None else int(min_same)
+        if not 0 <= min_same <= 0xFFFFFFFF:
+            raise ValueError("min_same must fit 32 bits")
+        cap = min(nq * self.n, max(1024, 64 * nq))  # first guess; one retry with the exact total when it is short
+        on_device = hasattr(rows, "data_ptr")
+        if on_device:
+            import torch
+
+            dev = rows.device
+            st = torch.cuda.current_stream(dev).cuda_stream
+            off = torch.empty(nq + 1, dtype=torch.int64, device=dev)
+            total = torch.zeros((), dtype=torch.int64, device=dev)
+            while True:
+                ref = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+                same = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+                dist = torch.empty(max(cap, 1), dtype=torch.float64, device=dev)
+                _index_rc(_lib.lib().pg_mash_index_query_within_dev(self._h, rows.data_ptr(), nq, sq, min_same, off.data_ptr(), ref.data_ptr(),
+                                                                    same.data_ptr(), dist.data_ptr(), cap, total.data_ptr(), st))
+                self._dev_queried = dev
+                m = int(total.item())
+                if m <= cap:
+                    return off, ref[:m], same[:m], dist[:m]
+                cap = m
+        off = np.empty(nq + 1, dtype=np.uint64)
+        cnt = C.c_uint64(0)
+        while True:
+            ref = np.empty(max(cap, 1), dtype=np.uint32)
+            same = np.empty(max(cap, 1), dtype=np.uint32)
+            dist = np.empty(max(cap, 1), dtype=np.float64)
+            rc = _lib.lib().pg_mash_index_query_within(self._h, rows.ctypes.data, nq, sq, min_same, off.ctypes.data, ref.ctypes.data,
+                                                       same.ctypes.data, dist.ctypes.data, cap, C.byref(cnt))
+            if rc == _lib.PG_ERR_ARG and cnt.value > cap:
+                cap = int(cnt.value)
+                continue
+            _index_rc(rc)
+            m = int(cnt.value)
+            return off, ref[:m], same[:m], dist[:m]
+
     def close(self) -> None:
         if self._h is not None:
             if self._dev_queried is not None:  # results of device queries may still be in flight on torch's streams
