@@ -588,8 +588,8 @@ func FastqIngestRecords(text []byte) (bases []byte, offsets []uint64, spans []ui
 }
 
 // Index wraps a pg_mash_index: a reference sketch set copied to the device of the calling thread
-// (pg_thread_device / pg_init) and indexed there once.  It is read-only after NewIndex: any number of
-// goroutines may call Query at once.  Close must not run while a Query is in flight.
+// (pg_thread_device / pg_init) and indexed there once.  Any number of goroutines may call Query at once; Add
+// waits for the queries in flight and they wait for it.  Close must not run while a Query is in flight.
 type Index struct {
 	h *C.pg_mash_index
 }
@@ -608,6 +608,16 @@ func NewIndex(sketches []uint32, n, s int) (*Index, error) {
 		return nil, err
 	}
 	return &Index{h: h}, nil
+}
+
+// Add wraps pg_mash_index_add: n more sketches of s words each (full arrays, zero tails included) become
+// references len .. len + n - 1, merged into the index on the device.
+func (ix *Index) Add(sketches []uint32, n, s int) error {
+	var p *C.uint32_t
+	if len(sketches) > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
+	}
+	return locked(func() C.int { return C.pg_mash_index_add(ix.h, p, C.uint64_t(n), C.int32_t(s)) })
 }
 
 // Query wraps pg_mash_index_query: for each of nq query sketches of sq words, up to k references with

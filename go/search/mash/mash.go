@@ -6,6 +6,7 @@ package mash
 import (
 	"errors"
 	"fmt"
+	"sync"
 
 	"github.com/bebop/poly/internal/polyb200"
 )
@@ -246,6 +247,8 @@ type Neighbor struct {
 // copied; the references may be changed or dropped afterwards).  Safe for concurrent use; call Close when done.
 type Index struct {
 	ix *polyb200.Index
+	mu sync.Mutex // guards n and s, which Add changes
+	n  int
 	s  int
 }
 
@@ -268,7 +271,37 @@ func NewIndex(references []*Mash) (*Index, error) {
 	} else if err != nil {
 		return nil, err
 	}
-	return &Index{ix: ix, s: s}, nil
+	return &Index{ix: ix, n: len(references), s: s}, nil
+}
+
+// Add appends references of the index's SketchSize (any one SketchSize when the index holds none yet) on the
+// GPU: they take the next positions, and later queries answer as an index built over the whole list would.
+func (ix *Index) Add(references []*Mash) error {
+	if len(references) == 0 {
+		return nil
+	}
+	s := references[0].SketchSize
+	flat := make([]uint32, 0, len(references)*s)
+	for _, m := range references {
+		if m.SketchSize != s {
+			return errors.New("mash: every reference of an index must have the same SketchSize")
+		}
+		flat = append(flat, m.Sketches[:s]...)
+	}
+	ix.mu.Lock()
+	defer ix.mu.Unlock()
+	if ix.n > 0 && s != ix.s {
+		return errors.New("mash: every reference of an index must have the same SketchSize")
+	}
+	err := ix.ix.Add(flat, len(references), s)
+	if errors.Is(err, polyb200.ErrPanic) {
+		panic("runtime error: index out of range [-1]") // Similarity on a sketch of size 0 would
+	} else if err != nil {
+		return err
+	}
+	ix.n += len(references)
+	ix.s = s
+	return nil
 }
 
 // Nearest returns, for each query (all of one SketchSize), the k references with the largest matching counts
@@ -311,10 +344,12 @@ func (ix *Index) Within(queries []*Mash, maxDistance float64) ([][]Neighbor, err
 	if len(queries) > 0 {
 		sq = queries[0].SketchSize
 	}
+	ix.mu.Lock()
 	den := sq
 	if ix.s < den {
 		den = ix.s
 	}
+	ix.mu.Unlock()
 	minSame := 0
 	for minSame <= den && !(1-float64(minSame)/float64(den) <= maxDistance) {
 		minSame++

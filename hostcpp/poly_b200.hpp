@@ -346,6 +346,15 @@ public:
     Index(const Index &) = delete;
     Index &operator=(const Index &) = delete;
     ~Index() { pg_mash_index_free(h_); }
+    // Appends references on the device: they take the next ids, and later queries answer as an index built over
+    // the whole set would.  An empty index takes the batch's SketchSize.
+    void Add(const std::vector<Mash> &refs) {
+        int s;
+        const std::vector<uint32_t> flat = detail::FlatRows(refs, "references", &s);
+        int rc = pg_mash_index_add(h_, flat.data(), refs.size(), s);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+    }
     // For each query, up to k references with Same >= minSame, by Same descending and then Ref ascending.
     std::vector<std::vector<Neighbor>> Nearest(const std::vector<Mash> &queries, uint32_t k, uint32_t minSame = 1) const {
         int sq;

@@ -320,9 +320,12 @@ int pg_mash_dereplicate_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, u
  *   - the index lives on the device current for the calling thread at creation (pg_thread_device /
  *     pg_init); queries run on that device whatever thread calls them (the calling thread's current
  *     CUDA device is set to it).  _dev queries take device pointers on that device;
- *   - the index is read-only after creation: any number of threads may query one index at once.
- *     Freeing an index while a query on it is running, or while a _dev query is still enqueued on a
- *     stream that has not been synchronised, is the caller's error;
+ *   - the index changes only through pg_mash_index_add (below).  Each index has a reader-writer lock:
+ *     every query call, host or _dev, holds it shared while it reads the index and enqueues, and an add
+ *     holds it exclusively.  So any number of threads may query one index at once, and a query sees the
+ *     index either wholly before or wholly after an add.  Freeing an index or adding to it while a _dev
+ *     query on it is still enqueued on a stream that has not been synchronised is the caller's error (both
+ *     release device buffers the query reads), as is freeing it while any call on it is running;
  *   - create, create_dev and both query calls synchronise (the host chooses the kernels from the data);
  *     query_dev leaves its outputs on the device, ordered on `stream`.
  */
@@ -336,6 +339,39 @@ int pg_mash_index_query_dev(const pg_mash_index *ix, const uint32_t *d_queries, 
                             uint32_t min_same, uint32_t *d_hit_ref, uint32_t *d_hit_same, double *d_hit_distance,
                             uint32_t *d_n_hits, void *stream);
 int pg_mash_index_free(pg_mash_index *ix);
+
+/* ---- sketch index: growing it ----------------------------------------------------------------------
+ * pg_mash_index_add appends m sketches of size s (m x s full Go arrays, zero tail included, as create takes
+ * them) as references n .. n + m - 1.  The batch is copied; no caller pointer is retained.
+ *   - Invariant: for any split of a reference set R into R0, R1, ..., Rk, create(R0) followed by add(R1) ...
+ *     add(Rk) answers every later pg_mash_index_query / pg_mash_index_query_within call (host or _dev) with
+ *     the same hit_ref, hit_same, n_hits, hit_offsets and the same bytes of hit_distance as create(R).
+ *   - Sketch size: an index that holds no reference (n == 0, whatever s it was created with) takes the s of
+ *     the first non-empty batch; after that every batch must have the index's s.
+ *   - Errors, checked in this order: a null index is PG_ERR_ARG (no device is needed); m == 0 is valid and
+ *     changes nothing; s <= 0 is PG_ERR_PANIC, as in create; an s other than a non-empty index's s is
+ *     PG_ERR_ARG; n + m > 2^32 - 1 is PG_ERR_ARG (the join keys hold 32-bit ids), checked before any buffer
+ *     is read; a null buffer is PG_ERR_ARG.  PG_ERR_NOMEM when device memory runs out.  After any error
+ *     the index holds exactly what it held before and still answers queries.
+ *   - The join index: when every reference so far is ascending and the index has its (value, id) join, an
+ *     ascending batch is merged into it on the device, with no rebuild.  A batch with an unsorted sketch
+ *     drops the join, and from then on every query row is compared pairwise, as create does for a set with
+ *     an unsorted sketch.  An index without a join (unsorted references, values too skewed for the join, or
+ *     PG_K3_PAIRWISE at creation) stays without one; an empty index is indexed as create would index the
+ *     batch.  Answers are the same either way; only the speed differs.
+ *   - Device memory: the old and the new index are both held until the add completes.  With T old join
+ *     entries and M = m x s new ones the peak of a merge is the sum of the old sketches (4 n s bytes), the
+ *     new copy (4 (n + m) s bytes), the old entries (8 T bytes), the batch's keys and their sort (16 M bytes
+ *     plus CUB's temporary storage), the merged entries (8 (T + M) bytes) and the index's flags (n + m bytes);
+ *     the host call adds 4 m s bytes, the batch staged on the device.
+ *   - Synchronisation: both calls synchronise; the host must read how many batch sketches are unsorted to
+ *     choose the join update, as create does.  The _dev call reads d_sketches on `stream` and does its work
+ *     there.
+ *   - Threads: see the index block above; an add excludes every query and every other add on the index.
+ *     The lock prefers readers: an add waits until no query holds it, so a steady stream of overlapping
+ *     queries from many threads can delay an add for as long as the stream lasts. */
+int pg_mash_index_add(pg_mash_index *ix, const uint32_t *sketches, uint64_t m, int32_t s);
+int pg_mash_index_add_dev(pg_mash_index *ix, const uint32_t *d_sketches, uint64_t m, int32_t s, void *stream);
 
 /* ---- sketch index: every reference within a matching-count cut (radius query) ----------------------
  * The question "which references lie within Distance <= d of each query, however many there are", answered

@@ -75,6 +75,8 @@ _SIGS = {
     "pg_mash_index_query": (C.c_int, [C.c_void_p, _u32p, C.c_uint64, C.c_int32, C.c_uint32, C.c_uint32, _u32p, _u32p, _f64p, _u32p]),
     "pg_mash_index_query_dev": (C.c_int, [C.c_void_p, _u32p, C.c_uint64, C.c_int32, C.c_uint32, C.c_uint32, _u32p, _u32p, _f64p, _u32p, C.c_void_p]),
     "pg_mash_index_free": (C.c_int, [C.c_void_p]),
+    "pg_mash_index_add": (C.c_int, [C.c_void_p, _u32p, C.c_uint64, C.c_int32]),
+    "pg_mash_index_add_dev": (C.c_int, [C.c_void_p, _u32p, C.c_uint64, C.c_int32, C.c_void_p]),
     "pg_mash_index_query_within": (C.c_int, [C.c_void_p, _u32p, C.c_uint64, C.c_int32, C.c_uint32, _u64p, _u32p, _u32p, _f64p, C.c_uint64,
                                              C.POINTER(C.c_uint64)]),
     "pg_mash_index_query_within_dev": (C.c_int, [C.c_void_p, _u32p, C.c_uint64, C.c_int32, C.c_uint32, _u64p, _u32p, _u32p, _f64p, C.c_uint64,

@@ -6,6 +6,7 @@
 #include <cstring>
 #include <functional>
 #include <sched.h>
+#include <shared_mutex>
 #include <string>
 #include <thread>
 #include <vector>
@@ -16,6 +17,7 @@ struct pg_mash_index {
     int device;
     uint32_t *d_sk;        // the index's own copy of the n x s reference sketches
     pg::DistancePlan plan;  // sortedness flags + join index over d_sk
+    mutable std::shared_mutex rw;  // queries hold it shared while they read the plan and enqueue, an add exclusively
 };
 
 namespace pg {
@@ -468,6 +470,43 @@ static int index_create(const uint32_t *src, bool src_dev, uint64_t n, int32_t s
     return PG_OK;
 }
 
+// Appends m rows of size s from src (checked by the caller, who holds ix->rw exclusively): a new copy of the n + m
+// rows and the plan grown over it; the index takes both only once they are complete, so on an error it keeps
+// what it held.
+static int index_add(pg_mash_index *ix, const uint32_t *src, bool src_dev, uint64_t m, int32_t s, cudaStream_t st) {
+    const uint64_t n = ix->plan.n, old_words = n * (uint64_t)s, words = old_words + m * (uint64_t)s;
+    uint32_t *d_sk = nullptr;
+    cudaError_t e = cudaMallocAsync(&d_sk, words * 4, st);
+    if (e != cudaSuccess) { cudaGetLastError(); set_error("cudaMallocAsync(%llu) for the index failed", (unsigned long long)(words * 4)); return PG_ERR_NOMEM; }
+    if (old_words) e = cudaMemcpyAsync(d_sk, ix->d_sk, old_words * 4, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_sk + old_words, src, (words - old_words) * 4, src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st);
+    int rc = e == cudaSuccess ? PG_OK : cuda_fail(e, "index copy", __FILE__, __LINE__);
+    DistancePlan plan;
+    if (rc == PG_OK) rc = distance_plan_grow(ix->plan, d_sk, m, s, st, &plan);
+    if (rc == PG_OK) { e = cudaStreamSynchronize(st); if (e != cudaSuccess) rc = cuda_fail(e, "index add", __FILE__, __LINE__); }
+    if (rc != PG_OK) {
+        distance_plan_destroy(plan, st);
+        cudaFreeAsync(d_sk, st);
+        cudaStreamSynchronize(st);
+        return rc;
+    }
+    distance_plan_destroy(ix->plan, st);
+    if (ix->d_sk) cudaFreeAsync(ix->d_sk, st);
+    ix->d_sk = d_sk;
+    ix->plan = plan;
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
+}
+
+// The argument rules of pg_mash_index_add after the null index and m == 0, in their order
+static int index_add_check(const pg_mash_index *ix, const void *sketches, uint64_t m, int32_t s) {
+    if (s <= 0) { set_error("index over sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
+    if (ix->plan.n && s != ix->plan.s) { set_error("sketches of size %d added to an index of size %d", s, ix->plan.s); return PG_ERR_ARG; }
+    if (m > 0xffffffffull - ix->plan.n) { set_error("%llu + %llu references exceed 2^32 - 1", (unsigned long long)ix->plan.n, (unsigned long long)m); return PG_ERR_ARG; }
+    if (!sketches) { set_error("null buffer"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
 }  // namespace
 }  // namespace pg
 
@@ -839,6 +878,7 @@ int pg_mash_index_query_dev(const pg_mash_index *ix, const uint32_t *d_queries, 
     if (!ix) { set_error("null index"); return PG_ERR_ARG; }
     int rc = use_device(ix->device);
     if (rc != PG_OK) return rc;
+    std::shared_lock<std::shared_mutex> lk(ix->rw);
     return launch_index_query(ix->plan, d_queries, nq, sq, top_k, min_same, d_hit_ref, d_hit_same, d_hit_distance, d_n_hits,
                               (cudaStream_t)stream);
 }
@@ -852,6 +892,7 @@ int pg_mash_index_query(const pg_mash_index *ix, const uint32_t *queries, uint64
     if (nq == 0) return PG_OK;
     if (sq <= 0) { set_error("query sketches of size %d: the reference panics (Sketches[-1])", sq); return PG_ERR_PANIC; }
     if (!queries) { set_error("null buffer"); return PG_ERR_ARG; }
+    std::shared_lock<std::shared_mutex> lk(ix->rw);
     HostCall c;
     const uint64_t slots = nq * (uint64_t)top_k;
     const uint32_t *d_q = c.upload(queries, nq * (uint64_t)sq);
@@ -875,6 +916,7 @@ int pg_mash_index_query_within_dev(const pg_mash_index *ix, const uint32_t *d_qu
     if (!ix) { set_error("null index"); return PG_ERR_ARG; }
     int rc = use_device(ix->device);
     if (rc != PG_OK) return rc;
+    std::shared_lock<std::shared_mutex> lk(ix->rw);
     return launch_index_within(ix->plan, d_queries, nq, sq, min_same, d_hit_offsets, d_hit_ref, d_hit_same, d_hit_distance, hits_cap,
                                d_n_hits, (cudaStream_t)stream);
 }
@@ -886,6 +928,7 @@ int pg_mash_index_query_within(const pg_mash_index *ix, const uint32_t *queries,
     int rc = use_device(ix->device);
     if (rc != PG_OK) return rc;
     if (n_hits) *n_hits = 0;
+    std::shared_lock<std::shared_mutex> lk(ix->rw);
     if (min_same == 0) { set_error("min_same 0 would list all %llu x %llu pairs", (unsigned long long)nq, (unsigned long long)ix->plan.n); return PG_ERR_ARG; }
     if (nq == 0) {
         if (hit_offsets) hit_offsets[0] = 0;
@@ -907,6 +950,32 @@ int pg_mash_index_query_within(const pg_mash_index *ix, const uint32_t *queries,
     const bool counting = !hit_ref && !hit_same && !hit_distance;  // no list to overflow
     return finish_capped(c, d_n, counting ? ~0ull : hits_cap, n_hits ? n_hits : &total,
                          {{hit_ref, d_ref, 4}, {hit_same, d_same, 4}, {hit_distance, d_dist, 8}}, "hits_cap", "hits");
+}
+
+// ---------------------------------------------------------------------------------
+// Sketch index: growing it
+// ---------------------------------------------------------------------------------
+int pg_mash_index_add(pg_mash_index *ix, const uint32_t *sketches, uint64_t m, int32_t s) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    if (m == 0) return PG_OK;
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> lk(ix->rw);
+    if ((rc = index_add_check(ix, sketches, m, s)) != PG_OK) return rc;
+    HostCall c;
+    const uint32_t *d_b = c.upload(sketches, m * (uint64_t)s);
+    if ((rc = c.error()) || (rc = index_add(ix, d_b, true, m, s, c.st))) return rc;
+    return c.finish();
+}
+
+int pg_mash_index_add_dev(pg_mash_index *ix, const uint32_t *d_sketches, uint64_t m, int32_t s, void *stream) {
+    if (!ix) { set_error("null index"); return PG_ERR_ARG; }
+    if (m == 0) return PG_OK;
+    int rc = use_device(ix->device);
+    if (rc != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> lk(ix->rw);
+    if ((rc = index_add_check(ix, d_sketches, m, s)) != PG_OK) return rc;
+    return index_add(ix, d_sketches, true, m, s, (cudaStream_t)stream);
 }
 
 int pg_mash_index_free(pg_mash_index *ix) {

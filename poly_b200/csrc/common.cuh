@@ -189,6 +189,7 @@ struct JoinIndex {
     uint64_t *entries = nullptr, *start = nullptr;
     uint32_t *vmax = nullptr;  // device word: the largest value, which sets the bucket scale (hist_kernel)
     uint64_t nb = 0, n = 0;
+    uint64_t largest = 0;  // entries of the largest bucket: join_emit needs <= JOIN_CAP, the probe has no limit
     int s = 0;
     bool ok = false;
 };
@@ -201,6 +202,7 @@ __device__ __forceinline__ uint32_t join_bucket(uint32_t v, uint64_t scale, uint
     return min((uint32_t)(((uint64_t)v * scale) >> 32), nb - 1);
 }
 int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinIndex *ix);
+int join_merge(const JoinIndex &old, const uint32_t *d_batch, uint64_t m, cudaStream_t st, JoinIndex *out);
 int join_emit(const JoinIndex &ix, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st);
 void join_free(JoinIndex &ix, cudaStream_t st);
 // distance.cu: a plan = sortedness flags (+ join index when every sketch is ascending)
@@ -214,6 +216,10 @@ struct DistancePlan {
 int distance_plan_create(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, DistancePlan *plan);
 int distance_plan_rows(const DistancePlan &plan, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st);
 void distance_plan_destroy(DistancePlan &plan, cudaStream_t st);
+// The plan over n + m sketches of size s whose first n are plan's: d_sk holds all n + m rows.  Flags of the new
+// rows; the join merged (every new row ascending), dropped (one is not) or still absent; an empty plan is created
+// afresh.  plan is not changed; on an error nothing of *out remains allocated.
+int distance_plan_grow(const DistancePlan &plan, const uint32_t *d_sk, uint64_t m, int s, cudaStream_t st, DistancePlan *out);
 // distance.cu: rows per dense tile of the passes that consume a plan's tiles on the device (sparse pairs, cluster,
 // dereplicate); n > 0
 uint64_t distance_tile_rows(uint64_t n, uint64_t rows);

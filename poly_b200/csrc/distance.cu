@@ -286,6 +286,33 @@ int distance_plan_create(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t s
     return PG_OK;
 }
 
+int distance_plan_grow(const DistancePlan &plan, const uint32_t *d_sk, uint64_t m, int s, cudaStream_t st, DistancePlan *out) {
+    const uint64_t n = plan.n;
+    int rc = PG_OK;
+    if (n == 0) {  // nothing to keep: the plan create would build over the batch
+        rc = distance_plan_create(d_sk, m, s, st, out);
+    } else {
+        *out = DistancePlan();
+        out->d_sk = d_sk; out->n = n + m; out->s = s;
+        uint32_t n_unsorted = 1;
+        cudaError_t e = cudaMallocAsync(&out->d_flag, n + m + 8, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(out->d_flag, plan.d_flag, n, cudaMemcpyDeviceToDevice, st);
+        if (e != cudaSuccess) rc = cuda_fail(e, "plan flags", __FILE__, __LINE__);
+        uint32_t *d_unsorted = reinterpret_cast<uint32_t *>(out->d_flag + ((n + m + 3) & ~3ull));
+        if (rc == PG_OK) rc = launch_sorted_flags(d_sk + n * (uint64_t)s, m, s, out->d_flag + n, d_unsorted, st);
+        if (rc == PG_OK) {
+            e = cudaMemcpyAsync(&n_unsorted, d_unsorted, 4, cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+            if (e != cudaSuccess) rc = cuda_fail(e, "plan flags", __FILE__, __LINE__);
+        }
+        // a join and an ascending batch: merge; an unsorted row in the batch leaves every row to the pairwise
+        // kernel, as create does for such a set; a plan without a join stays without one
+        if (rc == PG_OK && plan.join.ok && n_unsorted == 0) rc = join_merge(plan.join, d_sk + n * (uint64_t)s, m, st, &out->join);
+    }
+    if (rc != PG_OK) distance_plan_destroy(*out, st);
+    return rc;
+}
+
 void distance_plan_destroy(DistancePlan &plan, cudaStream_t st) {
     join_free(plan.join, st);
     if (plan.d_flag) cudaFreeAsync(plan.d_flag, st);

@@ -17,6 +17,11 @@
 // data is so skewed that a bucket cannot fit shared memory even with the finest bucketing, the
 // caller falls back to the pairwise kernel (distance.cu).
 #include <algorithm>
+#include <cstdlib>
+#include <vector>
+
+#include <cub/device/device_merge.cuh>
+#include <cub/device/device_radix_sort.cuh>
 
 #include "common.cuh"
 
@@ -38,11 +43,17 @@ __global__ void max_value_kernel(const uint32_t *__restrict__ sk, uint64_t n, ui
     if ((threadIdx.x & 31) == 0) atomicMax(vmax, m);
 }
 
-__global__ void hist_kernel(const uint32_t *__restrict__ sk, uint64_t total, const uint32_t *__restrict__ vmax,
+// the value of a sketch word, or of a (value << 32 | id) join key
+__device__ __forceinline__ uint32_t join_value(uint32_t v) { return v; }
+__device__ __forceinline__ uint32_t join_value(uint64_t key) { return (uint32_t)(key >> 32); }
+
+// bucket counts of `total` values: the words of a sketch set (join_build) or the keys of a merged index (join_merge)
+template <typename T>
+__global__ void hist_kernel(const T *__restrict__ src, uint64_t total, const uint32_t *__restrict__ vmax,
                             uint32_t nbuckets, uint32_t *__restrict__ hist) {
     const uint64_t scale = join_bucket_scale(nbuckets, *vmax);
     for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
-        const uint32_t b = join_bucket(__ldg(sk + e), scale, nbuckets);
+        const uint32_t b = join_bucket(join_value(__ldg(src + e)), scale, nbuckets);
         // consecutive elements of an ascending row mostly share a bucket: aggregate per warp
         const uint32_t peers = __match_any_sync(__activemask(), b);
         if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&hist[b], __popc(peers));
@@ -72,6 +83,35 @@ __global__ void scan_kernel(const uint32_t *__restrict__ hist, uint32_t nbuckets
     __syncthreads();
     uint64_t run = s_part[tid];
     for (uint32_t i = lo; i < hi; ++i) { start[i] = run; run += hist[i]; }
+}
+
+// The keys (v << 32 | id0 + row) of `total` words of ascending rows of s words, and their largest value into *vmax.
+__global__ void batch_keys_kernel(const uint32_t *__restrict__ sk, uint64_t total, uint32_t s, uint64_t id0,
+                                  uint64_t *__restrict__ keys, uint32_t *__restrict__ vmax) {
+    uint32_t m = 0;
+    for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t v = __ldg(sk + e);
+        keys[e] = ((uint64_t)v << 32) | (id0 + e / s);
+        m = max(m, v);
+    }
+    for (int d = 16; d > 0; d >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
+    if ((threadIdx.x & 31) == 0) atomicMax(vmax, m);
+}
+
+// Merge-path cut points of the merge of the sorted keys a[0, na) and b[0, nb) (no key in both): cut[k] = the
+// number of a's keys among the first min(k * piece, na + nb) keys of the merged order.
+__global__ void merge_cuts_kernel(const uint64_t *__restrict__ a, uint64_t na, const uint64_t *__restrict__ b, uint64_t nb, uint64_t piece,
+                                  uint64_t ncuts, uint64_t *__restrict__ cut) {
+    for (uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; k < ncuts; k += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t d = min(k * piece, na + nb);
+        uint64_t lo = d > nb ? d - nb : 0, hi = min(d, na);
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi) >> 1;
+            if (a[mid] < b[d - 1 - mid]) lo = mid + 1;
+            else hi = mid;
+        }
+        cut[k] = lo;
+    }
 }
 
 __global__ void scatter_kernel(const uint32_t *__restrict__ sk, uint64_t total, uint32_t s,
@@ -254,6 +294,13 @@ __global__ void same_to_distance_kernel(const uint32_t *__restrict__ same, uint6
         dist[i] = 1 - (double)same[i] / (double)s;  // mash.go:134,139
 }
 
+// the first bucket count tried for `total` entries: ~2k entries a bucket, at most 2^22 buckets
+uint64_t join_first_nb(uint64_t total) {
+    uint64_t nb = 1;
+    while (nb * 2048 < total) nb <<= 1;
+    return std::min<uint64_t>(nb, 1u << 22);
+}
+
 }  // namespace
 
 // Builds the bucketed (value, id) index of n ascending sketches.  ix->ok == false means "not
@@ -269,9 +316,7 @@ int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinInd
     const unsigned sms = (unsigned)sm_count();
     max_value_kernel<<<sms * 4, 256, 0, st>>>(d_sk, n, (uint32_t)s, d_scalars);
     note_launch("max_value_kernel");
-    uint64_t nb = 1;
-    while (nb * 2048 < total) nb <<= 1;
-    nb = std::min<uint64_t>(std::max<uint64_t>(nb, 1), 1u << 22);
+    uint64_t nb = join_first_nb(total);
     for (int attempt = 0; attempt < 3 && !ix->ok; ++attempt) {
         uint32_t *d_hist = nullptr, *d_cursor = nullptr;
         uint64_t *d_start = nullptr;
@@ -280,7 +325,7 @@ int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinInd
         PG_CUDA(cudaMallocAsync(&d_start, (nb + 1) * 8, st));
         PG_CUDA(cudaMemsetAsync(d_hist, 0, nb * 4, st));
         PG_CUDA(cudaMemsetAsync(d_cursor, 0, nb * 4, st));
-        hist_kernel<<<sms * 16, 256, 0, st>>>(d_sk, total, d_scalars, (uint32_t)nb, d_hist);
+        hist_kernel<uint32_t><<<sms * 16, 256, 0, st>>>(d_sk, total, d_scalars, (uint32_t)nb, d_hist);
         note_launch("hist_kernel");
         scan_kernel<<<1, 1024, 0, st>>>(d_hist, (uint32_t)nb, d_start, d_scalars + 1);
         note_launch("scan_kernel");
@@ -295,7 +340,7 @@ int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinInd
             { const int rc_ = func_smem((const void *)bucket_sort_kernel, JOIN_CAP * 8); if (rc_ != PG_OK) return rc_; }
             bucket_sort_kernel<<<(unsigned)std::min<uint64_t>(nb, (uint64_t)sms * 24), JOIN_THREADS, JOIN_CAP * 8, st>>>(d_entries, d_start, (uint32_t)nb);
             note_launch("bucket_sort_kernel");
-            ix->entries = d_entries; ix->start = d_start; ix->nb = nb; ix->ok = true;
+            ix->entries = d_entries; ix->start = d_start; ix->nb = nb; ix->largest = largest; ix->ok = true;
         } else {
             cudaFreeAsync(d_start, st);
         }
@@ -313,8 +358,87 @@ int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinInd
     return PG_OK;
 }
 
+// The index of n + m ascending sketches from old's n and the m rows of d_batch (ascending, ids n .. n + m - 1):
+// the batch's keys sorted, merged with old's entries (the entries are globally sorted by key, bucket after bucket,
+// and no batch key equals an old one), then bucketed afresh for the new total with the first-choice bucket count
+// and vmax = max(old, batch).  Buckets are not bounded by JOIN_CAP: the probe searches them in global memory, and
+// join_emit refuses such an index.  CUB's merge counts keys in int, so the merged order is cut into pieces of at
+// most 2^31 - 1 keys (PG_JOIN_MERGE_PIECE: fewer) at merge-path cut points, each merged by one call; reading the
+// cut points is one more synchronisation when there is more than one piece.  old is not changed; on an error
+// nothing of *out remains allocated.  One synchronisation at the end, to read the largest bucket.
+int join_merge(const JoinIndex &old, const uint32_t *d_batch, uint64_t m, cudaStream_t st, JoinIndex *out) {
+    *out = JoinIndex();
+    const uint64_t T = old.n * (uint64_t)old.s, M = m * (uint64_t)old.s, total = T + M;
+    uint64_t piece = 0x7fffffffull;
+    if (const char *e = getenv("PG_JOIN_MERGE_PIECE")) piece = std::max<uint64_t>(1, std::min<uint64_t>(piece, strtoull(e, nullptr, 10)));
+    StreamScratch tmp(st), keep(st);  // keep: the new index's buffers, released unless the merge succeeds
+    const uint64_t nb = join_first_nb(total);
+    uint64_t *d_entries = nullptr, *d_start = nullptr, *d_keys = nullptr, *d_sorted = nullptr;
+    uint32_t *d_scalars = nullptr, *d_hist = nullptr;  // [0] vmax, [1] largest bucket
+    PG_CUDA(keep.alloc(&d_entries, total));
+    PG_CUDA(keep.alloc(&d_start, nb + 1));
+    PG_CUDA(keep.alloc(&d_scalars, 2));
+    PG_CUDA(tmp.alloc(&d_keys, M));
+    PG_CUDA(tmp.alloc(&d_sorted, M));
+    PG_CUDA(tmp.alloc(&d_hist, nb));
+    PG_CUDA(cudaMemcpyAsync(d_scalars, old.vmax, 4, cudaMemcpyDeviceToDevice, st));
+    PG_CUDA(cudaMemsetAsync(d_scalars + 1, 0, 4, st));
+    PG_CUDA(cudaMemsetAsync(d_hist, 0, nb * 4, st));
+    const unsigned sms = (unsigned)sm_count();
+    batch_keys_kernel<<<(unsigned)std::min<uint64_t>((M + 255) / 256, (uint64_t)sms * 16), 256, 0, st>>>(d_batch, M, (uint32_t)old.s, old.n,
+                                                                                                         d_keys, d_scalars);
+    PG_LAUNCH_CHECK("batch_keys_kernel");
+    size_t bytes = 0, have = 0;
+    uint8_t *d_cub = nullptr;
+    PG_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, d_keys, d_sorted, M, 0, 64, st));
+    PG_CUDA(tmp.alloc(&d_cub, bytes));
+    have = bytes;
+    PG_CUDA(cub::DeviceRadixSort::SortKeys(d_cub, bytes, d_keys, d_sorted, M, 0, 64, st));
+    // piece k of the merged order is old.entries[cut[k], cut[k + 1]) and d_sorted[k * piece - cut[k], ...)
+    const uint64_t pieces = (total + piece - 1) / piece;
+    std::vector<uint64_t> cut(pieces + 1);
+    cut[0] = 0;
+    cut[pieces] = T;
+    if (pieces > 1) {
+        uint64_t *d_cut = nullptr;
+        PG_CUDA(tmp.alloc(&d_cut, pieces + 1));
+        merge_cuts_kernel<<<(unsigned)std::min<uint64_t>((pieces + 256) / 256, (uint64_t)sms * 4), 256, 0, st>>>(old.entries, T, d_sorted, M, piece,
+                                                                                                                pieces + 1, d_cut);
+        PG_LAUNCH_CHECK("merge_cuts_kernel");
+        PG_CUDA(cudaMemcpyAsync(cut.data(), d_cut, (pieces + 1) * 8, cudaMemcpyDeviceToHost, st));
+        PG_CUDA(cudaStreamSynchronize(st));
+    }
+    for (uint64_t k = 0; k < pieces; ++k) {
+        const uint64_t d0 = k * piece, d1 = std::min(total, d0 + piece);
+        const uint64_t a0 = cut[k], a1 = cut[k + 1], b0 = d0 - a0, b1 = d1 - a1;
+        PG_CUDA(cub::DeviceMerge::MergeKeys(nullptr, bytes, old.entries + a0, (int)(a1 - a0), d_sorted + b0, (int)(b1 - b0), d_entries + d0,
+                                            ::cuda::std::less<uint64_t>(), st));
+        if (bytes > have) {
+            PG_CUDA(tmp.alloc(&d_cub, bytes));
+            have = bytes;
+        }
+        PG_CUDA(cub::DeviceMerge::MergeKeys(d_cub, bytes, old.entries + a0, (int)(a1 - a0), d_sorted + b0, (int)(b1 - b0), d_entries + d0,
+                                            ::cuda::std::less<uint64_t>(), st));
+    }
+    hist_kernel<uint64_t><<<sms * 16, 256, 0, st>>>(d_entries, total, d_scalars, (uint32_t)nb, d_hist);
+    PG_LAUNCH_CHECK("hist_kernel");
+    scan_kernel<<<1, 1024, 0, st>>>(d_hist, (uint32_t)nb, d_start, d_scalars + 1);
+    PG_LAUNCH_CHECK("scan_kernel");
+    uint32_t largest = 0;
+    PG_CUDA(cudaMemcpyAsync(&largest, d_scalars + 1, 4, cudaMemcpyDeviceToHost, st));
+    PG_CUDA(cudaStreamSynchronize(st));
+    out->entries = d_entries; out->start = d_start; out->vmax = d_scalars;
+    out->nb = nb; out->n = old.n + m; out->s = old.s; out->largest = largest; out->ok = true;
+    keep.ptr.clear();
+    return PG_OK;
+}
+
 // Rows [row_begin, row_end) of the matching-count matrix from a built index.
 int join_emit(const JoinIndex &ix, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st) {
+    if (ix.largest > JOIN_CAP) {  // a merged index (join_merge): its buckets need not fit bucket_join_kernel's tile
+        set_error("join index bucket of %llu entries exceeds the join kernel's %d", (unsigned long long)ix.largest, JOIN_CAP);
+        return PG_ERR_UNSUPPORTED;
+    }
     const uint64_t rows = row_end - row_begin;
     const unsigned sms = (unsigned)sm_count();
     PG_CUDA(cudaMemsetAsync(d_same, 0, rows * ix.n * 4, st));

@@ -310,6 +310,32 @@ class SketchIndex:
         sk, _, _, s = sketchfile.load(path, pad_zero=True)
         return cls(sk[:, :s])
 
+    def add(self, sketches) -> int:
+        """Appends reference sketches (what the constructor takes) on the device: the batch's rows become
+        references n, n + 1, ..., and every later query answers as an index built over the concatenated set would.
+        An empty index takes the batch's sketch size.  Returns the id of the first added reference."""
+        if self._h is None:
+            raise ValueError("the index is closed")
+        rows = _sketch_rows(sketches)
+        m, s = int(rows.shape[0]), int(rows.shape[1])
+        first = self.n
+        if self._dev_queried is not None:  # the add releases buffers that device queries, on any stream, may still read
+            import torch
+
+            torch.cuda.synchronize(self._dev_queried)
+        if hasattr(rows, "data_ptr"):
+            import torch
+
+            rc = _lib.lib().pg_mash_index_add_dev(self._h, rows.data_ptr(), m, s, torch.cuda.current_stream(rows.device).cuda_stream)
+        else:
+            rc = _lib.lib().pg_mash_index_add(self._h, rows.ctypes.data, m, s)
+        _index_rc(rc)
+        if m:
+            self.n += m
+            if first == 0:
+                self.s = s
+        return first
+
     def nearest(self, queries, k: int, min_same: Optional[int] = None, max_distance: Optional[float] = None):
         """For each query sketch, the k references with the largest matching counts (same descending, then
         reference index ascending), keeping only same >= min_same (default 1) -- or, alternatively, only
