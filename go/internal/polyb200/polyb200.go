@@ -675,6 +675,68 @@ func (ix *Index) Close() error {
 	return locked(func() C.int { return C.pg_mash_index_free(h) })
 }
 
+// Dereplicator wraps a pg_mash_dereplicator: a dereplication that grows batch by batch on the device of the
+// calling thread.  Adds from several goroutines are serialised by the library.  Close must not run while an Add
+// is in flight.
+type Dereplicator struct {
+	h *C.pg_mash_dereplicator
+}
+
+// NewDereplicator wraps pg_mash_dereplicator_create for sketches of s words at same >= minSame.
+func NewDereplicator(s, minSame int, nearest bool) (*Dereplicator, error) {
+	flags := C.uint32_t(0)
+	if nearest {
+		flags = C.PG_DEREP_NEAREST
+	}
+	var h *C.pg_mash_dereplicator
+	if err := locked(func() C.int { return C.pg_mash_dereplicator_create(C.int32_t(s), C.uint32_t(minSame), flags, &h) }); err != nil {
+		return nil, err
+	}
+	return &Dereplicator{h: h}, nil
+}
+
+// Add wraps pg_mash_dereplicator_add: n sketches of s words each (full arrays, zero tails included) become sketches
+// first .. first + n - 1; rep[i] is the id of row i's representative (first + i for a new one).
+func (d *Dereplicator) Add(sketches []uint32, n, s int) (rep []uint32, first, nNew uint64, err error) {
+	rep = make([]uint32, n+1)
+	var p *C.uint32_t
+	if len(sketches) > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
+	}
+	var f, nn C.uint64_t
+	err = locked(func() C.int {
+		return C.pg_mash_dereplicator_add(d.h, p, C.uint64_t(n), C.int32_t(s), (*C.uint32_t)(unsafe.Pointer(&rep[0])), &f, &nn)
+	})
+	return rep[:n], uint64(f), uint64(nn), err
+}
+
+// Reps wraps pg_mash_dereplicator_reps: the ids of the representatives kept so far, ascending.
+func (d *Dereplicator) Reps() ([]uint32, error) {
+	var n C.uint64_t
+	ids := make([]uint32, 1)
+	for {
+		capIDs := len(ids) - 1
+		err := locked(func() C.int { return C.pg_mash_dereplicator_reps(d.h, (*C.uint32_t)(unsafe.Pointer(&ids[0])), C.uint64_t(capIDs), &n) })
+		if err == nil {
+			return ids[:n], nil
+		}
+		if int(n) <= capIDs {
+			return nil, err
+		}
+		ids = make([]uint32, int(n)+1) // an add kept more since the last call
+	}
+}
+
+// Close wraps pg_mash_dereplicator_free.
+func (d *Dereplicator) Close() error {
+	if d.h == nil {
+		return nil
+	}
+	h := d.h
+	d.h = nil
+	return locked(func() C.int { return C.pg_mash_dereplicator_free(h) })
+}
+
 // SeqhashBatch wraps pg_seqhash_batch: digest[32*i:32*i+32], errCode[i] and errPos[i] for each of the
 // sequences bases[offsets[i]:offsets[i+1]], all of one seqType (0 DNA, 1 RNA, 2 PROTEIN) and flags
 // (1 circular | 2 double-stranded).

@@ -236,6 +236,72 @@ func Dereplicate(sketches []*Mash, maxDistance float64, nearest bool) ([]int, er
 	return reps, nil
 }
 
+// Dereplicator is a dereplication that grows: each Add assigns a batch of sketches against the representatives kept
+// so far, on the GPU, without dereplicating the earlier sketches again.  Sketches are numbered in the order they are
+// added, and after any sequence of adds the concatenated results equal Dereplicate of the concatenated batches.
+// Safe for concurrent use; call Close when done.
+type Dereplicator struct {
+	d *polyb200.Dereplicator
+	s int
+}
+
+// NewDereplicator prepares a dereplication of sketches of SketchSize s at Distance <= maxDistance, with the
+// assignment of Dereplicate.  A maxDistance that every pair satisfies, or none can, is an error.
+func NewDereplicator(s int, maxDistance float64, nearest bool) (*Dereplicator, error) {
+	if s <= 0 {
+		panic("runtime error: index out of range [-1]") // Similarity on a sketch of size 0 would
+	}
+	minSame := 0
+	for minSame <= s && !(1-float64(minSame)/float64(s) <= maxDistance) {
+		minSame++
+	}
+	if minSame == 0 || minSame > s {
+		return nil, fmt.Errorf("mash: maxDistance %v links every pair or none", maxDistance)
+	}
+	d, err := polyb200.NewDereplicator(s, minSame, nearest)
+	if err != nil {
+		return nil, err
+	}
+	return &Dereplicator{d: d, s: s}, nil
+}
+
+// Add assigns a batch of sketches of the dereplicator's SketchSize.  rep[i] is the position, among every sketch
+// added so far, of the representative of sketches[i]; it is first + i when sketches[i] is a new representative.
+func (d *Dereplicator) Add(sketches []*Mash) (rep []int, first int, err error) {
+	flat := make([]uint32, 0, len(sketches)*d.s)
+	for _, m := range sketches {
+		if m.SketchSize != d.s {
+			return nil, 0, errors.New("mash: Dereplicator needs one common SketchSize")
+		}
+		flat = append(flat, m.Sketches[:d.s]...)
+	}
+	r, f, _, err := d.d.Add(flat, len(sketches), d.s)
+	if err != nil {
+		return nil, 0, err
+	}
+	rep = make([]int, len(r))
+	for i, x := range r {
+		rep[i] = int(x)
+	}
+	return rep, int(f), nil
+}
+
+// Reps returns the positions of the representatives kept so far, ascending.
+func (d *Dereplicator) Reps() ([]int, error) {
+	ids, err := d.d.Reps()
+	if err != nil {
+		return nil, err
+	}
+	out := make([]int, len(ids))
+	for i, x := range ids {
+		out[i] = int(x)
+	}
+	return out, nil
+}
+
+// Close releases the dereplicator's device memory.
+func (d *Dereplicator) Close() error { return d.d.Close() }
+
 // Neighbor is one reference of a Nearest result.
 type Neighbor struct {
 	Index    int     // position in the reference list given to NewIndex

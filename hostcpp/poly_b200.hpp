@@ -438,6 +438,50 @@ inline Representatives Dereplicate(const std::vector<Mash> &mashes, uint32_t min
     return out;
 }
 
+// A growing dereplication: each Add assigns a batch against the representatives kept so far, on the device.
+// Sketches are numbered in the order they are added, and the concatenated Rep of any sequence of Adds equals
+// Dereplicate of the concatenated batches.
+class Dereplicator {
+    pg_mash_dereplicator *h_ = nullptr;
+
+public:
+    Dereplicator(int sketchSize, uint32_t minSame, bool nearest = false) {
+        int rc = pg_mash_dereplicator_create(sketchSize, minSame, nearest ? PG_DEREP_NEAREST : 0u, &h_);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+    }
+    Dereplicator(const Dereplicator &) = delete;
+    Dereplicator &operator=(const Dereplicator &) = delete;
+    ~Dereplicator() { pg_mash_dereplicator_free(h_); }
+    // Rep[i] = the id of batch row i's representative (First + i for a new one); NReps = the new representatives
+    struct Batch {
+        std::vector<uint32_t> Rep;
+        uint64_t First = 0, NReps = 0;
+    };
+    Batch Add(const std::vector<Mash> &mashes) {
+        int s;
+        const std::vector<uint32_t> flat = detail::FlatRows(mashes, "sketches", &s);
+        Batch out;
+        out.Rep.resize(mashes.size());
+        int rc = pg_mash_dereplicator_add(h_, flat.data(), mashes.size(), s, out.Rep.data(), &out.First, &out.NReps);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+        return out;
+    }
+    // the ids of the representatives kept so far, ascending
+    std::vector<uint32_t> Reps() const {
+        uint64_t n = 0;
+        std::vector<uint32_t> ids;
+        int rc;
+        do {  // an add on another thread may keep more between two calls
+            ids.resize(n);
+            rc = pg_mash_dereplicator_reps(h_, ids.data(), ids.size(), &n);
+        } while (rc == PG_ERR_ARG && n > ids.size());
+        check(rc);
+        return ids;
+    }
+};
+
 }  // namespace mash
 
 namespace align {

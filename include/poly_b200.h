@@ -410,6 +410,56 @@ int pg_mash_index_query_within_dev(const pg_mash_index *ix, const uint32_t *d_qu
                                    uint32_t *d_hit_same, double *d_hit_distance, uint64_t hits_cap,
                                    uint64_t *d_n_hits, void *stream);
 
+/* ---- dereplicate: growing a dereplication ------------------------------------------------------------
+ * A dereplicator keeps the representatives of every sketch added so far and assigns each new batch against them
+ * on the device, so a growing collection is never dereplicated from scratch.  Sketches are numbered in the order
+ * they are added: the rows of a batch are ids first .. first + m - 1 (m x s full Go arrays, as pg_mash_dereplicate
+ * takes them).  The batch is copied; no caller pointer is retained.
+ *   - Invariant: split a set S of sketches of one size into B0, B1, ..., Bk and call add(B0) ... add(Bk).  The
+ *     concatenated rep outputs equal pg_mash_dereplicate(S, min_same, flags) and the n_new_reps add up to its n_reps,
+ *     in both modes and for any split, empty and one-row batches included.  rep values are global ids.
+ *   - Why it is exact: under the greedy rule a sketch's flag and assignment depend only on the representatives
+ *     before it.  So no earlier row ever changes, and a batch row is decided by the kept representatives linked to
+ *     it and by the batch's own representatives before it.  The first are found by a query of the batch against
+ *     the representative index (the query is the receiver; for one sketch size the count is symmetric, so it is the
+ *     dereplicate count, unsorted sketches included), the second by the dereplicate pass over the batch alone.
+ *   - Link rule, count and cut: those of pg_mash_dereplicate.  PG_DEREP_NEAREST is the only flag.
+ *   - Errors.  create checks, in this order: a flags bit other than PG_DEREP_NEAREST is PG_ERR_ARG; s <= 0 is
+ *     PG_ERR_PANIC (the rule dereplicate applies to a non-empty set); min_same == 0 or min_same > s is PG_ERR_ARG.
+ *     add (host and _dev) checks, in this order: a null dereplicator is PG_ERR_ARG (no device is needed); m == 0 is
+ *     valid and changes nothing (*first = n, *n_new_reps = 0); s <= 0 is PG_ERR_PANIC; an s other than the
+ *     dereplicator's is PG_ERR_ARG; n + m > 2^32 - 1 is PG_ERR_ARG, checked before any buffer is read; a null
+ *     buffer (sketches or rep) is PG_ERR_ARG.  PG_ERR_UNSUPPORTED and PG_ERR_NOMEM arise where the index query,
+ *     the dereplicate pass or the index add raise them.  After any error the dereplicator holds exactly what it
+ *     held before; only the caller's rep contents are then unspecified.  first and n_new_reps may be NULL.
+ *   - Representative index: pg_mash_dereplicator_index returns a borrowed, read-only pg_mash_index whose reference
+ *     p is the p-th representative in ascending id order, so the existing top-k and radius queries answer "which
+ *     kept sketch is this one closest to".  pg_mash_dereplicator_reps maps positions to ids: the first min(cap,
+ *     n_reps) ids into `ids` and their number into *n_reps; more than cap is PG_ERR_ARG after the first cap are
+ *     stored.  Ids are append-only, so a reps read made after a query covers every position that query returned.
+ *     The handle is valid until pg_mash_dereplicator_free and must not be passed to pg_mash_index_add or
+ *     pg_mash_index_free.  pg_mash_dereplicator_index(NULL) is NULL; pg_mash_dereplicator_free(NULL) is PG_OK.
+ *   - Synchronisation: an add synchronises, once each to read the batch's sortedness for the query, to plan the
+ *     batch's pass, to read how many new representatives there are, and in the index add; so first and n_new_reps
+ *     are host pointers in _dev too.  _dev reads d_sketches and writes d_rep on `stream`, where it does its work.
+ *   - Threads: adds on one dereplicator are serialised by its own lock, and reps waits for a running add.  An add
+ *     holds the representative index's reader-writer lock exclusively from start to end, so a query on the
+ *     borrowed index sees it wholly before or wholly after an add.  The dereplicator lives on the device current
+ *     at creation.
+ *   - Device memory of an add, with R kept representatives and R' new ones: the m x R counts of the query (in row
+ *     blocks of at most 2 GiB), the batch's distance plan and its tile of <= 8 GiB, 4 m bytes of rep (PG_DEREP_NEAREST
+ *     adds 8 m bytes of keys), the gathered new rows (4 R' s bytes) and ids (4 (R + R') bytes), and the peak of
+ *     pg_mash_index_add for R' rows; the host call adds 4 m s bytes, the batch staged on the device. */
+typedef struct pg_mash_dereplicator pg_mash_dereplicator;
+int pg_mash_dereplicator_create(int32_t s, uint32_t min_same, uint32_t flags, pg_mash_dereplicator **out);
+int pg_mash_dereplicator_add(pg_mash_dereplicator *d, const uint32_t *sketches, uint64_t m, int32_t s,
+                             uint32_t *rep, uint64_t *first, uint64_t *n_new_reps);
+int pg_mash_dereplicator_add_dev(pg_mash_dereplicator *d, const uint32_t *d_sketches, uint64_t m, int32_t s,
+                                 uint32_t *d_rep, uint64_t *first, uint64_t *n_new_reps, void *stream);
+int pg_mash_dereplicator_reps(const pg_mash_dereplicator *d, uint32_t *ids, uint64_t cap, uint64_t *n_reps);
+const pg_mash_index *pg_mash_dereplicator_index(const pg_mash_dereplicator *d);
+int pg_mash_dereplicator_free(pg_mash_dereplicator *d);
+
 /* ---- align.SmithWaterman score -- search/align/align.go:171-203 -------------------
  * One template against n queries.  query_is_a != 0: stringA = query (outer loop),
  * stringB = template; else swapped.  lut_a/lut_b: byte -> index into the first /

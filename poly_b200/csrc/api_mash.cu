@@ -20,6 +20,16 @@ struct pg_mash_index {
     mutable std::shared_mutex rw;  // queries hold it shared while they read the plan and enqueue, an add exclusively
 };
 
+struct pg_mash_dereplicator {
+    int device;
+    int32_t s;
+    uint32_t min_same, flags;
+    pg_mash_index *ix;  // the kept representatives, in id order; callers borrow it for queries
+    uint32_t *d_ids;    // ix's reference p is sketch d_ids[p] (ascending), ix->plan.n entries
+    uint64_t n;         // sketches added so far: the next batch's first id
+    mutable std::mutex mu;  // serialises adds, and reps against them
+};
+
 namespace pg {
 namespace {
 
@@ -507,6 +517,55 @@ static int index_add_check(const pg_mash_index *ix, const void *sketches, uint64
     return PG_OK;
 }
 
+// The argument rules of pg_mash_dereplicator_add after the null dereplicator and m == 0, in their order
+static int derep_add_check(const pg_mash_dereplicator *d, const void *sketches, uint64_t m, int32_t s, const void *rep) {
+    if (s <= 0) { set_error("sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
+    if (s != d->s) { set_error("sketches of size %d added to a dereplication of size %d", s, d->s); return PG_ERR_ARG; }
+    if (m > 0xffffffffull - d->n) { set_error("%llu + %llu sketches exceed 2^32 - 1", (unsigned long long)d->n, (unsigned long long)m); return PG_ERR_ARG; }
+    if (!sketches || !rep) { set_error("null buffer"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+// One batch of m rows on the device (checked by the caller, who holds d->mu and d->ix->rw exclusively): the batch's
+// global assignments into d_rep (and, when rep is not NULL, copied to the host with the count's one sync), then
+// the new representatives appended to the representative index and to the ids.  The dereplicator takes the grown
+// index, ids and n only once everything has succeeded, so on an error it keeps what it held.
+static int derep_add(pg_mash_dereplicator *d, const uint32_t *d_b, uint64_t m, uint32_t *d_rep, uint32_t *rep, uint64_t *n_new,
+                     cudaStream_t st) {
+    const uint64_t R = d->ix->plan.n, s = (uint64_t)d->s;
+    const uint32_t base = (uint32_t)d->n;
+    StreamScratch tmp(st);
+    unsigned long long *d_cnt = nullptr;
+    PG_CUDA(tmp.alloc(&d_cnt, 1));
+    int rc = launch_mash_derep_add(d->ix->plan, d->d_ids, d_b, m, d->s, d->min_same, d->flags, base, d_rep, d_cnt, st);
+    if (rc != PG_OK) return rc;
+    unsigned long long cnt = 0;
+    PG_CUDA(cudaMemcpyAsync(&cnt, d_cnt, 8, cudaMemcpyDeviceToHost, st));
+    if (rep) PG_CUDA(cudaMemcpyAsync(rep, d_rep, m * 4, cudaMemcpyDeviceToHost, st));
+    PG_CUDA(cudaStreamSynchronize(st));
+    if (cnt) {
+        uint32_t *d_rows = nullptr, *d_ids = nullptr;
+        if (tmp.alloc(&d_rows, cnt * s) != cudaSuccess || cudaMallocAsync(&d_ids, (R + cnt) * 4, st) != cudaSuccess) {
+            cudaGetLastError();
+            set_error("cudaMallocAsync for %llu new representatives failed", cnt);
+            return PG_ERR_NOMEM;
+        }
+        cudaError_t e = R ? cudaMemcpyAsync(d_ids, d->d_ids, R * 4, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
+        rc = e == cudaSuccess ? launch_derep_gather(d_b, m, d->s, base, d_rep, cnt, d_rows, d_ids + R, st) : cuda_fail(e, "ids copy", __FILE__, __LINE__);
+        if (rc == PG_OK) rc = index_add(d->ix, d_rows, true, cnt, d->s, st);  // synchronises; takes the rows only on success
+        if (rc != PG_OK) {
+            cudaFreeAsync(d_ids, st);
+            cudaStreamSynchronize(st);
+            return rc;
+        }
+        if (d->d_ids) cudaFreeAsync(d->d_ids, st);
+        d->d_ids = d_ids;
+    }
+    d->n += m;
+    *n_new = cnt;
+    return PG_OK;
+}
+
 }  // namespace
 }  // namespace pg
 
@@ -989,6 +1048,90 @@ int pg_mash_index_free(pg_mash_index *ix) {
     delete ix;
     PG_CUDA(cudaStreamSynchronize(st));
     return PG_OK;
+}
+
+// ---------------------------------------------------------------------------------
+// Growing a dereplication
+// ---------------------------------------------------------------------------------
+int pg_mash_dereplicator_create(int32_t s, uint32_t min_same, uint32_t flags, pg_mash_dereplicator **out) {
+    if (!out) { set_error("null dereplicator pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = mash_derep_check(1, s, min_same, flags);  // the rules dereplicate applies to a non-empty set
+    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+    pg_mash_index *ix = nullptr;
+    if ((rc = index_create(nullptr, false, 0, s, cur_ctx()->slots[0].stream, &ix)) != PG_OK) return rc;
+    *out = new pg_mash_dereplicator{ix->device, s, min_same, flags, ix, nullptr, 0};
+    return PG_OK;
+}
+
+int pg_mash_dereplicator_add(pg_mash_dereplicator *d, const uint32_t *sketches, uint64_t m, int32_t s, uint32_t *rep, uint64_t *first,
+                             uint64_t *n_new_reps) {
+    if (!d) { set_error("null dereplicator"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(d->mu);
+    if (first) *first = d->n;
+    if (n_new_reps) *n_new_reps = 0;
+    if (m == 0) return PG_OK;
+    int rc = derep_add_check(d, sketches, m, s, rep);
+    if (rc != PG_OK || (rc = use_device(d->device)) != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> wl(d->ix->rw);  // before the device lock, as the index's own add takes them
+    HostCall c;
+    const uint32_t *d_b = c.upload(sketches, m * (uint64_t)s);
+    uint32_t *d_rep = c.alloc<uint32_t>(m);
+    uint64_t n_new = 0;
+    if ((rc = c.error()) || (rc = derep_add(d, d_b, m, d_rep, rep, &n_new, c.st)) || (rc = c.finish())) return rc;
+    if (n_new_reps) *n_new_reps = n_new;
+    return PG_OK;
+}
+
+int pg_mash_dereplicator_add_dev(pg_mash_dereplicator *d, const uint32_t *d_sketches, uint64_t m, int32_t s, uint32_t *d_rep,
+                                 uint64_t *first, uint64_t *n_new_reps, void *stream) {
+    if (!d) { set_error("null dereplicator"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(d->mu);
+    if (first) *first = d->n;
+    if (n_new_reps) *n_new_reps = 0;
+    if (m == 0) return PG_OK;
+    int rc = derep_add_check(d, d_sketches, m, s, d_rep);
+    if (rc != PG_OK || (rc = use_device(d->device)) != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> wl(d->ix->rw);
+    uint64_t n_new = 0;
+    if ((rc = derep_add(d, d_sketches, m, d_rep, nullptr, &n_new, (cudaStream_t)stream)) != PG_OK) return rc;
+    if (n_new_reps) *n_new_reps = n_new;
+    return PG_OK;
+}
+
+int pg_mash_dereplicator_reps(const pg_mash_dereplicator *d, uint32_t *ids, uint64_t cap, uint64_t *n_reps) {
+    if (!d) { set_error("null dereplicator"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(d->mu);
+    const uint64_t R = d->ix->plan.n;
+    if (n_reps) *n_reps = R;
+    if (cap && !ids) { set_error("null buffer"); return PG_ERR_ARG; }
+    if (const uint64_t k = std::min(cap, R)) {
+        int rc = use_device(d->device);
+        if (rc != PG_OK) return rc;
+        HostCall c;
+        c.download(ids, d->d_ids, k);
+        if ((rc = c.finish()) != PG_OK) return rc;
+    }
+    if (R > cap) { set_error("%llu representatives exceed cap %llu", (unsigned long long)R, (unsigned long long)cap); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+const pg_mash_index *pg_mash_dereplicator_index(const pg_mash_dereplicator *d) { return d ? d->ix : nullptr; }
+
+int pg_mash_dereplicator_free(pg_mash_dereplicator *d) {
+    if (!d) return PG_OK;
+    int rc = use_device(d->device);
+    if (rc != PG_OK) return rc;
+    if (d->d_ids) {
+        std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+        cudaStream_t st = cur_ctx()->slots[0].stream;
+        cudaFreeAsync(d->d_ids, st);
+        cudaStreamSynchronize(st);
+    }
+    rc = pg_mash_index_free(d->ix);
+    delete d;
+    return rc;
 }
 
 }  // extern "C"

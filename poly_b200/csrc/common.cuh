@@ -264,6 +264,23 @@ int launch_index_query(const DistancePlan &plan, const uint32_t *d_q, uint64_t n
 // Argument rules and their order are those of pg_mash_index_query_within_dev.
 int launch_index_within(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, uint64_t *d_off,
                         uint32_t *d_ref, uint32_t *d_same, double *d_dist, uint64_t cap, uint64_t *d_total, cudaStream_t st);
+// mash_index.cu: for each of nq query sketches of size sq > 0, the first reference of plan's set with same >= min_same
+// (min_same >= 1; the query is the receiver) as d_rep[q] = d_ids[p], or with `nearest` the one with the largest
+// same, ties to the first, as d_key[q] = same << 32 | ~d_ids[p].  d_ids ascends with p.  Rows that link to no
+// reference are written 0xFFFFFFFF / 0; nothing is written when the set is empty (the caller initialises).
+int launch_index_link(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, const uint32_t *d_ids,
+                      bool nearest, uint32_t *d_rep, unsigned long long *d_key, cudaStream_t st);
+// mash_derep.cu: one batch of a growing dereplication.  The m x s batch d_b takes ids base .. base + m - 1; plan
+// holds the kept representatives (ids d_ids, ascending) of the rows before it.  Rows linked to a kept
+// representative are seeded from it (launch_index_link), then the batch is dereplicated on its own with the seeded
+// rows covered: d_rep[i] = the global id of batch row i's representative (base + i for a new one), and
+// *d_n_new = the number of new representatives.  Argument checks are the caller's.
+int launch_mash_derep_add(const DistancePlan &plan, const uint32_t *d_ids, const uint32_t *d_b, uint64_t m, int s, uint32_t min_same,
+                          uint32_t flags, uint32_t base, uint32_t *d_rep, unsigned long long *d_n_new, cudaStream_t st);
+// mash_derep.cu: the n_new rows of the batch with d_rep[i] == base + i, in order: their sketches to d_rows
+// (n_new x s) and their ids to d_ids
+int launch_derep_gather(const uint32_t *d_b, uint64_t m, int s, uint32_t base, const uint32_t *d_rep, uint64_t n_new, uint32_t *d_rows,
+                        uint32_t *d_ids, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).
 struct AlignScoring;

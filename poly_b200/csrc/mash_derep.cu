@@ -18,10 +18,19 @@
 //                       both order-independent.  Columns inside the sub-block get their assignment here too.
 // derep_finish_kernel : after the last tile: rep[i] = i for representatives, keys to indices, the count.
 //
+// A growing dereplication (launch_mash_derep_add) runs the same kernels over one batch whose rows are numbered from
+// an id base: rows linked to a kept representative of the earlier batches are seeded first (launch_index_link
+// writes rep / key there), the walk reads them as covered, and the marks and the finish write global ids
+// base + r.  All comparisons stay in batch rows.  derep_gather_kernel then lists the batch's new
+// representatives, in order, for the representative index.
+//
 // A representative's slot is never written (the marks only reach sketches linked to an earlier representative),
 // so "slot still unset" is exactly "representative" and no separate flag array is kept.  Stream order makes every
 // earlier mark visible to the next walk; the output depends on the input alone.
 #include <algorithm>
+
+#include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
 
 #include "common.cuh"
 
@@ -98,11 +107,12 @@ derep_walk_kernel(const uint32_t *__restrict__ bits, uint64_t a, uint32_t b, con
 }
 
 // The listed representatives' tile rows (tile row 0 is sketch row0), columns j > r.  One CTA step covers
-// kMarkCols columns of one representative with 16-byte loads, four per thread in flight.
+// kMarkCols columns of one representative with 16-byte loads, four per thread in flight.  Marks carry the
+// representative's id base + r.
 template <bool Nearest>
 __global__ void __launch_bounds__(256)
 derep_mark_kernel(const uint32_t *__restrict__ tile, uint64_t n, uint64_t row0, uint32_t min_same, const uint32_t *__restrict__ list,
-                  uint32_t *rep, unsigned long long *key) {
+                  uint32_t base, uint32_t *rep, unsigned long long *key) {
     const uint64_t chunks = (n + kMarkCols - 1) / kMarkCols;
     const uint64_t items = (uint64_t)list[0] * chunks;
     const bool vec = (n & 3) == 0;  // rows are 16-byte aligned
@@ -122,8 +132,8 @@ derep_mark_kernel(const uint32_t *__restrict__ tile, uint64_t n, uint64_t row0, 
             for (int t = 0; t < 4; ++t) {
                 const uint64_t j = j0 + t;
                 if (v[q][t] < min_same || j <= r) continue;
-                if (Nearest) atomicMax(key + j, (unsigned long long)v[q][t] << 32 | (uint32_t)~r);
-                else atomicMin(rep + j, r);
+                if (Nearest) atomicMax(key + j, (unsigned long long)v[q][t] << 32 | (uint32_t)~(base + r));
+                else atomicMin(rep + j, base + r);
             }
         }
     }
@@ -131,7 +141,7 @@ derep_mark_kernel(const uint32_t *__restrict__ tile, uint64_t n, uint64_t row0, 
 
 template <bool Nearest>
 __global__ void __launch_bounds__(256)
-derep_finish_kernel(uint32_t *__restrict__ rep, const unsigned long long *__restrict__ key, uint64_t n,
+derep_finish_kernel(uint32_t *__restrict__ rep, const unsigned long long *__restrict__ key, uint64_t n, uint32_t base,
                     unsigned long long *__restrict__ n_reps) {
     const uint32_t lane = threadIdx.x & 31u;
     uint32_t reps = 0;
@@ -139,7 +149,7 @@ derep_finish_kernel(uint32_t *__restrict__ rep, const unsigned long long *__rest
         const uint64_t i = i0 + lane;
         if (i >= n) continue;
         const bool self = Nearest ? key[i] == 0 : rep[i] == kNone;
-        if (self) rep[i] = (uint32_t)i;
+        if (self) rep[i] = base + (uint32_t)i;
         else if (Nearest) rep[i] = ~(uint32_t)key[i];
         reps += self;
     }
@@ -148,7 +158,7 @@ derep_finish_kernel(uint32_t *__restrict__ rep, const unsigned long long *__rest
 }
 
 template <bool Nearest>
-int derep_tiles(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t *d_rep, unsigned long long *d_key,
+int derep_tiles(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t base, uint32_t *d_rep, unsigned long long *d_key,
                 unsigned long long *d_n_reps, StreamScratch &tmp, cudaStream_t st) {
     uint32_t *d_bits = nullptr, *d_list = nullptr;
     if (tmp.alloc(&d_bits, kDerepRows * kWords + 1 + kDerepRows) != cudaSuccess) {
@@ -169,13 +179,13 @@ int derep_tiles(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint
             PG_LAUNCH_CHECK("derep_links_kernel");
             derep_walk_kernel<Nearest><<<1, 1024, b * kWords * 4, st>>>(d_bits, a, b, d_rep, d_key, d_list);
             PG_LAUNCH_CHECK("derep_walk_kernel");
-            derep_mark_kernel<Nearest><<<grid, 256, 0, st>>>(tile, n, rb, min_same, d_list, d_rep, d_key);
+            derep_mark_kernel<Nearest><<<grid, 256, 0, st>>>(tile, n, rb, min_same, d_list, base, d_rep, d_key);
             PG_LAUNCH_CHECK("derep_mark_kernel");
         }
         return PG_OK;
     });
     if (rc != PG_OK) return rc;
-    derep_finish_kernel<Nearest><<<(unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(d_rep, d_key, n, d_n_reps);
+    derep_finish_kernel<Nearest><<<(unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(d_rep, d_key, n, base, d_n_reps);
     PG_LAUNCH_CHECK("derep_finish_kernel");
     return PG_OK;
 }
@@ -195,7 +205,7 @@ int launch_mash_derep(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same
     StreamScratch tmp(st);  // keys (nearest), the sub-block's link bits and list: freed on every way out
     if (!(flags & PG_DEREP_NEAREST)) {
         PG_CUDA(cudaMemsetAsync(d_rep, 0xff, n * 4, st));  // kNone: the assignment is built in place
-        return derep_tiles<false>(d_sk, n, s, min_same, d_rep, nullptr, d_n_reps, tmp, st);
+        return derep_tiles<false>(d_sk, n, s, min_same, 0, d_rep, nullptr, d_n_reps, tmp, st);
     }
     unsigned long long *d_key = nullptr;
     if (tmp.alloc(&d_key, n) != cudaSuccess) {
@@ -204,7 +214,83 @@ int launch_mash_derep(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same
         return PG_ERR_NOMEM;
     }
     PG_CUDA(cudaMemsetAsync(d_key, 0, n * 8, st));
-    return derep_tiles<true>(d_sk, n, s, min_same, d_rep, d_key, d_n_reps, tmp, st);
+    return derep_tiles<true>(d_sk, n, s, min_same, 0, d_rep, d_key, d_n_reps, tmp, st);
+}
+
+int launch_mash_derep_add(const DistancePlan &plan, const uint32_t *d_ids, const uint32_t *d_b, uint64_t m, int s, uint32_t min_same,
+                          uint32_t flags, uint32_t base, uint32_t *d_rep, unsigned long long *d_n_new, cudaStream_t st) {
+    PG_CUDA(cudaMemsetAsync(d_n_new, 0, 8, st));
+    StreamScratch tmp(st);
+    const bool nearest = flags & PG_DEREP_NEAREST;
+    unsigned long long *d_key = nullptr;
+    if (!nearest) {
+        PG_CUDA(cudaMemsetAsync(d_rep, 0xff, m * 4, st));  // kNone, then the seeds
+    } else {
+        if (tmp.alloc(&d_key, m) != cudaSuccess) {
+            cudaGetLastError();
+            set_error("cudaMallocAsync(%llu) for the dereplication keys failed", (unsigned long long)(m * 8));
+            return PG_ERR_NOMEM;
+        }
+        PG_CUDA(cudaMemsetAsync(d_key, 0, m * 8, st));
+    }
+    int rc = launch_index_link(plan, d_b, m, s, min_same, d_ids, nearest, d_rep, d_key, st);
+    if (rc != PG_OK) return rc;
+    return nearest ? derep_tiles<true>(d_b, m, s, min_same, base, d_rep, d_key, d_n_new, tmp, st)
+                   : derep_tiles<false>(d_b, m, s, min_same, base, d_rep, nullptr, d_n_new, tmp, st);
+}
+
+namespace {
+
+// Batch row i is a new representative iff its slot holds its own id
+struct IsNewRep {
+    const uint32_t *rep;
+    uint32_t base;
+    __device__ bool operator()(uint32_t i) const { return rep[i] == base + i; }
+};
+
+// Row p of the list: sel[p]'s sketch to rows[p], its id to ids[p].  One warp per row.
+__global__ void __launch_bounds__(256)
+derep_gather_kernel(const uint32_t *__restrict__ b, uint32_t s, const uint32_t *__restrict__ sel, uint64_t n_sel, uint32_t base,
+                    uint32_t *__restrict__ rows, uint32_t *__restrict__ ids) {
+    const uint32_t lane = threadIdx.x & 31u;
+    for (uint64_t p = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < n_sel; p += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
+        const uint32_t i = sel[p];
+        const uint32_t *src = b + (uint64_t)i * s;
+        uint32_t *dst = rows + p * s;
+        for (uint32_t w = lane; w < s; w += 32) dst[w] = src[w];
+        if (lane == 0) ids[p] = base + i;
+    }
+}
+
+}  // namespace
+
+int launch_derep_gather(const uint32_t *d_b, uint64_t m, int s, uint32_t base, const uint32_t *d_rep, uint64_t n_new, uint32_t *d_rows,
+                        uint32_t *d_ids, cudaStream_t st) {
+    if (n_new == 0) return PG_OK;
+    StreamScratch tmp(st);
+    uint32_t *d_sel = nullptr;
+    unsigned long long *d_n_sel = nullptr;
+    if (tmp.alloc(&d_sel, n_new) != cudaSuccess || tmp.alloc(&d_n_sel, 1) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("cudaMallocAsync for the new representatives failed");
+        return PG_ERR_NOMEM;
+    }
+    // an order-preserving compaction of the batch rows: no atomic decides a position
+    const thrust::counting_iterator<uint32_t> rows(0);
+    const IsNewRep pred{d_rep, base};
+    size_t bytes = 0;
+    PG_CUDA(cub::DeviceSelect::If(nullptr, bytes, rows, d_sel, d_n_sel, (int64_t)m, pred, st));
+    uint8_t *d_tmp = nullptr;
+    if (tmp.alloc(&d_tmp, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("cudaMallocAsync(%zu) for the selection failed", bytes);
+        return PG_ERR_NOMEM;
+    }
+    PG_CUDA(cub::DeviceSelect::If(d_tmp, bytes, rows, d_sel, d_n_sel, (int64_t)m, pred, st));
+    const unsigned grid = (unsigned)std::min<uint64_t>((n_new + 7) / 8, (uint64_t)sm_count() * 16);
+    derep_gather_kernel<<<grid, 256, 0, st>>>(d_b, (uint32_t)s, d_sel, n_new, base, d_rows, d_ids);
+    PG_LAUNCH_CHECK("derep_gather_kernel");
+    return PG_OK;
 }
 
 }  // namespace pg

@@ -17,6 +17,9 @@
 //   index_within_count_kernel  one CTA per row: the number of counts >= min_same, scanned in place into the
 //                              CSR offsets (the entry before the block already holds the earlier blocks' total);
 //   index_within_fill_kernel   one CTA per row: an index-ordered compaction of the row into its CSR slice.
+// A growing dereplication (launch_index_link) seeds a batch from its kept representatives with a third:
+//   index_link_kernel<Nearest> one CTA per row: the first reference (or the closest, ties to the first) with
+//                              same >= min_same, written as the row's assignment or nearest key.
 #include <algorithm>
 #include <cstdlib>
 
@@ -338,6 +341,41 @@ index_within_fill_kernel(const uint32_t *__restrict__ acc, uint64_t n, uint64_t 
     }
 }
 
+// One CTA per query row: the best reference with same >= min_same as a 64-bit key, larger is better.  First
+// mode: 1 << 32 | ~p, so the smallest position p wins, and the scan stops after the first chunk that holds one;
+// nearest: same << 32 | ~p, the largest count and then the smallest position.  ids[p] is position p's id and
+// ascends with p, so position order is id order.  Row `row` gets rep[row] = ids[p] (first; 0xFFFFFFFF when
+// nothing links) or key[row] = same << 32 | ~ids[p] (nearest; 0 when nothing links): the slots derep_walk_kernel
+// reads as "covered by an earlier representative".
+template <bool Nearest>
+__global__ void __launch_bounds__(SEL_THREADS)
+index_link_kernel(const uint32_t *__restrict__ acc, uint64_t n, uint64_t row0, uint32_t min_same, const uint32_t *__restrict__ ids,
+                  uint32_t *__restrict__ rep, unsigned long long *__restrict__ key) {
+    __shared__ unsigned long long s_part[SEL_THREADS / 32];
+    const uint32_t *A = acc + (uint64_t)blockIdx.x * n;
+    const uint64_t row = row0 + blockIdx.x;
+    const bool vec = (n & 3) == 0;
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    unsigned long long best = 0;  // min_same >= 1: the zeros load_count_quad returns past n never count
+    for (uint64_t j0 = 0; j0 < n; j0 += 4ull * SEL_THREADS) {
+        const uint64_t j = j0 + 4ull * threadIdx.x;
+        uint32_t v[4];
+        load_count_quad(A, j, n, vec, v);
+#pragma unroll
+        for (int t = 0; t < 4; ++t)
+            if (v[t] >= min_same) best = max(best, (unsigned long long)(Nearest ? v[t] : 1u) << 32 | (uint32_t)~(j + t));
+        if (!Nearest && __syncthreads_or(best != 0)) break;  // the loop bounds are the same in every thread
+    }
+    for (int d = 16; d > 0; d >>= 1) best = max(best, (unsigned long long)__shfl_xor_sync(0xffffffffu, best, d));
+    if (lane == 0) s_part[warp] = best;
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    for (int w = 0; w < SEL_THREADS / 32; ++w) best = max(best, s_part[w]);
+    const uint32_t id = best ? ids[~(uint32_t)best] : NO_REF;
+    if (Nearest) key[row] = best ? (best & ~0xffffffffull) | (uint32_t)~id : 0ull;
+    else rep[row] = id;
+}
+
 // The accumulation loop of both query kinds (nq > 0, sq > 0): the queries' sortedness (the one host sync), the
 // probe / pairwise choice, and row blocks whose dense [rows][n] counts fit a 2 GiB budget.  consume(acc, rb, re)
 // runs once the counts of rows [rb, re) are enqueued into acc; the first code other than PG_OK is the result.
@@ -461,6 +499,22 @@ int launch_index_within(const DistancePlan &plan, const uint32_t *d_q, uint64_t 
     if (rc != PG_OK) return rc;
     if (d_total) PG_CUDA(cudaMemcpyAsync(d_total, d_off + nq, 8, cudaMemcpyDeviceToDevice, st));
     return PG_OK;
+}
+
+int launch_index_link(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, const uint32_t *d_ids,
+                      bool nearest, uint32_t *d_rep, unsigned long long *d_key, cudaStream_t st) {
+    if (nq == 0 || plan.n == 0) return PG_OK;
+    const uint64_t n = plan.n;
+    return index_blocks(plan, d_q, nq, sq, st, [&](const uint32_t *d_acc, uint64_t rb, uint64_t re) {
+        if (nearest) {
+            index_link_kernel<true><<<(unsigned)(re - rb), SEL_THREADS, 0, st>>>(d_acc, n, rb, min_same, d_ids, d_rep, d_key);
+            PG_LAUNCH_CHECK("index_link_kernel<true>");
+        } else {
+            index_link_kernel<false><<<(unsigned)(re - rb), SEL_THREADS, 0, st>>>(d_acc, n, rb, min_same, d_ids, d_rep, d_key);
+            PG_LAUNCH_CHECK("index_link_kernel<false>");
+        }
+        return PG_OK;
+    });
 }
 
 }  // namespace pg

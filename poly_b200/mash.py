@@ -12,6 +12,7 @@ path here beyond marshalling.
 from __future__ import annotations
 
 import ctypes as C
+import threading
 from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -541,6 +542,141 @@ def dereplicate(sketches, min_same: Optional[int] = None, max_distance: Optional
     nr = C.c_uint64(0)
     _index_rc(_lib.lib().pg_mash_dereplicate(rows.ctypes.data, n, s, min_same, flags, rep.ctypes.data, C.byref(nr)))
     return rep, int(nr.value)
+
+
+class _RepresentativeIndex(SketchIndex):
+    """The representative index a Dereplicator owns, borrowed for queries: it is grown only by the
+    dereplicator's adds and released with it."""
+
+    def __init__(self, h, s: int):
+        self._h = h
+        self._dev_queried = None
+        self.n, self.s = 0, s
+
+    def add(self, sketches) -> int:
+        raise ValueError("the representative index grows only through Dereplicator.add")
+
+    def close(self) -> None:
+        if self._h is not None and self._dev_queried is not None:
+            import torch
+
+            torch.cuda.synchronize(self._dev_queried)
+        self._h = None
+
+
+class Dereplicator:
+    """A dereplication that grows: each add assigns a new batch of sketches against the representatives kept so
+    far, on the device, without dereplicating the earlier sketches again.  Sketches are numbered in the order they
+    are added.  After any sequence of adds, the concatenated assignments equal dereplicate() of the concatenated
+    batches, with the same min_same / max_distance and nearest.
+
+    s: the sketch size of every batch.  A max_distance under which every pair links, or none can, is a ValueError.
+    The representatives are kept in a SketchIndex over them: nearest and within query it and give sketch ids."""
+
+    def __init__(self, s: int, min_same: Optional[int] = None, max_distance: Optional[float] = None, nearest: bool = False):
+        if (min_same is None) == (max_distance is None):
+            raise ValueError("give exactly one of min_same and max_distance")
+        s = int(s)
+        if max_distance is not None and s > 0:  # s <= 0: the library reports the reference's panic
+            min_same = min_same_for_distance(max_distance, s)
+            if min_same == 0:
+                raise ValueError(f"max_distance {max_distance!r} links every pair: every Distance is <= it")
+            if min_same == s + 1:
+                raise ValueError(f"max_distance {max_distance!r} links no pair: no Distance is <= it")
+        min_same = 1 if min_same is None else int(min_same)
+        if not 0 <= min_same <= 0xFFFFFFFF:
+            raise ValueError("min_same must fit 32 bits")
+        h = C.c_void_p()
+        _index_rc(_lib.lib().pg_mash_dereplicator_create(s, min_same, PG_DEREP_NEAREST if nearest else 0, C.byref(h)))
+        self._h = h
+        self._ix = _RepresentativeIndex(C.c_void_p(_lib.lib().pg_mash_dereplicator_index(h)), s)
+        self._lock = threading.Lock()
+        self.s, self.min_same, self.nearest_mode = s, min_same, bool(nearest)
+        self.n = 0
+
+    def add(self, sketches):
+        """Assigns a batch (what dereplicate takes): returns (rep [m] uint32, n_new_reps), rep holding global ids, so
+        row i of the batch is sketch first + i.  CUDA tensors give a CUDA int32 tensor (carrying the uint32 bits),
+        ordered on the current stream; the call itself synchronises."""
+        if self._h is None:
+            raise ValueError("the dereplicator is closed")
+        rows = _sketch_rows(sketches)
+        m, s = int(rows.shape[0]), int(rows.shape[1])
+        first, n_new = C.c_uint64(0), C.c_uint64(0)
+        if self._ix._dev_queried is not None:  # the add releases buffers that device queries, on any stream, may still read
+            import torch
+
+            torch.cuda.synchronize(self._ix._dev_queried)
+        if hasattr(rows, "data_ptr"):
+            import torch
+
+            rep = torch.empty(m, dtype=torch.int32, device=rows.device)
+            rc = _lib.lib().pg_mash_dereplicator_add_dev(self._h, rows.data_ptr(), m, s, rep.data_ptr(), C.byref(first), C.byref(n_new),
+                                                         torch.cuda.current_stream(rows.device).cuda_stream)
+        else:
+            rep = np.empty(m, dtype=np.uint32)
+            rc = _lib.lib().pg_mash_dereplicator_add(self._h, rows.ctypes.data, m, s, rep.ctypes.data, C.byref(first), C.byref(n_new))
+        _index_rc(rc)
+        with self._lock:
+            self.n = max(self.n, int(first.value) + m)
+            self._ix.n += int(n_new.value)
+        return rep, int(n_new.value)
+
+    def representatives(self) -> np.ndarray:
+        """The ids of the representatives kept so far, ascending: position p of the representative index is
+        sketch representatives()[p]."""
+        if self._h is None:
+            raise ValueError("the dereplicator is closed")
+        cnt = C.c_uint64(0)
+        cap = self._ix.n
+        while True:
+            ids = np.empty(max(cap, 1), dtype=np.uint32)
+            rc = _lib.lib().pg_mash_dereplicator_reps(self._h, ids.ctypes.data, cap, C.byref(cnt))
+            if rc == _lib.PG_ERR_ARG and cnt.value > cap:  # an add on another thread kept more
+                cap = int(cnt.value)
+                continue
+            _lib.check(rc)
+            return ids[: int(cnt.value)]
+
+    def _ids_of(self, ref, ids):
+        """Positions of the representative index -> sketch ids; the NO_REF slots stay as they are."""
+        if len(ids) == 0:  # no representative: every slot is NO_REF
+            return ref
+        if hasattr(ref, "data_ptr"):
+            import torch
+
+            t = torch.from_numpy(ids.view(np.int32)).to(ref.device)
+            return torch.where(ref == -1, ref, t[ref.clamp(min=0).long()])
+        return np.where(ref == NO_REF, ref, ids[np.where(ref == NO_REF, 0, ref)]).astype(np.uint32)
+
+    def nearest(self, queries, k: int, min_same: Optional[int] = None, max_distance: Optional[float] = None):
+        """SketchIndex.nearest over the representatives, with every hit given as its sketch id."""
+        ref, same, dist, nh = self._ix.nearest(queries, k, min_same=min_same, max_distance=max_distance)
+        return self._ids_of(ref, self.representatives()), same, dist, nh
+
+    def within(self, queries, min_same: Optional[int] = None, max_distance: Optional[float] = None):
+        """SketchIndex.within over the representatives, with every hit given as its sketch id."""
+        off, ref, same, dist = self._ix.within(queries, min_same=min_same, max_distance=max_distance)
+        return off, self._ids_of(ref, self.representatives()), same, dist
+
+    def close(self) -> None:
+        if self._h is not None:
+            self._ix.close()
+            h, self._h = self._h, None
+            _lib.check(_lib.lib().pg_mash_dereplicator_free(h))
+
+    def __enter__(self) -> "Dereplicator":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        if getattr(self, "_h", None) is not None:
+            try:
+                self.close()
+            except Exception:
+                pass
 
 
 # ---- single-process multi-GPU additions (pg_*_multi; SURVEY.md 8b / 8e) ----------------------------
