@@ -737,6 +737,64 @@ func (d *Dereplicator) Close() error {
 	return locked(func() C.int { return C.pg_mash_dereplicator_free(h) })
 }
 
+// Clusterer wraps a pg_mash_clusterer: a single-linkage clustering that grows batch by batch on the device of the
+// calling thread.  Adds from several goroutines are serialised by the library.  Close must not run while an Add
+// is in flight.
+type Clusterer struct {
+	h *C.pg_mash_clusterer
+}
+
+// NewClusterer wraps pg_mash_clusterer_create for sketches of s words at same >= minSame.
+func NewClusterer(s, minSame int) (*Clusterer, error) {
+	var h *C.pg_mash_clusterer
+	if err := locked(func() C.int { return C.pg_mash_clusterer_create(C.int32_t(s), C.uint32_t(minSame), &h) }); err != nil {
+		return nil, err
+	}
+	return &Clusterer{h: h}, nil
+}
+
+// Add wraps pg_mash_clusterer_add: n sketches of s words each (full arrays, zero tails included) become sketches
+// first .. first + n - 1; label[i] is row i's label after the add, nGroups every group, nLinks the links this add
+// found and nMerged the earlier groups it absorbed into another.
+func (c *Clusterer) Add(sketches []uint32, n, s int) (label []uint32, first, nGroups, nLinks, nMerged uint64, err error) {
+	label = make([]uint32, n+1)
+	var p *C.uint32_t
+	if len(sketches) > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
+	}
+	var f, g, l, m C.uint64_t
+	err = locked(func() C.int {
+		return C.pg_mash_clusterer_add(c.h, p, C.uint64_t(n), C.int32_t(s), (*C.uint32_t)(unsafe.Pointer(&label[0])), &f, &g, &l, &m)
+	})
+	return label[:n], uint64(f), uint64(g), uint64(l), uint64(m), err
+}
+
+// Labels wraps pg_mash_clusterer_labels: the current labels of sketches [begin, end).
+func (c *Clusterer) Labels(begin, end int) ([]uint32, error) {
+	size := 0
+	if end > begin {
+		size = end - begin
+	}
+	out := make([]uint32, size+1)
+	err := locked(func() C.int {
+		return C.pg_mash_clusterer_labels(c.h, C.uint64_t(begin), C.uint64_t(end), (*C.uint32_t)(unsafe.Pointer(&out[0])))
+	})
+	if err != nil {
+		return nil, err
+	}
+	return out[:size], nil
+}
+
+// Close wraps pg_mash_clusterer_free.
+func (c *Clusterer) Close() error {
+	if c.h == nil {
+		return nil
+	}
+	h := c.h
+	c.h = nil
+	return locked(func() C.int { return C.pg_mash_clusterer_free(h) })
+}
+
 // SeqhashBatch wraps pg_seqhash_batch: digest[32*i:32*i+32], errCode[i] and errPos[i] for each of the
 // sequences bases[offsets[i]:offsets[i+1]], all of one seqType (0 DNA, 1 RNA, 2 PROTEIN) and flags
 // (1 circular | 2 double-stranded).

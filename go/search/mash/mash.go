@@ -302,6 +302,94 @@ func (d *Dereplicator) Reps() ([]int, error) {
 // Close releases the dereplicator's device memory.
 func (d *Dereplicator) Close() error { return d.d.Close() }
 
+// Clusterer is a clustering that grows: each Add merges a batch of sketches into the single-linkage groups of the
+// sketches added so far, on the GPU, without clustering the earlier sketches again.  Sketches are numbered in the
+// order they are added, and after every add Labels equals Cluster of the concatenated batches.  Earlier labels
+// change when a batch joins two earlier groups (Merged > 0).  Safe for concurrent use; call Close when done.
+type Clusterer struct {
+	c  *polyb200.Clusterer
+	s  int
+	mu sync.Mutex
+	n  int
+}
+
+// ClusterBatch is the result of one Add.
+type ClusterBatch struct {
+	Labels []int // the label of each batch sketch after the add; batch[i] is sketch First + i
+	First  int
+	Groups int   // every group after the add
+	Links  int   // the links this add found
+	Merged int   // earlier groups absorbed into another by this add; 0 means no earlier label changed
+}
+
+// NewClusterer prepares a clustering of sketches of SketchSize s at Distance <= maxDistance, with the links of
+// Cluster.  A maxDistance that every pair satisfies, or none can, is an error.
+func NewClusterer(s int, maxDistance float64) (*Clusterer, error) {
+	if s <= 0 {
+		panic("runtime error: index out of range [-1]") // Similarity on a sketch of size 0 would
+	}
+	minSame := 0
+	for minSame <= s && !(1-float64(minSame)/float64(s) <= maxDistance) {
+		minSame++
+	}
+	if minSame == 0 || minSame > s {
+		return nil, fmt.Errorf("mash: maxDistance %v links every pair or none", maxDistance)
+	}
+	c, err := polyb200.NewClusterer(s, minSame)
+	if err != nil {
+		return nil, err
+	}
+	return &Clusterer{c: c, s: s}, nil
+}
+
+// Add merges a batch of sketches of the clusterer's SketchSize.
+func (c *Clusterer) Add(sketches []*Mash) (ClusterBatch, error) {
+	flat := make([]uint32, 0, len(sketches)*c.s)
+	for _, m := range sketches {
+		if m.SketchSize != c.s {
+			return ClusterBatch{}, errors.New("mash: Clusterer needs one common SketchSize")
+		}
+		flat = append(flat, m.Sketches[:c.s]...)
+	}
+	label, first, groups, links, merged, err := c.c.Add(flat, len(sketches), c.s)
+	if err != nil {
+		return ClusterBatch{}, err
+	}
+	out := ClusterBatch{Labels: make([]int, len(label)), First: int(first), Groups: int(groups), Links: int(links), Merged: int(merged)}
+	for i, x := range label {
+		out.Labels[i] = int(x)
+	}
+	c.mu.Lock()
+	if end := out.First + len(label); end > c.n {
+		c.n = end
+	}
+	c.mu.Unlock()
+	return out, nil
+}
+
+// N returns the number of sketches added through Add so far.
+func (c *Clusterer) N() int {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	return c.n
+}
+
+// Labels returns the current labels of sketches [begin, end).
+func (c *Clusterer) Labels(begin, end int) ([]int, error) {
+	ids, err := c.c.Labels(begin, end)
+	if err != nil {
+		return nil, err
+	}
+	out := make([]int, len(ids))
+	for i, x := range ids {
+		out[i] = int(x)
+	}
+	return out, nil
+}
+
+// Close releases the clusterer's device memory.
+func (c *Clusterer) Close() error { return c.c.Close() }
+
 // Neighbor is one reference of a Nearest result.
 type Neighbor struct {
 	Index    int     // position in the reference list given to NewIndex

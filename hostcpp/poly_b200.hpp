@@ -482,6 +482,47 @@ public:
     }
 };
 
+// A growing clustering: each Add merges a batch into the single-linkage groups of the sketches added so far, on
+// the device.  Sketches are numbered in the order they are added; after every Add, Labels() equals Cluster of the
+// concatenated batches, and the Links of the Adds sum to its Links.  Earlier labels change when a batch joins two
+// earlier groups (Merged > 0).
+class Clusterer {
+    pg_mash_clusterer *h_ = nullptr;
+
+public:
+    Clusterer(int sketchSize, uint32_t minSame) {
+        int rc = pg_mash_clusterer_create(sketchSize, minSame, &h_);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+    }
+    Clusterer(const Clusterer &) = delete;
+    Clusterer &operator=(const Clusterer &) = delete;
+    ~Clusterer() { pg_mash_clusterer_free(h_); }
+    // Labels = the batch rows' labels (global ids) after the add; Groups = every group after it; Links = the
+    // links this add found; Merged = the earlier groups it absorbed into another
+    struct Batch {
+        std::vector<uint32_t> Labels;
+        uint64_t First = 0, Groups = 0, Links = 0, Merged = 0;
+    };
+    Batch Add(const std::vector<Mash> &mashes) {
+        int s;
+        const std::vector<uint32_t> flat = detail::FlatRows(mashes, "sketches", &s);
+        Batch out;
+        out.Labels.resize(mashes.size());
+        int rc = pg_mash_clusterer_add(h_, flat.data(), mashes.size(), s, out.Labels.data(), &out.First, &out.Groups, &out.Links,
+                                       &out.Merged);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+        return out;
+    }
+    // the current labels of sketches [begin, end)
+    std::vector<uint32_t> Labels(uint64_t begin, uint64_t end) const {
+        std::vector<uint32_t> out(end > begin ? end - begin : 0);
+        check(pg_mash_clusterer_labels(h_, begin, end, out.data()));
+        return out;
+    }
+};
+
 }  // namespace mash
 
 namespace align {

@@ -460,6 +460,65 @@ int pg_mash_dereplicator_reps(const pg_mash_dereplicator *d, uint32_t *ids, uint
 const pg_mash_index *pg_mash_dereplicator_index(const pg_mash_dereplicator *d);
 int pg_mash_dereplicator_free(pg_mash_dereplicator *d);
 
+/* ---- cluster: growing a clustering -------------------------------------------------------------------
+ * A clusterer keeps an index over every sketch added so far and their single-linkage labels, and merges each new
+ * batch into the groups on the device, so a growing collection is never clustered from scratch.  Sketches are
+ * numbered in the order they are added: the rows of a batch are ids first .. first + m - 1 (m x s full Go arrays,
+ * as pg_mash_cluster takes them).  The batch is copied; no caller pointer is retained.
+ *   - Invariant: split a set S of sketches of one size into B0, B1, ..., Bk and call add(B0) ... add(Bk).  After
+ *     the add of Bj, labels(0, n) equals the labels of pg_mash_cluster(B0 .. Bj, min_same) and *n_groups its
+ *     group count; the add's label output is the slice [first, first + m) of those labels, and the *n_links of
+ *     the adds sum to its n_links.  This holds for any split, empty and one-row batches included.  Labels are
+ *     global ids.
+ *   - Why it is exact: single linkage is union-find over the links, so the components of B0 .. Bj are those of
+ *     B0 .. Bj-1 united with every link between a row of Bj and any earlier sketch and every link inside Bj.  The
+ *     first come from a query of Bj against the index of all earlier sketches (the batch row is the receiver;
+ *     for one sketch size the count is symmetric, so it is the cluster count, unsorted sketches included), the
+ *     second from the cluster pass over Bj alone (the lower row is the receiver).  Labels are the smallest id of
+ *     each group, which the input alone decides.
+ *   - Earlier labels can change: a batch row that links two earlier groups joins them, and the larger label is
+ *     retired.  *n_merged is the number of earlier groups absorbed into another by this add (roots r < first
+ *     whose label changed); 0 says no earlier label changed.  *n_links counts this add's links, cross and inner.
+ *   - Link rule, count and cut: those of pg_mash_cluster.
+ *   - Errors.  create checks, in this order: a null out is PG_ERR_ARG; s <= 0 is PG_ERR_PANIC (the rule cluster
+ *     applies to a non-empty set); min_same == 0 or min_same > s is PG_ERR_ARG.  add (host and _dev) checks, in
+ *     this order: a null clusterer is PG_ERR_ARG (no device is needed); m == 0 is valid and changes nothing
+ *     (*first = n, *n_groups = the current count, *n_links = *n_merged = 0); s <= 0 is PG_ERR_PANIC; an s other
+ *     than the clusterer's is PG_ERR_ARG; n + m > 2^32 - 1 is PG_ERR_ARG, checked before any buffer is read; a
+ *     null sketches buffer is PG_ERR_ARG.  PG_ERR_UNSUPPORTED and PG_ERR_NOMEM arise where the index query, the
+ *     cluster pass over the batch or the index add raise them.  After any error the clusterer's labels, index
+ *     and counts are exactly what they were; only the caller's label contents are then unspecified.  label and
+ *     every count pointer may be NULL.  labels: begin > end, end > n, or a null buffer with end > begin is
+ *     PG_ERR_ARG.
+ *   - The index: pg_mash_clusterer_index returns a borrowed, read-only pg_mash_index whose reference p is sketch
+ *     p, so "which group would this new sketch join" is a top-k or radius query followed by a labels read.  The
+ *     handle is valid until pg_mash_clusterer_free and must not be passed to pg_mash_index_add or
+ *     pg_mash_index_free.  pg_mash_clusterer_index(NULL) is NULL; pg_mash_clusterer_free(NULL) is PG_OK.
+ *   - Synchronisation: an add synchronises, to read the batch's sortedness for the query, to plan the batch's
+ *     pass, to read the counts, and in the index add; so the counts are host pointers in _dev too.  _dev reads
+ *     d_sketches and writes d_label on `stream`, where it does its work.  labels_dev copies on `stream` and does
+ *     not wait.  Enqueuing labels_dev or a _dev query on the borrowed index and then adding or freeing before
+ *     that stream is synchronised is the caller's error, as for the index.
+ *   - Threads: adds on one clusterer are serialised by its own lock, and label reads wait for a running add.  An
+ *     add holds the index's reader-writer lock exclusively from start to end (taken before the device lock), so
+ *     a query on the borrowed index sees it wholly before or wholly after an add.  The clusterer lives on the
+ *     device current at creation.
+ *   - Device memory of an add, with n sketches held: the m x n counts of the query (in row blocks of at most
+ *     2 GiB), the batch's distance plan and its tile of <= 8 GiB, the forest of the n + m sketches and their new
+ *     labels (4 (n + m) bytes each) while the old 4 n bytes of labels are held, and the peak of pg_mash_index_add
+ *     for m rows; the host call adds 4 m s bytes, the batch staged on the device.  The index holds 4 n s bytes of
+ *     sketches and its join at 8 bytes per entry: at 100 000 sketches of s = 2000, 0.8 GB and about 1.6 GB. */
+typedef struct pg_mash_clusterer pg_mash_clusterer;
+int pg_mash_clusterer_create(int32_t s, uint32_t min_same, pg_mash_clusterer **out);
+int pg_mash_clusterer_add(pg_mash_clusterer *c, const uint32_t *sketches, uint64_t m, int32_t s, uint32_t *label, uint64_t *first,
+                          uint64_t *n_groups, uint64_t *n_links, uint64_t *n_merged);
+int pg_mash_clusterer_add_dev(pg_mash_clusterer *c, const uint32_t *d_sketches, uint64_t m, int32_t s, uint32_t *d_label,
+                              uint64_t *first, uint64_t *n_groups, uint64_t *n_links, uint64_t *n_merged, void *stream);
+int pg_mash_clusterer_labels(const pg_mash_clusterer *c, uint64_t begin, uint64_t end, uint32_t *label);
+int pg_mash_clusterer_labels_dev(const pg_mash_clusterer *c, uint64_t begin, uint64_t end, uint32_t *d_label, void *stream);
+const pg_mash_index *pg_mash_clusterer_index(const pg_mash_clusterer *c);
+int pg_mash_clusterer_free(pg_mash_clusterer *c);
+
 /* ---- align.SmithWaterman score -- search/align/align.go:171-203 -------------------
  * One template against n queries.  query_is_a != 0: stringA = query (outer loop),
  * stringB = template; else swapped.  lut_a/lut_b: byte -> index into the first /

@@ -30,6 +30,16 @@ struct pg_mash_dereplicator {
     mutable std::mutex mu;  // serialises adds, and reps against them
 };
 
+struct pg_mash_clusterer {
+    int device;
+    int32_t s;
+    uint32_t min_same;
+    pg_mash_index *ix;      // every sketch added, in id order; callers borrow it for queries
+    uint32_t *d_label;      // label[i] = the smallest id of sketch i's group, ix->plan.n entries
+    uint64_t n, n_groups;   // sketches added so far (the next batch's first id) and their groups
+    mutable std::mutex mu;  // serialises adds, and label reads against them
+};
+
 namespace pg {
 namespace {
 
@@ -563,6 +573,46 @@ static int derep_add(pg_mash_dereplicator *d, const uint32_t *d_b, uint64_t m, u
     }
     d->n += m;
     *n_new = cnt;
+    return PG_OK;
+}
+
+// The argument rules of pg_mash_clusterer_add after the null clusterer and m == 0, in their order
+static int cluster_add_check(const pg_mash_clusterer *c, const void *sketches, uint64_t m, int32_t s) {
+    if (s <= 0) { set_error("sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
+    if (s != c->s) { set_error("sketches of size %d added to a clustering of size %d", s, c->s); return PG_ERR_ARG; }
+    if (m > 0xffffffffull - c->n) { set_error("%llu + %llu sketches exceed 2^32 - 1", (unsigned long long)c->n, (unsigned long long)m); return PG_ERR_ARG; }
+    if (!sketches) { set_error("null buffer"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+// One batch of m rows on the device (checked by the caller, who holds c->mu and c->ix->rw exclusively): the labels
+// of all n + m sketches into a new array, the batch's slice of them into d_out or out (either may be NULL), the
+// counts into cnt (links, groups, merged), then the batch appended to the index.  The clusterer takes the new
+// labels, n and the group count only once everything has succeeded, so on an error it keeps what it held.
+static int cluster_add(pg_mash_clusterer *c, const uint32_t *d_b, uint64_t m, uint32_t *d_out, uint32_t *out, unsigned long long cnt[3],
+                       cudaStream_t st) {
+    const uint64_t n = c->n;
+    StreamScratch tmp(st), keep(st);  // keep: the new labels, released unless the add succeeds
+    unsigned long long *d_cnt = nullptr;
+    uint32_t *d_label = nullptr;
+    PG_CUDA(tmp.alloc(&d_cnt, 3));
+    if (keep.alloc(&d_label, n + m) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("cudaMallocAsync(%llu) for the labels failed", (unsigned long long)((n + m) * 4));
+        return PG_ERR_NOMEM;
+    }
+    int rc = launch_mash_cluster_add(c->ix->plan, c->d_label, d_b, m, c->s, c->min_same, d_label, d_cnt, st);
+    if (rc != PG_OK) return rc;
+    PG_CUDA(cudaMemcpyAsync(cnt, d_cnt, 24, cudaMemcpyDeviceToHost, st));
+    if (out) PG_CUDA(cudaMemcpyAsync(out, d_label + n, m * 4, cudaMemcpyDeviceToHost, st));
+    if (d_out) PG_CUDA(cudaMemcpyAsync(d_out, d_label + n, m * 4, cudaMemcpyDeviceToDevice, st));
+    PG_CUDA(cudaStreamSynchronize(st));
+    if ((rc = index_add(c->ix, d_b, true, m, c->s, st)) != PG_OK) return rc;  // synchronises; takes the rows only on success
+    keep.ptr.clear();
+    if (c->d_label) cudaFreeAsync(c->d_label, st);
+    c->d_label = d_label;
+    c->n = n + m;
+    c->n_groups = cnt[1];
     return PG_OK;
 }
 
@@ -1131,6 +1181,110 @@ int pg_mash_dereplicator_free(pg_mash_dereplicator *d) {
     }
     rc = pg_mash_index_free(d->ix);
     delete d;
+    return rc;
+}
+
+// ---------------------------------------------------------------------------------
+// Growing a clustering
+// ---------------------------------------------------------------------------------
+int pg_mash_clusterer_create(int32_t s, uint32_t min_same, pg_mash_clusterer **out) {
+    if (!out) { set_error("null clusterer pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = mash_cluster_check(1, s, min_same);  // the rules cluster applies to a non-empty set
+    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+    pg_mash_index *ix = nullptr;
+    if ((rc = index_create(nullptr, false, 0, s, cur_ctx()->slots[0].stream, &ix)) != PG_OK) return rc;
+    *out = new pg_mash_clusterer{ix->device, s, min_same, ix, nullptr, 0, 0};
+    return PG_OK;
+}
+
+// The per-add outputs before any work: what an empty batch or an error reports
+static void cluster_add_outputs(const pg_mash_clusterer *c, uint64_t *first, uint64_t *n_groups, uint64_t *n_links, uint64_t *n_merged) {
+    if (first) *first = c->n;
+    if (n_groups) *n_groups = c->n_groups;
+    if (n_links) *n_links = 0;
+    if (n_merged) *n_merged = 0;
+}
+
+int pg_mash_clusterer_add(pg_mash_clusterer *c, const uint32_t *sketches, uint64_t m, int32_t s, uint32_t *label, uint64_t *first,
+                          uint64_t *n_groups, uint64_t *n_links, uint64_t *n_merged) {
+    if (!c) { set_error("null clusterer"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    cluster_add_outputs(c, first, n_groups, n_links, n_merged);
+    if (m == 0) return PG_OK;
+    int rc = cluster_add_check(c, sketches, m, s);
+    if (rc != PG_OK || (rc = use_device(c->device)) != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> wl(c->ix->rw);  // before the device lock, as the index's own add takes them
+    HostCall hc;
+    const uint32_t *d_b = hc.upload(sketches, m * (uint64_t)s);
+    unsigned long long cnt[3] = {};
+    if ((rc = hc.error()) || (rc = cluster_add(c, d_b, m, nullptr, label, cnt, hc.st)) || (rc = hc.finish())) return rc;
+    if (n_links) *n_links = cnt[0];
+    if (n_groups) *n_groups = cnt[1];
+    if (n_merged) *n_merged = cnt[2];
+    return PG_OK;
+}
+
+int pg_mash_clusterer_add_dev(pg_mash_clusterer *c, const uint32_t *d_sketches, uint64_t m, int32_t s, uint32_t *d_label, uint64_t *first,
+                              uint64_t *n_groups, uint64_t *n_links, uint64_t *n_merged, void *stream) {
+    if (!c) { set_error("null clusterer"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    cluster_add_outputs(c, first, n_groups, n_links, n_merged);
+    if (m == 0) return PG_OK;
+    int rc = cluster_add_check(c, d_sketches, m, s);
+    if (rc != PG_OK || (rc = use_device(c->device)) != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> wl(c->ix->rw);
+    unsigned long long cnt[3] = {};
+    if ((rc = cluster_add(c, d_sketches, m, d_label, nullptr, cnt, (cudaStream_t)stream)) != PG_OK) return rc;
+    if (n_links) *n_links = cnt[0];
+    if (n_groups) *n_groups = cnt[1];
+    if (n_merged) *n_merged = cnt[2];
+    return PG_OK;
+}
+
+static int cluster_labels_check(const pg_mash_clusterer *c, uint64_t begin, uint64_t end, const void *label) {
+    if (begin > end || end > c->n) {
+        set_error("labels [%llu, %llu) outside the %llu sketches added", (unsigned long long)begin, (unsigned long long)end, (unsigned long long)c->n);
+        return PG_ERR_ARG;
+    }
+    if (end > begin && !label) { set_error("null buffer"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+int pg_mash_clusterer_labels(const pg_mash_clusterer *c, uint64_t begin, uint64_t end, uint32_t *label) {
+    if (!c) { set_error("null clusterer"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    int rc = cluster_labels_check(c, begin, end, label);
+    if (rc != PG_OK || end == begin || (rc = use_device(c->device)) != PG_OK) return rc;
+    HostCall hc;
+    hc.download(label, c->d_label + begin, end - begin);
+    return hc.finish();
+}
+
+int pg_mash_clusterer_labels_dev(const pg_mash_clusterer *c, uint64_t begin, uint64_t end, uint32_t *d_label, void *stream) {
+    if (!c) { set_error("null clusterer"); return PG_ERR_ARG; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    int rc = cluster_labels_check(c, begin, end, d_label);
+    if (rc != PG_OK || end == begin || (rc = use_device(c->device)) != PG_OK) return rc;
+    PG_CUDA(cudaMemcpyAsync(d_label, c->d_label + begin, (end - begin) * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return PG_OK;
+}
+
+const pg_mash_index *pg_mash_clusterer_index(const pg_mash_clusterer *c) { return c ? c->ix : nullptr; }
+
+int pg_mash_clusterer_free(pg_mash_clusterer *c) {
+    if (!c) return PG_OK;
+    int rc = use_device(c->device);
+    if (rc != PG_OK) return rc;
+    if (c->d_label) {
+        std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+        cudaStream_t st = cur_ctx()->slots[0].stream;
+        cudaFreeAsync(c->d_label, st);
+        cudaStreamSynchronize(st);
+    }
+    rc = pg_mash_index_free(c->ix);
+    delete c;
     return rc;
 }
 

@@ -246,6 +246,18 @@ __device__ __forceinline__ void load_count_quad(const uint32_t *p, uint64_t i, u
 int mash_cluster_check(uint64_t n, int s, uint32_t min_same);
 int launch_mash_cluster(const uint32_t *d_sk, uint64_t n, int s, uint32_t min_same, uint32_t *d_label,
                         unsigned long long *d_n_groups, unsigned long long *d_n_links, cudaStream_t st);
+// mash_cluster.cu: the one scan of a rows x n array of counts into the union-find forest d_parent: entry (t, j)
+// with count >= min_same (>= 1) unites sketches row0 + t and col0 + j and adds one to *d_n_links; with upper only
+// where col0 + j > row0 + t.
+int launch_cluster_link(const uint32_t *d_counts, uint64_t rows, uint64_t n, uint64_t row0, uint64_t col0, bool upper, uint32_t min_same,
+                        uint32_t *d_parent, unsigned long long *d_n_links, cudaStream_t st);
+// mash_cluster.cu: one batch of a growing clustering.  plan holds the n sketches before it, d_old their labels;
+// the m x s batch d_b takes ids n .. n + m - 1.  d_label (n + m entries) gets the labels of all n + m sketches,
+// d_cnt[0] the links found (cross pairs counted with the batch row as the receiver, inner pairs with the lower
+// row), d_cnt[1] the groups, d_cnt[2] the earlier groups absorbed into another.  d_old is only read.  Argument
+// checks are the caller's.
+int launch_mash_cluster_add(const DistancePlan &plan, const uint32_t *d_old, const uint32_t *d_b, uint64_t m, int s, uint32_t min_same,
+                            uint32_t *d_label, unsigned long long *d_cnt, cudaStream_t st);
 // mash_derep.cu: greedy representatives at same >= min_same; rep[i] = i's representative (first or, with
 // PG_DEREP_NEAREST, nearest), the counter (may be NULL) = number of representatives.  mash_derep_check is the
 // argument rule of pg_mash_dereplicate: the flags, then mash_cluster_check.
@@ -270,6 +282,11 @@ int launch_index_within(const DistancePlan &plan, const uint32_t *d_q, uint64_t 
 // reference are written 0xFFFFFFFF / 0; nothing is written when the set is empty (the caller initialises).
 int launch_index_link(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, const uint32_t *d_ids,
                       bool nearest, uint32_t *d_rep, unsigned long long *d_key, cudaStream_t st);
+// mash_index.cu: for each of nq query sketches of size sq > 0, every reference p of plan's set with same >= min_same
+// (min_same >= 1; the query is the receiver) united with query q as sketch first + q in the forest d_parent
+// (launch_cluster_link), and the links counted into *d_n_links.  Nothing is done when the set is empty.
+int launch_index_cluster(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, uint64_t first,
+                         uint32_t *d_parent, unsigned long long *d_n_links, cudaStream_t st);
 // mash_derep.cu: one batch of a growing dereplication.  The m x s batch d_b takes ids base .. base + m - 1; plan
 // holds the kept representatives (ids d_ids, ascending) of the rows before it.  Rows linked to a kept
 // representative are seeded from it (launch_index_link), then the batch is dereplicated on its own with the seeded

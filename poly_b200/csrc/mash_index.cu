@@ -20,6 +20,9 @@
 // A growing dereplication (launch_index_link) seeds a batch from its kept representatives with a third:
 //   index_link_kernel<Nearest> one CTA per row: the first reference (or the closest, ties to the first) with
 //                              same >= min_same, written as the row's assignment or nearest key.
+// A growing clustering (launch_index_cluster) unites each batch row with every reference it links to with a
+// fourth, the scan of mash_cluster.cu (launch_cluster_link without its upper-triangle rule: each entry of the
+// block is one pair of a batch row and an earlier sketch).
 #include <algorithm>
 #include <cstdlib>
 
@@ -514,6 +517,15 @@ int launch_index_link(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq
             PG_LAUNCH_CHECK("index_link_kernel<false>");
         }
         return PG_OK;
+    });
+}
+
+int launch_index_cluster(const DistancePlan &plan, const uint32_t *d_q, uint64_t nq, int sq, uint32_t min_same, uint64_t first,
+                         uint32_t *d_parent, unsigned long long *d_n_links, cudaStream_t st) {
+    if (nq == 0 || plan.n == 0) return PG_OK;
+    const uint64_t n = plan.n;
+    return index_blocks(plan, d_q, nq, sq, st, [&](const uint32_t *d_acc, uint64_t rb, uint64_t re) {
+        return launch_cluster_link(d_acc, re - rb, n, first + rb, 0, false, min_same, d_parent, d_n_links, st);
     });
 }
 

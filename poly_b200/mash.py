@@ -545,16 +545,17 @@ def dereplicate(sketches, min_same: Optional[int] = None, max_distance: Optional
 
 
 class _RepresentativeIndex(SketchIndex):
-    """The representative index a Dereplicator owns, borrowed for queries: it is grown only by the
-    dereplicator's adds and released with it."""
+    """An index a growing grouping (Dereplicator, Clusterer) owns, borrowed for queries: it is grown only by its
+    owner's adds and released with it."""
 
-    def __init__(self, h, s: int):
+    def __init__(self, h, s: int, owner: str = "Dereplicator"):
         self._h = h
         self._dev_queried = None
         self.n, self.s = 0, s
+        self._owner = owner
 
     def add(self, sketches) -> int:
-        raise ValueError("the representative index grows only through Dereplicator.add")
+        raise ValueError(f"this index grows only through {self._owner}.add")
 
     def close(self) -> None:
         if self._h is not None and self._dev_queried is not None:
@@ -666,6 +667,100 @@ class Dereplicator:
             _lib.check(_lib.lib().pg_mash_dereplicator_free(h))
 
     def __enter__(self) -> "Dereplicator":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        if getattr(self, "_h", None) is not None:
+            try:
+                self.close()
+            except Exception:
+                pass
+
+
+class Clusterer:
+    """A clustering that grows: each add merges a new batch of sketches into the single-linkage groups of the
+    sketches added so far, on the device, without clustering the earlier sketches again.  Sketches are numbered in
+    the order they are added.  After every add, labels() equals cluster() of the concatenated batches, with the same
+    min_same / max_distance; earlier labels can change when a batch joins two earlier groups (n_merged > 0).
+
+    s: the sketch size of every batch.  A max_distance under which every pair links, or none can, is a ValueError.
+    Every sketch is kept in a SketchIndex (`index`, read-only, reference p is sketch p), so "which group would this
+    sketch join" is a nearest or within query followed by labels()."""
+
+    def __init__(self, s: int, min_same: Optional[int] = None, max_distance: Optional[float] = None):
+        if (min_same is None) == (max_distance is None):
+            raise ValueError("give exactly one of min_same and max_distance")
+        s = int(s)
+        if max_distance is not None and s > 0:  # s <= 0: the library reports the reference's panic
+            min_same = min_same_for_distance(max_distance, s)
+            if min_same == 0:
+                raise ValueError(f"max_distance {max_distance!r} links every pair: every Distance is <= it")
+            if min_same == s + 1:
+                raise ValueError(f"max_distance {max_distance!r} links no pair: no Distance is <= it")
+        min_same = 1 if min_same is None else int(min_same)
+        if not 0 <= min_same <= 0xFFFFFFFF:
+            raise ValueError("min_same must fit 32 bits")
+        h = C.c_void_p()
+        _index_rc(_lib.lib().pg_mash_clusterer_create(s, min_same, C.byref(h)))
+        self._h = h
+        self.index = _RepresentativeIndex(C.c_void_p(_lib.lib().pg_mash_clusterer_index(h)), s, "Clusterer")
+        self._lock = threading.Lock()
+        self.s, self.min_same = s, min_same
+        self.n = self.n_groups = self.n_links = 0
+
+    def add(self, sketches):
+        """Merges a batch (what cluster takes): returns (labels [m], n_groups, n_links, n_merged).  labels are the
+        global labels of the batch's rows (row i is sketch first + i) after this add; n_groups counts every group
+        after it, n_links the links this add found and n_merged the earlier groups it absorbed into another.  CUDA
+        tensors give a CUDA int32 tensor (carrying the uint32 bits), ordered on the current stream; the call itself
+        synchronises."""
+        if self._h is None:
+            raise ValueError("the clusterer is closed")
+        rows = _sketch_rows(sketches)
+        m, s = int(rows.shape[0]), int(rows.shape[1])
+        first, ng, nl, nm = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        if self.index._dev_queried is not None:  # the add releases buffers that device queries, on any stream, may still read
+            import torch
+
+            torch.cuda.synchronize(self.index._dev_queried)
+        if hasattr(rows, "data_ptr"):
+            import torch
+
+            labels = torch.empty(m, dtype=torch.int32, device=rows.device)
+            rc = _lib.lib().pg_mash_clusterer_add_dev(self._h, rows.data_ptr(), m, s, labels.data_ptr(), C.byref(first), C.byref(ng),
+                                                      C.byref(nl), C.byref(nm), torch.cuda.current_stream(rows.device).cuda_stream)
+        else:
+            labels = np.empty(m, dtype=np.uint32)
+            rc = _lib.lib().pg_mash_clusterer_add(self._h, rows.ctypes.data, m, s, labels.ctypes.data, C.byref(first), C.byref(ng),
+                                                  C.byref(nl), C.byref(nm))
+        _index_rc(rc)
+        with self._lock:
+            if int(first.value) + m >= self.n:  # the latest add of any thread
+                self.n, self.n_groups = int(first.value) + m, int(ng.value)
+            self.n_links += int(nl.value)
+            self.index.n = self.n
+        return labels, int(ng.value), int(nl.value), int(nm.value)
+
+    def labels(self, begin: int = 0, end: Optional[int] = None):
+        """The current labels of sketches [begin, end) (end defaults to every sketch added), uint32."""
+        if self._h is None:
+            raise ValueError("the clusterer is closed")
+        end = self.n if end is None else int(end)
+        begin = int(begin)
+        out = np.empty(max(end - begin, 0), dtype=np.uint32)
+        _lib.check(_lib.lib().pg_mash_clusterer_labels(self._h, begin, end, out.ctypes.data if len(out) else None))
+        return out
+
+    def close(self) -> None:
+        if self._h is not None:
+            self.index.close()
+            h, self._h = self._h, None
+            _lib.check(_lib.lib().pg_mash_clusterer_free(h))
+
+    def __enter__(self) -> "Clusterer":
         return self
 
     def __exit__(self, *exc) -> None:
