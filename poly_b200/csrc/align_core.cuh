@@ -24,8 +24,11 @@ __device__ __forceinline__ int addmax<int>(int a, int b, int c) {
     return __viaddmax_s32(a, b, c);
 }
 
-// The score of a row beyond the string: -2^29 / -2^61, below every valid cell, and diag + score
-// cannot overflow.
+// The score of a row beyond the string: -2^29 / -2^61, below every valid cell.  Near a limit of the
+// type, rows beyond the string can wrap: a global alignment's diag + score near the negative limit, or
+// a positive gap's running sums near the positive one.  That is harmless only because those rows are
+// never read: a row depends on smaller rows alone, the NW result comes from the string's last row, and
+// a positive gap masks them out of the SW maximum.
 template <typename T>
 struct NegBig {
     static constexpr T value = (T)0 - ((T)1 << (sizeof(T) * 8 - 3));
@@ -123,18 +126,27 @@ struct AlignScoring {
         for (int i = 0; i < n_a * n_b; ++i) m = std::max<int64_t>(m, table[i] < 0 ? -table[i] : table[i]);
         return m;
     }
-    int64_t abs_gap() const { return gap < 0 ? -gap : gap; }
 };
 
 // Scores take 32-bit arithmetic when score_bound(...) < SCORE32_LIMIT, 64-bit otherwise.
 constexpr long double SCORE32_LIMIT = 2.0e9L;
 
 // A bound on every DP value and on the operands of one add, for strings of which the shorter has at
-// most short_len symbols and the two together at most sum_len.  SW: values lie in [0, max|S| * short],
-// and one add puts max(|S|, |gap|) on top.  NW: every value lies within (sum + 2) * max(|S|, |gap|).
-inline long double score_bound(int global, int64_t amax, int64_t agap, uint64_t short_len, uint64_t sum_len) {
-    return global ? (long double)std::max(amax, agap) * (long double)(sum_len + 2)
-                  : (long double)amax * (long double)short_len + (long double)std::max(amax, agap);
+// most short_len symbols and the two together at most sum_len.  NW: a value is the sum of at most sum
+// steps of |S| or |gap|, so every value lies within (sum + 2) * max(|S|, |gap|).  SW with gap <= 0: values
+// lie in [0, max|S| * short], and one add puts max(|S|, |gap|) on top.  SW with gap > 0: H[i][j] >=
+// H[i][j-1] + gap, so values grow with the longer string too and take the NW bound.
+inline long double score_bound(int global, int64_t amax, int64_t gap, uint64_t short_len, uint64_t sum_len) {
+    const int64_t agap = gap < 0 ? -gap : gap;
+    return global || gap > 0 ? (long double)std::max(amax, agap) * (long double)(sum_len + 2)
+                             : (long double)amax * (long double)short_len + (long double)std::max(amax, agap);
+}
+
+// The packed 2 x int16 score kernel (sw_score.cu) takes a call when it is local with gap <= 0 and every
+// DP value stays below 2^14: below 16000 by the bound, and rows beyond a query (-16384 + a value >= 0, or
+// a value >= 0 + gap) stay above -2^15.  It holds two queries per thread, so a call needs two of them.
+inline bool score_packed16(int global, int64_t gap, long double bound, uint64_t nq) {
+    return !global && gap <= 0 && bound < 16000.0L && -gap < 16000 && nq >= 2;
 }
 
 // Device copy of the scoring: [lut_row: 256 int16][lut_col: 256 int16][tables in T].

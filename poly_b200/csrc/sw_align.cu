@@ -241,7 +241,7 @@ int launch_sw_align(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uin
         return launch_sw_align_long(d_q, d_qoff, nq, max_qlen, d_t, tlen, query_is_a, s, d_score, d_err, d_align_a, d_align_b,
                                     out_stride, d_len, d_status, st);
     }
-    if (score_bound(s.global, s.abs_max(), s.abs_gap(), 64, 64 + tlen) >= SCORE32_LIMIT) {
+    if (score_bound(s.global, s.abs_max(), s.gap, 64, 64 + tlen) >= SCORE32_LIMIT) {
         set_error("aligned strings need scores that fit 32 bits");
         return PG_ERR_UNSUPPORTED;
     }

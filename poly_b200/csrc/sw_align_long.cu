@@ -99,7 +99,7 @@ int launch_sw_align_long(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq
                          uint8_t *d_align_a, uint8_t *d_align_b, uint64_t out_stride, uint32_t *d_len, int32_t *d_status,
                          cudaStream_t st, const uint64_t *d_toff, const uint32_t *d_pq, const uint32_t *d_pt) {
     if (nq == 0) return PG_OK;
-    if (score_bound(1, s.abs_max(), s.abs_gap(), 0, max_qlen + tlen) >= SCORE32_LIMIT) {  // the NW bound for SW too
+    if (score_bound(1, s.abs_max(), s.gap, 0, max_qlen + tlen) >= SCORE32_LIMIT) {  // the NW bound for SW too
         set_error("aligned strings need scores that fit 32 bits");
         return PG_ERR_UNSUPPORTED;
     }

@@ -447,7 +447,7 @@ int launch_sw_score_pairs(const uint8_t *d_a, const uint64_t *d_aoff, uint64_t n
     p.b = d_b; p.boff = d_boff; p.nb = nb; p.max_lb = max_lb;
     p.pa = d_pa; p.pb = d_pb; p.n = n_pairs; p.n_a = s.n_a; p.n_b = s.n_b; p.min_class = 0;
     // the longest a and b of the call
-    if (score_bound(s.global, s.abs_max(), s.abs_gap(), std::min(max_la, max_lb), max_la + max_lb) < SCORE32_LIMIT)
+    if (score_bound(s.global, s.abs_max(), s.gap, std::min(max_la, max_lb), max_la + max_lb) < SCORE32_LIMIT)
         return run_pairs<int>(p, s, d_score, d_err, d_errpos, st);
     return run_pairs<long long>(p, s, d_score, d_err, d_errpos, st);
 }

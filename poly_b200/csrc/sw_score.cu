@@ -340,7 +340,7 @@ int run_sw(const SwParams &p, uint64_t max_qlen, const AlignScoring &s, int64_t 
                          d.tab, (T)gap, d_score, d_err, d_errpos);
         launched = true;
     };
-    // packed 2 x int16 kernel: local alignment, gap <= 0, every DP value < 2^14 (checked by the caller: x2_ok)
+    // packed 2 x int16 kernel: local alignment, gap <= 0, every DP value < 2^14 (x2_ok: score_packed16)
     auto try_x2 = [&](auto rows_tag) {
         constexpr int ROWS = decltype(rows_tag)::value;
         if (launched || max_qlen > (uint64_t)ROWS) return;
@@ -399,13 +399,9 @@ int launch_sw_score(const uint8_t *d_q, const uint64_t *d_qoff, uint64_t nq, uin
     p.global = s.global;
     p.n_q = query_is_a ? s.n_a : s.n_b;
     p.n_t = query_is_a ? s.n_b : s.n_a;
-    const int64_t agap = s.abs_gap();
-    const long double bound = score_bound(s.global, s.abs_max(), agap, std::min<uint64_t>(max_qlen, tlen), max_qlen + tlen);
-    if (bound < SCORE32_LIMIT) {
-        // two queries per register (2 x int16) when a local alignment's values stay below 2^14 and gap <= 0
-        const bool x2_ok = !s.global && s.gap <= 0 && bound < 16000.0L && agap < 16000 && nq >= 2;
-        return run_sw<int>(p, max_qlen, s, d_score, d_err, d_errpos, st, x2_ok);
-    }
+    const long double bound = score_bound(s.global, s.abs_max(), s.gap, std::min<uint64_t>(max_qlen, tlen), max_qlen + tlen);
+    if (bound < SCORE32_LIMIT)
+        return run_sw<int>(p, max_qlen, s, d_score, d_err, d_errpos, st, score_packed16(s.global, s.gap, bound, nq));
     return run_sw<long long>(p, max_qlen, s, d_score, d_err, d_errpos, st);
 }
 
