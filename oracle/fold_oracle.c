@@ -129,7 +129,12 @@ static double jacobsonStockmayer(int queryLen, int knownLen, double dGx, double 
     double gasConstant = 1.9872e-3;
     return dGx + 2.44 * gasConstant * temp * log((double)queryLen / (double)knownLen);
 }
-static double go_min(double a, double b) { /* math.Min for non-NaN operands */
+/* Go's math.Min, whose documented special cases come in this order: Min(x, -Inf) = Min(-Inf, x) = -Inf,
+ * Min(x, NaN) = Min(NaN, x) = NaN, Min(-0, +-0) = Min(+-0, -0) = -0 */
+static double go_min(double a, double b) {
+    if (isinf(a) && a < 0) return a;
+    if (isinf(b) && b < 0) return b;
+    if (isnan(a) || isnan(b)) return NAN;
     if (a == 0 && b == 0) return signbit(a) ? a : b;
     return a < b ? a : b;
 }
@@ -638,8 +643,12 @@ int fo_fold(const char *raw, int64_t n, double temp, double *mfe, char *db, int6
     return st;
 }
 
+/* operands of which = 5: an index of fo_probe names one of these */
+static const double go_min_operands[] = {-INFINITY, -1.0, -0.0, 0.0, 1.0, INFINITY, NAN};
+
 /* One of the reference's internal functions on a filled context (for the reference tests' pins):
- * which 0 stack(a,b,c,d), 1 Bulge(a,b,c,d), 2 hairpin(a,b), 3 internalLoop(a,b,c,d), 4 W(a,b).energy */
+ * which 0 stack(a,b,c,d), 1 Bulge(a,b,c,d), 2 hairpin(a,b), 3 internalLoop(a,b,c,d), 4 W(a,b).energy,
+ * 5 go_min(go_min_operands[a], go_min_operands[b]) */
 int fo_probe(const char *raw, int64_t n, double temp, int which, int a, int b, int cc, int d, double *out) {
     context c;
     char *upper = NULL;
@@ -650,6 +659,7 @@ int fo_probe(const char *raw, int64_t n, double temp, int which, int a, int b, i
         case 1: st = Bulge(a, b, cc, d, &c, out); break;
         case 2: st = hairpin(a, b, &c, out); break;
         case 3: st = internalLoop(a, b, cc, d, &c, out); break;
+        case 5: *out = go_min(go_min_operands[a], go_min_operands[b]); break;
         default: *out = W(a, b, &c).energy; st = c.err; break;
         }
     }

@@ -81,7 +81,12 @@ struct Item {
     __device__ int key(int a, int b, int cc, int d) const { return c(a) * 125 + c(b) * 25 + c(cc) * 5 + c(d); }
 };
 
+// Go's math.Min, whose documented special cases come in this order: Min(x, -Inf) = Min(-Inf, x) = -Inf,
+// Min(x, NaN) = Min(NaN, x) = NaN, Min(-0, +-0) = Min(+-0, -0) = -0
 __device__ inline double go_min(double a, double b) {
+    if (isinf(a) && a < 0) return a;
+    if (isinf(b) && b < 0) return b;
+    if (isnan(a) || isnan(b)) return NAN;
     if (a == 0 && b == 0) return signbit(a) ? a : b;
     return a < b ? a : b;
 }

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import math
 import os
 
 import numpy as np
@@ -75,8 +76,9 @@ def fold(seq: bytes, temp: float, with_structs: bool = False):
 
 
 def probe(seq: bytes, temp: float, which: str, *idx) -> tuple:
-    """(status, value) of stack / Bulge / hairpin / internalLoop / W on the filled context of seq."""
-    code = {"stack": 0, "Bulge": 1, "hairpin": 2, "internalLoop": 3, "W": 4}[which]
+    """(status, value) of stack / Bulge / hairpin / internalLoop / W on the filled context of seq, or of
+    go_min on operands named by index (go_min below)."""
+    code = {"stack": 0, "Bulge": 1, "hairpin": 2, "internalLoop": 3, "W": 4, "go_min": 5}[which]
     a = list(idx) + [0] * (4 - len(idx))
     out = C.c_double()
     st = lib().fo_probe(seq, len(seq), temp, code, a[0], a[1], a[2], a[3], C.byref(out))
@@ -87,6 +89,18 @@ def pair(seq: bytes, a: int, b: int, c: int, d: int) -> str:
     out = C.create_string_buffer(6)
     lib().fo_pair(seq, a, b, c, d, out)
     return out.value.decode()
+
+
+GO_MIN_OPERANDS = (-math.inf, -1.0, -0.0, 0.0, 1.0, math.inf, math.nan)  # fold_oracle.c's go_min_operands
+
+
+def go_min(a: float, b: float) -> float:
+    """The restatement's math.Min of two operands from GO_MIN_OPERANDS."""
+    ix = lambda x: next(i for i, v in enumerate(GO_MIN_OPERANDS) if (math.isnan(v) and math.isnan(x)) or
+                        (v == x and math.copysign(1, v) == math.copysign(1, x)))
+    st, out = probe(b"ACGT", 37.0, "go_min", ix(a), ix(b))
+    assert st == OK
+    return out
 
 
 def fold_batch(seqs, temp: float, threads: int = 16):

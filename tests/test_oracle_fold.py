@@ -106,6 +106,57 @@ def test_empty_result_mfe_is_inf():
     assert fold.Result().MinimumFreeEnergy() == math.inf and fold.Result().DotBracket() == ""
 
 
+NAN, INF = math.nan, math.inf
+
+
+@pytest.mark.parametrize("a,b,want", [
+    (-1.0, 1.0, -1.0), (1.0, -1.0, -1.0),     # ordered operands
+    (1.0, -INF, -INF), (-INF, 1.0, -INF),     # -Inf wins over anything ...
+    (NAN, -INF, -INF), (-INF, NAN, -INF),     # ... NaN included
+    (NAN, 1.0, NAN), (1.0, NAN, NAN),         # NaN next, whichever side it is on
+    (INF, NAN, NAN), (NAN, NAN, NAN),
+    (-0.0, 0.0, -0.0), (0.0, -0.0, -0.0),     # -0 below +0
+    (0.0, 0.0, 0.0), (-0.0, -0.0, -0.0), (INF, 1.0, 1.0),
+])
+def test_go_min_is_math_min(a, b, want):
+    # Go's math.Min: Min(x, -Inf) = Min(-Inf, x) = -Inf, Min(x, NaN) = Min(NaN, x) = NaN,
+    # Min(-0, +-0) = Min(+-0, -0) = -0, in that order of precedence
+    got = fo.go_min(a, b)
+    if math.isnan(want):
+        assert math.isnan(got)
+    else:
+        assert got == want and math.copysign(1.0, got) == math.copysign(1.0, want)
+
+
+def test_branch_heavy_item_fits_the_kernel_capacities():
+    # fold.cu keeps a W cell's branch list in an arena slot of (d + 1) / 5 entries (d = end - start) and the
+    # traceback's pending branches in a 256-entry stack.  Replay the traceback's order on the restatement's
+    # structure list: each chain of V cells pops one pending branch; a multibranch ends its chain and pushes
+    # its branches (its "BIFURCATION:<u>n/<h>h" description counts the closing pair too).
+    import fold_designs
+
+    st, _, _, structs = fo.fold(fold_designs.branch_heavy().encode(), 37.0, with_structs=True)
+    assert st == fo.OK
+    largest, largest_cap, depth, pending, chain = 0, 0, 0, 1, False
+    for _, desc, [(s, e)] in structs:
+        if not chain:
+            pending -= 1
+            chain = True
+        if desc.startswith("BIFURCATION"):
+            nb = int(desc.split("/")[1].rstrip("h")) - 1
+            cap = (e - s + 1) // 5
+            assert nb <= cap, (s, e, nb, cap)
+            largest, largest_cap = max((largest, largest_cap), (nb, cap))
+            pending += nb
+            depth = max(depth, pending)
+            chain = False
+        elif desc.startswith("HAIRPIN") or desc == "":  # no inner pair: the chain ends
+            chain = False
+    assert pending == 0 and not chain
+    print(f"largest branch list {largest} of a slot of {largest_cap}; deepest pending branches {depth} of 256")
+    assert largest >= 3 and 10 <= depth <= 256
+
+
 def _inc_tables():
     text = open(os.path.join(ROOT, "poly_b200", "csrc", "fold_tables.inc")).read()
     out = {}
