@@ -795,6 +795,62 @@ func (c *Clusterer) Close() error {
 	return locked(func() C.int { return C.pg_mash_clusterer_free(h) })
 }
 
+// Screen wraps a pg_mash_screen: a reference sketch set and a pool of reads on the device of the calling thread.
+// Close must not run while another call on it is in flight.
+type Screen struct {
+	h *C.pg_mash_screen
+	n int
+}
+
+// NewScreen wraps pg_mash_screen_create for n references of s words each (full arrays, zero tails included) and
+// k-mer size k.
+func NewScreen(sketches []uint32, n, s, k int) (*Screen, error) {
+	var h *C.pg_mash_screen
+	var p *C.uint32_t
+	if len(sketches) > 0 {
+		p = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
+	}
+	if err := locked(func() C.int { return C.pg_mash_screen_create(p, C.uint64_t(n), C.int32_t(s), C.int32_t(k), &h) }); err != nil {
+		return nil, err
+	}
+	return &Screen{h: h, n: n}, nil
+}
+
+// Add wraps pg_mash_screen_add: every window of the reads is counted into the pool.
+func (sc *Screen) Add(reads []string) error {
+	if len(reads) == 0 {
+		return nil
+	}
+	bases, offsets := Flatten(reads)
+	return locked(func() C.int {
+		return C.pg_mash_screen_add(sc.h, (*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(len(reads)))
+	})
+}
+
+// Reset wraps pg_mash_screen_reset: the pool is emptied.
+func (sc *Screen) Reset() error { return locked(func() C.int { return C.pg_mash_screen_reset(sc.h) }) }
+
+// Results wraps pg_mash_screen_results: per reference, the shared hash count, the containment and the median
+// multiplicity of the pool so far.
+func (sc *Screen) Results() (shared []uint32, containment []float64, multiplicity []uint64, err error) {
+	shared, containment, multiplicity = make([]uint32, sc.n+1), make([]float64, sc.n+1), make([]uint64, sc.n+1)
+	err = locked(func() C.int {
+		return C.pg_mash_screen_results(sc.h, (*C.uint32_t)(unsafe.Pointer(&shared[0])), (*C.double)(unsafe.Pointer(&containment[0])),
+			(*C.uint64_t)(unsafe.Pointer(&multiplicity[0])))
+	})
+	return shared[:sc.n], containment[:sc.n], multiplicity[:sc.n], err
+}
+
+// Close wraps pg_mash_screen_free.
+func (sc *Screen) Close() error {
+	if sc.h == nil {
+		return nil
+	}
+	h := sc.h
+	sc.h = nil
+	return locked(func() C.int { return C.pg_mash_screen_free(h) })
+}
+
 // SeqhashBatch wraps pg_seqhash_batch: digest[32*i:32*i+32], errCode[i] and errPos[i] for each of the
 // sequences bases[offsets[i]:offsets[i+1]], all of one seqType (0 DNA, 1 RNA, 2 PROTEIN) and flags
 // (1 circular | 2 double-stranded).

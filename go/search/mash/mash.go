@@ -6,6 +6,7 @@ package mash
 import (
 	"errors"
 	"fmt"
+	"math"
 	"sync"
 
 	"github.com/bebop/poly/internal/polyb200"
@@ -389,6 +390,71 @@ func (c *Clusterer) Labels(begin, end int) ([]int, error) {
 
 // Close releases the clusterer's device memory.
 func (c *Clusterer) Close() error { return c.c.Close() }
+
+// Screen is Mash Screen (Ondov et al. 2019) on the GPU: which of a set of reference sketches a pool of reads
+// contains.  Add counts every window a Sketch would hash of every read (forward strand, raw bytes) into the pool;
+// Results gives, per reference, Shared = the sum over hashes v of min(c_ref(v), c_pool(v)), Containment = Shared /
+// SketchSize and Multiplicity = the lower median pool count of the shared hashes.  Any split of the pool into Adds
+// gives the same Results, and Reset empties the pool.  Identity is Containment^(1/kmerSize), computed on the host.
+// Call Close when done.
+type Screen struct {
+	sc *polyb200.Screen
+	k  int
+}
+
+// ScreenResult is the answer for one reference.
+type ScreenResult struct {
+	Shared       int
+	Containment  float64
+	Multiplicity uint64
+	Identity     float64
+}
+
+// NewScreen prepares a screen against refs, which must share one SketchSize, for k-mers of kmerSize (the size they
+// were sketched with; it is not checked, as Similarity does not check it).
+func NewScreen(refs []*Mash, kmerSize int) (*Screen, error) {
+	s := 0
+	if len(refs) > 0 {
+		s = refs[0].SketchSize
+	}
+	flat := make([]uint32, 0, len(refs)*s)
+	for _, m := range refs {
+		if m.SketchSize != s {
+			return nil, errors.New("mash: Screen needs one common SketchSize")
+		}
+		flat = append(flat, m.Sketches[:s]...)
+	}
+	if len(refs) > 0 && s <= 0 {
+		panic("runtime error: index out of range [-1]") // Similarity on a sketch of size 0 would
+	}
+	sc, err := polyb200.NewScreen(flat, len(refs), s, kmerSize)
+	if err != nil {
+		return nil, err
+	}
+	return &Screen{sc: sc, k: kmerSize}, nil
+}
+
+// Add counts the windows of reads into the pool.
+func (s *Screen) Add(reads []string) error { return s.sc.Add(reads) }
+
+// Reset empties the pool.
+func (s *Screen) Reset() error { return s.sc.Reset() }
+
+// Results returns one ScreenResult per reference, in the order given to NewScreen.
+func (s *Screen) Results() ([]ScreenResult, error) {
+	shared, cont, mult, err := s.sc.Results()
+	if err != nil {
+		return nil, err
+	}
+	out := make([]ScreenResult, len(shared))
+	for i := range out {
+		out[i] = ScreenResult{Shared: int(shared[i]), Containment: cont[i], Multiplicity: mult[i], Identity: math.Pow(cont[i], 1/float64(s.k))}
+	}
+	return out, nil
+}
+
+// Close releases the screen's device memory.
+func (s *Screen) Close() error { return s.sc.Close() }
 
 // Neighbor is one reference of a Nearest result.
 type Neighbor struct {

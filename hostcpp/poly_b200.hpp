@@ -19,6 +19,7 @@
 // repository can compile and run (tests/test_gpu_hostcpp.py).  No compute happens here.
 #pragma once
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -519,6 +520,52 @@ public:
     std::vector<uint32_t> Labels(uint64_t begin, uint64_t end) const {
         std::vector<uint32_t> out(end > begin ? end - begin : 0);
         check(pg_mash_clusterer_labels(h_, begin, end, out.data()));
+        return out;
+    }
+};
+
+// Mash Screen on the device (pg_mash_screen): which references of a sketch set a pool of reads contains.  Add hashes
+// every window a Sketch would hash of every read into the pool; Results gives, per reference, Shared = sum over v of
+// min(c_r(v), c_pool(v)), Containment = Shared / s and Multiplicity = the lower median pool count of the shared
+// hashes.  Any split of the pool into Adds gives the same Results; Reset empties the pool.
+class Screen {
+    pg_mash_screen *h_ = nullptr;
+    size_t n_ = 0;
+    int k_ = 0;
+
+public:
+    Screen(const std::vector<Mash> &refs, int kmerSize) : n_(refs.size()), k_(kmerSize) {
+        int s;
+        const std::vector<uint32_t> flat = detail::FlatRows(refs, "references", &s);
+        int rc = pg_mash_screen_create(flat.data(), refs.size(), s, kmerSize, &h_);
+        if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
+        check(rc);
+    }
+    Screen(const Screen &) = delete;
+    Screen &operator=(const Screen &) = delete;
+    ~Screen() { pg_mash_screen_free(h_); }
+    void Add(const std::vector<std::string> &reads) {
+        const Flat f(reads);
+        check(pg_mash_screen_add(h_, f.bases.data(), f.offsets.data(), reads.size()));
+    }
+    void Reset() { check(pg_mash_screen_reset(h_)); }
+    struct Result {
+        std::vector<uint32_t> Shared;
+        std::vector<double> Containment;
+        std::vector<uint64_t> Multiplicity;
+    };
+    Result Results() const {
+        Result r;
+        r.Shared.resize(n_);
+        r.Containment.resize(n_);
+        r.Multiplicity.resize(n_);
+        check(pg_mash_screen_results(h_, r.Shared.data(), r.Containment.data(), r.Multiplicity.data()));
+        return r;
+    }
+    // Mash Screen's identity estimate, Containment^(1/k), on the host
+    std::vector<double> Identity() const {
+        std::vector<double> out = Results().Containment;
+        for (double &c : out) c = std::pow(c, 1.0 / k_);
         return out;
     }
 };

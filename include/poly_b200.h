@@ -519,6 +519,60 @@ int pg_mash_clusterer_labels_dev(const pg_mash_clusterer *c, uint64_t begin, uin
 const pg_mash_index *pg_mash_clusterer_index(const pg_mash_clusterer *c);
 int pg_mash_clusterer_free(pg_mash_clusterer *c);
 
+/* ---- screen: which references of a sketch set a pool of reads contains --------------------------------
+ * Mash Screen (Ondov et al., Genome Biol 20:232, 2019): every k-mer window of a pool of reads is hashed, and each
+ * reference sketch is asked how many of its hashes the pool holds and how often.  A screen holds n reference
+ * sketches of size s (n x s full Go arrays, zero tail included, as pg_mash_index_create takes them), a k-mer size k
+ * and a running pool, which adds grow and reset empties.
+ *   - Windows: a pool read of length L contributes the windows (*Mash).Sketch hashes, positions 0 .. L - k - 1
+ *     (the last k-mer is never hashed, mash.go:73; L <= k gives none), each hashed by murmur3.Sum32 over its raw
+ *     bytes: forward strand, case-sensitive, any byte value.  k is not checked against the references, as in the
+ *     reference; pass the k the sketches were made with.
+ *   - Counts: c_pool(v) = the windows of every read of every add since creation or the last reset whose hash is v;
+ *     c_r(v) = the words of reference r equal to v, taken as given (zero-tail words are the value 0; unsorted
+ *     fill-regime sketches are allowed).
+ *   - Results for reference r: shared[r] = sum over v of min(c_r(v), c_pool(v)), the multiset count Similarity
+ *     uses; containment[r] = (double)shared[r] / (double)s; multiplicity[r] = the lower median (element
+ *     floor((m - 1) / 2) of m in ascending order) of the multiset in which each v with c_pool(v) >= 1 contributes
+ *     the value c_pool(v) min(c_r(v), c_pool(v)) times; 0 when shared[r] == 0.  Mash Screen's identity,
+ *     containment^(1/k), is left to the caller.
+ *   - Split invariance: for any split of a pool into adds (empty and one-read adds included) the results equal
+ *     those of one add of the concatenation; after a reset the screen answers as a freshly created one.
+ *   - Errors, checked in this order: a null screen or out is PG_ERR_ARG (no device is needed); k < 0 is
+ *     PG_ERR_ARG, as for the sketch calls; s <= 0 with n > 0 is PG_ERR_PANIC, as for index create; n > 2^32 - 1 is
+ *     PG_ERR_ARG (the keys hold 32-bit ids); a null buffer is PG_ERR_ARG.  n == 0 and n_reads == 0 are valid (an
+ *     add of no read changes nothing and needs no buffer).  Offsets that decrease in a host add are PG_ERR_ARG.
+ *     Any output of results may be NULL.  PG_ERR_NOMEM when device memory runs out.  After any error the screen
+ *     holds what it held before.
+ *   - _dev offsets: add_dev trusts d_offsets as pg_mash_sketch_batch_dev does.  With non-decreasing offsets it
+ *     counts exactly the windows above.  Offsets that decrease give unspecified counts, but no byte outside
+ *     [d_offsets[0], d_offsets[n_reads]) is read and no memory outside the screen is written.
+ *   - Ownership, device and threads, as for pg_mash_index: create copies everything (no caller pointer is kept)
+ *     and the screen lives on the device current at creation.  Each screen has a reader-writer lock: add, add_dev
+ *     and reset hold it exclusively, results and results_dev shared, while they enqueue.  The host calls
+ *     synchronise (create also to size its buffers).  add_dev and results_dev only enqueue on `stream`; add_dev
+ *     makes no host decision that depends on the data.  Work enqueued by _dev calls on different streams is ordered
+ *     by the caller: results see an add_dev only once its stream is ordered before them (a host call runs on the
+ *     library's own stream), and freeing or resetting a screen while a _dev call on it is still enqueued on an
+ *     unsynchronised stream is the caller's error.
+ *   - Counter width: pool counts are 64-bit, so a pool of more than 2^32 windows with one hash stays exact.
+ *     multiplicity is uint64; shared <= s.
+ *   - Device memory: with D distinct values among the n s words, a screen holds 8 n s bytes of sorted keys,
+ *     4 D of values, 8 D of counts and 8 (ceil(D / 4) + 1) of directory.  Create adds, while it runs, 8 n s bytes
+ *     of unsorted keys, 8 n s of values and CUB's sort storage (the host call also stages 4 n s bytes of sketches);
+ *     results add 16 n s bytes of multiplicity slots, 4 n of counts and CUB's segmented-sort storage; the host
+ *     add stages the pool's bytes and offsets. */
+typedef struct pg_mash_screen pg_mash_screen;
+int pg_mash_screen_create(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, pg_mash_screen **out);
+int pg_mash_screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, void *stream, pg_mash_screen **out);
+int pg_mash_screen_add(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads);
+int pg_mash_screen_add_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_reads, void *stream);
+int pg_mash_screen_reset(pg_mash_screen *sc);
+int pg_mash_screen_results(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity);
+int pg_mash_screen_results_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity,
+                               void *stream);
+int pg_mash_screen_free(pg_mash_screen *sc);
+
 /* ---- align.SmithWaterman score -- search/align/align.go:171-203 -------------------
  * One template against n queries.  query_is_a != 0: stringA = query (outer loop),
  * stringB = template; else swapped.  lut_a/lut_b: byte -> index into the first /

@@ -1,6 +1,6 @@
 // api_mash.cu -- the C ABI of poly's mash: Sketch on device and host buffers (the pipelined host path),
 // the single-process multi-GPU entry points, Similarity / Distance, the groups and the representatives of a
-// sketch set and the sketch index.
+// sketch set, the sketch index and the screen.
 #include <algorithm>
 #include <atomic>
 #include <cstring>
@@ -38,6 +38,13 @@ struct pg_mash_clusterer {
     uint32_t *d_label;      // label[i] = the smallest id of sketch i's group, ix->plan.n entries
     uint64_t n, n_groups;   // sketches added so far (the next batch's first id) and their groups
     mutable std::mutex mu;  // serialises adds, and label reads against them
+};
+
+struct pg_mash_screen {
+    int device;
+    int32_t k;
+    pg::ScreenIndex ix;            // the sorted reference keys, their distinct values and the pool counts
+    mutable std::shared_mutex rw;  // results hold it shared while they enqueue, an add or a reset exclusively
 };
 
 namespace pg {
@@ -615,6 +622,17 @@ static int cluster_add(pg_mash_clusterer *c, const uint32_t *d_b, uint64_t m, ui
     c->n_groups = cnt[1];
     return PG_OK;
 }
+
+// The argument rules of pg_mash_screen_create after the null out pointer, in their order
+static int screen_create_check(const void *sketches, uint64_t n, int32_t s, int32_t k) {
+    if (k < 0) { set_error("k-mer size %d < 0", k); return PG_ERR_ARG; }
+    if (n && s <= 0) { set_error("screen over sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
+    if (n > 0xffffffffull) { set_error("%llu references exceed 2^32 - 1", (unsigned long long)n); return PG_ERR_ARG; }
+    if (n && !sketches) { set_error("null buffer"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+static pg_mash_screen *screen_new(int32_t k, const ScreenIndex &ix) { return new pg_mash_screen{cur_ctx()->device, k, ix}; }
 
 }  // namespace
 }  // namespace pg
@@ -1286,6 +1304,110 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c) {
     rc = pg_mash_index_free(c->ix);
     delete c;
     return rc;
+}
+
+// ---------------------------------------------------------------------------------
+// Screen: which references a pool of reads contains
+// ---------------------------------------------------------------------------------
+int pg_mash_screen_create(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, pg_mash_screen **out) {
+    if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = screen_create_check(sketches, n, s, k);
+    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
+    ScreenIndex ix;
+    {
+        HostCall c;
+        const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)std::max(s, 0));
+        if ((rc = c.error()) || (rc = screen_build(d_sk, n, s, c.st, &ix))) return rc;
+        if ((rc = c.finish()) != PG_OK) {
+            screen_free(ix, c.st);
+            return rc;
+        }
+    }
+    *out = screen_new(k, ix);
+    return PG_OK;
+}
+
+int pg_mash_screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, void *stream, pg_mash_screen **out) {
+    if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = screen_create_check(d_sketches, n, s, k);
+    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
+    ScreenIndex ix;
+    if ((rc = screen_build(d_sketches, n, s, (cudaStream_t)stream, &ix)) != PG_OK) return rc;
+    *out = screen_new(k, ix);
+    return PG_OK;
+}
+
+int pg_mash_screen_add(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    if (n_reads == 0) return PG_OK;
+    if (!bases || !offsets) { set_error("null buffer"); return PG_ERR_ARG; }
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> lk(sc->rw);
+    HostCall c;
+    const Ragged<uint8_t> r = c.ragged(bases, offsets, n_reads);
+    if ((rc = c.error()) || (rc = screen_add(sc->ix, sc->k, r.base, r.off, n_reads, c.st))) return rc;
+    return c.finish();
+}
+
+int pg_mash_screen_add_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_reads, void *stream) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    if (n_reads == 0) return PG_OK;
+    if (!d_bases || !d_offsets) { set_error("null buffer"); return PG_ERR_ARG; }
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> lk(sc->rw);
+    return screen_add(sc->ix, sc->k, d_bases, d_offsets, n_reads, (cudaStream_t)stream);
+}
+
+int pg_mash_screen_reset(pg_mash_screen *sc) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> lk(sc->rw);
+    HostCall c;
+    if ((rc = screen_reset(sc->ix, c.st)) != PG_OK) return rc;
+    return c.finish();
+}
+
+int pg_mash_screen_results(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::shared_lock<std::shared_mutex> lk(sc->rw);
+    const uint64_t n = sc->ix.n;
+    if (n == 0 || (!shared && !containment && !multiplicity)) return PG_OK;
+    HostCall c;
+    uint32_t *d_sh = shared ? c.alloc<uint32_t>(n) : nullptr;
+    double *d_c = containment ? c.alloc<double>(n) : nullptr;
+    uint64_t *d_m = multiplicity ? c.alloc<uint64_t>(n) : nullptr;
+    if ((rc = c.error()) || (rc = screen_results(sc->ix, d_sh, d_c, d_m, c.st))) return rc;
+    c.download(shared, d_sh, n);
+    c.download(containment, d_c, n);
+    c.download(multiplicity, d_m, n);
+    return c.finish();
+}
+
+int pg_mash_screen_results_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity, void *stream) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::shared_lock<std::shared_mutex> lk(sc->rw);
+    return screen_results(sc->ix, d_shared, d_containment, d_multiplicity, (cudaStream_t)stream);
+}
+
+int pg_mash_screen_free(pg_mash_screen *sc) {
+    if (!sc) return PG_OK;
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+    cudaStream_t st = cur_ctx()->slots[0].stream;
+    screen_free(sc->ix, st);
+    delete sc;
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
 }
 
 }  // extern "C"

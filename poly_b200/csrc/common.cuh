@@ -201,6 +201,9 @@ __device__ __forceinline__ uint64_t join_bucket_scale(uint32_t nb, uint32_t vmax
 __device__ __forceinline__ uint32_t join_bucket(uint32_t v, uint64_t scale, uint32_t nb) {
     return min((uint32_t)(((uint64_t)v * scale) >> 32), nb - 1);
 }
+// The keys (v << 32 | id0 + e / s) of the `total` words d_sk[e] of rows of s words, in any order, and atomicMax of
+// their largest value into *d_vmax
+int launch_batch_keys(const uint32_t *d_sk, uint64_t total, uint32_t s, uint64_t id0, uint64_t *d_keys, uint32_t *d_vmax, cudaStream_t st);
 int join_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, JoinIndex *ix);
 int join_merge(const JoinIndex &old, const uint32_t *d_batch, uint64_t m, cudaStream_t st, JoinIndex *out);
 int join_emit(const JoinIndex &ix, uint64_t row_begin, uint64_t row_end, uint32_t *d_same, double *d_dist, cudaStream_t st);
@@ -298,6 +301,27 @@ int launch_mash_derep_add(const DistancePlan &plan, const uint32_t *d_ids, const
 // (n_new x s) and their ids to d_ids
 int launch_derep_gather(const uint32_t *d_b, uint64_t m, int s, uint32_t base, const uint32_t *d_rep, uint64_t n_new, uint32_t *d_rows,
                         uint32_t *d_ids, cudaStream_t st);
+// mash_screen.cu: a screen's device state.  keys: the n x s (value << 32 | id) keys of the reference words, sorted;
+// vals: the D distinct values, ascending; cnt: the pool count of each; dir: nb + 1 entries, dir[b] = the first
+// distinct value in bucket b of join_bucket over [0, vmax].
+struct ScreenIndex {
+    uint64_t *keys = nullptr, *dir = nullptr;
+    uint32_t *vals = nullptr;
+    unsigned long long *cnt = nullptr;
+    uint64_t n = 0, D = 0;
+    int s = 0;
+    uint32_t nb = 0, vmax = 0;
+};
+// Builds the screen of n reference rows of s > 0 words (any order, zero tails included) with zero counts;
+// synchronises st.  On an error nothing of *out is allocated.
+int screen_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, ScreenIndex *out);
+// Counts every window of reads [0, n_reads) of the ragged pool (d_bases, d_off) into ix.cnt; only enqueues, and
+// reads no byte outside [d_off[0], d_off[n_reads]) whatever the offsets hold.
+int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_reads, cudaStream_t st);
+int screen_reset(const ScreenIndex &ix, cudaStream_t st);
+// shared, containment and multiplicity of every reference (any output may be NULL); only enqueues
+int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st);
+void screen_free(ScreenIndex &ix, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).
 struct AlignScoring;

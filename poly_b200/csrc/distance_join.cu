@@ -85,7 +85,7 @@ __global__ void scan_kernel(const uint32_t *__restrict__ hist, uint32_t nbuckets
     for (uint32_t i = lo; i < hi; ++i) { start[i] = run; run += hist[i]; }
 }
 
-// The keys (v << 32 | id0 + row) of `total` words of ascending rows of s words, and their largest value into *vmax.
+// The keys (v << 32 | id0 + row) of `total` words of rows of s words, and their largest value into *vmax.
 __global__ void batch_keys_kernel(const uint32_t *__restrict__ sk, uint64_t total, uint32_t s, uint64_t id0,
                                   uint64_t *__restrict__ keys, uint32_t *__restrict__ vmax) {
     uint32_t m = 0;
@@ -303,6 +303,13 @@ uint64_t join_first_nb(uint64_t total) {
 
 }  // namespace
 
+int launch_batch_keys(const uint32_t *d_sk, uint64_t total, uint32_t s, uint64_t id0, uint64_t *d_keys, uint32_t *d_vmax, cudaStream_t st) {
+    if (total == 0) return PG_OK;
+    batch_keys_kernel<<<(unsigned)std::min<uint64_t>((total + 255) / 256, (uint64_t)sm_count() * 16), 256, 0, st>>>(d_sk, total, s, id0, d_keys, d_vmax);
+    PG_LAUNCH_CHECK("batch_keys_kernel");
+    return PG_OK;
+}
+
 // Builds the bucketed (value, id) index of n ascending sketches.  ix->ok == false means "not
 // applicable" (skewed data: a bucket would not fit shared memory) and the caller must use the
 // pairwise kernel.
@@ -385,9 +392,7 @@ int join_merge(const JoinIndex &old, const uint32_t *d_batch, uint64_t m, cudaSt
     PG_CUDA(cudaMemsetAsync(d_scalars + 1, 0, 4, st));
     PG_CUDA(cudaMemsetAsync(d_hist, 0, nb * 4, st));
     const unsigned sms = (unsigned)sm_count();
-    batch_keys_kernel<<<(unsigned)std::min<uint64_t>((M + 255) / 256, (uint64_t)sms * 16), 256, 0, st>>>(d_batch, M, (uint32_t)old.s, old.n,
-                                                                                                         d_keys, d_scalars);
-    PG_LAUNCH_CHECK("batch_keys_kernel");
+    { const int rc_ = launch_batch_keys(d_batch, M, (uint32_t)old.s, old.n, d_keys, d_scalars, st); if (rc_ != PG_OK) return rc_; }
     size_t bytes = 0, have = 0;
     uint8_t *d_cub = nullptr;
     PG_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, d_keys, d_sorted, M, 0, 64, st));

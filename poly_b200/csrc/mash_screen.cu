@@ -1,0 +1,378 @@
+// mash_screen.cu -- the screen: for each reference sketch of a set, how many of its hashes a pool of reads
+// contains and how often (Mash Screen's containment and median multiplicity, Ondov et al. 2019), counted from
+// every k-mer window of the pool.
+//
+// Create (screen_build, once per reference set):
+//   1. the (value << 32 | id) keys of the n x s reference words (launch_batch_keys), their largest value vmax;
+//   2. one CUB radix sort of the keys; the D distinct values, ascending (CUB Unique), and a directory of
+//      nb = ceil(D / 4) value buckets over [0, vmax] (join_bucket, the join index's mapping): dir[b] is the first
+//      distinct value in bucket b, so a lookup is two directory reads and a binary search over ~4 values;
+//   3. one 64-bit pool counter per distinct value, zeroed.
+// Add (the hot path, screen_add): the pool's bytes are cut into fixed chunks, whatever the read lengths; a
+// CTA stages a chunk (plus the k - 1 byte halo) in shared memory and each thread walks W consecutive windows
+// of it with the register-ring murmur3 walk of K1 (kmer_walk.cuh).  A window hash above vmax is dropped by one
+// compare, which is almost every window when the references are bottom-s sketches of large genomes.  The
+// rest are checked against the read boundaries (a binary search over the offsets, then a cursor) and looked
+// up; hits are aggregated per warp on equal counters (__match_any_sync) before one atomicAdd.  k outside the
+// walk's instantiated set hashes each window from global memory.
+// Results (screen_results): one pass over the sorted keys.  The c_r(v) words of reference r equal to v are one
+// run of equal keys, and the first min(c_r(v), c_pool(v)) of them count; each counted word appends c_pool(v)
+// to its reference's segment of s slots.  A CUB segmented sort of the segments then gives the lower median.
+#include <algorithm>
+#include <climits>
+
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_segmented_sort.cuh>
+#include <cub/device/device_select.cuh>
+
+#include "common.cuh"
+#include "kmer_walk.cuh"
+#include "murmur3.cuh"
+
+namespace pg {
+
+namespace {
+
+constexpr int SCREEN_THREADS = 256;
+
+// what the add kernels read of a screen
+struct ScreenLookup {
+    const uint32_t *vals;     // [D] distinct reference values, ascending
+    const uint64_t *dir;      // [nb + 1]
+    unsigned long long *cnt;  // [D] pool counts
+    uint32_t nb, vmax;
+};
+
+// the index d of value h among the distinct values, if h is one of them
+__device__ __forceinline__ bool screen_find(const ScreenLookup &L, uint64_t scale, uint32_t h, uint64_t *d) {
+    const uint32_t b = join_bucket(h, scale, L.nb);
+    uint64_t lo = L.dir[b], hi = L.dir[b + 1];
+    const uint64_t end = hi;
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi) >> 1;
+        if (L.vals[mid] < h) lo = mid + 1;
+        else hi = mid;
+    }
+    *d = lo;
+    return lo < end && L.vals[lo] == h;
+}
+
+// Whether the window at byte p is one of its read's: p + k < the end of the read that holds p, the first offset
+// above p.  j caches the index of that offset (~0 = not searched yet); a thread's windows only move forward.
+__device__ __forceinline__ bool window_in_read(const uint64_t *off, uint64_t n_reads, uint64_t p, uint32_t k, uint64_t &j) {
+    if (j == ~0ull) {
+        uint64_t lo = 0, hi = n_reads + 1;
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi) >> 1;
+            if (off[mid] > p) hi = mid;
+            else lo = mid + 1;
+        }
+        j = lo;
+    }
+    while (j <= n_reads && off[j] <= p) ++j;
+    return j <= n_reads && p + k < off[j];
+}
+
+// One window of every lane of a converged warp; cand: the lane's hash h is <= vmax.  Lanes that hit the same
+// counter add to it once, with their number.
+__device__ __forceinline__ void screen_hit(const ScreenLookup &L, uint64_t scale, const uint64_t *off, uint64_t n_reads, bool cand, uint64_t p,
+                                           uint32_t k, uint32_t h, uint64_t &j) {
+    uint64_t d = ~0ull;
+    const bool hit = cand && window_in_read(off, n_reads, p, k, j) && screen_find(L, scale, h, &d);
+    const unsigned peers = __match_any_sync(0xffffffffu, hit ? d : ~0ull);
+    if (hit && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&L.cnt[d], (unsigned long long)__popc(peers));
+}
+
+// windows per thread of the walk kernel: whole groups of NB word steps, about 64
+__host__ __device__ constexpr uint32_t screen_span(int nb) { return 4u * nb * (16 / nb > 0 ? 16 / nb : 1); }
+
+// EMIT of the walk: the hash of window p0 + i + R_.  The vote keeps the common case (no lane has a candidate) to
+// one compare and one vote per window.
+#define PG_SCREEN_EMIT(R_, H_)                                                                                              \
+    {                                                                                                                       \
+        const bool cand_ = (H_) <= L.vmax;                                                                                  \
+        if (__any_sync(0xffffffffu, cand_)) screen_hit(L, scale, off, n_reads, cand_, p0 + i + (R_), (uint32_t)K, (H_), j); \
+    }
+
+// The walk path (k in WalkKs).  Persistent CTAs take chunks of SCREEN_THREADS x W windows of the pool
+// [off[0], off[n_reads]); thread t walks windows [t W, t W + W) of the chunk.  The chunk's bytes, its look-ahead
+// and the 16-byte alignment head are staged in shared memory with 16-byte loads; bytes outside the pool are
+// zeros and are never read from global memory.
+template <int K>
+__global__ void __launch_bounds__(SCREEN_THREADS, 2)
+screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ off, uint64_t n_reads, const ScreenLookup L,
+                   uint32_t lut_stride) {
+    PG_WALK_CONSTANTS;
+    constexpr uint32_t W = screen_span(NB);
+    constexpr uint32_t CHUNK = SCREEN_THREADS * W;
+    constexpr uint32_t STAGE = CHUNK + 128;  // + head (< 16) + the walk's look-ahead (< 4 NB + 20 bytes)
+    constexpr uint32_t nk = W;               // PG_KMER_STEP's bound; unchecked steps never test it
+    __shared__ __align__(16) uint8_t s_in[STAGE];
+    __shared__ __align__(16) uint32_t s_lut[LUT ? 256 : 4];
+    const uint32_t tid = threadIdx.x;
+    if (LUT)
+        for (uint32_t x = tid; x < 256; x += SCREEN_THREADS) s_lut[x] = g_kmix_byte.v[x];
+    const uint64_t lo = off[0], hi = max(off[n_reads], lo);
+    const uint64_t chunks = (hi - lo + CHUNK - 1) / CHUNK;
+    const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
+    const uint32_t lut_base = smem_u32(s_lut);
+
+    for (uint64_t c = blockIdx.x; c < chunks; c += gridDim.x) {
+        const uint64_t P0 = lo + c * CHUNK;
+        const uint32_t head = (uint32_t)((uintptr_t)(bases + P0) & 15u);
+        const int64_t q_base = (int64_t)P0 - (int64_t)head;  // pool position of staged byte 0
+        const uint8_t *g = bases + P0 - head;
+        __syncthreads();  // the previous chunk's walk is done with s_in (and, the first time, s_lut is written)
+        for (uint32_t x = tid; x < STAGE / 16; x += SCREEN_THREADS) {
+            const int64_t q = q_base + 16 * (int64_t)x;
+            uint4 v;
+            if (q >= (int64_t)lo && q + 16 <= (int64_t)hi) {
+                v = __ldg(reinterpret_cast<const uint4 *>(g) + x);
+            } else {
+                uint8_t b[16];
+#pragma unroll
+                for (int t = 0; t < 16; ++t) b[t] = (q + t >= (int64_t)lo && q + t < (int64_t)hi) ? __ldg(g + 16 * x + t) : (uint8_t)0;
+                v = make_uint4(b[0] | b[1] << 8 | b[2] << 16 | (uint32_t)b[3] << 24, b[4] | b[5] << 8 | b[6] << 16 | (uint32_t)b[7] << 24,
+                               b[8] | b[9] << 8 | b[10] << 16 | (uint32_t)b[11] << 24, b[12] | b[13] << 8 | b[14] << 16 | (uint32_t)b[15] << 24);
+            }
+            reinterpret_cast<uint4 *>(s_in)[x] = v;
+        }
+        __syncthreads();
+
+        const uint32_t b0 = head + tid * W;
+        const uint32_t *sw = reinterpret_cast<const uint32_t *>(s_in) + (b0 >> 2);
+        const uint32_t sh = (b0 & 3u) * 8u;
+        const uint8_t *sb = s_in + b0 + 4 * NB;  // tail byte of window i is sb[i]
+        const uint64_t p0 = P0 + tid * W;        // pool position of window 0
+        uint64_t j = ~0ull;
+
+        PG_WALK_PROLOGUE
+        uint32_t i = 0;
+        while (i < W) {  // every lane runs the same steps, so the warp is converged at each window
+#pragma unroll
+            for (int u = 0; u < NB; ++u) PG_KMER_STEP(u, false, PG_SCREEN_EMIT)
+        }
+    }
+}
+
+// Any other k (0 included): window p of the pool is hashed from global memory by thread p of a CTA-uniform
+// grid-stride loop, so that every lane of a warp runs the same iterations.
+__global__ void __launch_bounds__(SCREEN_THREADS)
+screen_generic_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ off, uint64_t n_reads, uint32_t k, const ScreenLookup L) {
+    const uint64_t lo = off[0], hi = max(off[n_reads], lo);
+    const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
+    for (uint64_t base = lo + (uint64_t)blockIdx.x * SCREEN_THREADS; base < hi; base += (uint64_t)gridDim.x * SCREEN_THREADS) {
+        const uint64_t p = base + threadIdx.x;
+        uint32_t h = 0;
+        bool cand = false;
+        if (p < hi && hi - p > k) {
+            const uint8_t *w = bases + p;
+            h = mm3_bytes([w](uint32_t x) { return __ldg(w + x); }, k);
+            cand = h <= L.vmax;
+        }
+        if (__any_sync(0xffffffffu, cand)) {
+            uint64_t j = ~0ull;
+            screen_hit(L, scale, off, n_reads, cand, p, k, h, j);
+        }
+    }
+}
+
+__global__ void screen_values_kernel(const uint64_t *__restrict__ keys, uint64_t total, uint32_t *__restrict__ vals) {
+    for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x)
+        vals[e] = (uint32_t)(keys[e] >> 32);
+}
+
+// dir[b] = the first distinct value index in bucket b or above, for b in [0, nb]; dir[nb] = D
+__global__ void screen_dir_kernel(const uint32_t *__restrict__ vals, uint64_t D, uint32_t nb, uint32_t vmax, uint64_t *__restrict__ dir) {
+    const uint64_t scale = join_bucket_scale(nb, vmax);
+    for (uint64_t d = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; d < D; d += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t b = join_bucket(vals[d], scale, nb);
+        const uint32_t first = d ? join_bucket(vals[d - 1], scale, nb) + 1 : 0;
+        for (uint32_t x = first; x <= b; ++x) dir[x] = d;  // buckets (the previous value's, b]
+        if (d + 1 == D)
+            for (uint64_t x = (uint64_t)b + 1; x <= nb; ++x) dir[x] = D;
+    }
+}
+
+// Entry e of the sorted keys counts when its rank in its run of equal keys (one reference's copies of one value,
+// at most s long) is below the value's pool count; it then appends that count to its reference's segment.
+__global__ void screen_count_kernel(const uint64_t *__restrict__ keys, uint64_t total, uint32_t s, const ScreenLookup L, uint32_t *__restrict__ fill,
+                                    unsigned long long *__restrict__ mult) {
+    const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
+    for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t key = keys[e];
+        uint64_t lo = e >= s - 1 ? e - (s - 1) : 0, hi = e;  // the run's first entry: the lower bound of key in [e - s + 1, e]
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi) >> 1;
+            if (keys[mid] < key) lo = mid + 1;
+            else hi = mid;
+        }
+        uint64_t d = 0;
+        screen_find(L, scale, (uint32_t)(key >> 32), &d);  // every reference value is present
+        const unsigned long long c = L.cnt[d];
+        if (e - lo < c) {
+            const uint32_t id = (uint32_t)key;
+            const uint32_t pos = atomicAdd(&fill[id], 1u);
+            mult[(uint64_t)id * s + pos] = c;
+        }
+    }
+}
+
+// segment r of a sort group of rows [g0, g0 + rows): [r s, r s + fill[g0 + r]) of the group's slots
+__global__ void screen_segments_kernel(const uint32_t *__restrict__ fill, uint64_t rows, uint32_t s, int *__restrict__ beg, int *__restrict__ end) {
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (uint64_t)gridDim.x * blockDim.x) {
+        beg[r] = (int)(r * s);
+        end[r] = (int)(r * s + fill[r]);
+    }
+}
+
+__global__ void screen_final_kernel(const uint32_t *__restrict__ fill, const unsigned long long *__restrict__ sorted, uint64_t n, uint32_t s,
+                                    uint32_t *__restrict__ shared, double *__restrict__ containment, uint64_t *__restrict__ multiplicity) {
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t m = fill[r];
+        if (shared) shared[r] = m;
+        if (containment) containment[r] = (double)m / (double)s;
+        if (multiplicity) multiplicity[r] = m ? sorted[r * s + (m - 1) / 2] : 0;  // the lower median
+    }
+}
+
+ScreenLookup lookup_of(const ScreenIndex &ix) { return ScreenLookup{ix.vals, ix.dir, ix.cnt, ix.nb, ix.vmax}; }
+
+unsigned grid_of(uint64_t work) { return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((work + 255) / 256, (uint64_t)sm_count() * 16)); }
+
+template <int K>
+int launch_screen_walk(const ScreenIndex &ix, const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_reads, cudaStream_t st) {
+    uint64_t grid = 0;  // persistent: the pool's size is on the device, so the grid is what is resident at once
+    { const int rc_ = resident_blocks((const void *)screen_walk_kernel<K>, SCREEN_THREADS, 0, ~0ull, &grid); if (rc_ != PG_OK) return rc_; }
+    screen_walk_kernel<K><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, lookup_of(ix), 4u);
+    PG_LAUNCH_CHECK("screen_walk_kernel");
+    return PG_OK;
+}
+
+}  // namespace
+
+void screen_free(ScreenIndex &ix, cudaStream_t st) {
+    for (void *p : {(void *)ix.keys, (void *)ix.vals, (void *)ix.cnt, (void *)ix.dir})
+        if (p) cudaFreeAsync(p, st);
+    ix = ScreenIndex();
+}
+
+int screen_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, ScreenIndex *out) {
+    ScreenIndex ix;
+    ix.n = n;
+    ix.s = s;
+    const uint64_t total = n * (uint64_t)std::max(s, 0);
+    if (total == 0) {
+        *out = ix;
+        return PG_OK;
+    }
+    int rc = [&]() -> int {
+        StreamScratch tmp(st);
+        uint64_t *d_keys = nullptr;
+        uint32_t *d_v = nullptr, *d_u = nullptr;
+        unsigned long long *d_scal = nullptr;  // [0]: vmax (low word), [1]: D
+        auto nomem = [&](cudaError_t e) { set_error("cudaMallocAsync for the screen failed: %s", cudaGetErrorString(e)); cudaGetLastError(); return PG_ERR_NOMEM; };
+        cudaError_t e;
+        if ((e = tmp.alloc(&d_keys, total)) != cudaSuccess || (e = tmp.alloc(&d_scal, 2)) != cudaSuccess ||
+            (e = cudaMallocAsync(&ix.keys, total * 8, st)) != cudaSuccess)
+            return nomem(e);
+        PG_CUDA(cudaMemsetAsync(d_scal, 0, 16, st));
+        const int krc = launch_batch_keys(d_sk, total, (uint32_t)s, 0, d_keys, (uint32_t *)d_scal, st);
+        if (krc != PG_OK) return krc;
+        size_t bytes = 0;
+        uint8_t *d_cub = nullptr;
+        PG_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, d_keys, ix.keys, total, 0, 64, st));
+        if ((e = tmp.alloc(&d_cub, bytes)) != cudaSuccess) return nomem(e);
+        PG_CUDA(cub::DeviceRadixSort::SortKeys(d_cub, bytes, d_keys, ix.keys, total, 0, 64, st));
+        if ((e = tmp.alloc(&d_v, total)) != cudaSuccess || (e = tmp.alloc(&d_u, total)) != cudaSuccess) return nomem(e);
+        screen_values_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, d_v);
+        PG_LAUNCH_CHECK("screen_values_kernel");
+        bytes = 0;
+        PG_CUDA(cub::DeviceSelect::Unique(nullptr, bytes, d_v, d_u, d_scal + 1, (int64_t)total, st));
+        if ((e = tmp.alloc(&d_cub, bytes)) != cudaSuccess) return nomem(e);
+        PG_CUDA(cub::DeviceSelect::Unique(d_cub, bytes, d_v, d_u, d_scal + 1, (int64_t)total, st));
+        unsigned long long h_scal[2] = {0, 0};
+        PG_CUDA(cudaMemcpyAsync(h_scal, d_scal, 16, cudaMemcpyDeviceToHost, st));
+        PG_CUDA(cudaStreamSynchronize(st));
+        ix.vmax = (uint32_t)h_scal[0];
+        ix.D = h_scal[1];
+        ix.nb = (uint32_t)((ix.D + 3) / 4);
+        if ((e = cudaMallocAsync(&ix.vals, ix.D * 4, st)) != cudaSuccess || (e = cudaMallocAsync(&ix.cnt, ix.D * 8, st)) != cudaSuccess ||
+            (e = cudaMallocAsync(&ix.dir, ((uint64_t)ix.nb + 1) * 8, st)) != cudaSuccess)
+            return nomem(e);
+        PG_CUDA(cudaMemcpyAsync(ix.vals, d_u, ix.D * 4, cudaMemcpyDeviceToDevice, st));
+        PG_CUDA(cudaMemsetAsync(ix.cnt, 0, ix.D * 8, st));
+        screen_dir_kernel<<<grid_of(ix.D), 256, 0, st>>>(ix.vals, ix.D, ix.nb, ix.vmax, ix.dir);
+        PG_LAUNCH_CHECK("screen_dir_kernel");
+        return PG_OK;
+    }();
+    if (rc == PG_OK) { cudaError_t e = cudaStreamSynchronize(st); if (e != cudaSuccess) rc = cuda_fail(e, "screen build", __FILE__, __LINE__); }
+    if (rc != PG_OK) {
+        screen_free(ix, st);
+        cudaStreamSynchronize(st);
+        return rc;
+    }
+    *out = ix;
+    return PG_OK;
+}
+
+int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_reads, cudaStream_t st) {
+    if (n_reads == 0 || ix.D == 0) return PG_OK;
+    int rc = PG_OK;
+    if (with_walk_k(k, [&](auto kk) { rc = launch_screen_walk<decltype(kk)::value>(ix, d_bases, d_off, n_reads, st); })) return rc;
+    uint64_t grid = 0;
+    if ((rc = resident_blocks((const void *)screen_generic_kernel, SCREEN_THREADS, 0, ~0ull, &grid)) != PG_OK) return rc;
+    screen_generic_kernel<<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix));
+    PG_LAUNCH_CHECK("screen_generic_kernel");
+    return PG_OK;
+}
+
+int screen_reset(const ScreenIndex &ix, cudaStream_t st) {
+    if (ix.D) PG_CUDA(cudaMemsetAsync(ix.cnt, 0, ix.D * 8, st));
+    return PG_OK;
+}
+
+int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
+    const uint64_t n = ix.n, s = (uint64_t)std::max(ix.s, 0), total = n * s;
+    if (n == 0 || (!d_shared && !d_cont && !d_mult)) return PG_OK;
+    StreamScratch tmp(st);
+    uint32_t *d_fill = nullptr;
+    unsigned long long *d_m = nullptr, *d_sorted = nullptr;
+    int *d_beg = nullptr, *d_end = nullptr;
+    // the segmented sort counts in int: groups of whole rows of at most INT_MAX slots
+    const uint64_t rows_per = std::max<uint64_t>(1, (uint64_t)INT_MAX / s);
+    const uint64_t group = std::min(rows_per, n);
+    cudaError_t e;
+    if ((e = tmp.alloc(&d_fill, n)) != cudaSuccess || (e = tmp.alloc(&d_m, total)) != cudaSuccess || (e = tmp.alloc(&d_sorted, total)) != cudaSuccess ||
+        (e = tmp.alloc(&d_beg, group)) != cudaSuccess || (e = tmp.alloc(&d_end, group)) != cudaSuccess) {
+        set_error("cudaMallocAsync for the screen results failed: %s", cudaGetErrorString(e));
+        cudaGetLastError();
+        return PG_ERR_NOMEM;
+    }
+    PG_CUDA(cudaMemsetAsync(d_fill, 0, n * 4, st));
+    screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, lookup_of(ix), d_fill, d_m);
+    PG_LAUNCH_CHECK("screen_count_kernel");
+    size_t have = 0;
+    uint8_t *d_cub = nullptr;
+    for (uint64_t g0 = 0; g0 < n; g0 += group) {
+        const uint64_t rows = std::min(group, n - g0);
+        screen_segments_kernel<<<grid_of(rows), 256, 0, st>>>(d_fill + g0, rows, (uint32_t)s, d_beg, d_end);
+        PG_LAUNCH_CHECK("screen_segments_kernel");
+        size_t bytes = 0;
+        PG_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, bytes, d_m + g0 * s, d_sorted + g0 * s, (int)(rows * s), (int)rows, d_beg, d_end, st));
+        if (bytes > have) {
+            if ((e = tmp.alloc(&d_cub, bytes)) != cudaSuccess) {
+                set_error("cudaMallocAsync(%zu) for the screen results failed", bytes);
+                cudaGetLastError();
+                return PG_ERR_NOMEM;
+            }
+            have = bytes;
+        }
+        PG_CUDA(cub::DeviceSegmentedSort::SortKeys(d_cub, bytes, d_m + g0 * s, d_sorted + g0 * s, (int)(rows * s), (int)rows, d_beg, d_end, st));
+    }
+    screen_final_kernel<<<grid_of(n), 256, 0, st>>>(d_fill, d_sorted, n, (uint32_t)s, d_shared, d_cont, d_mult);
+    PG_LAUNCH_CHECK("screen_final_kernel");
+    return PG_OK;
+}
+
+}  // namespace pg

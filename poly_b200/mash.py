@@ -774,6 +774,117 @@ class Clusterer:
                 pass
 
 
+class Screen:
+    """Mash Screen (Ondov et al., Genome Biol 20:232, 2019) on the GPU: which references of a sketch set a pool of
+    reads contains.  Every k-mer window a (*Mash).Sketch would hash (positions 0 .. L - k - 1 of each read, forward
+    strand, raw bytes) is counted into the pool; results() then gives, for each reference r, shared[r] = the sum
+    over hashes v of min(c_r(v), c_pool(v)), containment[r] = shared[r] / s, and multiplicity[r] = the lower median
+    of c_pool(v) over the shared hashes, each counted min(c_r(v), c_pool(v)) times (0 when nothing is shared).
+
+    sketches: [n, s] uint32 (full Go arrays, zero tail included), a CUDA tensor of that shape, or a list of Mash of
+    one SketchSize; k: the k-mer size they were sketched with (not checked, as in the reference).  The pool grows with
+    each add, in any split, and reset() empties it.  Reverse-complement windows are not counted: the references hash
+    the forward strand only.  The screen copies the sketches; it lives on the device current at creation."""
+
+    def __init__(self, sketches, k: int):
+        rows = _sketch_rows(sketches)
+        n, s = int(rows.shape[0]), int(rows.shape[1])
+        if not -(1 << 31) <= k < (1 << 31):
+            raise PolyError(_lib.PG_ERR_ARG, f"k-mer size {k} does not fit 32 bits")
+        h = C.c_void_p()
+        if hasattr(rows, "data_ptr"):
+            import torch
+
+            rc = _lib.lib().pg_mash_screen_create_dev(rows.data_ptr(), n, s, k, torch.cuda.current_stream(rows.device).cuda_stream, C.byref(h))
+        else:
+            rc = _lib.lib().pg_mash_screen_create(rows.ctypes.data, n, s, k, C.byref(h))
+        _index_rc(rc)
+        self._h = h
+        self._dev_used = None
+        self.n, self.s, self.k = n, s, int(k)
+
+    def _live(self):
+        if self._h is None:
+            raise ValueError("the screen is closed")
+        return self._h
+
+    def _sync_dev(self):
+        """Host calls run on the library's own stream: wait for device adds enqueued on torch's streams."""
+        if self._dev_used is not None:
+            import torch
+
+            torch.cuda.synchronize(self._dev_used)
+
+    def add(self, reads) -> None:
+        """Adds host reads to the pool: a list of str / bytes / uint8 arrays, or (bases, offsets) as flatten returns."""
+        h = self._live()
+        if isinstance(reads, tuple) and len(reads) == 2 and isinstance(reads[0], np.ndarray):
+            bases, offsets = np.ascontiguousarray(reads[0], np.uint8), np.ascontiguousarray(reads[1], np.uint64)
+        else:
+            bases, offsets = flatten(reads)
+        n_reads = max(len(offsets) - 1, 0)
+        if n_reads == 0:
+            return
+        if len(bases) == 0:
+            bases = np.zeros(1, np.uint8)
+        self._sync_dev()
+        _lib.check(_lib.lib().pg_mash_screen_add(h, bases.ctypes.data, offsets.ctypes.data, n_reads))
+
+    def add_dev(self, d_bases, d_offsets, stream=None) -> None:
+        """Adds reads already on the device: uint8 bases and int64 (uint64 bits) offsets tensors, read i being
+        d_bases[d_offsets[i] : d_offsets[i + 1]].  Only enqueues, on `stream` (default: the current stream)."""
+        h = self._live()
+        import torch
+
+        n_reads = max(int(d_offsets.numel()) - 1, 0)
+        if n_reads == 0:
+            return
+        st = (stream if stream is not None else torch.cuda.current_stream(d_bases.device)).cuda_stream
+        _lib.check(_lib.lib().pg_mash_screen_add_dev(h, d_bases.data_ptr(), d_offsets.data_ptr(), n_reads, st))
+        self._dev_used = d_bases.device
+
+    def reset(self) -> None:
+        """Empties the pool: the screen then answers as a freshly created one."""
+        h = self._live()
+        self._sync_dev()
+        _lib.check(_lib.lib().pg_mash_screen_reset(h))
+
+    def results(self):
+        """(shared [n] uint32, containment [n] float64, multiplicity [n] uint64) of the pool so far."""
+        h = self._live()
+        self._sync_dev()
+        shared = np.zeros(self.n, np.uint32)
+        cont = np.zeros(self.n, np.float64)
+        mult = np.zeros(self.n, np.uint64)
+        _lib.check(_lib.lib().pg_mash_screen_results(h, shared.ctypes.data, cont.ctypes.data, mult.ctypes.data))
+        return shared, cont, mult
+
+    def identity(self) -> np.ndarray:
+        """Mash Screen's identity estimate containment ** (1 / k), computed on the host from results()."""
+        if self.k <= 0:
+            raise ValueError("identity needs k > 0")
+        return self.results()[1] ** (1.0 / self.k)
+
+    def close(self) -> None:
+        if self._h is not None:
+            self._sync_dev()
+            h, self._h = self._h, None
+            _lib.check(_lib.lib().pg_mash_screen_free(h))
+
+    def __enter__(self) -> "Screen":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        if getattr(self, "_h", None) is not None:
+            try:
+                self.close()
+            except Exception:
+                pass
+
+
 # ---- single-process multi-GPU additions (pg_*_multi; SURVEY.md 8b / 8e) ----------------------------
 def _device_list(devices):
     if devices is None:
