@@ -841,6 +841,17 @@ func (sc *Screen) Results() (shared []uint32, containment []float64, multiplicit
 	return shared[:sc.n], containment[:sc.n], multiplicity[:sc.n], err
 }
 
+// Winners wraps pg_mash_screen_winners: the three arrays of Results after Mash Screen's winner-take-all, each pool
+// hash given to the reference that holds it with the largest first-pass shared count (ties to the smallest index).
+func (sc *Screen) Winners() (shared []uint32, containment []float64, multiplicity []uint64, err error) {
+	shared, containment, multiplicity = make([]uint32, sc.n+1), make([]float64, sc.n+1), make([]uint64, sc.n+1)
+	err = locked(func() C.int {
+		return C.pg_mash_screen_winners(sc.h, (*C.uint32_t)(unsafe.Pointer(&shared[0])), (*C.double)(unsafe.Pointer(&containment[0])),
+			(*C.uint64_t)(unsafe.Pointer(&multiplicity[0])))
+	})
+	return shared[:sc.n], containment[:sc.n], multiplicity[:sc.n], err
+}
+
 // Close wraps pg_mash_screen_free.
 func (sc *Screen) Close() error {
 	if sc.h == nil {

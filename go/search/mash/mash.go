@@ -394,8 +394,9 @@ func (c *Clusterer) Close() error { return c.c.Close() }
 // Screen is Mash Screen (Ondov et al. 2019) on the GPU: which of a set of reference sketches a pool of reads
 // contains.  Add counts every window a Sketch would hash of every read (forward strand, raw bytes) into the pool;
 // Results gives, per reference, Shared = the sum over hashes v of min(c_ref(v), c_pool(v)), Containment = Shared /
-// SketchSize and Multiplicity = the lower median pool count of the shared hashes.  Any split of the pool into Adds
-// gives the same Results, and Reset empties the pool.  Identity is Containment^(1/kmerSize), computed on the host.
+// SketchSize and Multiplicity = the lower median pool count of the shared hashes; Winners gives them after Mash
+// Screen's winner-take-all.  Any split of the pool into Adds gives the same Results and Winners, and Reset empties
+// the pool.  Identity is Containment^(1/kmerSize), computed on the host.
 // Call Close when done.
 type Screen struct {
 	sc *polyb200.Screen
@@ -442,7 +443,18 @@ func (s *Screen) Reset() error { return s.sc.Reset() }
 
 // Results returns one ScreenResult per reference, in the order given to NewScreen.
 func (s *Screen) Results() ([]ScreenResult, error) {
-	shared, cont, mult, err := s.sc.Results()
+	return s.resultsOf(s.sc.Results())
+}
+
+// Winners returns one ScreenResult per reference after Mash Screen's winner-take-all (mash screen -w): each pool
+// hash is given to the reference that holds it with the largest Shared of Results, a tie to the smallest index, and
+// every field is recomputed over the hashes a reference won.  Sibling strains of the one a pool came from then stop
+// reporting the hashes it explains better.
+func (s *Screen) Winners() ([]ScreenResult, error) {
+	return s.resultsOf(s.sc.Winners())
+}
+
+func (s *Screen) resultsOf(shared []uint32, cont []float64, mult []uint64, err error) ([]ScreenResult, error) {
 	if err != nil {
 		return nil, err
 	}

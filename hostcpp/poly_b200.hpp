@@ -527,7 +527,8 @@ public:
 // Mash Screen on the device (pg_mash_screen): which references of a sketch set a pool of reads contains.  Add hashes
 // every window a Sketch would hash of every read into the pool; Results gives, per reference, Shared = sum over v of
 // min(c_r(v), c_pool(v)), Containment = Shared / s and Multiplicity = the lower median pool count of the shared
-// hashes.  Any split of the pool into Adds gives the same Results; Reset empties the pool.
+// hashes; Winners gives them after Mash Screen's winner-take-all.  Any split of the pool into Adds gives the same
+// Results and Winners; Reset empties the pool.
 class Screen {
     pg_mash_screen *h_ = nullptr;
     size_t n_ = 0;
@@ -560,6 +561,16 @@ public:
         r.Containment.resize(n_);
         r.Multiplicity.resize(n_);
         check(pg_mash_screen_results(h_, r.Shared.data(), r.Containment.data(), r.Multiplicity.data()));
+        return r;
+    }
+    // Mash Screen's winner-take-all: each pool hash goes to the reference that holds it with the largest Shared of
+    // Results (ties to the smallest index), and the three arrays are recomputed over the hashes each one won
+    Result Winners() const {
+        Result r;
+        r.Shared.resize(n_);
+        r.Containment.resize(n_);
+        r.Multiplicity.resize(n_);
+        check(pg_mash_screen_winners(h_, r.Shared.data(), r.Containment.data(), r.Multiplicity.data()));
         return r;
     }
     // Mash Screen's identity estimate, Containment^(1/k), on the host

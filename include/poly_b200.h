@@ -536,21 +536,34 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c);
  *     floor((m - 1) / 2) of m in ascending order) of the multiset in which each v with c_pool(v) >= 1 contributes
  *     the value c_pool(v) min(c_r(v), c_pool(v)) times; 0 when shared[r] == 0.  Mash Screen's identity,
  *     containment^(1/k), is left to the caller.
- *   - Split invariance: for any split of a pool into adds (empty and one-read adds included) the results equal
- *     those of one add of the concatenation; after a reset the screen answers as a freshly created one.
+ *   - Winners (winners, winners_dev), Mash Screen's winner-take-all (mash screen -w): each value v with
+ *     c_pool(v) >= 1 is given to one of its contenders, the references r with c_r(v) >= 1: the one with the largest
+ *     shared[r] of results (the first pass), a tie to the smallest reference index.  All references of a screen have
+ *     one s, so this is Mash's order by identity (shared / s)^(1/k), exact for every k (0 included); Mash breaks its
+ *     ties by genome length, which a screen does not hold, so the tie rule is this library's own.  The reallocation
+ *     is done once, from the first-pass scores, as in Mash.  winners then returns the three arrays of results over
+ *     the values each reference won: shared_w[r] = sum over v won by r of min(c_r(v), c_pool(v)) (<= shared[r]),
+ *     containment_w[r] = shared_w[r] / s, multiplicity_w[r] = the lower median of c_pool(v) over the won values,
+ *     each counted min(c_r(v), c_pool(v)) times, 0 when r won nothing.  Zero-tail words take part as any other word
+ *     (the value 0 has every zero-tailed reference as a contender).  A reference that shares no pool value with
+ *     another reference keeps its results, and with n == 1 winners equals results.  The output does not depend on
+ *     the order of the device's atomics, and winners leaves the screen as it was.
+ *   - Split invariance: for any split of a pool into adds (empty and one-read adds included) the results and the
+ *     winners equal those of one add of the concatenation; after a reset the screen answers as a freshly created one.
  *   - Errors, checked in this order: a null screen or out is PG_ERR_ARG (no device is needed); k < 0 is
  *     PG_ERR_ARG, as for the sketch calls; s <= 0 with n > 0 is PG_ERR_PANIC, as for index create; n > 2^32 - 1 is
  *     PG_ERR_ARG (the keys hold 32-bit ids); a null buffer is PG_ERR_ARG.  n == 0 and n_reads == 0 are valid (an
  *     add of no read changes nothing and needs no buffer).  Offsets that decrease in a host add are PG_ERR_ARG.
- *     Any output of results may be NULL.  PG_ERR_NOMEM when device memory runs out.  After any error the screen
+ *     Any output of results or winners may be NULL.  PG_ERR_NOMEM when device memory runs out.  After any error the screen
  *     holds what it held before.
  *   - _dev offsets: add_dev trusts d_offsets as pg_mash_sketch_batch_dev does.  With non-decreasing offsets it
  *     counts exactly the windows above.  Offsets that decrease give unspecified counts, but no byte outside
  *     [d_offsets[0], d_offsets[n_reads]) is read and no memory outside the screen is written.
  *   - Ownership, device and threads, as for pg_mash_index: create copies everything (no caller pointer is kept)
  *     and the screen lives on the device current at creation.  Each screen has a reader-writer lock: add, add_dev
- *     and reset hold it exclusively, results and results_dev shared, while they enqueue.  The host calls
- *     synchronise (create also to size its buffers).  add_dev and results_dev only enqueue on `stream`; add_dev
+ *     and reset hold it exclusively, results, winners and their _dev forms shared, while they enqueue.  The host
+ *     calls synchronise (create also to size its buffers).  add_dev, results_dev and winners_dev only enqueue on
+ *     `stream`; add_dev
  *     makes no host decision that depends on the data.  Work enqueued by _dev calls on different streams is ordered
  *     by the caller: results see an add_dev only once its stream is ordered before them (a host call runs on the
  *     library's own stream), and freeing or resetting a screen while a _dev call on it is still enqueued on an
@@ -560,8 +573,8 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c);
  *   - Device memory: with D distinct values among the n s words, a screen holds 8 n s bytes of sorted keys,
  *     4 D of values, 8 D of counts and 8 (ceil(D / 4) + 1) of directory.  Create adds, while it runs, 8 n s bytes
  *     of unsorted keys, 8 n s of values and CUB's sort storage (the host call also stages 4 n s bytes of sketches);
- *     results add 16 n s bytes of multiplicity slots, 4 n of counts and CUB's segmented-sort storage; the host
- *     add stages the pool's bytes and offsets. */
+ *     results add 16 n s bytes of multiplicity slots, 4 n of counts and CUB's segmented-sort storage; winners adds
+ *     to those 8 D bytes of votes; the host add stages the pool's bytes and offsets. */
 typedef struct pg_mash_screen pg_mash_screen;
 int pg_mash_screen_create(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, pg_mash_screen **out);
 int pg_mash_screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, void *stream, pg_mash_screen **out);
@@ -570,6 +583,9 @@ int pg_mash_screen_add_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uin
 int pg_mash_screen_reset(pg_mash_screen *sc);
 int pg_mash_screen_results(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity);
 int pg_mash_screen_results_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity,
+                               void *stream);
+int pg_mash_screen_winners(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity);
+int pg_mash_screen_winners_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity,
                                void *stream);
 int pg_mash_screen_free(pg_mash_screen *sc);
 

@@ -634,6 +634,36 @@ static int screen_create_check(const void *sketches, uint64_t n, int32_t s, int3
 
 static pg_mash_screen *screen_new(int32_t k, const ScreenIndex &ix) { return new pg_mash_screen{cur_ctx()->device, k, ix}; }
 
+// results and winners: the same rules, locking and copies around a different tally
+using ScreenTally = int (*)(const ScreenIndex &, uint32_t *, double *, uint64_t *, cudaStream_t);
+
+static int screen_tally_host(const pg_mash_screen *sc, ScreenTally tally, uint32_t *shared, double *containment, uint64_t *multiplicity) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::shared_lock<std::shared_mutex> lk(sc->rw);
+    const uint64_t n = sc->ix.n;
+    if (n == 0 || (!shared && !containment && !multiplicity)) return PG_OK;
+    HostCall c;
+    uint32_t *d_sh = shared ? c.alloc<uint32_t>(n) : nullptr;
+    double *d_c = containment ? c.alloc<double>(n) : nullptr;
+    uint64_t *d_m = multiplicity ? c.alloc<uint64_t>(n) : nullptr;
+    if ((rc = c.error()) || (rc = tally(sc->ix, d_sh, d_c, d_m, c.st))) return rc;
+    c.download(shared, d_sh, n);
+    c.download(containment, d_c, n);
+    c.download(multiplicity, d_m, n);
+    return c.finish();
+}
+
+static int screen_tally_dev(const pg_mash_screen *sc, ScreenTally tally, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity,
+                            void *stream) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    int rc = use_device(sc->device);
+    if (rc != PG_OK) return rc;
+    std::shared_lock<std::shared_mutex> lk(sc->rw);
+    return tally(sc->ix, d_shared, d_containment, d_multiplicity, (cudaStream_t)stream);
+}
+
 }  // namespace
 }  // namespace pg
 
@@ -1373,29 +1403,19 @@ int pg_mash_screen_reset(pg_mash_screen *sc) {
 }
 
 int pg_mash_screen_results(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity) {
-    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
-    int rc = use_device(sc->device);
-    if (rc != PG_OK) return rc;
-    std::shared_lock<std::shared_mutex> lk(sc->rw);
-    const uint64_t n = sc->ix.n;
-    if (n == 0 || (!shared && !containment && !multiplicity)) return PG_OK;
-    HostCall c;
-    uint32_t *d_sh = shared ? c.alloc<uint32_t>(n) : nullptr;
-    double *d_c = containment ? c.alloc<double>(n) : nullptr;
-    uint64_t *d_m = multiplicity ? c.alloc<uint64_t>(n) : nullptr;
-    if ((rc = c.error()) || (rc = screen_results(sc->ix, d_sh, d_c, d_m, c.st))) return rc;
-    c.download(shared, d_sh, n);
-    c.download(containment, d_c, n);
-    c.download(multiplicity, d_m, n);
-    return c.finish();
+    return screen_tally_host(sc, screen_results, shared, containment, multiplicity);
 }
 
 int pg_mash_screen_results_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity, void *stream) {
-    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
-    int rc = use_device(sc->device);
-    if (rc != PG_OK) return rc;
-    std::shared_lock<std::shared_mutex> lk(sc->rw);
-    return screen_results(sc->ix, d_shared, d_containment, d_multiplicity, (cudaStream_t)stream);
+    return screen_tally_dev(sc, screen_results, d_shared, d_containment, d_multiplicity, stream);
+}
+
+int pg_mash_screen_winners(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity) {
+    return screen_tally_host(sc, screen_winners, shared, containment, multiplicity);
+}
+
+int pg_mash_screen_winners_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity, void *stream) {
+    return screen_tally_dev(sc, screen_winners, d_shared, d_containment, d_multiplicity, stream);
 }
 
 int pg_mash_screen_free(pg_mash_screen *sc) {

@@ -321,6 +321,9 @@ int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint6
 int screen_reset(const ScreenIndex &ix, cudaStream_t st);
 // shared, containment and multiplicity of every reference (any output may be NULL); only enqueues
 int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st);
+// the same three arrays over the words each value's winner-take-all vote gave their reference: a value the pool holds
+// goes to the reference that holds it with the largest first-pass shared (ties to the smallest id); only enqueues
+int screen_winners(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st);
 void screen_free(ScreenIndex &ix, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).

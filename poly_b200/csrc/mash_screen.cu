@@ -18,6 +18,9 @@
 // Results (screen_results): one pass over the sorted keys.  The c_r(v) words of reference r equal to v are one
 // run of equal keys, and the first min(c_r(v), c_pool(v)) of them count; each counted word appends c_pool(v)
 // to its reference's segment of s slots.  A CUB segmented sort of the segments then gives the lower median.
+// Winners (screen_winners, Mash Screen's winner-take-all): the same count pass without the segments gives each
+// reference's first-pass shared; then every value the pool holds votes among its contenders, one run of keys
+// (screen_vote_kernel), and the count pass above runs again over the won words only.
 #include <algorithm>
 #include <climits>
 
@@ -194,10 +197,15 @@ __global__ void screen_dir_kernel(const uint32_t *__restrict__ vals, uint64_t D,
     }
 }
 
+// The winner of a vote word fill << 32 | (0xFFFFFFFF - id): its largest value has the largest first-pass shared,
+// ties to the smallest id.
+__device__ __forceinline__ uint32_t vote_id(unsigned long long w) { return 0xFFFFFFFFu - (uint32_t)w; }
+
 // Entry e of the sorted keys counts when its rank in its run of equal keys (one reference's copies of one value,
-// at most s long) is below the value's pool count; it then appends that count to its reference's segment.
-__global__ void screen_count_kernel(const uint64_t *__restrict__ keys, uint64_t total, uint32_t s, const ScreenLookup L, uint32_t *__restrict__ fill,
-                                    unsigned long long *__restrict__ mult) {
+// at most s long) is below the value's pool count, and, given a vote (win != null), when its reference won the
+// value; it then appends that count to its reference's segment (mult != null).
+__global__ void screen_count_kernel(const uint64_t *__restrict__ keys, uint64_t total, uint32_t s, const ScreenLookup L,
+                                    const unsigned long long *__restrict__ win, uint32_t *__restrict__ fill, unsigned long long *__restrict__ mult) {
     const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
     for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t key = keys[e];
@@ -210,11 +218,43 @@ __global__ void screen_count_kernel(const uint64_t *__restrict__ keys, uint64_t 
         uint64_t d = 0;
         screen_find(L, scale, (uint32_t)(key >> 32), &d);  // every reference value is present
         const unsigned long long c = L.cnt[d];
-        if (e - lo < c) {
-            const uint32_t id = (uint32_t)key;
+        const uint32_t id = (uint32_t)key;
+        if (e - lo < c && (!win || vote_id(win[d]) == id)) {
             const uint32_t pos = atomicAdd(&fill[id], 1u);
-            mult[(uint64_t)id * s + pos] = c;
+            if (mult) mult[(uint64_t)id * s + pos] = c;
         }
+    }
+}
+
+// The winner-take-all vote.  The first entry of each (value, id) run whose value the pool holds proposes
+// fill[id] << 32 | (0xFFFFFFFF - id) for the value; win[d] keeps the largest, whatever the order of the atomics.
+// A value's keys are adjacent, so the lanes of a warp that hold it are consecutive: they reduce to one proposal
+// (a segmented max over shuffles) before one atomic, and a proposal no larger than win[d] as read is dropped (win
+// only grows, so a stale read drops nothing that could win).  A value held by every reference thus costs at most one
+// atomic per warp, and far fewer once its leader is in.
+__global__ void screen_vote_kernel(const uint64_t *__restrict__ keys, uint64_t total, const ScreenLookup L, const uint32_t *__restrict__ fill,
+                                   unsigned long long *win) {
+    const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
+    const int lane = (int)(threadIdx.x & 31);
+    // a warp-uniform trip count: every lane reaches the shuffles
+    for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x; base < total; base += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t e = base + threadIdx.x;
+        uint64_t d = ~0ull;  // past the end: a segment of its own, after every value
+        unsigned long long p = 0;
+        if (e < total) {
+            const uint64_t key = keys[e];
+            screen_find(L, scale, (uint32_t)(key >> 32), &d);
+            const uint32_t id = (uint32_t)key;
+            if (L.cnt[d] && (e == 0 || keys[e - 1] != key)) p = (unsigned long long)fill[id] << 32 | (0xFFFFFFFFu - id);
+        }
+        const unsigned peers = __match_any_sync(0xffffffffu, d);
+        const int last = 31 - __clz(peers);
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {  // lane i ends with the max over lanes [i, last]
+            const unsigned long long q = __shfl_down_sync(0xffffffffu, p, o);
+            if (lane + o <= last) p = max(p, q);
+        }
+        if (p && lane == __ffs(peers) - 1 && p > win[d]) atomicMax(&win[d], p);
     }
 }
 
@@ -332,25 +372,38 @@ int screen_reset(const ScreenIndex &ix, cudaStream_t st) {
     return PG_OK;
 }
 
-int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
+namespace {
+
+// The tail of results and winners: the count pass over the words that count (all of them, or given a vote the won
+// ones), the segmented sort of each reference's pool counts and the final arrays.
+int screen_tally(const ScreenIndex &ix, bool winners, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
     const uint64_t n = ix.n, s = (uint64_t)std::max(ix.s, 0), total = n * s;
     if (n == 0 || (!d_shared && !d_cont && !d_mult)) return PG_OK;
     StreamScratch tmp(st);
     uint32_t *d_fill = nullptr;
-    unsigned long long *d_m = nullptr, *d_sorted = nullptr;
+    unsigned long long *d_m = nullptr, *d_sorted = nullptr, *d_win = nullptr;
     int *d_beg = nullptr, *d_end = nullptr;
     // the segmented sort counts in int: groups of whole rows of at most INT_MAX slots
     const uint64_t rows_per = std::max<uint64_t>(1, (uint64_t)INT_MAX / s);
     const uint64_t group = std::min(rows_per, n);
     cudaError_t e;
     if ((e = tmp.alloc(&d_fill, n)) != cudaSuccess || (e = tmp.alloc(&d_m, total)) != cudaSuccess || (e = tmp.alloc(&d_sorted, total)) != cudaSuccess ||
-        (e = tmp.alloc(&d_beg, group)) != cudaSuccess || (e = tmp.alloc(&d_end, group)) != cudaSuccess) {
+        (e = tmp.alloc(&d_beg, group)) != cudaSuccess || (e = tmp.alloc(&d_end, group)) != cudaSuccess ||
+        (winners && (e = tmp.alloc(&d_win, ix.D)) != cudaSuccess)) {
         set_error("cudaMallocAsync for the screen results failed: %s", cudaGetErrorString(e));
         cudaGetLastError();
         return PG_ERR_NOMEM;
     }
     PG_CUDA(cudaMemsetAsync(d_fill, 0, n * 4, st));
-    screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, lookup_of(ix), d_fill, d_m);
+    if (winners) {  // the first pass's shared of every reference, then the vote
+        PG_CUDA(cudaMemsetAsync(d_win, 0, ix.D * 8, st));
+        screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, lookup_of(ix), nullptr, d_fill, nullptr);
+        PG_LAUNCH_CHECK("screen_count_kernel");
+        screen_vote_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, lookup_of(ix), d_fill, d_win);
+        PG_LAUNCH_CHECK("screen_vote_kernel");
+        PG_CUDA(cudaMemsetAsync(d_fill, 0, n * 4, st));
+    }
+    screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, lookup_of(ix), d_win, d_fill, d_m);
     PG_LAUNCH_CHECK("screen_count_kernel");
     size_t have = 0;
     uint8_t *d_cub = nullptr;
@@ -373,6 +426,16 @@ int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, ui
     screen_final_kernel<<<grid_of(n), 256, 0, st>>>(d_fill, d_sorted, n, (uint32_t)s, d_shared, d_cont, d_mult);
     PG_LAUNCH_CHECK("screen_final_kernel");
     return PG_OK;
+}
+
+}  // namespace
+
+int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
+    return screen_tally(ix, false, d_shared, d_cont, d_mult, st);
+}
+
+int screen_winners(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
+    return screen_tally(ix, true, d_shared, d_cont, d_mult, st);
 }
 
 }  // namespace pg

@@ -859,6 +859,19 @@ class Screen:
         _lib.check(_lib.lib().pg_mash_screen_results(h, shared.ctypes.data, cont.ctypes.data, mult.ctypes.data))
         return shared, cont, mult
 
+    def winners(self):
+        """Mash Screen's winner-take-all (mash screen -w): each pool hash goes to the reference that holds it with
+        the largest first-pass shared (ties to the smallest index), and the (shared, containment, multiplicity) of
+        results() are recomputed over the hashes each reference won.  A strain's siblings then stop reporting the
+        hashes it explains better.  The screen is left as it was."""
+        h = self._live()
+        self._sync_dev()
+        shared = np.zeros(self.n, np.uint32)
+        cont = np.zeros(self.n, np.float64)
+        mult = np.zeros(self.n, np.uint64)
+        _lib.check(_lib.lib().pg_mash_screen_winners(h, shared.ctypes.data, cont.ctypes.data, mult.ctypes.data))
+        return shared, cont, mult
+
     def identity(self) -> np.ndarray:
         """Mash Screen's identity estimate containment ** (1 / k), computed on the host from results()."""
         if self.k <= 0:
