@@ -795,25 +795,34 @@ func (c *Clusterer) Close() error {
 	return locked(func() C.int { return C.pg_mash_clusterer_free(h) })
 }
 
-// Screen wraps a pg_mash_screen: a reference sketch set and a pool of reads on the device of the calling thread.
-// Close must not run while another call on it is in flight.
+// Screen wraps a pg_mash_screen: a reference sketch set and one pool of reads per sample on the device of the
+// calling thread.  Close must not run while another call on it is in flight.
 type Screen struct {
-	h *C.pg_mash_screen
-	n int
+	h       *C.pg_mash_screen
+	n       int
+	samples int
 }
 
 // NewScreen wraps pg_mash_screen_create for n references of s words each (full arrays, zero tails included) and
 // k-mer size k.
-func NewScreen(sketches []uint32, n, s, k int) (*Screen, error) {
+func NewScreen(sketches []uint32, n, s, k int) (*Screen, error) { return NewScreenSamples(sketches, n, s, k, 1) }
+
+// NewScreenSamples wraps pg_mash_screen_create_samples: NewScreen with one pool for each of `samples` samples.
+func NewScreenSamples(sketches []uint32, n, s, k, samples int) (*Screen, error) {
 	var h *C.pg_mash_screen
 	var p *C.uint32_t
 	if len(sketches) > 0 {
 		p = (*C.uint32_t)(unsafe.Pointer(&sketches[0]))
 	}
-	if err := locked(func() C.int { return C.pg_mash_screen_create(p, C.uint64_t(n), C.int32_t(s), C.int32_t(k), &h) }); err != nil {
+	if samples < 0 || uint64(samples) > 0xffffffff {
+		return nil, errors.New("polyb200: sample count does not fit 32 bits")
+	}
+	if err := locked(func() C.int {
+		return C.pg_mash_screen_create_samples(p, C.uint64_t(n), C.int32_t(s), C.int32_t(k), C.uint32_t(samples), &h)
+	}); err != nil {
 		return nil, err
 	}
-	return &Screen{h: h, n: n}, nil
+	return &Screen{h: h, n: n, samples: samples}, nil
 }
 
 // Add wraps pg_mash_screen_add: every window of the reads is counted into the pool.
@@ -827,7 +836,22 @@ func (sc *Screen) Add(reads []string) error {
 	})
 }
 
-// Reset wraps pg_mash_screen_reset: the pool is emptied.
+// AddSamples wraps pg_mash_screen_add_samples: every window of reads[i] is counted into the pool of sample ids[i].
+func (sc *Screen) AddSamples(reads []string, ids []uint32) error {
+	if len(ids) != len(reads) {
+		return errors.New("polyb200: one sample id per read")
+	}
+	if len(reads) == 0 {
+		return nil
+	}
+	bases, offsets := Flatten(reads)
+	return locked(func() C.int {
+		return C.pg_mash_screen_add_samples(sc.h, (*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])),
+			(*C.uint32_t)(unsafe.Pointer(&ids[0])), C.uint64_t(len(reads)))
+	})
+}
+
+// Reset wraps pg_mash_screen_reset: the pool of every sample is emptied.
 func (sc *Screen) Reset() error { return locked(func() C.int { return C.pg_mash_screen_reset(sc.h) }) }
 
 // Results wraps pg_mash_screen_results: per reference, the shared hash count, the containment and the median
@@ -850,6 +874,34 @@ func (sc *Screen) Winners() (shared []uint32, containment []float64, multiplicit
 			(*C.uint64_t)(unsafe.Pointer(&multiplicity[0])))
 	})
 	return shared[:sc.n], containment[:sc.n], multiplicity[:sc.n], err
+}
+
+// ResultsSamples wraps pg_mash_screen_results_samples: the arrays of Results for samples [first, first+count),
+// row-major (element (q-first)*n + r).
+func (sc *Screen) ResultsSamples(first, count int) (shared []uint32, containment []float64, multiplicity []uint64, err error) {
+	return sc.table(true, first, count)
+}
+
+// WinnersSamples wraps pg_mash_screen_winners_samples: the arrays of Winners for samples [first, first+count), each
+// sample voting alone, row-major as ResultsSamples.
+func (sc *Screen) WinnersSamples(first, count int) (shared []uint32, containment []float64, multiplicity []uint64, err error) {
+	return sc.table(false, first, count)
+}
+
+func (sc *Screen) table(results bool, first, count int) (shared []uint32, containment []float64, multiplicity []uint64, err error) {
+	if first < 0 || count < 0 || first+count > sc.samples {
+		return nil, nil, nil, errors.New("polyb200: sample rows out of range")
+	}
+	m := sc.n * count
+	shared, containment, multiplicity = make([]uint32, m+1), make([]float64, m+1), make([]uint64, m+1)
+	err = locked(func() C.int {
+		sh, c, mu := (*C.uint32_t)(unsafe.Pointer(&shared[0])), (*C.double)(unsafe.Pointer(&containment[0])), (*C.uint64_t)(unsafe.Pointer(&multiplicity[0]))
+		if results {
+			return C.pg_mash_screen_results_samples(sc.h, C.uint32_t(first), C.uint32_t(count), sh, c, mu)
+		}
+		return C.pg_mash_screen_winners_samples(sc.h, C.uint32_t(first), C.uint32_t(count), sh, c, mu)
+	})
+	return shared[:m], containment[:m], multiplicity[:m], err
 }
 
 // Close wraps pg_mash_screen_free.

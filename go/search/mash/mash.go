@@ -396,7 +396,10 @@ func (c *Clusterer) Close() error { return c.c.Close() }
 // Results gives, per reference, Shared = the sum over hashes v of min(c_ref(v), c_pool(v)), Containment = Shared /
 // SketchSize and Multiplicity = the lower median pool count of the shared hashes; Winners gives them after Mash
 // Screen's winner-take-all.  Any split of the pool into Adds gives the same Results and Winners, and Reset empties
-// the pool.  Identity is Containment^(1/kmerSize), computed on the host.
+// the pool.  Identity is Containment^(1/kmerSize), computed on the host.  A screen made by NewScreenSamples holds one
+// pool per sample of a multiplexed run: AddSamples tags each read with its sample, and ResultsSamples and
+// WinnersSamples answer, for each sample, what a screen fed only that sample's reads would answer.  Add counts into
+// sample 0, and Results and Winners answer for it.
 // Call Close when done.
 type Screen struct {
 	sc *polyb200.Screen
@@ -413,7 +416,10 @@ type ScreenResult struct {
 
 // NewScreen prepares a screen against refs, which must share one SketchSize, for k-mers of kmerSize (the size they
 // were sketched with; it is not checked, as Similarity does not check it).
-func NewScreen(refs []*Mash, kmerSize int) (*Screen, error) {
+func NewScreen(refs []*Mash, kmerSize int) (*Screen, error) { return NewScreenSamples(refs, kmerSize, 1) }
+
+// NewScreenSamples is NewScreen with one pool for each of `samples` samples (samples >= 1).
+func NewScreenSamples(refs []*Mash, kmerSize int, samples int) (*Screen, error) {
 	s := 0
 	if len(refs) > 0 {
 		s = refs[0].SketchSize
@@ -428,7 +434,7 @@ func NewScreen(refs []*Mash, kmerSize int) (*Screen, error) {
 	if len(refs) > 0 && s <= 0 {
 		panic("runtime error: index out of range [-1]") // Similarity on a sketch of size 0 would
 	}
-	sc, err := polyb200.NewScreen(flat, len(refs), s, kmerSize)
+	sc, err := polyb200.NewScreenSamples(flat, len(refs), s, kmerSize, samples)
 	if err != nil {
 		return nil, err
 	}
@@ -438,7 +444,19 @@ func NewScreen(refs []*Mash, kmerSize int) (*Screen, error) {
 // Add counts the windows of reads into the pool.
 func (s *Screen) Add(reads []string) error { return s.sc.Add(reads) }
 
-// Reset empties the pool.
+// AddSamples counts the windows of reads[i] into the pool of sample samples[i].
+func (s *Screen) AddSamples(reads []string, samples []int) error {
+	ids := make([]uint32, len(samples))
+	for i, q := range samples {
+		if q < 0 || uint64(q) > 0xffffffff {
+			return errors.New("mash: sample id does not fit 32 bits")
+		}
+		ids[i] = uint32(q)
+	}
+	return s.sc.AddSamples(reads, ids)
+}
+
+// Reset empties the pool of every sample.
 func (s *Screen) Reset() error { return s.sc.Reset() }
 
 // Results returns one ScreenResult per reference, in the order given to NewScreen.
@@ -452,6 +470,33 @@ func (s *Screen) Results() ([]ScreenResult, error) {
 // reporting the hashes it explains better.
 func (s *Screen) Winners() ([]ScreenResult, error) {
 	return s.resultsOf(s.sc.Winners())
+}
+
+// ResultsSamples returns, for each sample q in [first, first+count), one ScreenResult per reference.
+func (s *Screen) ResultsSamples(first, count int) ([][]ScreenResult, error) {
+	return s.rowsOf(count)(s.sc.ResultsSamples(first, count))
+}
+
+// WinnersSamples returns Winners for each sample q in [first, first+count); every sample votes alone.
+func (s *Screen) WinnersSamples(first, count int) ([][]ScreenResult, error) {
+	return s.rowsOf(count)(s.sc.WinnersSamples(first, count))
+}
+
+func (s *Screen) rowsOf(count int) func([]uint32, []float64, []uint64, error) ([][]ScreenResult, error) {
+	return func(shared []uint32, cont []float64, mult []uint64, err error) ([][]ScreenResult, error) {
+		flat, err := s.resultsOf(shared, cont, mult, err)
+		if err != nil {
+			return nil, err
+		}
+		out := make([][]ScreenResult, count)
+		if count > 0 {
+			n := len(flat) / count
+			for q := range out {
+				out[q] = flat[q*n : (q+1)*n]
+			}
+		}
+		return out, nil
+	}
 }
 
 func (s *Screen) resultsOf(shared []uint32, cont []float64, mult []uint64, err error) ([]ScreenResult, error) {

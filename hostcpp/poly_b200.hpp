@@ -528,17 +528,19 @@ public:
 // every window a Sketch would hash of every read into the pool; Results gives, per reference, Shared = sum over v of
 // min(c_r(v), c_pool(v)), Containment = Shared / s and Multiplicity = the lower median pool count of the shared
 // hashes; Winners gives them after Mash Screen's winner-take-all.  Any split of the pool into Adds gives the same
-// Results and Winners; Reset empties the pool.
+// Results and Winners; Reset empties the pool.  A screen of several samples holds one pool per sample over the
+// one reference set: AddSamples tags each read with its sample, and row q of ResultsSamples / WinnersSamples is what
+// a one-sample screen fed only sample q's reads answers.  Add counts into sample 0; Results and Winners give row 0.
 class Screen {
     pg_mash_screen *h_ = nullptr;
     size_t n_ = 0;
     int k_ = 0;
 
 public:
-    Screen(const std::vector<Mash> &refs, int kmerSize) : n_(refs.size()), k_(kmerSize) {
+    Screen(const std::vector<Mash> &refs, int kmerSize, uint32_t samples = 1) : n_(refs.size()), k_(kmerSize) {
         int s;
         const std::vector<uint32_t> flat = detail::FlatRows(refs, "references", &s);
-        int rc = pg_mash_screen_create(flat.data(), refs.size(), s, kmerSize, &h_);
+        int rc = pg_mash_screen_create_samples(flat.data(), refs.size(), s, kmerSize, samples, &h_);
         if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
         check(rc);
     }
@@ -548,6 +550,12 @@ public:
     void Add(const std::vector<std::string> &reads) {
         const Flat f(reads);
         check(pg_mash_screen_add(h_, f.bases.data(), f.offsets.data(), reads.size()));
+    }
+    // read i goes to sample ids[i]; an id that is not a sample is an error and nothing is added
+    void AddSamples(const std::vector<std::string> &reads, const std::vector<uint32_t> &ids) {
+        if (ids.size() != reads.size()) throw std::invalid_argument("one sample id per read");
+        const Flat f(reads);
+        check(pg_mash_screen_add_samples(h_, f.bases.data(), f.offsets.data(), ids.data(), reads.size()));
     }
     void Reset() { check(pg_mash_screen_reset(h_)); }
     struct Result {
@@ -573,10 +581,29 @@ public:
         check(pg_mash_screen_winners(h_, r.Shared.data(), r.Containment.data(), r.Multiplicity.data()));
         return r;
     }
+    // Results and Winners of samples [first, first + count), one Result per sample, from one call each
+    std::vector<Result> ResultsSamples(uint32_t first, uint32_t count) const { return Table(pg_mash_screen_results_samples, first, count); }
+    std::vector<Result> WinnersSamples(uint32_t first, uint32_t count) const { return Table(pg_mash_screen_winners_samples, first, count); }
     // Mash Screen's identity estimate, Containment^(1/k), on the host
     std::vector<double> Identity() const {
         std::vector<double> out = Results().Containment;
         for (double &c : out) c = std::pow(c, 1.0 / k_);
+        return out;
+    }
+
+private:
+    using TableFn = int (*)(const pg_mash_screen *, uint32_t, uint32_t, uint32_t *, double *, uint64_t *);
+    std::vector<Result> Table(TableFn fn, uint32_t first, uint32_t count) const {
+        std::vector<uint32_t> shared(n_ * count);
+        std::vector<double> cont(n_ * count);
+        std::vector<uint64_t> mult(n_ * count);
+        check(fn(h_, first, count, shared.data(), cont.data(), mult.data()));
+        std::vector<Result> out(count);
+        for (uint32_t q = 0; q < count; ++q) {
+            out[q].Shared.assign(shared.begin() + q * n_, shared.begin() + (q + 1) * n_);
+            out[q].Containment.assign(cont.begin() + q * n_, cont.begin() + (q + 1) * n_);
+            out[q].Multiplicity.assign(mult.begin() + q * n_, mult.begin() + (q + 1) * n_);
+        }
         return out;
     }
 };

@@ -571,10 +571,31 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c);
  *   - Counter width: pool counts are 64-bit, so a pool of more than 2^32 windows with one hash stays exact.
  *     multiplicity is uint64; shared <= s.
  *   - Device memory: with D distinct values among the n s words, a screen holds 8 n s bytes of sorted keys,
- *     4 D of values, 8 D of counts and 8 (ceil(D / 4) + 1) of directory.  Create adds, while it runs, 8 n s bytes
+ *     4 D of values, 8 (D + 1) of counts and 8 (ceil(D / 4) + 1) of directory.  Create adds, while it runs, 8 n s bytes
  *     of unsorted keys, 8 n s of values and CUB's sort storage (the host call also stages 4 n s bytes of sketches);
  *     results add 16 n s bytes of multiplicity slots, 4 n of counts and CUB's segmented-sort storage; winners adds
- *     to those 8 D bytes of votes; the host add stages the pool's bytes and offsets. */
+ *     to those 8 D bytes of votes; the host add stages the pool's bytes and offsets.
+ *   - Several samples (create_samples, add_samples, results_samples, winners_samples and their _dev forms): a screen
+ *     holds S = n_samples >= 1 pools over one reference index, and each read of add_samples carries a sample id
+ *     (one uint32 per read).  c_pool,q(v) = the windows (as above) with hash v of the reads tagged q, over every add
+ *     since creation or the last reset.  Row q of results_samples is results with c_pool,q in place of c_pool; row q
+ *     of winners_samples is the winner-take-all with sample q's own first-pass shared (samples never vote together:
+ *     a value present in samples 1 and 2 is allocated in each apart).  Sample independence: row q equals, byte for
+ *     byte, what a fresh pg_mash_screen_create screen answers after one add of only sample q's reads in the same
+ *     order; a sample that received no reads has an all-zero row.  Split invariance holds per sample, for any mix
+ *     of host and _dev adds; reset empties every sample.  results_samples and winners_samples write rows
+ *     [first, first + count) of the [S][n] table, row-major: out[(q - first) * n + r]; any output may be NULL.
+ *   - The single-sample calls on any screen: create and create_dev make S = 1; add and add_dev count every read into
+ *     sample 0; results, results_dev, winners and winners_dev return row 0.
+ *   - Errors of the sample calls, added to the order above: n_samples == 0 is PG_ERR_ARG, after the n > 2^32 - 1
+ *     rule and before the null-buffer rule.  A null id array with n_reads > 0 is PG_ERR_ARG.  In a host add a sample
+ *     id >= S is PG_ERR_ARG, checked on the host before anything is copied or launched (the screen keeps what it
+ *     held).  first + count > S is PG_ERR_ARG.  add_samples_dev trusts d_sample_ids as it trusts d_offsets: a read
+ *     whose id is >= S contributes nothing, and no memory outside the screen is written.
+ *   - Device memory with S samples: the counters take 8 (S D + 1) bytes (one sink counter for reads whose id is not
+ *     a sample); create returns PG_ERR_NOMEM when they do not fit.  results_samples and winners_samples tally the
+ *     samples in groups of g = max(1, min(count, 2^28 / (n s))): their scratch is that of results (or winners) times
+ *     g, at most 16 x 2^28 bytes of slots when n s <= 2^28, whatever S is. */
 typedef struct pg_mash_screen pg_mash_screen;
 int pg_mash_screen_create(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, pg_mash_screen **out);
 int pg_mash_screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, void *stream, pg_mash_screen **out);
@@ -587,6 +608,21 @@ int pg_mash_screen_results_dev(const pg_mash_screen *sc, uint32_t *d_shared, dou
 int pg_mash_screen_winners(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity);
 int pg_mash_screen_winners_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity,
                                void *stream);
+int pg_mash_screen_create_samples(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, pg_mash_screen **out);
+int pg_mash_screen_create_samples_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, void *stream,
+                                      pg_mash_screen **out);
+int pg_mash_screen_add_samples(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, const uint32_t *sample_ids, uint64_t n_reads);
+int pg_mash_screen_add_samples_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uint64_t *d_offsets, const uint32_t *d_sample_ids,
+                                   uint64_t n_reads, void *stream);
+/* rows [first, first + count) of the [S][n] table, row-major: out[(q - first) * n + r]; any output may be NULL */
+int pg_mash_screen_results_samples(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *shared, double *containment,
+                                   uint64_t *multiplicity);
+int pg_mash_screen_results_samples_dev(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_containment,
+                                       uint64_t *d_multiplicity, void *stream);
+int pg_mash_screen_winners_samples(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *shared, double *containment,
+                                   uint64_t *multiplicity);
+int pg_mash_screen_winners_samples_dev(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_containment,
+                                       uint64_t *d_multiplicity, void *stream);
 int pg_mash_screen_free(pg_mash_screen *sc);
 
 /* ---- align.SmithWaterman score -- search/align/align.go:171-203 -------------------

@@ -106,6 +106,14 @@ _SIGS = {
     "pg_mash_screen_results_dev": (C.c_int, [C.c_void_p, _u32p, _f64p, _u64p, C.c_void_p]),
     "pg_mash_screen_winners": (C.c_int, [C.c_void_p, _u32p, _f64p, _u64p]),
     "pg_mash_screen_winners_dev": (C.c_int, [C.c_void_p, _u32p, _f64p, _u64p, C.c_void_p]),
+    "pg_mash_screen_create_samples": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.POINTER(C.c_void_p)]),
+    "pg_mash_screen_create_samples_dev": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "pg_mash_screen_add_samples": (C.c_int, [C.c_void_p, _u8p, _u64p, _u32p, C.c_uint64]),
+    "pg_mash_screen_add_samples_dev": (C.c_int, [C.c_void_p, _u8p, _u64p, _u32p, C.c_uint64, C.c_void_p]),
+    "pg_mash_screen_results_samples": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _u32p, _f64p, _u64p]),
+    "pg_mash_screen_results_samples_dev": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _u32p, _f64p, _u64p, C.c_void_p]),
+    "pg_mash_screen_winners_samples": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _u32p, _f64p, _u64p]),
+    "pg_mash_screen_winners_samples_dev": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _u32p, _f64p, _u64p, C.c_void_p]),
     "pg_mash_screen_free": (C.c_int, [C.c_void_p]),
     "pg_sw_score_batch": (C.c_int, [_u8p, _u64p, C.c_uint64, _u8p, C.c_uint64, C.c_int32, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p]),
     "pg_sw_score_batch_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_uint64, _u8p, C.c_uint64, C.c_int32, _i16p, _i16p, _i64p, C.c_int32, C.c_int32, C.c_int64, _i64p, _i32p, _i64p, C.c_void_p]),

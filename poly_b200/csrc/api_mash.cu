@@ -624,44 +624,119 @@ static int cluster_add(pg_mash_clusterer *c, const uint32_t *d_b, uint64_t m, ui
 }
 
 // The argument rules of pg_mash_screen_create after the null out pointer, in their order
-static int screen_create_check(const void *sketches, uint64_t n, int32_t s, int32_t k) {
+static int screen_create_check(const void *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples) {
     if (k < 0) { set_error("k-mer size %d < 0", k); return PG_ERR_ARG; }
     if (n && s <= 0) { set_error("screen over sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
     if (n > 0xffffffffull) { set_error("%llu references exceed 2^32 - 1", (unsigned long long)n); return PG_ERR_ARG; }
+    if (n_samples == 0) { set_error("a screen of 0 samples"); return PG_ERR_ARG; }
     if (n && !sketches) { set_error("null buffer"); return PG_ERR_ARG; }
     return PG_OK;
 }
 
 static pg_mash_screen *screen_new(int32_t k, const ScreenIndex &ix) { return new pg_mash_screen{cur_ctx()->device, k, ix}; }
 
-// results and winners: the same rules, locking and copies around a different tally
-using ScreenTally = int (*)(const ScreenIndex &, uint32_t *, double *, uint64_t *, cudaStream_t);
+static int screen_create_host(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, pg_mash_screen **out) {
+    if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = screen_create_check(sketches, n, s, k, n_samples);
+    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
+    ScreenIndex ix;
+    {
+        HostCall c;
+        const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)std::max(s, 0));
+        if ((rc = c.error()) || (rc = screen_build(d_sk, n, s, n_samples, c.st, &ix))) return rc;
+        if ((rc = c.finish()) != PG_OK) {
+            screen_free(ix, c.st);
+            return rc;
+        }
+    }
+    *out = screen_new(k, ix);
+    return PG_OK;
+}
 
-static int screen_tally_host(const pg_mash_screen *sc, ScreenTally tally, uint32_t *shared, double *containment, uint64_t *multiplicity) {
+static int screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, void *stream,
+                             pg_mash_screen **out) {
+    if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    int rc = screen_create_check(d_sketches, n, s, k, n_samples);
+    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
+    ScreenIndex ix;
+    if ((rc = screen_build(d_sketches, n, s, n_samples, (cudaStream_t)stream, &ix)) != PG_OK) return rc;
+    *out = screen_new(k, ix);
+    return PG_OK;
+}
+
+// A host add; ids == null: every read is sample 0.  The ids are checked against the screen's samples before any
+// copy or launch.
+static int screen_add_host(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, const uint32_t *ids, uint64_t n_reads) {
     if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    if (n_reads == 0) return PG_OK;
+    if (!bases || !offsets) { set_error("null buffer"); return PG_ERR_ARG; }
+    const uint32_t samples = sc->ix.samples;  // fixed at creation
+    if (ids)
+        for (uint64_t i = 0; i < n_reads; ++i)
+            if (ids[i] >= samples) {
+                set_error("read %llu has sample id %u, the screen has %u samples", (unsigned long long)i, ids[i], samples);
+                return PG_ERR_ARG;
+            }
     int rc = use_device(sc->device);
     if (rc != PG_OK) return rc;
-    std::shared_lock<std::shared_mutex> lk(sc->rw);
-    const uint64_t n = sc->ix.n;
-    if (n == 0 || (!shared && !containment && !multiplicity)) return PG_OK;
+    std::unique_lock<std::shared_mutex> lk(sc->rw);
     HostCall c;
-    uint32_t *d_sh = shared ? c.alloc<uint32_t>(n) : nullptr;
-    double *d_c = containment ? c.alloc<double>(n) : nullptr;
-    uint64_t *d_m = multiplicity ? c.alloc<uint64_t>(n) : nullptr;
-    if ((rc = c.error()) || (rc = tally(sc->ix, d_sh, d_c, d_m, c.st))) return rc;
-    c.download(shared, d_sh, n);
-    c.download(containment, d_c, n);
-    c.download(multiplicity, d_m, n);
+    const Ragged<uint8_t> r = c.ragged(bases, offsets, n_reads);
+    const uint32_t *d_ids = ids ? c.upload(ids, n_reads) : nullptr;
+    if ((rc = c.error()) || (rc = screen_add(sc->ix, sc->k, r.base, r.off, d_ids, n_reads, c.st))) return rc;
     return c.finish();
 }
 
-static int screen_tally_dev(const pg_mash_screen *sc, ScreenTally tally, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity,
-                            void *stream) {
+// add_dev and add_samples_dev; ids == null: every read is sample 0
+static int screen_add_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uint64_t *d_offsets, const uint32_t *d_ids, uint64_t n_reads,
+                          void *stream) {
     if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    if (n_reads == 0) return PG_OK;
+    if (!d_bases || !d_offsets) { set_error("null buffer"); return PG_ERR_ARG; }
     int rc = use_device(sc->device);
     if (rc != PG_OK) return rc;
+    std::unique_lock<std::shared_mutex> lk(sc->rw);
+    return screen_add(sc->ix, sc->k, d_bases, d_offsets, d_ids, n_reads, (cudaStream_t)stream);
+}
+
+// results and winners: the same rules, locking and copies around a different tally, over rows [first, first + count)
+using ScreenTally = int (*)(const ScreenIndex &, uint32_t, uint32_t, uint32_t *, double *, uint64_t *, cudaStream_t);
+
+static int screen_rows_check(const pg_mash_screen *sc, uint32_t first, uint32_t count) {
+    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
+    if ((uint64_t)first + count > sc->ix.samples) {
+        set_error("rows [%u, %llu) of a screen of %u samples", first, (unsigned long long)first + count, sc->ix.samples);
+        return PG_ERR_ARG;
+    }
+    return PG_OK;
+}
+
+static int screen_tally_host(const pg_mash_screen *sc, ScreenTally tally, uint32_t first, uint32_t count, uint32_t *shared, double *containment,
+                             uint64_t *multiplicity) {
+    int rc = screen_rows_check(sc, first, count);
+    if (rc != PG_OK || (rc = use_device(sc->device)) != PG_OK) return rc;
     std::shared_lock<std::shared_mutex> lk(sc->rw);
-    return tally(sc->ix, d_shared, d_containment, d_multiplicity, (cudaStream_t)stream);
+    const uint64_t m = sc->ix.n * count;
+    if (m == 0 || (!shared && !containment && !multiplicity)) return PG_OK;
+    HostCall c;
+    uint32_t *d_sh = shared ? c.alloc<uint32_t>(m) : nullptr;
+    double *d_c = containment ? c.alloc<double>(m) : nullptr;
+    uint64_t *d_m = multiplicity ? c.alloc<uint64_t>(m) : nullptr;
+    if ((rc = c.error()) || (rc = tally(sc->ix, first, count, d_sh, d_c, d_m, c.st))) return rc;
+    c.download(shared, d_sh, m);
+    c.download(containment, d_c, m);
+    c.download(multiplicity, d_m, m);
+    return c.finish();
+}
+
+static int screen_tally_dev(const pg_mash_screen *sc, ScreenTally tally, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_containment,
+                            uint64_t *d_multiplicity, void *stream) {
+    int rc = screen_rows_check(sc, first, count);
+    if (rc != PG_OK || (rc = use_device(sc->device)) != PG_OK) return rc;
+    std::shared_lock<std::shared_mutex> lk(sc->rw);
+    return tally(sc->ix, first, count, d_shared, d_containment, d_multiplicity, (cudaStream_t)stream);
 }
 
 }  // namespace
@@ -1340,56 +1415,39 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c) {
 // Screen: which references a pool of reads contains
 // ---------------------------------------------------------------------------------
 int pg_mash_screen_create(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, pg_mash_screen **out) {
-    if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
-    *out = nullptr;
-    int rc = screen_create_check(sketches, n, s, k);
-    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
-    ScreenIndex ix;
-    {
-        HostCall c;
-        const uint32_t *d_sk = c.upload(sketches, n * (uint64_t)std::max(s, 0));
-        if ((rc = c.error()) || (rc = screen_build(d_sk, n, s, c.st, &ix))) return rc;
-        if ((rc = c.finish()) != PG_OK) {
-            screen_free(ix, c.st);
-            return rc;
-        }
-    }
-    *out = screen_new(k, ix);
-    return PG_OK;
+    return screen_create_host(sketches, n, s, k, 1, out);
 }
 
 int pg_mash_screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, void *stream, pg_mash_screen **out) {
-    if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
-    *out = nullptr;
-    int rc = screen_create_check(d_sketches, n, s, k);
-    if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
-    ScreenIndex ix;
-    if ((rc = screen_build(d_sketches, n, s, (cudaStream_t)stream, &ix)) != PG_OK) return rc;
-    *out = screen_new(k, ix);
-    return PG_OK;
+    return screen_create_dev(d_sketches, n, s, k, 1, stream, out);
+}
+
+int pg_mash_screen_create_samples(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, pg_mash_screen **out) {
+    return screen_create_host(sketches, n, s, k, n_samples, out);
+}
+
+int pg_mash_screen_create_samples_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, void *stream,
+                                      pg_mash_screen **out) {
+    return screen_create_dev(d_sketches, n, s, k, n_samples, stream, out);
 }
 
 int pg_mash_screen_add(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads) {
-    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
-    if (n_reads == 0) return PG_OK;
-    if (!bases || !offsets) { set_error("null buffer"); return PG_ERR_ARG; }
-    int rc = use_device(sc->device);
-    if (rc != PG_OK) return rc;
-    std::unique_lock<std::shared_mutex> lk(sc->rw);
-    HostCall c;
-    const Ragged<uint8_t> r = c.ragged(bases, offsets, n_reads);
-    if ((rc = c.error()) || (rc = screen_add(sc->ix, sc->k, r.base, r.off, n_reads, c.st))) return rc;
-    return c.finish();
+    return screen_add_host(sc, bases, offsets, nullptr, n_reads);
 }
 
 int pg_mash_screen_add_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_reads, void *stream) {
-    if (!sc) { set_error("null screen"); return PG_ERR_ARG; }
-    if (n_reads == 0) return PG_OK;
-    if (!d_bases || !d_offsets) { set_error("null buffer"); return PG_ERR_ARG; }
-    int rc = use_device(sc->device);
-    if (rc != PG_OK) return rc;
-    std::unique_lock<std::shared_mutex> lk(sc->rw);
-    return screen_add(sc->ix, sc->k, d_bases, d_offsets, n_reads, (cudaStream_t)stream);
+    return screen_add_dev(sc, d_bases, d_offsets, nullptr, n_reads, stream);
+}
+
+int pg_mash_screen_add_samples(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, const uint32_t *sample_ids, uint64_t n_reads) {
+    if (sc && n_reads && !sample_ids) { set_error("null sample ids"); return PG_ERR_ARG; }
+    return screen_add_host(sc, bases, offsets, sample_ids, n_reads);
+}
+
+int pg_mash_screen_add_samples_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uint64_t *d_offsets, const uint32_t *d_sample_ids,
+                                   uint64_t n_reads, void *stream) {
+    if (sc && n_reads && !d_sample_ids) { set_error("null sample ids"); return PG_ERR_ARG; }
+    return screen_add_dev(sc, d_bases, d_offsets, d_sample_ids, n_reads, stream);
 }
 
 int pg_mash_screen_reset(pg_mash_screen *sc) {
@@ -1403,19 +1461,39 @@ int pg_mash_screen_reset(pg_mash_screen *sc) {
 }
 
 int pg_mash_screen_results(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity) {
-    return screen_tally_host(sc, screen_results, shared, containment, multiplicity);
+    return screen_tally_host(sc, screen_results, 0, 1, shared, containment, multiplicity);
 }
 
 int pg_mash_screen_results_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity, void *stream) {
-    return screen_tally_dev(sc, screen_results, d_shared, d_containment, d_multiplicity, stream);
+    return screen_tally_dev(sc, screen_results, 0, 1, d_shared, d_containment, d_multiplicity, stream);
 }
 
 int pg_mash_screen_winners(const pg_mash_screen *sc, uint32_t *shared, double *containment, uint64_t *multiplicity) {
-    return screen_tally_host(sc, screen_winners, shared, containment, multiplicity);
+    return screen_tally_host(sc, screen_winners, 0, 1, shared, containment, multiplicity);
 }
 
 int pg_mash_screen_winners_dev(const pg_mash_screen *sc, uint32_t *d_shared, double *d_containment, uint64_t *d_multiplicity, void *stream) {
-    return screen_tally_dev(sc, screen_winners, d_shared, d_containment, d_multiplicity, stream);
+    return screen_tally_dev(sc, screen_winners, 0, 1, d_shared, d_containment, d_multiplicity, stream);
+}
+
+int pg_mash_screen_results_samples(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *shared, double *containment,
+                                   uint64_t *multiplicity) {
+    return screen_tally_host(sc, screen_results, first, count, shared, containment, multiplicity);
+}
+
+int pg_mash_screen_results_samples_dev(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_containment,
+                                       uint64_t *d_multiplicity, void *stream) {
+    return screen_tally_dev(sc, screen_results, first, count, d_shared, d_containment, d_multiplicity, stream);
+}
+
+int pg_mash_screen_winners_samples(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *shared, double *containment,
+                                   uint64_t *multiplicity) {
+    return screen_tally_host(sc, screen_winners, first, count, shared, containment, multiplicity);
+}
+
+int pg_mash_screen_winners_samples_dev(const pg_mash_screen *sc, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_containment,
+                                       uint64_t *d_multiplicity, void *stream) {
+    return screen_tally_dev(sc, screen_winners, first, count, d_shared, d_containment, d_multiplicity, stream);
 }
 
 int pg_mash_screen_free(pg_mash_screen *sc) {

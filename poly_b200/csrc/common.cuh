@@ -302,8 +302,9 @@ int launch_mash_derep_add(const DistancePlan &plan, const uint32_t *d_ids, const
 int launch_derep_gather(const uint32_t *d_b, uint64_t m, int s, uint32_t base, const uint32_t *d_rep, uint64_t n_new, uint32_t *d_rows,
                         uint32_t *d_ids, cudaStream_t st);
 // mash_screen.cu: a screen's device state.  keys: the n x s (value << 32 | id) keys of the reference words, sorted;
-// vals: the D distinct values, ascending; cnt: the pool count of each; dir: nb + 1 entries, dir[b] = the first
-// distinct value in bucket b of join_bucket over [0, vmax].
+// vals: the D distinct values, ascending; cnt: the pool count of each value in each of the `samples` samples,
+// value-major (cnt[d * samples + q]), and one sink counter after them; dir: nb + 1 entries, dir[b] = the first distinct value in bucket b of
+// join_bucket over [0, vmax].
 struct ScreenIndex {
     uint64_t *keys = nullptr, *dir = nullptr;
     uint32_t *vals = nullptr;
@@ -311,19 +312,26 @@ struct ScreenIndex {
     uint64_t n = 0, D = 0;
     int s = 0;
     uint32_t nb = 0, vmax = 0;
+    uint32_t samples = 1;
 };
-// Builds the screen of n reference rows of s > 0 words (any order, zero tails included) with zero counts;
-// synchronises st.  On an error nothing of *out is allocated.
-int screen_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, ScreenIndex *out);
-// Counts every window of reads [0, n_reads) of the ragged pool (d_bases, d_off) into ix.cnt; only enqueues, and
+// Builds the screen of n reference rows of s > 0 words (any order, zero tails included) with zero counts for
+// samples >= 1 samples; synchronises st.  On an error nothing of *out is allocated.
+int screen_build(const uint32_t *d_sk, uint64_t n, int s, uint32_t samples, cudaStream_t st, ScreenIndex *out);
+// Counts every window of reads [0, n_reads) of the ragged pool (d_bases, d_off) into ix.cnt, read i into sample
+// d_ids[i] (sample 0 when d_ids is null; a read whose id is >= ix.samples counts nowhere); only enqueues, and
 // reads no byte outside [d_off[0], d_off[n_reads]) whatever the offsets hold.
-int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_reads, cudaStream_t st);
+int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, const uint32_t *d_ids, uint64_t n_reads,
+               cudaStream_t st);
 int screen_reset(const ScreenIndex &ix, cudaStream_t st);
-// shared, containment and multiplicity of every reference (any output may be NULL); only enqueues
-int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st);
-// the same three arrays over the words each value's winner-take-all vote gave their reference: a value the pool holds
-// goes to the reference that holds it with the largest first-pass shared (ties to the smallest id); only enqueues
-int screen_winners(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st);
+// shared, containment and multiplicity of every reference for samples [first, first + count), row-major
+// (out[(q - first) * n + r]; any output may be NULL; first + count <= ix.samples); only enqueues
+int screen_results(const ScreenIndex &ix, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_cont, uint64_t *d_mult,
+                   cudaStream_t st);
+// the same three arrays over the words each value's winner-take-all vote gave their reference: a value a sample holds
+// goes to the reference that holds it with the largest first-pass shared of that sample (ties to the smallest id);
+// only enqueues
+int screen_winners(const ScreenIndex &ix, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_cont, uint64_t *d_mult,
+                   cudaStream_t st);
 void screen_free(ScreenIndex &ix, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).

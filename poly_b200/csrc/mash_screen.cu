@@ -7,20 +7,24 @@
 //   2. one CUB radix sort of the keys; the D distinct values, ascending (CUB Unique), and a directory of
 //      nb = ceil(D / 4) value buckets over [0, vmax] (join_bucket, the join index's mapping): dir[b] is the first
 //      distinct value in bucket b, so a lookup is two directory reads and a binary search over ~4 values;
-//   3. one 64-bit pool counter per distinct value, zeroed.
+//   3. one 64-bit pool counter per distinct value and sample, zeroed.
+// Several samples: every read of an add carries a sample id, and each distinct value has one counter per sample,
+// value-major (cnt[d * S + q]), so a tally reads the samples of a group at one value from one line.
 // Add (the hot path, screen_add): the pool's bytes are cut into fixed chunks, whatever the read lengths; a
 // CTA stages a chunk (plus the k - 1 byte halo) in shared memory and each thread walks W consecutive windows
 // of it with the register-ring murmur3 walk of K1 (kmer_walk.cuh).  A window hash above vmax is dropped by one
 // compare, which is almost every window when the references are bottom-s sketches of large genomes.  The
 // rest are checked against the read boundaries (a binary search over the offsets, then a cursor) and looked
-// up; hits are aggregated per warp on equal counters (__match_any_sync) before one atomicAdd.  k outside the
-// walk's instantiated set hashes each window from global memory.
+// up; a hit takes its read's sample id and is aggregated per warp on equal counters (__match_any_sync) before one
+// atomicAdd.  k outside the walk's instantiated set hashes each window from global memory.
 // Results (screen_results): one pass over the sorted keys.  The c_r(v) words of reference r equal to v are one
 // run of equal keys, and the first min(c_r(v), c_pool(v)) of them count; each counted word appends c_pool(v)
 // to its reference's segment of s slots.  A CUB segmented sort of the segments then gives the lower median.
+// Samples are tallied in groups whose slots stay under SCREEN_GROUP_SLOTS: one count pass, one segmented sort and
+// one final kernel per group.
 // Winners (screen_winners, Mash Screen's winner-take-all): the same count pass without the segments gives each
 // reference's first-pass shared; then every value the pool holds votes among its contenders, one run of keys
-// (screen_vote_kernel), and the count pass above runs again over the won words only.
+// (screen_vote_kernel, per sample), and the count pass above runs again over the won words only.
 #include <algorithm>
 #include <climits>
 
@@ -37,13 +41,19 @@ namespace pg {
 namespace {
 
 constexpr int SCREEN_THREADS = 256;
+// A tally's multiplicity slots (8 bytes each, twice: unsorted and sorted) for one group of samples: the group is as
+// many samples as fit, at least one.  The segmented sort counts its items in int, so the bound stays below INT_MAX.
+constexpr uint64_t SCREEN_GROUP_SLOTS = 1ull << 28;
+static_assert(SCREEN_GROUP_SLOTS <= (uint64_t)INT_MAX, "a sample group is one segmented sort");
 
-// what the add kernels read of a screen
+// what the add and tally kernels read of a screen
 struct ScreenLookup {
     const uint32_t *vals;     // [D] distinct reference values, ascending
     const uint64_t *dir;      // [nb + 1]
-    unsigned long long *cnt;  // [D] pool counts
-    uint32_t nb, vmax;
+    unsigned long long *cnt;  // [D][samples] pool counts, value-major, then the sink
+    const uint32_t *ids;      // the add's per-read sample ids; null: every read is sample 0
+    uint64_t sink;            // D samples: the counter of windows whose read's id is not a sample, never read
+    uint32_t nb, vmax, samples;
 };
 
 // the index d of value h among the distinct values, if h is one of them
@@ -76,12 +86,21 @@ __device__ __forceinline__ bool window_in_read(const uint64_t *off, uint64_t n_r
     return j <= n_reads && p + k < off[j];
 }
 
-// One window of every lane of a converged warp; cand: the lane's hash h is <= vmax.  Lanes that hit the same
-// counter add to it once, with their number.
+// One window of every lane of a converged warp; cand: the lane's hash h is <= vmax.  With SAMPLES, a hit counts into
+// its read's sample, ids[j - 1] (j: the first offset above p; sample 0 when ids is null), or into the sink when that
+// id is not a sample: a select rather than one more condition on the hit, which keeps the walk kernels at their
+// registers.  Without SAMPLES (one sample, no ids) d is the counter, as in a single-sample screen.  Lanes that hit
+// the same counter add to it once, with their number.
+template <bool SAMPLES>
 __device__ __forceinline__ void screen_hit(const ScreenLookup &L, uint64_t scale, const uint64_t *off, uint64_t n_reads, bool cand, uint64_t p,
                                            uint32_t k, uint32_t h, uint64_t &j) {
     uint64_t d = ~0ull;
-    const bool hit = cand && window_in_read(off, n_reads, p, k, j) && screen_find(L, scale, h, &d);
+    bool hit = cand && window_in_read(off, n_reads, p, k, j) && screen_find(L, scale, h, &d);
+    if (SAMPLES && hit) {
+        const uint32_t q = L.ids ? __ldg(L.ids + (j - 1)) : 0u;
+        d = q < L.samples ? d * L.samples + q : L.sink;
+    }
+
     const unsigned peers = __match_any_sync(0xffffffffu, hit ? d : ~0ull);
     if (hit && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&L.cnt[d], (unsigned long long)__popc(peers));
 }
@@ -94,14 +113,14 @@ __host__ __device__ constexpr uint32_t screen_span(int nb) { return 4u * nb * (1
 #define PG_SCREEN_EMIT(R_, H_)                                                                                              \
     {                                                                                                                       \
         const bool cand_ = (H_) <= L.vmax;                                                                                  \
-        if (__any_sync(0xffffffffu, cand_)) screen_hit(L, scale, off, n_reads, cand_, p0 + i + (R_), (uint32_t)K, (H_), j); \
+        if (__any_sync(0xffffffffu, cand_)) screen_hit<SAMPLES>(L, scale, off, n_reads, cand_, p0 + i + (R_), (uint32_t)K, (H_), j); \
     }
 
 // The walk path (k in WalkKs).  Persistent CTAs take chunks of SCREEN_THREADS x W windows of the pool
 // [off[0], off[n_reads]); thread t walks windows [t W, t W + W) of the chunk.  The chunk's bytes, its look-ahead
 // and the 16-byte alignment head are staged in shared memory with 16-byte loads; bytes outside the pool are
 // zeros and are never read from global memory.
-template <int K>
+template <int K, bool SAMPLES>
 __global__ void __launch_bounds__(SCREEN_THREADS, 2)
 screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ off, uint64_t n_reads, const ScreenLookup L,
                    uint32_t lut_stride) {
@@ -160,6 +179,7 @@ screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict
 
 // Any other k (0 included): window p of the pool is hashed from global memory by thread p of a CTA-uniform
 // grid-stride loop, so that every lane of a warp runs the same iterations.
+template <bool SAMPLES>
 __global__ void __launch_bounds__(SCREEN_THREADS)
 screen_generic_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ off, uint64_t n_reads, uint32_t k, const ScreenLookup L) {
     const uint64_t lo = off[0], hi = max(off[n_reads], lo);
@@ -175,7 +195,7 @@ screen_generic_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restr
         }
         if (__any_sync(0xffffffffu, cand)) {
             uint64_t j = ~0ull;
-            screen_hit(L, scale, off, n_reads, cand, p, k, h, j);
+            screen_hit<SAMPLES>(L, scale, off, n_reads, cand, p, k, h, j);
         }
     }
 }
@@ -201,11 +221,14 @@ __global__ void screen_dir_kernel(const uint32_t *__restrict__ vals, uint64_t D,
 // ties to the smallest id.
 __device__ __forceinline__ uint32_t vote_id(unsigned long long w) { return 0xFFFFFFFFu - (uint32_t)w; }
 
-// Entry e of the sorted keys counts when its rank in its run of equal keys (one reference's copies of one value,
-// at most s long) is below the value's pool count, and, given a vote (win != null), when its reference won the
-// value; it then appends that count to its reference's segment (mult != null).
-__global__ void screen_count_kernel(const uint64_t *__restrict__ keys, uint64_t total, uint32_t s, const ScreenLookup L,
-                                    const unsigned long long *__restrict__ win, uint32_t *__restrict__ fill, unsigned long long *__restrict__ mult) {
+// For each sample t of the group [q0, q0 + g): entry e of the sorted keys counts when its rank in its run of equal
+// keys (one reference's copies of one value, at most s long) is below the value's pool count in the sample, and,
+// given a vote (win != null, [D][g]), when its reference won the value in the sample; it then appends that count to
+// its reference's segment of the sample, row t n + id (mult != null).  The run start and the value index are found
+// once for every sample.
+__global__ void screen_count_kernel(const uint64_t *__restrict__ keys, uint64_t total, uint32_t s, const ScreenLookup L, uint32_t q0, uint32_t g,
+                                    uint64_t n, const unsigned long long *__restrict__ win, uint32_t *__restrict__ fill,
+                                    unsigned long long *__restrict__ mult) {
     const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
     for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t key = keys[e];
@@ -217,44 +240,54 @@ __global__ void screen_count_kernel(const uint64_t *__restrict__ keys, uint64_t 
         }
         uint64_t d = 0;
         screen_find(L, scale, (uint32_t)(key >> 32), &d);  // every reference value is present
-        const unsigned long long c = L.cnt[d];
+        const unsigned long long *cnt = L.cnt + d * L.samples + q0;
         const uint32_t id = (uint32_t)key;
-        if (e - lo < c && (!win || vote_id(win[d]) == id)) {
-            const uint32_t pos = atomicAdd(&fill[id], 1u);
-            if (mult) mult[(uint64_t)id * s + pos] = c;
+        for (uint32_t t = 0; t < g; ++t) {
+            const unsigned long long c = cnt[t];
+            if (e - lo < c && (!win || vote_id(win[d * g + t]) == id)) {
+                const uint64_t row = t * n + id;
+                const uint32_t pos = atomicAdd(&fill[row], 1u);
+                if (mult) mult[row * s + pos] = c;
+            }
         }
     }
 }
 
-// The winner-take-all vote.  The first entry of each (value, id) run whose value the pool holds proposes
-// fill[id] << 32 | (0xFFFFFFFF - id) for the value; win[d] keeps the largest, whatever the order of the atomics.
+// The winner-take-all vote, for each sample t of the group [q0, q0 + g) apart.  The first entry of each (value, id)
+// run whose value the sample holds proposes fill[t n + id] << 32 | (0xFFFFFFFF - id) for the value; win[d g + t]
+// keeps the largest, whatever the order of the atomics.
 // A value's keys are adjacent, so the lanes of a warp that hold it are consecutive: they reduce to one proposal
 // (a segmented max over shuffles) before one atomic, and a proposal no larger than win[d] as read is dropped (win
 // only grows, so a stale read drops nothing that could win).  A value held by every reference thus costs at most one
 // atomic per warp, and far fewer once its leader is in.
-__global__ void screen_vote_kernel(const uint64_t *__restrict__ keys, uint64_t total, const ScreenLookup L, const uint32_t *__restrict__ fill,
-                                   unsigned long long *win) {
+__global__ void screen_vote_kernel(const uint64_t *__restrict__ keys, uint64_t total, const ScreenLookup L, uint32_t q0, uint32_t g, uint64_t n,
+                                   const uint32_t *__restrict__ fill, unsigned long long *win) {
     const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
     const int lane = (int)(threadIdx.x & 31);
     // a warp-uniform trip count: every lane reaches the shuffles
     for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x; base < total; base += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t e = base + threadIdx.x;
         uint64_t d = ~0ull;  // past the end: a segment of its own, after every value
-        unsigned long long p = 0;
+        uint32_t id = 0;
+        bool lead = false;  // the first entry of its (value, id) run
         if (e < total) {
             const uint64_t key = keys[e];
             screen_find(L, scale, (uint32_t)(key >> 32), &d);
-            const uint32_t id = (uint32_t)key;
-            if (L.cnt[d] && (e == 0 || keys[e - 1] != key)) p = (unsigned long long)fill[id] << 32 | (0xFFFFFFFFu - id);
+            id = (uint32_t)key;
+            lead = e == 0 || keys[e - 1] != key;
         }
         const unsigned peers = __match_any_sync(0xffffffffu, d);
         const int last = 31 - __clz(peers);
+        for (uint32_t t = 0; t < g; ++t) {  // g is uniform: every lane reaches the shuffles
+            unsigned long long p = 0;
+            if (lead && L.cnt[d * L.samples + q0 + t]) p = (unsigned long long)fill[t * n + id] << 32 | (0xFFFFFFFFu - id);
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {  // lane i ends with the max over lanes [i, last]
-            const unsigned long long q = __shfl_down_sync(0xffffffffu, p, o);
-            if (lane + o <= last) p = max(p, q);
+            for (int o = 1; o < 32; o <<= 1) {  // lane i ends with the max over lanes [i, last]
+                const unsigned long long q = __shfl_down_sync(0xffffffffu, p, o);
+                if (lane + o <= last) p = max(p, q);
+            }
+            if (p && lane == __ffs(peers) - 1 && p > win[d * g + t]) atomicMax(&win[d * g + t], p);
         }
-        if (p && lane == __ffs(peers) - 1 && p > win[d]) atomicMax(&win[d], p);
     }
 }
 
@@ -276,15 +309,18 @@ __global__ void screen_final_kernel(const uint32_t *__restrict__ fill, const uns
     }
 }
 
-ScreenLookup lookup_of(const ScreenIndex &ix) { return ScreenLookup{ix.vals, ix.dir, ix.cnt, ix.nb, ix.vmax}; }
+ScreenLookup lookup_of(const ScreenIndex &ix, const uint32_t *ids = nullptr) {
+    return ScreenLookup{ix.vals, ix.dir, ix.cnt, ids, ix.D * ix.samples, ix.nb, ix.vmax, ix.samples};
+}
 
 unsigned grid_of(uint64_t work) { return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((work + 255) / 256, (uint64_t)sm_count() * 16)); }
 
-template <int K>
-int launch_screen_walk(const ScreenIndex &ix, const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_reads, cudaStream_t st) {
+template <int K, bool SAMPLES>
+int launch_screen_walk(const ScreenIndex &ix, const uint8_t *d_bases, const uint64_t *d_off, const uint32_t *d_ids, uint64_t n_reads,
+                       cudaStream_t st) {
     uint64_t grid = 0;  // persistent: the pool's size is on the device, so the grid is what is resident at once
-    { const int rc_ = resident_blocks((const void *)screen_walk_kernel<K>, SCREEN_THREADS, 0, ~0ull, &grid); if (rc_ != PG_OK) return rc_; }
-    screen_walk_kernel<K><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, lookup_of(ix), 4u);
+    { const int rc_ = resident_blocks((const void *)screen_walk_kernel<K, SAMPLES>, SCREEN_THREADS, 0, ~0ull, &grid); if (rc_ != PG_OK) return rc_; }
+    screen_walk_kernel<K, SAMPLES><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, lookup_of(ix, d_ids), 4u);
     PG_LAUNCH_CHECK("screen_walk_kernel");
     return PG_OK;
 }
@@ -297,10 +333,11 @@ void screen_free(ScreenIndex &ix, cudaStream_t st) {
     ix = ScreenIndex();
 }
 
-int screen_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, ScreenIndex *out) {
+int screen_build(const uint32_t *d_sk, uint64_t n, int s, uint32_t samples, cudaStream_t st, ScreenIndex *out) {
     ScreenIndex ix;
     ix.n = n;
     ix.s = s;
+    ix.samples = samples;
     const uint64_t total = n * (uint64_t)std::max(s, 0);
     if (total == 0) {
         *out = ix;
@@ -337,11 +374,16 @@ int screen_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, Scree
         ix.vmax = (uint32_t)h_scal[0];
         ix.D = h_scal[1];
         ix.nb = (uint32_t)((ix.D + 3) / 4);
-        if ((e = cudaMallocAsync(&ix.vals, ix.D * 4, st)) != cudaSuccess || (e = cudaMallocAsync(&ix.cnt, ix.D * 8, st)) != cudaSuccess ||
+        uint64_t cnt_bytes = 0;
+        if (__builtin_mul_overflow(ix.D, (uint64_t)samples, &cnt_bytes) || __builtin_mul_overflow(cnt_bytes + 1, (uint64_t)8, &cnt_bytes)) {
+            set_error("%llu values x %u samples of counters overflow 64 bits", (unsigned long long)ix.D, samples);
+            return PG_ERR_NOMEM;
+        }
+        if ((e = cudaMallocAsync(&ix.vals, ix.D * 4, st)) != cudaSuccess || (e = cudaMallocAsync(&ix.cnt, cnt_bytes, st)) != cudaSuccess ||
             (e = cudaMallocAsync(&ix.dir, ((uint64_t)ix.nb + 1) * 8, st)) != cudaSuccess)
             return nomem(e);
         PG_CUDA(cudaMemcpyAsync(ix.vals, d_u, ix.D * 4, cudaMemcpyDeviceToDevice, st));
-        PG_CUDA(cudaMemsetAsync(ix.cnt, 0, ix.D * 8, st));
+        PG_CUDA(cudaMemsetAsync(ix.cnt, 0, cnt_bytes, st));
         screen_dir_kernel<<<grid_of(ix.D), 256, 0, st>>>(ix.vals, ix.D, ix.nb, ix.vmax, ix.dir);
         PG_LAUNCH_CHECK("screen_dir_kernel");
         return PG_OK;
@@ -356,86 +398,107 @@ int screen_build(const uint32_t *d_sk, uint64_t n, int s, cudaStream_t st, Scree
     return PG_OK;
 }
 
-int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_reads, cudaStream_t st) {
+// One sample and no ids take the kernels without the sample step, the single-sample screen's; anything else the
+// kernels with it.
+int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, const uint32_t *d_ids, uint64_t n_reads,
+               cudaStream_t st) {
     if (n_reads == 0 || ix.D == 0) return PG_OK;
+    const bool samples = d_ids || ix.samples != 1;
     int rc = PG_OK;
-    if (with_walk_k(k, [&](auto kk) { rc = launch_screen_walk<decltype(kk)::value>(ix, d_bases, d_off, n_reads, st); })) return rc;
+    if (with_walk_k(k, [&](auto kk) {
+            constexpr int K = decltype(kk)::value;
+            rc = samples ? launch_screen_walk<K, true>(ix, d_bases, d_off, d_ids, n_reads, st) : launch_screen_walk<K, false>(ix, d_bases, d_off, d_ids, n_reads, st);
+        }))
+        return rc;
+    const void *fn = samples ? (const void *)screen_generic_kernel<true> : (const void *)screen_generic_kernel<false>;
     uint64_t grid = 0;
-    if ((rc = resident_blocks((const void *)screen_generic_kernel, SCREEN_THREADS, 0, ~0ull, &grid)) != PG_OK) return rc;
-    screen_generic_kernel<<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix));
+    if ((rc = resident_blocks(fn, SCREEN_THREADS, 0, ~0ull, &grid)) != PG_OK) return rc;
+    if (samples) screen_generic_kernel<true><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix, d_ids));
+    else screen_generic_kernel<false><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix, d_ids));
     PG_LAUNCH_CHECK("screen_generic_kernel");
     return PG_OK;
 }
 
 int screen_reset(const ScreenIndex &ix, cudaStream_t st) {
-    if (ix.D) PG_CUDA(cudaMemsetAsync(ix.cnt, 0, ix.D * 8, st));
+    if (ix.D) PG_CUDA(cudaMemsetAsync(ix.cnt, 0, (ix.D * ix.samples + 1) * 8, st));
     return PG_OK;
 }
 
 namespace {
 
-// The tail of results and winners: the count pass over the words that count (all of them, or given a vote the won
-// ones), the segmented sort of each reference's pool counts and the final arrays.
-int screen_tally(const ScreenIndex &ix, bool winners, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
+// The tail of results and winners for samples [first, first + count): per group of g samples (g n s slots at most
+// SCREEN_GROUP_SLOTS, or one sample), the count pass over the words that count (all of them, or given a vote the won
+// ones), the segmented sort of each (sample, reference) segment of pool counts and the final arrays, written straight
+// into rows [q - first, q - first + g) of the outputs.  One sample is one group: the launches of a single-sample screen.
+int screen_tally(const ScreenIndex &ix, bool winners, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_cont, uint64_t *d_mult,
+                 cudaStream_t st) {
     const uint64_t n = ix.n, s = (uint64_t)std::max(ix.s, 0), total = n * s;
-    if (n == 0 || (!d_shared && !d_cont && !d_mult)) return PG_OK;
+    if (n == 0 || count == 0 || (!d_shared && !d_cont && !d_mult)) return PG_OK;
     StreamScratch tmp(st);
     uint32_t *d_fill = nullptr;
     unsigned long long *d_m = nullptr, *d_sorted = nullptr, *d_win = nullptr;
     int *d_beg = nullptr, *d_end = nullptr;
-    // the segmented sort counts in int: groups of whole rows of at most INT_MAX slots
-    const uint64_t rows_per = std::max<uint64_t>(1, (uint64_t)INT_MAX / s);
-    const uint64_t group = std::min(rows_per, n);
+    const uint64_t group = std::max<uint64_t>(1, std::min<uint64_t>(count, SCREEN_GROUP_SLOTS / total));
+    // the segmented sort counts in int: one sort per chunk of whole rows of at most INT_MAX slots
+    const uint64_t chunk = std::min(std::max<uint64_t>(1, (uint64_t)INT_MAX / s), group * n);
     cudaError_t e;
-    if ((e = tmp.alloc(&d_fill, n)) != cudaSuccess || (e = tmp.alloc(&d_m, total)) != cudaSuccess || (e = tmp.alloc(&d_sorted, total)) != cudaSuccess ||
-        (e = tmp.alloc(&d_beg, group)) != cudaSuccess || (e = tmp.alloc(&d_end, group)) != cudaSuccess ||
-        (winners && (e = tmp.alloc(&d_win, ix.D)) != cudaSuccess)) {
+    if ((e = tmp.alloc(&d_fill, group * n)) != cudaSuccess || (e = tmp.alloc(&d_m, group * total)) != cudaSuccess ||
+        (e = tmp.alloc(&d_sorted, group * total)) != cudaSuccess || (e = tmp.alloc(&d_beg, chunk)) != cudaSuccess ||
+        (e = tmp.alloc(&d_end, chunk)) != cudaSuccess || (winners && (e = tmp.alloc(&d_win, group * ix.D)) != cudaSuccess)) {
         set_error("cudaMallocAsync for the screen results failed: %s", cudaGetErrorString(e));
         cudaGetLastError();
         return PG_ERR_NOMEM;
     }
-    PG_CUDA(cudaMemsetAsync(d_fill, 0, n * 4, st));
-    if (winners) {  // the first pass's shared of every reference, then the vote
-        PG_CUDA(cudaMemsetAsync(d_win, 0, ix.D * 8, st));
-        screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, lookup_of(ix), nullptr, d_fill, nullptr);
-        PG_LAUNCH_CHECK("screen_count_kernel");
-        screen_vote_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, lookup_of(ix), d_fill, d_win);
-        PG_LAUNCH_CHECK("screen_vote_kernel");
-        PG_CUDA(cudaMemsetAsync(d_fill, 0, n * 4, st));
-    }
-    screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, lookup_of(ix), d_win, d_fill, d_m);
-    PG_LAUNCH_CHECK("screen_count_kernel");
     size_t have = 0;
     uint8_t *d_cub = nullptr;
-    for (uint64_t g0 = 0; g0 < n; g0 += group) {
-        const uint64_t rows = std::min(group, n - g0);
-        screen_segments_kernel<<<grid_of(rows), 256, 0, st>>>(d_fill + g0, rows, (uint32_t)s, d_beg, d_end);
-        PG_LAUNCH_CHECK("screen_segments_kernel");
-        size_t bytes = 0;
-        PG_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, bytes, d_m + g0 * s, d_sorted + g0 * s, (int)(rows * s), (int)rows, d_beg, d_end, st));
-        if (bytes > have) {
-            if ((e = tmp.alloc(&d_cub, bytes)) != cudaSuccess) {
-                set_error("cudaMallocAsync(%zu) for the screen results failed", bytes);
-                cudaGetLastError();
-                return PG_ERR_NOMEM;
-            }
-            have = bytes;
+    const ScreenLookup L = lookup_of(ix);
+    for (uint64_t q0 = first; q0 < (uint64_t)first + count; q0 += group) {
+        const uint32_t g = (uint32_t)std::min<uint64_t>(group, (uint64_t)first + count - q0);
+        const uint64_t rows = g * n, out = (q0 - first) * n;
+        PG_CUDA(cudaMemsetAsync(d_fill, 0, rows * 4, st));
+        if (winners) {  // the first pass's shared of every (sample, reference), then the vote
+            PG_CUDA(cudaMemsetAsync(d_win, 0, g * ix.D * 8, st));
+            screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, L, (uint32_t)q0, g, n, nullptr, d_fill, nullptr);
+            PG_LAUNCH_CHECK("screen_count_kernel");
+            screen_vote_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, L, (uint32_t)q0, g, n, d_fill, d_win);
+            PG_LAUNCH_CHECK("screen_vote_kernel");
+            PG_CUDA(cudaMemsetAsync(d_fill, 0, rows * 4, st));
         }
-        PG_CUDA(cub::DeviceSegmentedSort::SortKeys(d_cub, bytes, d_m + g0 * s, d_sorted + g0 * s, (int)(rows * s), (int)rows, d_beg, d_end, st));
+        screen_count_kernel<<<grid_of(total), 256, 0, st>>>(ix.keys, total, (uint32_t)s, L, (uint32_t)q0, g, n, d_win, d_fill, d_m);
+        PG_LAUNCH_CHECK("screen_count_kernel");
+        for (uint64_t r0 = 0; r0 < rows; r0 += chunk) {
+            const uint64_t rr = std::min(chunk, rows - r0);
+            screen_segments_kernel<<<grid_of(rr), 256, 0, st>>>(d_fill + r0, rr, (uint32_t)s, d_beg, d_end);
+            PG_LAUNCH_CHECK("screen_segments_kernel");
+            size_t bytes = 0;
+            PG_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, bytes, d_m + r0 * s, d_sorted + r0 * s, (int)(rr * s), (int)rr, d_beg, d_end, st));
+            if (bytes > have) {
+                if ((e = tmp.alloc(&d_cub, bytes)) != cudaSuccess) {
+                    set_error("cudaMallocAsync(%zu) for the screen results failed", bytes);
+                    cudaGetLastError();
+                    return PG_ERR_NOMEM;
+                }
+                have = bytes;
+            }
+            PG_CUDA(cub::DeviceSegmentedSort::SortKeys(d_cub, bytes, d_m + r0 * s, d_sorted + r0 * s, (int)(rr * s), (int)rr, d_beg, d_end, st));
+        }
+        screen_final_kernel<<<grid_of(rows), 256, 0, st>>>(d_fill, d_sorted, rows, (uint32_t)s, d_shared ? d_shared + out : nullptr,
+                                                           d_cont ? d_cont + out : nullptr, d_mult ? d_mult + out : nullptr);
+        PG_LAUNCH_CHECK("screen_final_kernel");
     }
-    screen_final_kernel<<<grid_of(n), 256, 0, st>>>(d_fill, d_sorted, n, (uint32_t)s, d_shared, d_cont, d_mult);
-    PG_LAUNCH_CHECK("screen_final_kernel");
     return PG_OK;
 }
 
 }  // namespace
 
-int screen_results(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
-    return screen_tally(ix, false, d_shared, d_cont, d_mult, st);
+int screen_results(const ScreenIndex &ix, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_cont, uint64_t *d_mult,
+                   cudaStream_t st) {
+    return screen_tally(ix, false, first, count, d_shared, d_cont, d_mult, st);
 }
 
-int screen_winners(const ScreenIndex &ix, uint32_t *d_shared, double *d_cont, uint64_t *d_mult, cudaStream_t st) {
-    return screen_tally(ix, true, d_shared, d_cont, d_mult, st);
+int screen_winners(const ScreenIndex &ix, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_cont, uint64_t *d_mult,
+                   cudaStream_t st) {
+    return screen_tally(ix, true, first, count, d_shared, d_cont, d_mult, st);
 }
 
 }  // namespace pg

@@ -784,24 +784,33 @@ class Screen:
     sketches: [n, s] uint32 (full Go arrays, zero tail included), a CUDA tensor of that shape, or a list of Mash of
     one SketchSize; k: the k-mer size they were sketched with (not checked, as in the reference).  The pool grows with
     each add, in any split, and reset() empties it.  Reverse-complement windows are not counted: the references hash
-    the forward strand only.  The screen copies the sketches; it lives on the device current at creation."""
+    the forward strand only.  The screen copies the sketches; it lives on the device current at creation.
 
-    def __init__(self, sketches, k: int):
+    samples: the number of pools the screen holds over the one reference index (a multiplexed run's barcodes).  Each
+    read of an add goes to one sample; row q of results_samples / winners_samples is exactly what a one-sample
+    screen fed only sample q's reads would answer.  With the default samples=1 and sample=0 everything is the
+    single-pool screen."""
+
+    def __init__(self, sketches, k: int, samples: int = 1):
         rows = _sketch_rows(sketches)
         n, s = int(rows.shape[0]), int(rows.shape[1])
         if not -(1 << 31) <= k < (1 << 31):
             raise PolyError(_lib.PG_ERR_ARG, f"k-mer size {k} does not fit 32 bits")
+        samples = int(samples)
+        if not 0 <= samples < (1 << 32):
+            raise PolyError(_lib.PG_ERR_ARG, f"{samples} samples do not fit 32 bits")
         h = C.c_void_p()
         if hasattr(rows, "data_ptr"):
             import torch
 
-            rc = _lib.lib().pg_mash_screen_create_dev(rows.data_ptr(), n, s, k, torch.cuda.current_stream(rows.device).cuda_stream, C.byref(h))
+            rc = _lib.lib().pg_mash_screen_create_samples_dev(rows.data_ptr(), n, s, k, samples, torch.cuda.current_stream(rows.device).cuda_stream,
+                                                              C.byref(h))
         else:
-            rc = _lib.lib().pg_mash_screen_create(rows.ctypes.data, n, s, k, C.byref(h))
+            rc = _lib.lib().pg_mash_screen_create_samples(rows.ctypes.data, n, s, k, samples, C.byref(h))
         _index_rc(rc)
         self._h = h
         self._dev_used = None
-        self.n, self.s, self.k = n, s, int(k)
+        self.n, self.s, self.k, self.samples = n, s, int(k), samples
 
     def _live(self):
         if self._h is None:
@@ -815,32 +824,61 @@ class Screen:
 
             torch.cuda.synchronize(self._dev_used)
 
-    def add(self, reads) -> None:
-        """Adds host reads to the pool: a list of str / bytes / uint8 arrays, or (bases, offsets) as flatten returns."""
+    def add(self, reads, sample=0) -> None:
+        """Adds host reads to the pool: a list of str / bytes / uint8 arrays, or (bases, offsets) as flatten returns.
+        sample: the sample every read goes to (an int), or one sample id per read (a uint32 array)."""
         h = self._live()
         if isinstance(reads, tuple) and len(reads) == 2 and isinstance(reads[0], np.ndarray):
             bases, offsets = np.ascontiguousarray(reads[0], np.uint8), np.ascontiguousarray(reads[1], np.uint64)
         else:
             bases, offsets = flatten(reads)
         n_reads = max(len(offsets) - 1, 0)
+        ids = self._sample_ids(sample, n_reads)
         if n_reads == 0:
             return
         if len(bases) == 0:
             bases = np.zeros(1, np.uint8)
         self._sync_dev()
-        _lib.check(_lib.lib().pg_mash_screen_add(h, bases.ctypes.data, offsets.ctypes.data, n_reads))
+        if ids is None:
+            _lib.check(_lib.lib().pg_mash_screen_add(h, bases.ctypes.data, offsets.ctypes.data, n_reads))
+        else:
+            _lib.check(_lib.lib().pg_mash_screen_add_samples(h, bases.ctypes.data, offsets.ctypes.data, ids.ctypes.data, n_reads))
 
-    def add_dev(self, d_bases, d_offsets, stream=None) -> None:
+    def _sample_ids(self, sample, n_reads):
+        """None for sample 0 (the single-sample add), else the uint32 id of every read."""
+        if np.ndim(sample) == 0:
+            q = int(sample)
+            if not 0 <= q < self.samples:
+                raise PolyError(_lib.PG_ERR_ARG, f"sample {q} of a screen of {self.samples} samples")
+            return None if q == 0 else np.full(n_reads, q, np.uint32)
+        ids = np.asarray(sample)
+        if ids.dtype.kind not in "iu":
+            raise ValueError("sample ids must be integers")
+        if ids.shape != (n_reads,):
+            raise ValueError(f"{ids.shape[0] if ids.ndim == 1 else ids.shape} sample ids for {n_reads} reads")
+        if len(ids) and (ids.min() < 0 or ids.max() > 0xFFFFFFFF):
+            raise ValueError("sample ids must fit uint32")
+        return np.ascontiguousarray(ids, np.uint32)
+
+    def add_dev(self, d_bases, d_offsets, stream=None, d_samples=None) -> None:
         """Adds reads already on the device: uint8 bases and int64 (uint64 bits) offsets tensors, read i being
-        d_bases[d_offsets[i] : d_offsets[i + 1]].  Only enqueues, on `stream` (default: the current stream)."""
+        d_bases[d_offsets[i] : d_offsets[i + 1]].  d_samples: None (every read is sample 0) or an int32 / uint32
+        tensor of one sample id per read, trusted as the offsets are: a read whose id is not a sample counts
+        nowhere.  Only enqueues, on `stream` (default: the current stream)."""
         h = self._live()
         import torch
 
         n_reads = max(int(d_offsets.numel()) - 1, 0)
+        if d_samples is not None:
+            if d_samples.element_size() != 4 or d_samples.numel() != n_reads or not d_samples.is_contiguous():
+                raise ValueError("d_samples must be a contiguous 32-bit tensor of one id per read")
         if n_reads == 0:
             return
         st = (stream if stream is not None else torch.cuda.current_stream(d_bases.device)).cuda_stream
-        _lib.check(_lib.lib().pg_mash_screen_add_dev(h, d_bases.data_ptr(), d_offsets.data_ptr(), n_reads, st))
+        if d_samples is None:
+            _lib.check(_lib.lib().pg_mash_screen_add_dev(h, d_bases.data_ptr(), d_offsets.data_ptr(), n_reads, st))
+        else:
+            _lib.check(_lib.lib().pg_mash_screen_add_samples_dev(h, d_bases.data_ptr(), d_offsets.data_ptr(), d_samples.data_ptr(), n_reads, st))
         self._dev_used = d_bases.device
 
     def reset(self) -> None:
@@ -849,34 +887,44 @@ class Screen:
         self._sync_dev()
         _lib.check(_lib.lib().pg_mash_screen_reset(h))
 
-    def results(self):
-        """(shared [n] uint32, containment [n] float64, multiplicity [n] uint64) of the pool so far."""
+    def _table(self, fn, first, count):
         h = self._live()
+        first = int(first)
+        count = self.samples - first if count is None else int(count)
+        if not (0 <= first < (1 << 32) and 0 <= count < (1 << 32)):
+            raise PolyError(_lib.PG_ERR_ARG, f"rows [{first}, {first + count}) of a screen of {self.samples} samples")
         self._sync_dev()
-        shared = np.zeros(self.n, np.uint32)
-        cont = np.zeros(self.n, np.float64)
-        mult = np.zeros(self.n, np.uint64)
-        _lib.check(_lib.lib().pg_mash_screen_results(h, shared.ctypes.data, cont.ctypes.data, mult.ctypes.data))
+        shared = np.zeros((max(count, 0), self.n), np.uint32)
+        cont = np.zeros(shared.shape, np.float64)
+        mult = np.zeros(shared.shape, np.uint64)
+        _lib.check(fn(h, first, count, shared.ctypes.data, cont.ctypes.data, mult.ctypes.data))
         return shared, cont, mult
 
-    def winners(self):
+    def results(self, sample: int = 0):
+        """(shared [n] uint32, containment [n] float64, multiplicity [n] uint64) of the pool (of sample `sample`) so far."""
+        return tuple(x[0] for x in self._table(_lib.lib().pg_mash_screen_results_samples, sample, 1))
+
+    def results_samples(self, first: int = 0, count: Optional[int] = None):
+        """results() of samples [first, first + count) (count defaults to every sample from first) from one call:
+        (shared, containment, multiplicity), each [count, n]."""
+        return self._table(_lib.lib().pg_mash_screen_results_samples, first, count)
+
+    def winners(self, sample: int = 0):
         """Mash Screen's winner-take-all (mash screen -w): each pool hash goes to the reference that holds it with
         the largest first-pass shared (ties to the smallest index), and the (shared, containment, multiplicity) of
         results() are recomputed over the hashes each reference won.  A strain's siblings then stop reporting the
-        hashes it explains better.  The screen is left as it was."""
-        h = self._live()
-        self._sync_dev()
-        shared = np.zeros(self.n, np.uint32)
-        cont = np.zeros(self.n, np.float64)
-        mult = np.zeros(self.n, np.uint64)
-        _lib.check(_lib.lib().pg_mash_screen_winners(h, shared.ctypes.data, cont.ctypes.data, mult.ctypes.data))
-        return shared, cont, mult
+        hashes it explains better.  Each sample votes alone.  The screen is left as it was."""
+        return tuple(x[0] for x in self._table(_lib.lib().pg_mash_screen_winners_samples, sample, 1))
 
-    def identity(self) -> np.ndarray:
-        """Mash Screen's identity estimate containment ** (1 / k), computed on the host from results()."""
+    def winners_samples(self, first: int = 0, count: Optional[int] = None):
+        """winners() of samples [first, first + count) from one call: (shared, containment, multiplicity), each [count, n]."""
+        return self._table(_lib.lib().pg_mash_screen_winners_samples, first, count)
+
+    def identity(self, sample: int = 0) -> np.ndarray:
+        """Mash Screen's identity estimate containment ** (1 / k), computed on the host from results(sample)."""
         if self.k <= 0:
             raise ValueError("identity needs k > 0")
-        return self.results()[1] ** (1.0 / self.k)
+        return self.results(sample)[1] ** (1.0 / self.k)
 
     def close(self) -> None:
         if self._h is not None:
