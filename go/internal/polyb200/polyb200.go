@@ -87,6 +87,21 @@ func SketchBatch(bases []byte, offsets []uint64, k, s int, rowStride int) (out [
 	return out, count, status, check(rc)
 }
 
+// SketchGroups wraps pg_mash_sketch_groups: group g is records [groupOffsets[g], groupOffsets[g+1]) of the ragged
+// batch (bases, offsets); row g of out (s words) holds the smallest count[g] distinct window hashes of the group seen at
+// least minCopies times, ascending, then zeros.
+func SketchGroups(bases []byte, offsets []uint64, groupOffsets []uint64, k, s int, minCopies uint32) (out []uint32, count []uint32, err error) {
+	n, g := len(offsets)-1, len(groupOffsets)-1
+	out = make([]uint32, g*s+1)
+	count = make([]uint32, g+1)
+	err = locked(func() C.int {
+		return C.pg_mash_sketch_groups((*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n),
+			(*C.uint64_t)(unsafe.Pointer(&groupOffsets[0])), C.uint64_t(g), C.int32_t(k), C.int32_t(s), C.uint32_t(minCopies),
+			(*C.uint32_t)(unsafe.Pointer(&out[0])), C.uint64_t(s), (*C.uint32_t)(unsafe.Pointer(&count[0])))
+	})
+	return out[:g*s], count[:g], err
+}
+
 func devicePtr(devices []int32) (*C.int32_t, C.int32_t) {
 	if len(devices) == 0 {
 		return nil, 0 // all visible GPUs

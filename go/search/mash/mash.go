@@ -91,6 +91,32 @@ func SketchBatch(sequences []string, kmerSize, sketchSize int) []*Mash {
 	return res
 }
 
+// SketchGroups returns one sketch per group of sequences: a draft assembly's contigs (`mash sketch genome.fa`) or a
+// sample's reads (`mash sketch -r -m minCopies`).  Each holds the smallest sketchSize distinct window hashes of its
+// group seen at least minCopies times, ascending, then a zero tail when fewer qualify.  Windows never cross a
+// sequence.  The sketches compare with Similarity and Distance like those of Sketch.
+func SketchGroups(groups [][]string, kmerSize, sketchSize, minCopies int) ([]*Mash, error) {
+	if minCopies < 1 || minCopies > math.MaxUint32 {
+		return nil, fmt.Errorf("mash: minCopies %d out of range", minCopies)
+	}
+	var seqs []string
+	goff := make([]uint64, 1, len(groups)+1)
+	for _, g := range groups {
+		seqs = append(seqs, g...)
+		goff = append(goff, uint64(len(seqs)))
+	}
+	bases, offsets := polyb200.Flatten(seqs)
+	out, _, err := polyb200.SketchGroups(bases, offsets, goff, kmerSize, sketchSize, uint32(minCopies))
+	if err != nil {
+		return nil, err
+	}
+	res := make([]*Mash, len(groups))
+	for g := range groups {
+		res[g] = &Mash{KmerSize: kmerSize, SketchSize: sketchSize, Sketches: out[g*sketchSize : (g+1)*sketchSize : (g+1)*sketchSize]}
+	}
+	return res, nil
+}
+
 // DistanceMatrix returns D[i][j] = sketches[i].Distance(sketches[j]) for sketches of one common SketchSize.
 func DistanceMatrix(sketches []*Mash) [][]float64 {
 	n := len(sketches)

@@ -132,6 +132,30 @@ inline std::vector<Mash> SketchBatch(const std::vector<std::string> &seqs, int k
     return res;
 }
 
+// One Mash per group of sequences (an assembly's contigs, a sample's reads): the smallest s distinct window hashes of
+// the group seen at least minCopies times, ascending, then a zero tail (`mash sketch`, `mash sketch -r -m`).  Windows
+// never cross a sequence.  count (may be null) receives how many values each group holds.
+inline std::vector<Mash> SketchGroups(const std::vector<std::vector<std::string>> &groups, int k, int s, uint32_t minCopies,
+                                      std::vector<uint32_t> *count = nullptr) {
+    std::vector<std::string> seqs;
+    std::vector<uint64_t> goff(1, 0);
+    for (const auto &g : groups) {
+        seqs.insert(seqs.end(), g.begin(), g.end());
+        goff.push_back(seqs.size());
+    }
+    Flat f(seqs);
+    const uint64_t stride = (uint64_t)std::max(s, 1);
+    std::vector<uint32_t> out(groups.size() * stride), cnt(groups.size());
+    check(pg_mash_sketch_groups(f.bases.data(), f.offsets.data(), seqs.size(), goff.data(), groups.size(), k, s, minCopies,
+                                out.data(), stride, cnt.data()));
+    std::vector<Mash> res;
+    res.reserve(groups.size());
+    for (size_t g = 0; g < groups.size(); ++g)
+        res.push_back(Mash{k, s, std::vector<uint32_t>(out.begin() + g * stride, out.begin() + (g + 1) * stride)});
+    if (count) *count = cnt;
+    return res;
+}
+
 // In-place form: `slab` holds the Sketches arrays of seqs.size() Mash values back to back (n x s words).  Row i
 // receives its min(len_i - k, s) words, the rest of the row is left as it is -- what (*Mash).Sketch does to an
 // existing Mash (mash.go:73-80); a zeroed slab ends up as n fresh sketches.  Returns the per-read counts.

@@ -28,7 +28,8 @@
  *     pg_seqhash_batch_dev (waits for earlier work on the stream to read the total length, but not
  *     for its own kernels), and
  *     pg_mash_sketch_batch_dev for ragged batches the threshold path does not take
- *     (s < 2, or more than 4 Mi row x item slots) when they hold few long sequences;
+ *     (s < 2, or more than 4 Mi row x item slots) when they hold few long sequences, and
+ *     pg_mash_sketch_groups_dev (it sizes and decides its passes over hash ranges on the host);
  *   - a ragged batch of n items passes n + 1 offsets, item i being [offsets[i], offsets[i+1]).
  *     Offsets must not decrease: the host-pointer entry points return PG_ERR_ARG if they do,
  *     without launching anything;
@@ -159,6 +160,42 @@ int pg_mash_sketch_uniform_gather_dev(const uint8_t *d_bases, uint64_t n_local, 
 int pg_mash_sketch_uniform_scatter_dev(const uint8_t *d_bases, uint64_t n_local, uint32_t read_len,
                                        int32_t k, int32_t s, void *const *dst_ptrs, int32_t n_dst,
                                        int32_t self, uint64_t row_offset, void *stream);
+
+/* ---- grouped sketch: one sketch per group of records (`mash sketch genome.fa`, `mash sketch -r -m M reads.fq`) ----
+ * A draft assembly is many contigs and a read set many reads; Mash sketches each as one set.  Records are ragged
+ * as in pg_mash_sketch_batch (record i = bases[offsets[i] .. offsets[i+1])); group g is records
+ * [group_offsets[g], group_offsets[g+1]).  The groups partition the records: group_offsets[0] == 0,
+ * group_offsets[n_groups] == n_records, never decreasing; empty groups are allowed.
+ *   - Windows: a record of length L contributes the windows (*Mash).Sketch hashes, positions 0 .. L - k - 1
+ *     (mash.go:73; none when L <= k), each murmur3.Sum32 over its raw bytes: forward strand, case-sensitive, any
+ *     byte value, as the screen counts them.  No window crosses a record.
+ *   - c_g(v) = the windows of group g's records whose hash is v.  Row g = the distinct values v with
+ *     c_g(v) >= min_copies in ascending order, the smallest count[g] = min(q_g, s) of them (q_g: how many qualify),
+ *     then zeros up to row_stride.  The row is a set (no value twice) and always ascending, also when q_g < s; a
+ *     real hash can be 0, so count[g] tells the tail apart.  A group of one record with L - k >= s, min_copies 1 and
+ *     no repeated value in its bottom-s multiset gives pg_mash_sketch_batch's row of that record, word for word.
+ *   - Row g depends only on the multiset of group g's windows: not on the order of its records, the order of the
+ *     groups, the other groups of the call or how a batch of groups is split over calls.  Rows are exact: whatever
+ *     passes the device takes, every count is exact.
+ *   - Errors, checked in this order before any device work: a null out or count with n_groups > 0; k < 0 (as for
+ *     the sketch calls); s < 1; min_copies < 1; row_stride < s; a null buffer with work to do (group_offsets and
+ *     offsets when n_groups > 0; bases when the records hold a byte, or in _dev when n_records > 0); in the host call, group offsets that do not partition
+ *     the records or record offsets that decrease: all PG_ERR_ARG.  PG_ERR_NOMEM when device memory runs out.
+ *     n_groups == 0 is valid and needs no buffers.  _dev trusts its offsets as pg_mash_sketch_batch_dev does.
+ *   - Passes: pass t counts, for every group still open, the windows whose hash lies in the group's next range of
+ *     values into an open-addressing table; values with count >= min_copies are appended to the row.  The first
+ *     range admits about s + 6 sqrt(s) + 48 windows, so a genome of distinct windows finishes in one pass; a read set
+ *     filtered at min_copies >= 2 takes a few.  Later passes walk only the records of open groups.  _dev
+ *     synchronises `stream` (the host decides the passes).
+ *   - Device memory: 8 (n_records + 1) x 2 + 16 (n_groups + 1) + 32 n_groups bytes besides the caller's buffers,
+ *     and per pass 32 bytes per table slot, at most 2^26 slots (2 GiB); a table holds twice the distinct values its
+ *     range is expected to admit.  The host call also stages the bases, offsets, rows and counts. */
+int pg_mash_sketch_groups(const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets,
+                          uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t *out, uint64_t row_stride,
+                          uint32_t *count);
+int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
+                              uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t *d_out, uint64_t row_stride,
+                              uint32_t *d_count, void *stream);
 
 /* ---- single-process multi-GPU (SURVEY.md 8b "multi-GPU variants taking a device count", 8e) ----
  * What a Go host calls to reach all GPUs of the box with ONE call: reads are independent

@@ -52,6 +52,9 @@ _SIGS = {
     "pg_mash_sketch_uniform": (C.c_int, [_u8p, C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _i32p]),
     "pg_mash_sketch_batch_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _u32p, _i32p, C.c_void_p]),
     "pg_mash_sketch_uniform_dev": (C.c_int, [_u8p, C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _i32p, C.c_void_p]),
+    "pg_mash_sketch_groups": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _u32p]),
+    "pg_mash_sketch_groups_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _u32p,
+                                            C.c_void_p]),
     "pg_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p]),
     "pg_ipc_import": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "pg_ipc_close": (C.c_int, [C.c_void_p]),

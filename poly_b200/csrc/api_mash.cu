@@ -739,6 +739,17 @@ static int screen_tally_dev(const pg_mash_screen *sc, ScreenTally tally, uint32_
     return tally(sc->ix, first, count, d_shared, d_containment, d_multiplicity, (cudaStream_t)stream);
 }
 
+// The argument rules of pg_mash_sketch_groups and its _dev form that need no buffer, in their order
+static int sketch_groups_check(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t row_stride, const void *out,
+                               const void *count) {
+    if (n_groups && (!out || !count)) { set_error("null out or count"); return PG_ERR_ARG; }
+    if (k < 0) { set_error("kmerSize %d < 0: the reference panics (slice bounds)", k); return PG_ERR_ARG; }
+    if (s < 1) { set_error("sketchSize %d < 1: a grouped sketch holds at least one value", s); return PG_ERR_ARG; }
+    if (min_copies < 1) { set_error("min_copies 0: every value occurs at least once"); return PG_ERR_ARG; }
+    if (row_stride < (uint64_t)s) { set_error("row_stride %llu < sketchSize %d", (unsigned long long)row_stride, s); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
 }  // namespace
 }  // namespace pg
 
@@ -774,6 +785,42 @@ int pg_mash_sketch_batch_dev(const uint8_t *d_bases, const uint64_t *d_offsets, 
     if ((rc = check_row_stride(row_stride, max_read_len, k, s, flags)) != PG_OK) return rc;
     return launch_sketch_ragged(d_bases, d_offsets, n_reads, max_read_len, k, s, flags, d_out,
                                 row_stride, d_count, d_status, (cudaStream_t)stream);
+}
+
+int pg_mash_sketch_groups(const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets, uint64_t n_groups,
+                          int32_t k, int32_t s, uint32_t min_copies, uint32_t *out, uint64_t row_stride, uint32_t *count) {
+    int rc = sketch_groups_check(n_groups, k, s, min_copies, row_stride, out, count);
+    if (rc != PG_OK || n_groups == 0) return rc;
+    if (!group_offsets || !offsets || (!bases && offsets[n_records] != offsets[0])) { set_error("null buffer"); return PG_ERR_ARG; }
+    uint64_t longest = 0;  // the groups partition the records: ragged offsets over the records, from 0 to n_records
+    if ((rc = check_ragged(group_offsets, n_groups, &longest)) != PG_OK) return rc;
+    if (group_offsets[0] != 0 || group_offsets[n_groups] != n_records) {
+        set_error("group offsets run from %llu to %llu, not over the %llu records", (unsigned long long)group_offsets[0],
+                  (unsigned long long)group_offsets[n_groups], (unsigned long long)n_records);
+        return PG_ERR_ARG;
+    }
+    if ((rc = check_ragged(offsets, n_records, &longest)) != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
+    HostCall c;
+    const Ragged<uint8_t> r = c.ragged(bases, offsets, n_records);
+    const uint64_t *d_goff = c.upload(group_offsets, n_groups + 1);
+    uint32_t *d_out = c.alloc<uint32_t>(n_groups * row_stride);
+    uint32_t *d_count = c.alloc<uint32_t>(n_groups);
+    if ((rc = c.error()) || (rc = sketch_groups(r.base, r.off, n_records, d_goff, n_groups, k, s, min_copies, d_out, row_stride, d_count, c.st)))
+        return rc;
+    c.download(out, d_out, n_groups * row_stride);
+    c.download(count, d_count, n_groups);
+    return c.finish();
+}
+
+int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
+                              uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t *d_out, uint64_t row_stride,
+                              uint32_t *d_count, void *stream) {
+    int rc = sketch_groups_check(n_groups, k, s, min_copies, row_stride, d_out, d_count);
+    if (rc != PG_OK || n_groups == 0) return rc;
+    if (!d_group_offsets || !d_offsets || (n_records && !d_bases)) { set_error("null buffer"); return PG_ERR_ARG; }
+    if ((rc = ensure_device()) != PG_OK) return rc;
+    return sketch_groups(d_bases, d_offsets, n_records, d_group_offsets, n_groups, k, s, min_copies, d_out, row_stride, d_count,
+                         (cudaStream_t)stream);
 }
 
 int pg_mash_sketch_uniform_gather_dev(const uint8_t *d_bases, uint64_t n_local, uint32_t read_len,

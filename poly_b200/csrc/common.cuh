@@ -333,6 +333,11 @@ int screen_results(const ScreenIndex &ix, uint32_t first, uint32_t count, uint32
 int screen_winners(const ScreenIndex &ix, uint32_t first, uint32_t count, uint32_t *d_shared, double *d_cont, uint64_t *d_mult,
                    cudaStream_t st);
 void screen_free(ScreenIndex &ix, cudaStream_t st);
+// sketch_groups.cu: row g of d_out (row_stride words, zeroed past its count) = the smallest min(q_g, s) distinct window
+// hashes of group g's records [d_goff[g], d_goff[g + 1]) that occur at least m times, ascending; d_count[g] = how many.
+// Decides its passes on the host, so it synchronises st.  Argument checks are the caller's.
+int sketch_groups(const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_records, const uint64_t *d_goff, uint64_t n_groups, int k, int s,
+                  uint32_t m, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).
 struct AlignScoring;

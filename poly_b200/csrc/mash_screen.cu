@@ -35,6 +35,7 @@
 #include "common.cuh"
 #include "kmer_walk.cuh"
 #include "murmur3.cuh"
+#include "walk_chunk.cuh"
 
 namespace pg {
 
@@ -70,22 +71,6 @@ __device__ __forceinline__ bool screen_find(const ScreenLookup &L, uint64_t scal
     return lo < end && L.vals[lo] == h;
 }
 
-// Whether the window at byte p is one of its read's: p + k < the end of the read that holds p, the first offset
-// above p.  j caches the index of that offset (~0 = not searched yet); a thread's windows only move forward.
-__device__ __forceinline__ bool window_in_read(const uint64_t *off, uint64_t n_reads, uint64_t p, uint32_t k, uint64_t &j) {
-    if (j == ~0ull) {
-        uint64_t lo = 0, hi = n_reads + 1;
-        while (lo < hi) {
-            const uint64_t mid = (lo + hi) >> 1;
-            if (off[mid] > p) hi = mid;
-            else lo = mid + 1;
-        }
-        j = lo;
-    }
-    while (j <= n_reads && off[j] <= p) ++j;
-    return j <= n_reads && p + k < off[j];
-}
-
 // One window of every lane of a converged warp; cand: the lane's hash h is <= vmax.  With SAMPLES, a hit counts into
 // its read's sample, ids[j - 1] (j: the first offset above p; sample 0 when ids is null), or into the sink when that
 // id is not a sample: a select rather than one more condition on the hit, which keeps the walk kernels at their
@@ -105,9 +90,6 @@ __device__ __forceinline__ void screen_hit(const ScreenLookup &L, uint64_t scale
     if (hit && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&L.cnt[d], (unsigned long long)__popc(peers));
 }
 
-// windows per thread of the walk kernel: whole groups of NB word steps, about 64
-__host__ __device__ constexpr uint32_t screen_span(int nb) { return 4u * nb * (16 / nb > 0 ? 16 / nb : 1); }
-
 // EMIT of the walk: the hash of window p0 + i + R_.  The vote keeps the common case (no lane has a candidate) to
 // one compare and one vote per window.
 #define PG_SCREEN_EMIT(R_, H_)                                                                                              \
@@ -125,7 +107,7 @@ __global__ void __launch_bounds__(SCREEN_THREADS, 2)
 screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ off, uint64_t n_reads, const ScreenLookup L,
                    uint32_t lut_stride) {
     PG_WALK_CONSTANTS;
-    constexpr uint32_t W = screen_span(NB);
+    constexpr uint32_t W = walk_span(NB);
     constexpr uint32_t CHUNK = SCREEN_THREADS * W;
     constexpr uint32_t STAGE = CHUNK + 128;  // + head (< 16) + the walk's look-ahead (< 4 NB + 20 bytes)
     constexpr uint32_t nk = W;               // PG_KMER_STEP's bound; unchecked steps never test it
@@ -141,24 +123,9 @@ screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict
 
     for (uint64_t c = blockIdx.x; c < chunks; c += gridDim.x) {
         const uint64_t P0 = lo + c * CHUNK;
-        const uint32_t head = (uint32_t)((uintptr_t)(bases + P0) & 15u);
-        const int64_t q_base = (int64_t)P0 - (int64_t)head;  // pool position of staged byte 0
-        const uint8_t *g = bases + P0 - head;
+        const uint32_t head = chunk_head(bases, P0);
         __syncthreads();  // the previous chunk's walk is done with s_in (and, the first time, s_lut is written)
-        for (uint32_t x = tid; x < STAGE / 16; x += SCREEN_THREADS) {
-            const int64_t q = q_base + 16 * (int64_t)x;
-            uint4 v;
-            if (q >= (int64_t)lo && q + 16 <= (int64_t)hi) {
-                v = __ldg(reinterpret_cast<const uint4 *>(g) + x);
-            } else {
-                uint8_t b[16];
-#pragma unroll
-                for (int t = 0; t < 16; ++t) b[t] = (q + t >= (int64_t)lo && q + t < (int64_t)hi) ? __ldg(g + 16 * x + t) : (uint8_t)0;
-                v = make_uint4(b[0] | b[1] << 8 | b[2] << 16 | (uint32_t)b[3] << 24, b[4] | b[5] << 8 | b[6] << 16 | (uint32_t)b[7] << 24,
-                               b[8] | b[9] << 8 | b[10] << 16 | (uint32_t)b[11] << 24, b[12] | b[13] << 8 | b[14] << 16 | (uint32_t)b[15] << 24);
-            }
-            reinterpret_cast<uint4 *>(s_in)[x] = v;
-        }
+        stage_chunk<STAGE, SCREEN_THREADS>(s_in, bases, P0, head, lo, hi);
         __syncthreads();
 
         const uint32_t b0 = head + tid * W;

@@ -173,6 +173,74 @@ def SketchBatch(sequences: Sequence[BytesLike], kmer_size: int, sketch_size: int
     return res
 
 
+def _group_args(k: int, s: int, min_copies: int) -> None:
+    if not 0 <= k < (1 << 31):
+        raise PolyError(_lib.PG_ERR_ARG, f"k-mer size {k}: need 0 <= k < 2^31")
+    if not 1 <= s < (1 << 31):
+        raise PolyError(_lib.PG_ERR_ARG, f"sketch size {s}: need 1 <= s < 2^31")
+    if not 1 <= min_copies < (1 << 32):
+        raise PolyError(_lib.PG_ERR_ARG, f"min_copies {min_copies}: need 1 <= min_copies < 2^32")
+
+
+def sketch_groups(bases, offsets, group_offsets, k: int, s: int, min_copies: int = 1):
+    """One sketch per group of records (Mash's `mash sketch` of a multi-FASTA file, or `-r -m min_copies` of a read
+    set): group g is records [group_offsets[g], group_offsets[g+1]) of the ragged batch (bases, offsets).  Row g holds
+    the smallest min(q_g, s) distinct window hashes of the group that occur at least min_copies times, ascending, then
+    zeros; count[g] is how many.  Windows never cross a record.  Returns (rows [G, s] uint32, count [G] uint32): NumPy
+    arrays for host inputs; for CUDA tensor inputs (uint8 bases, int64 offsets holding uint64 bits) int32 CUDA tensors
+    holding the uint32 bits, computed on the current stream (the call waits for it)."""
+    k, s, min_copies = int(k), int(s), int(min_copies)
+    _group_args(k, s, min_copies)
+    if hasattr(bases, "data_ptr"):
+        import torch
+
+        G = max(int(group_offsets.numel()) - 1, 0)
+        n = max(int(offsets.numel()) - 1, 0)
+        for name, t in (("offsets", offsets), ("group_offsets", group_offsets)):
+            if t.element_size() != 8 or not t.is_contiguous():
+                raise ValueError(f"{name} must be a contiguous 64-bit tensor")
+        rows = torch.empty((G, s), dtype=torch.int32, device=bases.device)
+        count = torch.empty(G, dtype=torch.int32, device=bases.device)
+        st = torch.cuda.current_stream(bases.device).cuda_stream
+        _lib.check(_lib.lib().pg_mash_sketch_groups_dev(bases.data_ptr() if bases.numel() else None, offsets.data_ptr() if n or G else None, n,
+                                                        group_offsets.data_ptr() if G else None, G, k, s, min_copies, rows.data_ptr(), s,
+                                                        count.data_ptr(), st))
+        return rows, count
+    bases = np.ascontiguousarray(bases, dtype=np.uint8)
+    offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+    group_offsets = np.ascontiguousarray(group_offsets, dtype=np.uint64)
+    if offsets.ndim != 1 or group_offsets.ndim != 1 or len(offsets) < 1 or len(group_offsets) < 1:
+        raise ValueError("offsets and group_offsets must be 1-d with at least one entry")
+    n, G = len(offsets) - 1, len(group_offsets) - 1
+    rows = np.zeros((G, s), np.uint32)
+    count = np.zeros(G, np.uint32)
+    if len(bases) == 0:
+        bases = np.zeros(1, np.uint8)
+    _lib.check(_lib.lib().pg_mash_sketch_groups(bases.ctypes.data, offsets.ctypes.data, n, group_offsets.ctypes.data, G, k, s, min_copies,
+                                                rows.ctypes.data, s, count.ctypes.data))
+    return rows, count
+
+
+def SketchGroups(groups: Sequence[Sequence[BytesLike]], kmer_size: int, sketch_size: int, min_copies: int = 1) -> List[Mash]:
+    """[][]string -> []*Mash: one Mash per group of sequences (an assembly's contigs, a sample's reads), holding the
+    smallest sketch_size distinct window hashes of the group seen at least min_copies times, ascending, and a zero
+    tail when fewer qualify.  The result compares with Similarity / Distance and feeds every sketch-set call."""
+    if isinstance(groups, (str, bytes)) or any(isinstance(g, (str, bytes, bytearray, np.ndarray)) for g in groups):
+        raise ValueError("groups must be a list of lists of sequences")
+    seqs = [q for g in groups for q in g]
+    bases, offsets = flatten(seqs)
+    goff = np.zeros(len(groups) + 1, np.uint64)
+    if groups:
+        goff[1:] = np.cumsum([len(g) for g in groups], dtype=np.uint64)
+    rows, count = sketch_groups(bases, offsets, goff, kmer_size, sketch_size, min_copies)
+    res = []
+    for g in range(len(groups)):
+        m = Mash(kmer_size, sketch_size)
+        m.Sketches[:] = rows[g]
+        res.append(m)
+    return res
+
+
 def similarity_pairs(mashes: Sequence[Mash], pairs: np.ndarray):
     """Explicit pair list (receiver, argument) over sketches of mixed sizes -> (same, similarity, distance)."""
     arrs = [np.ascontiguousarray(m.Sketches[: m.SketchSize], dtype=np.uint32) for m in mashes]
