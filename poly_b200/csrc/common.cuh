@@ -35,6 +35,9 @@ int func_smem(const void *kernel, size_t bytes);
 // Grid of a kernel that loops over its work items: func_smem, then as many CTAs as are resident at once (at least
 // one per SM), but no more than `work` (runtime.cu)
 int resident_blocks(const void *kernel, int threads, size_t smem, uint64_t work, uint64_t *blocks);
+// The n_reads + 1 offsets of a ragged batch copied to the host, for launchers that cut a batch into launch groups by
+// row length; synchronises st (runtime.cu)
+int host_row_starts(const uint64_t *d_offsets, uint64_t n_reads, cudaStream_t st, std::vector<uint64_t> &off);
 
 // transform.complementTable (transform.go:78-109): every unlisted byte maps to 0, including the DNA
 // letters U and Z.  Seqhash reads it on upper-cased bytes; the clone ligation on fragments as given.

@@ -68,6 +68,13 @@ int resident_blocks(const void *fn, int threads, size_t smem, uint64_t work, uin
     return PG_OK;
 }
 
+int host_row_starts(const uint64_t *d_offsets, uint64_t n_reads, cudaStream_t st, std::vector<uint64_t> &off) {
+    off.resize(n_reads + 1);
+    PG_CUDA(cudaMemcpyAsync(off.data(), d_offsets, (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
+}
+
 // create (once) the context of `device`; g_init_mu held
 static int ctx_create_locked(int device) {
     DevCtx &c = g_ctx[device];

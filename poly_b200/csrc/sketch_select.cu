@@ -989,11 +989,12 @@ static int try_select_sliced(const uint8_t *d_bases, const uint64_t *d_offsets, 
     *sliced = false;
     const uint64_t slots = (uint64_t)sm_count() * 3;
     if (s < 2 || n_reads > 4 * slots) return PG_OK;  // s == 1 needs the positional panic rule; enough rows already
-    std::vector<uint64_t> off(n_reads + 1);
+    std::vector<uint64_t> off;
     if (d_offsets) {
-        PG_CUDA(cudaMemcpyAsync(off.data(), d_offsets, (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaStreamSynchronize(st));
+        const int rc = host_row_starts(d_offsets, n_reads, st, off);
+        if (rc != PG_OK) return rc;
     } else {
+        off.resize(n_reads + 1);
         for (uint64_t r = 0; r <= n_reads; ++r) off[r] = r * (uint64_t)read_len;
     }
     uint64_t total = 0, rows_sel = 0;
@@ -1066,8 +1067,8 @@ static int launch_select_thresh(const uint8_t *d_bases, const uint64_t *d_offset
     const uint32_t mu = (uint32_t)s + 6u * (uint32_t)ceil(sqrt((double)s)) + 48u;
     uint32_t cap = mu + 8u * (uint32_t)ceil(sqrt((double)mu)) + 96u;
     cap = (cap + 3u) & ~3u;
+    // smem_b stays below 80 KiB for every s <= SEL_MAX_S (tests/test_sketch_smem.py checks each s)
     const size_t smem_a = SeltGeom<K>::SMEM_BYTES, smem_b = SeltSelLayout(cap).bytes();
-    if (smem_b > 220 * 1024) return PG_OK;
     // admission probability of the longest rows: below 1/512 a warp step (128 hashes) admits something a quarter of the time
     const uint32_t tm1_u = d_offsets ? 0u : selt_threshold_m1(nmax, mu);  // every row of a fixed-length batch has n == nmax
     const bool rare = (uint64_t)mu * 512 < nmax;

@@ -179,9 +179,8 @@ int launch_sketch_select_large(const uint8_t *d_bases, const uint64_t *d_offsets
     // row starts on the host: groups are cut where the temporaries reach the budget
     std::vector<uint64_t> off;
     if (d_offsets) {
-        off.resize(n_reads + 1);
-        PG_CUDA(cudaMemcpyAsync(off.data(), d_offsets, (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
-        PG_CUDA(cudaStreamSynchronize(st));
+        const int rc = host_row_starts(d_offsets, n_reads, st, off);
+        if (rc != PG_OK) return rc;
     }
     auto row_beg = [&](uint64_t r) -> uint64_t { return d_offsets ? off[r] : r * (uint64_t)read_len; };
     uint64_t P = 2;

@@ -185,6 +185,29 @@ def test_select_regime_long_reads_with_pruning(gpu, oracle):
     assert rc == 0 and not status.any()
     assert np.array_equal(count, np.minimum(np.maximum(np.array(lens) - k, 0), s))
     assert np.array_equal(out, want)
+    # A larger ragged batch that K2t declines: about 25 k short reads with two 8 Mbp rows and a stretch of fill-only rows
+    # between them.  It has too many rows to slice, so the streaming kernel takes every select-regime row directly.
+    lens = [int(x) for x in rng.integers(100, 3_000, 6_000)] + [8_000_000] + [int(x) for x in rng.integers(0, s + k, 12_000)] + \
+           [8_000_003] + [int(x) for x in rng.integers(100, 3_000, 6_000)]
+    n_rows = len(lens)
+    assert n_rows > 4 * 3 * sms.value and n_rows * -(-(max(lens) - k) // (8 * 32 * 60)) > 4 << 20
+    seqs = [bytes(rng.choice(list(b"ACGT"), size=l).astype(np.uint8)) for l in lens]
+    bases, offsets = mash.flatten(seqs)
+    d_bases = torch.from_numpy(bases).to(dev)
+    d_off = torch.from_numpy(offsets.astype(np.int64)).to(dev)
+    d_out = torch.empty((n_rows, s), dtype=torch.int32, device=dev)
+    d_count = torch.empty(n_rows, dtype=torch.int32, device=dev)
+    d_status = torch.empty(n_rows, dtype=torch.int32, device=dev)
+    before = L_.pg_launch_count()
+    _lib.check(L_.pg_mash_sketch_batch_dev(d_bases.data_ptr(), d_off.data_ptr(), n_rows, max(lens), k, s, _lib.PG_SKETCH_PAD_ZERO,
+                                           d_out.data_ptr(), s, d_count.data_ptr(), d_status.data_ptr(), st))
+    assert L_.pg_launch_count() - before == 2 and L_.pg_last_kernel() == b"sketch_select_walk_kernel"  # the fill kernel, then K2w
+    torch.cuda.synchronize(dev)
+    out, count, status = d_out.cpu().numpy().view(np.uint32), d_count.cpu().numpy(), d_status.cpu().numpy()
+    rc, want = oracle.sketch_batch(bases, offsets, k, s, variant=1, nthreads=os.cpu_count() or 1)
+    assert rc == 0 and not status.any()
+    assert np.array_equal(count, np.minimum(np.maximum(np.array(lens) - k, 0), s))
+    assert np.array_equal(out, want)
 
 
 def test_cfg3_shape_sample_golden(gpu, oracle):

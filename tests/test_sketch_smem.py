@@ -80,6 +80,7 @@ int main() {
             const SeltSelLayout b(cap);
             CHECK(b.bytes() == ((((size_t)cap + 3) & ~(size_t)3) + 2048 + 16) * 4, "K2t B cap=%u", cap);
             CHECK(b.tmp == 0 && b.cur >= cap && b.cur % 4 == 0 && b.flag == b.cur + SEL_NBK && b.words > b.flag, "K2t B cap=%u regions", cap);
+            CHECK(b.bytes() <= 80 * 1024, "K2t B s=%u cap=%u: %zu bytes of shared memory", s, cap, b.bytes());
         }
     }
     // K1: 2 input stages | out tile [32][nk]

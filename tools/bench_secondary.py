@@ -1,9 +1,12 @@
 #!/usr/bin/env python
 """Timings of the non-headline kernels on their BASELINE configs (device-resident, CUDA events):
-cfg3 (100k x 10 kbp, k=31, s=2000: K2 sketch + K3 all-pairs on a row block) and cfg5
+cfg3 (100k x 10 kbp, k=31, s=2000: K2 sketch + K3 all-pairs on a row block), ragged K2 batches of genomes
+among short reads, and cfg5
 (1M x 25 bp primers vs a 10 kb template: K4 SW score, K5 Tm).  Prints one JSON line per kernel;
 copy into profiles/.  Not the driver's bench (that is bench.py)."""
 import argparse
+import ctypes as C
+import hashlib
 import json
 import os
 import sys
@@ -19,7 +22,7 @@ ap.add_argument("--reads", type=int, default=100_000)
 ap.add_argument("--rows", type=int, default=512, help="row block of the all-pairs matrix to time")
 ap.add_argument("--primers", type=int, default=1_000_000)
 ap.add_argument("--iters", type=int, default=3)
-ap.add_argument("--only-k2", action="store_true", help="stop after the K2 legs (cfg3, genomes, one genome, K2x)")
+ap.add_argument("--only-k2", action="store_true", help="stop after the K2 legs (cfg3, genomes, one genome, K2x, ragged)")
 args = ap.parse_args()
 
 L = _lib.lib()
@@ -71,7 +74,56 @@ gx = d_xsk.cpu().numpy().view(np.uint32)
 print(json.dumps({"kernel": "K2x large sketch (64 x 4 Mbp genomes, s = 100000)", "k": gk, "s": xs, "ms": ms_x, "gbases_per_s": xn * gL / ms_x / 1e6,
                   "ascending": bool((np.diff(gx.astype(np.int64), axis=1) >= 0).all()),
                   "head_equals_s1000_sketch": bool((gx[:, :gs] == g[:xn]).all()), "kernel_name": L.pg_last_kernel().decode()}))
-del d_gen, d_xsk
+del d_xsk
+
+
+# ---- ragged select-regime batches (k = 21, s = 1000) through pg_mash_sketch_batch_dev ----------------------------------
+# K2t cuts a ragged batch past 4 Mi row x work-item slots of its longest row into launch groups by each group's own
+# longest row; (a) and (b) are past that bound, (c) is a control under it.  The SHA-256 of rows and counts lets two
+# builds of the library be compared for identical results.
+def sha(*arrays):
+    h = hashlib.sha256()
+    for a in arrays:
+        h.update(memoryview(np.ascontiguousarray(a)).cast("B"))
+    return h.hexdigest()[:16]
+
+
+def ragged_leg(name, d_src, lens):
+    offs = np.zeros(len(lens) + 1, dtype=np.int64)
+    offs[1:] = np.cumsum(lens)
+    assert offs[-1] <= d_src.numel()
+    d_o = torch.from_numpy(offs).to(dev)
+    d_out = torch.empty((len(lens), gs), dtype=torch.int32, device=dev)
+    d_c = torch.empty(len(lens), dtype=torch.int32, device=dev)
+
+    def call():
+        _lib.check(L.pg_mash_sketch_batch_dev(d_src.data_ptr(), d_o.data_ptr(), len(lens), int(max(lens)), gk, gs, _lib.PG_SKETCH_PAD_ZERO,
+                                              d_out.data_ptr(), gs, d_c.data_ptr(), None, st))
+    ms = timed(call)
+    n0 = L.pg_launch_count()
+    call()
+    launches = L.pg_launch_count() - n0
+    torch.cuda.synchronize()
+    print(json.dumps({"kernel": f"K2 ragged sketch ({name})", "k": gk, "s": gs, "rows": len(lens), "bases": int(offs[-1]), "ms": ms,
+                      "gbases_per_s": float(offs[-1]) / ms / 1e6, "launches": launches, "kernel_name": L.pg_last_kernel().decode(),
+                      "sha256": sha(d_out.cpu().numpy(), d_c.cpu().numpy())}))
+
+
+rng_r = np.random.default_rng(21)
+sms = C.c_int(0)
+_lib.check(L.pg_device_sm_count(C.byref(sms)))
+n_a = 4 * 3 * sms.value - 1
+lens_a = [((4 << 20) // n_a + 1) * 8 * 32 * 60 + gk] + [int(x) for x in rng_r.integers(2_000, 60_000, 10)] + \
+         [int(x) for x in rng_r.integers(0, gs + gk, n_a - 11)]
+rng_r.shuffle(lens_a)
+ragged_leg(f"a: {n_a} rows, one of {lens_a[int(np.argmax(lens_a))] / 1e6:.1f} Mbp", d_gen, lens_a)
+ragged_leg("b: 100 k x 150 bp reads, 8 x 5 Mbp genomes among them", d_gen, ([150] * 12_500 + [5_000_000]) * 8)
+del d_gen
+cn, cL = 1000, 5_000_000
+d_c5 = torch.empty(cn * cL, dtype=torch.uint8, device=dev)
+_lib.check(L.pg_synth_reads_dev(d_c5.data_ptr(), 0, cn, cL, synth.SEED_READS + 11, 0, 1, st))
+ragged_leg("c: 1000 genomes of 5 Mbp - [0, 1000) bp, under the bound", d_c5, [cL - int(x) for x in rng_r.integers(0, 1000, cn)])
+del d_c5
 if args.only_k2:
     sys.exit(0)
 rows = min(args.rows, n)
@@ -121,7 +173,6 @@ print(json.dumps({"kernel": "K1r ragged fill (2M reads, len 100..150)", "ms": ms
 del rag, d_rout
 
 # ---- widened rows: FASTQ ingest (8f.2) and batched DesignPrimers (8f.3) ------------------------
-import ctypes as C
 from poly_b200 import pcr  # noqa: E402
 
 nrec = 2_000_000
