@@ -102,6 +102,66 @@ func SketchGroups(bases []byte, offsets []uint64, groupOffsets []uint64, k, s in
 	return out[:g*s], count[:g], err
 }
 
+// Sketcher wraps a pg_mash_sketcher: nGroups grouped sketches grown in place, batch by batch, on the device of the
+// calling thread.  Close must not run while another call on it is in flight.
+type Sketcher struct {
+	h    *C.pg_mash_sketcher
+	n, s int
+}
+
+// NewSketcher wraps pg_mash_sketcher_create (maxValues: the most distinct values a group keeps between adds).
+func NewSketcher(nGroups uint64, k, s int, minCopies uint32, maxValues uint64) (*Sketcher, error) {
+	var h *C.pg_mash_sketcher
+	if err := locked(func() C.int {
+		return C.pg_mash_sketcher_create(C.uint64_t(nGroups), C.int32_t(k), C.int32_t(s), C.uint32_t(minCopies), C.uint64_t(maxValues), &h)
+	}); err != nil {
+		return nil, err
+	}
+	return &Sketcher{h: h, n: int(nGroups), s: s}, nil
+}
+
+// Add wraps pg_mash_sketcher_add: records [groupOffsets[i], groupOffsets[i+1]) of the ragged batch (bases, offsets) go
+// to group firstGroup + i.
+func (sk *Sketcher) Add(bases []byte, offsets []uint64, groupOffsets []uint64, firstGroup uint64) error {
+	n, g := len(offsets)-1, len(groupOffsets)-1
+	if n <= 0 {
+		return nil
+	}
+	var b *C.uint8_t
+	if len(bases) > 0 {
+		b = (*C.uint8_t)(unsafe.Pointer(&bases[0]))
+	}
+	return locked(func() C.int {
+		return C.pg_mash_sketcher_add(sk.h, b, (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n),
+			(*C.uint64_t)(unsafe.Pointer(&groupOffsets[0])), C.uint64_t(firstGroup), C.uint64_t(g))
+	})
+}
+
+// Rows wraps pg_mash_sketcher_rows over every group: s words per group, the values each row holds, whether it is
+// complete, and the values each group keeps.
+func (sk *Sketcher) Rows() (out []uint32, count []uint32, complete []bool, held []uint64, err error) {
+	out, count, c, held := make([]uint32, sk.n*sk.s+1), make([]uint32, sk.n+1), make([]uint8, sk.n+1), make([]uint64, sk.n+1)
+	err = locked(func() C.int {
+		return C.pg_mash_sketcher_rows(sk.h, 0, C.uint64_t(sk.n), (*C.uint32_t)(unsafe.Pointer(&out[0])), C.uint64_t(sk.s),
+			(*C.uint32_t)(unsafe.Pointer(&count[0])), (*C.uint8_t)(unsafe.Pointer(&c[0])), (*C.uint64_t)(unsafe.Pointer(&held[0])))
+	})
+	complete = make([]bool, sk.n)
+	for i := range complete {
+		complete[i] = c[i] != 0
+	}
+	return out[:sk.n*sk.s], count[:sk.n], complete, held[:sk.n], err
+}
+
+// Close wraps pg_mash_sketcher_free.
+func (sk *Sketcher) Close() error {
+	if sk.h == nil {
+		return nil
+	}
+	h := sk.h
+	sk.h = nil
+	return locked(func() C.int { return C.pg_mash_sketcher_free(h) })
+}
+
 func devicePtr(devices []int32) (*C.int32_t, C.int32_t) {
 	if len(devices) == 0 {
 		return nil, 0 // all visible GPUs

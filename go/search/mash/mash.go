@@ -117,6 +117,66 @@ func SketchGroups(groups [][]string, kmerSize, sketchSize, minCopies int) ([]*Ma
 	return res, nil
 }
 
+// Sketcher grows SketchGroups in place: nGroups sketches fed batch by batch, for read sets larger than the GPU or a
+// host can stage.  Per group it keeps a cap (2^32 at first, never growing) and every value below it with its count
+// saturated at minCopies; after an add the cap is the smallest of the old cap, the sketchSize-th value seen minCopies
+// times plus one, and the (maxValues+1)-th distinct value.  A sketch is complete when it holds sketchSize values or
+// its cap is still 2^32: a complete sketch equals SketchGroups over every sequence added to the group, whatever the
+// split, and every sketch is a prefix of that one.  With minCopies 1 every sketch is complete.  Call Close when done.
+type Sketcher struct {
+	sk           *polyb200.Sketcher
+	k, s, groups int
+}
+
+// NewSketcher prepares nGroups sketches; maxValues <= 0 means 64 * sketchSize.
+func NewSketcher(nGroups, kmerSize, sketchSize, minCopies, maxValues int) (*Sketcher, error) {
+	if nGroups < 0 || minCopies < 1 || minCopies > math.MaxUint32 {
+		return nil, fmt.Errorf("mash: nGroups %d or minCopies %d out of range", nGroups, minCopies)
+	}
+	if maxValues <= 0 {
+		maxValues = 64 * sketchSize
+	}
+	sk, err := polyb200.NewSketcher(uint64(nGroups), kmerSize, sketchSize, uint32(minCopies), uint64(maxValues))
+	if err != nil {
+		return nil, err
+	}
+	return &Sketcher{sk: sk, k: kmerSize, s: sketchSize, groups: nGroups}, nil
+}
+
+// Add counts the sequences of groups[i] into group firstGroup + i.
+func (s *Sketcher) Add(groups [][]string, firstGroup int) error {
+	if firstGroup < 0 {
+		return fmt.Errorf("mash: firstGroup %d out of range", firstGroup)
+	}
+	var seqs []string
+	goff := make([]uint64, 1, len(groups)+1)
+	for _, g := range groups {
+		seqs = append(seqs, g...)
+		goff = append(goff, uint64(len(seqs)))
+	}
+	if len(seqs) == 0 {
+		return nil
+	}
+	bases, offsets := polyb200.Flatten(seqs)
+	return s.sk.Add(bases, offsets, goff, uint64(firstGroup))
+}
+
+// Sketches returns one sketch per group so far, and whether each is complete.
+func (s *Sketcher) Sketches() ([]*Mash, []bool, error) {
+	out, _, complete, _, err := s.sk.Rows()
+	if err != nil {
+		return nil, nil, err
+	}
+	res := make([]*Mash, s.groups)
+	for g := range res {
+		res[g] = &Mash{KmerSize: s.k, SketchSize: s.s, Sketches: out[g*s.s : (g+1)*s.s : (g+1)*s.s]}
+	}
+	return res, complete, nil
+}
+
+// Close releases the sketcher's device memory.
+func (s *Sketcher) Close() error { return s.sk.Close() }
+
 // DistanceMatrix returns D[i][j] = sketches[i].Distance(sketches[j]) for sketches of one common SketchSize.
 func DistanceMatrix(sketches []*Mash) [][]float64 {
 	n := len(sketches)

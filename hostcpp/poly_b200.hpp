@@ -156,6 +156,53 @@ inline std::vector<Mash> SketchGroups(const std::vector<std::vector<std::string>
     return res;
 }
 
+// Grouped sketches grown in place (pg_mash_sketcher): nGroups sketches fed batch by batch, each add counting its
+// sequences into one group or a run of groups.  A row is complete when it holds s values or the group's cap is still
+// 2^32; a complete row equals SketchGroups over every sequence added to the group, whatever the split, and every row
+// is a prefix of it.  maxValues (0: 64 s) is the most distinct values a group keeps between adds.
+class Sketcher {
+public:
+    Sketcher(uint64_t nGroups, int k, int s, uint32_t minCopies, uint64_t maxValues = 0) : k_(k), s_(s), n_(nGroups) {
+        check(pg_mash_sketcher_create(nGroups, k, s, minCopies, maxValues ? maxValues : 64 * (uint64_t)std::max(s, 1), &h_));
+    }
+    Sketcher(const Sketcher &) = delete;
+    Sketcher &operator=(const Sketcher &) = delete;
+    ~Sketcher() { pg_mash_sketcher_free(h_); }
+    // sequences of groups [firstGroup, firstGroup + groups.size()), groups[i] going to group firstGroup + i
+    void Add(const std::vector<std::vector<std::string>> &groups, uint64_t firstGroup = 0) {
+        std::vector<std::string> seqs;
+        std::vector<uint64_t> goff(1, 0);
+        for (const auto &g : groups) {
+            seqs.insert(seqs.end(), g.begin(), g.end());
+            goff.push_back(seqs.size());
+        }
+        Flat f(seqs);
+        check(pg_mash_sketcher_add(h_, f.bases.data(), f.offsets.data(), seqs.size(), goff.data(), firstGroup, groups.size()));
+    }
+    void AddRecords(uint64_t group, const std::vector<std::string> &seqs) { Add({seqs}, group); }
+    // one Mash per group; count, complete and held (each may be null) receive the row sizes, whether each row is
+    // complete, and the values each group holds
+    std::vector<Mash> Sketches(std::vector<uint32_t> *count = nullptr, std::vector<uint8_t> *complete = nullptr,
+                               std::vector<uint64_t> *held = nullptr) const {
+        std::vector<uint32_t> out(n_ * s_), cnt(n_);
+        std::vector<uint8_t> c(n_);
+        std::vector<uint64_t> h(n_);
+        check(pg_mash_sketcher_rows(h_, 0, n_, out.data(), s_, cnt.data(), c.data(), h.data()));
+        std::vector<Mash> res;
+        res.reserve(n_);
+        for (uint64_t g = 0; g < n_; ++g) res.push_back(Mash{k_, s_, std::vector<uint32_t>(out.begin() + g * s_, out.begin() + (g + 1) * s_)});
+        if (count) *count = cnt;
+        if (complete) *complete = c;
+        if (held) *held = h;
+        return res;
+    }
+
+private:
+    pg_mash_sketcher *h_ = nullptr;
+    int k_, s_;
+    uint64_t n_;
+};
+
 // In-place form: `slab` holds the Sketches arrays of seqs.size() Mash values back to back (n x s words).  Row i
 // receives its min(len_i - k, s) words, the rest of the row is left as it is -- what (*Mash).Sketch does to an
 // existing Mash (mash.go:73-80); a zeroed slab ends up as n fresh sketches.  Returns the per-read counts.

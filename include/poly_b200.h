@@ -29,7 +29,8 @@
  *     for its own kernels), and
  *     pg_mash_sketch_batch_dev for ragged batches the threshold path does not take
  *     (s < 2, or more than 4 Mi row x item slots) when they hold few long sequences, and
- *     pg_mash_sketch_groups_dev (it sizes and decides its passes over hash ranges on the host);
+ *     pg_mash_sketch_groups_dev and pg_mash_sketcher_add_dev (they size and decide their passes over hash ranges on
+ *     the host);
  *   - a ragged batch of n items passes n + 1 offsets, item i being [offsets[i], offsets[i+1]).
  *     Offsets must not decrease: the host-pointer entry points return PG_ERR_ARG if they do,
  *     without launching anything;
@@ -196,6 +197,64 @@ int pg_mash_sketch_groups(const uint8_t *bases, const uint64_t *offsets, uint64_
 int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
                               uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t *d_out, uint64_t row_stride,
                               uint32_t *d_count, void *stream);
+
+/* ---- grouped sketch grown in place: read sets larger than device memory, added batch by batch ----
+ * A sketcher holds G groups (fixed at create), k, s, m = min_copies and a budget B = max_values: the most distinct
+ * values one group keeps between adds.  Windows are exactly those of pg_mash_sketch_groups: positions 0 .. L - k - 1
+ * of each record, murmur3 over the raw bytes, forward strand, never crossing a record.  c_g(v) = the windows of every
+ * record added to group g so far whose hash is v.
+ *   - Per group the sketcher keeps a cap C_g, which starts at 2^32 and never grows, and a state: every value v < C_g
+ *     with c_g(v) >= 1, and beside each one min(c_g(v), m).  Invariant: every count below C_g is exact.  An add of
+ *     records to group g:
+ *       1. V = the distinct values below the old C_g, with counts over the old state plus this batch's windows;
+ *          Q = {v in V : c >= m}.
+ *       2. t_s = (s-th smallest value of Q) + 1, or 2^32 if |Q| < s.  Lossless: counts only grow, so no value at or
+ *          above t_s can ever enter the row.
+ *       3. t_B = the (B+1)-th smallest value of V, or 2^32 if |V| <= B.  This is the budget.
+ *       4. C_g = min(C_g, t_s, t_B); the state keeps V below it.
+ *     Batch windows at or above the old C_g are discarded.  Groups that get no records in an add are unchanged.
+ *   - Rows, readable at any time, changing nothing: row g holds the values of Q below C_g, ascending: n_values[g] =
+ *     min(|Q below C_g|, s) of them, then zeros up to row_stride.  complete[g] = (n_values[g] == s) || (C_g == 2^32).
+ *     held[g] = the number of values in the state.
+ *   - Properties:
+ *       complete => equal: if complete[g], row g and n_values[g] equal pg_mash_sketch_groups over the concatenation
+ *         of every record added to g, byte for byte, whatever the split (empty adds, one-record adds, a group spread
+ *         over many adds, adds that start or end inside a group);
+ *       always a prefix: row g is always the first n_values[g] words of that one-shot row (the values below C_g are
+ *         the smallest qualifying values overall, and their counts are exact);
+ *       with m = 1 every group is always complete and held[g] <= s after every add.
+ *     held shows how close a group is to its budget; an incomplete group asks for a larger max_values.
+ *   - Batch layout: records [group_offsets[i], group_offsets[i+1]) of the batch belong to group first_group + i, with
+ *     group_offsets[0] == 0 and group_offsets[n_batch_groups] == n_records (the one-shot layout with a group base).
+ *   - Errors, checked in this order before any device work (PG_ERR_ARG):
+ *       create: a null out; n_groups == 0 or n_groups > 2^32 - 1; k < 0; s < 1; min_copies < 1; max_values < s.
+ *       add: a null sketcher (no device needed); n_records == 0 with n_batch_groups == 0 is a valid no-op;
+ *         first_group + n_batch_groups > G; n_records == 0 is then a valid no-op; a null offsets or group_offsets, or a
+ *         null bases (in the host add only when the records hold a byte); in the host add, group offsets that do not
+ *         partition the records, or record offsets that decrease.  add_dev trusts its offsets.
+ *       rows: a null sketcher; first + count > G; row_stride < s; a null out or n_values with count > 0.  complete and
+ *         held may be NULL.
+ *     PG_ERR_NOMEM when memory runs out.  After any error the sketcher holds exactly what it held before: an add builds
+ *     the new state in new buffers and swaps it in at the end.
+ *   - Synchronisation: add_dev synchronises its stream (the host plans the passes); rows_dev only enqueues, and a later
+ *     add waits for it on the device before it releases the state rows_dev reads.
+ *   - Threads: one lock per sketcher; adds are serialised and rows waits for a running add.  The sketcher lives on the
+ *     device current at create.
+ *   - Device memory: the state takes 8 bytes per held value (uint32 value, uint32 saturated count), plus 8 (G + 1)
+ *     bytes of segment offsets and 8 G of caps.  During an add: the old and the new state together, the add's list of
+ *     kept values (12 bytes each, twice while it is sorted), and per pass 44 bytes per table slot, at most 2^26 slots;
+ *     a table holds twice the distinct values its range is expected to admit.  The host add also stages the batch. */
+typedef struct pg_mash_sketcher pg_mash_sketcher;
+int pg_mash_sketcher_create(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t max_values, pg_mash_sketcher **out);
+int pg_mash_sketcher_add(pg_mash_sketcher *sk, const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets,
+                         uint64_t first_group, uint64_t n_batch_groups);
+int pg_mash_sketcher_add_dev(pg_mash_sketcher *sk, const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records,
+                             const uint64_t *d_group_offsets, uint64_t first_group, uint64_t n_batch_groups, void *stream);
+int pg_mash_sketcher_rows(const pg_mash_sketcher *sk, uint64_t first, uint64_t count, uint32_t *out, uint64_t row_stride, uint32_t *n_values,
+                          uint8_t *complete, uint64_t *held);
+int pg_mash_sketcher_rows_dev(const pg_mash_sketcher *sk, uint64_t first, uint64_t count, uint32_t *d_out, uint64_t row_stride,
+                              uint32_t *d_n_values, uint8_t *d_complete, uint64_t *d_held, void *stream);
+int pg_mash_sketcher_free(pg_mash_sketcher *sk);
 
 /* ---- single-process multi-GPU (SURVEY.md 8b "multi-GPU variants taking a device count", 8e) ----
  * What a Go host calls to reach all GPUs of the box with ONE call: reads are independent

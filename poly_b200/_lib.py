@@ -55,6 +55,12 @@ _SIGS = {
     "pg_mash_sketch_groups": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _u32p]),
     "pg_mash_sketch_groups_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _u32p,
                                             C.c_void_p]),
+    "pg_mash_sketcher_create": (C.c_int, [C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_uint64, C.POINTER(C.c_void_p)]),
+    "pg_mash_sketcher_add": (C.c_int, [C.c_void_p, _u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_uint64]),
+    "pg_mash_sketcher_add_dev": (C.c_int, [C.c_void_p, _u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_uint64, C.c_void_p]),
+    "pg_mash_sketcher_rows": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, _u32p, C.c_uint64, _u32p, _u8p, _u64p]),
+    "pg_mash_sketcher_rows_dev": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, _u32p, C.c_uint64, _u32p, _u8p, _u64p, C.c_void_p]),
+    "pg_mash_sketcher_free": (C.c_int, [C.c_void_p]),
     "pg_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p]),
     "pg_ipc_import": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "pg_ipc_close": (C.c_int, [C.c_void_p]),

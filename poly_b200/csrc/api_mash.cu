@@ -47,6 +47,13 @@ struct pg_mash_screen {
     mutable std::shared_mutex rw;  // results hold it shared while they enqueue, an add or a reset exclusively
 };
 
+struct pg_mash_sketcher {
+    int device;
+    pg::SketcherState st;
+    cudaEvent_t read;       // recorded behind every rows_dev: an add waits for it before it frees the old state
+    mutable std::mutex mu;  // serialises adds, and rows against them
+};
+
 namespace pg {
 namespace {
 
@@ -750,6 +757,38 @@ static int sketch_groups_check(uint64_t n_groups, int32_t k, int32_t s, uint32_t
     return PG_OK;
 }
 
+// The argument rules of pg_mash_sketcher_add and its _dev form that need no buffer content, in their order; *work:
+// whether the add has records to count
+static int sketcher_add_check(const pg_mash_sketcher *sk, const void *bases, const uint64_t *offsets, uint64_t n_records, const void *group_offsets,
+                              uint64_t first, uint64_t nb, bool host, bool *work) {
+    *work = false;
+    if (!sk) { set_error("null sketcher"); return PG_ERR_ARG; }
+    if (n_records == 0 && nb == 0) return PG_OK;
+    if (first > sk->st.G || nb > sk->st.G - first) {
+        set_error("groups [%llu, %llu + %llu) of a sketcher of %llu groups", (unsigned long long)first, (unsigned long long)first,
+                  (unsigned long long)nb, (unsigned long long)sk->st.G);
+        return PG_ERR_ARG;
+    }
+    if (n_records == 0) return PG_OK;
+    // bases may be null in the host add when the records hold no byte
+    if (!offsets || !group_offsets || (!bases && (!host || offsets[n_records] != offsets[0]))) { set_error("null buffer"); return PG_ERR_ARG; }
+    *work = true;
+    return PG_OK;
+}
+
+// The argument rules of pg_mash_sketcher_rows and its _dev form, in their order
+static int sketcher_rows_check(const pg_mash_sketcher *sk, uint64_t first, uint64_t count, const void *out, uint64_t row_stride, const void *n_values) {
+    if (!sk) { set_error("null sketcher"); return PG_ERR_ARG; }
+    if (first > sk->st.G || count > sk->st.G - first) {
+        set_error("rows [%llu, %llu + %llu) of a sketcher of %llu groups", (unsigned long long)first, (unsigned long long)first,
+                  (unsigned long long)count, (unsigned long long)sk->st.G);
+        return PG_ERR_ARG;
+    }
+    if (row_stride < (uint64_t)sk->st.s) { set_error("row_stride %llu < sketchSize %d", (unsigned long long)row_stride, sk->st.s); return PG_ERR_ARG; }
+    if (count && (!out || !n_values)) { set_error("null out or n_values"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
 }  // namespace
 }  // namespace pg
 
@@ -821,6 +860,122 @@ int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets,
     if ((rc = ensure_device()) != PG_OK) return rc;
     return sketch_groups(d_bases, d_offsets, n_records, d_group_offsets, n_groups, k, s, min_copies, d_out, row_stride, d_count,
                          (cudaStream_t)stream);
+}
+
+int pg_mash_sketcher_create(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t max_values, pg_mash_sketcher **out) {
+    if (!out) { set_error("null sketcher pointer"); return PG_ERR_ARG; }
+    *out = nullptr;
+    if (n_groups == 0 || n_groups > 0xffffffffull) { set_error("a sketcher of %llu groups: need 1 .. 2^32 - 1", (unsigned long long)n_groups); return PG_ERR_ARG; }
+    if (k < 0) { set_error("kmerSize %d < 0: the reference panics (slice bounds)", k); return PG_ERR_ARG; }
+    if (s < 1) { set_error("sketchSize %d < 1: a grouped sketch holds at least one value", s); return PG_ERR_ARG; }
+    if (min_copies < 1) { set_error("min_copies 0: every value occurs at least once"); return PG_ERR_ARG; }
+    if (max_values < (uint64_t)s) { set_error("max_values %llu < sketchSize %d", (unsigned long long)max_values, s); return PG_ERR_ARG; }
+    int rc = ensure_device();
+    if (rc != PG_OK) return rc;
+    pg_mash_sketcher *sk = nullptr;
+    try {
+        sk = new pg_mash_sketcher();
+        sk->st.seg.reserve(n_groups + 1);
+        sk->st.cap.reserve(n_groups);
+    } catch (const std::bad_alloc &) {
+        delete sk;
+        set_error("host memory for %llu groups", (unsigned long long)n_groups);
+        return PG_ERR_NOMEM;
+    }
+    sk->device = cur_ctx()->device;
+    sk->st.G = n_groups;
+    sk->st.B = max_values;
+    sk->st.k = k;
+    sk->st.s = s;
+    sk->st.m = min_copies;
+    std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+    cudaStream_t st = cur_ctx()->slots[0].stream;
+    cudaError_t e = cudaEventCreateWithFlags(&sk->read, cudaEventDisableTiming);
+    if (e != cudaSuccess) {
+        delete sk;
+        return cuda_fail(e, "cudaEventCreate", __FILE__, __LINE__);
+    }
+    if ((rc = sketcher_init(sk->st, st)) != PG_OK) {
+        cudaEventDestroy(sk->read);
+        delete sk;
+        return rc;
+    }
+    *out = sk;
+    return PG_OK;
+}
+
+int pg_mash_sketcher_add(pg_mash_sketcher *sk, const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets,
+                         uint64_t first_group, uint64_t n_batch_groups) {
+    bool work = false;
+    int rc = sketcher_add_check(sk, bases, offsets, n_records, group_offsets, first_group, n_batch_groups, true, &work);
+    if (rc != PG_OK || !work) return rc;
+    uint64_t longest = 0;  // the batch's groups partition its records
+    if ((rc = check_ragged(group_offsets, n_batch_groups, &longest)) != PG_OK) return rc;
+    if (group_offsets[0] != 0 || group_offsets[n_batch_groups] != n_records) {
+        set_error("group offsets run from %llu to %llu, not over the %llu records", (unsigned long long)group_offsets[0],
+                  (unsigned long long)group_offsets[n_batch_groups], (unsigned long long)n_records);
+        return PG_ERR_ARG;
+    }
+    if ((rc = check_ragged(offsets, n_records, &longest)) != PG_OK || (rc = use_device(sk->device)) != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(sk->mu);
+    HostCall c;
+    const Ragged<uint8_t> r = c.ragged(bases, offsets, n_records);
+    const uint64_t *d_goff = c.upload(group_offsets, n_batch_groups + 1);
+    if ((rc = c.error())) return rc;
+    PG_CUDA(cudaStreamWaitEvent(c.st, sk->read, 0));
+    if ((rc = sketcher_add(sk->st, r.base, r.off, n_records, d_goff, first_group, n_batch_groups, c.st))) return rc;
+    return c.finish();
+}
+
+int pg_mash_sketcher_add_dev(pg_mash_sketcher *sk, const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records,
+                             const uint64_t *d_group_offsets, uint64_t first_group, uint64_t n_batch_groups, void *stream) {
+    bool work = false;
+    int rc = sketcher_add_check(sk, d_bases, d_offsets, n_records, d_group_offsets, first_group, n_batch_groups, false, &work);
+    if (rc != PG_OK || !work || (rc = use_device(sk->device)) != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(sk->mu);
+    PG_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, sk->read, 0));
+    return sketcher_add(sk->st, d_bases, d_offsets, n_records, d_group_offsets, first_group, n_batch_groups, (cudaStream_t)stream);
+}
+
+int pg_mash_sketcher_rows(const pg_mash_sketcher *sk, uint64_t first, uint64_t count, uint32_t *out, uint64_t row_stride, uint32_t *n_values,
+                          uint8_t *complete, uint64_t *held) {
+    int rc = sketcher_rows_check(sk, first, count, out, row_stride, n_values);
+    if (rc != PG_OK || count == 0 || (rc = use_device(sk->device)) != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(sk->mu);
+    HostCall c;
+    uint32_t *d_out = c.alloc<uint32_t>(count * row_stride), *d_n = c.alloc<uint32_t>(count);
+    uint8_t *d_c = complete ? c.alloc<uint8_t>(count) : nullptr;
+    uint64_t *d_h = held ? c.alloc<uint64_t>(count) : nullptr;
+    if ((rc = c.error()) || (rc = sketcher_rows(sk->st, first, count, d_out, row_stride, d_n, d_c, d_h, c.st))) return rc;
+    c.download(out, d_out, count * row_stride);
+    c.download(n_values, d_n, count);
+    c.download(complete, d_c, count);
+    c.download(held, d_h, count);
+    return c.finish();
+}
+
+int pg_mash_sketcher_rows_dev(const pg_mash_sketcher *sk, uint64_t first, uint64_t count, uint32_t *d_out, uint64_t row_stride, uint32_t *d_n_values,
+                              uint8_t *d_complete, uint64_t *d_held, void *stream) {
+    int rc = sketcher_rows_check(sk, first, count, d_out, row_stride, d_n_values);
+    if (rc != PG_OK || count == 0 || (rc = use_device(sk->device)) != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(sk->mu);
+    if ((rc = sketcher_rows(sk->st, first, count, d_out, row_stride, d_n_values, d_complete, d_held, (cudaStream_t)stream)) != PG_OK) return rc;
+    PG_CUDA(cudaEventRecord(sk->read, (cudaStream_t)stream));
+    return PG_OK;
+}
+
+int pg_mash_sketcher_free(pg_mash_sketcher *sk) {
+    if (!sk) return PG_OK;
+    int rc = use_device(sk->device);
+    if (rc != PG_OK) return rc;
+    std::lock_guard<std::mutex> lk(cur_ctx()->mu);
+    cudaStream_t st = cur_ctx()->slots[0].stream;
+    cudaStreamWaitEvent(st, sk->read, 0);
+    sketcher_free(sk->st, st);
+    cudaEventDestroy(sk->read);
+    delete sk;
+    PG_CUDA(cudaStreamSynchronize(st));
+    return PG_OK;
 }
 
 int pg_mash_sketch_uniform_gather_dev(const uint8_t *d_bases, uint64_t n_local, uint32_t read_len,

@@ -341,6 +341,28 @@ void screen_free(ScreenIndex &ix, cudaStream_t st);
 // Decides its passes on the host, so it synchronises st.  Argument checks are the caller's.
 int sketch_groups(const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_records, const uint64_t *d_goff, uint64_t n_groups, int k, int s,
                   uint32_t m, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, cudaStream_t st);
+// The state of a grouped sketch grown in place (pg_mash_sketcher): per group g its cap C_g and every value v < C_g
+// seen so far with min(c_g(v), m), ascending in segment [seg[g], seg[g + 1]) of val / cnt.  The host keeps seg and
+// cap too, to plan the passes.
+struct SketcherState {
+    uint64_t G = 0, B = 0;  // groups, most values a group keeps
+    int k = 0, s = 0;
+    uint32_t m = 1;
+    std::vector<uint64_t> seg, cap;
+    uint32_t *d_val = nullptr, *d_cnt = nullptr;  // seg[G] entries
+    uint64_t *d_seg = nullptr, *d_cap = nullptr;  // G + 1 and G
+};
+// an empty state of G groups (every cap 2^32); synchronises st
+int sketcher_init(SketcherState &S, cudaStream_t st);
+// Adds records [d_goff[i], d_goff[i + 1]) of the batch to group first + i, i < nb (d_goff[0] = 0, d_goff[nb] =
+// n_records).  Builds the new state in new buffers and takes it only on success; synchronises st.
+int sketcher_add(SketcherState &S, const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_records, const uint64_t *d_goff, uint64_t first,
+                 uint64_t nb, cudaStream_t st);
+// rows [first, first + count): the first s qualifying values of each state segment, then zeros to row_stride, their
+// number, complete and held (either may be null); only enqueues
+int sketcher_rows(const SketcherState &S, uint64_t first, uint64_t count, uint32_t *d_out, uint64_t row_stride, uint32_t *d_n, uint8_t *d_complete,
+                  uint64_t *d_held, cudaStream_t st);
+void sketcher_free(SketcherState &S, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).
 struct AlignScoring;

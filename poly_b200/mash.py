@@ -241,6 +241,123 @@ def SketchGroups(groups: Sequence[Sequence[BytesLike]], kmer_size: int, sketch_s
     return res
 
 
+class Sketcher:
+    """Grouped sketches grown in place (pg_mash_sketcher): n_groups sketches fed batch by batch, for read sets larger
+    than the device or a host can stage.  Each add counts the windows of its records into their groups; rows() reads
+    them at any time.  Per group the sketcher keeps a cap C (2^32 at first, never growing) and every value below it
+    with its count saturated at min_copies: after an add the cap is the smallest of the old cap, the s-th value seen
+    min_copies times plus one, and the (max_values + 1)-th distinct value.  A row is complete when it holds s values
+    or its cap is still 2^32; a complete row equals sketch_groups over every record added to the group, whatever the
+    split, and every row is a prefix of that row.  With min_copies = 1 every row is complete.  max_values defaults to
+    64 s; an incomplete row asks for a larger one.  The sketcher lives on the device current at creation."""
+
+    def __init__(self, n_groups: int, k: int, s: int, min_copies: int = 1, max_values: Optional[int] = None):
+        n_groups, k, s, min_copies = int(n_groups), int(k), int(s), int(min_copies)
+        _group_args(k, s, min_copies)
+        max_values = 64 * s if max_values is None else int(max_values)
+        if not 0 <= n_groups < (1 << 64) or not 0 <= max_values < (1 << 64):
+            raise PolyError(_lib.PG_ERR_ARG, f"n_groups {n_groups} and max_values {max_values} must fit uint64")
+        h = C.c_void_p()
+        _lib.check(_lib.lib().pg_mash_sketcher_create(n_groups, k, s, min_copies, max_values, C.byref(h)))
+        self._h = h
+        self._dev_used = None
+        self.n_groups, self.k, self.s, self.min_copies, self.max_values = n_groups, k, s, min_copies, max_values
+
+    def _live(self):
+        if self._h is None:
+            raise ValueError("the sketcher is closed")
+        return self._h
+
+    def _sync_dev(self):
+        """Host calls run on the library's own stream: wait for device work enqueued on torch's streams."""
+        if self._dev_used is not None:
+            import torch
+
+            torch.cuda.synchronize(self._dev_used)
+
+    def add(self, bases, offsets, group_offsets, first_group: int = 0) -> None:
+        """Adds records [group_offsets[i], group_offsets[i+1]) of the ragged batch (bases, offsets) to group
+        first_group + i.  NumPy arrays go through the host add; CUDA tensors (uint8 bases, int64 offsets holding uint64
+        bits) through add_dev on the current stream, which the call waits for."""
+        h = self._live()
+        first_group = int(first_group)
+        if not 0 <= first_group < (1 << 64):
+            raise PolyError(_lib.PG_ERR_ARG, f"first group {first_group} does not fit uint64")
+        if hasattr(bases, "data_ptr"):
+            import torch
+
+            for name, t in (("offsets", offsets), ("group_offsets", group_offsets)):
+                if t.element_size() != 8 or not t.is_contiguous():
+                    raise ValueError(f"{name} must be a contiguous 64-bit tensor")
+            n, nb = max(int(offsets.numel()) - 1, 0), max(int(group_offsets.numel()) - 1, 0)
+            st = torch.cuda.current_stream(bases.device).cuda_stream
+            _lib.check(_lib.lib().pg_mash_sketcher_add_dev(h, bases.data_ptr() if bases.numel() else None, offsets.data_ptr() if n else None, n,
+                                                           group_offsets.data_ptr() if nb else None, first_group, nb, st))
+            self._dev_used = bases.device
+            return
+        bases = np.ascontiguousarray(bases, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        group_offsets = np.ascontiguousarray(group_offsets, dtype=np.uint64)
+        if offsets.ndim != 1 or group_offsets.ndim != 1 or len(offsets) < 1 or len(group_offsets) < 1:
+            raise ValueError("offsets and group_offsets must be 1-d with at least one entry")
+        if len(bases) == 0:
+            bases = np.zeros(1, np.uint8)
+        self._sync_dev()
+        _lib.check(_lib.lib().pg_mash_sketcher_add(h, bases.ctypes.data, offsets.ctypes.data, len(offsets) - 1, group_offsets.ctypes.data,
+                                                   first_group, len(group_offsets) - 1))
+
+    def add_records(self, group: int, seqs: Sequence[BytesLike]) -> None:
+        """Adds the sequences seqs (str / bytes / uint8 arrays) to one group."""
+        bases, offsets = flatten(seqs)
+        self.add(bases, offsets, np.array([0, len(offsets) - 1], np.uint64), group)
+
+    def rows(self, first: int = 0, count: Optional[int] = None):
+        """(rows [count, s] uint32, count [count] uint32, complete [count] bool, held [count] uint64) of groups
+        [first, first + count) (count defaults to every group from first).  Changes nothing."""
+        h = self._live()
+        first = int(first)
+        count = self.n_groups - first if count is None else int(count)
+        if not (0 <= first < (1 << 64) and 0 <= count < (1 << 64)):
+            raise PolyError(_lib.PG_ERR_ARG, f"rows [{first}, {first + count}) of a sketcher of {self.n_groups} groups")
+        self._sync_dev()
+        n = max(count, 0) if first + count <= self.n_groups else 0
+        rows = np.zeros((n, self.s), np.uint32)
+        cnt = np.zeros(n, np.uint32)
+        complete = np.zeros(n, np.uint8)
+        held = np.zeros(n, np.uint64)
+        _lib.check(_lib.lib().pg_mash_sketcher_rows(h, first, count, rows.ctypes.data, self.s, cnt.ctypes.data, complete.ctypes.data, held.ctypes.data))
+        return rows, cnt, complete.astype(bool), held
+
+    def sketches(self) -> List[Mash]:
+        """One Mash per group, as SketchGroups returns them."""
+        rows = self.rows()[0]
+        res = []
+        for g in range(self.n_groups):
+            m = Mash(self.k, self.s)
+            m.Sketches[:] = rows[g]
+            res.append(m)
+        return res
+
+    def close(self) -> None:
+        if self._h is not None:
+            self._sync_dev()
+            h, self._h = self._h, None
+            _lib.check(_lib.lib().pg_mash_sketcher_free(h))
+
+    def __enter__(self) -> "Sketcher":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        if getattr(self, "_h", None) is not None:
+            try:
+                self.close()
+            except Exception:
+                pass
+
+
 def similarity_pairs(mashes: Sequence[Mash], pairs: np.ndarray):
     """Explicit pair list (receiver, argument) over sketches of mixed sizes -> (same, similarity, distance)."""
     arrs = [np.ascontiguousarray(m.Sketches[: m.SketchSize], dtype=np.uint32) for m in mashes]
