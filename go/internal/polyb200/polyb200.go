@@ -91,12 +91,21 @@ func SketchBatch(bases []byte, offsets []uint64, k, s int, rowStride int) (out [
 // batch (bases, offsets); row g of out (s words) holds the smallest count[g] distinct window hashes of the group seen at
 // least minCopies times, ascending, then zeros.
 func SketchGroups(bases []byte, offsets []uint64, groupOffsets []uint64, k, s int, minCopies uint32) (out []uint32, count []uint32, err error) {
+	return SketchGroupsFlags(bases, offsets, groupOffsets, k, s, minCopies, 0)
+}
+
+// KmerCanonical is PG_KMER_CANONICAL: windows 0 .. L-k of each record, each hashing the smaller of itself and its
+// reverse complement.
+const KmerCanonical = uint32(C.PG_KMER_CANONICAL)
+
+// SketchGroupsFlags wraps pg_mash_sketch_groups_flags: SketchGroups with flags (0 or KmerCanonical).
+func SketchGroupsFlags(bases []byte, offsets []uint64, groupOffsets []uint64, k, s int, minCopies, flags uint32) (out []uint32, count []uint32, err error) {
 	n, g := len(offsets)-1, len(groupOffsets)-1
 	out = make([]uint32, g*s+1)
 	count = make([]uint32, g+1)
 	err = locked(func() C.int {
-		return C.pg_mash_sketch_groups((*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n),
-			(*C.uint64_t)(unsafe.Pointer(&groupOffsets[0])), C.uint64_t(g), C.int32_t(k), C.int32_t(s), C.uint32_t(minCopies),
+		return C.pg_mash_sketch_groups_flags((*C.uint8_t)(unsafe.Pointer(&bases[0])), (*C.uint64_t)(unsafe.Pointer(&offsets[0])), C.uint64_t(n),
+			(*C.uint64_t)(unsafe.Pointer(&groupOffsets[0])), C.uint64_t(g), C.int32_t(k), C.int32_t(s), C.uint32_t(minCopies), C.uint32_t(flags),
 			(*C.uint32_t)(unsafe.Pointer(&out[0])), C.uint64_t(s), (*C.uint32_t)(unsafe.Pointer(&count[0])))
 	})
 	return out[:g*s], count[:g], err
@@ -111,9 +120,15 @@ type Sketcher struct {
 
 // NewSketcher wraps pg_mash_sketcher_create (maxValues: the most distinct values a group keeps between adds).
 func NewSketcher(nGroups uint64, k, s int, minCopies uint32, maxValues uint64) (*Sketcher, error) {
+	return NewSketcherFlags(nGroups, k, s, minCopies, maxValues, 0)
+}
+
+// NewSketcherFlags wraps pg_mash_sketcher_create_flags: NewSketcher with flags (0 or KmerCanonical).
+func NewSketcherFlags(nGroups uint64, k, s int, minCopies uint32, maxValues uint64, flags uint32) (*Sketcher, error) {
 	var h *C.pg_mash_sketcher
 	if err := locked(func() C.int {
-		return C.pg_mash_sketcher_create(C.uint64_t(nGroups), C.int32_t(k), C.int32_t(s), C.uint32_t(minCopies), C.uint64_t(maxValues), &h)
+		return C.pg_mash_sketcher_create_flags(C.uint64_t(nGroups), C.int32_t(k), C.int32_t(s), C.uint32_t(minCopies), C.uint64_t(maxValues),
+			C.uint32_t(flags), &h)
 	}); err != nil {
 		return nil, err
 	}
@@ -884,6 +899,11 @@ func NewScreen(sketches []uint32, n, s, k int) (*Screen, error) { return NewScre
 
 // NewScreenSamples wraps pg_mash_screen_create_samples: NewScreen with one pool for each of `samples` samples.
 func NewScreenSamples(sketches []uint32, n, s, k, samples int) (*Screen, error) {
+	return NewScreenFlags(sketches, n, s, k, samples, 0)
+}
+
+// NewScreenFlags wraps pg_mash_screen_create_flags: NewScreenSamples with flags (0 or KmerCanonical).
+func NewScreenFlags(sketches []uint32, n, s, k, samples int, flags uint32) (*Screen, error) {
 	var h *C.pg_mash_screen
 	var p *C.uint32_t
 	if len(sketches) > 0 {
@@ -893,7 +913,7 @@ func NewScreenSamples(sketches []uint32, n, s, k, samples int) (*Screen, error) 
 		return nil, errors.New("polyb200: sample count does not fit 32 bits")
 	}
 	if err := locked(func() C.int {
-		return C.pg_mash_screen_create_samples(p, C.uint64_t(n), C.int32_t(s), C.int32_t(k), C.uint32_t(samples), &h)
+		return C.pg_mash_screen_create_flags(p, C.uint64_t(n), C.int32_t(s), C.int32_t(k), C.uint32_t(samples), C.uint32_t(flags), &h)
 	}); err != nil {
 		return nil, err
 	}

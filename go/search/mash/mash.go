@@ -96,6 +96,17 @@ func SketchBatch(sequences []string, kmerSize, sketchSize int) []*Mash {
 // group seen at least minCopies times, ascending, then a zero tail when fewer qualify.  Windows never cross a
 // sequence.  The sketches compare with Similarity and Distance like those of Sketch.
 func SketchGroups(groups [][]string, kmerSize, sketchSize, minCopies int) ([]*Mash, error) {
+	return sketchGroups(groups, kmerSize, sketchSize, minCopies, 0)
+}
+
+// SketchGroupsCanonical is SketchGroups over canonical k-mers, as Mash hashes them: the windows 0 .. L-k of each
+// sequence, each the smaller of itself and its reverse complement, so contigs of either orientation and reads of either
+// strand count as one (kmerSize >= 1).
+func SketchGroupsCanonical(groups [][]string, kmerSize, sketchSize, minCopies int) ([]*Mash, error) {
+	return sketchGroups(groups, kmerSize, sketchSize, minCopies, polyb200.KmerCanonical)
+}
+
+func sketchGroups(groups [][]string, kmerSize, sketchSize, minCopies int, flags uint32) ([]*Mash, error) {
 	if minCopies < 1 || minCopies > math.MaxUint32 {
 		return nil, fmt.Errorf("mash: minCopies %d out of range", minCopies)
 	}
@@ -106,7 +117,7 @@ func SketchGroups(groups [][]string, kmerSize, sketchSize, minCopies int) ([]*Ma
 		goff = append(goff, uint64(len(seqs)))
 	}
 	bases, offsets := polyb200.Flatten(seqs)
-	out, _, err := polyb200.SketchGroups(bases, offsets, goff, kmerSize, sketchSize, uint32(minCopies))
+	out, _, err := polyb200.SketchGroupsFlags(bases, offsets, goff, kmerSize, sketchSize, uint32(minCopies), flags)
 	if err != nil {
 		return nil, err
 	}
@@ -130,13 +141,23 @@ type Sketcher struct {
 
 // NewSketcher prepares nGroups sketches; maxValues <= 0 means 64 * sketchSize.
 func NewSketcher(nGroups, kmerSize, sketchSize, minCopies, maxValues int) (*Sketcher, error) {
+	return newSketcher(nGroups, kmerSize, sketchSize, minCopies, maxValues, 0)
+}
+
+// NewSketcherCanonical is NewSketcher over canonical k-mers (see SketchGroupsCanonical, whose sketches its complete
+// sketches equal).
+func NewSketcherCanonical(nGroups, kmerSize, sketchSize, minCopies, maxValues int) (*Sketcher, error) {
+	return newSketcher(nGroups, kmerSize, sketchSize, minCopies, maxValues, polyb200.KmerCanonical)
+}
+
+func newSketcher(nGroups, kmerSize, sketchSize, minCopies, maxValues int, flags uint32) (*Sketcher, error) {
 	if nGroups < 0 || minCopies < 1 || minCopies > math.MaxUint32 {
 		return nil, fmt.Errorf("mash: nGroups %d or minCopies %d out of range", nGroups, minCopies)
 	}
 	if maxValues <= 0 {
 		maxValues = 64 * sketchSize
 	}
-	sk, err := polyb200.NewSketcher(uint64(nGroups), kmerSize, sketchSize, uint32(minCopies), uint64(maxValues))
+	sk, err := polyb200.NewSketcherFlags(uint64(nGroups), kmerSize, sketchSize, uint32(minCopies), uint64(maxValues), flags)
 	if err != nil {
 		return nil, err
 	}
@@ -478,7 +499,8 @@ func (c *Clusterer) Labels(begin, end int) ([]int, error) {
 func (c *Clusterer) Close() error { return c.c.Close() }
 
 // Screen is Mash Screen (Ondov et al. 2019) on the GPU: which of a set of reference sketches a pool of reads
-// contains.  Add counts every window a Sketch would hash of every read (forward strand, raw bytes) into the pool;
+// contains.  Add counts every window a Sketch would hash of every read (forward strand, raw bytes; canonical k-mers for
+// NewScreenCanonical) into the pool;
 // Results gives, per reference, Shared = the sum over hashes v of min(c_ref(v), c_pool(v)), Containment = Shared /
 // SketchSize and Multiplicity = the lower median pool count of the shared hashes; Winners gives them after Mash
 // Screen's winner-take-all.  Any split of the pool into Adds gives the same Results and Winners, and Reset empties
@@ -506,6 +528,16 @@ func NewScreen(refs []*Mash, kmerSize int) (*Screen, error) { return NewScreenSa
 
 // NewScreenSamples is NewScreen with one pool for each of `samples` samples (samples >= 1).
 func NewScreenSamples(refs []*Mash, kmerSize int, samples int) (*Screen, error) {
+	return newScreen(refs, kmerSize, samples, 0)
+}
+
+// NewScreenCanonical is NewScreenSamples counting canonical k-mers, for refs sketched the same way (SketchGroupsCanonical;
+// the mode, like kmerSize, is not checked), so reads of both strands count.
+func NewScreenCanonical(refs []*Mash, kmerSize int, samples int) (*Screen, error) {
+	return newScreen(refs, kmerSize, samples, polyb200.KmerCanonical)
+}
+
+func newScreen(refs []*Mash, kmerSize int, samples int, flags uint32) (*Screen, error) {
 	s := 0
 	if len(refs) > 0 {
 		s = refs[0].SketchSize
@@ -520,7 +552,7 @@ func NewScreenSamples(refs []*Mash, kmerSize int, samples int) (*Screen, error) 
 	if len(refs) > 0 && s <= 0 {
 		panic("runtime error: index out of range [-1]") // Similarity on a sketch of size 0 would
 	}
-	sc, err := polyb200.NewScreenSamples(flat, len(refs), s, kmerSize, samples)
+	sc, err := polyb200.NewScreenFlags(flat, len(refs), s, kmerSize, samples, flags)
 	if err != nil {
 		return nil, err
 	}

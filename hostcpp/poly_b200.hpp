@@ -134,9 +134,10 @@ inline std::vector<Mash> SketchBatch(const std::vector<std::string> &seqs, int k
 
 // One Mash per group of sequences (an assembly's contigs, a sample's reads): the smallest s distinct window hashes of
 // the group seen at least minCopies times, ascending, then a zero tail (`mash sketch`, `mash sketch -r -m`).  Windows
-// never cross a sequence.  count (may be null) receives how many values each group holds.
+// never cross a sequence.  count (may be null) receives how many values each group holds.  canonical hashes canonical
+// k-mers (PG_KMER_CANONICAL: windows 0 .. L - k, each the smaller of itself and its reverse complement).
 inline std::vector<Mash> SketchGroups(const std::vector<std::vector<std::string>> &groups, int k, int s, uint32_t minCopies,
-                                      std::vector<uint32_t> *count = nullptr) {
+                                      std::vector<uint32_t> *count = nullptr, bool canonical = false) {
     std::vector<std::string> seqs;
     std::vector<uint64_t> goff(1, 0);
     for (const auto &g : groups) {
@@ -146,8 +147,8 @@ inline std::vector<Mash> SketchGroups(const std::vector<std::vector<std::string>
     Flat f(seqs);
     const uint64_t stride = (uint64_t)std::max(s, 1);
     std::vector<uint32_t> out(groups.size() * stride), cnt(groups.size());
-    check(pg_mash_sketch_groups(f.bases.data(), f.offsets.data(), seqs.size(), goff.data(), groups.size(), k, s, minCopies,
-                                out.data(), stride, cnt.data()));
+    check(pg_mash_sketch_groups_flags(f.bases.data(), f.offsets.data(), seqs.size(), goff.data(), groups.size(), k, s, minCopies,
+                                      canonical ? PG_KMER_CANONICAL : 0u, out.data(), stride, cnt.data()));
     std::vector<Mash> res;
     res.reserve(groups.size());
     for (size_t g = 0; g < groups.size(); ++g)
@@ -159,11 +160,13 @@ inline std::vector<Mash> SketchGroups(const std::vector<std::vector<std::string>
 // Grouped sketches grown in place (pg_mash_sketcher): nGroups sketches fed batch by batch, each add counting its
 // sequences into one group or a run of groups.  A row is complete when it holds s values or the group's cap is still
 // 2^32; a complete row equals SketchGroups over every sequence added to the group, whatever the split, and every row
-// is a prefix of it.  maxValues (0: 64 s) is the most distinct values a group keeps between adds.
+// is a prefix of it.  maxValues (0: 64 s) is the most distinct values a group keeps between adds.  canonical counts
+// canonical k-mers, as SketchGroups(..., canonical = true).
 class Sketcher {
 public:
-    Sketcher(uint64_t nGroups, int k, int s, uint32_t minCopies, uint64_t maxValues = 0) : k_(k), s_(s), n_(nGroups) {
-        check(pg_mash_sketcher_create(nGroups, k, s, minCopies, maxValues ? maxValues : 64 * (uint64_t)std::max(s, 1), &h_));
+    Sketcher(uint64_t nGroups, int k, int s, uint32_t minCopies, uint64_t maxValues = 0, bool canonical = false) : k_(k), s_(s), n_(nGroups) {
+        check(pg_mash_sketcher_create_flags(nGroups, k, s, minCopies, maxValues ? maxValues : 64 * (uint64_t)std::max(s, 1),
+                                            canonical ? PG_KMER_CANONICAL : 0u, &h_));
     }
     Sketcher(const Sketcher &) = delete;
     Sketcher &operator=(const Sketcher &) = delete;
@@ -602,16 +605,17 @@ public:
 // Results and Winners; Reset empties the pool.  A screen of several samples holds one pool per sample over the
 // one reference set: AddSamples tags each read with its sample, and row q of ResultsSamples / WinnersSamples is what
 // a one-sample screen fed only sample q's reads answers.  Add counts into sample 0; Results and Winners give row 0.
+// canonical counts canonical k-mers (PG_KMER_CANONICAL), for references sketched the same way.
 class Screen {
     pg_mash_screen *h_ = nullptr;
     size_t n_ = 0;
     int k_ = 0;
 
 public:
-    Screen(const std::vector<Mash> &refs, int kmerSize, uint32_t samples = 1) : n_(refs.size()), k_(kmerSize) {
+    Screen(const std::vector<Mash> &refs, int kmerSize, uint32_t samples = 1, bool canonical = false) : n_(refs.size()), k_(kmerSize) {
         int s;
         const std::vector<uint32_t> flat = detail::FlatRows(refs, "references", &s);
-        int rc = pg_mash_screen_create_samples(flat.data(), refs.size(), s, kmerSize, samples, &h_);
+        int rc = pg_mash_screen_create_flags(flat.data(), refs.size(), s, kmerSize, samples, canonical ? PG_KMER_CANONICAL : 0u, &h_);
         if (rc == PG_ERR_PANIC) throw GoPanic("index out of range [-1]");
         check(rc);
     }

@@ -162,6 +162,29 @@ int pg_mash_sketch_uniform_scatter_dev(const uint8_t *d_bases, uint64_t n_local,
                                        int32_t k, int32_t s, void *const *dst_ptrs, int32_t n_dst,
                                        int32_t self, uint64_t row_offset, void *stream);
 
+/* ---- canonical k-mers: PG_KMER_CANONICAL, a flag of the grouped sketch, the sketcher and the screen ----
+ * Mash hashes canonical k-mers: a k-mer and its reverse complement are one k-mer, so contigs of either orientation and
+ * reads of either strand meet.  With the flag (pg_mash_sketch_groups_flags, pg_mash_sketcher_create_flags,
+ * pg_mash_screen_create_flags and their _dev forms) the windows of a record of length L >= k >= 1 are:
+ *   - Windows: positions 0 .. L - k, so L - k + 1 of them and none when L < k.  This is Mash's k-mer set, one more than
+ *     the forward mode's L - k: the forward mode skips the last window (mash.go:73), which would break strand
+ *     symmetry.  No window crosses a record.
+ *   - Canonical form: for w = bases[p .. p+k), rc(w)[i] = complement(w[k-1-i]), complement being
+ *     transform.complementTable (upper- and lower-case IUPAC letters; every unlisted byte maps to 0).
+ *     canon(w) = w if w <= rc(w) in unsigned byte order (memcmp), else rc(w).
+ *   - Hash: murmur3.Sum32(canon(w)), the same MurmurHash3_x86_32 with seed 0 over k raw bytes as the forward mode.
+ *     Case is not folded and no byte is skipped.
+ *   - Strand symmetry: a record whose bytes all lie in ABCDGHKMNRSTVWY and their lower case may be replaced by its
+ *     reverse complement without changing any row, count or screen result.
+ *   - Counting: min_copies and the screen's pool counts count a k-mer and its reverse complement together.
+ *   - Mash's choice: on upper-case ACGT the canonical strand is Mash's (memcmp(kmer_fwd, kmer_rev) <= 0); only the
+ *     hash function differs from Mash.
+ * Everything else (rows, min_copies, the sketcher's caps, budget and completeness, the screen's results, winners and
+ * samples) is as documented for each call, over this window multiset instead of the forward one.  Errors, added right
+ * after each call's k < 0 rule: a flag bit other than PG_KMER_CANONICAL, and k == 0 with PG_KMER_CANONICAL (no strand to
+ * choose), both PG_ERR_ARG before any device work.  flags == 0 is the call without the flag, byte for byte. */
+#define PG_KMER_CANONICAL 1u
+
 /* ---- grouped sketch: one sketch per group of records (`mash sketch genome.fa`, `mash sketch -r -m M reads.fq`) ----
  * A draft assembly is many contigs and a read set many reads; Mash sketches each as one set.  Records are ragged
  * as in pg_mash_sketch_batch (record i = bases[offsets[i] .. offsets[i+1])); group g is records
@@ -169,7 +192,8 @@ int pg_mash_sketch_uniform_scatter_dev(const uint8_t *d_bases, uint64_t n_local,
  * group_offsets[n_groups] == n_records, never decreasing; empty groups are allowed.
  *   - Windows: a record of length L contributes the windows (*Mash).Sketch hashes, positions 0 .. L - k - 1
  *     (mash.go:73; none when L <= k), each murmur3.Sum32 over its raw bytes: forward strand, case-sensitive, any
- *     byte value, as the screen counts them.  No window crosses a record.
+ *     byte value, as the screen counts them.  No window crosses a record.  pg_mash_sketch_groups_flags (+ _dev) with
+ *     PG_KMER_CANONICAL takes the canonical windows instead (above).
  *   - c_g(v) = the windows of group g's records whose hash is v.  Row g = the distinct values v with
  *     c_g(v) >= min_copies in ascending order, the smallest count[g] = min(q_g, s) of them (q_g: how many qualify),
  *     then zeros up to row_stride.  The row is a set (no value twice) and always ascending, also when q_g < s; a
@@ -181,7 +205,8 @@ int pg_mash_sketch_uniform_scatter_dev(const uint8_t *d_bases, uint64_t n_local,
  *   - Errors, checked in this order before any device work: a null out or count with n_groups > 0; k < 0 (as for
  *     the sketch calls); s < 1; min_copies < 1; row_stride < s; a null buffer with work to do (group_offsets and
  *     offsets when n_groups > 0; bases when the records hold a byte, or in _dev when n_records > 0); in the host call, group offsets that do not partition
- *     the records or record offsets that decrease: all PG_ERR_ARG.  PG_ERR_NOMEM when device memory runs out.
+ *     the records or record offsets that decrease: all PG_ERR_ARG.  The _flags forms check their flags right after
+ *     k < 0 (above).  PG_ERR_NOMEM when device memory runs out.
  *     n_groups == 0 is valid and needs no buffers.  _dev trusts its offsets as pg_mash_sketch_batch_dev does.
  *   - Passes: pass t counts, for every group still open, the windows whose hash lies in the group's next range of
  *     values into an open-addressing table; values with count >= min_copies are appended to the row.  The first
@@ -197,11 +222,20 @@ int pg_mash_sketch_groups(const uint8_t *bases, const uint64_t *offsets, uint64_
 int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
                               uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t *d_out, uint64_t row_stride,
                               uint32_t *d_count, void *stream);
+/* the same with flags (0 or PG_KMER_CANONICAL) after min_copies; flags == 0 is the call above */
+int pg_mash_sketch_groups_flags(const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets,
+                                uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t flags, uint32_t *out,
+                                uint64_t row_stride, uint32_t *count);
+int pg_mash_sketch_groups_flags_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
+                                    uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t flags, uint32_t *d_out,
+                                    uint64_t row_stride, uint32_t *d_count, void *stream);
 
 /* ---- grouped sketch grown in place: read sets larger than device memory, added batch by batch ----
  * A sketcher holds G groups (fixed at create), k, s, m = min_copies and a budget B = max_values: the most distinct
  * values one group keeps between adds.  Windows are exactly those of pg_mash_sketch_groups: positions 0 .. L - k - 1
- * of each record, murmur3 over the raw bytes, forward strand, never crossing a record.  c_g(v) = the windows of every
+ * of each record, murmur3 over the raw bytes, forward strand, never crossing a record; a sketcher made by
+ * pg_mash_sketcher_create_flags with PG_KMER_CANONICAL takes the canonical windows (above) in every add, and the
+ * one-shot call it equals is then pg_mash_sketch_groups_flags with the same flag.  c_g(v) = the windows of every
  * record added to group g so far whose hash is v.
  *   - Per group the sketcher keeps a cap C_g, which starts at 2^32 and never grows, and a state: every value v < C_g
  *     with c_g(v) >= 1, and beside each one min(c_g(v), m).  Invariant: every count below C_g is exact.  An add of
@@ -227,7 +261,8 @@ int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets,
  *   - Batch layout: records [group_offsets[i], group_offsets[i+1]) of the batch belong to group first_group + i, with
  *     group_offsets[0] == 0 and group_offsets[n_batch_groups] == n_records (the one-shot layout with a group base).
  *   - Errors, checked in this order before any device work (PG_ERR_ARG):
- *       create: a null out; n_groups == 0 or n_groups > 2^32 - 1; k < 0; s < 1; min_copies < 1; max_values < s.
+ *       create: a null out; n_groups == 0 or n_groups > 2^32 - 1; k < 0; (create_flags: an unknown flag bit; k == 0
+ *         with PG_KMER_CANONICAL); s < 1; min_copies < 1; max_values < s.
  *       add: a null sketcher (no device needed); n_records == 0 with n_batch_groups == 0 is a valid no-op;
  *         first_group + n_batch_groups > G; n_records == 0 is then a valid no-op; a null offsets or group_offsets, or a
  *         null bases (in the host add only when the records hold a byte); in the host add, group offsets that do not
@@ -246,6 +281,9 @@ int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets,
  *     a table holds twice the distinct values its range is expected to admit.  The host add also stages the batch. */
 typedef struct pg_mash_sketcher pg_mash_sketcher;
 int pg_mash_sketcher_create(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t max_values, pg_mash_sketcher **out);
+/* the same with flags (0 or PG_KMER_CANONICAL): the mode belongs to the sketcher, add and rows are unchanged */
+int pg_mash_sketcher_create_flags(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t max_values, uint32_t flags,
+                                  pg_mash_sketcher **out);
 int pg_mash_sketcher_add(pg_mash_sketcher *sk, const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets,
                          uint64_t first_group, uint64_t n_batch_groups);
 int pg_mash_sketcher_add_dev(pg_mash_sketcher *sk, const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records,
@@ -623,7 +661,9 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c);
  *   - Windows: a pool read of length L contributes the windows (*Mash).Sketch hashes, positions 0 .. L - k - 1
  *     (the last k-mer is never hashed, mash.go:73; L <= k gives none), each hashed by murmur3.Sum32 over its raw
  *     bytes: forward strand, case-sensitive, any byte value.  k is not checked against the references, as in the
- *     reference; pass the k the sketches were made with.
+ *     reference; pass the k the sketches were made with.  A screen made by create_flags (+ _dev) with
+ *     PG_KMER_CANONICAL counts the canonical windows (above) in every add; like k, the mode is not checked against
+ *     the sketches' (pass sketches made in the same mode, e.g. by pg_mash_sketch_groups_flags).
  *   - Counts: c_pool(v) = the windows of every read of every add since creation or the last reset whose hash is v;
  *     c_r(v) = the words of reference r equal to v, taken as given (zero-tail words are the value 0; unsorted
  *     fill-regime sketches are allowed).
@@ -647,7 +687,8 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c);
  *   - Split invariance: for any split of a pool into adds (empty and one-read adds included) the results and the
  *     winners equal those of one add of the concatenation; after a reset the screen answers as a freshly created one.
  *   - Errors, checked in this order: a null screen or out is PG_ERR_ARG (no device is needed); k < 0 is
- *     PG_ERR_ARG, as for the sketch calls; s <= 0 with n > 0 is PG_ERR_PANIC, as for index create; n > 2^32 - 1 is
+ *     PG_ERR_ARG, as for the sketch calls; (create_flags: an unknown flag bit, then k == 0 with PG_KMER_CANONICAL,
+ *     PG_ERR_ARG); s <= 0 with n > 0 is PG_ERR_PANIC, as for index create; n > 2^32 - 1 is
  *     PG_ERR_ARG (the keys hold 32-bit ids); a null buffer is PG_ERR_ARG.  n == 0 and n_reads == 0 are valid (an
  *     add of no read changes nothing and needs no buffer).  Offsets that decrease in a host add are PG_ERR_ARG.
  *     Any output of results or winners may be NULL.  PG_ERR_NOMEM when device memory runs out.  After any error the screen
@@ -707,6 +748,12 @@ int pg_mash_screen_winners_dev(const pg_mash_screen *sc, uint32_t *d_shared, dou
 int pg_mash_screen_create_samples(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, pg_mash_screen **out);
 int pg_mash_screen_create_samples_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, void *stream,
                                       pg_mash_screen **out);
+/* create_samples with flags (0 or PG_KMER_CANONICAL): the mode belongs to the screen, like k; every add, results and
+ * winners call is unchanged */
+int pg_mash_screen_create_flags(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, uint32_t flags,
+                                pg_mash_screen **out);
+int pg_mash_screen_create_flags_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, uint32_t flags,
+                                    void *stream, pg_mash_screen **out);
 int pg_mash_screen_add_samples(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, const uint32_t *sample_ids, uint64_t n_reads);
 int pg_mash_screen_add_samples_dev(pg_mash_screen *sc, const uint8_t *d_bases, const uint64_t *d_offsets, const uint32_t *d_sample_ids,
                                    uint64_t n_reads, void *stream);

@@ -16,6 +16,7 @@ PG_OK, PG_ERR_CUDA, PG_ERR_ARG, PG_ERR_NO_DEVICE, PG_ERR_PANIC, PG_ERR_UNSUPPORT
 PG_ITEM_OK, PG_ITEM_PANIC, PG_ITEM_UNSUPPORTED = 0, 1, 2
 PG_SKETCH_PAD_ZERO = 1
 PG_SKETCH_TAIL_KEEP = 2
+PG_KMER_CANONICAL = 1
 
 
 class PolyError(RuntimeError):
@@ -55,7 +56,12 @@ _SIGS = {
     "pg_mash_sketch_groups": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _u32p]),
     "pg_mash_sketch_groups_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, _u32p, C.c_uint64, _u32p,
                                             C.c_void_p]),
+    "pg_mash_sketch_groups_flags": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32, _u32p,
+                                              C.c_uint64, _u32p]),
+    "pg_mash_sketch_groups_flags_dev": (C.c_int, [_u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32,
+                                                  _u32p, C.c_uint64, _u32p, C.c_void_p]),
     "pg_mash_sketcher_create": (C.c_int, [C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_uint64, C.POINTER(C.c_void_p)]),
+    "pg_mash_sketcher_create_flags": (C.c_int, [C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_uint64, C.c_uint32, C.POINTER(C.c_void_p)]),
     "pg_mash_sketcher_add": (C.c_int, [C.c_void_p, _u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_uint64]),
     "pg_mash_sketcher_add_dev": (C.c_int, [C.c_void_p, _u8p, _u64p, C.c_uint64, _u64p, C.c_uint64, C.c_uint64, C.c_void_p]),
     "pg_mash_sketcher_rows": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, _u32p, C.c_uint64, _u32p, _u8p, _u64p]),
@@ -117,6 +123,9 @@ _SIGS = {
     "pg_mash_screen_winners_dev": (C.c_int, [C.c_void_p, _u32p, _f64p, _u64p, C.c_void_p]),
     "pg_mash_screen_create_samples": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.POINTER(C.c_void_p)]),
     "pg_mash_screen_create_samples_dev": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "pg_mash_screen_create_flags": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]),
+    "pg_mash_screen_create_flags_dev": (C.c_int, [_u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_uint32, C.c_uint32, C.c_void_p,
+                                                  C.POINTER(C.c_void_p)]),
     "pg_mash_screen_add_samples": (C.c_int, [C.c_void_p, _u8p, _u64p, _u32p, C.c_uint64]),
     "pg_mash_screen_add_samples_dev": (C.c_int, [C.c_void_p, _u8p, _u64p, _u32p, C.c_uint64, C.c_void_p]),
     "pg_mash_screen_results_samples": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, _u32p, _f64p, _u64p]),

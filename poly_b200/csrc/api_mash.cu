@@ -630,9 +630,18 @@ static int cluster_add(pg_mash_clusterer *c, const uint32_t *d_b, uint64_t m, ui
     return PG_OK;
 }
 
+// The k-mer mode rules that follow the k < 0 rule of the grouped sketch, the sketcher and the screen: a known flag, and a
+// strand to choose (k >= 1) in canonical mode
+static int kmer_flags_check(int32_t k, uint32_t flags) {
+    if (flags & ~(uint32_t)PG_KMER_CANONICAL) { set_error("unknown k-mer flags 0x%x", flags & ~(uint32_t)PG_KMER_CANONICAL); return PG_ERR_ARG; }
+    if ((flags & PG_KMER_CANONICAL) && k == 0) { set_error("canonical k-mers of size 0: no strand to choose"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
 // The argument rules of pg_mash_screen_create after the null out pointer, in their order
-static int screen_create_check(const void *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples) {
+static int screen_create_check(const void *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, uint32_t flags) {
     if (k < 0) { set_error("k-mer size %d < 0", k); return PG_ERR_ARG; }
+    if (int rc = kmer_flags_check(k, flags)) return rc;
     if (n && s <= 0) { set_error("screen over sketches of size %d: the reference panics (Sketches[-1])", s); return PG_ERR_PANIC; }
     if (n > 0xffffffffull) { set_error("%llu references exceed 2^32 - 1", (unsigned long long)n); return PG_ERR_ARG; }
     if (n_samples == 0) { set_error("a screen of 0 samples"); return PG_ERR_ARG; }
@@ -640,12 +649,15 @@ static int screen_create_check(const void *sketches, uint64_t n, int32_t s, int3
     return PG_OK;
 }
 
-static pg_mash_screen *screen_new(int32_t k, const ScreenIndex &ix) { return new pg_mash_screen{cur_ctx()->device, k, ix}; }
+static pg_mash_screen *screen_new(int32_t k, uint32_t flags, ScreenIndex ix) {
+    ix.canon = (flags & PG_KMER_CANONICAL) != 0;
+    return new pg_mash_screen{cur_ctx()->device, k, ix};
+}
 
-static int screen_create_host(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, pg_mash_screen **out) {
+static int screen_create_host(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, uint32_t flags, pg_mash_screen **out) {
     if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
     *out = nullptr;
-    int rc = screen_create_check(sketches, n, s, k, n_samples);
+    int rc = screen_create_check(sketches, n, s, k, n_samples, flags);
     if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
     ScreenIndex ix;
     {
@@ -657,19 +669,19 @@ static int screen_create_host(const uint32_t *sketches, uint64_t n, int32_t s, i
             return rc;
         }
     }
-    *out = screen_new(k, ix);
+    *out = screen_new(k, flags, ix);
     return PG_OK;
 }
 
-static int screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, void *stream,
+static int screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, uint32_t flags, void *stream,
                              pg_mash_screen **out) {
     if (!out) { set_error("null screen pointer"); return PG_ERR_ARG; }
     *out = nullptr;
-    int rc = screen_create_check(d_sketches, n, s, k, n_samples);
+    int rc = screen_create_check(d_sketches, n, s, k, n_samples, flags);
     if (rc != PG_OK || (rc = ensure_device()) != PG_OK) return rc;
     ScreenIndex ix;
     if ((rc = screen_build(d_sketches, n, s, n_samples, (cudaStream_t)stream, &ix)) != PG_OK) return rc;
-    *out = screen_new(k, ix);
+    *out = screen_new(k, flags, ix);
     return PG_OK;
 }
 
@@ -747,10 +759,11 @@ static int screen_tally_dev(const pg_mash_screen *sc, ScreenTally tally, uint32_
 }
 
 // The argument rules of pg_mash_sketch_groups and its _dev form that need no buffer, in their order
-static int sketch_groups_check(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t row_stride, const void *out,
+static int sketch_groups_check(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t flags, uint64_t row_stride, const void *out,
                                const void *count) {
     if (n_groups && (!out || !count)) { set_error("null out or count"); return PG_ERR_ARG; }
     if (k < 0) { set_error("kmerSize %d < 0: the reference panics (slice bounds)", k); return PG_ERR_ARG; }
+    if (int rc = kmer_flags_check(k, flags)) return rc;
     if (s < 1) { set_error("sketchSize %d < 1: a grouped sketch holds at least one value", s); return PG_ERR_ARG; }
     if (min_copies < 1) { set_error("min_copies 0: every value occurs at least once"); return PG_ERR_ARG; }
     if (row_stride < (uint64_t)s) { set_error("row_stride %llu < sketchSize %d", (unsigned long long)row_stride, s); return PG_ERR_ARG; }
@@ -826,9 +839,10 @@ int pg_mash_sketch_batch_dev(const uint8_t *d_bases, const uint64_t *d_offsets, 
                                 row_stride, d_count, d_status, (cudaStream_t)stream);
 }
 
-int pg_mash_sketch_groups(const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets, uint64_t n_groups,
-                          int32_t k, int32_t s, uint32_t min_copies, uint32_t *out, uint64_t row_stride, uint32_t *count) {
-    int rc = sketch_groups_check(n_groups, k, s, min_copies, row_stride, out, count);
+int pg_mash_sketch_groups_flags(const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets,
+                                uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t flags, uint32_t *out, uint64_t row_stride,
+                                uint32_t *count) {
+    int rc = sketch_groups_check(n_groups, k, s, min_copies, flags, row_stride, out, count);
     if (rc != PG_OK || n_groups == 0) return rc;
     if (!group_offsets || !offsets || (!bases && offsets[n_records] != offsets[0])) { set_error("null buffer"); return PG_ERR_ARG; }
     uint64_t longest = 0;  // the groups partition the records: ragged offsets over the records, from 0 to n_records
@@ -844,29 +858,48 @@ int pg_mash_sketch_groups(const uint8_t *bases, const uint64_t *offsets, uint64_
     const uint64_t *d_goff = c.upload(group_offsets, n_groups + 1);
     uint32_t *d_out = c.alloc<uint32_t>(n_groups * row_stride);
     uint32_t *d_count = c.alloc<uint32_t>(n_groups);
-    if ((rc = c.error()) || (rc = sketch_groups(r.base, r.off, n_records, d_goff, n_groups, k, s, min_copies, d_out, row_stride, d_count, c.st)))
+    const bool canon = (flags & PG_KMER_CANONICAL) != 0;
+    if ((rc = c.error()) || (rc = sketch_groups(r.base, r.off, n_records, d_goff, n_groups, k, s, min_copies, canon, d_out, row_stride, d_count, c.st)))
         return rc;
     c.download(out, d_out, n_groups * row_stride);
     c.download(count, d_count, n_groups);
     return c.finish();
 }
 
-int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
-                              uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t *d_out, uint64_t row_stride,
-                              uint32_t *d_count, void *stream) {
-    int rc = sketch_groups_check(n_groups, k, s, min_copies, row_stride, d_out, d_count);
+int pg_mash_sketch_groups(const uint8_t *bases, const uint64_t *offsets, uint64_t n_records, const uint64_t *group_offsets, uint64_t n_groups,
+                          int32_t k, int32_t s, uint32_t min_copies, uint32_t *out, uint64_t row_stride, uint32_t *count) {
+    return pg_mash_sketch_groups_flags(bases, offsets, n_records, group_offsets, n_groups, k, s, min_copies, 0, out, row_stride, count);
+}
+
+int pg_mash_sketch_groups_flags_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
+                                    uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t flags, uint32_t *d_out,
+                                    uint64_t row_stride, uint32_t *d_count, void *stream) {
+    int rc = sketch_groups_check(n_groups, k, s, min_copies, flags, row_stride, d_out, d_count);
     if (rc != PG_OK || n_groups == 0) return rc;
     if (!d_group_offsets || !d_offsets || (n_records && !d_bases)) { set_error("null buffer"); return PG_ERR_ARG; }
     if ((rc = ensure_device()) != PG_OK) return rc;
-    return sketch_groups(d_bases, d_offsets, n_records, d_group_offsets, n_groups, k, s, min_copies, d_out, row_stride, d_count,
-                         (cudaStream_t)stream);
+    return sketch_groups(d_bases, d_offsets, n_records, d_group_offsets, n_groups, k, s, min_copies, (flags & PG_KMER_CANONICAL) != 0, d_out,
+                         row_stride, d_count, (cudaStream_t)stream);
+}
+
+int pg_mash_sketch_groups_dev(const uint8_t *d_bases, const uint64_t *d_offsets, uint64_t n_records, const uint64_t *d_group_offsets,
+                              uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint32_t *d_out, uint64_t row_stride,
+                              uint32_t *d_count, void *stream) {
+    return pg_mash_sketch_groups_flags_dev(d_bases, d_offsets, n_records, d_group_offsets, n_groups, k, s, min_copies, 0, d_out, row_stride,
+                                           d_count, stream);
 }
 
 int pg_mash_sketcher_create(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t max_values, pg_mash_sketcher **out) {
+    return pg_mash_sketcher_create_flags(n_groups, k, s, min_copies, max_values, 0, out);
+}
+
+int pg_mash_sketcher_create_flags(uint64_t n_groups, int32_t k, int32_t s, uint32_t min_copies, uint64_t max_values, uint32_t flags,
+                                  pg_mash_sketcher **out) {
     if (!out) { set_error("null sketcher pointer"); return PG_ERR_ARG; }
     *out = nullptr;
     if (n_groups == 0 || n_groups > 0xffffffffull) { set_error("a sketcher of %llu groups: need 1 .. 2^32 - 1", (unsigned long long)n_groups); return PG_ERR_ARG; }
     if (k < 0) { set_error("kmerSize %d < 0: the reference panics (slice bounds)", k); return PG_ERR_ARG; }
+    if (int rc = kmer_flags_check(k, flags)) return rc;
     if (s < 1) { set_error("sketchSize %d < 1: a grouped sketch holds at least one value", s); return PG_ERR_ARG; }
     if (min_copies < 1) { set_error("min_copies 0: every value occurs at least once"); return PG_ERR_ARG; }
     if (max_values < (uint64_t)s) { set_error("max_values %llu < sketchSize %d", (unsigned long long)max_values, s); return PG_ERR_ARG; }
@@ -888,6 +921,7 @@ int pg_mash_sketcher_create(uint64_t n_groups, int32_t k, int32_t s, uint32_t mi
     sk->st.k = k;
     sk->st.s = s;
     sk->st.m = min_copies;
+    sk->st.canon = (flags & PG_KMER_CANONICAL) != 0;
     std::lock_guard<std::mutex> lk(cur_ctx()->mu);
     cudaStream_t st = cur_ctx()->slots[0].stream;
     cudaError_t e = cudaEventCreateWithFlags(&sk->read, cudaEventDisableTiming);
@@ -1617,20 +1651,29 @@ int pg_mash_clusterer_free(pg_mash_clusterer *c) {
 // Screen: which references a pool of reads contains
 // ---------------------------------------------------------------------------------
 int pg_mash_screen_create(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, pg_mash_screen **out) {
-    return screen_create_host(sketches, n, s, k, 1, out);
+    return screen_create_host(sketches, n, s, k, 1, 0, out);
 }
 
 int pg_mash_screen_create_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, void *stream, pg_mash_screen **out) {
-    return screen_create_dev(d_sketches, n, s, k, 1, stream, out);
+    return screen_create_dev(d_sketches, n, s, k, 1, 0, stream, out);
 }
 
 int pg_mash_screen_create_samples(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, pg_mash_screen **out) {
-    return screen_create_host(sketches, n, s, k, n_samples, out);
+    return screen_create_host(sketches, n, s, k, n_samples, 0, out);
+}
+
+int pg_mash_screen_create_flags(const uint32_t *sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, uint32_t flags, pg_mash_screen **out) {
+    return screen_create_host(sketches, n, s, k, n_samples, flags, out);
+}
+
+int pg_mash_screen_create_flags_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, uint32_t flags, void *stream,
+                                    pg_mash_screen **out) {
+    return screen_create_dev(d_sketches, n, s, k, n_samples, flags, stream, out);
 }
 
 int pg_mash_screen_create_samples_dev(const uint32_t *d_sketches, uint64_t n, int32_t s, int32_t k, uint32_t n_samples, void *stream,
                                       pg_mash_screen **out) {
-    return screen_create_dev(d_sketches, n, s, k, n_samples, stream, out);
+    return screen_create_dev(d_sketches, n, s, k, n_samples, 0, stream, out);
 }
 
 int pg_mash_screen_add(pg_mash_screen *sc, const uint8_t *bases, const uint64_t *offsets, uint64_t n_reads) {

@@ -316,6 +316,7 @@ struct ScreenIndex {
     int s = 0;
     uint32_t nb = 0, vmax = 0;
     uint32_t samples = 1;
+    bool canon = false;  // adds count canonical k-mers (PG_KMER_CANONICAL)
 };
 // Builds the screen of n reference rows of s > 0 words (any order, zero tails included) with zero counts for
 // samples >= 1 samples; synchronises st.  On an error nothing of *out is allocated.
@@ -338,9 +339,10 @@ int screen_winners(const ScreenIndex &ix, uint32_t first, uint32_t count, uint32
 void screen_free(ScreenIndex &ix, cudaStream_t st);
 // sketch_groups.cu: row g of d_out (row_stride words, zeroed past its count) = the smallest min(q_g, s) distinct window
 // hashes of group g's records [d_goff[g], d_goff[g + 1]) that occur at least m times, ascending; d_count[g] = how many.
-// Decides its passes on the host, so it synchronises st.  Argument checks are the caller's.
+// canon: canonical k-mers (PG_KMER_CANONICAL).  Decides its passes on the host, so it synchronises st.  Argument checks
+// are the caller's.
 int sketch_groups(const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_records, const uint64_t *d_goff, uint64_t n_groups, int k, int s,
-                  uint32_t m, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, cudaStream_t st);
+                  uint32_t m, bool canon, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, cudaStream_t st);
 // The state of a grouped sketch grown in place (pg_mash_sketcher): per group g its cap C_g and every value v < C_g
 // seen so far with min(c_g(v), m), ascending in segment [seg[g], seg[g + 1]) of val / cnt.  The host keeps seg and
 // cap too, to plan the passes.
@@ -348,6 +350,7 @@ struct SketcherState {
     uint64_t G = 0, B = 0;  // groups, most values a group keeps
     int k = 0, s = 0;
     uint32_t m = 1;
+    bool canon = false;  // canonical k-mers (PG_KMER_CANONICAL)
     std::vector<uint64_t> seg, cap;
     uint32_t *d_val = nullptr, *d_cnt = nullptr;  // seg[G] entries
     uint64_t *d_seg = nullptr, *d_cap = nullptr;  // G + 1 and G

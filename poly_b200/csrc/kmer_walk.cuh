@@ -159,6 +159,105 @@ bool with_walk_k(int k, F &&f) { return with_k_in(WalkKs{}, k, f); }
             _Pragma("unroll") for (int q = 0; q < NB; ++q) ring[r][q] = t_[q];                 \
         }                                                                                      \
     }
+// ---- the canonical walk (PG_KMER_CANONICAL): each window hashes the smaller of itself and its reverse complement.
+// Beside s_in the chunk is staged complemented (c[q] = complement(byte q)).  The reverse strand's block j of the
+// window at p is the byte-reversed complemented word at p + k - 4 - 4j, so its pre-mix R(q) = kmix(bswap(cword(q)))
+// is shared between windows like the forward K(q): a second ring, rring[r][*], holds R(4q + r + TAIL) of the last NB
+// word steps, fed by a complemented stream that runs TAIL bytes ahead of the forward one (cw, csh).  Its tail is the
+// complemented bytes p .. p + TAIL - 1 in reverse.  The strand is decided before hashing: w's first 4 bytes as a
+// big-endian word (from a third stream, l_*, the forward bytes at the window itself) against rc(w)'s, which are
+// cword(p + k - 4) read little-endian, the previous step's complemented word (cprev); only a tie compares further
+// bytes.  The NB rounds and the fmix then run once, each block selected from the chosen ring.  Extra locals:
+//   cw, csh                complemented staged words from byte b0 + TAIL, funnel-shift amount
+//   sbf, sbc               s_in + b0 and s_rc + b0: forward and complemented byte of window i is sbf[i], sbc[i]
+
+// Whether rc(w) < w, given that their first 4 bytes are equal: bytes 4 .. K - 1 of w (f) against those of rc(w)
+// (complemented bytes of w read backwards, c).
+template <int K>
+__device__ __forceinline__ bool canon_tie(const uint8_t *f, const uint8_t *c) {
+    for (int t = 4; t < K; ++t) {
+        const uint8_t a = f[t], b = c[K - 1 - t];
+        if (a != b) return b < a;
+    }
+    return false;
+}
+
+// rc(w)'s tail: complemented bytes p + TAIL - 1 .. p of the window at p, little-endian
+template <int TAIL>
+__device__ __forceinline__ uint32_t canon_tail(const uint8_t *c) {
+    uint32_t t = 0;
+#pragma unroll
+    for (int x = 0; x < TAIL; ++x) t |= (uint32_t)c[x] << (8 * (TAIL - 1 - x));
+    return t;
+}
+
+// After PG_WALK_PROLOGUE: the complemented stream, its ring and cprev, and the lagging forward stream.
+#define PG_CANON_PROLOGUE                                                                      \
+    uint32_t craw_a = cw[0], craw_b = cw[1];                                                   \
+    uint32_t c_cur = __funnelshift_r(craw_a, craw_b, csh);                                     \
+    craw_a = craw_b; craw_b = cw[2];                                                           \
+    uint32_t c_nxt = __funnelshift_r(craw_a, craw_b, csh);                                     \
+    craw_a = craw_b; craw_b = cw[3];                                                           \
+    const uint32_t *cwp = cw + 4;                                                              \
+    uint32_t rring[4][NB], cprev[4];                                                           \
+    _Pragma("unroll") for (int q = 0; q < NB; ++q) {                                           \
+        _Pragma("unroll") for (int r = 0; r < 4; ++r) {                                        \
+            cprev[r] = __funnelshift_r(c_cur, c_nxt, 8 * r);                                   \
+            rring[r][q] = mm3_kmix(__byte_perm(cprev[r], 0, 0x0123));                          \
+        }                                                                                      \
+        c_cur = c_nxt;                                                                         \
+        c_nxt = __funnelshift_r(craw_a, craw_b, csh);                                          \
+        craw_a = craw_b;                                                                       \
+        craw_b = *cwp++;                                                                       \
+    }                                                                                          \
+    uint32_t lraw_a = sw[0], lraw_b = sw[1];                                                   \
+    uint32_t l_cur = __funnelshift_r(lraw_a, lraw_b, sh);                                      \
+    lraw_a = lraw_b; lraw_b = sw[2];                                                           \
+    uint32_t l_nxt = __funnelshift_r(lraw_a, lraw_b, sh);                                      \
+    lraw_a = lraw_b; lraw_b = sw[3];                                                           \
+    const uint32_t *lwp = sw + 4;
+
+// One canonical word step = 4 windows (ring slot U of both rings), unchecked.  EMIT(r, value) as PG_KMER_STEP.
+#define PG_KMER_STEP_CANON(U, EMIT)                                                            \
+    {                                                                                          \
+        uint32_t w[4], c[4];                                                                   \
+        uint32_t h[4];                                                                         \
+        _Pragma("unroll") for (int r = 0; r < 4; ++r) {                                        \
+            w[r] = __funnelshift_r(w_cur, w_nxt, 8 * r);                                       \
+            c[r] = __funnelshift_r(c_cur, c_nxt, 8 * r);                                       \
+            const uint32_t a_ = __byte_perm(__funnelshift_r(l_cur, l_nxt, 8 * r), 0, 0x0123);  \
+            bool rc_ = a_ > cprev[r];                                                          \
+            if (a_ == cprev[r]) rc_ = canon_tie<K>(sbf + i + r, sbc + i + r);                  \
+            uint32_t x = mm3_round0(rc_ ? rring[r][((U) + NB - 1) % NB] : ring[r][U]);         \
+            _Pragma("unroll") for (int j = 1; j < NB; ++j)                                     \
+                x = mm3_round(x, rc_ ? rring[r][((U) + NB - 1 - j) % NB] : ring[r][((U) + j) % NB]); \
+            if (LUT) x ^= lds_u32((rc_ ? sbc[i + r] : sb[i + r]) * lut_stride + lut_base);     \
+            else if (TAIL) x ^= mm3_kmix(rc_ ? canon_tail<TAIL>(sbc + i + r) : w[r] & TAILMASK); \
+            x ^= (uint32_t)K;                                                                  \
+            h[r] = mm3_fmix(x);                                                                \
+            ring[r][U] = mm3_kmix(w[r]);                                                       \
+            rring[r][U] = mm3_kmix(__byte_perm(c[r], 0, 0x0123));                              \
+            cprev[r] = c[r];                                                                   \
+        }                                                                                      \
+        EMIT(0, h[0]);                                                                         \
+        EMIT(1, h[1]);                                                                         \
+        EMIT(2, h[2]);                                                                         \
+        EMIT(3, h[3]);                                                                         \
+        w_cur = w_nxt;                                                                         \
+        w_nxt = __funnelshift_r(raw_a, raw_b, sh);                                             \
+        raw_a = raw_b;                                                                         \
+        raw_b = *swp++;                                                                        \
+        c_cur = c_nxt;                                                                         \
+        c_nxt = __funnelshift_r(craw_a, craw_b, csh);                                          \
+        craw_a = craw_b;                                                                       \
+        craw_b = *cwp++;                                                                       \
+        l_cur = l_nxt;                                                                         \
+        l_nxt = __funnelshift_r(lraw_a, lraw_b, sh);                                           \
+        lraw_a = lraw_b;                                                                       \
+        lraw_b = *lwp++;                                                                       \
+        i += 4;                                                                                \
+    }
+
 // positional store: hash of k-mer i + r -> my_out[i + r]
 #define PG_EMIT_POSITIONAL(R_, H_) my_out[i + (R_)] = (H_)
 #define PG_K1_STEP(U, CHECKED) PG_KMER_STEP(U, CHECKED, PG_EMIT_POSITIONAL)

@@ -25,6 +25,8 @@
 // Winners (screen_winners, Mash Screen's winner-take-all): the same count pass without the segments gives each
 // reference's first-pass shared; then every value the pool holds votes among its contenders, one run of keys
 // (screen_vote_kernel, per sample), and the count pass above runs again over the won words only.
+// A canonical screen (PG_KMER_CANONICAL, ix.canon) adds with the CANON instantiations of the walk and generic kernels:
+// windows 0 .. L - k of each read, each the smaller of itself and its reverse complement (walk_chunk.cuh).
 #include <algorithm>
 #include <climits>
 
@@ -76,11 +78,11 @@ __device__ __forceinline__ bool screen_find(const ScreenLookup &L, uint64_t scal
 // id is not a sample: a select rather than one more condition on the hit, which keeps the walk kernels at their
 // registers.  Without SAMPLES (one sample, no ids) d is the counter, as in a single-sample screen.  Lanes that hit
 // the same counter add to it once, with their number.
-template <bool SAMPLES>
+template <bool SAMPLES, bool CANON>
 __device__ __forceinline__ void screen_hit(const ScreenLookup &L, uint64_t scale, const uint64_t *off, uint64_t n_reads, bool cand, uint64_t p,
                                            uint32_t k, uint32_t h, uint64_t &j) {
     uint64_t d = ~0ull;
-    bool hit = cand && window_in_read(off, n_reads, p, k, j) && screen_find(L, scale, h, &d);
+    bool hit = cand && window_in_read<CANON>(off, n_reads, p, k, j) && screen_find(L, scale, h, &d);
     if (SAMPLES && hit) {
         const uint32_t q = L.ids ? __ldg(L.ids + (j - 1)) : 0u;
         d = q < L.samples ? d * L.samples + q : L.sink;
@@ -95,14 +97,14 @@ __device__ __forceinline__ void screen_hit(const ScreenLookup &L, uint64_t scale
 #define PG_SCREEN_EMIT(R_, H_)                                                                                              \
     {                                                                                                                       \
         const bool cand_ = (H_) <= L.vmax;                                                                                  \
-        if (__any_sync(0xffffffffu, cand_)) screen_hit<SAMPLES>(L, scale, off, n_reads, cand_, p0 + i + (R_), (uint32_t)K, (H_), j); \
+        if (__any_sync(0xffffffffu, cand_)) screen_hit<SAMPLES, CANON>(L, scale, off, n_reads, cand_, p0 + i + (R_), (uint32_t)K, (H_), j); \
     }
 
 // The walk path (k in WalkKs).  Persistent CTAs take chunks of SCREEN_THREADS x W windows of the pool
 // [off[0], off[n_reads]); thread t walks windows [t W, t W + W) of the chunk.  The chunk's bytes, its look-ahead
 // and the 16-byte alignment head are staged in shared memory with 16-byte loads; bytes outside the pool are
 // zeros and are never read from global memory.
-template <int K, bool SAMPLES>
+template <int K, bool SAMPLES, bool CANON>
 __global__ void __launch_bounds__(SCREEN_THREADS, 2)
 screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ off, uint64_t n_reads, const ScreenLookup L,
                    uint32_t lut_stride) {
@@ -111,11 +113,18 @@ screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict
     constexpr uint32_t CHUNK = SCREEN_THREADS * W;
     constexpr uint32_t STAGE = CHUNK + 128;  // + head (< 16) + the walk's look-ahead (< 4 NB + 20 bytes)
     constexpr uint32_t nk = W;               // PG_KMER_STEP's bound; unchecked steps never test it
-    __shared__ __align__(16) uint8_t s_in[STAGE];
+    // CANON: the complemented copy s_rc and the complement table s_comp follow the chunk
+    __shared__ __align__(16) uint8_t s_in[CANON ? 2 * STAGE + 256 : STAGE];
     __shared__ __align__(16) uint32_t s_lut[LUT ? 256 : 4];
+    uint8_t *s_rc = nullptr, *s_comp = nullptr;
     const uint32_t tid = threadIdx.x;
     if (LUT)
         for (uint32_t x = tid; x < 256; x += SCREEN_THREADS) s_lut[x] = g_kmix_byte.v[x];
+    if constexpr (CANON) {
+        s_rc = s_in + STAGE;
+        s_comp = s_in + 2 * STAGE;
+        for (uint32_t x = tid; x < 256; x += SCREEN_THREADS) s_comp[x] = complement((uint8_t)x);
+    }
     const uint64_t lo = off[0], hi = max(off[n_reads], lo);
     const uint64_t chunks = (hi - lo + CHUNK - 1) / CHUNK;
     const uint64_t scale = join_bucket_scale(L.nb, L.vmax);
@@ -125,7 +134,8 @@ screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict
         const uint64_t P0 = lo + c * CHUNK;
         const uint32_t head = chunk_head(bases, P0);
         __syncthreads();  // the previous chunk's walk is done with s_in (and, the first time, s_lut is written)
-        stage_chunk<STAGE, SCREEN_THREADS>(s_in, bases, P0, head, lo, hi);
+        if constexpr (CANON) stage_chunk<STAGE, SCREEN_THREADS, true>(s_in, bases, P0, head, lo, hi, s_rc, s_comp);
+        else stage_chunk<STAGE, SCREEN_THREADS>(s_in, bases, P0, head, lo, hi);
         __syncthreads();
 
         const uint32_t b0 = head + tid * W;
@@ -135,18 +145,31 @@ screen_walk_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict
         const uint64_t p0 = P0 + tid * W;        // pool position of window 0
         uint64_t j = ~0ull;
 
-        PG_WALK_PROLOGUE
-        uint32_t i = 0;
-        while (i < W) {  // every lane runs the same steps, so the warp is converged at each window
+        if constexpr (CANON) {
+            const uint8_t *sbf = s_in + b0, *sbc = s_rc + b0;
+            const uint32_t *cw = reinterpret_cast<const uint32_t *>(s_rc) + ((b0 + TAIL) >> 2);
+            const uint32_t csh = ((b0 + TAIL) & 3u) * 8u;
+            PG_WALK_PROLOGUE
+            PG_CANON_PROLOGUE
+            uint32_t i = 0;
+            while (i < W) {
 #pragma unroll
-            for (int u = 0; u < NB; ++u) PG_KMER_STEP(u, false, PG_SCREEN_EMIT)
+                for (int u = 0; u < NB; ++u) PG_KMER_STEP_CANON(u, PG_SCREEN_EMIT)
+            }
+        } else {
+            PG_WALK_PROLOGUE
+            uint32_t i = 0;
+            while (i < W) {  // every lane runs the same steps, so the warp is converged at each window
+#pragma unroll
+                for (int u = 0; u < NB; ++u) PG_KMER_STEP(u, false, PG_SCREEN_EMIT)
+            }
         }
     }
 }
 
-// Any other k (0 included): window p of the pool is hashed from global memory by thread p of a CTA-uniform
-// grid-stride loop, so that every lane of a warp runs the same iterations.
-template <bool SAMPLES>
+// Any other k (0 included, but not in canonical mode): window p of the pool is hashed from global memory by thread p
+// of a CTA-uniform grid-stride loop, so that every lane of a warp runs the same iterations.
+template <bool SAMPLES, bool CANON>
 __global__ void __launch_bounds__(SCREEN_THREADS)
 screen_generic_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restrict__ off, uint64_t n_reads, uint32_t k, const ScreenLookup L) {
     const uint64_t lo = off[0], hi = max(off[n_reads], lo);
@@ -155,14 +178,13 @@ screen_generic_kernel(const uint8_t *__restrict__ bases, const uint64_t *__restr
         const uint64_t p = base + threadIdx.x;
         uint32_t h = 0;
         bool cand = false;
-        if (p < hi && hi - p > k) {
-            const uint8_t *w = bases + p;
-            h = mm3_bytes([w](uint32_t x) { return __ldg(w + x); }, k);
+        if (p < hi && window_fits<CANON>(hi - p, k)) {
+            h = window_hash<CANON>(bases + p, k);
             cand = h <= L.vmax;
         }
         if (__any_sync(0xffffffffu, cand)) {
             uint64_t j = ~0ull;
-            screen_hit<SAMPLES>(L, scale, off, n_reads, cand, p, k, h, j);
+            screen_hit<SAMPLES, CANON>(L, scale, off, n_reads, cand, p, k, h, j);
         }
     }
 }
@@ -282,13 +304,34 @@ ScreenLookup lookup_of(const ScreenIndex &ix, const uint32_t *ids = nullptr) {
 
 unsigned grid_of(uint64_t work) { return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((work + 255) / 256, (uint64_t)sm_count() * 16)); }
 
-template <int K, bool SAMPLES>
+template <int K, bool SAMPLES, bool CANON>
 int launch_screen_walk(const ScreenIndex &ix, const uint8_t *d_bases, const uint64_t *d_off, const uint32_t *d_ids, uint64_t n_reads,
                        cudaStream_t st) {
     uint64_t grid = 0;  // persistent: the pool's size is on the device, so the grid is what is resident at once
-    { const int rc_ = resident_blocks((const void *)screen_walk_kernel<K, SAMPLES>, SCREEN_THREADS, 0, ~0ull, &grid); if (rc_ != PG_OK) return rc_; }
-    screen_walk_kernel<K, SAMPLES><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, lookup_of(ix, d_ids), 4u);
+    { const int rc_ = resident_blocks((const void *)screen_walk_kernel<K, SAMPLES, CANON>, SCREEN_THREADS, 0, ~0ull, &grid); if (rc_ != PG_OK) return rc_; }
+    screen_walk_kernel<K, SAMPLES, CANON><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, lookup_of(ix, d_ids), 4u);
     PG_LAUNCH_CHECK("screen_walk_kernel");
+    return PG_OK;
+}
+
+// the add in one mode: screen_walk_kernel for k in WalkKs, screen_generic_kernel for any other k
+template <bool CANON>
+int screen_add_mode(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, const uint32_t *d_ids, uint64_t n_reads,
+                    cudaStream_t st) {
+    const bool samples = d_ids || ix.samples != 1;
+    int rc = PG_OK;
+    if (with_walk_k(k, [&](auto kk) {
+            constexpr int K = decltype(kk)::value;
+            rc = samples ? launch_screen_walk<K, true, CANON>(ix, d_bases, d_off, d_ids, n_reads, st)
+                         : launch_screen_walk<K, false, CANON>(ix, d_bases, d_off, d_ids, n_reads, st);
+        }))
+        return rc;
+    const void *fn = samples ? (const void *)screen_generic_kernel<true, CANON> : (const void *)screen_generic_kernel<false, CANON>;
+    uint64_t grid = 0;
+    if ((rc = resident_blocks(fn, SCREEN_THREADS, 0, ~0ull, &grid)) != PG_OK) return rc;
+    if (samples) screen_generic_kernel<true, CANON><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix, d_ids));
+    else screen_generic_kernel<false, CANON><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix, d_ids));
+    PG_LAUNCH_CHECK("screen_generic_kernel");
     return PG_OK;
 }
 
@@ -370,20 +413,7 @@ int screen_build(const uint32_t *d_sk, uint64_t n, int s, uint32_t samples, cuda
 int screen_add(const ScreenIndex &ix, int k, const uint8_t *d_bases, const uint64_t *d_off, const uint32_t *d_ids, uint64_t n_reads,
                cudaStream_t st) {
     if (n_reads == 0 || ix.D == 0) return PG_OK;
-    const bool samples = d_ids || ix.samples != 1;
-    int rc = PG_OK;
-    if (with_walk_k(k, [&](auto kk) {
-            constexpr int K = decltype(kk)::value;
-            rc = samples ? launch_screen_walk<K, true>(ix, d_bases, d_off, d_ids, n_reads, st) : launch_screen_walk<K, false>(ix, d_bases, d_off, d_ids, n_reads, st);
-        }))
-        return rc;
-    const void *fn = samples ? (const void *)screen_generic_kernel<true> : (const void *)screen_generic_kernel<false>;
-    uint64_t grid = 0;
-    if ((rc = resident_blocks(fn, SCREEN_THREADS, 0, ~0ull, &grid)) != PG_OK) return rc;
-    if (samples) screen_generic_kernel<true><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix, d_ids));
-    else screen_generic_kernel<false><<<(unsigned)grid, SCREEN_THREADS, 0, st>>>(d_bases, d_off, n_reads, (uint32_t)k, lookup_of(ix, d_ids));
-    PG_LAUNCH_CHECK("screen_generic_kernel");
-    return PG_OK;
+    return ix.canon ? screen_add_mode<true>(ix, k, d_bases, d_off, d_ids, n_reads, st) : screen_add_mode<false>(ix, k, d_bases, d_off, d_ids, n_reads, st);
 }
 
 int screen_reset(const ScreenIndex &ix, cudaStream_t st) {

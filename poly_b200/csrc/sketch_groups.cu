@@ -19,6 +19,10 @@
 // admits every window and sorts them out with a forward cursor over the group byte offsets.  Per window: one range
 // compare and a warp vote, as in the screen; the rare admitted windows then take window_in_read and one table add per
 // distinct (group, value) of the warp.
+//
+// Canonical mode (PG_KMER_CANONICAL) is the template parameter CANON of the walk, generic and window-count kernels:
+// windows 0 .. L - k of each record, each hashing the smaller of itself and its reverse complement (walk_chunk.cuh,
+// kmer_walk.cuh).  Everything after the walk is the same.
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -120,6 +124,7 @@ __device__ __forceinline__ void table_add(const PassArgs &A, const GroupPass &g,
 // windows all lie in group g that compare was exact; a mixed thread (its windows cross a group end or the span end)
 // admits every window, and here finds the group of window p with its forward cursor g and applies that group's range.
 // Lanes with the same (group, hash) add once, with their number.
+template <bool CANON>
 __device__ __forceinline__ void group_hit(const PassArgs &A, bool cand, bool mixed, uint64_t &g, uint64_t send, uint64_t p, uint32_t k, uint32_t h,
                                           uint64_t &j) {
     if (cand && mixed) {
@@ -130,7 +135,7 @@ __device__ __forceinline__ void group_hit(const PassArgs &A, bool cand, bool mix
             cand = (uint64_t)(h - A.gp[g].lo) < A.gp[g].width;
         }
     }
-    const bool hit = cand && window_in_read(A.off, A.n_records, p, k, j);
+    const bool hit = cand && window_in_read<CANON>(A.off, A.n_records, p, k, j);
     const unsigned long long key = hit ? (g << 32 | h) : ~0ull;
     const unsigned peers = __match_any_sync(0xffffffffu, key);
     if (hit && (int)(threadIdx.x & 31) == __ffs(peers) - 1) table_add(A, A.gp[g], h, (unsigned)__popc(peers));
@@ -140,10 +145,10 @@ __device__ __forceinline__ void group_hit(const PassArgs &A, bool cand, bool mix
 #define PG_GROUPS_EMIT(R_, H_)                                                                                              \
     {                                                                                                                       \
         const bool cand_ = (uint32_t)((H_) - lo) <= wm1;                                                                    \
-        if (__any_sync(0xffffffffu, cand_)) group_hit(A, cand_, mixed, g, send, p0 + i + (R_), (uint32_t)K, (H_), j);       \
+        if (__any_sync(0xffffffffu, cand_)) group_hit<CANON>(A, cand_, mixed, g, send, p0 + i + (R_), (uint32_t)K, (H_), j);\
     }
 
-template <int K>
+template <int K, bool CANON>
 __global__ void __launch_bounds__(GS_THREADS, 2) groups_walk_kernel(const uint8_t *__restrict__ bases, const PassArgs A, uint64_t chunks,
                                                                     uint32_t lut_stride) {
     PG_WALK_CONSTANTS;
@@ -151,12 +156,19 @@ __global__ void __launch_bounds__(GS_THREADS, 2) groups_walk_kernel(const uint8_
     constexpr uint32_t CHUNK = GS_THREADS * W;
     constexpr uint32_t STAGE = CHUNK + 128;  // + head (< 16) + the walk's look-ahead (< 4 NB + 20 bytes)
     constexpr uint32_t nk = W;
-    __shared__ __align__(16) uint8_t s_in[STAGE];
+    // CANON: the complemented copy s_rc and the complement table s_comp follow the chunk
+    __shared__ __align__(16) uint8_t s_in[CANON ? 2 * STAGE + 256 : STAGE];
     __shared__ __align__(16) uint32_t s_lut[LUT ? 256 : 4];
     __shared__ uint64_t s_g[2];  // the groups of the chunk's first and last window
+    uint8_t *s_rc = nullptr, *s_comp = nullptr;
     const uint32_t tid = threadIdx.x;
     if (LUT)
         for (uint32_t x = tid; x < 256; x += GS_THREADS) s_lut[x] = g_kmix_byte.v[x];
+    if constexpr (CANON) {
+        s_rc = s_in + STAGE;
+        s_comp = s_in + 2 * STAGE;
+        for (uint32_t x = tid; x < 256; x += GS_THREADS) s_comp[x] = complement((uint8_t)x);
+    }
     const uint32_t lut_base = smem_u32(s_lut);
 
     for (uint64_t c = blockIdx.x; c < chunks; c += gridDim.x) {
@@ -168,7 +180,8 @@ __global__ void __launch_bounds__(GS_THREADS, 2) groups_walk_kernel(const uint8_
             s_g[0] = group_of(A.gbyte, A.n_groups, P0);
             s_g[1] = group_of(A.gbyte, A.n_groups, min(P0 + CHUNK, send) - 1);
         }
-        stage_chunk<STAGE, GS_THREADS>(s_in, bases, P0, head, sp.beg, sp.end);
+        if constexpr (CANON) stage_chunk<STAGE, GS_THREADS, true>(s_in, bases, P0, head, sp.beg, sp.end, s_rc, s_comp);
+        else stage_chunk<STAGE, GS_THREADS>(s_in, bases, P0, head, sp.beg, sp.end);
         __syncthreads();
 
         const uint32_t b0 = head + tid * W;
@@ -191,16 +204,31 @@ __global__ void __launch_bounds__(GS_THREADS, 2) groups_walk_kernel(const uint8_
             wm1 = mixed ? 0xFFFFFFFFu : (uint32_t)(A.gp[g].width - 1);  // a group of the pass has width >= 1
         }
 
-        PG_WALK_PROLOGUE
-        uint32_t i = 0;
-        while (i < W) {
+        if constexpr (CANON) {
+            const uint8_t *sbf = s_in + b0, *sbc = s_rc + b0;
+            const uint32_t *cw = reinterpret_cast<const uint32_t *>(s_rc) + ((b0 + TAIL) >> 2);
+            const uint32_t csh = ((b0 + TAIL) & 3u) * 8u;
+            PG_WALK_PROLOGUE
+            PG_CANON_PROLOGUE
+            uint32_t i = 0;
+            while (i < W) {
 #pragma unroll
-            for (int u = 0; u < NB; ++u) PG_KMER_STEP(u, false, PG_GROUPS_EMIT)
+                for (int u = 0; u < NB; ++u) PG_KMER_STEP_CANON(u, PG_GROUPS_EMIT)
+            }
+        } else {
+            PG_WALK_PROLOGUE
+            uint32_t i = 0;
+            while (i < W) {
+#pragma unroll
+                for (int u = 0; u < NB; ++u) PG_KMER_STEP(u, false, PG_GROUPS_EMIT)
+            }
         }
     }
 }
 
-// Any other k (0 included): one window per thread from global memory, over chunks of GS_THREADS bytes of the spans.
+// Any other k (0 included, but not in canonical mode): one window per thread from global memory, over chunks of
+// GS_THREADS bytes of the spans.
+template <bool CANON>
 __global__ void __launch_bounds__(GS_THREADS) groups_generic_kernel(const uint8_t *__restrict__ bases, const PassArgs A, uint64_t chunks, uint32_t k) {
     for (uint64_t c = blockIdx.x; c < chunks; c += gridDim.x) {
         const Span sp = A.spans[span_of(A.spans, A.n_spans, c)];
@@ -208,24 +236,24 @@ __global__ void __launch_bounds__(GS_THREADS) groups_generic_kernel(const uint8_
         uint32_t h = 0;
         bool cand = false;
         uint64_t g = 0;
-        if (p < sp.end && sp.end - p > k) {
-            const uint8_t *w = bases + p;
-            h = mm3_bytes([w](uint32_t x) { return __ldg(w + x); }, k);
+        if (p < sp.end && window_fits<CANON>(sp.end - p, k)) {
+            h = window_hash<CANON>(bases + p, k);
             g = group_of(A.gbyte, A.n_groups, p);
             cand = (uint64_t)(h - A.gp[g].lo) < A.gp[g].width;
         }
         if (__any_sync(0xffffffffu, cand)) {
             uint64_t j = ~0ull;
-            group_hit(A, cand, false, g, sp.end, p, k, h, j);
+            group_hit<CANON>(A, cand, false, g, sp.end, p, k, h, j);
         }
     }
 }
 
-// windows of each record, max(len - k, 0)
+// windows of each record, max(len - k, 0) (canonical: max(len - k + 1, 0))
+template <bool CANON>
 __global__ void groups_windows_kernel(const uint64_t *__restrict__ off, uint64_t n, uint32_t k, uint64_t *__restrict__ win) {
     for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t len = off[r + 1] - off[r];
-        win[r] = len > k ? len - k : 0;
+        win[r] = CANON ? (len >= k ? len - k + 1 : 0) : (len > k ? len - k : 0);
     }
 }
 
@@ -430,7 +458,7 @@ int gs_nomem(cudaError_t e) {
 
 // per group of a batch: its windows wg[g] and the byte offset of its first record gbyte[g] (G + 1 of them), on the
 // host and in *d_gbyte (from tmp)
-int group_sizes(const uint64_t *d_off, uint64_t n_records, const uint64_t *d_goff, uint64_t G, int k, StreamScratch &tmp, std::vector<uint64_t> &wg,
+int group_sizes(const uint64_t *d_off, uint64_t n_records, const uint64_t *d_goff, uint64_t G, int k, bool canon, StreamScratch &tmp, std::vector<uint64_t> &wg,
                 std::vector<uint64_t> &gbyte, uint64_t **d_gbyte, cudaStream_t st) {
     cudaError_t e;
     uint64_t *d_win = nullptr, *d_pre = nullptr, *d_wg = nullptr;
@@ -438,7 +466,8 @@ int group_sizes(const uint64_t *d_off, uint64_t n_records, const uint64_t *d_gof
         (e = tmp.alloc(&d_wg, G)) != cudaSuccess || (e = tmp.alloc(d_gbyte, G + 1)) != cudaSuccess)
         return gs_nomem(e);
     PG_CUDA(cudaMemsetAsync(d_win + n_records, 0, 8, st));
-    groups_windows_kernel<<<grid_for(n_records), 256, 0, st>>>(d_off, n_records, (uint32_t)k, d_win);
+    if (canon) groups_windows_kernel<true><<<grid_for(n_records), 256, 0, st>>>(d_off, n_records, (uint32_t)k, d_win);
+    else groups_windows_kernel<false><<<grid_for(n_records), 256, 0, st>>>(d_off, n_records, (uint32_t)k, d_win);
     PG_LAUNCH_CHECK("groups_windows_kernel");
     {
         size_t bytes = 0;
@@ -511,35 +540,40 @@ uint64_t walk_chunk_bytes(int k) {
 }
 
 // a pass's walk over its spans: groups_walk_kernel<k> for k in WalkKs, groups_generic_kernel for any other k
-int launch_walk(const uint8_t *d_bases, const PassArgs &args, uint64_t chunks, int k, cudaStream_t st) {
-    if (!chunks) return PG_OK;
+template <bool CANON>
+int launch_walk_mode(const uint8_t *d_bases, const PassArgs &args, uint64_t chunks, int k, cudaStream_t st) {
     uint64_t grid = 0;
     int rc = PG_OK;
     const bool walk = with_walk_k(k, [&](auto kk) {
         constexpr int K = decltype(kk)::value;
-        if ((rc = resident_blocks((const void *)groups_walk_kernel<K>, GS_THREADS, 0, chunks, &grid)) != PG_OK) return;
-        groups_walk_kernel<K><<<(unsigned)grid, GS_THREADS, 0, st>>>(d_bases, args, chunks, 4u);
+        if ((rc = resident_blocks((const void *)groups_walk_kernel<K, CANON>, GS_THREADS, 0, chunks, &grid)) != PG_OK) return;
+        groups_walk_kernel<K, CANON><<<(unsigned)grid, GS_THREADS, 0, st>>>(d_bases, args, chunks, 4u);
     });
     if (!walk) {
-        if ((rc = resident_blocks((const void *)groups_generic_kernel, GS_THREADS, 0, chunks, &grid)) != PG_OK) return rc;
-        groups_generic_kernel<<<(unsigned)grid, GS_THREADS, 0, st>>>(d_bases, args, chunks, (uint32_t)k);
+        if ((rc = resident_blocks((const void *)groups_generic_kernel<CANON>, GS_THREADS, 0, chunks, &grid)) != PG_OK) return rc;
+        groups_generic_kernel<CANON><<<(unsigned)grid, GS_THREADS, 0, st>>>(d_bases, args, chunks, (uint32_t)k);
     }
     if (rc != PG_OK) return rc;
     PG_LAUNCH_CHECK(walk ? "groups_walk_kernel" : "groups_generic_kernel");
     return PG_OK;
 }
 
+int launch_walk(const uint8_t *d_bases, const PassArgs &args, uint64_t chunks, int k, bool canon, cudaStream_t st) {
+    if (!chunks) return PG_OK;
+    return canon ? launch_walk_mode<true>(d_bases, args, chunks, k, st) : launch_walk_mode<false>(d_bases, args, chunks, k, st);
+}
+
 }  // namespace
 
 int sketch_groups(const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_records, const uint64_t *d_goff, uint64_t G, int k, int s,
-                  uint32_t m, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, cudaStream_t st) {
+                  uint32_t m, bool canon, uint32_t *d_out, uint64_t row_stride, uint32_t *d_count, cudaStream_t st) {
     if (G == 0) return PG_OK;
     StreamScratch tmp(st);
     cudaError_t e;
     PG_CUDA(cudaMemsetAsync(d_out, 0, G * row_stride * 4, st));
     std::vector<uint64_t> wg, gbyte;
     uint64_t *d_gbyte = nullptr;
-    int rc = group_sizes(d_off, n_records, d_goff, G, k, tmp, wg, gbyte, &d_gbyte, st);
+    int rc = group_sizes(d_off, n_records, d_goff, G, k, canon, tmp, wg, gbyte, &d_gbyte, st);
     if (rc != PG_OK) return rc;
 
     const double mu = admit_target((double)s);
@@ -595,7 +629,7 @@ int sketch_groups(const uint8_t *d_bases, const uint64_t *d_off, uint64_t n_reco
         PG_CUDA(cudaMemsetAsync(d_n, 0, 8, st));
 
         const PassArgs args{d_off, n_records, d_gbyte, G, d_gp, d_spans, (uint32_t)spans.size(), d_keys, d_cnt, d_claims, d_ovf};
-        if ((rc = launch_walk(d_bases, args, chunks, k, st)) != PG_OK) return rc;
+        if ((rc = launch_walk(d_bases, args, chunks, k, canon, st)) != PG_OK) return rc;
         groups_collect_kernel<<<grid_for(slots), 256, 0, st>>>(d_keys, d_cnt, d_slot_of, slots, m, d_col, d_n, d_qual);
         PG_LAUNCH_CHECK("groups_collect_kernel");
         unsigned long long n_col = 0;
@@ -688,7 +722,7 @@ int sketcher_add(SketcherState &S, const uint8_t *d_bases, const uint64_t *d_off
     cudaError_t e;
     std::vector<uint64_t> wg, gbyte;
     uint64_t *d_gbyte = nullptr;
-    int rc = group_sizes(d_off, n_records, d_goff, nb, S.k, tmp, wg, gbyte, &d_gbyte, st);
+    int rc = group_sizes(d_off, n_records, d_goff, nb, S.k, S.canon, tmp, wg, gbyte, &d_gbyte, st);
     if (rc != PG_OK) return rc;
     const uint64_t B = S.B;
     const uint32_t s = (uint32_t)S.s, m = S.m;
@@ -766,7 +800,7 @@ int sketcher_add(SketcherState &S, const uint8_t *d_bases, const uint64_t *d_off
         // a pass is always 4 launches (seed, walk, collect, cut), so that a caller can count passes
         sketcher_seed_kernel<<<grid_for(old_n), 256, 0, st>>>(S.d_val, S.d_cnt, S.d_seg + first, nb, args);
         PG_LAUNCH_CHECK("sketcher_seed_kernel");
-        if ((rc = launch_walk(d_bases, args, chunks, S.k, st)) != PG_OK) return rc;
+        if ((rc = launch_walk(d_bases, args, chunks, S.k, S.canon, st)) != PG_OK) return rc;
         sketcher_collect_kernel<<<grid_for(slots), 256, 0, st>>>(d_keys, d_cnt, d_slot_of, slots, m, d_col, d_ccnt, d_n, d_per);
         PG_LAUNCH_CHECK("sketcher_collect_kernel");
         unsigned long long n_col = 0;

@@ -182,11 +182,14 @@ def _group_args(k: int, s: int, min_copies: int) -> None:
         raise PolyError(_lib.PG_ERR_ARG, f"min_copies {min_copies}: need 1 <= min_copies < 2^32")
 
 
-def sketch_groups(bases, offsets, group_offsets, k: int, s: int, min_copies: int = 1):
+def sketch_groups(bases, offsets, group_offsets, k: int, s: int, min_copies: int = 1, canonical: bool = False):
     """One sketch per group of records (Mash's `mash sketch` of a multi-FASTA file, or `-r -m min_copies` of a read
     set): group g is records [group_offsets[g], group_offsets[g+1]) of the ragged batch (bases, offsets).  Row g holds
     the smallest min(q_g, s) distinct window hashes of the group that occur at least min_copies times, ascending, then
-    zeros; count[g] is how many.  Windows never cross a record.  Returns (rows [G, s] uint32, count [G] uint32): NumPy
+    zeros; count[g] is how many.  Windows never cross a record.  With canonical=False the windows are positions
+    0 .. L - k - 1 of each record, forward strand only; canonical=True (PG_KMER_CANONICAL) takes Mash's k-mer set,
+    positions 0 .. L - k, each hashing the smaller of itself and its reverse complement, so contigs of either
+    orientation and reads of either strand count as one (k >= 1).  Returns (rows [G, s] uint32, count [G] uint32): NumPy
     arrays for host inputs; for CUDA tensor inputs (uint8 bases, int64 offsets holding uint64 bits) int32 CUDA tensors
     holding the uint32 bits, computed on the current stream (the call waits for it)."""
     k, s, min_copies = int(k), int(s), int(min_copies)
@@ -202,9 +205,9 @@ def sketch_groups(bases, offsets, group_offsets, k: int, s: int, min_copies: int
         rows = torch.empty((G, s), dtype=torch.int32, device=bases.device)
         count = torch.empty(G, dtype=torch.int32, device=bases.device)
         st = torch.cuda.current_stream(bases.device).cuda_stream
-        _lib.check(_lib.lib().pg_mash_sketch_groups_dev(bases.data_ptr() if bases.numel() else None, offsets.data_ptr() if n or G else None, n,
-                                                        group_offsets.data_ptr() if G else None, G, k, s, min_copies, rows.data_ptr(), s,
-                                                        count.data_ptr(), st))
+        _lib.check(_lib.lib().pg_mash_sketch_groups_flags_dev(bases.data_ptr() if bases.numel() else None, offsets.data_ptr() if n or G else None,
+                                                              n, group_offsets.data_ptr() if G else None, G, k, s, min_copies, _kmer_flags(canonical),
+                                                              rows.data_ptr(), s, count.data_ptr(), st))
         return rows, count
     bases = np.ascontiguousarray(bases, dtype=np.uint8)
     offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
@@ -216,15 +219,21 @@ def sketch_groups(bases, offsets, group_offsets, k: int, s: int, min_copies: int
     count = np.zeros(G, np.uint32)
     if len(bases) == 0:
         bases = np.zeros(1, np.uint8)
-    _lib.check(_lib.lib().pg_mash_sketch_groups(bases.ctypes.data, offsets.ctypes.data, n, group_offsets.ctypes.data, G, k, s, min_copies,
-                                                rows.ctypes.data, s, count.ctypes.data))
+    _lib.check(_lib.lib().pg_mash_sketch_groups_flags(bases.ctypes.data, offsets.ctypes.data, n, group_offsets.ctypes.data, G, k, s, min_copies,
+                                                      _kmer_flags(canonical), rows.ctypes.data, s, count.ctypes.data))
     return rows, count
 
 
-def SketchGroups(groups: Sequence[Sequence[BytesLike]], kmer_size: int, sketch_size: int, min_copies: int = 1) -> List[Mash]:
+def _kmer_flags(canonical: bool) -> int:
+    return _lib.PG_KMER_CANONICAL if canonical else 0
+
+
+def SketchGroups(groups: Sequence[Sequence[BytesLike]], kmer_size: int, sketch_size: int, min_copies: int = 1,
+                 canonical: bool = False) -> List[Mash]:
     """[][]string -> []*Mash: one Mash per group of sequences (an assembly's contigs, a sample's reads), holding the
     smallest sketch_size distinct window hashes of the group seen at least min_copies times, ascending, and a zero
-    tail when fewer qualify.  The result compares with Similarity / Distance and feeds every sketch-set call."""
+    tail when fewer qualify.  canonical=True hashes canonical k-mers (see sketch_groups).  The result compares with
+    Similarity / Distance and feeds every sketch-set call."""
     if isinstance(groups, (str, bytes)) or any(isinstance(g, (str, bytes, bytearray, np.ndarray)) for g in groups):
         raise ValueError("groups must be a list of lists of sequences")
     seqs = [q for g in groups for q in g]
@@ -232,7 +241,7 @@ def SketchGroups(groups: Sequence[Sequence[BytesLike]], kmer_size: int, sketch_s
     goff = np.zeros(len(groups) + 1, np.uint64)
     if groups:
         goff[1:] = np.cumsum([len(g) for g in groups], dtype=np.uint64)
-    rows, count = sketch_groups(bases, offsets, goff, kmer_size, sketch_size, min_copies)
+    rows, count = sketch_groups(bases, offsets, goff, kmer_size, sketch_size, min_copies, canonical)
     res = []
     for g in range(len(groups)):
         m = Mash(kmer_size, sketch_size)
@@ -249,19 +258,22 @@ class Sketcher:
     min_copies times plus one, and the (max_values + 1)-th distinct value.  A row is complete when it holds s values
     or its cap is still 2^32; a complete row equals sketch_groups over every record added to the group, whatever the
     split, and every row is a prefix of that row.  With min_copies = 1 every row is complete.  max_values defaults to
-    64 s; an incomplete row asks for a larger one.  The sketcher lives on the device current at creation."""
+    64 s; an incomplete row asks for a larger one.  canonical=True counts canonical k-mers in every add, as
+    sketch_groups(..., canonical=True) does, and complete rows equal that call's.  The sketcher lives on the device
+    current at creation."""
 
-    def __init__(self, n_groups: int, k: int, s: int, min_copies: int = 1, max_values: Optional[int] = None):
+    def __init__(self, n_groups: int, k: int, s: int, min_copies: int = 1, max_values: Optional[int] = None, canonical: bool = False):
         n_groups, k, s, min_copies = int(n_groups), int(k), int(s), int(min_copies)
         _group_args(k, s, min_copies)
         max_values = 64 * s if max_values is None else int(max_values)
         if not 0 <= n_groups < (1 << 64) or not 0 <= max_values < (1 << 64):
             raise PolyError(_lib.PG_ERR_ARG, f"n_groups {n_groups} and max_values {max_values} must fit uint64")
         h = C.c_void_p()
-        _lib.check(_lib.lib().pg_mash_sketcher_create(n_groups, k, s, min_copies, max_values, C.byref(h)))
+        _lib.check(_lib.lib().pg_mash_sketcher_create_flags(n_groups, k, s, min_copies, max_values, _kmer_flags(canonical), C.byref(h)))
         self._h = h
         self._dev_used = None
         self.n_groups, self.k, self.s, self.min_copies, self.max_values = n_groups, k, s, min_copies, max_values
+        self.canonical = bool(canonical)
 
     def _live(self):
         if self._h is None:
@@ -968,15 +980,18 @@ class Screen:
 
     sketches: [n, s] uint32 (full Go arrays, zero tail included), a CUDA tensor of that shape, or a list of Mash of
     one SketchSize; k: the k-mer size they were sketched with (not checked, as in the reference).  The pool grows with
-    each add, in any split, and reset() empties it.  Reverse-complement windows are not counted: the references hash
-    the forward strand only.  The screen copies the sketches; it lives on the device current at creation.
+    each add, in any split, and reset() empties it.  With canonical=False reverse-complement windows are not counted:
+    the references hash the forward strand only.  canonical=True counts canonical k-mers (positions 0 .. L - k, each the
+    smaller of itself and its reverse complement), so reads of both strands count; pass sketches made the same way,
+    e.g. by sketch_groups(..., canonical=True) (the mode, like k, is not checked).  The screen copies the sketches; it
+    lives on the device current at creation.
 
     samples: the number of pools the screen holds over the one reference index (a multiplexed run's barcodes).  Each
     read of an add goes to one sample; row q of results_samples / winners_samples is exactly what a one-sample
     screen fed only sample q's reads would answer.  With the default samples=1 and sample=0 everything is the
     single-pool screen."""
 
-    def __init__(self, sketches, k: int, samples: int = 1):
+    def __init__(self, sketches, k: int, samples: int = 1, canonical: bool = False):
         rows = _sketch_rows(sketches)
         n, s = int(rows.shape[0]), int(rows.shape[1])
         if not -(1 << 31) <= k < (1 << 31):
@@ -988,14 +1003,15 @@ class Screen:
         if hasattr(rows, "data_ptr"):
             import torch
 
-            rc = _lib.lib().pg_mash_screen_create_samples_dev(rows.data_ptr(), n, s, k, samples, torch.cuda.current_stream(rows.device).cuda_stream,
-                                                              C.byref(h))
+            rc = _lib.lib().pg_mash_screen_create_flags_dev(rows.data_ptr(), n, s, k, samples, _kmer_flags(canonical),
+                                                            torch.cuda.current_stream(rows.device).cuda_stream, C.byref(h))
         else:
-            rc = _lib.lib().pg_mash_screen_create_samples(rows.ctypes.data, n, s, k, samples, C.byref(h))
+            rc = _lib.lib().pg_mash_screen_create_flags(rows.ctypes.data, n, s, k, samples, _kmer_flags(canonical), C.byref(h))
         _index_rc(rc)
         self._h = h
         self._dev_used = None
         self.n, self.s, self.k, self.samples = n, s, int(k), samples
+        self.canonical = bool(canonical)
 
     def _live(self):
         if self._h is None:
