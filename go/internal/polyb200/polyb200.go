@@ -304,6 +304,93 @@ func DistanceSparse(sketches []uint32, n, s int, rowBegin, rowEnd int, upper boo
 	}
 }
 
+// DistResult holds pg_mash_dist's nq x nr outputs, row-major with the query as the row.
+type DistResult struct {
+	Common, Denom    []uint32
+	Distance, PValue []float64
+}
+
+func u32p(a []uint32) *C.uint32_t {
+	if len(a) == 0 {
+		return nil
+	}
+	return (*C.uint32_t)(unsafe.Pointer(&a[0]))
+}
+
+func u64p(a []uint64) *C.uint64_t {
+	if len(a) == 0 {
+		return nil
+	}
+	return (*C.uint64_t)(unsafe.Pointer(&a[0]))
+}
+
+func f64p(a []float64) *C.double {
+	if len(a) == 0 {
+		return nil
+	}
+	return (*C.double)(unsafe.Pointer(&a[0]))
+}
+
+// Dist wraps pg_mash_dist: nq query rows against nr reference rows, each row s words (row stride s) holding count[i]
+// ascending values.  qLen and rLen (nil: no p-value) are the bases behind each sketch.
+func Dist(q, qCount []uint32, r, rCount []uint32, s, k int, qLen, rLen []uint64) (res DistResult, err error) {
+	nq, nr := len(qCount), len(rCount)
+	res = DistResult{make([]uint32, nq*nr), make([]uint32, nq*nr), make([]float64, nq*nr), nil}
+	if qLen != nil {
+		res.PValue = make([]float64, nq*nr)
+	}
+	err = locked(func() C.int {
+		return C.pg_mash_dist(u32p(q), u32p(qCount), C.uint64_t(nq), u32p(r), u32p(rCount), C.uint64_t(nr), C.uint64_t(s), C.int32_t(s), C.int32_t(k),
+			u64p(qLen), u64p(rLen), u32p(res.Common), u32p(res.Denom), f64p(res.Distance), f64p(res.PValue))
+	})
+	return res, err
+}
+
+// DistPairs holds pg_mash_dist_within's list, in the call's (unspecified) order.
+type DistPairs struct {
+	Q, R, Common, Denom []uint32
+	Distance, PValue    []float64
+}
+
+// DistWithin wraps pg_mash_dist_within: the pairs of Dist with distance <= maxDistance and p-value <= maxPValue;
+// upper keeps r > q only (nq == nr).  qLen and rLen may be nil when maxPValue >= 1 (no p-value then).
+func DistWithin(q, qCount []uint32, r, rCount []uint32, s, k int, qLen, rLen []uint64, maxDistance, maxPValue float64, upper bool) (DistPairs, error) {
+	nq, nr := len(qCount), len(rCount)
+	flags := C.uint32_t(0)
+	if upper {
+		flags = C.PG_PAIRS_UPPER
+	}
+	capPairs := 4*nq + 1024
+	for {
+		p := DistPairs{make([]uint32, capPairs), make([]uint32, capPairs), make([]uint32, capPairs), make([]uint32, capPairs),
+			make([]float64, capPairs), nil}
+		if qLen != nil {
+			p.PValue = make([]float64, capPairs)
+		}
+		var cnt C.uint64_t
+		var rc C.int
+		err := locked(func() C.int {
+			rc = C.pg_mash_dist_within(u32p(q), u32p(qCount), C.uint64_t(nq), u32p(r), u32p(rCount), C.uint64_t(nr), C.uint64_t(s), C.int32_t(s),
+				C.int32_t(k), u64p(qLen), u64p(rLen), C.double(maxDistance), C.double(maxPValue), flags, u32p(p.Q), u32p(p.R), u32p(p.Common),
+				u32p(p.Denom), f64p(p.Distance), f64p(p.PValue), C.uint64_t(capPairs), &cnt)
+			return rc
+		})
+		if rc == C.PG_ERR_ARG && int(cnt) > capPairs { // the buffers were too small: the call reports the size it needs
+			capPairs = int(cnt)
+			continue
+		}
+		if err != nil {
+			return DistPairs{}, err
+		}
+		n := int(cnt)
+		p.Q, p.R, p.Common, p.Denom, p.Distance = p.Q[:n], p.R[:n], p.Common[:n], p.Denom[:n], p.Distance[:n]
+		if p.PValue != nil {
+			p.PValue = p.PValue[:n]
+		}
+		return p, nil
+	}
+}
+
 // Cluster wraps pg_mash_cluster: single-linkage groups of n sketches of size s, sketches i < j being linked when
 // sketches[i].Similarity(sketches[j]) counts at least minSame matching hashes (the lower index is the receiver).
 // label[i] is the smallest index of i's group; nGroups counts the groups and nLinks the linked pairs.

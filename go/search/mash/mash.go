@@ -7,6 +7,7 @@ import (
 	"errors"
 	"fmt"
 	"math"
+	"sort"
 	"sync"
 
 	"github.com/bebop/poly/internal/polyb200"
@@ -126,6 +127,113 @@ func sketchGroups(groups [][]string, kmerSize, sketchSize, minCopies int, flags 
 		res[g] = &Mash{KmerSize: kmerSize, SketchSize: sketchSize, Sketches: out[g*sketchSize : (g+1)*sketchSize : (g+1)*sketchSize]}
 	}
 	return res, nil
+}
+
+// DistResult is Dist's answer for every (query, reference) pair, row-major with the query as the row:
+// index q*len(refs) + r.
+type DistResult = polyb200.DistResult
+
+// DistPairs is DistWithin's answer, sorted by (query, reference).
+type DistPairs = polyb200.DistPairs
+
+// distRows lays a sketch set out as the C ABI's rows.  A *Mash holds no count, so a sketch's count is the length of the
+// strictly ascending prefix of Sketches; a sketch whose words are all zero is empty.  This reads the sketches of
+// SketchGroups and Sketcher exactly (their rows are ascending with a zero tail); a real hash of 0 can only open a row,
+// and is counted there when the row goes on.
+func distRows(set []*Mash, s int) (rows, count []uint32, err error) {
+	rows, count = make([]uint32, len(set)*s), make([]uint32, len(set))
+	for i, m := range set {
+		if m.SketchSize != s || len(m.Sketches) < s {
+			return nil, nil, fmt.Errorf("mash: sketch %d has SketchSize %d, want %d", i, m.SketchSize, s)
+		}
+		copy(rows[i*s:(i+1)*s], m.Sketches[:s])
+		n := 0
+		if s > 0 && (m.Sketches[0] != 0 || (s > 1 && m.Sketches[1] != 0)) {
+			n = 1
+			for n < s && m.Sketches[n] > m.Sketches[n-1] {
+				n++
+			}
+		}
+		count[i] = uint32(n)
+	}
+	return rows, count, nil
+}
+
+func distInputs(queries, refs []*Mash) (s, k int, err error) {
+	switch {
+	case len(queries) > 0:
+		s, k = queries[0].SketchSize, queries[0].KmerSize
+	case len(refs) > 0:
+		s, k = refs[0].SketchSize, refs[0].KmerSize
+	default:
+		return 1, 1, nil
+	}
+	for _, m := range append(append([]*Mash{}, queries...), refs...) {
+		if m.KmerSize != k {
+			return 0, 0, fmt.Errorf("mash: sketches of kmerSize %d and %d", k, m.KmerSize)
+		}
+	}
+	return s, k, nil
+}
+
+// Dist is `mash dist` over grouped sketches: for every query and reference, Mash's shared count among the bottom
+// SketchSize values of the pair's union (Denom = min(SketchSize, union size)), the distance -ln(2J/(1+J))/k with
+// J = Common/Denom, and the p-value from the genome lengths (bases behind each sketch; nil lengths: no p-value).
+// Unlike Distance, a sketch with fewer than SketchSize values compares as the set it is.  All sketches share one
+// SketchSize and KmerSize.  A sketch's count is the length of the strictly ascending prefix of its Sketches, and a
+// sketch of all zeros is empty: what SketchGroups and Sketcher return.
+func Dist(queries, refs []*Mash, qLen, rLen []uint64) (DistResult, error) {
+	s, k, err := distInputs(queries, refs)
+	if err != nil {
+		return DistResult{}, err
+	}
+	q, qc, err := distRows(queries, s)
+	if err != nil {
+		return DistResult{}, err
+	}
+	r, rc, err := distRows(refs, s)
+	if err != nil {
+		return DistResult{}, err
+	}
+	return polyb200.Dist(q, qc, r, rc, s, k, qLen, rLen)
+}
+
+// DistWithin is `mash dist -d maxDistance -v maxPValue` (upper: `mash triangle`, a set against itself, reference >
+// query only): the pairs of Dist within both limits, sorted by (query, reference).  Counts are read as in Dist.
+func DistWithin(queries, refs []*Mash, qLen, rLen []uint64, maxDistance, maxPValue float64, upper bool) (DistPairs, error) {
+	s, k, err := distInputs(queries, refs)
+	if err != nil {
+		return DistPairs{}, err
+	}
+	q, qc, err := distRows(queries, s)
+	if err != nil {
+		return DistPairs{}, err
+	}
+	r, rc, err := distRows(refs, s)
+	if err != nil {
+		return DistPairs{}, err
+	}
+	p, err := polyb200.DistWithin(q, qc, r, rc, s, k, qLen, rLen, maxDistance, maxPValue, upper)
+	if err != nil {
+		return DistPairs{}, err
+	}
+	order := make([]int, len(p.Q))
+	for i := range order {
+		order[i] = i
+	}
+	sort.Slice(order, func(a, b int) bool {
+		x, y := order[a], order[b]
+		return p.Q[x] < p.Q[y] || (p.Q[x] == p.Q[y] && p.R[x] < p.R[y])
+	})
+	out := DistPairs{}
+	for _, i := range order {
+		out.Q, out.R = append(out.Q, p.Q[i]), append(out.R, p.R[i])
+		out.Common, out.Denom, out.Distance = append(out.Common, p.Common[i]), append(out.Denom, p.Denom[i]), append(out.Distance, p.Distance[i])
+		if p.PValue != nil {
+			out.PValue = append(out.PValue, p.PValue[i])
+		}
+	}
+	return out, nil
 }
 
 // Sketcher grows SketchGroups in place: nGroups sketches fed batch by batch, for read sets larger than the GPU or a

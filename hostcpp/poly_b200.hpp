@@ -206,6 +206,88 @@ private:
     uint64_t n_;
 };
 
+// Mash distance between grouped sketches (`mash dist`): queries and refs as SketchGroups / Sketcher::Sketches return
+// them, with their counts; one SketchSize for all.  Outputs are nq x nr, row-major, query = row: common and denom from
+// Mash's compareSketches (denom = min(s, |A u B|), common = shared values among the denom smallest of A u B), distance =
+// -ln(2J / (1 + J)) / k, and p = Mash's p-value from the genome lengths (bases per sketch, >= 1).  Without lengths
+// (both empty) pValue stays empty.
+struct DistResult {
+    std::vector<uint32_t> common, denom;
+    std::vector<double> distance, pValue;
+};
+// the pairs with distance <= maxDistance and p <= maxPValue (upper: r > q only, for a set against itself), sorted by (q, r)
+struct DistPairs {
+    std::vector<uint32_t> q, r, common, denom;
+    std::vector<double> distance, pValue;
+};
+namespace detail {
+inline int dist_slab(const std::vector<Mash> &set, const std::vector<uint32_t> &count, int s, std::vector<uint32_t> &rows) {
+    if (count.size() != set.size()) throw std::invalid_argument("one count per sketch");
+    rows.assign(set.size() * (size_t)std::max(s, 1), 0);
+    for (size_t i = 0; i < set.size(); ++i) {
+        if (set[i].SketchSize != s || (int)set[i].Sketches.size() < s) throw std::invalid_argument("sketches of one SketchSize");
+        std::copy(set[i].Sketches.begin(), set[i].Sketches.begin() + s, rows.begin() + i * (size_t)s);
+    }
+    return s;
+}
+inline int dist_size(const std::vector<Mash> &q, const std::vector<Mash> &r) {
+    return !q.empty() ? q[0].SketchSize : !r.empty() ? r[0].SketchSize : 1;
+}
+inline void dist_lengths(const std::vector<uint64_t> &qLen, const std::vector<uint64_t> &rLen, size_t nq, size_t nr) {
+    if (qLen.empty() != rLen.empty()) throw std::invalid_argument("pass both length vectors, or neither");
+    if (!qLen.empty() && (qLen.size() != nq || rLen.size() != nr)) throw std::invalid_argument("one length per sketch");
+}
+}  // namespace detail
+
+inline DistResult Dist(const std::vector<Mash> &queries, const std::vector<uint32_t> &qCount, const std::vector<Mash> &refs,
+                       const std::vector<uint32_t> &rCount, int k, const std::vector<uint64_t> &qLen = {}, const std::vector<uint64_t> &rLen = {}) {
+    const int s = detail::dist_size(queries, refs);
+    std::vector<uint32_t> q, r;
+    detail::dist_slab(queries, qCount, s, q);
+    detail::dist_slab(refs, rCount, s, r);
+    detail::dist_lengths(qLen, rLen, queries.size(), refs.size());
+    const size_t n = queries.size() * refs.size();
+    DistResult out{std::vector<uint32_t>(n), std::vector<uint32_t>(n), std::vector<double>(n), std::vector<double>(qLen.empty() ? 0 : n)};
+    check(pg_mash_dist(q.data(), qCount.data(), queries.size(), r.data(), rCount.data(), refs.size(), (uint64_t)s, s, k,
+                       qLen.empty() ? nullptr : qLen.data(), rLen.empty() ? nullptr : rLen.data(), out.common.data(), out.denom.data(),
+                       out.distance.data(), qLen.empty() ? nullptr : out.pValue.data()));
+    return out;
+}
+
+inline DistPairs DistWithin(const std::vector<Mash> &queries, const std::vector<uint32_t> &qCount, const std::vector<Mash> &refs,
+                            const std::vector<uint32_t> &rCount, int k, const std::vector<uint64_t> &qLen = {}, const std::vector<uint64_t> &rLen = {},
+                            double maxDistance = 1.0, double maxPValue = 1.0, bool upper = false) {
+    const int s = detail::dist_size(queries, refs);
+    std::vector<uint32_t> q, r;
+    detail::dist_slab(queries, qCount, s, q);
+    detail::dist_slab(refs, rCount, s, r);
+    detail::dist_lengths(qLen, rLen, queries.size(), refs.size());
+    const bool p = !qLen.empty();
+    uint64_t cap = std::max<uint64_t>(1024, 4 * queries.size()), n = 0;
+    DistPairs out;
+    for (;;) {
+        out = DistPairs{std::vector<uint32_t>(cap), std::vector<uint32_t>(cap), std::vector<uint32_t>(cap), std::vector<uint32_t>(cap),
+                        std::vector<double>(cap), std::vector<double>(p ? cap : 0)};
+        const int rc = pg_mash_dist_within(q.data(), qCount.data(), queries.size(), r.data(), rCount.data(), refs.size(), (uint64_t)s, s, k,
+                                           p ? qLen.data() : nullptr, p ? rLen.data() : nullptr, maxDistance, maxPValue, upper ? PG_PAIRS_UPPER : 0u,
+                                           out.q.data(), out.r.data(), out.common.data(), out.denom.data(), out.distance.data(),
+                                           p ? out.pValue.data() : nullptr, cap, &n);
+        if (rc == PG_ERR_ARG && n > cap) { cap = n; continue; }
+        check(rc);
+        break;
+    }
+    std::vector<size_t> order(n);
+    for (size_t i = 0; i < n; ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return out.q[a] != out.q[b] ? out.q[a] < out.q[b] : out.r[a] < out.r[b]; });
+    DistPairs sorted;
+    for (size_t i : order) {
+        sorted.q.push_back(out.q[i]); sorted.r.push_back(out.r[i]); sorted.common.push_back(out.common[i]); sorted.denom.push_back(out.denom[i]);
+        sorted.distance.push_back(out.distance[i]);
+        if (p) sorted.pValue.push_back(out.pValue[i]);
+    }
+    return sorted;
+}
+
 // In-place form: `slab` holds the Sketches arrays of seqs.size() Mash values back to back (n x s words).  Row i
 // receives its min(len_i - k, s) words, the rest of the row is left as it is -- what (*Mash).Sketch does to an
 // existing Mash (mash.go:73-80); a zeroed slab ends up as n fresh sketches.  Returns the per-read counts.

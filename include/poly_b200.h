@@ -294,6 +294,65 @@ int pg_mash_sketcher_rows_dev(const pg_mash_sketcher *sk, uint64_t first, uint64
                               uint32_t *d_n_values, uint8_t *d_complete, uint64_t *d_held, void *stream);
 int pg_mash_sketcher_free(pg_mash_sketcher *sk);
 
+/* ---- Mash distance between grouped sketches (`mash dist`, `mash dist -d D -v P`, `mash triangle`) ----
+ * Inputs are rows as pg_mash_sketch_groups and pg_mash_sketcher_rows write them: rows is n x row_stride uint32 and row
+ * i holds count[i] <= s strictly ascending values (unsigned order) in its first words; one s and one k for the call.
+ * For query row A (a values) and reference row B (b values), Mash's compareSketches loop:
+ *     i = j = common = denom = 0
+ *     while denom < s and i < a and j < b:
+ *         if A[i] < B[j]: i++   elif B[j] < A[i]: j++   else: i++; j++; common++
+ *         denom++
+ *     if denom < s: denom += min(a - i, s - denom); denom += min(b - j, s - denom)
+ * That is, denom = min(s, |A u B|) and common = the shared values among the denom smallest values of A u B.
+ *   - distance: +0.0 if common == denom (two empty rows included); 1.0 if common == 0; else -log(2J / (1 + J)) / k with
+ *     J = (double)common / denom, clamped to 1.0 when larger.  Mash's estimate of the per-base mutation rate (1 - ANI).
+ *   - p-value (Mash's pValue): 1.0 if common == 0.  Else pQ = 1 / (1 + 4^k / len_q), pR likewise with len_r, 4^k being the
+ *     double ldexp(1, 2k); r = pQ pR / (pQ + pR - pQ pR), taken as 0 when that denominator is 0; p = P[Binomial(denom, r)
+ *     >= common] (GSL's gsl_cdf_binomial_Q(common - 1, r, denom)), 0 when r == 0.  Computed on the device in double from
+ *     the incomplete beta function (log-gamma prefactor, continued fraction); values below about 1e-300 may come out as 0.
+ *     len is the number of bases Mash records for a sketch (an assembly: the sum of its record lengths), >= 1.
+ *   - Properties: swapping the query and reference sets together with their lengths transposes all four outputs bit
+ *     for bit (every formula is symmetric); a row against itself gives common = denom = count and distance 0.  The call
+ *     cannot tell an incomplete sketcher row (complete[g] == 0) from a small group: passing complete rows is the
+ *     caller's job, as k and the canonical mode are.
+ *   - Unlike (*Mash).Distance (pg_mash_distance_block), a row with fewer than s values compares as the set it is: the
+ *     reference's range early-out makes such a row, whose tail is zeros, distance 1 from everything, itself included.
+ * pg_mash_dist (dense, `mash dist`): common, denom, distance and p_value are nq x nr, row-major, query = row; any may be
+ * NULL.  A row block is a slice of the queries.
+ * pg_mash_dist_within (filtered, `mash dist -d -v`, `mash triangle`): the pairs (pair_q[t], pair_r[t]) with distance <=
+ * max_distance and p <= max_p_value, in no particular order, with their common, denom, distance and p_value (each may
+ * be NULL).  PG_PAIRS_UPPER keeps only r > q (a set against itself: needs nq == nr).  *n_pairs receives the number of
+ * qualifying pairs; if it exceeds pairs_cap the first pairs_cap are stored and the call returns PG_ERR_ARG (as
+ * pg_mash_distance_sparse).  The _dev form takes a DEVICE counter d_n_pairs (set on the stream, may exceed pairs_cap)
+ * and does not block.
+ *   - Lengths may be NULL only when p_value is NULL and, in the filtered form, max_p_value >= 1 (no p-value is computed).
+ *   - Errors, checked in this order before any device work, all PG_ERR_ARG: nq or nr > 2^32 - 1; k < 1; s < 1;
+ *     row_stride < s; a null rows or count on a non-empty side; null lengths on a non-empty side when a p-value is
+ *     needed; in the filtered form a NaN limit, a flag bit other than PG_PAIRS_UPPER, PG_PAIRS_UPPER with nq != nr, a
+ *     null pair_q, pair_r or n_pairs; in the host forms only, a count > s, a row that is not strictly ascending, or a
+ *     length of 0 where lengths are read.  The _dev forms trust their rows (as _dev calls trust offsets) and read only the
+ *     first count words of each.  nq == 0 or nr == 0 is valid.
+ *   - Device: one warp merges a pair, over at most 2 s items of the merge.  Rows of s <= 3418 are staged in shared
+ *     memory; larger s reads them from global memory.  Both forms only enqueue (_dev) or wait for their own stream.
+ *   - Device memory: the _dev forms allocate nothing.  pg_mash_dist stages the references (4 nr (row_stride + 1) bytes,
+ *     + 8 nr with lengths) and cuts the queries into blocks whose outputs (4 or 8 bytes per requested output per pair)
+ *     stay under 1 GiB, with each block's query rows.  pg_mash_dist_within stages both sets and pairs_cap entries of
+ *     every requested list (8 bytes of pair ids, 4 + 4 + 8 + 8 for the others). */
+int pg_mash_dist(const uint32_t *q_rows, const uint32_t *q_count, uint64_t nq, const uint32_t *r_rows, const uint32_t *r_count, uint64_t nr,
+                 uint64_t row_stride, int32_t s, int32_t k, const uint64_t *q_length, const uint64_t *r_length, uint32_t *common, uint32_t *denom,
+                 double *distance, double *p_value);
+int pg_mash_dist_dev(const uint32_t *d_q_rows, const uint32_t *d_q_count, uint64_t nq, const uint32_t *d_r_rows, const uint32_t *d_r_count, uint64_t nr,
+                     uint64_t row_stride, int32_t s, int32_t k, const uint64_t *d_q_length, const uint64_t *d_r_length, uint32_t *d_common,
+                     uint32_t *d_denom, double *d_distance, double *d_p_value, void *stream);
+int pg_mash_dist_within(const uint32_t *q_rows, const uint32_t *q_count, uint64_t nq, const uint32_t *r_rows, const uint32_t *r_count, uint64_t nr,
+                        uint64_t row_stride, int32_t s, int32_t k, const uint64_t *q_length, const uint64_t *r_length, double max_distance,
+                        double max_p_value, uint32_t flags, uint32_t *pair_q, uint32_t *pair_r, uint32_t *common, uint32_t *denom, double *distance,
+                        double *p_value, uint64_t pairs_cap, uint64_t *n_pairs);
+int pg_mash_dist_within_dev(const uint32_t *d_q_rows, const uint32_t *d_q_count, uint64_t nq, const uint32_t *d_r_rows, const uint32_t *d_r_count,
+                            uint64_t nr, uint64_t row_stride, int32_t s, int32_t k, const uint64_t *d_q_length, const uint64_t *d_r_length,
+                            double max_distance, double max_p_value, uint32_t flags, uint32_t *d_pair_q, uint32_t *d_pair_r, uint32_t *d_common,
+                            uint32_t *d_denom, double *d_distance, double *d_p_value, uint64_t pairs_cap, uint64_t *d_n_pairs, void *stream);
+
 /* ---- single-process multi-GPU (SURVEY.md 8b "multi-GPU variants taking a device count", 8e) ----
  * What a Go host calls to reach all GPUs of the box with ONE call: reads are independent
  * (mash.go:68-104 touches only its receiver), so the batch is cut into contiguous shards, one per

@@ -17,6 +17,7 @@ PG_ITEM_OK, PG_ITEM_PANIC, PG_ITEM_UNSUPPORTED = 0, 1, 2
 PG_SKETCH_PAD_ZERO = 1
 PG_SKETCH_TAIL_KEEP = 2
 PG_KMER_CANONICAL = 1
+PG_PAIRS_UPPER = 1
 
 
 class PolyError(RuntimeError):
@@ -67,6 +68,16 @@ _SIGS = {
     "pg_mash_sketcher_rows": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, _u32p, C.c_uint64, _u32p, _u8p, _u64p]),
     "pg_mash_sketcher_rows_dev": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, _u32p, C.c_uint64, _u32p, _u8p, _u64p, C.c_void_p]),
     "pg_mash_sketcher_free": (C.c_int, [C.c_void_p]),
+    "pg_mash_dist": (C.c_int, [_u32p, _u32p, C.c_uint64, _u32p, _u32p, C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, _u64p, _u64p, _u32p, _u32p,
+                               _f64p, _f64p]),
+    "pg_mash_dist_dev": (C.c_int, [_u32p, _u32p, C.c_uint64, _u32p, _u32p, C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, _u64p, _u64p, _u32p,
+                                   _u32p, _f64p, _f64p, C.c_void_p]),
+    "pg_mash_dist_within": (C.c_int, [_u32p, _u32p, C.c_uint64, _u32p, _u32p, C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, _u64p, _u64p,
+                                      C.c_double, C.c_double, C.c_uint32, _u32p, _u32p, _u32p, _u32p, _f64p, _f64p, C.c_uint64,
+                                      C.POINTER(C.c_uint64)]),
+    "pg_mash_dist_within_dev": (C.c_int, [_u32p, _u32p, C.c_uint64, _u32p, _u32p, C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, _u64p, _u64p,
+                                          C.c_double, C.c_double, C.c_uint32, _u32p, _u32p, _u32p, _u32p, _f64p, _f64p, C.c_uint64,
+                                          _u64p, C.c_void_p]),
     "pg_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p]),
     "pg_ipc_import": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "pg_ipc_close": (C.c_int, [C.c_void_p]),

@@ -3,6 +3,7 @@
 // sketch set, the sketch index and the screen.
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstring>
 #include <functional>
 #include <sched.h>
@@ -801,6 +802,66 @@ static int sketcher_rows_check(const pg_mash_sketcher *sk, uint64_t first, uint6
     if (count && (!out || !n_values)) { set_error("null out or n_values"); return PG_ERR_ARG; }
     return PG_OK;
 }
+
+// The argument rules of pg_mash_dist(_within) and their _dev forms that need no buffer content, in their order.
+// need_len: a p-value is computed.
+static int dist_check(uint64_t nq, uint64_t nr, int32_t s, int32_t k, uint64_t row_stride, const void *q_rows, const void *q_count, const void *r_rows,
+                      const void *r_count, bool need_len, const void *q_length, const void *r_length) {
+    if (nq > 0xffffffffull || nr > 0xffffffffull) {
+        set_error("%llu queries x %llu references: each side holds at most 2^32 - 1 rows", (unsigned long long)nq, (unsigned long long)nr);
+        return PG_ERR_ARG;
+    }
+    if (k < 1) { set_error("kmerSize %d < 1", k); return PG_ERR_ARG; }
+    if (s < 1) { set_error("sketchSize %d < 1", s); return PG_ERR_ARG; }
+    if (row_stride < (uint64_t)s) { set_error("row_stride %llu < sketchSize %d", (unsigned long long)row_stride, s); return PG_ERR_ARG; }
+    if ((nq && (!q_rows || !q_count)) || (nr && (!r_rows || !r_count))) { set_error("null rows or count"); return PG_ERR_ARG; }
+    if (need_len && ((nq && !q_length) || (nr && !r_length))) { set_error("null lengths: the p-value needs them"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+// the rules of the filtered form that follow dist_check, in their order
+static int dist_within_check(uint64_t nq, uint64_t nr, double max_distance, double max_p_value, uint32_t flags, const void *pair_q, const void *pair_r,
+                             const void *n_pairs) {
+    if (std::isnan(max_distance) || std::isnan(max_p_value)) { set_error("NaN limit"); return PG_ERR_ARG; }
+    if (flags & ~PG_PAIRS_UPPER) { set_error("unknown flag bits 0x%x", flags & ~PG_PAIRS_UPPER); return PG_ERR_ARG; }
+    if ((flags & PG_PAIRS_UPPER) && nq != nr) {
+        set_error("PG_PAIRS_UPPER needs one set: %llu queries, %llu references", (unsigned long long)nq, (unsigned long long)nr);
+        return PG_ERR_ARG;
+    }
+    if (!pair_q || !pair_r || !n_pairs) { set_error("null pair_q, pair_r or n_pairs"); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+// The host forms' checks of the rows themselves: counts <= s, strictly ascending rows, lengths >= 1
+static int dist_rows_check(const uint32_t *rows, const uint32_t *count, uint64_t n, int32_t s, uint64_t row_stride, const uint64_t *len, const char *side) {
+    for (uint64_t i = 0; i < n; ++i) {
+        if (count[i] > (uint32_t)s) {
+            set_error("%s row %llu holds %u values > sketchSize %d", side, (unsigned long long)i, count[i], s);
+            return PG_ERR_ARG;
+        }
+        const uint32_t *row = rows + i * row_stride;
+        for (uint32_t w = 1; w < count[i]; ++w)
+            if (row[w] <= row[w - 1]) {
+                set_error("%s row %llu is not strictly ascending at word %u", side, (unsigned long long)i, w);
+                return PG_ERR_ARG;
+            }
+    }
+    if (len)
+        for (uint64_t i = 0; i < n; ++i)
+            if (len[i] == 0) { set_error("%s length %llu is 0", side, (unsigned long long)i); return PG_ERR_ARG; }
+    return PG_OK;
+}
+
+static DistArgs dist_args(const uint32_t *q_rows, const uint32_t *q_count, uint64_t nq, const uint32_t *r_rows, const uint32_t *r_count, uint64_t nr,
+                          uint64_t row_stride, int32_t s, int32_t k, const uint64_t *q_len, const uint64_t *r_len) {
+    DistArgs g{};
+    g.q_rows = q_rows; g.q_count = q_count; g.r_rows = r_rows; g.r_count = r_count;
+    g.nq = nq; g.nr = nr; g.stride = row_stride; g.s = s; g.k = k; g.q_len = q_len; g.r_len = r_len;
+    return g;
+}
+
+// device bytes of the dense host form's outputs per block; the queries are cut into blocks that fit
+constexpr uint64_t DIST_BLOCK_BYTES = 1ull << 30;
 
 }  // namespace
 }  // namespace pg
@@ -1751,6 +1812,105 @@ int pg_mash_screen_free(pg_mash_screen *sc) {
     delete sc;
     PG_CUDA(cudaStreamSynchronize(st));
     return PG_OK;
+}
+
+// ---------------------------------------------------------------------------------
+// Mash distance between grouped sketches
+// ---------------------------------------------------------------------------------
+int pg_mash_dist_dev(const uint32_t *d_q_rows, const uint32_t *d_q_count, uint64_t nq, const uint32_t *d_r_rows, const uint32_t *d_r_count, uint64_t nr,
+                     uint64_t row_stride, int32_t s, int32_t k, const uint64_t *d_q_length, const uint64_t *d_r_length, uint32_t *d_common,
+                     uint32_t *d_denom, double *d_distance, double *d_p_value, void *stream) {
+    int rc = dist_check(nq, nr, s, k, row_stride, d_q_rows, d_q_count, d_r_rows, d_r_count, d_p_value != nullptr, d_q_length, d_r_length);
+    if (rc != PG_OK || nq == 0 || nr == 0 || !(d_common || d_denom || d_distance || d_p_value)) return rc;
+    if ((rc = ensure_device()) != PG_OK) return rc;
+    DistArgs g = dist_args(d_q_rows, d_q_count, nq, d_r_rows, d_r_count, nr, row_stride, s, k, d_q_length, d_r_length);
+    g.common = d_common; g.denom = d_denom; g.distance = d_distance; g.p_value = d_p_value;
+    return launch_mash_dist(g, false, (cudaStream_t)stream);
+}
+
+int pg_mash_dist(const uint32_t *q_rows, const uint32_t *q_count, uint64_t nq, const uint32_t *r_rows, const uint32_t *r_count, uint64_t nr,
+                 uint64_t row_stride, int32_t s, int32_t k, const uint64_t *q_length, const uint64_t *r_length, uint32_t *common, uint32_t *denom,
+                 double *distance, double *p_value) {
+    const bool need_len = p_value != nullptr;
+    int rc = dist_check(nq, nr, s, k, row_stride, q_rows, q_count, r_rows, r_count, need_len, q_length, r_length);
+    if (rc != PG_OK || (rc = dist_rows_check(q_rows, q_count, nq, s, row_stride, need_len ? q_length : nullptr, "query")) != PG_OK ||
+        (rc = dist_rows_check(r_rows, r_count, nr, s, row_stride, need_len ? r_length : nullptr, "reference")) != PG_OK)
+        return rc;
+    const uint64_t per_pair = (common ? 4 : 0) + (denom ? 4 : 0) + (distance ? 8 : 0) + (p_value ? 8 : 0);
+    if (nq == 0 || nr == 0 || per_pair == 0) return PG_OK;
+    if ((rc = ensure_device()) != PG_OK) return rc;
+    const uint64_t rows_per = std::max<uint64_t>(1, std::min<uint64_t>(nq, DIST_BLOCK_BYTES / (nr * per_pair)));
+    HostCall c;
+    const uint32_t *d_r = c.upload(r_rows, nr * row_stride), *d_rc = c.upload(r_count, nr);
+    const uint64_t *d_rl = need_len ? c.upload(r_length, nr) : nullptr;
+    uint32_t *d_q = c.alloc<uint32_t>(rows_per * row_stride), *d_qc = c.alloc<uint32_t>(rows_per);
+    uint64_t *d_ql = need_len ? c.alloc<uint64_t>(rows_per) : nullptr;
+    uint32_t *d_common = common ? c.alloc<uint32_t>(rows_per * nr) : nullptr, *d_denom = denom ? c.alloc<uint32_t>(rows_per * nr) : nullptr;
+    double *d_dist = distance ? c.alloc<double>(rows_per * nr) : nullptr, *d_p = p_value ? c.alloc<double>(rows_per * nr) : nullptr;
+    if ((rc = c.error()) != PG_OK) return rc;
+    for (uint64_t b = 0; b < nq; b += rows_per) {
+        const uint64_t m = std::min(rows_per, nq - b);
+        c.put(d_q, q_rows + b * row_stride, m * row_stride);
+        c.put(d_qc, q_count + b, m);
+        if (need_len) c.put(d_ql, q_length + b, m);
+        DistArgs g = dist_args(d_q, d_qc, m, d_r, d_rc, nr, row_stride, s, k, d_ql, d_rl);
+        g.q0 = b; g.common = d_common; g.denom = d_denom; g.distance = d_dist; g.p_value = d_p;
+        if ((rc = c.error()) != PG_OK || (rc = launch_mash_dist(g, false, c.st)) != PG_OK) return rc;
+        if (common) c.download(common + b * nr, d_common, m * nr);
+        if (denom) c.download(denom + b * nr, d_denom, m * nr);
+        if (distance) c.download(distance + b * nr, d_dist, m * nr);
+        if (p_value) c.download(p_value + b * nr, d_p, m * nr);
+    }
+    return c.finish();
+}
+
+int pg_mash_dist_within_dev(const uint32_t *d_q_rows, const uint32_t *d_q_count, uint64_t nq, const uint32_t *d_r_rows, const uint32_t *d_r_count,
+                            uint64_t nr, uint64_t row_stride, int32_t s, int32_t k, const uint64_t *d_q_length, const uint64_t *d_r_length,
+                            double max_distance, double max_p_value, uint32_t flags, uint32_t *d_pair_q, uint32_t *d_pair_r, uint32_t *d_common,
+                            uint32_t *d_denom, double *d_distance, double *d_p_value, uint64_t pairs_cap, uint64_t *d_n_pairs, void *stream) {
+    const bool need_len = d_p_value != nullptr || max_p_value < 1.0;
+    int rc = dist_check(nq, nr, s, k, row_stride, d_q_rows, d_q_count, d_r_rows, d_r_count, need_len, d_q_length, d_r_length);
+    if (rc != PG_OK || (rc = dist_within_check(nq, nr, max_distance, max_p_value, flags, d_pair_q, d_pair_r, d_n_pairs)) != PG_OK ||
+        (rc = ensure_device()) != PG_OK)
+        return rc;
+    PG_CUDA(cudaMemsetAsync(d_n_pairs, 0, sizeof(uint64_t), (cudaStream_t)stream));
+    DistArgs g = dist_args(d_q_rows, d_q_count, nq, d_r_rows, d_r_count, nr, row_stride, s, k, d_q_length, d_r_length);
+    g.max_distance = max_distance; g.max_p_value = max_p_value; g.upper = (flags & PG_PAIRS_UPPER) != 0;
+    g.pair_q = d_pair_q; g.pair_r = d_pair_r; g.common = d_common; g.denom = d_denom; g.distance = d_distance; g.p_value = d_p_value;
+    g.cap = pairs_cap; g.n_pairs = (unsigned long long *)d_n_pairs;
+    return launch_mash_dist(g, true, (cudaStream_t)stream);
+}
+
+int pg_mash_dist_within(const uint32_t *q_rows, const uint32_t *q_count, uint64_t nq, const uint32_t *r_rows, const uint32_t *r_count, uint64_t nr,
+                        uint64_t row_stride, int32_t s, int32_t k, const uint64_t *q_length, const uint64_t *r_length, double max_distance,
+                        double max_p_value, uint32_t flags, uint32_t *pair_q, uint32_t *pair_r, uint32_t *common, uint32_t *denom, double *distance,
+                        double *p_value, uint64_t pairs_cap, uint64_t *n_pairs) {
+    const bool need_len = p_value != nullptr || max_p_value < 1.0;
+    int rc = dist_check(nq, nr, s, k, row_stride, q_rows, q_count, r_rows, r_count, need_len, q_length, r_length);
+    if (rc != PG_OK || (rc = dist_within_check(nq, nr, max_distance, max_p_value, flags, pair_q, pair_r, n_pairs)) != PG_OK ||
+        (rc = dist_rows_check(q_rows, q_count, nq, s, row_stride, need_len ? q_length : nullptr, "query")) != PG_OK ||
+        (rc = dist_rows_check(r_rows, r_count, nr, s, row_stride, need_len ? r_length : nullptr, "reference")) != PG_OK)
+        return rc;
+    *n_pairs = 0;
+    if (nq == 0 || nr == 0) return PG_OK;
+    if ((rc = ensure_device()) != PG_OK) return rc;
+    HostCall c;
+    const uint32_t *d_q = c.upload(q_rows, nq * row_stride), *d_qc = c.upload(q_count, nq);
+    const uint32_t *d_r = c.upload(r_rows, nr * row_stride), *d_rc = c.upload(r_count, nr);
+    const uint64_t *d_ql = need_len ? c.upload(q_length, nq) : nullptr, *d_rl = need_len ? c.upload(r_length, nr) : nullptr;
+    uint32_t *d_pq = c.alloc<uint32_t>(pairs_cap), *d_pr = c.alloc<uint32_t>(pairs_cap);
+    uint32_t *d_c = common ? c.alloc<uint32_t>(pairs_cap) : nullptr, *d_d = denom ? c.alloc<uint32_t>(pairs_cap) : nullptr;
+    double *d_dist = distance ? c.alloc<double>(pairs_cap) : nullptr, *d_p = p_value ? c.alloc<double>(pairs_cap) : nullptr;
+    unsigned long long *d_n = c.alloc<unsigned long long>(1, true);
+    if ((rc = c.error()) != PG_OK) return rc;
+    DistArgs g = dist_args(d_q, d_qc, nq, d_r, d_rc, nr, row_stride, s, k, d_ql, d_rl);
+    g.max_distance = max_distance; g.max_p_value = max_p_value; g.upper = (flags & PG_PAIRS_UPPER) != 0;
+    g.pair_q = d_pq; g.pair_r = d_pr; g.common = d_c; g.denom = d_d; g.distance = d_dist; g.p_value = d_p;
+    g.cap = pairs_cap; g.n_pairs = d_n;
+    if ((rc = launch_mash_dist(g, true, c.st)) != PG_OK) return rc;
+    return finish_capped(c, d_n, pairs_cap, n_pairs,
+                         {{pair_q, d_pq, 4}, {pair_r, d_pr, 4}, {common, d_c, 4}, {denom, d_d, 4}, {distance, d_dist, 8}, {p_value, d_p, 8}},
+                         "pairs_cap", "pairs");
 }
 
 }  // extern "C"

@@ -366,6 +366,26 @@ int sketcher_add(SketcherState &S, const uint8_t *d_bases, const uint64_t *d_off
 int sketcher_rows(const SketcherState &S, uint64_t first, uint64_t count, uint32_t *d_out, uint64_t row_stride, uint32_t *d_n, uint8_t *d_complete,
                   uint64_t *d_held, cudaStream_t st);
 void sketcher_free(SketcherState &S, cudaStream_t st);
+// mash_dist.cu: Mash distance of a block of queries against references (pg_mash_dist / pg_mash_dist_within).  Query q of
+// the block is global query q0 + q; rows are row-major at `stride` words, count[i] values each (<= s, ascending).
+// q_len / r_len are read only when a p-value is needed.  Dense: outputs at q * nr + r (each may be null).  List: the
+// pairs with distance <= max_distance and p <= max_p_value (r > q0 + q with upper) go to slots of an atomic counter, the
+// first cap of them stored.
+struct DistArgs {
+    const uint32_t *q_rows, *q_count, *r_rows, *r_count;
+    uint64_t nq, nr, stride, q0;
+    int s, k;
+    const uint64_t *q_len, *r_len;
+    uint32_t *common, *denom;
+    double *distance, *p_value;
+    double max_distance, max_p_value;
+    bool upper;
+    uint32_t *pair_q, *pair_r;
+    uint64_t cap;
+    unsigned long long *n_pairs;
+};
+// only enqueues
+int launch_mash_dist(const DistArgs &g, bool list, cudaStream_t st);
 // Alignment launchers: the scoring (byte LUTs, table, gap, local / global) is an AlignScoring of host
 // pointers (align_core.cuh).
 struct AlignScoring;

@@ -370,6 +370,125 @@ class Sketcher:
                 pass
 
 
+def _dist_inputs(q_rows, q_count, r_rows, r_count, k: int, q_length, r_length):
+    """Shared checks of dist / dist_within: one s (the rows' width) for both sides, k and lengths given together."""
+    k = int(k)
+    if not 1 <= k < (1 << 31):
+        raise PolyError(_lib.PG_ERR_ARG, f"k-mer size {k}: need 1 <= k < 2^31")
+    if len(q_rows.shape) != 2 or len(r_rows.shape) != 2 or q_rows.shape[1] != r_rows.shape[1]:
+        raise ValueError("q_rows and r_rows must be 2-d with one common width s")
+    if tuple(q_count.shape) != (q_rows.shape[0],) or tuple(r_count.shape) != (r_rows.shape[0],):
+        raise ValueError("count arrays must hold one entry per row")
+    if (q_length is None) != (r_length is None):
+        raise ValueError("pass both q_length and r_length, or neither")
+    if q_length is not None and (tuple(q_length.shape) != (q_rows.shape[0],) or tuple(r_length.shape) != (r_rows.shape[0],)):
+        raise ValueError("length arrays must hold one entry per row")
+    s = int(q_rows.shape[1])
+    if not 1 <= s < (1 << 31):
+        raise PolyError(_lib.PG_ERR_ARG, f"sketch size {s}: need 1 <= s < 2^31")
+    return k, s
+
+
+def _torch_dist_inputs(q_rows, q_count, r_rows, r_count, q_length, r_length):
+    for name, t, size in (("q_rows", q_rows, 4), ("q_count", q_count, 4), ("r_rows", r_rows, 4), ("r_count", r_count, 4),
+                          ("q_length", q_length, 8), ("r_length", r_length, 8)):
+        if t is not None and (not t.is_cuda or t.element_size() != size or not t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous CUDA tensor of {size}-byte elements")
+
+
+def dist(q_rows, q_count, r_rows, r_count, k: int, q_length=None, r_length=None):
+    """Mash distance of every query row against every reference row (`mash dist`): rows and counts as sketch_groups or
+    Sketcher.rows return them, one sketch size s (the rows' width) for both sides.  For a pair, denom = min(s, |A u B|)
+    and common = the shared values among the denom smallest values of A u B (Mash's compareSketches); distance =
+    -ln(2J / (1 + J)) / k with J = common / denom (0 when common == denom, 1 when common == 0, at most 1); p_value =
+    Mash's p-value, P[Binomial(denom, r) >= common] with r from k and the two genome lengths (bases per sketch, >= 1).
+    Returns (common, denom, distance, p_value), each [nq, nr] with the query as the row; p_value is None without
+    lengths.  NumPy inputs (uint32 rows and counts, uint64 lengths) give NumPy outputs; CUDA tensors (int32 holding the
+    uint32 bits, int64 lengths) give CUDA tensors (common and denom int32 holding uint32 bits), computed by the _dev
+    form on the current stream without waiting for it."""
+    k, s = _dist_inputs(q_rows, q_count, r_rows, r_count, k, q_length, r_length)
+    nq, nr = int(q_rows.shape[0]), int(r_rows.shape[0])
+    want_p = q_length is not None
+    if hasattr(q_rows, "data_ptr"):
+        import torch
+
+        _torch_dist_inputs(q_rows, q_count, r_rows, r_count, q_length, r_length)
+        dev = q_rows.device
+        common = torch.empty((nq, nr), dtype=torch.int32, device=dev)
+        denom = torch.empty((nq, nr), dtype=torch.int32, device=dev)
+        distance = torch.empty((nq, nr), dtype=torch.float64, device=dev)
+        p = torch.empty((nq, nr), dtype=torch.float64, device=dev) if want_p else None
+        st = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(_lib.lib().pg_mash_dist_dev(_lib.ptr(q_rows), _lib.ptr(q_count), nq, _lib.ptr(r_rows), _lib.ptr(r_count), nr, s, s, k,
+                                               _lib.ptr(q_length), _lib.ptr(r_length), _lib.ptr(common), _lib.ptr(denom), _lib.ptr(distance),
+                                               _lib.ptr(p), st))
+        return common, denom, distance, p
+    q_rows, r_rows = np.ascontiguousarray(q_rows, np.uint32), np.ascontiguousarray(r_rows, np.uint32)
+    q_count, r_count = np.ascontiguousarray(q_count, np.uint32), np.ascontiguousarray(r_count, np.uint32)
+    if want_p:
+        q_length, r_length = np.ascontiguousarray(q_length, np.uint64), np.ascontiguousarray(r_length, np.uint64)
+    common, denom = np.zeros((nq, nr), np.uint32), np.zeros((nq, nr), np.uint32)
+    distance = np.zeros((nq, nr), np.float64)
+    p = np.zeros((nq, nr), np.float64) if want_p else None
+    _lib.check(_lib.lib().pg_mash_dist(_lib.ptr(q_rows), _lib.ptr(q_count), nq, _lib.ptr(r_rows), _lib.ptr(r_count), nr, s, s, k, _lib.ptr(q_length),
+                                       _lib.ptr(r_length), _lib.ptr(common), _lib.ptr(denom), _lib.ptr(distance), _lib.ptr(p)))
+    return common, denom, distance, p
+
+
+def dist_within(q_rows, q_count, r_rows, r_count, k: int, q_length=None, r_length=None, max_distance: float = 1.0, max_p_value: float = 1.0,
+                upper: bool = False):
+    """The pairs of dist with distance <= max_distance and p-value <= max_p_value (`mash dist -d D -v P`); upper=True
+    keeps only r > q, for a set against itself (`mash triangle`; needs nq == nr).  max_p_value < 1 needs the lengths.
+    Returns (pair_q, pair_r, common, denom, distance, p_value) sorted by (q, r); p_value is None without lengths.  NumPy
+    inputs give NumPy outputs; CUDA tensors go through the _dev form on the current stream, and the call waits for it to
+    read the pair count."""
+    k, s = _dist_inputs(q_rows, q_count, r_rows, r_count, k, q_length, r_length)
+    nq, nr = int(q_rows.shape[0]), int(r_rows.shape[0])
+    want_p = q_length is not None
+    flags = _lib.PG_PAIRS_UPPER if upper else 0
+    max_distance, max_p_value = float(max_distance), float(max_p_value)
+    cap = max(1024, 4 * nq)
+    if hasattr(q_rows, "data_ptr"):
+        import torch
+
+        _torch_dist_inputs(q_rows, q_count, r_rows, r_count, q_length, r_length)
+        dev = q_rows.device
+        st = torch.cuda.current_stream(dev).cuda_stream
+        d_n = torch.zeros(1, dtype=torch.int64, device=dev)
+        while True:
+            out = [torch.empty(cap, dtype=dt, device=dev) for dt in (torch.int32, torch.int32, torch.int32, torch.int32, torch.float64)]
+            p = torch.empty(cap, dtype=torch.float64, device=dev) if want_p else None
+            _lib.check(_lib.lib().pg_mash_dist_within_dev(_lib.ptr(q_rows), _lib.ptr(q_count), nq, _lib.ptr(r_rows), _lib.ptr(r_count), nr, s, s, k,
+                                                          _lib.ptr(q_length), _lib.ptr(r_length), max_distance, max_p_value, flags,
+                                                          *[_lib.ptr(t) for t in out], _lib.ptr(p), cap, _lib.ptr(d_n), st))
+            n = int(d_n.item())
+            if n <= cap:
+                break
+            cap = n
+        pq, pr, c, d, dist_ = (t[:n] for t in out)
+        order = torch.argsort(pq.to(torch.int64) * max(nr, 1) + pr.to(torch.int64))
+        return pq[order], pr[order], c[order], d[order], dist_[order], (p[:n][order] if want_p else None)
+    q_rows, r_rows = np.ascontiguousarray(q_rows, np.uint32), np.ascontiguousarray(r_rows, np.uint32)
+    q_count, r_count = np.ascontiguousarray(q_count, np.uint32), np.ascontiguousarray(r_count, np.uint32)
+    if want_p:
+        q_length, r_length = np.ascontiguousarray(q_length, np.uint64), np.ascontiguousarray(r_length, np.uint64)
+    while True:
+        pq, pr, c, d = (np.zeros(cap, np.uint32) for _ in range(4))
+        dist_ = np.zeros(cap, np.float64)
+        p = np.zeros(cap, np.float64) if want_p else None
+        cnt = C.c_uint64(0)
+        rc = _lib.lib().pg_mash_dist_within(_lib.ptr(q_rows), _lib.ptr(q_count), nq, _lib.ptr(r_rows), _lib.ptr(r_count), nr, s, s, k,
+                                            _lib.ptr(q_length), _lib.ptr(r_length), max_distance, max_p_value, flags, pq.ctypes.data, pr.ctypes.data,
+                                            c.ctypes.data, d.ctypes.data, dist_.ctypes.data, _lib.ptr(p), cap, C.byref(cnt))
+        if rc == _lib.PG_ERR_ARG and cnt.value > cap:
+            cap = int(cnt.value)
+            continue
+        _lib.check(rc)
+        n = int(cnt.value)
+        order = np.lexsort((pr[:n], pq[:n]))
+        return pq[:n][order], pr[:n][order], c[:n][order], d[:n][order], dist_[:n][order], (p[:n][order] if want_p else None)
+
+
 def similarity_pairs(mashes: Sequence[Mash], pairs: np.ndarray):
     """Explicit pair list (receiver, argument) over sketches of mixed sizes -> (same, similarity, distance)."""
     arrs = [np.ascontiguousarray(m.Sketches[: m.SketchSize], dtype=np.uint32) for m in mashes]
