@@ -309,7 +309,10 @@ int pg_mash_sketcher_free(pg_mash_sketcher *sk);
  *   - p-value (Mash's pValue): 1.0 if common == 0.  Else pQ = 1 / (1 + 4^k / len_q), pR likewise with len_r, 4^k being the
  *     double ldexp(1, 2k); r = pQ pR / (pQ + pR - pQ pR), taken as 0 when that denominator is 0; p = P[Binomial(denom, r)
  *     >= common] (GSL's gsl_cdf_binomial_Q(common - 1, r, denom)), 0 when r == 0.  Computed on the device in double from
- *     the incomplete beta function (log-gamma prefactor, continued fraction); values below about 1e-300 may come out as 0.
+ *     the incomplete beta function: its prefactor as a binomial density in Loader's saddle-point form (no log-gamma
+ *     differences), then the continued fraction.  Tested against an exact tail for denom up to 2^24: where the exact
+ *     p >= 1e-300 the relative error is at most tol(denom) = 4e-12 max(1, sqrt(denom / 10^4)), plus 4 eps |d ln p /
+ *     d ln r| for one ulp of r; below 1e-300 the value is in [0, 2e-300].  Never NaN or -0.0.
  *     len is the number of bases Mash records for a sketch (an assembly: the sum of its record lengths), >= 1.
  *   - Properties: swapping the query and reference sets together with their lengths transposes all four outputs bit
  *     for bit (every formula is symmetric); a row against itself gives common = denom = count and distance 0.  The call

@@ -131,7 +131,57 @@ __device__ double mash_distance(uint32_t common, uint32_t denom, int k) {
     return d > 1.0 ? 1.0 : d;
 }
 
-// P[Binomial(denom, r) >= common] = I_r(common, denom - common + 1), Mash's pValue
+// Stirling's remainder ln n! - (n + 1/2) ln n + n - ln sqrt(2 pi) of n = 1 .. 15, each the double nearest
+//   mpmath (dps 40): loggamma(n + 1) - (n + mpf(1) / 2) * log(n) + n - log(2 * pi) / 2
+__constant__ double STIRLERR_SMALL[15] = {
+    0.08106146679532726,  0.0413406959554093,    0.02767792568499834,  0.020790672103765093, 0.016644691189821193,
+    0.013876128823070748, 0.01189670994589177,   0.010411265261972096, 0.009255462182712733, 0.00833056343336287,
+    0.007573675487951841, 0.00694284010720953,   0.006408994188004207, 0.0059513701127588475, 0.005554733551962801};
+
+// Stirling's remainder of an integer n >= 1: the table, then the series 1/12n - 1/360n^3 + 1/1260n^5 - ... cut where
+// its next term is below 1e-16
+__device__ double stirlerr(double n) {
+    if (n <= 15.0) return STIRLERR_SMALL[(int)n - 1];
+    const double S0 = 1.0 / 12, S1 = 1.0 / 360, S2 = 1.0 / 1260, S3 = 1.0 / 1680, S4 = 1.0 / 1188;
+    const double nn = n * n;
+    if (n > 500.0) return (S0 - S1 / nn) / n;
+    if (n > 80.0) return (S0 - (S1 - S2 / nn) / nn) / n;
+    if (n > 35.0) return (S0 - (S1 - (S2 - S3 / nn) / nn) / nn) / n;
+    return (S0 - (S1 - (S2 - (S3 - S4 / nn) / nn) / nn) / nn) / n;
+}
+
+// The deviance x ln(x / m) + m - x (x, m > 0), by its series in v = (x - m) / (x + m) when x is near m, where the
+// closed form cancels
+__device__ double bd0(double x, double m) {
+    if (fabs(x - m) < 0.1 * (x + m)) {
+        double v = (x - m) / (x + m), s = (x - m) * v, ej = 2.0 * x * v;
+        v *= v;
+        for (int j = 1; j < 1000; ++j) {
+            ej *= v;
+            const double s1 = s + ej / (2 * j + 1);
+            if (s1 == s) return s1;
+            s = s1;
+        }
+        return s;
+    }
+    return x * log(x / m) + m - x;
+}
+
+// P[Binomial(n, r) = x] for integers 0 <= x <= n, 0 < r < 1, in Loader's saddle-point form: the Stirling remainders
+// and the two deviances are each small where the density is not, so no large terms cancel
+__device__ double dbinom(uint32_t x, uint32_t n, double r) {
+    const double dn = n, dx = x;
+    if (x == 0) return exp(dn * log1p(-r));
+    if (x == n) return exp(dn * log(r));
+    const double lc = stirlerr(dn) - stirlerr(dx) - stirlerr(dn - dx) - bd0(dx, dn * r) - bd0(dn - dx, fma(-dn, r, dn));
+    const double lf = 1.8378770664093453 + log(dx) + log1p(-dx / dn);  // ln(2 pi x (n - x) / n); the constant is ln 2 pi
+    return exp(lc - 0.5 * lf);
+}
+
+// P[Binomial(denom, r) >= common] = I_r(common, denom - common + 1), Mash's pValue.  With a = common and
+// b = denom - common + 1 the incomplete beta's prefactor x^a (1 - x)^b / (a B(a, b)) is (1 - r) dbinom(common), and
+// with a and b swapped r dbinom(common - 1), which keeps full precision at any denom where log-gamma differences
+// would not.
 __device__ double mash_p_value(uint32_t common, uint32_t denom, int k, uint64_t len_q, uint64_t len_r) {
     if (common == 0) return 1.0;
     const double four_k = ldexp(1.0, 2 * k);
@@ -141,9 +191,8 @@ __device__ double mash_p_value(uint32_t common, uint32_t denom, int k, uint64_t 
     if (!(r > 0.0)) return 0.0;
     if (r >= 1.0) return 1.0;
     const double a = common, b = (double)denom - common + 1.0;
-    const double lbt = lgamma(a + b) - lgamma(a) - lgamma(b) + a * log(r) + b * log1p(-r);
-    if (r < (a + 1.0) / (a + b + 2.0)) return exp(lbt) * beta_cf(a, b, r) / a;
-    return 1.0 - exp(lbt) * beta_cf(b, a, 1.0 - r) / b;
+    if (r < (a + 1.0) / (a + b + 2.0)) return dbinom(common, denom, r) * beta_cf(a, b, r) * (1.0 - r);
+    return 1.0 - r * dbinom(common - 1, denom, r) * beta_cf(b, a, 1.0 - r);
 }
 
 // Lane `lane` < nt of the warp finishes pair (q, r0 + lane) of the block with counts (c, d)
