@@ -8,6 +8,7 @@ package clone
 
 import (
 	"errors"
+	"math"
 	"strings"
 
 	"github.com/bebop/poly/internal/polyb200"
@@ -36,13 +37,19 @@ type Enzyme struct {
 	RecognitionSite string
 }
 
-// ErrUnsupported is returned for a non-literal pattern, or a part or fragment with a byte >= 0x80
-// (strings.ToUpper would re-encode it).  It is the error the library wrappers return for PG_ERR_UNSUPPORTED.
+// ErrUnsupported is returned for a non-literal pattern, a Skip or OverheadLength outside int32, or a part or
+// fragment with a byte >= 0x80 (strings.ToUpper would re-encode it).  It is the error the library wrappers return for PG_ERR_UNSUPPORTED.
 var ErrUnsupported = polyb200.ErrCloneUnsupported
 
 func (e Enzyme) lib() (polyb200.CloneEnzyme, error) {
 	for _, p := range []string{e.RegexpFor, e.RegexpRev} {
 		if p == "" || len(p) > 32 || strings.ContainsAny(p, "\\.+*?()|[]{}^$\x00") || strings.IndexFunc(p, func(r rune) bool { return r >= 0x80 }) >= 0 {
+			return polyb200.CloneEnzyme{}, ErrUnsupported
+		}
+	}
+	// pg_clone_enzyme holds Skip and OverheadLength as int32: a wider value would wrap
+	for _, v := range []int{e.Skip, e.OverheadLength} {
+		if v < math.MinInt32 || v > math.MaxInt32 {
 			return polyb200.CloneEnzyme{}, ErrUnsupported
 		}
 	}

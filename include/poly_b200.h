@@ -1137,7 +1137,10 @@ int pg_fragment_next_overhangs_batch(const uint8_t *overhangs, const uint64_t *o
 /* ---- clone.CutWithEnzyme / CircularLigate / GoldenGate -- clone/clone.go:138-355 --------------------
  * An enzyme: RegexpFor and RegexpRev as literal sites (1..32 bytes of 0x01..0x7f; anything else is
  * PG_ERR_UNSUPPORTED: the library does not implement Go's regexp language), Skip, OverheadLength and
- * RecognitionSite.  Palindromic = RecognitionSite equals its reverse complement (checks.IsPalindromic). */
+ * RecognitionSite.  Palindromic = RecognitionSite equals its reverse complement (checks.IsPalindromic).
+ * Skip and OverheadLength are Go ints held here as int32: only -2^31 .. 2^31 - 1 is supported, and the
+ * Python and Go bindings refuse a wider value as unsupported instead of narrowing it (a wrapped Skip cuts
+ * somewhere else). */
 typedef struct {
     const uint8_t *forward_site;
     uint32_t forward_len;

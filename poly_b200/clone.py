@@ -8,7 +8,8 @@ libpolyb200's host code, and every construct it closes is built and seqhashed on
 
 Enzyme sites must be plain literals (the reference compiles them as regexps; this library does not
 implement Go's regexp language): a pattern with a regexp metacharacter raises `UnsupportedError`, as does
-a part with a byte >= 0x80 (strings.ToUpper would re-encode it).
+a part with a byte >= 0x80 (strings.ToUpper would re-encode it).  Skip and OverheadLength must fit in
+int32 (the C ABI's width); a wider value raises `UnsupportedError` rather than wrapping.
 """
 from __future__ import annotations
 
@@ -57,6 +58,10 @@ class Enzyme:
         for p in (self.RegexpFor, self.RegexpRev):
             if not p or any(ch in _META for ch in p) or not p.isascii() or "\0" in p or len(p) > 32:
                 raise UnsupportedError(f"enzyme {self.Name}: pattern {p!r} is not a literal of 1..32 ASCII bytes (only literal sites are supported)")
+        for field in ("Skip", "OverheadLength"):  # pg_clone_enzyme holds them as int32; a wider value would wrap
+            v = getattr(self, field)
+            if not -(1 << 31) <= v < (1 << 31):
+                raise UnsupportedError(f"enzyme {self.Name}: {field} = {v} is outside int32 (only -2^31 .. 2^31 - 1 are supported)")
 
 
 class EnzymeNotFound(KeyError):

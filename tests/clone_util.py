@@ -1,7 +1,9 @@
 """Seeded clone workloads for the tests and tools/bench_clone.py: a digest-screen library with planted
-sites, and combinatorial Golden Gate libraries (a backbone plus positions x variants with distinct
-junction overhangs)."""
+sites, combinatorial Golden Gate libraries (a backbone plus positions x variants with distinct
+junction overhangs), and random ligation reactions over a small overhang alphabet."""
 from __future__ import annotations
+
+import random
 
 import numpy as np
 
@@ -93,3 +95,11 @@ def combinatorial_library(positions: int, variants: int, insert_len: int, backbo
         for _ in range(variants):
             parts.append((two_sites(lambda: flank() + b"GGTCTCA" + O[i] + bytes(body(insert_len)) + O[i + 1] + b"AGAGACC" + flank()), False))
     return parts, variants ** positions
+
+
+def random_reaction(rng: random.Random):
+    """Fragments over a small overhang alphabet: shared, reverse-complementary and palindromic overhangs, and
+    repeated sequences, so attaches in both orientations, loops and duplicate clones all occur."""
+    ohs = [b"AATT", b"GCGC", b"ACGT", b"GGAC", b"GTCC", b"TTAG", b"CTAA", b"CAGT"][: rng.randint(2, 8)]
+    seqs_ = [bytes(rng.choice(b"ACGT") for _ in range(rng.randint(0, 12))) for _ in range(rng.randint(1, 4))]
+    return [(rng.choice(seqs_), rng.choice(ohs), rng.choice(ohs)) for _ in range(rng.randint(1, 6))]

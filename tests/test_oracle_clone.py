@@ -10,6 +10,7 @@ import pytest
 
 import clone_oracle as co
 import seqhash_oracle
+from clone_util import random_reaction
 
 FIX = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "clone", "clone_fixtures.json")))
 BSAI, BSAI_RC = b"GGTCTCAATGC", b"ATGCAGAGACC"
@@ -109,14 +110,6 @@ def test_deferred_hash_matches_eager_on_fixtures(test):
         frags += co.cut(seq, circ, True, "BbsI")[1]
     _deferred_equals_eager(frags)
     _deferred_equals_eager([(b"AAAAAA", b"GTTG", b"CTAT"), (b"AAAAAA", b"CAAC", b"ATAG")])
-
-
-def random_reaction(rng: random.Random):
-    """Fragments over a small overhang alphabet: shared, reverse-complementary and palindromic overhangs, and
-    repeated sequences, so attaches in both orientations, loops and duplicate clones all occur."""
-    ohs = [b"AATT", b"GCGC", b"ACGT", b"GGAC", b"GTCC", b"TTAG", b"CTAA", b"CAGT"][: rng.randint(2, 8)]
-    seqs_ = [bytes(rng.choice(b"ACGT") for _ in range(rng.randint(0, 12))) for _ in range(rng.randint(1, 4))]
-    return [(rng.choice(seqs_), rng.choice(ohs), rng.choice(ohs)) for _ in range(rng.randint(1, 6))]
 
 
 def test_deferred_hash_matches_eager_on_random_reactions():
